@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — rows/s of the projection -> fp64->fp32 cast -> histogram hot path on B200.
+"""bench.py — rows/s of the projection -> fp64->fp32 cast -> histogram hot path on H100.
 
 Workloads (BASELINE.json ``configs``; SURVEY.md §8d):
 
@@ -21,6 +21,10 @@ Output: ONE JSON line on rank 0.
     python bench.py --workload m               # config M
     torchrun ... bench.py --gpus 8             # one rank per GPU
     python bench.py --impl reference           # CPU arm: the oracle port on all host cores
+    python bench.py --dump-outputs DIR         # also write the last timed step's outputs as DIR/<name>.npy
+
+Nothing is built or written inside the repository tree: ``__graft_entry__.build()`` compiles libloexec.so and the C
+oracle beforehand.
 """
 from __future__ import annotations
 
@@ -85,7 +89,7 @@ def peaks() -> tuple[float, str]:
             return float(json.loads(p.read_text())["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "H100 SXM data sheet 3.35 TB/s HBM3 (not a measured peak)"
 
 
 def workload_text(workload: str, rows: int, ncols: int, k: int) -> str:
@@ -98,7 +102,7 @@ def workload_text(workload: str, rows: int, ncols: int, k: int) -> str:
 
 
 class ClockSampler:
-    """SM clock / power / throttle reasons sampled DURING the timed region (B200_PROFILING.md 'clocks line').
+    """SM clock / power / throttle reasons sampled DURING the timed region.
     NVML is polled from a thread every ~2 ms (the timed region of an 8-GPU run lasts ~15 ms: `nvidia-smi -lms` cannot
     go below 100 ms and would see it once at best); `nvidia-smi -lms 100` is the fallback when NVML is not importable.
     Every sample is stamped on receipt and only those inside [mark_start, mark_end] are summarised."""
@@ -224,8 +228,6 @@ def cpu_pass_setup(workload: str, sample_rows: int, ncols: int):
     (parallel first touch: every page lives on the NUMA node of the thread that reads it), returns one_pass()."""
     os.environ.setdefault("OMP_PROC_BIND", "close")
     os.environ.setdefault("OMP_PLACES", "cores")
-    from learningorchestra_b200.build import build_oracle
-    build_oracle()
     import ctypes as C
     from oracle import cport
     threads = cport.use_all_cores()
@@ -461,13 +463,39 @@ def load_goldens(workload: str, rows: int, ncols: int):
     return g
 
 
+DUMP_SAMPLE_BLOCKS, DUMP_BLOCK_ROWS = 64, 4096      # projected-table sample: 64 seeded runs of 4096 rows per column
+
+
+def dump_outputs(path: Path, workload: str, sh, out, k: int, rank: int) -> None:
+    """What the timed call returned in its last step, for comparing two builds output for output: the merged counts
+    (``counts.npy``, k x bins, float64 holds every uint64 count exactly) and, where the step writes a projected fp32
+    table, the same fixed seeded sample of its rows in every run (``projected_sample.npy``, k x rows, and the row
+    numbers in ``projected_sample_rows.npy``; rank 0's shard when N > 1).  At most 64 MB in all."""
+    if rank != 0:
+        return
+    path.mkdir(parents=True, exist_ok=True)
+    if workload != "s10":
+        counts = sh.result(k * (256 if workload == "m" else NBINS)).reshape(k, -1)
+        np.save(path / "counts.npy", counts.astype(np.float64))
+    if out is not None:
+        shard = out.shards[0]
+        nblocks = min(DUMP_SAMPLE_BLOCKS, max(1, shard.nrows // DUMP_BLOCK_ROWS))
+        span = max(1, shard.nrows - DUMP_BLOCK_ROWS + 1)
+        starts = np.sort(np.random.default_rng(SEED).choice(span, size=min(nblocks, span), replace=False))
+        n = min(DUMP_BLOCK_ROWS, shard.nrows)
+        rows = np.concatenate([np.arange(s, s + n) for s in starts])
+        sample = np.stack([np.concatenate([shard.to_numpy(j, int(s), n) for s in starts]) for j in range(k)])
+        np.save(path / "projected_sample.npy", sample.astype(np.float32))
+        np.save(path / "projected_sample_rows.npy", rows.astype(np.float64))
+    log(f"outputs of the last timed step written to {path}")
+
+
 def run_gpu(args) -> int:
     real_stdout = _claim_stdout()
     import torch
     import torch.distributed as dist
 
     from learningorchestra_b200 import _native as N
-    from learningorchestra_b200.build import build_native
     from learningorchestra_b200.engine import Engine
     from learningorchestra_b200.sharding import ShardedEngine
 
@@ -481,10 +509,6 @@ def run_gpu(args) -> int:
     torch.cuda.set_device(local_rank)
     if world > 1:
         dist.init_process_group("nccl", device_id=torch.device("cuda", local_rank))
-    if rank == 0:
-        build_native()                      # no-op when the in-tree .so is newer than its sources
-    if world > 1:
-        dist.barrier()                      # nobody loads libloexec.so while rank 0 might be rewriting it
 
     w = args.workload
     eng = Engine(local_rank)
@@ -561,6 +585,8 @@ def run_gpu(args) -> int:
     torch.cuda.synchronize()
     sampler.mark_end()
     launches = eng.launch_count - launches0 - 1          # the barrier launch is outside the timed region
+    if args.dump_outputs:
+        dump_outputs(Path(args.dump_outputs), w, sh, out, k, rank)
     for _ in range(5):                                   # the same step in isolation (event-bracketed, serialised)
         step(True)
     torch.cuda.synchronize()
@@ -709,9 +735,9 @@ def run_gpu(args) -> int:
                            "merge inside the streaming kernel: column-last CTAs push with system-scope RED.64 into rank 0's "
                            "matrix over NVLink (CUDA IPC), arrival + root epilogue in-kernel, one launch per step"))
                                       if world > 1 else "single GPU",
-                       "l2": (f"inputs larger than L2: {gb_in:.2f} GB read per GPU per step (L2 = 126 MB), no flush needed"
+                       "l2": (f"inputs larger than L2: {gb_in:.2f} GB read per GPU per step (L2 = 50 MB), no flush needed"
                               if gb_in > 0.5 else
-                              f"{gb_in * 1e3:.0f} MB read per GPU per step: NOT larger than L2 (126 MB) at this N; "
+                              f"{gb_in * 1e3:.0f} MB read per GPU per step: NOT larger than L2 (50 MB) at this N; "
                               "latency-dominated, reported in microseconds")},
             "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
                          "traffic": None, "peak_source": peak_src, "kernel": W["kernel"],
@@ -726,16 +752,6 @@ def run_gpu(args) -> int:
             line["cpu_baseline"] = cpu
         if executor:
             line["e2e_executor"] = executor
-        tr = ROOT / "profiles" / "traffic.json"
-        if tr.exists():
-            try:
-                key = {"s100": "k_project_cast_hist_bytes_per_launch", "m": "k_hist_u8_cols_bytes_per_launch"}.get(w)
-                full = json.loads(tr.read_text()).get(key) if key else None      # ncu, one full-size launch
-                line["roofline"]["traffic"] = full * nrows / W["rows"] if full else None
-                line["roofline"]["traffic_source"] = ("ncu --set full dram__bytes_read+write of one full-size launch "
-                                                      "(profiles/), scaled to this launch's rows")
-            except Exception:
-                pass
         _emit(real_stdout, line)
         if parity.get("ok") is False or (e2e and e2e.get("counts_match_golden") is False):
             log("PARITY FAILURE:", json.dumps(parity), json.dumps(e2e))
@@ -774,6 +790,8 @@ def main():
                     help="serialise consecutive steps completely (no programmatic dependent launch between them)")
     ap.add_argument("--merge", default="auto", choices=["auto", "nccl", "p2p", "peer"],
                     help="N > 1: how partial histograms are merged (in-kernel peer-memory merge, or NCCL all-reduce)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write what the last one computed as DIR/<name>.npy (rank 0)")
     args = ap.parse_args()
     args.rows = args.rows or WORKLOADS[args.workload]["rows"]
     args.cols = args.cols or WORKLOADS[args.workload]["cols"]

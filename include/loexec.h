@@ -1,5 +1,5 @@
 /*
- * loexec.h — C ABI of libloexec.so, the B200-native (sm_100a) executor for
+ * loexec.h — C ABI of libloexec.so, the H100-native (sm_90a) executor for
  * learningOrchestra's projection -> type-cast -> histogram hot path.
  *
  * The reference has no native boundary on this path: it crosses from Python

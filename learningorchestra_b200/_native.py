@@ -2,7 +2,7 @@
 
 The library is loaded from ``learningorchestra_b200/lib/libloexec.so`` (built in-tree by
 ``learningorchestra_b200.build``).  There is no Python or CPU fallback: if the library is missing
-or no B200 is visible, importing this module still works (so CPU-only hosts can run the host-logic
+or no H100 is visible, importing this module still works (so CPU-only hosts can run the host-logic
 tests) but the first call raises :class:`LoexecError`.
 """
 from __future__ import annotations

@@ -1,6 +1,6 @@
 """In-tree build of the native pieces.
 
-* ``learningorchestra_b200/lib/libloexec.so`` — the product: sm_100a kernels + C ABI
+* ``learningorchestra_b200/lib/libloexec.so`` — the product: sm_90a kernels + C ABI
   (``include/loexec.h``), compiled with nvcc (cross-compiles without a GPU).
 * ``oracle/_build/liboracle.so`` — the CPU oracle's C restatement (test infrastructure,
   gcc + OpenMP).  Building the checker is not using it: nothing in this package loads it.
@@ -23,7 +23,7 @@ ORACLE_SRC = ROOT / "oracle" / "bsem.c"
 ORACLE_LIB = ROOT / "oracle" / "_build" / "liboracle.so"
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-std=c++17", "-lineinfo",
     "-Xcompiler", "-fPIC,-O2,-Wall",
     "-shared", "-cudart", "static",

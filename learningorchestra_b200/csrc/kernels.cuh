@@ -1,4 +1,4 @@
-// kernels.cuh — sm_100a device code of libloexec: projection + cast + histogram.
+// kernels.cuh — sm_90a device code of libloexec: projection + cast + histogram.
 //
 // Replaces (reference paths under /root/reference/microservices):
 //   projection_image/projection.py:38-43          column subset copy        -> K1
@@ -7,11 +7,11 @@
 //
 // Design (see DESIGN.md §3):
 //   * table = columnar slabs in HBM; a work tile is (projected column j, kTileRows rows), one tile per CTA
-//     (the grid de-phases itself: a persistent, lockstep variant measured 20 % slower).
-//   * k_project_cast_hist: every thread streams 32-byte (LDG.E.256) vectors of its column slab with
+//     (the grid de-phases itself; a persistent variant runs its CTAs in lock step).
+//   * k_project_cast_hist: every thread streams 32-byte vectors (two LDG.E.128 each) of its column slab with
 //     L1::no_allocate / L2::evict_first through a 2 x 5-vector register pipeline, converts, and streams the
 //     result out with st.cs.  k_project_cast_hist_tma is the same tile fed by cp.async.bulk + mbarriers
-//     (opt-in; measured equal).
+//     (opt-in).
 //   * histogram = PRIVATE PER-THREAD BYTE COUNTERS in shared memory, laid out so that thread t only ever
 //     touches bank (t % 32): word w of thread t lives at smem word w*kThreads + t.  Increment = plain
 //     LDS.U8 / IADD / STS.U8 (f64 kernel) or one ATOMS.ADD on the containing word (byte kernel) — no bank
@@ -23,7 +23,7 @@
 //     (k_project_cast_hist_bins) drop the byte fields: 32-bit counters in lane slots shared by the CTA's warps, bank =
 //     lane, the counter address one PRMT (bytes) or one shift-add (bins) away from the value, ONE ATOMS per element, a
 //     CTA streams a long chunk of its column and folds once.  The per-thread byte-counter variants of K4
-//     (k_hist_u8_cols<ALIGNED, MODE>) stay behind LOEXEC_U8_MODE as the measured history (DESIGN.md §3.4).
+//     (k_hist_u8_cols<ALIGNED, MODE>) stay behind LOEXEC_U8_MODE as alternatives (DESIGN.md §3.4).
 //   * several GPUs (GroupStep): the bins go to the device's own matrix; the CTA finishing a column's last tile pushes
 //     the column to the root GPU with system-scope RED.64 over NVLink, the last pusher arrives, the root's last CTA
 //     moves the merged matrix out — merge, arrival and epilogue ride inside the one streaming launch per step.
@@ -39,12 +39,13 @@
 namespace lo {
 
 constexpr int kThreads      = 256;                 // threads per CTA
-constexpr int kVec          = 4;                   // f64 elements per 32-byte load
+constexpr int kVec          = 4;                   // f64 elements per 32-byte vector (two 16-byte loads)
 constexpr int kBatch        = 4;                   // vector loads in flight per thread
 constexpr int kBatches      = 15;
 constexpr int kVecPerThread = kBatch * kBatches;   // 60
 constexpr int kElemsPerThread = kVec * kVecPerThread;      // 240 <= 255 (byte counter bound)
 constexpr int kTileRows     = kThreads * kElemsPerThread;  // 61440 rows per tile
+constexpr int kHalf         = kThreads * kVec / 2;         // second pair of a thread's vector (ldg_split4_stream)
 constexpr int kHistRows     = 64;                  // smem words per thread (256 bins / 4)
 constexpr int kHistSmemBytes = (kHistRows * kThreads + 256) * 4;   // 66560 B -> 3 CTAs / SM
 
@@ -125,9 +126,21 @@ struct GroupStep {
 // ---------------------------------------------------------------------------------------------
 // streaming memory ops
 // ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ void ldg256_stream(const double *p, double (&v)[4]) {
-    asm volatile("ld.global.nc.L1::no_allocate.L2::evict_first.v4.f64 {%0,%1,%2,%3}, [%4];"
-                 : "=d"(v[0]), "=d"(v[1]), "=d"(v[2]), "=d"(v[3]) : "l"(p));
+// sm_90 loads and stores at most 16 bytes per thread.  A thread's four f64 of a CTA-wide block are therefore two pairs:
+// {p[0], p[1]} and {p[half], p[half + 1]} with p = block + 2 * tid and half = 2 * threads, so each instruction of a warp
+// covers 512 contiguous bytes (the layout the TMA kernel reads from its staging ring).  On sm_90 the L2 evict-first
+// priority of 128-bit loads is an L2::cache_hint policy operand.
+__device__ __forceinline__ uint64_t l2_evict_first_policy() {
+    uint64_t pol;
+    asm("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
+    return pol;
+}
+__device__ __forceinline__ void ldg_split4_stream(const double *p, long long half, double (&v)[4]) {
+    const uint64_t pol = l2_evict_first_policy();
+    asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.v2.f64 {%0,%1}, [%2], %3;"
+                 : "=d"(v[0]), "=d"(v[1]) : "l"(p), "l"(pol));
+    asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.v2.f64 {%0,%1}, [%2], %3;"
+                 : "=d"(v[2]), "=d"(v[3]) : "l"(p + half), "l"(pol));
 }
 __device__ __forceinline__ double ldg64_stream(const double *p) {
     double v;
@@ -145,11 +158,14 @@ __device__ __forceinline__ uint32_t ldg8_stream(const uint8_t *p) {
     asm volatile("ld.global.nc.L1::no_allocate.u8 %0, [%1];" : "=r"(v) : "l"(p));
     return v;
 }
-__device__ __forceinline__ void stg128_stream(float *p, float a, float b, float c, float d) {
-    asm volatile("st.global.cs.v4.f32 [%0], {%1,%2,%3,%4};" :: "l"(p), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
+// the stores matching ldg_split4_stream: {a, b} at p, {c, d} at p + half
+__device__ __forceinline__ void stg_split4_stream(float *p, long long half, float a, float b, float c, float d) {
+    asm volatile("st.global.cs.v2.f32 [%0], {%1,%2};" :: "l"(p), "f"(a), "f"(b) : "memory");
+    asm volatile("st.global.cs.v2.f32 [%0], {%1,%2};" :: "l"(p + half), "f"(c), "f"(d) : "memory");
 }
-__device__ __forceinline__ void stg256_stream(double *p, const double (&v)[4]) {
-    asm volatile("st.global.cs.v4.f64 [%0], {%1,%2,%3,%4};" :: "l"(p), "d"(v[0]), "d"(v[1]), "d"(v[2]), "d"(v[3]) : "memory");
+__device__ __forceinline__ void stg_split4_stream(double *p, long long half, const double (&v)[4]) {
+    asm volatile("st.global.cs.v2.f64 [%0], {%1,%2};" :: "l"(p), "d"(v[0]), "d"(v[1]) : "memory");
+    asm volatile("st.global.cs.v2.f64 [%0], {%1,%2};" :: "l"(p + half), "d"(v[2]), "d"(v[3]) : "memory");
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -462,7 +478,7 @@ __device__ __forceinline__ void group_finish_column(const GroupStep &G, unsigned
 // K1+K2+K3: fused projection + cast + histogram over f64 column slabs
 //   OUT: 0 = no projected output (histogram only), 1 = f32 (cast), 2 = f64 (copy)
 //   HIST: accumulate per-column fixed-width histogram of the cast value
-//   ALIGNED: column slabs (in and out) are 32-byte aligned -> 256-bit loads, 128/256-bit stores
+//   ALIGNED: column slabs (in and out) are 32-byte aligned -> 128-bit loads, 64/128-bit stores
 // grid.x = k * tiles_per_col ; tile index fastest along rows
 // ---------------------------------------------------------------------------------------------
 template <int OUT, bool HIST, bool ALIGNED, bool FASTDIV>
@@ -497,14 +513,15 @@ k_project_cast_hist(const char *__restrict__ in_base, long long in_pitch,
 
     if (ALIGNED && n == kTileRows) {
         // full tile (all but the last tile of a column): no bounds checks, register-pipelined loads.
-        // vector index of (batch b, slot u) = (b*kPfBatch + u)*kThreads + tid  ->  warp-contiguous 1 KiB
+        // (batch b, slot u) is the CTA-wide block (b*kPfBatch + u) of kThreads*kVec elements; the thread's four are
+        // {2t, 2t+1} of its first half and of its second half (ldg_split4_stream)
         double v[kPfBuf][kPfBatch][4];
-        const double *src = in + (long long)threadIdx.x * kVec;
+        const double *src = in + 2 * (long long)threadIdx.x;
 #pragma unroll
         for (int pb = 0; pb < kPfBuf - 1; ++pb)
 #pragma unroll
             for (int u = 0; u < kPfBatch; ++u)
-                ldg256_stream(src + (long long)(pb * kPfBatch + u) * kThreads * kVec, v[pb][u]);
+                ldg_split4_stream(src + (long long)(pb * kPfBatch + u) * kThreads * kVec, kHalf, v[pb][u]);
         if (HIST) zero_private(smem, rows);        // the first batch's DRAM latency overlaps the clearing and its barrier
 #pragma unroll 1
         for (int b0 = 0; b0 < kPfBatches; b0 += kPfBuf) {
@@ -515,15 +532,16 @@ k_project_cast_hist(const char *__restrict__ in_base, long long in_pitch,
                 if (nb < kPfBatches) {
 #pragma unroll
                     for (int u = 0; u < kPfBatch; ++u)
-                        ldg256_stream(src + (long long)(nb * kPfBatch + u) * kThreads * kVec, v[(s + kPfBuf - 1) % kPfBuf][u]);
+                        ldg_split4_stream(src + (long long)(nb * kPfBatch + u) * kThreads * kVec, kHalf,
+                                          v[(s + kPfBuf - 1) % kPfBuf][u]);
                 }
 #pragma unroll
                 for (int u = 0; u < kPfBatch; ++u) {
-                    const long long e = ((long long)(b * kPfBatch + u) * kThreads + threadIdx.x) * kVec;
+                    const long long e = (long long)(b * kPfBatch + u) * kThreads * kVec + 2 * threadIdx.x;
                     float f0 = cast_f64_f32(v[s][u][0]), f1 = cast_f64_f32(v[s][u][1]);
                     float f2 = cast_f64_f32(v[s][u][2]), f3 = cast_f64_f32(v[s][u][3]);
-                    if (OUT == 1) stg128_stream(out32 + e, f0, f1, f2, f3);
-                    if (OUT == 2) stg256_stream(out64 + e, v[s][u]);
+                    if (OUT == 1) stg_split4_stream(out32 + e, kHalf, f0, f1, f2, f3);
+                    if (OUT == 2) stg_split4_stream(out64 + e, kHalf, v[s][u]);
                     if (HIST)
                         bump4(priv, bin_index_f32<FASTDIV>(f0, B), bin_index_f32<FASTDIV>(f1, B),
                               bin_index_f32<FASTDIV>(f2, B), bin_index_f32<FASTDIV>(f3, B));
@@ -534,36 +552,37 @@ k_project_cast_hist(const char *__restrict__ in_base, long long in_pitch,
         if (HIST) zero_private(smem, rows);
 #pragma unroll 1
         for (int b = 0; b < kBatches; ++b) {
-            const long long e0 = ((long long)b * kBatch * kThreads + threadIdx.x) * kVec;   // first element of vector 0
+            const long long e0 = (long long)b * kBatch * kThreads * kVec + 2 * threadIdx.x;   // first element of vector 0
             if (e0 >= n) break;
             double v[kBatch][4];
-            if (e0 + (long long)(kBatch - 1) * kThreads * kVec + kVec <= n) {
+            if (e0 + (long long)(kBatch - 1) * kThreads * kVec + kHalf + 2 <= n) {
                 // whole batch in range: all loads first (MLP), then convert/store/bin
 #pragma unroll
-                for (int u = 0; u < kBatch; ++u) ldg256_stream(in + e0 + (long long)u * kThreads * kVec, v[u]);
+                for (int u = 0; u < kBatch; ++u) ldg_split4_stream(in + e0 + (long long)u * kThreads * kVec, kHalf, v[u]);
 #pragma unroll
                 for (int u = 0; u < kBatch; ++u) {
                     const long long e = e0 + (long long)u * kThreads * kVec;
                     float f0 = cast_f64_f32(v[u][0]), f1 = cast_f64_f32(v[u][1]);
                     float f2 = cast_f64_f32(v[u][2]), f3 = cast_f64_f32(v[u][3]);
-                    if (OUT == 1) stg128_stream(out32 + e, f0, f1, f2, f3);
-                    if (OUT == 2) stg256_stream(out64 + e, v[u]);
+                    if (OUT == 1) stg_split4_stream(out32 + e, kHalf, f0, f1, f2, f3);
+                    if (OUT == 2) stg_split4_stream(out64 + e, kHalf, v[u]);
                     if (HIST)
                         bump4(priv, bin_index_f32<FASTDIV>(f0, B), bin_index_f32<FASTDIV>(f1, B),
                               bin_index_f32<FASTDIV>(f2, B), bin_index_f32<FASTDIV>(f3, B));
                 }
             } else {
-                // ragged end of the column: element-wise
+                // ragged end of the column: element-wise over the same four positions per vector
 #pragma unroll 1
                 for (int u = 0; u < kBatch; ++u) {
                     const long long e = e0 + (long long)u * kThreads * kVec;
 #pragma unroll 1
                     for (int q = 0; q < kVec; ++q) {
-                        if (e + q < n) {
-                            double x = ldg64_stream(in + e + q);
+                        const long long eq = e + (q & 1) + (q >> 1) * kHalf;
+                        if (eq < n) {
+                            double x = ldg64_stream(in + eq);
                             float  f = cast_f64_f32(x);
-                            if (OUT == 1) out32[e + q] = f;
-                            if (OUT == 2) out64[e + q] = x;
+                            if (OUT == 1) out32[eq] = f;
+                            if (OUT == 2) out64[eq] = x;
                             if (HIST) bin_f32<FASTDIV>(priv, f, B);
                         }
                     }
@@ -649,18 +668,19 @@ k_project_cast_hist_bins(const char *__restrict__ in_base, long long in_pitch, c
     };
     long long done = 0;
     if (aligned) {
-        const double *src = in + (long long)threadIdx.x * kVec;
+        constexpr long long kWBHalf = kWBThreads * kVec / 2;
+        const double *src = in + 2 * (long long)threadIdx.x;
 #pragma unroll 1
         for (; done + kWBRoundRows <= n; done += kWBRoundRows) {
             double v[kWBVecs][4];
 #pragma unroll
-            for (int u = 0; u < kWBVecs; ++u) ldg256_stream(src + done + (long long)u * kWBThreads * kVec, v[u]);
+            for (int u = 0; u < kWBVecs; ++u) ldg_split4_stream(src + done + (long long)u * kWBThreads * kVec, kWBHalf, v[u]);
 #pragma unroll
             for (int u = 0; u < kWBVecs; ++u) {
-                const long long e = done + ((long long)u * kWBThreads + threadIdx.x) * kVec;
+                const long long e = done + (long long)u * kWBThreads * kVec + 2 * threadIdx.x;
                 const float f0 = cast_f64_f32(v[u][0]), f1 = cast_f64_f32(v[u][1]), f2 = cast_f64_f32(v[u][2]), f3 = cast_f64_f32(v[u][3]);
-                if (OUT == 1) stg128_stream(out32 + e, f0, f1, f2, f3);
-                if (OUT == 2) stg256_stream(out64 + e, v[u]);
+                if (OUT == 1) stg_split4_stream(out32 + e, kWBHalf, f0, f1, f2, f3);
+                if (OUT == 2) stg_split4_stream(out64 + e, kWBHalf, v[u]);
                 count(f0); count(f1); count(f2); count(f3);
             }
         }
@@ -691,7 +711,7 @@ k_project_cast_hist_bins(const char *__restrict__ in_base, long long in_pitch, c
 // K1+K2+K3, TMA form (LOEXEC_TMA=1): the same tile, but the column slab is staged into shared memory by the
 // bulk-copy engine (cp.async.bulk global -> shared, completion on an mbarrier) through a kTmaStages-deep ring
 // driven by one producer thread; the 256 consumer threads read their 32 bytes from the ring instead of
-// issuing LDG.E.256 themselves.  Built to answer "would TMA staging beat the register pipeline?" with a
+// issuing the 128-bit loads themselves.  Built to answer "would TMA staging beat the register pipeline?" with a
 // measurement (DESIGN.md §3.8); arithmetic, tile shape, private histograms and results are identical.
 // Full, 32-byte-aligned tiles only — the host routes everything else to k_project_cast_hist.
 // ---------------------------------------------------------------------------------------------
@@ -778,7 +798,7 @@ k_project_cast_hist_tma(const char *__restrict__ in_base, long long in_pitch,
         double *out64 = (OUT == 2) ? reinterpret_cast<double *>(out_base + (long long)j * out_pitch) + r0 : nullptr;
         const int lane = threadIdx.x & 31;
 #ifndef LO_TMA_UNROLL
-#define LO_TMA_UNROLL 1     // measured: 1 -> 5.49-5.64 ms, 2 -> 5.85, 3 -> 6.3 (100M x 32 fused)
+#define LO_TMA_UNROLL 1
 #endif
         static_assert(kTmaRounds % LO_TMA_UNROLL == 0, "rounds per tile must be a multiple of the unroll");
 #pragma unroll 1
@@ -861,7 +881,7 @@ k_project_cast_hist_tma(const char *__restrict__ in_base, long long in_pitch,
 // How one byte becomes a counter update (template parameter MODE of k_hist_u8_cols; LOEXEC_U8_MODE picks at launch):
 //   2: two LDS.U8 / IADD / STS.U8 round trips per 16-bit pair (bump2), no atomics
 //   4: ONE conflict-free ATOMS.ADD per byte on the 32-bit word holding the counter, offsets / shifts pulled out
-//      of the input word with PRMT (round 1's best: 0.41 of the HBM peak, ALU-pipe bound: ncu "math pipe throttle")
+//      of the input word with PRMT (ALU-pipe bound)
 //   5: like 4, per-byte arithmetic written as masks + multiply-adds (ptxas turns the constant multiplies into
 //      LEA.HI / IMAD.SHL and balances the two integer pipes itself)
 //   7: the counter word's whole shared-memory address from ONE PRMT (thread bits pre-merged into the row bytes), the
@@ -909,7 +929,7 @@ __device__ __forceinline__ void atoms_add(uint32_t addr, uint32_t v) {
 }
 
 // shared-window address at which a block's dynamic shared memory starts when the kernel has no static shared memory:
-// the 1 KiB sm_100 reserves per block.  Mode 7 puts it in the atomics' immediate offset; the kernel traps if it is wrong.
+// the 1 KiB sm_90 reserves per block (lo_init checks the size).  Mode 7 puts it in the atomics' immediate offset; the kernel traps if it is wrong.
 #define LO_SMEM_WINDOW_BASE 1024
 __device__ __forceinline__ void atoms_add_base(uint32_t offset, uint32_t v) {
     asm volatile("red.shared.add.u32 [%0+1024], %1;" :: "r"(offset), "r"(v) : "memory");
@@ -946,7 +966,7 @@ __device__ __forceinline__ void bump_word(uint8_t *priv, uint32_t x, const U8Con
         //     [ (4t) & 0xFF | (b & 0xFC) + ((4t) >> 8) | 0 | 0 ];
         // `rows` carries (b_q & 0xFC) | ((4t) >> 8) in byte q (K.p8 = ((4t) >> 8) * 0x01010101), so PRMT(rows, 4t) takes
         // byte q of rows as byte 1 and bytes 0, 2, 3 from 4t.  The start of the dynamic shared memory in the shared
-        // window — kSmemWindowBase, the 1 KiB the system reserves per block on sm_100; checked at kernel start — rides
+        // window — kSmemWindowBase, the 1 KiB the system reserves per block on sm_90; checked at kernel start — rides
         // in the atomic's immediate offset, so no add is needed either.  The field value 1 << 8 * (b & 3) is a
         // wrap-mode funnel shift (reads only bits 0..4 of the count); its count for byte 0 needs no extraction.
         const uint32_t t4 = K.p3;                                                   // 4 * t
@@ -954,8 +974,8 @@ __device__ __forceinline__ void bump_word(uint8_t *priv, uint32_t x, const U8Con
         const uint32_t shifts = (x & 0x03030303u) << 3;
         if (MODE == 10) {
             // mode 10: the three count extractions as the HIGH word of a widening multiply by 2^24 / 2^16 / 2^8 held as
-            // DATA (so ptxas cannot turn them back into SHF): FMA pipe instead of ALU pipe (scripts/probes/atoms_probe:
-            // the ALU pipe's 64 lane-ops per clock per SM, not the atomics, is what the per-byte arithmetic runs into)
+            // DATA (so ptxas cannot turn them back into SHF): FMA pipe instead of ALU pipe
+            // (the ALU pipe's 64 lane-ops per clock per SM, not the atomics, is what the per-byte arithmetic runs into)
             atoms_add_base(__byte_perm(rows, t4, 0x7604u), one_shl_wrap(shifts));
             atoms_add_base(__byte_perm(rows, t4, 0x7614u), one_shl_wrap(mul_wide_hi(shifts, K.p24)));
             atoms_add_base(__byte_perm(rows, t4, 0x7624u), one_shl_wrap(mul_wide_hi(shifts, K.p16)));
@@ -1147,8 +1167,8 @@ k_hist_u8_cols(const uint8_t *__restrict__ in_base, long long in_pitch, long lon
 
 // ---------------------------------------------------------------------------------------------
 // K4, wide form (LOEXEC_U8_MODE=8): 512 threads per CTA, TWO threads per private histogram.
-// The 256-thread kernel is latency-bound at the 24 warps per SM its 256 B of counters per thread allow (ncu: issue
-// slots 46 % busy, no pipe saturated).  Increments are shared-memory atomics anyway, so threads t and t + 256 —
+// The 256-thread kernel is latency-bound at the 24 warps per SM its 256 B of counters per thread allow (no pipe
+// saturated).  Increments are shared-memory atomics anyway, so threads t and t + 256 —
 // different warps, same lane, hence the same private bank and still conflict-free inside every warp — can share one
 // histogram as long as the two together stay below 256 elements per tile: 7 vectors of 16 bytes each (2 x 112 = 224).
 // Same shared memory per CTA, twice the warps (48 per SM), half the registers per thread (<= 40).
@@ -1317,8 +1337,8 @@ k_hist_u8_cols_wide(const uint8_t *__restrict__ in_base, long long in_pitch, lon
 
 // ---------------------------------------------------------------------------------------------
 // K4, lane-slot form (LOEXEC_U8_MODE=11): 32-bit counters shared by all warps of the CTA.
-// scripts/probes/atoms_probe measured what bounds the per-thread byte counters: not the atomic unit (1.58 conflict-free
-// ATOMS per clock per SM with operands ready) but the arithmetic that turns a byte into (counter word, byte field):
+// What bounds the per-thread byte counters is not the atomic unit (conflict-free
+// ATOMS with their operands ready retire fast enough) but the arithmetic that turns a byte into (counter word, byte field):
 // mask, PRMT, shift extraction, 1 << n.  This layout needs none of it.  The CTA keeps ONE histogram of 256 bins x 64
 // slots of 32-bit counters (64 KiB): slot = lane + 32 * (warp & 1), counter of (bin b, slot s) at byte b * 256 + 4 * s.
 //   * bank = (b * 64 + s) mod 32 = lane: every warp instruction is conflict-free, whatever the data;
@@ -1335,8 +1355,8 @@ constexpr int kU8LRoundRows = kU8LThreads * 4 * kU8VecBytes;      // 32 768 rows
 
 // VAR bit 0: the increment is an opaque register (ATOMS.ADD) instead of the literal 1 (ptxas picks ATOMS.POPC.INC)
 // VAR bit 1: one register set copied per round instead of two alternating sets;  bit 2: no two-compare quick reject
-// before the run test.  LOEXEC_U8_MODE 11 = VAR 2 (shipped: the copy form is 2-3 % faster than alternating sets,
-// profiles/r02_u8_sweep_lanes_loop_forms.json), 12 = VAR 3, 13 = VAR 0, 14 = VAR 6
+// before the run test.  LOEXEC_U8_MODE 11 = VAR 2 (shipped: the copy form),
+// 12 = VAR 3, 13 = VAR 0, 14 = VAR 6
 template <int VAR>
 __global__ void __launch_bounds__(kU8LThreads, 3)
 k_hist_u8_cols_lanes(const uint8_t *__restrict__ in_base, long long in_pitch, long long nrows,

@@ -1,7 +1,7 @@
 // loexec.cu — host side of libloexec.so: the C ABI declared in include/loexec.h.
 //
 // Nothing here computes on the CPU: every entry point either moves bytes or launches the
-// sm_100a kernels in kernels.cuh.  There is no fallback path; without a Blackwell device
+// sm_90a kernels in kernels.cuh.  There is no fallback path; without a Hopper device
 // lo_init() fails and nothing else is callable.
 #include "loexec.h"
 #include "kernels.cuh"
@@ -260,9 +260,8 @@ int launch_f64(lo_ctx *ctx, const lo_table *in, const lo_table *out, int32_t out
         return LO_OK;
     }
     // one tile (kTileRows rows of one projected column) per CTA.  A tapered tail — the last wave cut into short
-    // tiles — was built and measured in round 2 (profiles/r02_tile_sweep.json): equal or slower at every shard size
-    // (12.5 M rows x 32: 0.752 ms uniform vs 0.752 - 0.764 tapered; 100 M: 2 % slower), and the runtime tile shape cost
-    // the uniform case 3 % (5.71 vs 5.53 ms, same box, scripts/ab_libs.py), so tiles are compile-time uniform again.
+    // tiles — was built and was not faster, and a runtime tile shape slows the uniform case, so tiles are compile-time
+    // uniform.
     const unsigned tiles_per_col = (unsigned)((in->nrows + lo::kTileRows - 1) / lo::kTileRows);
     const unsigned long long blocks = (unsigned long long)tiles_per_col * (unsigned)P.k;
     if (blocks > 0x7fffffffull) return fail(LO_ERR_INVALID, "table too large for one launch (%llu tiles)", blocks);
@@ -389,7 +388,7 @@ int hist_u8_impl(lo_ctx *ctx, const lo_table *in, const int32_t *col_idx, int32_
     int64_t tile_rows = !wide ? lo::kU8TileRows : mode == 8 ? lo::kU8WTileRows2 : lo::kU8WTileRows4;
     if (lanes) {
         // chunk of a column per CTA, a multiple of the 32 Ki-row round: long chunks amortise the 64 KiB clear + fold
-        // (8 rounds measured best on 1 M+ row tables, one chunk per column on 125 K-row shards: r02_u8_sweep_chunks.json)
+        // (up to 8 rounds, one chunk per column on short shards)
         const int64_t slots = (int64_t)ctx->sm_count * 3;
         int64_t want = (in->nrows * (int64_t)std::min<int32_t>(k, lo::kMaxColsU8)) / slots;
         want = std::max<int64_t>(lo::kU8LRoundRows, std::min<int64_t>(want, 8 * (int64_t)lo::kU8LRoundRows));
@@ -528,7 +527,7 @@ struct StageLease {
 
 // rows per chunk of the *_host pipeline: ~LOEXEC_CHUNK_MB (default 512) MiB of input per chunk, whole tiles
 int64_t chunk_rows_for(int64_t nrows, int32_t k, size_t elem_bytes, int64_t tile_rows) {
-    size_t mb = 256;   // measured on B200/PCIe5: 64 MiB -> 40 GB/s, 256 -> 47.8, 1024 -> 49.4 H2D with D2H running
+    size_t mb = 256;   // large enough that per-copy submission cost is small against the PCIe transfer itself
     if (const char *e = getenv("LOEXEC_CHUNK_MB")) {
         long v = atol(e);
         if (v >= 1 && v <= 8192) mb = (size_t)v;
@@ -572,9 +571,15 @@ int lo_init(int device, lo_ctx **out) {
     if (device < 0 || device >= n) return fail(LO_ERR_INVALID, "device %d outside [0, %d)", device, n);
     cudaDeviceProp prop;
     LO_CUDA(cudaGetDeviceProperties(&prop, device));
-    if (prop.major != 10)
-        return fail(LO_ERR_NO_DEVICE, "device %d is sm_%d%d; libloexec is built for sm_100a only", device,
+    if (prop.major != 9 || prop.minor != 0)
+        return fail(LO_ERR_NO_DEVICE, "device %d is sm_%d%d; libloexec is built for sm_90a only", device,
                     prop.major, prop.minor);
+    // the byte-histogram kernels put the start of dynamic shared memory (after this reserve) in an immediate offset
+    int reserved = 0;
+    LO_CUDA(cudaDeviceGetAttribute(&reserved, cudaDevAttrReservedSharedMemoryPerBlock, device));
+    if (reserved != LO_SMEM_WINDOW_BASE)
+        return fail(LO_ERR_NO_DEVICE, "device %d reserves %d bytes of shared memory per block, the kernels assume %d",
+                    device, reserved, LO_SMEM_WINDOW_BASE);
     LO_CUDA(cudaSetDevice(device));
     lo_ctx *ctx = new (std::nothrow) lo_ctx;
     if (!ctx) return fail(LO_ERR_NOMEM, "out of host memory");
@@ -586,7 +591,7 @@ int lo_init(int device, lo_ctx **out) {
         LO_CUDA(cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking));
         // scratch of the parser / group-by calls comes from the device's stream-ordered pool: keep up to 8 GiB of it
         // mapped between calls (the default threshold of 0 hands everything back at every synchronise, and the next
-        // call pays the mapping again: ~5 ms of a 9 ms call on 20 M rows)
+        // call pays the mapping again)
         cudaMemPool_t pool = nullptr;
         LO_CUDA(cudaDeviceGetDefaultMemPool(&pool, device));
         uint64_t keep = 8ull << 30;
@@ -947,7 +952,7 @@ namespace {
 
 // One chunk of k host columns <-> k staging slabs.  Host columns that sit at a constant stride (one 2-D array, the
 // usual case: a numpy matrix, an Arrow table's buffers from one allocation) go as ONE strided 2-D copy per run instead
-// of one copy per column: 784 byte columns x 5 chunks were 3 920 submissions of 192 KiB each (27 GB/s); a run is one.
+// of one copy per column: 784 byte columns x 5 chunks would be 3 920 small submissions; a run is one.
 int copy_cols(char *dev_base, int64_t dev_pitch, const void *const *host_cols, int64_t host_off, size_t bytes, int32_t k,
               bool to_device, cudaStream_t s) {
     for (int32_t j = 0; j < k;) {

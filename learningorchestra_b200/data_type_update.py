@@ -13,7 +13,7 @@ methods, in-place conversion of the input collection, same ``finished`` False ->
 * ``"string"`` (``data_type_update.py:22-28``): ``str(v)`` / ``None -> ""`` is text formatting of Python
   objects in the document adapter and stays on the host (SURVEY.md §8a row a5: out of the GPU's scope).
 * ``"float32"`` (this build's optional extension): the B-semantics cast of SURVEY.md §0 — numeric values
-  go through the sm_100a kernel (fp64 -> fp32 round-to-nearest-even) and are stored back widened.
+  go through the sm_90a kernel (fp64 -> fp32 round-to-nearest-even) and are stored back widened.
 """
 from __future__ import annotations
 

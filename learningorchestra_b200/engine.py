@@ -1,7 +1,7 @@
 """Engine — the handle the reference's ``spark_session`` slot receives in this build.
 
 Thin object layer over the C ABI (``include/loexec.h``): device-resident columnar tables and the
-projection / cast / histogram entry points.  All computation happens in libloexec's sm_100a
+projection / cast / histogram entry points.  All computation happens in libloexec's sm_90a
 kernels; nothing here falls back to numpy.
 
 Reference boundary this replaces: ``projection_image/server.py:51-69`` builds a ``SparkSession``
@@ -157,7 +157,7 @@ class DeviceTable:
 
 
 class Engine:
-    """One libloexec context = one B200.  ``Engine(device)`` raises LoexecError without a GPU."""
+    """One libloexec context = one H100.  ``Engine(device)`` raises LoexecError without a GPU."""
 
     def __init__(self, device: int = 0):
         self._lib = N.load()

@@ -8,7 +8,7 @@ Reference job (``projection.py:32-48``): Spark loads the input collection, drops
   adapter — there is no arithmetic to put on a GPU, and the values must come back untouched (strings
   included).
 * ``cast_to="float32"`` (this build's optional extension, REST key ``castTo``): the selected columns must
-  be numeric; they go through the fused sm_100a kernel (projection + fp64->fp32 RNE cast, and with
+  be numeric; they go through the fused sm_90a kernel (projection + fp64->fp32 RNE cast, and with
   ``bins`` a fixed-width histogram in the same pass) via ``lo_project_cast_hist_host``.
 """
 from __future__ import annotations

@@ -188,7 +188,7 @@ def main() -> None:
     from .sharding import open_engine
 
     devs = os.environ.get("LOEXEC_DEVICES") or os.environ.get("LOEXEC_DEVICE")
-    engine = open_engine([int(d) for d in devs.split(",")] if devs else None)       # fails loudly without a B200
+    engine = open_engine([int(d) for d in devs.split(",")] if devs else None)       # fails loudly without an H100
     app = create_app(None, engine)
     run_simple(os.environ.get("LOEXEC_HOST", "127.0.0.1"), int(os.environ.get("LOEXEC_PORT", "5001")), app, threaded=True)
 

@@ -115,7 +115,7 @@ class GroupCounts:
 
 
 class ShardedEngine:
-    """Several B200s behind the same methods as :class:`~learningorchestra_b200.engine.Engine`.
+    """Several H100s behind the same methods as :class:`~learningorchestra_b200.engine.Engine`.
 
     Everything multi-GPU lives in the library (``lo_group_*`` in ``include/loexec.h``): the peer mappings, the
     in-kernel merge of the partial histograms over NVLink, the NCCL fallback.  This class only forms the group and

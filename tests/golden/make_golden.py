@@ -1,9 +1,9 @@
 """Generates the R-semantics golden fixtures by EXECUTING THE REFERENCE'S OWN FILES
 (``data_type_update.py`` and ``histogram.py`` import only the stdlib) against the in-memory
-``MemoryDatabase`` of oracle/rsem.py.  Needs /root/reference, which exists only in the build
-container; the JSON it writes is committed and is all the tests read.
+``MemoryDatabase`` of oracle/rsem.py.  Needs a checkout of the upstream learningOrchestra repository;
+the JSON it writes is committed and is all the tests read.
 
-    python tests/golden/make_golden.py
+    python tests/golden/make_golden.py /path/to/learningOrchestra
 
 What is pinned by the reference's code itself: the per-document cast (every branch of
 ``DataType.field_converter``), the ``finished`` flag protocol, the histogram result-document shape.
@@ -16,7 +16,7 @@ from pathlib import Path
 
 HERE = Path(__file__).resolve().parent
 ROOT = HERE.parent.parent
-REF = Path("/root/reference/microservices")
+REF = Path(sys.argv[1] if len(sys.argv) > 1 else ".") / "microservices"
 sys.path.insert(0, str(ROOT))
 
 from oracle import rsem  # noqa: E402
@@ -48,7 +48,7 @@ class MetadataStandIn:
 
 def main():
     if not REF.exists():
-        raise SystemExit("/root/reference is not mounted: fixtures can only be regenerated in the build container")
+        raise SystemExit(f"{REF} not found: pass the path of a learningOrchestra checkout")
     dtu = load_reference(REF / "data_type_handler_image" / "data_type_update.py", "ref_data_type_update")
     hst = load_reference(REF / "histogram_image" / "histogram.py", "ref_histogram")
 

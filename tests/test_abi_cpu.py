@@ -1,4 +1,4 @@
-"""CPU: libloexec.so builds for sm_100a, loads, and exports exactly what include/loexec.h declares.
+"""CPU: libloexec.so builds for sm_90a, loads, and exports exactly what include/loexec.h declares.
 No compute calls are made here (there is no GPU and no CPU fallback)."""
 import ctypes
 import re
@@ -27,13 +27,13 @@ def test_every_declared_symbol_is_exported_and_bound(built):
     assert lib.lo_abi_version() == _native.LO_ABI_VERSION
 
 
-def test_library_is_sm100a_native_code(built):
+def test_library_is_sm90a_native_code(built):
     from learningorchestra_b200 import _native
     out = subprocess.run(["cuobjdump", "-lelf", str(_native.LIB_PATH)], capture_output=True, text=True).stdout
-    assert "sm_100a" in out, out
+    assert "sm_90a" in out, out
     full = subprocess.run(["cuobjdump", "-sass", str(_native.LIB_PATH)], capture_output=True, text=True).stdout
     sass = full.split("Function : _ZN2lo19k_project_cast_histILi1ELb1ELb1ELb1EEE")[1].split("Function :")[0]
-    assert "LDG.E.NA.EFL2.256" in sass or "LDG.E" in sass      # 256-bit streaming loads
+    assert "LDG.E.NA.128" in sass                               # 128-bit streaming loads
     assert "STS.U8" in sass and "LDS.U8" in sass                # private byte-counter histogram, no ATOMS
     assert "ATOMS" not in sass
     assert "RED.E.ADD.64.STRONG.SYS" in sass or "REDG.E.ADD.64.STRONG.SYS" in sass    # in-kernel merge: pushes at system scope
@@ -43,7 +43,7 @@ def test_library_is_sm100a_native_code(built):
 def test_lane_slot_kernels_issue_one_shared_atomic_per_element(built):
     """The shipped byte-histogram kernel is the lane-slot form: per 64 input bytes 64 PRMT (the counter address straight from
     the input word) and 64 shared-memory atomics with the reserved-smem base in the immediate, 128-bit streaming loads, a
-    RED.64 flush; the wide-bin kernel counts with shared atomics too and keeps the 256-bit loads."""
+    RED.64 flush; the wide-bin kernel counts with shared atomics too and streams with 128-bit loads."""
     from learningorchestra_b200 import _native
     sass = subprocess.run(["cuobjdump", "-sass", str(_native.LIB_PATH)], capture_output=True, text=True).stdout
     lanes = sass.split("Function : _ZN2lo20k_hist_u8_cols_lanesILi2EEE")[1].split("Function :")[0]
@@ -53,7 +53,7 @@ def test_lane_slot_kernels_issue_one_shared_atomic_per_element(built):
     assert "LDS.U8" not in lanes and "STS.U8" not in lanes
     assert "REDG.E.ADD.64.STRONG.GPU" in lanes or "RED.E.ADD.64.STRONG.GPU" in lanes
     bins = sass.split("Function : _ZN2lo24k_project_cast_hist_binsILi1ELb1EEE")[1].split("Function :")[0]
-    assert "ATOMS" in bins and "F2F.F32.F64" in bins and ".256" in bins
+    assert "ATOMS" in bins and "F2F.F32.F64" in bins and "LDG.E.NA.128" in bins
 
 
 def test_tma_variant_is_compiled_with_bulk_copy_and_mbarriers(built):
