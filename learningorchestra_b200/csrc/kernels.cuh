@@ -14,16 +14,14 @@
 //     (opt-in).
 //   * histogram = PRIVATE PER-THREAD BYTE COUNTERS in shared memory, laid out so that thread t only ever
 //     touches bank (t % 32): word w of thread t lives at smem word w*kThreads + t.  Increment = plain
-//     LDS.U8 / IADD / STS.U8 (f64 kernel) or one ATOMS.ADD on the containing word (byte kernel) — no bank
-//     conflicts, and the cost is independent of the value distribution (a constant column is as fast as a
-//     uniform one).  A thread handles <= 255 elements per tile so a byte never wraps; the CTA then folds the 256
-//     private histograms (LDS.128, packed 16-bit adds, a transposing warp butterfly) and issues one RED.64 per
-//     non-empty bin.
-//   * byte columns (k_hist_u8_cols_lanes, the shipped K4) and histograms of more than 256 bins
-//     (k_project_cast_hist_bins) drop the byte fields: 32-bit counters in lane slots shared by the CTA's warps, bank =
-//     lane, the counter address one PRMT (bytes) or one shift-add (bins) away from the value, ONE ATOMS per element, a
-//     CTA streams a long chunk of its column and folds once.  The per-thread byte-counter variants of K4
-//     (k_hist_u8_cols<ALIGNED, MODE>) stay behind LOEXEC_U8_MODE as alternatives (DESIGN.md §3.4).
+//     LDS.U8 / IADD / STS.U8 — no bank conflicts, and the cost is independent of the value distribution (a
+//     constant column is as fast as a uniform one).  A thread handles <= 255 elements per tile so a byte never
+//     wraps; the CTA then folds the 256 private histograms (LDS.128, packed 16-bit adds, a transposing warp
+//     butterfly) and issues one RED.64 per non-empty bin.
+//   * byte columns (K4, k_hist_u8_cols_lanes) and histograms of more than 256 bins (k_project_cast_hist_bins) drop
+//     the byte fields: 32-bit counters in lane slots shared by the CTA's warps, bank = lane, the counter address one
+//     PRMT (bytes) or one shift-add (bins) away from the value, ONE ATOMS per element, a CTA streams a long chunk of
+//     its column and folds once.
 //   * several GPUs (GroupStep): the bins go to the device's own matrix; the CTA finishing a column's last tile pushes
 //     the column to the root GPU with system-scope RED.64 over NVLink, the last pusher arrives, the root's last CTA
 //     moves the merged matrix out — merge, arrival and epilogue ride inside the one streaming launch per step.
@@ -65,11 +63,8 @@ constexpr int kPfBuf     = LO_PF_NBUF;
 constexpr int kPfBatches = kVecPerThread / kPfBatch;
 static_assert(kVecPerThread % kPfBatch == 0 && kPfBatches % kPfBuf == 0, "pipeline shape must tile the 60 vectors");
 
-constexpr int kU8VecBytes   = 16;
-constexpr int kU8Batch      = 5;
-constexpr int kU8Batches    = 3;
-constexpr int kU8ElemsPerThread = kU8VecBytes * kU8Batch * kU8Batches;  // 240
-constexpr int kU8TileRows   = kThreads * kU8ElemsPerThread;             // 61440
+constexpr int kU8VecBytes      = 16;
+constexpr int kU8HostChunkRows = 61440;   // row granularity of the *_host byte pipeline's chunks
 
 constexpr int kMaxColsF64   = 128;   // projected columns per launch (by-value kernel parameter)
 constexpr int kMaxColsU8    = 1024;
@@ -85,9 +80,6 @@ struct ColsF64 {
 
 struct ColsU8 {
     int32_t k;
-    // powers of two handed to the kernel as DATA (constant bank): ptxas cannot strength-reduce a multiply by them into
-    // LEA / SHF, so the shift-and-add stays an IMAD / IMAD.HI on the FMA pipe (k_hist_u8_cols mode 6)
-    uint32_t p8, p11, p16, p19, p24, p27, p3;
     int32_t col[kMaxColsU8];
 };
 
@@ -876,469 +868,9 @@ k_project_cast_hist_tma(const char *__restrict__ in_base, long long in_pitch,
 }
 
 // ---------------------------------------------------------------------------------------------
-// K4: per-column 256-bin value counts of byte columns
-// ---------------------------------------------------------------------------------------------
-// How one byte becomes a counter update (template parameter MODE of k_hist_u8_cols; LOEXEC_U8_MODE picks at launch):
-//   2: two LDS.U8 / IADD / STS.U8 round trips per 16-bit pair (bump2), no atomics
-//   4: ONE conflict-free ATOMS.ADD per byte on the 32-bit word holding the counter, offsets / shifts pulled out
-//      of the input word with PRMT (ALU-pipe bound)
-//   5: like 4, per-byte arithmetic written as masks + multiply-adds (ptxas turns the constant multiplies into
-//      LEA.HI / IMAD.SHL and balances the two integer pipes itself)
-//   7: the counter word's whole shared-memory address from ONE PRMT (thread bits pre-merged into the row bytes), the
-//      field value from one wrap-mode funnel shift, the run test once per 80-byte batch: ~4.7 instead of ~6.3
-//      instructions per byte
-//   11: k_hist_u8_cols_lanes — 32-bit counters in 64 lane slots shared by all warps of the CTA: one PRMT + one ATOMS per
-//       byte (shipped; 12-14: its measurement variants)
-//   8 / 9: k_hist_u8_cols_wide<2 / 4> — mode 7's arithmetic with 512 / 1024 threads per CTA, two / four threads per
-//      private histogram (48 / 64 warps per SM)
-//   6: like 5 with the powers of two passed as kernel DATA so the shift-and-adds stay IMAD / IMAD.HI on the FMA
-//      pipe and only the masks and the final 1 << n are ALU-pipe work
-#ifndef LO_U8_MODE_DEFAULT
-#define LO_U8_MODE_DEFAULT 11
-#endif
-
-// two increments with overlapped latencies (one compare instead of bump4's six)
-__device__ __forceinline__ void bump2(uint8_t *priv, uint32_t b0, uint32_t b1) {
-    uint8_t *p0 = priv + bin_byte_offset(b0), *p1 = priv + bin_byte_offset(b1);
-    uint32_t c0 = *p0, c1 = *p1;
-    c0 += 1;
-    c1 += 1 + (b1 == b0);
-    *p0 = (uint8_t)c0;
-    *p1 = (uint8_t)c1;
-}
-
-__device__ __forceinline__ uint32_t mad_lo(uint32_t a, uint32_t b, uint32_t c) {
-    uint32_t d;
-    asm("mad.lo.u32 %0, %1, %2, %3;" : "=r"(d) : "r"(a), "r"(b), "r"(c));
-    return d;
-}
-__device__ __forceinline__ uint32_t mad_hi(uint32_t a, uint32_t b, uint32_t c) {
-    uint32_t d;
-    asm("mad.hi.u32 %0, %1, %2, %3;" : "=r"(d) : "r"(a), "r"(b), "r"(c));
-    return d;
-}
-__device__ __forceinline__ uint32_t one_shl_wrap(uint32_t n) {       // 1 << (n & 31): SHF.L.W, no clamp code
-    uint32_t d;
-    asm("shf.l.wrap.b32 %0, %1, %2, %3;" : "=r"(d) : "r"(0u), "r"(1u), "r"(n));
-    return d;
-}
-// no return value: the shared-memory atomic is fire-and-forget (a lane-private bank, so conflict-free; a byte field
-// cannot carry into its neighbour because a thread adds at most 240 per tile)
-__device__ __forceinline__ void atoms_add(uint32_t addr, uint32_t v) {
-    asm volatile("red.shared.add.u32 [%0], %1;" :: "r"(addr), "r"(v) : "memory");
-}
-
-// shared-window address at which a block's dynamic shared memory starts when the kernel has no static shared memory:
-// the 1 KiB sm_90 reserves per block (lo_init checks the size).  Mode 7 puts it in the atomics' immediate offset; the kernel traps if it is wrong.
-#define LO_SMEM_WINDOW_BASE 1024
-__device__ __forceinline__ void atoms_add_base(uint32_t offset, uint32_t v) {
-    asm volatile("red.shared.add.u32 [%0+1024], %1;" :: "r"(offset), "r"(v) : "memory");
-}
-static_assert(LO_SMEM_WINDOW_BASE == 1024, "keep the immediate in atoms_add_base in sync");
-
-__device__ __forceinline__ uint32_t mul_wide_hi(uint32_t a, uint32_t b) {       // (a * b) >> 32 through IMAD.WIDE.U32
-    unsigned long long d;
-    asm("mul.wide.u32 %0, %1, %2;" : "=l"(d) : "r"(a), "r"(b));
-    return (uint32_t)(d >> 32);
-}
-
-struct U8Consts { uint32_t p8, p11, p16, p19, p24, p27, p3; };
-
-template <int MODE>
-__device__ __forceinline__ void bump_word(uint8_t *priv, uint32_t x, const U8Consts &K) {
-    if (MODE == 2) {
-        bump2(priv, x & 0xFFu, (x >> 8) & 0xFFu);
-        bump2(priv, (x >> 16) & 0xFFu, x >> 24);
-    } else if (MODE == 4) {
-        // the four word-row offsets and the four field shifts of a 32-bit word of input computed together
-        // (two LOP3 + one SHL for four bytes) and pulled apart with PRMT straight into position
-        const uint32_t rows   = x & 0xFCFCFCFCu;            // byte q: (b_q & 0xFC)   -> word-row offset / 256
-        const uint32_t shifts = (x & 0x03030303u) << 3;     // byte q: (b_q & 3) * 8  -> bit position of the counter
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-            const uint32_t off = __byte_perm(rows, 0u, 0x4404u | (uint32_t)(q << 4));     // byte q moved to bits 8..15
-            const uint32_t sh  = __byte_perm(shifts, 0u, 0x4440u | (uint32_t)q);          // byte q moved to bits 0..7
-            atomicAdd(reinterpret_cast<uint32_t *>(priv + off), 1u << sh);
-        }
-    } else if (MODE == 7 || MODE == 10) {
-        // The counter word's offset inside the histogram in ONE PRMT.  The word of thread t for byte value b is at
-        // (b >> 2) * 1024 + 4 * t from the start of the dynamic shared memory, i.e. byte by byte
-        //     [ (4t) & 0xFF | (b & 0xFC) + ((4t) >> 8) | 0 | 0 ];
-        // `rows` carries (b_q & 0xFC) | ((4t) >> 8) in byte q (K.p8 = ((4t) >> 8) * 0x01010101), so PRMT(rows, 4t) takes
-        // byte q of rows as byte 1 and bytes 0, 2, 3 from 4t.  The start of the dynamic shared memory in the shared
-        // window — kSmemWindowBase, the 1 KiB the system reserves per block on sm_90; checked at kernel start — rides
-        // in the atomic's immediate offset, so no add is needed either.  The field value 1 << 8 * (b & 3) is a
-        // wrap-mode funnel shift (reads only bits 0..4 of the count); its count for byte 0 needs no extraction.
-        const uint32_t t4 = K.p3;                                                   // 4 * t
-        const uint32_t rows   = (x & 0xFCFCFCFCu) | K.p8;
-        const uint32_t shifts = (x & 0x03030303u) << 3;
-        if (MODE == 10) {
-            // mode 10: the three count extractions as the HIGH word of a widening multiply by 2^24 / 2^16 / 2^8 held as
-            // DATA (so ptxas cannot turn them back into SHF): FMA pipe instead of ALU pipe
-            // (the ALU pipe's 64 lane-ops per clock per SM, not the atomics, is what the per-byte arithmetic runs into)
-            atoms_add_base(__byte_perm(rows, t4, 0x7604u), one_shl_wrap(shifts));
-            atoms_add_base(__byte_perm(rows, t4, 0x7614u), one_shl_wrap(mul_wide_hi(shifts, K.p24)));
-            atoms_add_base(__byte_perm(rows, t4, 0x7624u), one_shl_wrap(mul_wide_hi(shifts, K.p16)));
-            atoms_add_base(__byte_perm(rows, t4, 0x7634u), one_shl_wrap(mul_wide_hi(shifts, K.p11)));
-        } else {
-            atoms_add_base(__byte_perm(rows, t4, 0x7604u), one_shl_wrap(shifts));       // byte 0 of x
-            atoms_add_base(__byte_perm(rows, t4, 0x7614u), one_shl_wrap(shifts >> 8));
-            atoms_add_base(__byte_perm(rows, t4, 0x7624u), one_shl_wrap(shifts >> 16));
-            atoms_add_base(__byte_perm(rows, t4, 0x7634u), one_shl_wrap(shifts >> 24));
-        }
-    } else {
-        // counter word of byte q (value b): priv + (b >> 2) * 1024; field at bit 8 * (b & 3).  Address =
-        // (x & mask_q) * 2^s + priv, shift count = (x & 0x03030303) moved to bits 3..4 (SHF.L.W reads bits 0..4 only)
-        const uint32_t ps = (uint32_t)__cvta_generic_to_shared(priv);
-        const uint32_t m  = x & 0x03030303u;
-        const uint32_t p8 = MODE == 6 ? K.p8 : 256u, p24 = MODE == 6 ? K.p24 : 1u << 24, p16 = MODE == 6 ? K.p16 : 1u << 16;
-        const uint32_t p3 = MODE == 6 ? K.p3 : 8u, p27 = MODE == 6 ? K.p27 : 1u << 27, p19 = MODE == 6 ? K.p19 : 1u << 19;
-        const uint32_t p11 = MODE == 6 ? K.p11 : 1u << 11;
-        const uint32_t a0 = mad_lo(x & 0x000000FCu, p8, ps);
-        const uint32_t a1 = (x & 0x0000FC00u) + ps;
-        const uint32_t a2 = mad_hi(x & 0x00FC0000u, p24, ps);
-        const uint32_t a3 = mad_hi(x & 0xFC000000u, p16, ps);
-        const uint32_t s0 = mad_lo(m, p3, 0u);             // m << 3
-        const uint32_t s1 = mad_hi(m, p27, 0u);            // m >> 5   (bits 3..4 = b1 & 3, bits 0..2 = 0)
-        const uint32_t s2 = mad_hi(m, p19, 0u);            // m >> 13
-        const uint32_t s3 = mad_hi(m, p11, 0u);            // m >> 21
-        atoms_add(a0, one_shl_wrap(s0));
-        atoms_add(a1, one_shl_wrap(s1));
-        atoms_add(a2, one_shl_wrap(s2));
-        atoms_add(a3, one_shl_wrap(s3));
-    }
-}
-
-// mode 7: the run test is taken once per BATCH of kU8Batch vectors (80 bytes per thread) instead of once per vector:
-// a constant column passes it for every batch, a mixed column pays 0.2 instead of 0.5 instructions per byte for it
-template <int MODE>
-__device__ __forceinline__ uint32_t bump_batch(uint8_t *priv, const uint4 (&v)[kU8Batch], const U8Consts &K) {
-    const uint32_t splat = __byte_perm(v[0].x, 0, 0x0000);
-    uint32_t diff = 0u;
-#pragma unroll
-    for (int u = 0; u < kU8Batch; ++u) diff |= (v[u].x ^ splat) | (v[u].y ^ splat) | (v[u].z ^ splat) | (v[u].w ^ splat);
-    if (__all_sync(__activemask(), diff == 0u)) {
-        uint8_t *p = priv + bin_byte_offset(v[0].x & 0xFFu);
-        *p = (uint8_t)(*p + 16 * kU8Batch);
-        return 0u;
-    }
-#pragma unroll
-    for (int u = 0; u < kU8Batch; ++u) {
-        bump_word<MODE>(priv, v[u].x, K); bump_word<MODE>(priv, v[u].y, K);
-        bump_word<MODE>(priv, v[u].z, K); bump_word<MODE>(priv, v[u].w, K);
-    }
-    return 1u;
-}
-
-// one 16-byte vector.  Run fast path: when every ACTIVE lane of the warp holds sixteen equal bytes
-// (constant columns: image borders, flags, padding) the whole vector is one counter += 16.  The vote
-// only keeps the branch warp-uniform (mixed data never executes both sides); correctness does not
-// depend on it, so it is taken over __activemask() — the ragged last tile runs with partial warps and a
-// full-mask vote there would wait forever for lanes that already left the loop.
-template <int MODE>
-__device__ __forceinline__ void bump_vec16(uint8_t *priv, const uint4 &v, const U8Consts &K) {
-    const uint32_t splat = __byte_perm(v.x, 0, 0x0000);
-    const bool run = (v.x == splat) & (v.y == splat) & (v.z == splat) & (v.w == splat);
-    if (__all_sync(__activemask(), run)) {
-        uint8_t *p = priv + bin_byte_offset(v.x & 0xFFu);
-        *p = (uint8_t)(*p + 16);
-        return;
-    }
-    bump_word<MODE>(priv, v.x, K); bump_word<MODE>(priv, v.y, K);
-    bump_word<MODE>(priv, v.z, K); bump_word<MODE>(priv, v.w, K);
-}
-
-template <bool ALIGNED, int MODE>
-__global__ void __launch_bounds__(kThreads, 3)
-k_hist_u8_cols(const uint8_t *__restrict__ in_base, long long in_pitch, long long nrows,
-               unsigned tiles_per_col, unsigned long long *__restrict__ counts,
-               const __grid_constant__ ColsU8 P, const __grid_constant__ GroupStep G) {
-    extern __shared__ uint32_t smem[];
-    if (G.overlap) asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-    const unsigned j    = blockIdx.x / tiles_per_col;
-    const unsigned tile = blockIdx.x - j * tiles_per_col;
-    const long long r0  = (long long)tile * kU8TileRows;
-    const long long n   = min((long long)kU8TileRows, nrows - r0);
-    const uint8_t *in   = in_base + (long long)P.col[j] * in_pitch + r0;
-    uint8_t *priv = reinterpret_cast<uint8_t *>(smem) + 4 * threadIdx.x;
-    U8Consts K = {P.p8, P.p11, P.p16, P.p19, P.p24, P.p27, P.p3};
-    if (MODE == 7 || MODE == 10) {
-        if ((uint32_t)__cvta_generic_to_shared(smem) != LO_SMEM_WINDOW_BASE) __trap();    // mode 7's immediate offset
-        K.p11 = K.p8;                              // 2^8 as data (mode 10's >> 24)
-        K.p3 = 4u * threadIdx.x;
-        K.p8 = ((4u * threadIdx.x) >> 8) * 0x01010101u;
-    }
-    if (ALIGNED && n == kU8TileRows) {
-        // full tile: batch b+1's five 16-byte loads are in flight while batch b is being counted (register double
-        // buffer, as in the f64 kernel; without it every warp idles on its own loads between batches).  The first
-        // batch is requested BEFORE the counters are cleared, so its DRAM latency overlaps the clearing and its barrier.
-        uint4 v[2][kU8Batch];
-        const uint8_t *src = in + (long long)threadIdx.x * kU8VecBytes;
-#pragma unroll
-        for (int u = 0; u < kU8Batch; ++u) v[0][u] = ldg128_stream(src + (long long)u * kThreads * kU8VecBytes);
-        zero_private(smem, kHistRows);
-        uint32_t mixed = 0u, first = 0u;          // MODE 7: did any batch of this thread leave the run path / its first byte
-#pragma unroll
-        for (int b = 0; b < kU8Batches; ++b) {
-            if (b + 1 < kU8Batches) {
-#pragma unroll
-                for (int u = 0; u < kU8Batch; ++u)
-                    v[(b + 1) & 1][u] = ldg128_stream(src + (long long)((b + 1) * kU8Batch + u) * kThreads * kU8VecBytes);
-            }
-            if (MODE == 7 || MODE == 10) {
-                if (b == 0) first = v[0][0].x & 0xFFu;
-                mixed |= bump_batch<MODE>(priv, v[b & 1], K) | ((v[b & 1][0].x & 0xFFu) ^ first);
-            } else {
-#pragma unroll
-                for (int u = 0; u < kU8Batch; ++u) bump_vec16<MODE>(priv, v[b & 1][u], K);
-            }
-        }
-        if (MODE == 7 || MODE == 10) {
-            // Constant tile (image borders, flags, padding: every byte of the 61 440 equal): nothing to fold — one RED
-            // of the tile's row count.  CTA-uniform decision: every thread stayed on the run path with one value of
-            // its own, then all those values are compared through one word of the (not yet used) fold scratch.
-            uint32_t *scratch = smem + kHistRows * kThreads;
-            if (__syncthreads_and(mixed == 0u)) {
-                if (threadIdx.x == 0) *scratch = first;
-                __syncthreads();
-                if (__syncthreads_and(first == *scratch)) {
-                    if (G.mode != 0) group_wait_generation(G);
-                    unsigned long long *dst = (G.mode == 0 ? counts : G.local) + (long long)j * 256 + first;
-                    if (threadIdx.x == 0)
-                        asm volatile("red.relaxed.gpu.global.add.u64 [%0], %1;" :: "l"(dst), "l"((unsigned long long)kU8TileRows) : "memory");
-                    if (G.mode != 0) group_finish_column(G, j, 256, P.k, tiles_per_col, smem);
-                    return;
-                }
-            }
-        }
-    } else if (ALIGNED) {
-        zero_private(smem, kHistRows);
-#pragma unroll 1
-        for (int b = 0; b < kU8Batches; ++b) {
-            const long long e0 = ((long long)b * kU8Batch * kThreads + threadIdx.x) * kU8VecBytes;
-            if (e0 >= n) break;
-            if (e0 + (long long)(kU8Batch - 1) * kThreads * kU8VecBytes + kU8VecBytes <= n) {
-                uint4 v[kU8Batch];
-#pragma unroll
-                for (int u = 0; u < kU8Batch; ++u) v[u] = ldg128_stream(in + e0 + (long long)u * kThreads * kU8VecBytes);
-#pragma unroll
-                for (int u = 0; u < kU8Batch; ++u) bump_vec16<(MODE == 7 || MODE == 10) ? 4 : MODE>(priv, v[u], K);
-            } else {
-                // the batch straddles the end of the column: whole 16-byte vectors still go through the vector path
-                // (all loads of the batch in flight together), only the last partial vector is read byte by byte.
-                // bump_vec16's warp vote is taken over the active lanes, so the divergence here is safe.
-                uint4 v[kU8Batch];
-                bool whole[kU8Batch];
-#pragma unroll
-                for (int u = 0; u < kU8Batch; ++u) {
-                    const long long e = e0 + (long long)u * kThreads * kU8VecBytes;
-                    whole[u] = e + kU8VecBytes <= n;
-                    if (whole[u]) v[u] = ldg128_stream(in + e);
-                }
-#pragma unroll
-                for (int u = 0; u < kU8Batch; ++u) {
-                    const long long e = e0 + (long long)u * kThreads * kU8VecBytes;
-                    if (whole[u]) {
-                        bump_vec16<(MODE == 7 || MODE == 10) ? 4 : MODE>(priv, v[u], K);
-                    } else if (e < n) {
-#pragma unroll 1
-                        for (int q = 0; q < kU8VecBytes && e + q < n; ++q) bump(priv, ldg8_stream(in + e + q));
-                    }
-                }
-            }
-        }
-    } else {
-        zero_private(smem, kHistRows);
-#pragma unroll 1
-        for (int i = 0; i < kU8ElemsPerThread; ++i) {
-            const long long e = (long long)i * kThreads + threadIdx.x;
-            if (e >= n) break;
-            bump(priv, ldg8_stream(in + e));
-        }
-    }
-    if (G.mode == 0) {
-        fold_and_flush(smem, kHistRows, 256, counts + (long long)j * 256);
-    } else {
-        group_wait_generation(G);
-        fold_and_flush(smem, kHistRows, 256, G.local + (long long)j * 256);
-        group_finish_column(G, j, 256, P.k, tiles_per_col, smem);
-    }
-}
-
-// ---------------------------------------------------------------------------------------------
-// K4, wide form (LOEXEC_U8_MODE=8): 512 threads per CTA, TWO threads per private histogram.
-// The 256-thread kernel is latency-bound at the 24 warps per SM its 256 B of counters per thread allow (no pipe
-// saturated).  Increments are shared-memory atomics anyway, so threads t and t + 256 —
-// different warps, same lane, hence the same private bank and still conflict-free inside every warp — can share one
-// histogram as long as the two together stay below 256 elements per tile: 7 vectors of 16 bytes each (2 x 112 = 224).
-// Same shared memory per CTA, twice the warps (48 per SM), half the registers per thread (<= 40).
-// ---------------------------------------------------------------------------------------------
-// TPH = threads per private histogram: 2 -> 512 threads x 7 vectors (224 elements per histogram), 3 CTAs / SM, 48 warps;
-//                                       4 -> 1024 threads x 3 vectors (192 elements), 2 CTAs / SM, 64 warps (<= 32 registers)
-template <int TPH> struct U8Wide {
-    static constexpr int kThreadsW  = 256 * TPH;
-    static constexpr int kVecs      = TPH == 2 ? 7 : 3;
-    static constexpr int kVecsA     = TPH == 2 ? 4 : 3;                       // first batch
-    static constexpr int kVecsB     = kVecs - kVecsA;                         // second batch (0 for TPH = 4)
-    static constexpr int kMinCtas   = TPH == 2 ? 3 : 2;
-    static constexpr int kTileRows  = kThreadsW * kVecs * kU8VecBytes;        // 57 344 / 49 152 bytes of one column
-    static_assert(TPH * kVecs * kU8VecBytes <= 255, "a byte counter must not wrap");
-};
-constexpr int kU8WTileRows2 = U8Wide<2>::kTileRows, kU8WTileRows4 = U8Wide<4>::kTileRows;
-
-// one run-tested batch of NV vectors for the shared-histogram kernel: everything is an atomic (the partner thread
-// may be updating the same word)
-template <int NV>
-__device__ __forceinline__ uint32_t bump_batch_shared(const uint4 (&v)[NV], uint32_t t4, uint32_t tidhi4) {
-    const uint32_t splat = __byte_perm(v[0].x, 0, 0x0000);
-    uint32_t diff = 0u;
-#pragma unroll
-    for (int u = 0; u < NV; ++u) diff |= (v[u].x ^ splat) | (v[u].y ^ splat) | (v[u].z ^ splat) | (v[u].w ^ splat);
-    if (__all_sync(__activemask(), diff == 0u)) {
-        const uint32_t b = v[0].x & 0xFFu;
-        atoms_add_base(((b & 0xFCu) << 8) | t4, (uint32_t)(16 * NV) << ((b & 3u) << 3));
-        return 0u;
-    }
-#pragma unroll
-    for (int u = 0; u < NV; ++u) {
-        const uint32_t w[4] = {v[u].x, v[u].y, v[u].z, v[u].w};
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-            const uint32_t rows   = (w[q] & 0xFCFCFCFCu) | tidhi4;
-            const uint32_t shifts = (w[q] & 0x03030303u) << 3;
-            atoms_add_base(__byte_perm(rows, t4, 0x7604u), one_shl_wrap(shifts));
-            atoms_add_base(__byte_perm(rows, t4, 0x7614u), one_shl_wrap(shifts >> 8));
-            atoms_add_base(__byte_perm(rows, t4, 0x7624u), one_shl_wrap(shifts >> 16));
-            atoms_add_base(__byte_perm(rows, t4, 0x7634u), one_shl_wrap(shifts >> 24));
-        }
-    }
-    return 1u;
-}
-
-// fold for NW = 16 or 32 warps: warp wp owns rows wp, wp + NW, ... (64 / NW rows -> R = 128 / NW packed registers);
-// transposing butterfly over the top log2(R) lane bits, plain butterfly over the rest
-template <int NW>
-__device__ __forceinline__ void fold_and_flush_wide(uint32_t *smem, unsigned long long *counts) {
-    constexpr int kRowsPerWarp = kHistRows / NW, R = 2 * kRowsPerWarp;        // NW 16 -> 4 rows, R 8 ; NW 32 -> 2 rows, R 4
-    uint32_t *folded = smem + kHistRows * kThreads;   // 256 words
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    __syncthreads();
-    uint32_t r[R];
-#pragma unroll
-    for (int i = 0; i < kRowsPerWarp; ++i) {
-        const int w = warp + NW * i;
-        const uint4 a = *reinterpret_cast<const uint4 *>(smem + w * kThreads + 4 * lane);
-        const uint4 b = *reinterpret_cast<const uint4 *>(smem + w * kThreads + 128 + 4 * lane);
-        const uint32_t x[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
-        uint32_t even = 0u, odd = 0u;
-#pragma unroll
-        for (int q = 0; q < 8; ++q) {
-            even += x[q] & 0x00FF00FFu;
-            odd  += __byte_perm(x[q], 0u, 0x4341u);
-        }
-        r[2 * i] = even;
-        r[2 * i + 1] = odd;
-    }
-    int bit = 16;
-#pragma unroll
-    for (int half = R / 2; half >= 1; half >>= 1, bit >>= 1) {
-        const bool upper = (lane & bit) != 0;
-#pragma unroll
-        for (int i = 0; i < half; ++i) {
-            const uint32_t send = upper ? r[i] : r[i + half];
-            const uint32_t keep = upper ? r[i + half] : r[i];
-            r[i] = keep + __shfl_xor_sync(0xffffffffu, send, bit);
-        }
-    }
-    uint32_t total = r[0];
-    constexpr int kPlainBits = 32 / R;                   // lanes that still hold partial sums of the same register
-#pragma unroll
-    for (int s2 = kPlainBits / 2; s2 >= 1; s2 >>= 1) total += __shfl_xor_sync(0xffffffffu, total, s2);
-    if ((lane & (kPlainBits - 1)) == 0) {
-        const int idx = (lane / kPlainBits) & (R - 1);
-        const int w = warp + NW * (idx >> 1), parity = idx & 1;
-        folded[4 * w + parity]     = total & 0xFFFFu;
-        folded[4 * w + 2 + parity] = total >> 16;
-    }
-    __syncthreads();
-    if (threadIdx.x < 256) {
-        const uint32_t c = folded[threadIdx.x];
-        if (c) asm volatile("red.relaxed.gpu.global.add.u64 [%0], %1;" :: "l"(counts + threadIdx.x), "l"((unsigned long long)c) : "memory");
-    }
-}
-
-template <int TPH>
-__global__ void __launch_bounds__(U8Wide<TPH>::kThreadsW, U8Wide<TPH>::kMinCtas)
-k_hist_u8_cols_wide(const uint8_t *__restrict__ in_base, long long in_pitch, long long nrows,
-                    unsigned tiles_per_col, unsigned long long *__restrict__ counts,
-                    const __grid_constant__ ColsU8 P, const __grid_constant__ GroupStep G) {
-    using W = U8Wide<TPH>;
-    extern __shared__ uint32_t smem[];
-    if (G.overlap) asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-    const unsigned j    = blockIdx.x / tiles_per_col;
-    const unsigned tile = blockIdx.x - j * tiles_per_col;
-    const long long r0  = (long long)tile * W::kTileRows;
-    const long long n   = min((long long)W::kTileRows, nrows - r0);
-    const uint8_t *in   = in_base + (long long)P.col[j] * in_pitch + r0;
-    const uint32_t t4 = 4u * (threadIdx.x & 255u);                       // byte offset of this thread's histogram column
-    const uint32_t tidhi4 = (t4 >> 8) * 0x01010101u;
-    if ((uint32_t)__cvta_generic_to_shared(smem) != LO_SMEM_WINDOW_BASE) __trap();     // immediate offset of the atomics
-    unsigned long long *dst = (G.mode == 0 ? counts : G.local) + (long long)j * 256;
-
-    auto clear = [&]() {
-        uint4 *p = reinterpret_cast<uint4 *>(smem);
-        for (int i = threadIdx.x; i < kHistRows * (kThreads / 4); i += W::kThreadsW) p[i] = make_uint4(0u, 0u, 0u, 0u);
-        __syncthreads();
-    };
-
-    if (n == W::kTileRows) {
-        uint4 va[W::kVecsA];
-        const uint8_t *src = in + (long long)threadIdx.x * kU8VecBytes;
-#pragma unroll
-        for (int u = 0; u < W::kVecsA; ++u) va[u] = ldg128_stream(src + (long long)u * W::kThreadsW * kU8VecBytes);
-        clear();                                                          // overlaps the first loads' DRAM latency
-        const uint32_t first = va[0].x & 0xFFu;
-        uint32_t mixed;
-        if (W::kVecsB > 0) {
-            uint4 vb[W::kVecsB > 0 ? W::kVecsB : 1];
-#pragma unroll
-            for (int u = 0; u < W::kVecsB; ++u) vb[u] = ldg128_stream(src + (long long)(W::kVecsA + u) * W::kThreadsW * kU8VecBytes);
-            mixed = bump_batch_shared<W::kVecsA>(va, t4, tidhi4);
-            mixed |= bump_batch_shared<(W::kVecsB > 0 ? W::kVecsB : 1)>(vb, t4, tidhi4) | ((vb[0].x & 0xFFu) ^ first);
-        } else {
-            mixed = bump_batch_shared<W::kVecsA>(va, t4, tidhi4);
-        }
-        // constant tile: one RED of the tile's row count instead of the fold (see k_hist_u8_cols)
-        uint32_t *scratch = smem + kHistRows * kThreads;
-        if (__syncthreads_and(mixed == 0u)) {
-            if (threadIdx.x == 0) *scratch = first;
-            __syncthreads();
-            if (__syncthreads_and(first == *scratch)) {
-                if (G.mode != 0) group_wait_generation(G);
-                if (threadIdx.x == 0)
-                    asm volatile("red.relaxed.gpu.global.add.u64 [%0], %1;" :: "l"(dst + first), "l"((unsigned long long)W::kTileRows) : "memory");
-                if (G.mode != 0) group_finish_column(G, j, 256, P.k, tiles_per_col, smem);
-                return;
-            }
-        }
-    } else {
-        // ragged last tile of a column: byte by byte (atomics: the histogram is shared with the partner threads)
-        clear();
-#pragma unroll 1
-        for (long long e = threadIdx.x; e < n; e += W::kThreadsW) {
-            const uint32_t b = ldg8_stream(in + e);
-            atoms_add_base(((b & 0xFCu) << 8) | t4, 1u << ((b & 3u) << 3));
-        }
-    }
-    if (G.mode != 0) group_wait_generation(G);
-    fold_and_flush_wide<W::kThreadsW / 32>(smem, dst);
-    if (G.mode != 0) group_finish_column(G, j, 256, P.k, tiles_per_col, smem);
-}
-
-// ---------------------------------------------------------------------------------------------
-// K4, lane-slot form (LOEXEC_U8_MODE=11): 32-bit counters shared by all warps of the CTA.
-// What bounds the per-thread byte counters is not the atomic unit (conflict-free
-// ATOMS with their operands ready retire fast enough) but the arithmetic that turns a byte into (counter word, byte field):
+// K4: per-column 256-bin value counts of byte columns; 32-bit counters in lane slots shared by all warps of the CTA.
+// Per-thread byte counters (the f64 kernel's layout) are not bounded by the atomic unit here (conflict-free ATOMS with
+// their operands ready retire fast enough) but by the arithmetic that turns a byte into (counter word, byte field):
 // mask, PRMT, shift extraction, 1 << n.  This layout needs none of it.  The CTA keeps ONE histogram of 256 bins x 64
 // slots of 32-bit counters (64 KiB): slot = lane + 32 * (warp & 1), counter of (bin b, slot s) at byte b * 256 + 4 * s.
 //   * bank = (b * 64 + s) mod 32 = lane: every warp instruction is conflict-free, whatever the data;
@@ -1349,15 +881,23 @@ k_hist_u8_cols_wide(const uint8_t *__restrict__ in_base, long long in_pitch, lon
 //     thread t sums the 64 slots of bin t (rotated start: conflict-free) and issues one RED.64.
 // Per byte: one PRMT + one ATOMS.ADD (+ 1/4 of a LOP3 for the run test).
 // ---------------------------------------------------------------------------------------------
+
+// shared-window address at which a block's dynamic shared memory starts when the kernel has no static shared memory:
+// the 1 KiB sm_90 reserves per block (lo_init checks the size).  The atomics carry it in their immediate offset; the
+// kernel traps if it is wrong.  No return value: the shared-memory atomic is fire-and-forget.
+#define LO_SMEM_WINDOW_BASE 1024
+__device__ __forceinline__ void atoms_add_base(uint32_t offset, uint32_t v) {
+    asm volatile("red.shared.add.u32 [%0+1024], %1;" :: "r"(offset), "r"(v) : "memory");
+}
+static_assert(LO_SMEM_WINDOW_BASE == 1024, "keep the immediate in atoms_add_base in sync");
+
 constexpr int kU8LThreads   = 512;
 constexpr int kU8LSmemBytes = 256 * 64 * 4;                       // 64 KiB
 constexpr int kU8LRoundRows = kU8LThreads * 4 * kU8VecBytes;      // 32 768 rows per loop iteration (4 vectors per thread)
 
-// VAR bit 0: the increment is an opaque register (ATOMS.ADD) instead of the literal 1 (ptxas picks ATOMS.POPC.INC)
-// VAR bit 1: one register set copied per round instead of two alternating sets;  bit 2: no two-compare quick reject
-// before the run test.  LOEXEC_U8_MODE 11 = VAR 2 (shipped: the copy form),
-// 12 = VAR 3, 13 = VAR 0, 14 = VAR 6
-template <int VAR>
+// ALIGNED = false: the slab's base or pitch is not a multiple of 16 bytes (a wrapped foreign table), so there are no
+// 128-bit loads: every byte of the chunk is one 8-bit load and one atomic.
+template <bool ALIGNED>
 __global__ void __launch_bounds__(kU8LThreads, 3)
 k_hist_u8_cols_lanes(const uint8_t *__restrict__ in_base, long long in_pitch, long long nrows,
                      unsigned chunks_per_col, long long chunk_rows, unsigned long long *__restrict__ counts,
@@ -1371,13 +911,11 @@ k_hist_u8_cols_lanes(const uint8_t *__restrict__ in_base, long long in_pitch, lo
     const uint8_t *in    = in_base + (long long)P.col[j] * in_pitch + r0;
     if ((uint32_t)__cvta_generic_to_shared(smem) != LO_SMEM_WINDOW_BASE) __trap();     // immediate offset of the atomics
     const uint32_t slot4 = 4u * ((threadIdx.x & 31u) + 32u * ((threadIdx.x >> 5) & 1u));
-    uint32_t one = 1u;
-    if (VAR & 1) one = P.p8 >> 8;                    // a kernel parameter: ptxas cannot fold it into POPC.INC
     const uint8_t *src = in + (long long)threadIdx.x * kU8VecBytes;
     constexpr long long kStride = (long long)kU8LThreads * kU8VecBytes;        // bytes between a thread's vectors
 
-    const long long rounds = n / kU8LRoundRows;
-    uint4 a[4], b[4];                                   // one set in flight while the other is counted
+    const long long rounds = ALIGNED ? n / kU8LRoundRows : 0;
+    uint4 a[4], b[4];                                   // loads land in a[] while a copy in b[] is counted
     auto load_round = [&](uint4 (&d)[4], long long r) {
 #pragma unroll
         for (int u = 0; u < 4; ++u) d[u] = ldg128_stream(src + r * kU8LRoundRows + u * kStride);
@@ -1392,17 +930,17 @@ k_hist_u8_cols_lanes(const uint8_t *__restrict__ in_base, long long in_pitch, lo
         const uint32_t w[4] = {x.x, x.y, x.z, x.w};
 #pragma unroll
         for (int q = 0; q < 4; ++q) {
-            atoms_add_base(__byte_perm(w[q], slot4, 0x6504u), one);
-            atoms_add_base(__byte_perm(w[q], slot4, 0x6514u), one);
-            atoms_add_base(__byte_perm(w[q], slot4, 0x6524u), one);
-            atoms_add_base(__byte_perm(w[q], slot4, 0x6534u), one);
+            atoms_add_base(__byte_perm(w[q], slot4, 0x6504u), 1u);
+            atoms_add_base(__byte_perm(w[q], slot4, 0x6514u), 1u);
+            atoms_add_base(__byte_perm(w[q], slot4, 0x6524u), 1u);
+            atoms_add_base(__byte_perm(w[q], slot4, 0x6534u), 1u);
         }
     };
     auto count_round = [&](const uint4 (&c)[4]) {
         // a warp whose 2 KiB are one value (constant columns: borders, flags, padding) issues one atomic per lane;
         // two compares reject mixed data before the full test is paid
         const uint32_t splat = __byte_perm(c[0].x, 0, 0x0000);
-        if ((VAR & 4) || __all_sync(0xffffffffu, (c[0].x == splat) & (c[3].w == splat))) {
+        if (__all_sync(0xffffffffu, (c[0].x == splat) & (c[3].w == splat))) {
             uint32_t diff = 0u;
 #pragma unroll
             for (int u = 0; u < 4; ++u) diff |= (c[u].x ^ splat) | (c[u].y ^ splat) | (c[u].z ^ splat) | (c[u].w ^ splat);
@@ -1414,26 +952,14 @@ k_hist_u8_cols_lanes(const uint8_t *__restrict__ in_base, long long in_pitch, lo
 #pragma unroll
         for (int u = 0; u < 4; ++u) count_vec(c[u]);
     };
-    long long r = 0;
-    if (VAR & 2) {                                       // loads land in a[], a copy is counted
 #pragma unroll 1
-        for (; r < rounds; ++r) {
+    for (long long r = 0; r < rounds; ++r) {
 #pragma unroll
-            for (int u = 0; u < 4; ++u) b[u] = a[u];
-            if (r + 1 < rounds) load_round(a, r + 1);
-            count_round(b);
-        }
-    } else {
-#pragma unroll 1
-        for (; r + 2 <= rounds; r += 2) {
-            load_round(b, r + 1);
-            count_round(a);
-            if (r + 2 < rounds) load_round(a, r + 2);
-            count_round(b);
-        }
-        if (r < rounds) count_round(a);
+        for (int u = 0; u < 4; ++u) b[u] = a[u];
+        if (r + 1 < rounds) load_round(a, r + 1);
+        count_round(b);
     }
-    {   // rest of the chunk (< one round): every whole vector requested before the first is counted, then single bytes
+    if (ALIGNED) {   // rest of the chunk (< one round): every whole vector requested before the first is counted, then single bytes
         const long long base = rounds * kU8LRoundRows;
         bool have[4];
 #pragma unroll
@@ -1445,7 +971,10 @@ k_hist_u8_cols_lanes(const uint8_t *__restrict__ in_base, long long in_pitch, lo
         for (int u = 0; u < 4; ++u)
             if (have[u]) count_vec(a[u]);
         const long long q = base + ((n - base) / kU8VecBytes) * kU8VecBytes + threadIdx.x;
-        if (q < n) atoms_add_base((ldg8_stream(in + q) << 8) | slot4, one);
+        if (q < n) atoms_add_base((ldg8_stream(in + q) << 8) | slot4, 1u);
+    } else {
+#pragma unroll 1
+        for (long long e = threadIdx.x; e < n; e += kU8LThreads) atoms_add_base((ldg8_stream(in + e) << 8) | slot4, 1u);
     }
     __syncthreads();
     if (G.mode != 0) group_wait_generation(G);

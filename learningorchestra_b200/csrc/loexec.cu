@@ -184,25 +184,14 @@ int configure_kernels() {
     LO_TRY(allow_smem_hist<0>());
     LO_TRY(allow_smem_hist<1>());
     LO_TRY(allow_smem_hist<2>());
-    LO_TRY(allow_smem(lo::k_hist_u8_cols<true, 2>));
-    LO_TRY(allow_smem(lo::k_hist_u8_cols<true, 4>));
-    LO_TRY(allow_smem(lo::k_hist_u8_cols<true, 5>));
-    LO_TRY(allow_smem(lo::k_hist_u8_cols<true, 6>));
-    LO_TRY(allow_smem(lo::k_hist_u8_cols<true, 7>));
-    LO_TRY(allow_smem(lo::k_hist_u8_cols<true, 10>));
-    LO_CUDA(cudaFuncSetAttribute(lo::k_hist_u8_cols_lanes<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, lo::kU8LSmemBytes));
-    LO_CUDA(cudaFuncSetAttribute(lo::k_hist_u8_cols_lanes<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, lo::kU8LSmemBytes));
-    LO_CUDA(cudaFuncSetAttribute(lo::k_hist_u8_cols_lanes<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, lo::kU8LSmemBytes));
-    LO_CUDA(cudaFuncSetAttribute(lo::k_hist_u8_cols_lanes<6>, cudaFuncAttributeMaxDynamicSharedMemorySize, lo::kU8LSmemBytes));
+    LO_CUDA(cudaFuncSetAttribute(lo::k_hist_u8_cols_lanes<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, lo::kU8LSmemBytes));
+    LO_CUDA(cudaFuncSetAttribute(lo::k_hist_u8_cols_lanes<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, lo::kU8LSmemBytes));
     LO_CUDA(cudaFuncSetAttribute(lo::k_project_cast_hist_bins<0, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, lo::kWBSmemWordsMax * 4));
     LO_CUDA(cudaFuncSetAttribute(lo::k_project_cast_hist_bins<1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, lo::kWBSmemWordsMax * 4));
     LO_CUDA(cudaFuncSetAttribute(lo::k_project_cast_hist_bins<2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, lo::kWBSmemWordsMax * 4));
     LO_CUDA(cudaFuncSetAttribute(lo::k_project_cast_hist_bins<0, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, lo::kWBSmemWordsMax * 4));
     LO_CUDA(cudaFuncSetAttribute(lo::k_project_cast_hist_bins<1, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, lo::kWBSmemWordsMax * 4));
     LO_CUDA(cudaFuncSetAttribute(lo::k_project_cast_hist_bins<2, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, lo::kWBSmemWordsMax * 4));
-    LO_TRY(allow_smem(lo::k_hist_u8_cols_wide<2>));
-    LO_TRY(allow_smem(lo::k_hist_u8_cols_wide<4>));
-    LO_TRY(allow_smem(lo::k_hist_u8_cols<false, 4>));
     return LO_OK;
 }
 
@@ -381,55 +370,25 @@ int hist_u8_impl(lo_ctx *ctx, const lo_table *in, const int32_t *col_idx, int32_
     if (in->nrows == 0 && !group) return LO_OK;
     const lo::GroupStep &G = group ? *group : kNoGroup;
     const bool aligned = ((uintptr_t)in->base % 16 == 0) && (in->pitch % 16 == 0);
-    int mode = LO_U8_MODE_DEFAULT;
-    if (const char *e = getenv("LOEXEC_U8_MODE")) mode = atoi(e);       // measurement knob (scripts/u8_sweep.py)
-    const bool wide = aligned && (mode == 8 || mode == 9);
-    const bool lanes = aligned && mode >= 11 && mode <= 14;
-    int64_t tile_rows = !wide ? lo::kU8TileRows : mode == 8 ? lo::kU8WTileRows2 : lo::kU8WTileRows4;
-    if (lanes) {
-        // chunk of a column per CTA, a multiple of the 32 Ki-row round: long chunks amortise the 64 KiB clear + fold
-        // (up to 8 rounds, one chunk per column on short shards)
-        const int64_t slots = (int64_t)ctx->sm_count * 3;
-        int64_t want = (in->nrows * (int64_t)std::min<int32_t>(k, lo::kMaxColsU8)) / slots;
-        want = std::max<int64_t>(lo::kU8LRoundRows, std::min<int64_t>(want, 8 * (int64_t)lo::kU8LRoundRows));
-        if (const char *e = getenv("LOEXEC_U8_CHUNK_ROUNDS")) want = std::max<int64_t>(1, atoll(e)) * lo::kU8LRoundRows;
-        tile_rows = (want / lo::kU8LRoundRows) * lo::kU8LRoundRows;
-    }
-    const unsigned tiles_per_col = (unsigned)((in->nrows + tile_rows - 1) / tile_rows);
+    // chunk of a column per CTA, a multiple of the 32 Ki-row round: long chunks amortise the 64 KiB clear + fold
+    // (up to 8 rounds, one chunk per column on short shards)
+    const int64_t slots = (int64_t)ctx->sm_count * 3;
+    int64_t want = (in->nrows * (int64_t)std::min<int32_t>(k, lo::kMaxColsU8)) / slots;
+    want = std::max<int64_t>(lo::kU8LRoundRows, std::min<int64_t>(want, 8 * (int64_t)lo::kU8LRoundRows));
+    const int64_t chunk_rows = (want / lo::kU8LRoundRows) * lo::kU8LRoundRows;
+    const unsigned chunks_per_col = (unsigned)((in->nrows + chunk_rows - 1) / chunk_rows);
     for (int32_t c0 = 0; c0 < k; c0 += lo::kMaxColsU8) {
         lo::ColsU8 P;
         P.k = std::min<int32_t>(lo::kMaxColsU8, k - c0);
-        P.p8 = 1u << 8; P.p11 = 1u << 11; P.p16 = 1u << 16; P.p19 = 1u << 19; P.p24 = 1u << 24; P.p27 = 1u << 27; P.p3 = 1u << 3;
         for (int j = 0; j < P.k; ++j) P.col[j] = col_idx[c0 + j];
-        const unsigned long long blocks = (unsigned long long)tiles_per_col * (unsigned)P.k;
+        const unsigned long long blocks = (unsigned long long)chunks_per_col * (unsigned)P.k;
         if (blocks > 0x7fffffffull) return fail(LO_ERR_INVALID, "table too large for one launch");
         unsigned long long *cnt = (unsigned long long *)counts_dev + (int64_t)c0 * 256;
         const uint8_t *ib = (const uint8_t *)in->base;
         const long long ip = in->pitch, nr = in->nrows;
-#define LO_U8_LAUNCH(AL, MD)                                                                                      \
-    LO_CUDA(launch_kernel(lo::k_hist_u8_cols<AL, MD>, (unsigned)blocks, lo::kThreads, (size_t)lo::kHistSmemBytes, s, \
-                          G.overlap != 0, ib, ip, nr, tiles_per_col, cnt, P, G))
-        if (!aligned)       LO_U8_LAUNCH(false, 4);
-        else if (mode == 8) LO_CUDA(launch_kernel(lo::k_hist_u8_cols_wide<2>, (unsigned)blocks, 512u, (size_t)lo::kHistSmemBytes, s,
-                                                  G.overlap != 0, ib, ip, nr, tiles_per_col, cnt, P, G));
-        else if (mode == 11) LO_CUDA(launch_kernel(lo::k_hist_u8_cols_lanes<2>, (unsigned)blocks, (unsigned)lo::kU8LThreads, (size_t)lo::kU8LSmemBytes, s,
-                                                  G.overlap != 0, ib, ip, nr, tiles_per_col, (long long)tile_rows, cnt, P, G));
-        else if (mode == 12) LO_CUDA(launch_kernel(lo::k_hist_u8_cols_lanes<3>, (unsigned)blocks, (unsigned)lo::kU8LThreads, (size_t)lo::kU8LSmemBytes, s,
-                                                  G.overlap != 0, ib, ip, nr, tiles_per_col, (long long)tile_rows, cnt, P, G));
-        else if (mode == 13) LO_CUDA(launch_kernel(lo::k_hist_u8_cols_lanes<0>, (unsigned)blocks, (unsigned)lo::kU8LThreads, (size_t)lo::kU8LSmemBytes, s,
-                                                  G.overlap != 0, ib, ip, nr, tiles_per_col, (long long)tile_rows, cnt, P, G));
-        else if (mode == 14) LO_CUDA(launch_kernel(lo::k_hist_u8_cols_lanes<6>, (unsigned)blocks, (unsigned)lo::kU8LThreads, (size_t)lo::kU8LSmemBytes, s,
-                                                  G.overlap != 0, ib, ip, nr, tiles_per_col, (long long)tile_rows, cnt, P, G));
-        else if (mode == 9) LO_CUDA(launch_kernel(lo::k_hist_u8_cols_wide<4>, (unsigned)blocks, 1024u, (size_t)lo::kHistSmemBytes, s,
-                                                  G.overlap != 0, ib, ip, nr, tiles_per_col, cnt, P, G));
-        else if (mode == 2) LO_U8_LAUNCH(true, 2);
-        else if (mode == 4) LO_U8_LAUNCH(true, 4);
-        else if (mode == 5) LO_U8_LAUNCH(true, 5);
-        else if (mode == 6) LO_U8_LAUNCH(true, 6);
-        else if (mode == 10) LO_U8_LAUNCH(true, 10);
-        else if (mode == 7) LO_U8_LAUNCH(true, 7);
-        else                return fail(LO_ERR_INVALID, "unknown LOEXEC_U8_MODE %d", mode);
-#undef LO_U8_LAUNCH
+        LO_CUDA(launch_kernel(aligned ? lo::k_hist_u8_cols_lanes<true> : lo::k_hist_u8_cols_lanes<false>, (unsigned)blocks,
+                              (unsigned)lo::kU8LThreads, (size_t)lo::kU8LSmemBytes, s, G.overlap != 0,
+                              ib, ip, nr, chunks_per_col, (long long)chunk_rows, cnt, P, G));
         LO_CUDA(cudaGetLastError());
         ctx->launches.fetch_add(1, std::memory_order_relaxed);
     }
@@ -574,7 +533,7 @@ int lo_init(int device, lo_ctx **out) {
     if (prop.major != 9 || prop.minor != 0)
         return fail(LO_ERR_NO_DEVICE, "device %d is sm_%d%d; libloexec is built for sm_90a only", device,
                     prop.major, prop.minor);
-    // the byte-histogram kernels put the start of dynamic shared memory (after this reserve) in an immediate offset
+    // the byte-histogram kernel puts the start of dynamic shared memory (after this reserve) in an immediate offset
     int reserved = 0;
     LO_CUDA(cudaDeviceGetAttribute(&reserved, cudaDevAttrReservedSharedMemoryPerBlock, device));
     if (reserved != LO_SMEM_WINDOW_BASE)
@@ -1109,7 +1068,7 @@ int lo_hist_u8_cols_host(lo_ctx *ctx, const uint8_t *const *in_cols, int64_t nro
     if (!counts) return fail(LO_ERR_INVALID, "counts is NULL");
     std::vector<int32_t> ident(k);
     for (int j = 0; j < k; ++j) ident[j] = j;
-    return host_pipeline(ctx, (const void *const *)in_cols, LO_U8, nrows, k, nullptr, LO_U8, lo::kU8TileRows,
+    return host_pipeline(ctx, (const void *const *)in_cols, LO_U8, nrows, k, nullptr, LO_U8, lo::kU8HostChunkRows,
                          (size_t)k * 256, counts, timing, [&](lo_table *tin, lo_table *, unsigned long long *cdev, cudaStream_t cs) {
                              return hist_u8_impl(ctx, tin, ident.data(), k, (uint64_t *)cdev, cs);
                          });

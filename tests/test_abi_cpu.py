@@ -46,7 +46,7 @@ def test_lane_slot_kernels_issue_one_shared_atomic_per_element(built):
     RED.64 flush; the wide-bin kernel counts with shared atomics too and streams with 128-bit loads."""
     from learningorchestra_b200 import _native
     sass = subprocess.run(["cuobjdump", "-sass", str(_native.LIB_PATH)], capture_output=True, text=True).stdout
-    lanes = sass.split("Function : _ZN2lo20k_hist_u8_cols_lanesILi2EEE")[1].split("Function :")[0]
+    lanes = sass.split("Function : _ZN2lo20k_hist_u8_cols_lanesILb1EEE")[1].split("Function :")[0]
     atoms = [l for l in lanes.splitlines() if "ATOMS" in l]
     assert len(atoms) >= 128 and all("+0x400]" in l for l in atoms if "POPC.INC" in l)
     assert lanes.count("PRMT") >= 128 and "LDG.E.NA.128" in lanes or "LDG.E.128" in lanes
@@ -91,20 +91,20 @@ def test_package_never_imports_the_oracle():
                 for line in text.splitlines() if "oracle" in line.lower()), path
 
 
-def _build_c_consumer():
+def _build_c_consumer(out_dir: Path) -> Path:
+    """Compile tests/native/abi_smoke.c into ``out_dir`` (a temporary directory: the checkout may be read-only)."""
     from learningorchestra_b200 import _native
-    exe = ROOT / "tests" / "native" / "_build" / "abi_smoke"
-    exe.parent.mkdir(exist_ok=True)
+    exe = out_dir / "abi_smoke"
     subprocess.run(["gcc", "-std=c99", "-Wall", "-Werror", "-O1", "-I", str(ROOT / "include"),
                     str(ROOT / "tests" / "native" / "abi_smoke.c"), "-o", str(exe),
                     "-L", str(_native.LIB_PATH.parent), "-lloexec", f"-Wl,-rpath,{_native.LIB_PATH.parent}"], check=True)
     return exe
 
 
-def test_plain_c_program_links_against_the_abi(built):
+def test_plain_c_program_links_against_the_abi(built, tmp_path):
     """include/loexec.h is plain C99 and the .so links without any C++ / CUDA / torch on the consumer side."""
     import torch
-    exe = _build_c_consumer()
+    exe = _build_c_consumer(tmp_path)
     out = subprocess.run([str(exe)], capture_output=True, text=True, timeout=120)
     if torch.cuda.is_available():
         assert out.returncode == 0, out.stderr

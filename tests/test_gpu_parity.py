@@ -187,21 +187,33 @@ def test_hist_u8_all_values_and_constant(engine):
     t.free()
 
 
-@pytest.mark.parametrize("mode", ["2", "4", "5", "6", "7", "8", "9", "10", "11", "12", "13", "14"])
-def test_hist_u8_every_kernel_variant(engine, monkeypatch, mode):
-    """Every selectable form of the byte-histogram kernel (LOEXEC_U8_MODE; 8 = the 512-thread shared-histogram kernel
-    with its own tile size) gives the oracle's counts: ragged sizes, full tiles, constant columns, every byte value."""
-    monkeypatch.setenv("LOEXEC_U8_MODE", mode)
-    wide_tile = 512 * 7 * 16 if mode != "9" else 1024 * 3 * 16
-    rng = np.random.default_rng(int(mode))
-    for nrows in (1, 17, 4097, TILE, TILE + 1, wide_tile, 2 * wide_tile + 777, 3 * TILE + 5):
-        table = np.stack([rng.integers(0, 256, nrows, dtype=np.uint8), np.full(nrows, 0, np.uint8), np.full(nrows, 200, np.uint8),
-                          np.arange(nrows, dtype=np.uint64).astype(np.uint8), bn.synth_u8(SEED, 300, 0, nrows),
-                          np.where(np.arange(nrows) < nrows // 2, 7, 9).astype(np.uint8)])
+@pytest.mark.parametrize("nrows", [1, 17, 4097, 32_767, 32_768, 32_769, TILE + 1, 3 * TILE + 5, 5 * 2 ** 20 + 3])
+@pytest.mark.parametrize("aligned", [True, False], ids=["aligned", "unaligned"])
+def test_hist_u8_lane_slot_kernel(engine, aligned, nrows):
+    """The byte-histogram kernel gives the oracle's counts on random, constant, every-value, MNIST-shaped and two-valued
+    columns, at sizes on both sides of its 32 Ki-row round and, at 5 Mi + 3 rows, in chunks of several rounds with a
+    ragged last chunk.  A wrapped slab at base + 1 with an odd pitch cannot take 16-byte loads and is counted byte by
+    byte by the same kernel."""
+    rng = np.random.default_rng(nrows)
+    table = np.stack([rng.integers(0, 256, nrows, dtype=np.uint8), np.full(nrows, 0, np.uint8), np.full(nrows, 200, np.uint8),
+                      np.arange(nrows, dtype=np.uint64).astype(np.uint8), bn.synth_u8(SEED, 300, 0, nrows),
+                      np.where(np.arange(nrows) < nrows // 2, 7, 9).astype(np.uint8)])
+    big = None
+    if aligned:
         t = engine.table_from_numpy(table)
-        got = engine.hist_u8_cols(t, range(6)).to_numpy()
-        np.testing.assert_array_equal(got, bn.hist_u8_cols(table, range(6)), err_msg=f"mode {mode} nrows {nrows}")
-        t.free()
+    else:
+        pitch = (nrows + 2) | 1
+        flat = np.zeros(1 + 6 * pitch, np.uint8)
+        for c in range(6):
+            flat[1 + c * pitch: 1 + c * pitch + nrows] = table[c]
+        big = engine.table("u8", flat.size, 1)
+        big.upload(0, flat)
+        t = engine.wrap("u8", nrows, 6, big.base_ptr + 1, pitch)
+    got = engine.hist_u8_cols(t, range(6)).to_numpy()
+    np.testing.assert_array_equal(got, bn.hist_u8_cols(table, range(6)))
+    t.free()
+    if big is not None:
+        big.free()
 
 
 def test_unaligned_wrapped_tables(engine):
@@ -366,10 +378,10 @@ def test_concurrent_callers_share_one_engine(engine):
     assert not errors, errors
 
 
-def test_plain_c_consumer_runs_the_hot_path(engine):
+def test_plain_c_consumer_runs_the_hot_path(engine, tmp_path):
     import subprocess
     from test_abi_cpu import _build_c_consumer
-    out = subprocess.run([str(_build_c_consumer())], capture_output=True, text=True, timeout=120)
+    out = subprocess.run([str(_build_c_consumer(tmp_path))], capture_output=True, text=True, timeout=120)
     assert out.returncode == 0 and "abi_smoke ok" in out.stdout, out.stderr
 
 
