@@ -92,8 +92,8 @@ typedef struct lo_host_timing {
     double h2d_bytes;  /* bytes copied host -> device                    */
     double d2h_bytes;  /* bytes copied device -> host                    */
     int64_t launches;  /* kernels launched                               */
-    double kernel_ms;  /* device time of the call's kernels between two events on its stream (parser, group-by); 0 for the
-                          chunked pipelines, whose kernels overlap their copies   */
+    double kernel_ms;  /* device time of the call's kernels between two events on its stream (parser, formatter,
+                          group-by); 0 for the chunked pipelines, whose kernels overlap their copies   */
 } lo_host_timing;
 
 /* ---- context ------------------------------------------------------------------------- */
@@ -304,6 +304,19 @@ int lo_value_counts_str_host(lo_ctx *ctx, const uint8_t *chars, const int64_t *o
 #define LO_NUM_UNSUPPORTED 4
 int lo_parse_number_host(lo_ctx *ctx, const uint8_t *chars, const int64_t *offsets, int64_t n,
                          double *values, uint8_t *status, lo_host_timing *timing);
+
+/* Number -> text for one column: the reference's "string" cast, str(v) / None -> "" (data_type_handler_image/
+ * data_type_update.py:22-28), for every cell at once on the GPU.  The inverse of lo_parse_number_host.
+ * status[i] uses the LO_NUM_* codes above: FLOAT -> repr(float) (shortest round-trip digits, CPython's notation),
+ * INTEGER -> str(int) (values[i] finite and integral; every digit of the exact value), EMPTY -> "".  Any other status,
+ * or an INTEGER cell that is not finite and integral -> LO_ERR_INVALID, the message names the first such row.
+ * offsets: host int64[n+1], always written, offsets[0] == 0; cell i is chars[offsets[i] .. offsets[i+1]) (the layout of
+ * an Arrow large_string array).  chars: written when chars_capacity >= offsets[n]; chars == NULL with
+ * chars_capacity == 0 asks for the sizes only; a non-NULL buffer that is too small -> LO_ERR_INVALID (offsets still
+ * written).  One cell is at most LO_FORMAT_MAX_CELL bytes (a FLOAT cell at most 24). */
+#define LO_FORMAT_MAX_CELL 310
+int lo_format_number_host(lo_ctx *ctx, const double *values, const uint8_t *status, int64_t n,
+                          int64_t *offsets, uint8_t *chars, int64_t chars_capacity, lo_host_timing *timing);
 
 /* Per-column min and max of the CAST fp32 values over finite entries (NaN / +-inf ignored): the
  * range pre-pass for a histogram request that carries no range (SURVEY.md §2.1 C2).

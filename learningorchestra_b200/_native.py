@@ -33,6 +33,7 @@ LO_GROUP_BLOB_BYTES = 512
 LO_GROUP_MAX_DEVICES = 16
 LO_GROUP_MAX_COUNTS = 262144
 LO_NUM_FLOAT, LO_NUM_INTEGER, LO_NUM_EMPTY, LO_NUM_INVALID, LO_NUM_UNSUPPORTED = 0, 1, 2, 3, 4
+LO_FORMAT_MAX_CELL = 310
 LO_ABI_VERSION = 3
 
 _ERR_NAMES = {
@@ -120,6 +121,7 @@ SIGNATURES = {
     "lo_value_counts_f64_host": (C.c_int, [_P, _P, C.c_int64, _P, _P, C.c_int64, C.POINTER(C.c_int64), C.POINTER(HostTiming)]),
     "lo_value_counts_str_host": (C.c_int, [_P, _P, _P, C.c_int64, _P, _P, C.c_int64, C.POINTER(C.c_int64), C.POINTER(HostTiming)]),
     "lo_parse_number_host": (C.c_int, [_P, _P, _P, C.c_int64, _P, _P, C.POINTER(HostTiming)]),
+    "lo_format_number_host": (C.c_int, [_P, _P, _P, C.c_int64, _P, _P, C.c_int64, C.POINTER(HostTiming)]),
     "lo_minmax_cast_host": (C.c_int, [_P, C.POINTER(_P), C.c_int64, C.c_int32, _P, _P, _P, C.POINTER(HostTiming)]),
 }
 

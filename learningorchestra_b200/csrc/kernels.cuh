@@ -27,12 +27,14 @@
 //     moves the merged matrix out — merge, arrival and epilogue ride inside the one streaming launch per step.
 //   * bin index = trunc(RN((x - lo) / w)) computed without a divide (hoisted reciprocal + two FMA
 //     corrections, proven and exhaustively self-tested equal to the IEEE quotient; bin_index_f32).
-//   * also here: k_parse_number (CPython float() on the GPU, parse_number.cuh), k_hash_count_f64 / _str
+//   * also here: k_parse_number (CPython float() on the GPU, parse_number.cuh), k_format_number_len / _write (its
+//     inverse, CPython str(), format_number.cuh), k_hash_count_f64 / _str
 //     (exact group-by), k_minmax_cast, the group's small kernels (push, big-matrix merge, barrier), generators, checksum.
 #pragma once
 #include <cstdint>
 #include <cuda_runtime.h>
 #include "parse_number.cuh"
+#include "format_number.cuh"
 
 namespace lo {
 
@@ -1336,6 +1338,27 @@ __global__ void k_parse_number(const uint8_t *__restrict__ chars, const long lon
         value_bits[i] = bits;
         status[i] = st;
     }
+}
+
+// R-semantics cast "string" (data_type_update.py:22-28): str(v) / None -> "" of one cell per thread
+// (format_number.cuh).  Pass 1 writes each cell's length (the input of the offsets scan) and the first row whose status
+// or value cannot be formatted; pass 2 writes each cell's text at its scanned offset.  Both run the same format_cell.
+__global__ void k_format_number_len(const unsigned long long *__restrict__ value_bits, const uint8_t *__restrict__ status,
+                                    long long n, long long *__restrict__ lengths, unsigned long long *__restrict__ first_bad) {
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+        int len = fmt::format_cell(value_bits[i], status[i], nullptr);
+        if (len < 0) {
+            atomicMin(first_bad, (unsigned long long)i);
+            len = 0;
+        }
+        lengths[i] = len;
+    }
+}
+
+__global__ void k_format_number_write(const unsigned long long *__restrict__ value_bits, const uint8_t *__restrict__ status,
+                                      long long n, const long long *__restrict__ offsets, uint8_t *__restrict__ chars) {
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+        fmt::format_cell(value_bits[i], status[i], chars + offsets[i]);
 }
 
 // exhaustive self-test: every one of the 2^32 fp32 bit patterns through both divide variants

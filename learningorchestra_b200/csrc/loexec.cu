@@ -6,6 +6,8 @@
 #include "loexec.h"
 #include "kernels.cuh"
 
+#include <cub/device/device_scan.cuh>
+
 #include <atomic>
 #include <condition_variable>
 #include <cctype>
@@ -1278,6 +1280,85 @@ int lo_parse_number_host(lo_ctx *ctx, const uint8_t *chars, const int64_t *offse
         timing->launches  = ctx->launches.load() - launches0;
         timing->kernel_ms = kt.ms();
     }
+    return LO_OK;
+}
+
+// number -> text for one column (R-semantics "string" cast): cell lengths, an exclusive scan of them into the Arrow
+// offsets, then every cell's text at its offset.  The offsets come back before the text is made, so the caller's
+// capacity is checked against the exact size and the device text buffer is allocated at that size.
+int lo_format_number_host(lo_ctx *ctx, const double *values, const uint8_t *status, int64_t n, int64_t *offsets,
+                          uint8_t *chars, int64_t chars_capacity, lo_host_timing *timing) {
+    LO_TRY(check_ctx(ctx));
+    if (n < 0 || chars_capacity < 0) return fail(LO_ERR_INVALID, "negative size");
+    if (!offsets) return fail(LO_ERR_INVALID, "offsets is NULL");
+    if (!chars && chars_capacity) return fail(LO_ERR_INVALID, "chars is NULL with chars_capacity %lld", (long long)chars_capacity);
+    offsets[0] = 0;
+    if (n == 0) return LO_OK;
+    if (!values || !status) return fail(LO_ERR_INVALID, "NULL argument");
+    const auto t0 = std::chrono::steady_clock::now();
+    const int64_t launches0 = ctx->launches.load();
+    unsigned long long *d_val = nullptr, *d_bad = nullptr;
+    uint8_t *d_status = nullptr, *d_chars = nullptr;
+    long long *d_off = nullptr;
+    void *d_tmp = nullptr;
+    size_t tmp_bytes = 0;
+    cudaStream_t s = ctx->stream;
+    DevTimer kt_len, kt_write;
+    const int grid = (int)std::min<int64_t>((n + 127) / 128, (int64_t)ctx->sm_count * 16);
+    cudaError_t e = cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, d_off, n + 1, s);
+    if (e == cudaSuccess) e = scratch_alloc(&d_val, (size_t)n * 8, s);
+    if (e == cudaSuccess) e = scratch_alloc(&d_status, (size_t)n, s);
+    if (e == cudaSuccess) e = scratch_alloc(&d_off, (size_t)(n + 1) * 8, s);
+    if (e == cudaSuccess) e = scratch_alloc(&d_bad, 8, s);
+    if (e == cudaSuccess) e = scratch_alloc((char **)&d_tmp, tmp_bytes, s);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(d_val, values, (size_t)n * 8, cudaMemcpyHostToDevice, s);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(d_status, status, (size_t)n, cudaMemcpyHostToDevice, s);
+    if (e == cudaSuccess) e = cudaMemsetAsync(d_bad, 0xFF, 8, s);
+    if (e == cudaSuccess) e = cudaMemsetAsync(d_off + n, 0, 8, s);           // the scan's last input: offsets[n] = total
+    if (e == cudaSuccess) e = kt_len.start(s);
+    if (e == cudaSuccess) {
+        lo::k_format_number_len<<<grid, 128, 0, s>>>(d_val, d_status, n, d_off, d_bad);
+        e = cudaGetLastError();
+        if (e == cudaSuccess) e = cub::DeviceScan::ExclusiveSum(d_tmp, tmp_bytes, d_off, n + 1, s);
+        ctx->launches.fetch_add(2, std::memory_order_relaxed);
+    }
+    if (e == cudaSuccess) e = kt_len.stop(s);
+    unsigned long long bad = ~0ull;
+    if (e == cudaSuccess) e = cudaMemcpyAsync(offsets, d_off, (size_t)(n + 1) * 8, cudaMemcpyDeviceToHost, s);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(&bad, d_bad, 8, cudaMemcpyDeviceToHost, s);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+    const int64_t total = e == cudaSuccess ? offsets[n] : 0;
+    const bool write = e == cudaSuccess && bad >= (unsigned long long)n && chars && total <= chars_capacity && total > 0;
+    if (write) {
+        e = scratch_alloc(&d_chars, (size_t)total, s);
+        if (e == cudaSuccess) e = kt_write.start(s);
+        if (e == cudaSuccess) {
+            lo::k_format_number_write<<<grid, 128, 0, s>>>(d_val, d_status, n, d_off, d_chars);
+            e = cudaGetLastError();
+            ctx->launches.fetch_add(1, std::memory_order_relaxed);
+        }
+        if (e == cudaSuccess) e = kt_write.stop(s);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(chars, d_chars, (size_t)total, cudaMemcpyDeviceToHost, s);
+    }
+    scratch_free(d_val, s); scratch_free(d_status, s); scratch_free(d_off, s); scratch_free(d_bad, s);
+    scratch_free(d_tmp, s); scratch_free(d_chars, s);
+    { const cudaError_t e2 = cudaStreamSynchronize(s); if (e == cudaSuccess) e = e2; }
+    if (e != cudaSuccess) return fail(e == cudaErrorMemoryAllocation ? LO_ERR_NOMEM : LO_ERR_CUDA, "format_number: %s", cudaGetErrorString(e));
+    if (timing) {
+        timing->total_ms  = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+        timing->h2d_bytes = (double)n * 9;
+        timing->d2h_bytes = (double)(n + 1) * 8 + 8 + (write ? (double)total : 0.0);
+        timing->launches  = ctx->launches.load() - launches0;
+        timing->kernel_ms = kt_len.ms() + kt_write.ms();
+    }
+    if (bad < (unsigned long long)n) {
+        const long long row = (long long)bad;
+        if (status[row] > LO_NUM_EMPTY)
+            return fail(LO_ERR_INVALID, "row %lld: status %u is not LO_NUM_FLOAT, LO_NUM_INTEGER or LO_NUM_EMPTY", row, (unsigned)status[row]);
+        return fail(LO_ERR_INVALID, "row %lld: LO_NUM_INTEGER value %.17g is not finite and integral", row, values[row]);
+    }
+    if (chars && total > chars_capacity)
+        return fail(LO_ERR_INVALID, "the text takes %lld bytes, chars_capacity is %lld", (long long)total, (long long)chars_capacity);
     return LO_OK;
 }
 

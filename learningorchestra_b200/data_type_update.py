@@ -10,8 +10,13 @@ methods, in-place conversion of the input collection, same ``finished`` False ->
   reference leaves it (``finished: False``).  Unicode digits / whitespace (``"１２"``, ``"٣.٥"``) are mapped to ASCII by
   the packer exactly as ``float(str)`` maps them (:func:`columnar.ascii_number_text`); a cell over 1 MiB fails the job
   loudly (no host ``float()`` fallback).
-* ``"string"`` (``data_type_update.py:22-28``): ``str(v)`` / ``None -> ""`` is text formatting of Python
-  objects in the document adapter and stays on the host (SURVEY.md §8a row a5: out of the GPU's scope).
+* ``"string"`` (``data_type_update.py:22-28``): ``str(v)`` / ``None -> ""``.  With an engine that has
+  ``format_number_host``, every number of the field is formatted ON THE GPU in one call (``lo_format_number_host`` ->
+  ``k_format_number_len`` / ``_write``: ``repr(float)`` with CPython's shortest round-trip digits, ``str(int)`` of
+  integral values, ``""`` for None), the parser's inverse.  A number column comes back as the Arrow ``large_string``
+  buffers of a new TextColumn; in documents, the cells that are binary64 numbers go to the device and everything else
+  (text, bools, ints beyond a double, other objects) keeps ``str()``.  A failing device call fails the job, with no host
+  retry.  An engine without the method (``engine=None``) formats with ``str()`` on the host.
 * ``"float32"`` (this build's optional extension): the B-semantics cast of SURVEY.md §0 — numeric values
   go through the sm_90a kernel (fp64 -> fp32 round-to-nearest-even) and are stored back widened.
 """
@@ -23,6 +28,18 @@ import numpy as np
 
 from . import columnar
 from .utils import record_exception
+
+
+def _is_binary64(cell) -> bool:
+    """A float, or an int (not a bool) that a double holds exactly: the cells the device formatter takes."""
+    if type(cell) is float:
+        return True
+    if type(cell) is not int:
+        return False
+    try:
+        return int(float(cell)) == cell
+    except OverflowError:
+        return False
 
 
 class DataType:
@@ -72,7 +89,12 @@ class DataType:
         if field_type == self.STRING_TYPE:
             if col.kind == "text":                     # str(v) of a str is itself; None -> ""
                 new = TextColumn(col.arr.fill_null("")) if col.arr.null_count else col
-            else:                                      # str(int) / repr(float): text formatting stays on the host (a5)
+            elif getattr(self.engine, "format_number_host", None) is not None:     # str(int) / repr(float) on the GPU
+                import pyarrow as pa
+                status = np.where(~col.valid, N.LO_NUM_EMPTY, np.where(col.is_int, N.LO_NUM_INTEGER, N.LO_NUM_FLOAT))
+                chars, offsets = self.engine.format_number_host(col.values, status.astype(np.uint8))
+                new = TextColumn(pa.LargeStringArray.from_buffers(len(col), pa.py_buffer(offsets), pa.py_buffer(chars)))
+            else:                                      # no device formatter: str() on the host
                 import pyarrow as pa
                 new = TextColumn(pa.array(["" if v is None else str(v) for v in col.to_pylist()], type=pa.large_string()))
             db.set_column(filename, field, new)
@@ -119,13 +141,31 @@ class DataType:
 
     def __to_text(self, rows, field):
         """``data_type_update.py:22-28``: ``None -> ""``, anything else ``str(v)``; the reference's guard
-        ``document[field] == str`` compares a value with the type object and is never true."""
-        changes = {}
+        ``document[field] == str`` compares a value with the type object and is never true.
+
+        With a device formatter the cells that are binary64 numbers — ``float``, and ``int`` whose value a double
+        holds exactly — are formatted on the GPU in one call (``repr(float)`` / ``str(int)``).  Text, ``bool``
+        (``str(True)`` is ``"True"``), ints beyond a double and other objects were never numbers the device holds and
+        keep ``str()`` on the host."""
+        from . import _native as N
+        fmt = getattr(self.engine, "format_number_host", None)
+        changes, device_ids, values, status = {}, [], [], []
         for row in rows:
             cell = row[field]
             if cell == str:
                 continue
+            if fmt is not None and _is_binary64(cell):
+                device_ids.append(row[self.DOCUMENT_ID_NAME])
+                values.append(float(cell))
+                status.append(N.LO_NUM_INTEGER if type(cell) is int else N.LO_NUM_FLOAT)
+                changes[row[self.DOCUMENT_ID_NAME]] = None          # keeps the document order; filled below
+                continue
             changes[row[self.DOCUMENT_ID_NAME]] = {field: "" if cell is None else str(cell)}
+        if device_ids:
+            chars, offsets = fmt(np.array(values, dtype=np.float64), np.array(status, dtype=np.uint8))
+            raw = chars.tobytes()
+            for j, doc_id in enumerate(device_ids):
+                changes[doc_id] = {field: raw[offsets[j]:offsets[j + 1]].decode("ascii")}
         return changes
 
     def __gpu_number(self, documents, field):

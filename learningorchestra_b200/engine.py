@@ -369,6 +369,34 @@ class Engine:
                                                    n, values.ctypes.data_as(C.c_void_p), status.ctypes.data_as(C.c_void_p), None))
         return values, status
 
+    def format_number_host(self, values: np.ndarray, status: np.ndarray, timing: dict | None = None):
+        """The inverse of :meth:`parse_number_packed`: values float64[n] and status uint8[n] (LO_NUM_FLOAT ->
+        ``repr(float)``, LO_NUM_INTEGER -> ``str(int)``, LO_NUM_EMPTY -> ``""``) become one packed text column
+        (chars uint8, offsets int64[n+1]) — the buffers of an Arrow ``large_string`` array.  Any other status, or an
+        INTEGER value that is not finite and integral, raises LoexecError naming the row.  ``timing``: a dict to receive
+        the call's lo_host_timing fields."""
+        values = np.ascontiguousarray(values, dtype=np.float64)
+        status = np.ascontiguousarray(status, dtype=np.uint8)
+        n = values.shape[0]
+        if status.shape != (n,):
+            raise ValueError("values and status must be 1-D arrays of the same length")
+        # one call: chars sized from an upper bound per cell (24 bytes covers every repr(float), 21 every int below
+        # 2^64), then trimmed to the exact total
+        big = np.abs(values) >= 2.0 ** 64
+        bound = np.where(status == N.LO_NUM_EMPTY, 0,
+                         np.where(status == N.LO_NUM_INTEGER, np.where(big, N.LO_FORMAT_MAX_CELL, 21), 24))
+        cap = int(bound.sum(dtype=np.int64))
+        chars = np.empty(max(cap, 1), dtype=np.uint8)
+        offsets = np.zeros(n + 1, dtype=np.int64)
+        t = N.HostTiming()
+        N.check(self._lib.lo_format_number_host(self._ctx, values.ctypes.data_as(C.c_void_p), status.ctypes.data_as(C.c_void_p),
+                                                n, offsets.ctypes.data_as(C.c_void_p), chars.ctypes.data_as(C.c_void_p), cap,
+                                                C.byref(t)))
+        if timing is not None:
+            timing.update(total_ms=t.total_ms, kernel_ms=t.kernel_ms, h2d_bytes=t.h2d_bytes, d2h_bytes=t.d2h_bytes,
+                          launches=t.launches)
+        return chars[:offsets[n]], offsets
+
     def value_counts_str_packed(self, chars: np.ndarray, offsets: np.ndarray):
         """(rep_rows int64[g], counts uint64[g]) of an already packed text column (offsets[0] == 0)."""
         n = offsets.shape[0] - 1

@@ -399,6 +399,9 @@ class ShardedEngine:
     def parse_number_packed(self, chars, offsets):
         return self.engines[0].parse_number_packed(chars, offsets)
 
+    def format_number_host(self, values, status, timing=None):
+        return self.engines[0].format_number_host(values, status, timing)
+
     def value_counts_str_packed(self, chars, offsets):
         return self.engines[0].value_counts_str_packed(chars, offsets)
 
