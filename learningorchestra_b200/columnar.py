@@ -81,20 +81,67 @@ def _numeric_column_loop(values):
     return out, valid, ("int" if all_int else "float")
 
 
-def auto_range(mins, maxs, nfinite):
-    """[lo, hi] per column for a binned request without ``range``, from the device's min / max / finite-count
-    pre-pass.  Degenerate cases get numpy.histogram's treatment instead of failing the job: no finite value ->
-    [0, 1]; constant column -> [v - 0.5, v + 0.5] (the neighbouring fp32 values where 0.5 is below half an ulp)."""
+def _bin_width_f32(lo, hi, nbins: int):
+    """(hi - lo) / nbins in fp32 round-to-nearest, as the histogram kernels compute it."""
+    with np.errstate(over="ignore", invalid="ignore"):
+        return np.float32(np.float32(np.float32(hi) - np.float32(lo)) / np.float32(nbins))
+
+
+def _f32_key(x) -> int:
+    """An integer that orders fp32 values as numbers do (-0.0 and +0.0 share 0)."""
+    b = int(np.float32(x).view(np.uint32))
+    return b if b < 0x80000000 else -(b & 0x7FFFFFFF)
+
+
+def _f32_of_key(k: int):
+    return np.uint32(k if k >= 0 else 0x80000000 | -k).view(np.float32)
+
+
+def auto_range(mins, maxs, nfinite, nbins: int):
+    """[lo, hi] per column for a ``nbins``-bin request without ``range``, from the device's min / max / finite-count
+    pre-pass.  Degenerate cases get a usable range instead of failing the job:
+
+    * no finite value: [0, 1], as numpy.histogram does for empty input;
+    * constant column v: [v - 0.5, v + 0.5] in fp32, numpy's rule.  Where 0.5 is below half an ulp (|v| >= 2^24) an edge
+      moves to the neighbouring fp32 value instead.  Where that neighbour overflows (v = +-FLT_MAX) the edge stays at v
+      and the other edge is the inward neighbour: the closed last (first) bin still holds v;
+    * (hi - lo) / nbins rounds to 0 in fp32 (min and max a few subnormals apart): hi rises to the smallest fp32 value for
+      which the width is positive.  The bins are about one subnormal ulp wide and max stays inside the range.
+
+    Where hi - lo overflows fp32 (e.g. min -3e38, max 3e38) no finite fp32 range has that width; [min, max] is returned
+    unchanged and the histogram call rejects it."""
+    nbins = int(nbins)
     lo = np.array(mins, dtype=np.float32)
     hi = np.array(maxs, dtype=np.float32)
+    inf = np.float32(np.inf)
     for j in range(lo.shape[0]):
         if int(nfinite[j]) == 0:
             lo[j], hi[j] = 0.0, 1.0
-        elif lo[j] == hi[j]:
+            continue
+        if lo[j] == hi[j]:
             v = lo[j]
             a, b = np.float32(v - np.float32(0.5)), np.float32(v + np.float32(0.5))
-            lo[j] = a if a != v else np.nextafter(v, np.float32(-np.inf), dtype=np.float32)
-            hi[j] = b if b != v else np.nextafter(v, np.float32(np.inf), dtype=np.float32)
+            with np.errstate(over="ignore"):
+                a = a if a != v else np.nextafter(v, -inf, dtype=np.float32)
+                b = b if b != v else np.nextafter(v, inf, dtype=np.float32)
+            if np.isinf(b):
+                b = v
+            if np.isinf(a):
+                a = v
+            lo[j], hi[j] = a, b
+        if _bin_width_f32(lo[j], hi[j], nbins) == 0:
+            # start above the answer (a width of one whole subnormal ulp per bin), then bisect on the ordered fp32 values
+            good = np.float32(float(lo[j]) + nbins * 2.0 ** -149)
+            while _bin_width_f32(lo[j], good, nbins) == 0:
+                good = np.nextafter(good, inf, dtype=np.float32)
+            bad_k, good_k = _f32_key(hi[j]), _f32_key(good)
+            while good_k - bad_k > 1:
+                mid = (good_k + bad_k) // 2
+                if _bin_width_f32(lo[j], _f32_of_key(mid), nbins) > 0:
+                    good_k = mid
+                else:
+                    bad_k = mid
+            hi[j] = _f32_of_key(good_k)
     return lo, hi
 
 

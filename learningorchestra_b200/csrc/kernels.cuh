@@ -1264,7 +1264,7 @@ __global__ void k_hash_compact(const unsigned long long *__restrict__ keys, cons
 // result is exact whatever the hash does.  Lanes of a warp with the same 64-bit hash are merged first
 // (match.any), after verifying byte equality with the group leader.
 // ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ unsigned long long hash_bytes(const uint8_t *p, long long len) {
+__host__ __device__ __forceinline__ unsigned long long hash_bytes(const uint8_t *p, long long len) {
     unsigned long long h = 0xCBF29CE484222325ull ^ (unsigned long long)len;
     for (long long i = 0; i < len; ++i) h = (h ^ p[i]) * 0x100000001B3ull;     // FNV-1a
     return splitmix64(h);

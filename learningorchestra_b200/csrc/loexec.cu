@@ -34,6 +34,9 @@ int fail(int code, const char *fmt, ...) {
     vsnprintf(buf, sizeof buf, fmt, ap);
     va_end(ap);
     g_err = buf;
+    // a failed runtime call also stays this thread's "last error" until read; read it here, or the next call's
+    // cudaGetLastError() after a launch would report it as its own (sticky errors of a broken context are unaffected)
+    (void)cudaGetLastError();
     return code;
 }
 
@@ -914,6 +917,9 @@ namespace {
 // One chunk of k host columns <-> k staging slabs.  Host columns that sit at a constant stride (one 2-D array, the
 // usual case: a numpy matrix, an Arrow table's buffers from one allocation) go as ONE strided 2-D copy per run instead
 // of one copy per column: 784 byte columns x 5 chunks would be 3 920 small submissions; a run is one.
+// Columns that are separate allocations can also sit at a constant stride (page-locked buffers allocated one after
+// another).  The runtime can reject a 2-D copy over such a run with cudaErrorInvalidValue, an argument check made
+// before anything is enqueued; the run is then copied column by column.
 int copy_cols(char *dev_base, int64_t dev_pitch, const void *const *host_cols, int64_t host_off, size_t bytes, int32_t k,
               bool to_device, cudaStream_t s) {
     for (int32_t j = 0; j < k;) {
@@ -923,16 +929,22 @@ int copy_cols(char *dev_base, int64_t dev_pitch, const void *const *host_cols, i
             while (e < k && (const char *)host_cols[e] - (const char *)host_cols[e - 1] == stride) ++e;
         else
             e = j + 1;
-        char *d = dev_base + (int64_t)j * dev_pitch;
-        char *h = (char *)host_cols[j] + host_off;
         if (e - j >= 2) {
-            if (to_device) LO_CUDA(cudaMemcpy2DAsync(d, (size_t)dev_pitch, h, (size_t)stride, bytes, (size_t)(e - j), cudaMemcpyHostToDevice, s));
-            else           LO_CUDA(cudaMemcpy2DAsync(h, (size_t)stride, d, (size_t)dev_pitch, bytes, (size_t)(e - j), cudaMemcpyDeviceToHost, s));
-        } else {
+            char *d = dev_base + (int64_t)j * dev_pitch;
+            char *h = (char *)host_cols[j] + host_off;
+            const cudaError_t r = to_device
+                ? cudaMemcpy2DAsync(d, (size_t)dev_pitch, h, (size_t)stride, bytes, (size_t)(e - j), cudaMemcpyHostToDevice, s)
+                : cudaMemcpy2DAsync(h, (size_t)stride, d, (size_t)dev_pitch, bytes, (size_t)(e - j), cudaMemcpyDeviceToHost, s);
+            if (r == cudaSuccess) { j = e; continue; }
+            if (r != cudaErrorInvalidValue) LO_CUDA(r);
+            (void)cudaGetLastError();
+        }
+        for (; j < e; ++j) {
+            char *d = dev_base + (int64_t)j * dev_pitch;
+            char *h = (char *)host_cols[j] + host_off;
             if (to_device) LO_CUDA(cudaMemcpyAsync(d, h, bytes, cudaMemcpyHostToDevice, s));
             else           LO_CUDA(cudaMemcpyAsync(h, d, bytes, cudaMemcpyDeviceToHost, s));
         }
-        j = e;
     }
     return LO_OK;
 }

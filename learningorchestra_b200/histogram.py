@@ -151,7 +151,7 @@ class Histogram:
         with self.engine.resident.lease(self.database_connector, parent_filename, fields) as data:
             cols = [data.column[f] for f in fields]            # nulls are NaN in the slabs: skipped by the kernel
             if value_range is None:
-                lo, hi = columnar.auto_range(*self.engine.minmax_cast(data.table, cols))   # constant / empty columns included
+                lo, hi = columnar.auto_range(*self.engine.minmax_cast(data.table, cols), bins)   # constant / empty columns included
             else:
                 lo = np.full(len(fields), value_range[0], np.float32)
                 hi = np.full(len(fields), value_range[1], np.float32)

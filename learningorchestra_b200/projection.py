@@ -99,7 +99,7 @@ class Projection:
             try:
                 if bins:
                     if value_range is None:
-                        lo, hi = columnar.auto_range(*self.__engine.minmax_cast(data.table, idx))
+                        lo, hi = columnar.auto_range(*self.__engine.minmax_cast(data.table, idx), int(bins))
                     else:
                         lo = np.full(len(selected), value_range[0], np.float32)
                         hi = np.full(len(selected), value_range[1], np.float32)
@@ -137,7 +137,7 @@ class Projection:
         counts = None
         if bins:
             if value_range is None:
-                lo, hi = columnar.auto_range(*self.__engine.minmax_cast_host(cols))
+                lo, hi = columnar.auto_range(*self.__engine.minmax_cast_host(cols), int(bins))
             else:
                 lo = np.full(len(selected), value_range[0], np.float32)
                 hi = np.full(len(selected), value_range[1], np.float32)

@@ -55,27 +55,47 @@ def bin_index_f32(x: np.ndarray, lo, hi, nbins: int) -> np.ndarray:
     return idx
 
 
-def auto_range(mins, maxs, nfinite):
-    """Range of a binned histogram request that carries no ``range`` (SURVEY.md §2.1 C2), per column, from the min /
-    max of the finite cast values.  B-semantics, frozen here (the reference defines no bins at all):
+def auto_range(mins, maxs, nfinite, nbins: int | None = None):
+    """Range of an ``nbins``-bin histogram request that carries no ``range`` (SURVEY.md §2.1 C2), per column, from the
+    min / max of the finite cast values.  B-semantics, frozen here (the reference defines no bins at all).  Without
+    ``nbins`` the last rule (which needs the bin count) is skipped; the result is the same for every column whose
+    min and max are at least 2^-133 apart, since no bin count up to LO_MAX_BINS can make their width round to 0:
 
     * no finite value (empty, all-null or all-NaN/inf column): [0, 1], as ``numpy.histogram`` does for empty input;
     * constant column (min == max): [min - 0.5, max + 0.5] in fp32, again numpy's rule; where +-0.5 is below half an
-      ulp (|v| >= 2^24) the edges move to the neighbouring fp32 values instead, so hi > lo always holds;
-    * otherwise [min, max] unchanged."""
+      ulp (|v| >= 2^24) the edges move to the neighbouring fp32 values instead, so hi > lo always holds; where such a
+      neighbour is +-inf (v = +-FLT_MAX) that edge stays at v and the other is the inward neighbour
+      (FLT_MAX -> [prev(FLT_MAX), FLT_MAX]: the closed last bin holds v);
+    * otherwise [min, max];
+    * then, if the fp32 width (hi - lo) / nbins rounds to 0, hi is raised to the smallest fp32 value h for which
+      (h - lo) / nbins does not (bins about one subnormal ulp wide, max still inside).
+    If hi - lo overflows fp32 the range is left as it is: no finite fp32 range of that width exists, and the histogram
+    rejects it."""
     lo = np.array(mins, dtype=np.float32).copy()
     hi = np.array(maxs, dtype=np.float32).copy()
     n = np.asarray(nfinite)
+    up, down = np.float32(np.inf), np.float32(-np.inf)
     for j in range(lo.shape[0]):
         if n[j] == 0:
             lo[j], hi[j] = np.float32(0.0), np.float32(1.0)
-        elif lo[j] == hi[j]:
-            a, b = np.float32(lo[j] - np.float32(0.5)), np.float32(hi[j] + np.float32(0.5))
-            if a == lo[j]:
-                a = np.nextafter(lo[j], np.float32(-np.inf), dtype=np.float32)
-            if b == hi[j]:
-                b = np.nextafter(hi[j], np.float32(np.inf), dtype=np.float32)
-            lo[j], hi[j] = a, b
+            continue
+        with np.errstate(over="ignore"):
+            if lo[j] == hi[j]:
+                v = lo[j]
+                a, b = np.float32(v - np.float32(0.5)), np.float32(v + np.float32(0.5))
+                if a == v:
+                    a = np.nextafter(v, down, dtype=np.float32)
+                if b == v:
+                    b = np.nextafter(v, up, dtype=np.float32)
+                if not np.isfinite(b):
+                    a, b = np.nextafter(v, down, dtype=np.float32), v
+                elif not np.isfinite(a):
+                    a, b = v, np.nextafter(v, up, dtype=np.float32)
+                lo[j], hi[j] = a, b
+            # the first fp32 value above max whose width is positive, one ulp at a time (at most about nbins / 2
+            # steps: the width is 0 only while hi - lo <= nbins * 2^-150)
+            while nbins is not None and bin_width(lo[j], hi[j], nbins) == 0:
+                hi[j] = np.nextafter(hi[j], up, dtype=np.float32)
     return lo, hi
 
 
