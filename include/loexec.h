@@ -151,6 +151,20 @@ int lo_table_checksum(lo_ctx *ctx, const lo_table *t, int32_t col, int64_t row_o
 int lo_selftest_fastdiv(lo_ctx *ctx, float lo, float hi, int32_t nbins, int *fast_path_used,
                         uint64_t *mismatches);
 
+/* Bin edges of the edge-table tile kernels (host only, no device needed): edges[0] = lo, edges[i] = the smallest fp32
+ * value in [lo, hi] whose bin is >= i (the next value above hi when bins i.. are empty), edges[nbins] = the next fp32
+ * value above hi.  edges: nbins + 1 floats. */
+int lo_hist_edges(float lo, float hi, int32_t nbins, float *edges);
+
+/* Every fp32 bit pattern through the edge-table binning of the tile kernels against the IEEE-divide bin (nbins <=
+ * LO_TILE_BINS).  *edges_used: whether histograms with this range take the edge-table kernels. */
+int lo_selftest_edges(lo_ctx *ctx, float lo, float hi, int32_t nbins, int *edges_used, uint64_t *mismatches);
+
+/* The context's cache of device edge tables: tables held now (at most 8, least recently used retired first), their
+ * bytes, and how many tile-kernel launches so far binned with the IEEE divide instead (bin widths outside
+ * [2^-100, 2^100]).  Any pointer may be NULL. */
+int lo_edge_tables_info(lo_ctx *ctx, int32_t *tables, uint64_t *bytes, int64_t *divide_launches);
+
 /* ---- the hot path, device-resident ------------------------------------------------------ */
 /* out[j][r] = cast(in[col_idx[j]][r]) for j < k.  in: LO_F64.  out: LO_F32 (fp64->fp32 RNE,
  * NaN -> 0x7fc00000) or LO_F64 (plain copy).  out->ncols >= k, out->nrows == in->nrows. */

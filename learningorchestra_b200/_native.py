@@ -87,6 +87,9 @@ SIGNATURES = {
     "lo_table_fill_synthetic_dev": (C.c_int, [_P, _P, C.c_int, C.c_uint64, C.c_int64, C.c_double, C.c_double, _P]),
     "lo_table_checksum": (C.c_int, [_P, _P, C.c_int32, C.c_int64, C.POINTER(C.c_uint64)]),
     "lo_selftest_fastdiv": (C.c_int, [_P, C.c_float, C.c_float, C.c_int32, C.POINTER(C.c_int), C.POINTER(C.c_uint64)]),
+    "lo_hist_edges": (C.c_int, [C.c_float, C.c_float, C.c_int32, _P]),
+    "lo_selftest_edges": (C.c_int, [_P, C.c_float, C.c_float, C.c_int32, C.POINTER(C.c_int), C.POINTER(C.c_uint64)]),
+    "lo_edge_tables_info": (C.c_int, [_P, C.POINTER(C.c_int32), C.POINTER(C.c_uint64), C.POINTER(C.c_int64)]),
     "lo_minmax_cast_dev": (C.c_int, [_P, _P, C.POINTER(C.c_int32), C.c_int32, _P, _P]),
     "lo_minmax_decode": (C.c_int, [_P, C.c_int32, _P, _P, _P]),
     "lo_project_cast_dev": (C.c_int, [_P, _P, C.POINTER(C.c_int32), C.c_int32, _P, _P]),

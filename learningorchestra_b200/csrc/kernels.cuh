@@ -25,8 +25,9 @@
 //   * several GPUs (GroupStep): the bins go to the device's own matrix; the CTA finishing a column's last tile pushes
 //     the column to the root GPU with system-scope RED.64 over NVLink, the last pusher arrives, the root's last CTA
 //     moves the merged matrix out — merge, arrival and epilogue ride inside the one streaming launch per step.
-//   * bin index = trunc(RN((x - lo) / w)) computed without a divide (hoisted reciprocal + two FMA
-//     corrections, proven and exhaustively self-tested equal to the IEEE quotient; bin_index_f32).
+//   * bin index = trunc(RN((x - lo) / w)): in the tile kernel from a table of exact bin edges (one FFMA estimate, one
+//     LDS.128, one comparison; edge_counter_offset), elsewhere without a divide (hoisted reciprocal + two FMA
+//     corrections; bin_index_f32) — both proven and exhaustively self-tested equal to the IEEE quotient.
 //   * also here: k_parse_number (CPython float() on the GPU, parse_number.cuh), k_format_number_len / _write (its
 //     inverse, CPython str(), format_number.cuh), k_hash_count_f64 / _str
 //     (exact group-by), k_minmax_cast, the group's small kernels (push, big-matrix merge, barrier), generators, checksum.
@@ -245,6 +246,64 @@ __device__ __forceinline__ void bump4(uint8_t *priv, int b0, int b1, int b2, int
     if (v3) *p3 = (uint8_t)c3;
 }
 
+// Binning from a bin-edge table (EDGES kernels, DESIGN.md §3.2.1).  bin_index_f32<false> is a monotone step function of the
+// fp32 value on [lo, hi], so it is fixed by its edges E[i] = the smallest fp32 f in [lo, hi] with bin(f) >= i.  The host
+// computes them exactly (hist_edges in loexec.cu) and passes E[0] = lo, E[1 .. nbins-1], E[nbins] = nextup(hi) per column.
+// Per element:
+//     t  = sat(RN(RN(f - lo) * r * 2^-9 + 2^-10)) * 2^9,  r = RN(1/w)          (one FADD, one FFMA.SAT)
+//     i0 = trunc(t)  in [0, 512]                         (FADD.RZ against 2^14: the integer part lands in the low bits)
+//     counter = f >= E[i0] ? counter(i0) : counter(i0 - 1)          (one LDS.128 of the table entry, FSETP, SEL)
+// For f in [lo, hi], |t - 0.5 - RN(RN(f - lo)/w)| <= (3 nbins + 4) 2^-24 < 0.5 whenever r and r 2^-9 are normal
+// (2^-100 <= w <= 2^100, edges_ok), so i0 is bin(f) or bin(f) + 1 and the one comparison picks the right one.  Below lo
+// (t < 1 or saturated to 0: i0 = 0, f < E[0] = lo), above hi (i0 >= nbins, f >= E[nbins] or E[i0 > nbins] = +inf) and
+// NaN (saturates to 0, fails every comparison) land on a per-thread trash counter instead of a bin, so the increment
+// needs no predicate.
+constexpr int      kEdgeSlots     = 513;                         // table entries, i0 = 0 .. 512
+constexpr uint32_t kTrashOffset   = kHistRows * kThreads * 4;    // byte offset (before 4*tid) of the trash counter: a
+                                                                 // word of the fold's scratch row, bank = tid % 32
+constexpr int      kEdgeSmemBytes = kHistSmemBytes + kEdgeSlots * 16;
+
+// entry i0: {E[i0] (+inf past nbins), counter offset of bin i0, of bin i0 - 1} with out-of-range bins -> trash
+__device__ __forceinline__ void load_edge_table(uint4 *tab, const float *__restrict__ E, int nbins) {
+    for (int i = threadIdx.x; i < kEdgeSlots; i += blockDim.x) {
+        const float e = i <= nbins ? E[i] : __int_as_float(0x7f800000);
+        const uint32_t off0  = i < nbins ? bin_byte_offset((uint32_t)i) : kTrashOffset;
+        const uint32_t offm1 = (i >= 1 && i <= nbins) ? bin_byte_offset((uint32_t)(i - 1)) : kTrashOffset;
+        tab[i] = make_uint4(__float_as_uint(e), off0, offm1, 0u);
+    }
+}
+
+struct EdgeParams {
+    float    lo, rs;     // rs = RN(1/w) * 2^-9
+    uint32_t tab_bits;   // shared-window address of the table minus 16 * 0x46800000 (mod 2^32): entry i0 of the
+                         // FADD.RZ result with bit pattern 0x46800000 + i0 is at tab_bits + 16 * bits, one LEA
+};
+
+__device__ __forceinline__ EdgeParams edge_params(float lo, float w, const uint4 *tab) {
+    // through a shuffle: ptxas cannot split the value back into window base + constant, which would cost an extra
+    // VIADD per element instead of one register operand of the LEA
+    const uint32_t base = __shfl_sync(0xffffffffu, (uint32_t)__cvta_generic_to_shared(tab) - 16u * 0x46800000u, 0);
+    return {lo, __frcp_rn(w) * 0x1p-9f, base};
+}
+
+// byte offset (before 4*tid) of f's counter: its bin's, or the trash counter
+__device__ __forceinline__ uint32_t edge_counter_offset(float f, const EdgeParams &E) {
+    const float t = __saturatef(__fmaf_rn(__fsub_rn(f, E.lo), E.rs, 0x1p-10f));
+    const uint32_t bits = __float_as_uint(__fadd_rz(t, 0x1p14f));                  // 2^14 + i0 * 2^-9
+    uint32_t e, off0, offm1, pad;
+    // the table is written before the barrier that precedes the streaming loop and is read-only afterwards
+    asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];"
+                 : "=r"(e), "=r"(off0), "=r"(offm1), "=r"(pad) : "r"(E.tab_bits + 16u * bits));
+    asm volatile("" :: "r"(pad));      // the entry's fourth word is padding
+    return f >= __uint_as_float(e) ? off0 : offm1;
+}
+
+// one increment, read-modify-write in program order: consecutive increments of one thread may hit the same counter
+__device__ __forceinline__ void bump_edge(uint8_t *priv, float f, const EdgeParams &E) {
+    uint8_t *p = priv + edge_counter_offset(f, E);
+    *p = (uint8_t)(*p + 1);
+}
+
 // ---------------------------------------------------------------------------------------------
 // CTA-wide fold of the private byte histograms -> RED.64 into counts[]
 // ---------------------------------------------------------------------------------------------
@@ -291,14 +350,18 @@ __device__ __forceinline__ void fold_and_flush(uint32_t *smem, int rows, int nbi
         r[2 * i] = even;
         r[2 * i + 1] = odd;
     }
+    // one step per power of two; `half` is a compile-time constant in every step, so r[] stays in registers
 #pragma unroll
-    for (int half = 8, bit = 16; half >= 1; half >>= 1, bit >>= 1) {
+    for (int s = 0; s < 4; ++s) {
+        const int half = 8 >> s, bit = 16 >> s;
         const bool upper = (lane & bit) != 0;
 #pragma unroll
-        for (int i = 0; i < half; ++i) {
-            const uint32_t send = upper ? r[i] : r[i + half];
-            const uint32_t keep = upper ? r[i + half] : r[i];
-            r[i] = keep + __shfl_xor_sync(0xffffffffu, send, bit);
+        for (int i = 0; i < 8; ++i) {
+            if (i < half) {
+                const uint32_t send = upper ? r[i] : r[i + half];
+                const uint32_t keep = upper ? r[i + half] : r[i];
+                r[i] = keep + __shfl_xor_sync(0xffffffffu, send, bit);
+            }
         }
     }
     const uint32_t total = r[0] + __shfl_xor_sync(0xffffffffu, r[0], 1);
@@ -473,14 +536,15 @@ __device__ __forceinline__ void group_finish_column(const GroupStep &G, unsigned
 //   OUT: 0 = no projected output (histogram only), 1 = f32 (cast), 2 = f64 (copy)
 //   HIST: accumulate per-column fixed-width histogram of the cast value
 //   ALIGNED: column slabs (in and out) are 32-byte aligned -> 128-bit loads, 64/128-bit stores
+//   EDGES: bin from the edge table `edges` (k x (nbins + 1) floats, edge_counter_offset); otherwise the IEEE divide
 // grid.x = k * tiles_per_col ; tile index fastest along rows
 // ---------------------------------------------------------------------------------------------
-template <int OUT, bool HIST, bool ALIGNED, bool FASTDIV>
+template <int OUT, bool HIST, bool ALIGNED, bool EDGES>
 __global__ void __launch_bounds__(kThreads, LO_MIN_CTAS)
 k_project_cast_hist(const char *__restrict__ in_base, long long in_pitch,
                     char *__restrict__ out_base, long long out_pitch,
                     long long nrows, unsigned tiles_per_col, unsigned long long *__restrict__ counts,
-                    const __grid_constant__ ColsF64 P, const __grid_constant__ GroupStep G) {
+                    const float *__restrict__ edges, const __grid_constant__ ColsF64 P, const __grid_constant__ GroupStep G) {
     extern __shared__ uint32_t smem[];
     // overlapped steps: the next launch may start filling SMs as soon as every CTA of this one is resident
     if (G.overlap) asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
@@ -504,6 +568,12 @@ k_project_cast_hist(const char *__restrict__ in_base, long long in_pitch,
         B.last = P.nbins - 1;
         rows = (P.nbins + 3) >> 2;
     }
+    EdgeParams E = {0.f, 0.f, 0u};
+    if (HIST && EDGES) {
+        uint4 *tab = reinterpret_cast<uint4 *>(reinterpret_cast<char *>(smem) + kHistSmemBytes);
+        load_edge_table(tab, edges + (long long)j * (P.nbins + 1), P.nbins);   // zero_private's barrier publishes it
+        E = edge_params(B.lo, B.w, tab);
+    }
 
     if (ALIGNED && n == kTileRows) {
         // full tile (all but the last tile of a column): no bounds checks, register-pipelined loads.
@@ -517,8 +587,13 @@ k_project_cast_hist(const char *__restrict__ in_base, long long in_pitch,
             for (int u = 0; u < kPfBatch; ++u)
                 ldg_split4_stream(src + (long long)(pb * kPfBatch + u) * kThreads * kVec, kHalf, v[pb][u]);
         if (HIST) zero_private(smem, rows);        // the first batch's DRAM latency overlaps the clearing and its barrier
+        // the addresses of a round of kPfBuf batches are fixed offsets from two pointers advanced once per round
+        const long long t2 = 2 * (long long)threadIdx.x;
 #pragma unroll 1
         for (int b0 = 0; b0 < kPfBatches; b0 += kPfBuf) {
+            const double *rsrc = src + (long long)b0 * (kPfBatch * kThreads * kVec);
+            float  *rout32 = (OUT == 1) ? out32 + t2 + (long long)b0 * (kPfBatch * kThreads * kVec) : nullptr;
+            double *rout64 = (OUT == 2) ? out64 + t2 + (long long)b0 * (kPfBatch * kThreads * kVec) : nullptr;
 #pragma unroll
             for (int s = 0; s < kPfBuf; ++s) {
                 const int b  = b0 + s;                 // batch being processed, lives in buffer s
@@ -526,19 +601,22 @@ k_project_cast_hist(const char *__restrict__ in_base, long long in_pitch,
                 if (nb < kPfBatches) {
 #pragma unroll
                     for (int u = 0; u < kPfBatch; ++u)
-                        ldg_split4_stream(src + (long long)(nb * kPfBatch + u) * kThreads * kVec, kHalf,
+                        ldg_split4_stream(rsrc + ((s + kPfBuf - 1) * kPfBatch + u) * kThreads * kVec, kHalf,
                                           v[(s + kPfBuf - 1) % kPfBuf][u]);
                 }
 #pragma unroll
                 for (int u = 0; u < kPfBatch; ++u) {
-                    const long long e = (long long)(b * kPfBatch + u) * kThreads * kVec + 2 * threadIdx.x;
+                    const int e = (s * kPfBatch + u) * kThreads * kVec;    // from rout32 / rout64
                     float f0 = cast_f64_f32(v[s][u][0]), f1 = cast_f64_f32(v[s][u][1]);
                     float f2 = cast_f64_f32(v[s][u][2]), f3 = cast_f64_f32(v[s][u][3]);
-                    if (OUT == 1) stg_split4_stream(out32 + e, kHalf, f0, f1, f2, f3);
-                    if (OUT == 2) stg_split4_stream(out64 + e, kHalf, v[s][u]);
-                    if (HIST)
-                        bump4(priv, bin_index_f32<FASTDIV>(f0, B), bin_index_f32<FASTDIV>(f1, B),
-                              bin_index_f32<FASTDIV>(f2, B), bin_index_f32<FASTDIV>(f3, B));
+                    if (OUT == 1) stg_split4_stream(rout32 + e, kHalf, f0, f1, f2, f3);
+                    if (OUT == 2) stg_split4_stream(rout64 + e, kHalf, v[s][u]);
+                    if (HIST && EDGES) {
+                        bump_edge(priv, f0, E); bump_edge(priv, f1, E); bump_edge(priv, f2, E); bump_edge(priv, f3, E);
+                    } else if (HIST) {
+                        bump4(priv, bin_index_f32<false>(f0, B), bin_index_f32<false>(f1, B),
+                              bin_index_f32<false>(f2, B), bin_index_f32<false>(f3, B));
+                    }
                 }
             }
         }
@@ -560,9 +638,12 @@ k_project_cast_hist(const char *__restrict__ in_base, long long in_pitch,
                     float f2 = cast_f64_f32(v[u][2]), f3 = cast_f64_f32(v[u][3]);
                     if (OUT == 1) stg_split4_stream(out32 + e, kHalf, f0, f1, f2, f3);
                     if (OUT == 2) stg_split4_stream(out64 + e, kHalf, v[u]);
-                    if (HIST)
-                        bump4(priv, bin_index_f32<FASTDIV>(f0, B), bin_index_f32<FASTDIV>(f1, B),
-                              bin_index_f32<FASTDIV>(f2, B), bin_index_f32<FASTDIV>(f3, B));
+                    if (HIST && EDGES) {
+                        bump_edge(priv, f0, E); bump_edge(priv, f1, E); bump_edge(priv, f2, E); bump_edge(priv, f3, E);
+                    } else if (HIST) {
+                        bump4(priv, bin_index_f32<false>(f0, B), bin_index_f32<false>(f1, B),
+                              bin_index_f32<false>(f2, B), bin_index_f32<false>(f3, B));
+                    }
                 }
             } else {
                 // ragged end of the column: element-wise over the same four positions per vector
@@ -577,7 +658,8 @@ k_project_cast_hist(const char *__restrict__ in_base, long long in_pitch,
                             float  f = cast_f64_f32(x);
                             if (OUT == 1) out32[eq] = f;
                             if (OUT == 2) out64[eq] = x;
-                            if (HIST) bin_f32<FASTDIV>(priv, f, B);
+                            if (HIST && EDGES) bump_edge(priv, f, E);
+                            else if (HIST) bin_f32<false>(priv, f, B);
                         }
                     }
                 }
@@ -594,7 +676,8 @@ k_project_cast_hist(const char *__restrict__ in_base, long long in_pitch,
             float  f = cast_f64_f32(x);
             if (OUT == 1) out32[e] = f;
             if (OUT == 2) out64[e] = x;
-            if (HIST) bin_f32<FASTDIV>(priv, f, B);
+            if (HIST && EDGES) bump_edge(priv, f, E);
+            else if (HIST) bin_f32<false>(priv, f, B);
         }
     }
 
@@ -1369,6 +1452,27 @@ __global__ void k_selftest_fastdiv(float lo, float hi, float w, int nbins, unsig
          i += (unsigned long long)gridDim.x * blockDim.x) {
         const float f = __uint_as_float((unsigned)i);
         bad += bin_index_f32<true>(f, B) != bin_index_f32<false>(f, B);
+    }
+#pragma unroll
+    for (int s = 16; s > 0; s >>= 1) bad += __shfl_xor_sync(0xffffffffu, bad, s);
+    if ((threadIdx.x & 31) == 0 && bad) atomicAdd(mismatches, bad);
+}
+
+// every fp32 bit pattern: the edge-table counter (edge_counter_offset, as the EDGES kernels use it) against the counter of
+// the IEEE-divide bin, or the trash counter where that skips the value
+__global__ void __launch_bounds__(256) k_selftest_edges(float lo, float hi, float w, int nbins, const float *edges,
+                                                        unsigned long long *mismatches) {
+    __shared__ uint4 tab[kEdgeSlots];
+    load_edge_table(tab, edges, nbins);
+    __syncthreads();
+    const EdgeParams E = edge_params(lo, w, tab);
+    const BinParams B = {lo, hi, w, __frcp_rn(w), nbins - 1};
+    unsigned long long bad = 0;
+    for (unsigned long long i = blockIdx.x * (unsigned long long)blockDim.x + threadIdx.x; i < (1ull << 32);
+         i += (unsigned long long)gridDim.x * blockDim.x) {
+        const float f = __uint_as_float((unsigned)i);
+        const int b = bin_index_f32<false>(f, B);
+        bad += edge_counter_offset(f, E) != (b >= 0 ? bin_byte_offset((uint32_t)b) : kTrashOffset);
     }
 #pragma unroll
     for (int s = 16; s > 0; s >>= 1) bad += __shfl_xor_sync(0xffffffffu, bad, s);

@@ -8,6 +8,7 @@
 
 #include <cub/device/device_scan.cuh>
 
+#include <algorithm>
 #include <atomic>
 #include <condition_variable>
 #include <cctype>
@@ -17,6 +18,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <memory>
 #include <mutex>
 #include <new>
 #include <string>
@@ -91,6 +93,20 @@ struct StageSet {
     cudaEvent_t  ev_h2d[kSlots] = {}, ev_k[kSlots] = {}, ev_d2h[kSlots] = {};
 };
 
+// One device bin-edge table of the EDGES tile kernels: k x (nbins + 1) floats, E[0] = lo, E[1 .. nbins-1],
+// E[nbins] = nextup(hi) per column.  Uploaded on the context's edge stream; every launch that reads it waits for `ready`
+// and records an event in `uses`, so a retired table is freed in stream order after its last reader.
+struct EdgeTable {
+    int32_t            nbins = 0;
+    std::vector<float> lo, hi;
+    float             *dev = nullptr;
+    size_t             bytes = 0;
+    cudaEvent_t        ready = nullptr;
+    std::vector<cudaEvent_t> uses;      // launches that read the table and may still be running
+    uint64_t           last_use = 0;
+};
+constexpr int kEdgeTables = 8;          // tables cached per context (least recently used one retired first)
+
 struct lo_ctx {
     int          device;
     int          sm_count;
@@ -105,6 +121,13 @@ struct lo_ctx {
     std::condition_variable pool_cv;
     std::vector<StageSet *> free_sets;
     int          nsets = 0;
+    // bin-edge tables of the EDGES tile kernels, one per (nbins, lo[], hi[]) of a launch, at most kEdgeTables; edge_mu
+    // is held from the lookup until the launch that reads the table has recorded its event
+    std::mutex   edge_mu;
+    cudaStream_t edge_stream = nullptr;
+    std::vector<std::unique_ptr<EdgeTable>> edge_tables;
+    uint64_t     edge_tick = 0;
+    std::atomic<int64_t> divide_launches{0};   // tile-kernel launches that binned with the IEEE divide (w outside the window)
 };
 
 namespace {
@@ -150,17 +173,17 @@ int check_spec(const lo_hist_spec *spec, int32_t k, float *w_out /* k */) {
 }
 
 template <typename K>
-int allow_smem(K kernel) {
-    LO_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, lo::kHistSmemBytes));
+int allow_smem(K kernel, int bytes) {
+    LO_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
     return LO_OK;
 }
 
 template <int OUT>
 int allow_smem_hist() {
-    LO_TRY(allow_smem(lo::k_project_cast_hist<OUT, true, true, true>));
-    LO_TRY(allow_smem(lo::k_project_cast_hist<OUT, true, true, false>));
-    LO_TRY(allow_smem(lo::k_project_cast_hist<OUT, true, false, true>));
-    LO_TRY(allow_smem(lo::k_project_cast_hist<OUT, true, false, false>));
+    LO_TRY(allow_smem(lo::k_project_cast_hist<OUT, true, true, true>, lo::kEdgeSmemBytes));
+    LO_TRY(allow_smem(lo::k_project_cast_hist<OUT, true, true, false>, lo::kHistSmemBytes));
+    LO_TRY(allow_smem(lo::k_project_cast_hist<OUT, true, false, true>, lo::kEdgeSmemBytes));
+    LO_TRY(allow_smem(lo::k_project_cast_hist<OUT, true, false, false>, lo::kHistSmemBytes));
     return LO_OK;
 }
 
@@ -172,6 +195,152 @@ bool fastdiv_ok(float w) {
     memcpy(&bits, &w, 4);
     if ((bits & 0x007FFFFFu) == 0x007FFFFFu) return false;
     return w >= 0x1p-100f && w <= 0x1p100f;
+}
+
+// The edge-table kernels need r = RN(1/w) and r * 2^-9 normal (kernels.cuh, edge_counter_offset).
+bool edges_ok(float w) { return w >= 0x1p-100f && w <= 0x1p100f; }
+
+// host twin of bin_index_f32<false> for f in [lo, hi]: fp32 RN subtract, fp32 RN divide, truncate, close the last bin
+int bin_ieee_host(float f, float lo, float w, int last) {
+    volatile float d = f - lo;
+    volatile float q = d / w;
+    const int i = (int)q;
+    return i < last ? i : last;
+}
+
+// fp32 <-> integer keys in value order (-0 and +0 share key 0)
+int32_t f32_key(float f) {
+    int32_t b;
+    memcpy(&b, &f, 4);
+    return b >= 0 ? b : -(b & 0x7FFFFFFF);
+}
+float key_f32(int32_t k) {
+    const uint32_t b = k >= 0 ? (uint32_t)k : (0x80000000u | (uint32_t)(-(int64_t)k));
+    float f;
+    memcpy(&f, &b, 4);
+    return f;
+}
+
+// E[0] = lo; E[i] = the smallest fp32 f in [lo, hi] with bin(f) >= i (nextup(hi) when no such f exists: bins i.. are
+// empty); E[nbins] = nextup(hi).  w as check_spec computes it.  Search over the ordered keys: start at lo + i*w, gallop
+// outwards until the edge is bracketed (a few ulps as a rule), then bisect; every answer is checked by the bracket
+// itself, the estimate only decides how fast it is found.
+void hist_edges(float lo, float hi, float w, int32_t nbins, float *E) {
+    const int last = nbins - 1;
+    const int64_t khi = f32_key(hi);
+    const float above = std::nextafter(hi, INFINITY);
+    auto at_or_above = [&](int64_t k, int32_t i) { return bin_ieee_host(key_f32((int32_t)k), lo, w, last) >= i; };
+    E[0] = lo;
+    int64_t floor_k = f32_key(lo);                         // every key below it bins below i (edges ascend)
+    for (int32_t i = 1; i < nbins; ++i) {
+        if (!at_or_above(khi, i)) { E[i] = above; continue; }
+        const int64_t g = std::min(khi, std::max(floor_k, (int64_t)f32_key((float)((double)lo + (double)i * w))));
+        int64_t a, b;                                      // invariant: key a bins below i (or a < floor_k), b at/above
+        if (at_or_above(g, i)) {
+            b = g;
+            for (int64_t step = 1;; step *= 2) {
+                a = b - step;
+                if (a < floor_k) { a = floor_k - 1; break; }
+                if (!at_or_above(a, i)) break;
+                b = a;
+            }
+        } else {
+            a = g;
+            for (int64_t step = 1;; step *= 2) {
+                b = a + step;
+                if (b >= khi) { b = khi; break; }
+                if (at_or_above(b, i)) break;
+                a = b;
+            }
+        }
+        while (b - a > 1) {
+            const int64_t m = a + (b - a) / 2;
+            if (at_or_above(m, i)) b = m; else a = m;
+        }
+        E[i] = key_f32((int32_t)b);
+        floor_k = b;
+    }
+    E[nbins] = above;
+}
+
+// Free a table in stream order: the edge stream waits for every launch that read it (and, by stream order, for its
+// upload), then frees it.  No host wait.
+void edge_retire(lo_ctx *ctx, EdgeTable *t) {
+    for (cudaEvent_t e : t->uses) {
+        cudaStreamWaitEvent(ctx->edge_stream, e, 0);
+        cudaEventDestroy(e);
+    }
+    t->uses.clear();
+    if (t->ready) cudaEventDestroy(t->ready);
+    if (t->dev) cudaFreeAsync(t->dev, ctx->edge_stream);
+    t->ready = nullptr;
+    t->dev = nullptr;
+}
+
+// The edge table of P's columns for a launch on stream s (ctx->edge_mu held by the caller until edge_used): cached, or
+// built now in place of the least recently used one.  *out = nullptr when a width is outside the window (IEEE kernels).
+int edge_acquire(lo_ctx *ctx, const lo::ColsF64 &P, cudaStream_t s, EdgeTable **out) {
+    *out = nullptr;
+    for (int j = 0; j < P.k; ++j)
+        if (!edges_ok(P.w[j])) return LO_OK;
+    EdgeTable *t = nullptr;
+    for (const auto &c : ctx->edge_tables)
+        if (c->nbins == P.nbins && (int)c->lo.size() == P.k && std::equal(c->lo.begin(), c->lo.end(), P.lo) &&
+            std::equal(c->hi.begin(), c->hi.end(), P.hi)) {
+            t = c.get();
+            break;
+        }
+    if (!t) {
+        if ((int)ctx->edge_tables.size() >= kEdgeTables) {
+            auto lru = std::min_element(ctx->edge_tables.begin(), ctx->edge_tables.end(),
+                                        [](const auto &x, const auto &y) { return x->last_use < y->last_use; });
+            edge_retire(ctx, lru->get());
+            ctx->edge_tables.erase(lru);
+        }
+        auto nt = std::make_unique<EdgeTable>();
+        nt->nbins = P.nbins;
+        nt->lo.assign(P.lo, P.lo + P.k);
+        nt->hi.assign(P.hi, P.hi + P.k);
+        const size_t n = (size_t)P.k * (P.nbins + 1);
+        nt->bytes = n * 4;
+        std::vector<float> h(n);
+        for (int j = 0; j < P.k; ++j) hist_edges(P.lo[j], P.hi[j], P.w[j], P.nbins, h.data() + (size_t)j * (P.nbins + 1));
+        // pageable source: the copy has taken the host bytes when it returns; `ready` marks its arrival on the device
+        cudaError_t e = cudaMallocAsync((void **)&nt->dev, nt->bytes, ctx->edge_stream);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(nt->dev, h.data(), nt->bytes, cudaMemcpyHostToDevice, ctx->edge_stream);
+        if (e == cudaSuccess) e = cudaEventCreateWithFlags(&nt->ready, cudaEventDisableTiming);
+        if (e == cudaSuccess) e = cudaEventRecord(nt->ready, ctx->edge_stream);
+        if (e != cudaSuccess) {
+            edge_retire(ctx, nt.get());
+            return fail(e == cudaErrorMemoryAllocation ? LO_ERR_NOMEM : LO_ERR_CUDA, "edge table upload: %s",
+                        cudaGetErrorString(e));
+        }
+        t = nt.get();
+        ctx->edge_tables.push_back(std::move(nt));
+    }
+    LO_CUDA(cudaStreamWaitEvent(s, t->ready, 0));
+    t->last_use = ++ctx->edge_tick;
+    *out = t;
+    return LO_OK;
+}
+
+// after a launch on s that reads t: remember it (and forget the readers that have finished)
+int edge_used(EdgeTable *t, cudaStream_t s) {
+    t->uses.erase(std::remove_if(t->uses.begin(), t->uses.end(), [](cudaEvent_t e) {
+                      if (cudaEventQuery(e) != cudaSuccess) return false;
+                      cudaEventDestroy(e);
+                      return true;
+                  }), t->uses.end());
+    (void)cudaGetLastError();       // cudaEventQuery's cudaErrorNotReady is not an error of this call
+    cudaEvent_t e = nullptr;
+    LO_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+    const cudaError_t r = cudaEventRecord(e, s);
+    if (r != cudaSuccess) {
+        cudaEventDestroy(e);
+        return fail(LO_ERR_CUDA, "edge table use: %s", cudaGetErrorString(r));
+    }
+    t->uses.push_back(e);
+    return LO_OK;
 }
 
 template <typename K>
@@ -225,10 +394,21 @@ cudaError_t launch_kernel(void (*kernel)(KArgs...), unsigned grid, unsigned bloc
 template <int OUT, bool HIST>
 int launch_f64(lo_ctx *ctx, const lo_table *in, const lo_table *out, int32_t out_col0,
                const lo::ColsF64 &P, unsigned long long *counts, bool aligned, const lo::GroupStep &G, cudaStream_t s) {
-    const size_t smem = HIST ? lo::kHistSmemBytes : 0;
+    std::unique_lock<std::mutex> edge_lock(ctx->edge_mu, std::defer_lock);
+    EdgeTable *et = nullptr;
+    if (HIST) {
+        edge_lock.lock();
+        LO_TRY(edge_acquire(ctx, P, s, &et));
+        if (!et) {
+            edge_lock.unlock();
+            ctx->divide_launches.fetch_add(1, std::memory_order_relaxed);
+        }
+    }
+    const float *edges = et ? et->dev : nullptr;
+    const size_t smem = !HIST ? 0 : edges ? lo::kEdgeSmemBytes : lo::kHistSmemBytes;
     char *out_base = out ? out->base + (int64_t)out_col0 * out->pitch : nullptr;
     const long long out_pitch = out ? out->pitch : 0;
-    bool fast = HIST;
+    bool fast = HIST;     // the TMA kernel's divide
     for (int j = 0; HIST && j < P.k; ++j) fast = fast && fastdiv_ok(P.w[j]);
     // LOEXEC_TMA=1: stage the slabs through shared memory with the bulk-copy engine (A/B variant, DESIGN §3.8).
     // Only full tiles; the ragged last tile of each column (and unaligned / slow-divide / group cases) keep the LDG kernel.
@@ -245,12 +425,13 @@ int launch_f64(lo_ctx *ctx, const lo_table *in, const lo_table *out, int32_t out
         // the remaining rows of every column: one ragged tile each, through the regular kernel on a row-offset view
         const char *ib = in->base + done * 8;
         char *ob = out ? out->base + done * (int64_t)dtype_size(out->dtype) + (int64_t)out_col0 * out->pitch : nullptr;
-        if (fast) lo::k_project_cast_hist<OUT, HIST, true, true><<<(unsigned)P.k, lo::kThreads, smem, s>>>(
-                      ib, in->pitch, ob, out_pitch, in->nrows - done, 1u, counts, P, kNoGroup);
-        else      lo::k_project_cast_hist<OUT, HIST, true, false><<<(unsigned)P.k, lo::kThreads, smem, s>>>(
-                      ib, in->pitch, ob, out_pitch, in->nrows - done, 1u, counts, P, kNoGroup);
+        if (edges) lo::k_project_cast_hist<OUT, HIST, true, true><<<(unsigned)P.k, lo::kThreads, smem, s>>>(
+                       ib, in->pitch, ob, out_pitch, in->nrows - done, 1u, counts, edges, P, kNoGroup);
+        else       lo::k_project_cast_hist<OUT, HIST, true, false><<<(unsigned)P.k, lo::kThreads, smem, s>>>(
+                       ib, in->pitch, ob, out_pitch, in->nrows - done, 1u, counts, edges, P, kNoGroup);
         LO_CUDA(cudaGetLastError());
         ctx->launches.fetch_add(1, std::memory_order_relaxed);
+        if (et) LO_TRY(edge_used(et, s));
         return LO_OK;
     }
     // one tile (kTileRows rows of one projected column) per CTA.  A tapered tail — the last wave cut into short
@@ -261,14 +442,15 @@ int launch_f64(lo_ctx *ctx, const lo_table *in, const lo_table *out, int32_t out
     if (blocks > 0x7fffffffull) return fail(LO_ERR_INVALID, "table too large for one launch (%llu tiles)", blocks);
     const char *ib = in->base;
     const long long ip = in->pitch, nr = in->nrows;
-#define LO_LAUNCH(AL, FD)                                                                                        \
-    LO_CUDA(launch_kernel(lo::k_project_cast_hist<OUT, HIST, AL, FD>, (unsigned)blocks, lo::kThreads, smem, s,    \
-                          G.overlap != 0, ib, ip, out_base, out_pitch, nr, tiles_per_col, counts, P, G))
-    if (aligned) { if (fast) LO_LAUNCH(true, true); else LO_LAUNCH(true, false); }
-    else         { if (fast) LO_LAUNCH(false, true); else LO_LAUNCH(false, false); }
+#define LO_LAUNCH(AL, ED)                                                                                        \
+    LO_CUDA(launch_kernel(lo::k_project_cast_hist<OUT, HIST, AL, ED>, (unsigned)blocks, lo::kThreads, smem, s,    \
+                          G.overlap != 0, ib, ip, out_base, out_pitch, nr, tiles_per_col, counts, edges, P, G))
+    if (aligned) { if (edges) LO_LAUNCH(true, true); else LO_LAUNCH(true, false); }
+    else         { if (edges) LO_LAUNCH(false, true); else LO_LAUNCH(false, false); }
 #undef LO_LAUNCH
     LO_CUDA(cudaGetLastError());
     ctx->launches.fetch_add(1, std::memory_order_relaxed);
+    if (et) LO_TRY(edge_used(et, s));
     return LO_OK;
 }
 
@@ -553,6 +735,7 @@ int lo_init(int device, lo_ctx **out) {
     ctx->stream = nullptr;
     auto setup = [&]() -> int {
         LO_CUDA(cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking));
+        LO_CUDA(cudaStreamCreateWithFlags(&ctx->edge_stream, cudaStreamNonBlocking));
         // scratch of the parser / group-by calls comes from the device's stream-ordered pool: keep up to 8 GiB of it
         // mapped between calls (the default threshold of 0 hands everything back at every synchronise, and the next
         // call pays the mapping again)
@@ -581,6 +764,12 @@ int lo_shutdown(lo_ctx *ctx) {
     cudaDeviceSynchronize();
     for (StageSet *st : ctx->free_sets) stage_set_destroy(st);
     ctx->free_sets.clear();
+    if (ctx->edge_stream) {
+        for (const auto &t : ctx->edge_tables) edge_retire(ctx, t.get());
+        cudaStreamSynchronize(ctx->edge_stream);
+        cudaStreamDestroy(ctx->edge_stream);
+    }
+    ctx->edge_tables.clear();
     if (ctx->stream) cudaStreamDestroy(ctx->stream);
     delete ctx;
     return LO_OK;
@@ -812,6 +1001,56 @@ int lo_selftest_fastdiv(lo_ctx *ctx, float lo_v, float hi_v, int32_t nbins, int 
     cudaFree(d);
     if (e != cudaSuccess) return fail(LO_ERR_CUDA, "selftest: %s", cudaGetErrorString(e));
     *mismatches = h;
+    return LO_OK;
+}
+
+int lo_hist_edges(float lo_v, float hi_v, int32_t nbins, float *edges) {
+    if (!edges) return fail(LO_ERR_INVALID, "edges is NULL");
+    lo_hist_spec spec = {nbins, 0, &lo_v, &hi_v};
+    float w = 0.f;
+    LO_TRY(check_spec(&spec, 1, &w));
+    hist_edges(lo_v, hi_v, w, nbins, edges);
+    return LO_OK;
+}
+
+int lo_edge_tables_info(lo_ctx *ctx, int32_t *tables, uint64_t *bytes, int64_t *divide_launches) {
+    if (!ctx) return fail(LO_ERR_INVALID, "ctx is NULL");
+    std::lock_guard<std::mutex> g(ctx->edge_mu);
+    uint64_t b = 0;
+    for (const auto &t : ctx->edge_tables) b += t->bytes;
+    if (tables) *tables = (int32_t)ctx->edge_tables.size();
+    if (bytes) *bytes = b;
+    if (divide_launches) *divide_launches = ctx->divide_launches.load(std::memory_order_relaxed);
+    return LO_OK;
+}
+
+int lo_selftest_edges(lo_ctx *ctx, float lo_v, float hi_v, int32_t nbins, int *edges_used, uint64_t *mismatches) {
+    LO_TRY(check_ctx(ctx));
+    if (!mismatches) return fail(LO_ERR_INVALID, "mismatches is NULL");
+    if (nbins > LO_TILE_BINS) return fail(LO_ERR_INVALID, "nbins = %d: the edge-table kernels take <= %d", nbins, LO_TILE_BINS);
+    lo_hist_spec spec = {nbins, 0, &lo_v, &hi_v};
+    float w = 0.f;
+    LO_TRY(check_spec(&spec, 1, &w));
+    if (edges_used) *edges_used = edges_ok(w) ? 1 : 0;
+    std::vector<float> h((size_t)nbins + 1);
+    hist_edges(lo_v, hi_v, w, nbins, h.data());
+    unsigned long long *d = nullptr;
+    float *E = nullptr;
+    LO_CUDA(cudaMalloc((void **)&d, 8 + h.size() * 4));
+    E = reinterpret_cast<float *>(d + 1);
+    cudaError_t e = cudaMemcpyAsync(E, h.data(), h.size() * 4, cudaMemcpyHostToDevice, ctx->stream);
+    if (e == cudaSuccess) e = cudaMemsetAsync(d, 0, 8, ctx->stream);
+    if (e == cudaSuccess) {
+        lo::k_selftest_edges<<<ctx->sm_count * 16, 256, 0, ctx->stream>>>(lo_v, hi_v, w, nbins, E, d);
+        e = cudaGetLastError();
+        ctx->launches.fetch_add(1, std::memory_order_relaxed);
+    }
+    unsigned long long bad = 0;
+    if (e == cudaSuccess) e = cudaMemcpyAsync(&bad, d, 8, cudaMemcpyDeviceToHost, ctx->stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
+    cudaFree(d);
+    if (e != cudaSuccess) return fail(LO_ERR_CUDA, "selftest: %s", cudaGetErrorString(e));
+    *mismatches = bad;
     return LO_OK;
 }
 

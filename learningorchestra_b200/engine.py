@@ -243,6 +243,18 @@ class Engine:
         N.check(self._lib.lo_selftest_fastdiv(self._ctx, float(lo), float(hi), int(nbins), C.byref(used), C.byref(bad)))
         return bool(used.value), int(bad.value)
 
+    def edge_tables_info(self) -> tuple[int, int, int]:
+        """(edge tables cached on the context, their bytes, tile launches that binned with the IEEE divide)."""
+        n, b, d = C.c_int32(), C.c_uint64(), C.c_int64()
+        N.check(self._lib.lo_edge_tables_info(self._ctx, C.byref(n), C.byref(b), C.byref(d)))
+        return int(n.value), int(b.value), int(d.value)
+
+    def selftest_edges(self, lo: float, hi: float, nbins: int) -> tuple[bool, int]:
+        """(edge-table kernels would be used, number of fp32 bit patterns whose counter differs from the IEEE-divide bin's)."""
+        used, bad = C.c_int(), C.c_uint64()
+        N.check(self._lib.lo_selftest_edges(self._ctx, float(lo), float(hi), int(nbins), C.byref(used), C.byref(bad)))
+        return bool(used.value), int(bad.value)
+
     # ---- hot path, device resident ---------------------------------------------------------------
     def _spec(self, k: int, nbins: int, lo, hi, flags: int = 0):
         lo_a = (C.c_float * k)(*[float(v) for v in np.broadcast_to(np.asarray(lo, dtype=np.float32), (k,))])
