@@ -338,6 +338,44 @@ int lo_format_number_host(lo_ctx *ctx, const double *values, const uint8_t *stat
 int lo_minmax_cast_host(lo_ctx *ctx, const double *const *in_cols, int64_t nrows, int32_t k,
                         float *mins, float *maxs, uint64_t *nfinite, lo_host_timing *timing);
 
+/* CSV text -> text columns: the reference's upload reader, csv.reader(codecs.iterdecode(response.iter_lines(),
+ * "utf-8"), delimiter=",", quotechar='"') followed by __treat_row (database_api_image/database.py:110-137), tokenised on
+ * the GPU.  Lines end at every run of '\r' / '\n' (blank lines vanish, a line break inside quotes is dropped); fields
+ * follow CPython's _csv reader with the default dialect; a field holds at most 131072 code points; UTF-8 is decoded
+ * strictly line by line; NUL is rejected (Python 3.7's _csv).  Record 0 is the header and fixes ncols; a data record
+ * with more fields keeps the first ncols, one with fewer fails.
+ *
+ * lo_csv_read_host copies the body to the device, tokenises it and keeps the columns of every record before the first
+ * failing one on the device.  info->records = header + kept data rows (0 when the header itself fails or the body has
+ * no record); info->fail_record = the failing record (-1: none), info->fail_kind = why, info->fail_pos = the byte
+ * offset the failure was raised at (line start for LO_CSV_BAD_UTF8 / LO_CSV_UNSUPPORTED; -1 for LO_CSV_SHORT_ROW and
+ * LO_CSV_EMPTY).  The device needs about the body, 0.5 bytes per body byte of scratch, 8 bytes per kept cell and the
+ * text; more than is free -> LO_ERR_NOMEM naming the size.
+ * lo_csv_columns_host: offsets host int64[ncols][records + 1] (column c's cell r = chars[offsets[c][r] ..
+ * offsets[c][r+1]), absolute in ONE column-major chars buffer: the buffers of Arrow large_string arrays) and chars
+ * (info->chars bytes; chars_capacity smaller -> LO_ERR_INVALID).  lo_csv_free releases the handle (NULL is fine). */
+#define LO_CSV_OK           0
+#define LO_CSV_SHORT_ROW    1   /* a data record has fewer fields than the header (IndexError in __treat_row)     */
+#define LO_CSV_FIELD_LIMIT  2   /* a field of more than 131072 code points (_csv.Error)                          */
+#define LO_CSV_BAD_UTF8     3   /* a line is not valid UTF-8 (UnicodeDecodeError)                                */
+#define LO_CSV_NUL          4   /* a line contains NUL (_csv.Error in Python 3.7)                                */
+#define LO_CSV_UNSUPPORTED  5   /* a line ends inside a UTF-8 sequence: the decoder would join it with the next   */
+#define LO_CSV_EMPTY        6   /* no record at all (StopIteration reading the header)                           */
+typedef struct lo_csv lo_csv;
+typedef struct lo_csv_info {
+    int64_t records;       /* header + kept data rows */
+    int64_t ncols;
+    int64_t chars;         /* bytes of text of all kept cells */
+    int64_t fail_record;
+    int32_t fail_kind;     /* LO_CSV_* */
+    int32_t pad;
+    int64_t fail_pos;
+} lo_csv_info;
+int lo_csv_read_host(lo_ctx *ctx, const uint8_t *body, int64_t nbytes, lo_csv **out, lo_csv_info *info,
+                     lo_host_timing *timing);
+int lo_csv_columns_host(lo_csv *h, int64_t *offsets, uint8_t *chars, int64_t chars_capacity, lo_host_timing *timing);
+int lo_csv_free(lo_csv *h);
+
 #ifdef __cplusplus
 }
 #endif

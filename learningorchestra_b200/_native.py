@@ -34,6 +34,7 @@ LO_GROUP_MAX_DEVICES = 16
 LO_GROUP_MAX_COUNTS = 262144
 LO_NUM_FLOAT, LO_NUM_INTEGER, LO_NUM_EMPTY, LO_NUM_INVALID, LO_NUM_UNSUPPORTED = 0, 1, 2, 3, 4
 LO_FORMAT_MAX_CELL = 310
+LO_CSV_OK, LO_CSV_SHORT_ROW, LO_CSV_FIELD_LIMIT, LO_CSV_BAD_UTF8, LO_CSV_NUL, LO_CSV_UNSUPPORTED, LO_CSV_EMPTY = range(7)
 LO_ABI_VERSION = 3
 
 _ERR_NAMES = {
@@ -60,6 +61,11 @@ class HistSpec(C.Structure):
 class HostTiming(C.Structure):
     _fields_ = [("total_ms", C.c_double), ("h2d_bytes", C.c_double), ("d2h_bytes", C.c_double),
                 ("launches", C.c_int64), ("kernel_ms", C.c_double)]
+
+
+class CsvInfo(C.Structure):
+    _fields_ = [("records", C.c_int64), ("ncols", C.c_int64), ("chars", C.c_int64), ("fail_record", C.c_int64),
+                ("fail_kind", C.c_int32), ("pad", C.c_int32), ("fail_pos", C.c_int64)]
 
 
 # every symbol include/loexec.h declares: name -> (restype, argtypes)
@@ -126,6 +132,9 @@ SIGNATURES = {
     "lo_parse_number_host": (C.c_int, [_P, _P, _P, C.c_int64, _P, _P, C.POINTER(HostTiming)]),
     "lo_format_number_host": (C.c_int, [_P, _P, _P, C.c_int64, _P, _P, C.c_int64, C.POINTER(HostTiming)]),
     "lo_minmax_cast_host": (C.c_int, [_P, C.POINTER(_P), C.c_int64, C.c_int32, _P, _P, _P, C.POINTER(HostTiming)]),
+    "lo_csv_read_host": (C.c_int, [_P, _P, C.c_int64, C.POINTER(_P), C.POINTER(CsvInfo), C.POINTER(HostTiming)]),
+    "lo_csv_columns_host": (C.c_int, [_P, _P, _P, C.c_int64, C.POINTER(HostTiming)]),
+    "lo_csv_free": (C.c_int, [_P]),
 }
 
 _lib = None

@@ -46,7 +46,8 @@ def _stale(target: Path, sources: list[Path]) -> bool:
 
 def build_native(force: bool = False, verbose: bool = False) -> Path:
     sources = [CSRC / "loexec.cu", CSRC / "group.inc", CSRC / "kernels.cuh", CSRC / "parse_number.cuh", CSRC / "pow5_table.inc",
-               CSRC / "format_number.cuh", CSRC / "ryu_pow5.inc", CSRC / "ryu_pow5_inv.inc", ROOT / "include" / "loexec.h"]
+               CSRC / "format_number.cuh", CSRC / "ryu_pow5.inc", CSRC / "ryu_pow5_inv.inc", CSRC / "csv.inc", CSRC / "csv_reader.cuh",
+               ROOT / "include" / "loexec.h"]
     if not force and not _stale(LIB_PATH, sources):
         return LIB_PATH
     LIB_DIR.mkdir(parents=True, exist_ok=True)

@@ -30,7 +30,7 @@ from collections import OrderedDict
 
 import numpy as np
 
-from .utils import DOCUMENT_ID_NAME, METADATA_DOCUMENT_ID, Database, _matches, _now
+from .utils import DOCUMENT_ID_NAME, METADATA_DOCUMENT_ID, Database, _matches, _now, record_exception
 
 
 class NumberColumn:
@@ -146,6 +146,67 @@ def column_from_values(values):
     return ObjectColumn(values)
 
 
+def _tokenize_pyarrow(source):
+    """(header names, Arrow columns, rows, None) by pyarrow.csv; every column read as text, a malformed body raises."""
+    import pyarrow as pa
+    import pyarrow.csv as pacsv
+    # the header first: every column is read as text
+    read = pacsv.ReadOptions(autogenerate_column_names=False)
+    head = pacsv.open_csv(source, read_options=read, parse_options=pacsv.ParseOptions(newlines_in_values=True)) \
+        if isinstance(source, str) else None
+    if head is not None:
+        raw_names = list(head.schema.names)
+        head.close()
+    else:
+        pos = source.tell()
+        first = source.readline()
+        source.seek(pos)
+        import csv as _csv
+        raw_names = next(_csv.reader([first.decode("utf-8") if isinstance(first, bytes) else first]))
+    conv = pacsv.ConvertOptions(column_types={n: pa.large_string() for n in raw_names}, strings_can_be_null=False,
+                                quoted_strings_can_be_null=False)
+    table = pacsv.read_csv(source, read_options=read, convert_options=conv,
+                           parse_options=pacsv.ParseOptions(newlines_in_values=True))
+    return list(table.schema.names), list(table.columns), table.num_rows, None
+
+
+def _csv_failure(kind, record, pos):
+    """The exception the reference's reader raises for a device reader failure (LO_CSV_*), for the metadata."""
+    import csv as _csv
+
+    from . import _native as N
+    at = f" (record {record}, byte {pos})"
+    if kind == N.LO_CSV_SHORT_ROW:
+        return IndexError(f"list index out of range: record {record} has fewer fields than the header")
+    if kind == N.LO_CSV_FIELD_LIMIT:
+        return _csv.Error(f"field larger than field limit (131072){at}")
+    if kind == N.LO_CSV_NUL:
+        return _csv.Error(f"line contains NUL{at}")
+    if kind == N.LO_CSV_BAD_UTF8:
+        return UnicodeDecodeError("utf-8", b"", 0, 0, f"invalid UTF-8 in the line starting at byte {pos} (record {record})")
+    if kind == N.LO_CSV_EMPTY:
+        return StopIteration("the body has no header")
+    return ValueError(f"a line ends inside a UTF-8 sequence{at}: not supported")
+
+
+def _tokenize_device(read_csv, source):
+    """(header cells or None, Arrow columns, rows, failure exception or None) by the engine's GPU reader; the columns
+    are zero-copy views of one shared chars buffer."""
+    import pyarrow as pa
+    if isinstance(source, str):
+        body = np.fromfile(source, dtype=np.uint8)
+    else:
+        data = source.read()
+        body = np.frombuffer(data.encode("utf-8") if isinstance(data, str) else data, dtype=np.uint8)
+    header, n, chars, offsets, failure = read_csv(body)
+    exc = None if failure is None else _csv_failure(*failure)
+    if header is None:
+        return None, [], 0, exc
+    data = pa.py_buffer(chars)
+    columns = [pa.LargeStringArray.from_buffers(n, pa.py_buffer(offsets[c, 1:]), data) for c in range(len(header))]
+    return header, columns, n, exc
+
+
 class _Table:
     def __init__(self, ids, columns):
         self.ids = np.ascontiguousarray(ids, dtype=np.int64)
@@ -245,38 +306,32 @@ class ColumnarDatabase(Database):
                 self._collections.setdefault(filename, []).extend(t.rows())
 
     # ---- the producer of the format: database_api_image/database.py:110-151 -------------------------------
-    def ingest_csv(self, filename, source, url=None):
+    def ingest_csv(self, filename, source, url=None, engine=None):
         """``POST /files``'s work: ``source`` is a path or a file object of CSV text.  Header sanitised with
         ``re.sub(r"\\W+", "", name)`` (``database.py:118-119``); every cell a string (``:124-137``); ``_id`` from 1;
         metadata document as ``database_api_image/utils.py:50-63`` writes it, ``finished`` flipped to True and
-        ``fields`` = the sanitised header at the end (``database.py:139-151``)."""
-        import pyarrow as pa
-        import pyarrow.csv as pacsv
+        ``fields`` = the sanitised header at the end (``database.py:139-151``).
+
+        With an engine that has ``read_csv_host`` the body is tokenised on the GPU with the reference's own
+        ``csv.reader`` rules: a body the reference fails on keeps the data rows before the failing record, ``finished``
+        stays False and the metadata's ``exception`` says why (a failing header stores no rows).  Without one, pyarrow
+        tokenises it and a malformed body raises."""
         self.insert_one_in_file(filename, {"datasetName": filename, "url": url, "timeCreated": _now(), "_id": 0,
                                            "finished": False, "type": "dataset/csv"})
-        # the header first: every column is read as text
-        read = pacsv.ReadOptions(autogenerate_column_names=False)
-        head = pacsv.open_csv(source, read_options=read, parse_options=pacsv.ParseOptions(newlines_in_values=True)) \
-            if isinstance(source, str) else None
-        if head is not None:
-            raw_names = list(head.schema.names)
-            head.close()
+        read_csv = getattr(engine, "read_csv_host", None)
+        if read_csv is None:
+            raw_names, columns, n, failure = _tokenize_pyarrow(source)
         else:
-            pos = source.tell()
-            first = source.readline()
-            source.seek(pos)
-            import csv as _csv
-            raw_names = next(_csv.reader([first.decode("utf-8") if isinstance(first, bytes) else first]))
-        conv = pacsv.ConvertOptions(column_types={n: pa.large_string() for n in raw_names}, strings_can_be_null=False,
-                                    quoted_strings_can_be_null=False)
-        table = pacsv.read_csv(source, read_options=read, convert_options=conv,
-                               parse_options=pacsv.ParseOptions(newlines_in_values=True))
-        names = [re.sub(r"\W+", "", n) for n in table.schema.names]
-        n = table.num_rows
+            raw_names, columns, n, failure = _tokenize_device(read_csv, source)
         cols = OrderedDict()
-        for name, chunked in zip(names, table.columns):
-            cols[name] = TextColumn(chunked)           # a repeated sanitised name keeps the LAST column, as dict(zip()) does
-        self.create_table(filename, np.arange(1, n + 1, dtype=np.int64), cols)
+        if raw_names is not None:
+            names = [re.sub(r"\W+", "", name) for name in raw_names]
+            for name, arr in zip(names, columns):
+                cols[name] = TextColumn(arr)           # a repeated sanitised name keeps the LAST column, as dict(zip()) does
+            self.create_table(filename, np.arange(1, n + 1, dtype=np.int64), cols)
+        if failure is not None:
+            record_exception(self, filename, failure)
+            return n
         self.update_one(filename, {"finished": True, "fields": list(cols)}, {"_id": 0})
         return n
 

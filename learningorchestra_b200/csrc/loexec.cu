@@ -1646,3 +1646,4 @@ int lo_minmax_cast_host(lo_ctx *ctx, const double *const *in_cols, int64_t nrows
 }  // extern "C"
 
 #include "group.inc"
+#include "csv.inc"

@@ -409,6 +409,38 @@ class Engine:
                           launches=t.launches)
         return chars[:offsets[n]], offsets
 
+    def read_csv_host(self, body, timing: dict | None = None):
+        """Tokenise a CSV upload on the GPU with the reference's ``csv.reader`` rules (``lo_csv_read_host``).
+
+        body: bytes-like or a contiguous uint8 array (pinned memory makes the copy faster).  Returns ``(header_cells,
+        nrows, chars, offsets, failure)``: the header's cells (None when the header itself fails or there is no
+        record), the number of data rows kept, one uint8 chars buffer and int64 ``offsets[ncols][nrows + 2]`` — column
+        c's cell r (r = 0 the header) is ``chars[offsets[c, r]:offsets[c, r + 1]]``, the offsets absolute in chars, so
+        ``offsets[c, 1:]`` are the Arrow offsets of column c's data rows.  failure: None or ``(kind, record, pos)`` with
+        kind an LO_CSV_* code, record the failing record (0 the header) and pos the byte offset it was raised at.
+        ``timing``: a dict to receive the calls' lo_host_timing fields, summed."""
+        buf = body if isinstance(body, np.ndarray) else np.frombuffer(body, dtype=np.uint8)
+        if buf.dtype != np.uint8 or buf.ndim != 1 or not buf.flags.c_contiguous:
+            raise ValueError("body must be bytes or a contiguous 1-D uint8 array")
+        h, info, t1, t2 = C.c_void_p(), N.CsvInfo(), N.HostTiming(), N.HostTiming()
+        N.check(self._lib.lo_csv_read_host(self._ctx, buf.ctypes.data_as(C.c_void_p), buf.size, C.byref(h), C.byref(info),
+                                           C.byref(t1)))
+        try:
+            offsets = np.empty((info.ncols, info.records + 1), dtype=np.int64)
+            chars = np.empty(max(info.chars, 1), dtype=np.uint8)
+            N.check(self._lib.lo_csv_columns_host(h, offsets.ctypes.data_as(C.c_void_p), chars.ctypes.data_as(C.c_void_p),
+                                                  chars.size, C.byref(t2)))
+        finally:
+            N.check(self._lib.lo_csv_free(h))
+        if timing is not None:
+            timing.update(total_ms=t1.total_ms + t2.total_ms, kernel_ms=t1.kernel_ms, h2d_bytes=t1.h2d_bytes,
+                          d2h_bytes=t1.d2h_bytes + t2.d2h_bytes, launches=t1.launches)
+        chars = chars[:info.chars]
+        header = [bytes(chars[offsets[c, 0]:offsets[c, 1]]).decode("utf-8") for c in range(info.ncols)] \
+            if info.records else None
+        failure = None if info.fail_kind == N.LO_CSV_OK else (int(info.fail_kind), int(info.fail_record), int(info.fail_pos))
+        return header, max(int(info.records) - 1, 0), chars, offsets, failure
+
     def value_counts_str_packed(self, chars: np.ndarray, offsets: np.ndarray):
         """(rep_rows int64[g], counts uint64[g]) of an already packed text column (offsets[0] == 0)."""
         n = offsets.shape[0] - 1

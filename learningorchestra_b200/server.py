@@ -145,7 +145,7 @@ class App:
         import os
         if not hasattr(self.database, "ingest_csv") or not os.path.isfile(path):
             return _json({MESSAGE_RESULT: "invalid url"}, HTTP_STATUS_CODE_NOT_ACCEPTABLE)
-        self.database.ingest_csv(filename, path, url=url)
+        self.database.ingest_csv(filename, path, url=url, engine=self.engine)
         return _json({MESSAGE_RESULT: f"{DATATYPE_URI_GET}{filename}?query={{}}&limit=10&skip=0"}, HTTP_STATUS_CODE_SUCCESS_CREATED)
 
     def _maybe_wait(self, job):

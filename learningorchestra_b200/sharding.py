@@ -402,6 +402,9 @@ class ShardedEngine:
     def format_number_host(self, values, status, timing=None):
         return self.engines[0].format_number_host(values, status, timing)
 
+    def read_csv_host(self, body, timing=None):
+        return self.engines[0].read_csv_host(body, timing)
+
     def value_counts_str_packed(self, chars, offsets):
         return self.engines[0].value_counts_str_packed(chars, offsets)
 
