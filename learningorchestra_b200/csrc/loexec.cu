@@ -22,6 +22,7 @@
 #include <mutex>
 #include <new>
 #include <string>
+#include <type_traits>
 #include <utility>
 #include <vector>
 
@@ -139,6 +140,13 @@ int check_ctx(const lo_ctx *ctx) {
     cudaError_t e = cudaSetDevice(ctx->device);
     if (e != cudaSuccess) return fail(LO_ERR_CUDA, "cudaSetDevice(%d): %s", ctx->device, cudaGetErrorString(e));
     return LO_OK;
+}
+
+// after n kernel launches on this thread: the launch error, or count them on the context
+cudaError_t launched(lo_ctx *ctx, int n) {
+    const cudaError_t e = cudaGetLastError();
+    if (e == cudaSuccess) ctx->launches.fetch_add(n, std::memory_order_relaxed);
+    return e;
 }
 
 bool aligned32(const lo_table *t) {
@@ -418,8 +426,7 @@ int launch_f64(lo_ctx *ctx, const lo_table *in, const lo_table *out, int32_t out
         if (tblocks > 0x7fffffffull) return fail(LO_ERR_INVALID, "table too large for one launch (%llu tiles)", tblocks);
         lo::k_project_cast_hist_tma<OUT, HIST, HIST><<<(unsigned)tblocks, lo::kThreads + 32, lo::kTmaSmemBytes, s>>>(
             in->base, in->pitch, out_base, out_pitch, in->nrows, full_tiles, counts, P);
-        LO_CUDA(cudaGetLastError());
-        ctx->launches.fetch_add(1, std::memory_order_relaxed);
+        LO_CUDA(launched(ctx, 1));
         const int64_t done = (int64_t)full_tiles * lo::kTileRows;
         if (done == in->nrows) return LO_OK;
         // the remaining rows of every column: one ragged tile each, through the regular kernel on a row-offset view
@@ -429,8 +436,7 @@ int launch_f64(lo_ctx *ctx, const lo_table *in, const lo_table *out, int32_t out
                        ib, in->pitch, ob, out_pitch, in->nrows - done, 1u, counts, edges, P, kNoGroup);
         else       lo::k_project_cast_hist<OUT, HIST, true, false><<<(unsigned)P.k, lo::kThreads, smem, s>>>(
                        ib, in->pitch, ob, out_pitch, in->nrows - done, 1u, counts, edges, P, kNoGroup);
-        LO_CUDA(cudaGetLastError());
-        ctx->launches.fetch_add(1, std::memory_order_relaxed);
+        LO_CUDA(launched(ctx, 1));
         if (et) LO_TRY(edge_used(et, s));
         return LO_OK;
     }
@@ -448,8 +454,7 @@ int launch_f64(lo_ctx *ctx, const lo_table *in, const lo_table *out, int32_t out
     if (aligned) { if (edges) LO_LAUNCH(true, true); else LO_LAUNCH(true, false); }
     else         { if (edges) LO_LAUNCH(false, true); else LO_LAUNCH(false, false); }
 #undef LO_LAUNCH
-    LO_CUDA(cudaGetLastError());
-    ctx->launches.fetch_add(1, std::memory_order_relaxed);
+    LO_CUDA(launched(ctx, 1));
     if (et) LO_TRY(edge_used(et, s));
     return LO_OK;
 }
@@ -484,8 +489,7 @@ int launch_f64_bins(lo_ctx *ctx, const lo_table *in, const lo_table *out, int32_
                                     ib, ip, out_base, out_pitch, nr, chunks_per_col, (long long)chunk_rows, slots_log2, (int)aligned, counts, P, G));
     else      LO_CUDA(launch_kernel(lo::k_project_cast_hist_bins<OUT, false>, (unsigned)blocks, (unsigned)lo::kWBThreads, smem, s, G.overlap != 0,
                                     ib, ip, out_base, out_pitch, nr, chunks_per_col, (long long)chunk_rows, slots_log2, (int)aligned, counts, P, G));
-    LO_CUDA(cudaGetLastError());
-    ctx->launches.fetch_add(1, std::memory_order_relaxed);
+    LO_CUDA(launched(ctx, 1));
     return LO_OK;
 }
 
@@ -576,8 +580,7 @@ int hist_u8_impl(lo_ctx *ctx, const lo_table *in, const int32_t *col_idx, int32_
         LO_CUDA(launch_kernel(aligned ? lo::k_hist_u8_cols_lanes<true> : lo::k_hist_u8_cols_lanes<false>, (unsigned)blocks,
                               (unsigned)lo::kU8LThreads, (size_t)lo::kU8LSmemBytes, s, G.overlap != 0,
                               ib, ip, nr, chunks_per_col, (long long)chunk_rows, cnt, P, G));
-        LO_CUDA(cudaGetLastError());
-        ctx->launches.fetch_add(1, std::memory_order_relaxed);
+        LO_CUDA(launched(ctx, 1));
     }
     return LO_OK;
 }
@@ -682,6 +685,116 @@ int64_t chunk_rows_for(int64_t nrows, int32_t k, size_t elem_bytes, int64_t tile
     int64_t rows = std::max<int64_t>(tile_rows, (target / tile_rows) * tile_rows);
     return std::min(rows, ((nrows + tile_rows - 1) / tile_rows) * tile_rows);
 }
+
+// min / max / count of the finite cast values of k resident columns: one launch per column into out_dev[3*j ..]
+int launch_minmax(lo_ctx *ctx, const lo_table *in, const int32_t *col_idx, int32_t k, unsigned long long *out_dev, cudaStream_t s) {
+    if (in->nrows == 0) return LO_OK;
+    for (int j = 0; j < k; ++j) {
+        dim3 grid((unsigned)std::min<int64_t>((in->nrows + 2047) / 2048, ctx->sm_count * 4), 1);
+        lo::k_minmax_cast<<<grid, 256, 0, s>>>(in->base + (int64_t)col_idx[j] * in->pitch, in->pitch, in->nrows, out_dev + 3 * j);
+        LO_CUDA(launched(ctx, 1));
+    }
+    return LO_OK;
+}
+
+// One call of an entry point that runs its kernels once, not in chunks: its stream, its first error, its scratch, its
+// kernel time (summed over timed sections) and its launch count.  Once a step has failed every later step does
+// nothing.  finish() frees the scratch, drains the stream and reports the first error ("<call>: <CUDA error string>",
+// LO_ERR_NOMEM for an allocation, LO_ERR_CUDA otherwise) or fills lo_host_timing.
+// Scratch is allocated and freed in stream order (cudaMallocAsync / cudaFreeAsync on the call's stream), so a call
+// neither synchronises the device (cudaFree does) nor touches the legacy default stream (cudaMemcpy does): other
+// jobs' streams keep running.
+struct HostCall {
+    lo_ctx *ctx;
+    const char *name;
+    cudaStream_t s;
+    int rc = LO_OK;
+    std::string msg;
+    std::vector<void *> scratch, kept;
+    std::vector<cudaEvent_t> marks;          // start, stop, start, stop, ... of the timed sections
+    double h2d = 0, d2h = 0;
+    const std::chrono::steady_clock::time_point t0 = std::chrono::steady_clock::now();
+    const int64_t launches0;
+
+    HostCall(lo_ctx *c, const char *call) : ctx(c), name(call), s(c->stream), launches0(c->launches.load()) {}
+    ~HostCall() {
+        release(scratch);
+        for (cudaEvent_t ev : marks) cudaEventDestroy(ev);
+    }
+    bool ok() const { return rc == LO_OK; }
+    void latch(cudaError_t e) {
+        if (!ok() || e == cudaSuccess) return;
+        rc = e == cudaErrorMemoryAllocation ? LO_ERR_NOMEM : LO_ERR_CUDA;
+        msg = std::string(name) + ": " + cudaGetErrorString(e);
+    }
+    template <typename F> void run(F f) { if (ok()) latch(f()); }               // f returns a cudaError_t
+    template <typename F> void check(F f) { if (ok() && (rc = f()) != LO_OK) msg = g_err; }   // f returns an LO_* code
+    // f enqueues n kernels: <<<>>> launches, or CUB calls that return their cudaError_t
+    template <typename F> void launch(int n, F f) {
+        if (!ok()) return;
+        if constexpr (std::is_void_v<decltype(f())>) f(); else latch(f());
+        if (ok()) latch(launched(ctx, n));
+    }
+    template <typename T> void alloc(T **p, size_t bytes) {
+        run([&] { return cudaMallocAsync((void **)p, bytes ? bytes : 1, s); });
+        if (ok()) scratch.push_back(*p);
+    }
+    // p outlives a successful call (the caller owns it then); a failed call frees it with the scratch
+    void keep(const void *p) {
+        auto it = std::find(scratch.begin(), scratch.end(), p);
+        if (it != scratch.end()) { kept.push_back(*it); scratch.erase(it); }
+    }
+    void drop(const void *p) {               // free one scratch buffer before the call ends
+        auto it = std::find(scratch.begin(), scratch.end(), p);
+        if (it != scratch.end()) { cudaFreeAsync(*it, s); scratch.erase(it); }
+    }
+    void to_dev(void *d, const void *h, size_t bytes) {
+        if (!ok() || !bytes) return;
+        latch(cudaMemcpyAsync(d, h, bytes, cudaMemcpyHostToDevice, s));
+        h2d += (double)bytes;
+    }
+    void to_host(void *h, const void *d, size_t bytes) {
+        if (!ok() || !bytes) return;
+        latch(cudaMemcpyAsync(h, d, bytes, cudaMemcpyDeviceToHost, s));
+        d2h += (double)bytes;
+    }
+    void memset(void *d, int v, size_t bytes) { run([&] { return cudaMemsetAsync(d, v, bytes, s); }); }
+    void sync() { run([&] { return cudaStreamSynchronize(s); }); }
+    void mark() {                            // start or end of a timed section
+        run([&] {
+            cudaEvent_t ev = nullptr;
+            const cudaError_t e = cudaEventCreate(&ev);
+            if (e != cudaSuccess) return e;
+            marks.push_back(ev);
+            return cudaEventRecord(ev, s);
+        });
+    }
+    void release(std::vector<void *> &v) {
+        for (void *p : v) cudaFreeAsync(p, s);
+        v.clear();
+    }
+    int finish(lo_host_timing *timing) {
+        release(scratch);
+        latch(cudaStreamSynchronize(s));
+        if (!ok()) {
+            release(kept);
+            return fail(rc, "%s", msg.c_str());
+        }
+        if (timing) {
+            double kernel_ms = 0;
+            for (size_t i = 0; i + 1 < marks.size(); i += 2) {
+                float t = 0.f;
+                if (cudaEventElapsedTime(&t, marks[i], marks[i + 1]) == cudaSuccess) kernel_ms += t;
+            }
+            timing->total_ms  = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+            timing->h2d_bytes = h2d;
+            timing->d2h_bytes = d2h;
+            timing->launches  = ctx->launches.load() - launches0;
+            timing->kernel_ms = kernel_ms;
+        }
+        return LO_OK;
+    }
+};
 
 }  // namespace
 
@@ -948,8 +1061,7 @@ int lo_table_fill_synthetic_dev(lo_ctx *ctx, lo_table *t, int kind, uint64_t see
     } else {
         return fail(LO_ERR_INVALID, "unknown generator kind %d", kind);
     }
-    LO_CUDA(cudaGetLastError());
-    ctx->launches.fetch_add(1, std::memory_order_relaxed);
+    LO_CUDA(launched(ctx, 1));
     return LO_OK;
 }
 
@@ -957,24 +1069,20 @@ int lo_table_checksum(lo_ctx *ctx, const lo_table *t, int32_t col, int64_t row_o
     LO_TRY(check_ctx(ctx));
     LO_TRY(check_range(t, col, 0, 0));
     if (!out) return fail(LO_ERR_INVALID, "out is NULL");
-    unsigned long long *d = nullptr;
-    LO_CUDA(cudaMalloc((void **)&d, 8));
-    cudaStream_t s = ctx->stream;
-    cudaError_t e = cudaMemsetAsync(d, 0, 8, s);
-    if (e == cudaSuccess && t->nrows > 0) {
-        const char *p = t->base + (int64_t)col * t->pitch;
-        const int grid = ctx->sm_count * 8;
-        if (t->dtype == LO_F64)      lo::k_checksum<double><<<grid, 256, 0, s>>>((const double *)p, t->nrows, row_offset, d);
-        else if (t->dtype == LO_F32) lo::k_checksum<float><<<grid, 256, 0, s>>>((const float *)p, t->nrows, row_offset, d);
-        else                         lo::k_checksum<uint8_t><<<grid, 256, 0, s>>>((const uint8_t *)p, t->nrows, row_offset, d);
-        e = cudaGetLastError();
-        ctx->launches.fetch_add(1, std::memory_order_relaxed);
-    }
-    unsigned long long h = 0;
-    if (e == cudaSuccess) e = cudaMemcpyAsync(&h, d, 8, cudaMemcpyDeviceToHost, s);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-    cudaFree(d);
-    if (e != cudaSuccess) return fail(LO_ERR_CUDA, "checksum: %s", cudaGetErrorString(e));
+    HostCall c(ctx, "checksum");
+    unsigned long long *d = nullptr, h = 0;
+    c.alloc(&d, 8);
+    c.memset(d, 0, 8);
+    if (t->nrows > 0)
+        c.launch(1, [&] {
+            const char *p = t->base + (int64_t)col * t->pitch;
+            const int grid = ctx->sm_count * 8;
+            if (t->dtype == LO_F64)      lo::k_checksum<double><<<grid, 256, 0, c.s>>>((const double *)p, t->nrows, row_offset, d);
+            else if (t->dtype == LO_F32) lo::k_checksum<float><<<grid, 256, 0, c.s>>>((const float *)p, t->nrows, row_offset, d);
+            else                         lo::k_checksum<uint8_t><<<grid, 256, 0, c.s>>>((const uint8_t *)p, t->nrows, row_offset, d);
+        });
+    c.to_host(&h, d, 8);
+    LO_TRY(c.finish(nullptr));
     *out = h;
     return LO_OK;
 }
@@ -987,19 +1095,13 @@ int lo_selftest_fastdiv(lo_ctx *ctx, float lo_v, float hi_v, int32_t nbins, int 
     float w = 0.f;
     LO_TRY(check_spec(&spec, 1, &w));
     if (fast_path_used) *fast_path_used = fastdiv_ok(w) ? 1 : 0;
-    unsigned long long *d = nullptr;
-    LO_CUDA(cudaMalloc((void **)&d, 8));
-    cudaError_t e = cudaMemsetAsync(d, 0, 8, ctx->stream);
-    if (e == cudaSuccess) {
-        lo::k_selftest_fastdiv<<<ctx->sm_count * 16, 256, 0, ctx->stream>>>(lo_v, hi_v, w, nbins, d);
-        e = cudaGetLastError();
-        ctx->launches.fetch_add(1, std::memory_order_relaxed);
-    }
-    unsigned long long h = 0;
-    if (e == cudaSuccess) e = cudaMemcpyAsync(&h, d, 8, cudaMemcpyDeviceToHost, ctx->stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
-    cudaFree(d);
-    if (e != cudaSuccess) return fail(LO_ERR_CUDA, "selftest: %s", cudaGetErrorString(e));
+    HostCall c(ctx, "selftest");
+    unsigned long long *d = nullptr, h = 0;
+    c.alloc(&d, 8);
+    c.memset(d, 0, 8);
+    c.launch(1, [&] { lo::k_selftest_fastdiv<<<ctx->sm_count * 16, 256, 0, c.s>>>(lo_v, hi_v, w, nbins, d); });
+    c.to_host(&h, d, 8);
+    LO_TRY(c.finish(nullptr));
     *mismatches = h;
     return LO_OK;
 }
@@ -1034,22 +1136,15 @@ int lo_selftest_edges(lo_ctx *ctx, float lo_v, float hi_v, int32_t nbins, int *e
     if (edges_used) *edges_used = edges_ok(w) ? 1 : 0;
     std::vector<float> h((size_t)nbins + 1);
     hist_edges(lo_v, hi_v, w, nbins, h.data());
-    unsigned long long *d = nullptr;
-    float *E = nullptr;
-    LO_CUDA(cudaMalloc((void **)&d, 8 + h.size() * 4));
-    E = reinterpret_cast<float *>(d + 1);
-    cudaError_t e = cudaMemcpyAsync(E, h.data(), h.size() * 4, cudaMemcpyHostToDevice, ctx->stream);
-    if (e == cudaSuccess) e = cudaMemsetAsync(d, 0, 8, ctx->stream);
-    if (e == cudaSuccess) {
-        lo::k_selftest_edges<<<ctx->sm_count * 16, 256, 0, ctx->stream>>>(lo_v, hi_v, w, nbins, E, d);
-        e = cudaGetLastError();
-        ctx->launches.fetch_add(1, std::memory_order_relaxed);
-    }
-    unsigned long long bad = 0;
-    if (e == cudaSuccess) e = cudaMemcpyAsync(&bad, d, 8, cudaMemcpyDeviceToHost, ctx->stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
-    cudaFree(d);
-    if (e != cudaSuccess) return fail(LO_ERR_CUDA, "selftest: %s", cudaGetErrorString(e));
+    HostCall c(ctx, "selftest");
+    unsigned long long *d = nullptr, bad = 0;
+    c.alloc(&d, 8 + h.size() * 4);
+    float *E = reinterpret_cast<float *>(d + 1);
+    c.to_dev(E, h.data(), h.size() * 4);
+    c.memset(d, 0, 8);
+    c.launch(1, [&] { lo::k_selftest_edges<<<ctx->sm_count * 16, 256, 0, c.s>>>(lo_v, hi_v, w, nbins, E, d); });
+    c.to_host(&bad, d, 8);
+    LO_TRY(c.finish(nullptr));
     *mismatches = bad;
     return LO_OK;
 }
@@ -1063,15 +1158,7 @@ int lo_minmax_cast_dev(lo_ctx *ctx, const lo_table *in, const int32_t *col_idx, 
     if (!out_dev) return fail(LO_ERR_INVALID, "out_dev is NULL");
     cudaStream_t s = pick(ctx, stream);
     LO_CUDA(cudaMemsetAsync(out_dev, 0, (size_t)k * 24, s));
-    if (in->nrows == 0) return LO_OK;
-    for (int j = 0; j < k; ++j) {
-        dim3 grid((unsigned)std::min<int64_t>((in->nrows + 2047) / 2048, ctx->sm_count * 4), 1);
-        lo::k_minmax_cast<<<grid, 256, 0, s>>>(in->base + (int64_t)col_idx[j] * in->pitch, in->pitch, in->nrows,
-                                               (unsigned long long *)out_dev + 3 * j);
-        LO_CUDA(cudaGetLastError());
-        ctx->launches.fetch_add(1, std::memory_order_relaxed);
-    }
-    return LO_OK;
+    return launch_minmax(ctx, in, col_idx, k, (unsigned long long *)out_dev, s);
 }
 
 // raw[3*k] (as downloaded from lo_minmax_cast_dev) -> mins / maxs / nfinite
@@ -1079,6 +1166,7 @@ int lo_minmax_decode(const uint64_t *raw, int32_t k, float *mins, float *maxs, u
     if (!raw || !mins || !maxs || !nfinite || k < 0) return fail(LO_ERR_INVALID, "bad arguments");
     for (int j = 0; j < k; ++j) {
         nfinite[j] = raw[(size_t)j * 3 + 2];
+        // the device kept min as ~ordered (so that zero-initialised memory is the identity) and max as ordered
         uint32_t omin = ~(uint32_t)raw[(size_t)j * 3 + 0], omax = (uint32_t)raw[(size_t)j * 3 + 1];
         auto unorder = [](uint32_t o) { uint32_t b = (o & 0x80000000u) ? (o ^ 0x80000000u) : ~o; float f; memcpy(&f, &b, 4); return f; };
         mins[j] = nfinite[j] ? unorder(omin) : 0.f;
@@ -1188,31 +1276,6 @@ int copy_cols(char *dev_base, int64_t dev_pitch, const void *const *host_cols, i
     return LO_OK;
 }
 
-// kernel time of a *_host call that runs its kernels once (parser, group-by): two events on the call's stream
-struct DevTimer {
-    cudaEvent_t a = nullptr, b = nullptr;
-    cudaError_t start(cudaStream_t s) {
-        cudaError_t e = cudaEventCreate(&a);
-        if (e == cudaSuccess) e = cudaEventCreate(&b);
-        if (e == cudaSuccess) e = cudaEventRecord(a, s);
-        return e;
-    }
-    cudaError_t stop(cudaStream_t s) { return cudaEventRecord(b, s); }
-    double ms() const {                       // after the stream was synchronised
-        float t = 0.f;
-        return (a && b && cudaEventElapsedTime(&t, a, b) == cudaSuccess) ? (double)t : 0.0;
-    }
-    ~DevTimer() { if (a) cudaEventDestroy(a); if (b) cudaEventDestroy(b); }
-};
-
-// scratch of one call: allocated and freed in stream order (cudaMallocAsync / cudaFreeAsync on the call's stream), so a
-// call neither synchronises the device (cudaFree does) nor touches the legacy default stream (cudaMemcpy does) — other
-// jobs' streams keep running
-template <typename T>
-cudaError_t scratch_alloc(T **p, size_t bytes, cudaStream_t s) { return cudaMallocAsync((void **)p, bytes ? bytes : 1, s); }
-template <typename T>
-void scratch_free(T *p, cudaStream_t s) { if (p) cudaFreeAsync((void *)p, s); }
-
 template <typename Launch>
 int host_pipeline(lo_ctx *ctx, const void *const *in_cols, int in_dtype, int64_t nrows, int32_t k,
                   void *const *out_cols, int out_dtype, int64_t tile_rows, size_t ncounts, uint64_t *counts_host,
@@ -1290,6 +1353,55 @@ int check_host_cols(const void *const *cols, int64_t nrows, int32_t k, const cha
     return LO_OK;
 }
 
+// the arguments of lo_project_cast_hist_host and lo_group_project_cast_hist_host (at most max_k columns), and the
+// column list 0 .. k-1 their pipelines project from the staged chunk
+int check_project_host(const double *const *in_cols, int64_t nrows, int32_t k, float *const *out_cols,
+                       const lo_hist_spec *spec, const uint64_t *counts, int32_t max_k, std::vector<int32_t> &ident) {
+    LO_TRY(check_host_cols((const void *const *)in_cols, nrows, k, "in_cols"));
+    if (out_cols) LO_TRY(check_host_cols((const void *const *)out_cols, nrows, k, "out_cols"));
+    if (!out_cols && !spec) return fail(LO_ERR_INVALID, "nothing to do: no out_cols and no spec");
+    if (spec && !counts) return fail(LO_ERR_INVALID, "counts is NULL");
+    if (k > max_k) return fail(LO_ERR_INVALID, "k must be <= %d", max_k);
+    std::vector<float> w(k);
+    if (spec) LO_TRY(check_spec(spec, k, w.data()));
+    ident.resize(k);
+    for (int j = 0; j < k; ++j) ident[j] = j;
+    return LO_OK;
+}
+
+// The rest of lo_value_counts_*_host once the input is on the device.  count_and_compact(keys, counts, slots, out,
+// out_n) launches the two kernels of the hash group-by: count into a table of `slots` slots (keys all ones, counts
+// zero), then compact the groups into out[0 .. out_n) (keys) and out[out_n .. 2 out_n) (counts), at most `capacity`
+// of them, and their number into out[2 out_n].  The first min(groups, capacity) of them are copied out.
+template <typename CountAndCompact>
+int value_counts_tail(HostCall &c, int64_t n, void *keys_out, uint64_t *counts_out, int64_t capacity, int64_t *ndistinct,
+                      lo_host_timing *timing, CountAndCompact count_and_compact) {
+    unsigned long long slots = 1024;
+    while (slots < 2ull * (unsigned long long)n) slots <<= 1;
+    const size_t out_n = (size_t)std::max<int64_t>(capacity, 1);
+    unsigned long long *d_keys = nullptr, *d_counts = nullptr, *d_out = nullptr;
+    c.alloc(&d_keys, slots * 8);
+    c.alloc(&d_counts, slots * 8);
+    c.alloc(&d_out, (2 * out_n + 1) * 8);
+    c.mark();
+    c.memset(d_keys, 0xFF, slots * 8);
+    c.memset(d_counts, 0, slots * 8);
+    c.memset(d_out + 2 * out_n, 0, 8);
+    c.launch(2, [&] { count_and_compact(d_keys, d_counts, slots, d_out, out_n); });
+    c.mark();
+    unsigned long long nd = 0;
+    c.to_host(&nd, d_out + 2 * out_n, 8);
+    c.sync();
+    const size_t take = (size_t)std::min<unsigned long long>(nd, (unsigned long long)capacity);
+    c.to_host(keys_out, d_out, take * 8);
+    c.to_host(counts_out, d_out + out_n, take * 8);
+    LO_TRY(c.finish(timing));
+    *ndistinct = (int64_t)nd;
+    if ((int64_t)nd > capacity)
+        return fail(LO_ERR_INVALID, "%llu distinct keys do not fit the caller's capacity %lld", nd, (long long)capacity);
+    return LO_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -1298,14 +1410,8 @@ int lo_project_cast_hist_host(lo_ctx *ctx, const double *const *in_cols, int64_t
                               float *const *out_cols, const lo_hist_spec *spec, uint64_t *counts,
                               lo_host_timing *timing) {
     LO_TRY(check_ctx(ctx));
-    LO_TRY(check_host_cols((const void *const *)in_cols, nrows, k, "in_cols"));
-    if (out_cols) LO_TRY(check_host_cols((const void *const *)out_cols, nrows, k, "out_cols"));
-    if (!out_cols && !spec) return fail(LO_ERR_INVALID, "nothing to do: no out_cols and no spec");
-    if (spec && !counts) return fail(LO_ERR_INVALID, "counts is NULL");
-    std::vector<float> w(k);
-    if (spec) LO_TRY(check_spec(spec, k, w.data()));
-    std::vector<int32_t> ident(k);
-    for (int j = 0; j < k; ++j) ident[j] = j;
+    std::vector<int32_t> ident;
+    LO_TRY(check_project_host(in_cols, nrows, k, out_cols, spec, counts, INT32_MAX, ident));
     const size_t ncounts = spec ? (size_t)k * (size_t)spec->nbins : 0;
     return host_pipeline(ctx, (const void *const *)in_cols, LO_F64, nrows, k, (void *const *)out_cols, LO_F32,
                          lo::kTileRows, ncounts, counts, timing,
@@ -1341,8 +1447,7 @@ int lo_value_counts_u32_host(lo_ctx *ctx, const uint32_t *codes, int64_t nrows, 
                                const int grid = ctx->sm_count * 8;
                                lo::k_count_codes_u32<<<grid, 256, 0, cs>>>(
                                    (const uint32_t *)tin->base, tin->nrows, ncodes, cdev);
-                               LO_CUDA(cudaGetLastError());
-                               ctx->launches.fetch_add(1, std::memory_order_relaxed);
+                               LO_CUDA(launched(ctx, 1));
                                return LO_OK;
                            });
     LO_TRY(rc);
@@ -1362,53 +1467,17 @@ int lo_value_counts_f64_host(lo_ctx *ctx, const double *values, int64_t n, doubl
     *ndistinct = 0;
     if (n == 0) return LO_OK;
     if (!values || (capacity > 0 && (!keys_out || !counts_out))) return fail(LO_ERR_INVALID, "NULL argument");
-    const auto t0 = std::chrono::steady_clock::now();
-    const int64_t launches0 = ctx->launches.load();
-    unsigned long long slots = 1024;
-    while (slots < 2ull * (unsigned long long)n) slots <<= 1;
+    HostCall c(ctx, "value_counts_f64");
     double *d_val = nullptr;
-    unsigned long long *d_keys = nullptr, *d_counts = nullptr, *d_out = nullptr;
-    const size_t out_n = (size_t)std::max<int64_t>(capacity, 1);
-    cudaStream_t s = ctx->stream;
-    DevTimer kt;
-    cudaError_t e = scratch_alloc(&d_val, (size_t)n * 8, s);
-    if (e == cudaSuccess) e = scratch_alloc(&d_keys, slots * 8, s);
-    if (e == cudaSuccess) e = scratch_alloc(&d_counts, slots * 8, s);
-    if (e == cudaSuccess) e = scratch_alloc(&d_out, (2 * out_n + 1) * 8, s);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(d_val, values, (size_t)n * 8, cudaMemcpyHostToDevice, s);
-    if (e == cudaSuccess) e = kt.start(s);
-    if (e == cudaSuccess) e = cudaMemsetAsync(d_keys, 0xFF, slots * 8, s);
-    if (e == cudaSuccess) e = cudaMemsetAsync(d_counts, 0, slots * 8, s);
-    if (e == cudaSuccess) e = cudaMemsetAsync(d_out + 2 * out_n, 0, 8, s);
-    if (e == cudaSuccess) {
-        const int grid = (int)std::min<int64_t>((n + 255) / 256, (int64_t)ctx->sm_count * 8);
-        lo::k_hash_count_f64<<<grid, 256, 0, s>>>(d_val, n, d_keys, d_counts, slots - 1);
-        lo::k_hash_compact<<<ctx->sm_count * 8, 256, 0, s>>>(d_keys, d_counts, slots, d_out, d_out + out_n,
-                                                              (unsigned long long)capacity, d_out + 2 * out_n);
-        e = cudaGetLastError();
-        ctx->launches.fetch_add(2, std::memory_order_relaxed);
-    }
-    if (e == cudaSuccess) e = kt.stop(s);
-    unsigned long long nd = 0;
-    if (e == cudaSuccess) e = cudaMemcpyAsync(&nd, d_out + 2 * out_n, 8, cudaMemcpyDeviceToHost, s);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-    const size_t take = (size_t)std::min<unsigned long long>(nd, (unsigned long long)capacity);
-    if (e == cudaSuccess && take) e = cudaMemcpyAsync(keys_out, d_out, take * 8, cudaMemcpyDeviceToHost, s);
-    if (e == cudaSuccess && take) e = cudaMemcpyAsync(counts_out, d_out + out_n, take * 8, cudaMemcpyDeviceToHost, s);
-    scratch_free(d_val, s); scratch_free(d_keys, s); scratch_free(d_counts, s); scratch_free(d_out, s);
-    { const cudaError_t e2 = cudaStreamSynchronize(s); if (e == cudaSuccess) e = e2; }
-    if (e != cudaSuccess) return fail(e == cudaErrorMemoryAllocation ? LO_ERR_NOMEM : LO_ERR_CUDA, "value_counts_f64: %s", cudaGetErrorString(e));
-    *ndistinct = (int64_t)nd;
-    if (timing) {
-        timing->total_ms  = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
-        timing->h2d_bytes = (double)n * 8;
-        timing->d2h_bytes = (double)take * 16 + 8;
-        timing->launches  = ctx->launches.load() - launches0;
-        timing->kernel_ms = kt.ms();
-    }
-    if ((int64_t)nd > capacity)
-        return fail(LO_ERR_INVALID, "%llu distinct keys do not fit the caller's capacity %lld", nd, (long long)capacity);
-    return LO_OK;
+    c.alloc(&d_val, (size_t)n * 8);
+    c.to_dev(d_val, values, (size_t)n * 8);
+    return value_counts_tail(c, n, keys_out, counts_out, capacity, ndistinct, timing,
+        [&](unsigned long long *keys, unsigned long long *counts, unsigned long long slots, unsigned long long *out, size_t out_n) {
+            const int grid = (int)std::min<int64_t>((n + 255) / 256, (int64_t)ctx->sm_count * 8);
+            lo::k_hash_count_f64<<<grid, 256, 0, c.s>>>(d_val, n, keys, counts, slots - 1);
+            lo::k_hash_compact<<<ctx->sm_count * 8, 256, 0, c.s>>>(keys, counts, slots, out, out + out_n,
+                                                                    (unsigned long long)capacity, out + 2 * out_n);
+        });
 }
 
 // exact value counts of one TEXT column (cells = chars[offsets[i] .. offsets[i+1])): GPU hash group-by on the bytes.
@@ -1426,56 +1495,20 @@ int lo_value_counts_str_host(lo_ctx *ctx, const uint8_t *chars, const int64_t *o
     if (offsets[0] != 0 || nbytes < 0 || (nbytes > 0 && !chars)) return fail(LO_ERR_INVALID, "offsets must start at 0 and be non-decreasing");
     for (int64_t i = 0; i < n; ++i)
         if (offsets[i + 1] < offsets[i]) return fail(LO_ERR_INVALID, "offsets must be non-decreasing (row %lld)", (long long)i);
-    const auto t0 = std::chrono::steady_clock::now();
-    const int64_t launches0 = ctx->launches.load();
-    unsigned long long nslots = 1024;
-    while (nslots < 2ull * (unsigned long long)n) nslots <<= 1;
-    const size_t out_n = (size_t)std::max<int64_t>(capacity, 1);
+    HostCall c(ctx, "value_counts_str");
     uint8_t *d_chars = nullptr;
     long long *d_off = nullptr;
-    unsigned long long *d_slots = nullptr, *d_counts = nullptr, *d_out = nullptr;
-    cudaStream_t s = ctx->stream;
-    DevTimer kt;
-    cudaError_t e = scratch_alloc(&d_chars, (size_t)nbytes, s);
-    if (e == cudaSuccess) e = scratch_alloc(&d_off, (size_t)(n + 1) * 8, s);
-    if (e == cudaSuccess) e = scratch_alloc(&d_slots, nslots * 8, s);
-    if (e == cudaSuccess) e = scratch_alloc(&d_counts, nslots * 8, s);
-    if (e == cudaSuccess) e = scratch_alloc(&d_out, (2 * out_n + 1) * 8, s);
-    if (e == cudaSuccess && nbytes) e = cudaMemcpyAsync(d_chars, chars, (size_t)nbytes, cudaMemcpyHostToDevice, s);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(d_off, offsets, (size_t)(n + 1) * 8, cudaMemcpyHostToDevice, s);
-    if (e == cudaSuccess) e = kt.start(s);
-    if (e == cudaSuccess) e = cudaMemsetAsync(d_slots, 0xFF, nslots * 8, s);
-    if (e == cudaSuccess) e = cudaMemsetAsync(d_counts, 0, nslots * 8, s);
-    if (e == cudaSuccess) e = cudaMemsetAsync(d_out + 2 * out_n, 0, 8, s);
-    if (e == cudaSuccess) {
-        const int grid = (int)std::min<int64_t>((n + 255) / 256, (int64_t)ctx->sm_count * 8);
-        lo::k_hash_count_str<<<grid, 256, 0, s>>>(d_chars, d_off, n, d_slots, d_counts, nslots - 1);
-        lo::k_hash_compact_str<<<ctx->sm_count * 8, 256, 0, s>>>(d_slots, d_counts, nslots, (long long *)d_out, d_out + out_n,
-                                                                  (unsigned long long)capacity, d_out + 2 * out_n);
-        e = cudaGetLastError();
-        ctx->launches.fetch_add(2, std::memory_order_relaxed);
-    }
-    if (e == cudaSuccess) e = kt.stop(s);
-    unsigned long long nd = 0;
-    if (e == cudaSuccess) e = cudaMemcpyAsync(&nd, d_out + 2 * out_n, 8, cudaMemcpyDeviceToHost, s);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-    const size_t take = (size_t)std::min<unsigned long long>(nd, (unsigned long long)capacity);
-    if (e == cudaSuccess && take) e = cudaMemcpyAsync(rep_rows_out, d_out, take * 8, cudaMemcpyDeviceToHost, s);
-    if (e == cudaSuccess && take) e = cudaMemcpyAsync(counts_out, d_out + out_n, take * 8, cudaMemcpyDeviceToHost, s);
-    scratch_free(d_chars, s); scratch_free(d_off, s); scratch_free(d_slots, s); scratch_free(d_counts, s); scratch_free(d_out, s);
-    { const cudaError_t e2 = cudaStreamSynchronize(s); if (e == cudaSuccess) e = e2; }
-    if (e != cudaSuccess) return fail(e == cudaErrorMemoryAllocation ? LO_ERR_NOMEM : LO_ERR_CUDA, "value_counts_str: %s", cudaGetErrorString(e));
-    *ndistinct = (int64_t)nd;
-    if (timing) {
-        timing->total_ms  = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
-        timing->h2d_bytes = (double)nbytes + (double)(n + 1) * 8;
-        timing->d2h_bytes = (double)take * 16 + 8;
-        timing->launches  = ctx->launches.load() - launches0;
-        timing->kernel_ms = kt.ms();
-    }
-    if ((int64_t)nd > capacity)
-        return fail(LO_ERR_INVALID, "%llu distinct keys do not fit the caller's capacity %lld", nd, (long long)capacity);
-    return LO_OK;
+    c.alloc(&d_chars, (size_t)nbytes);
+    c.alloc(&d_off, (size_t)(n + 1) * 8);
+    c.to_dev(d_chars, chars, (size_t)nbytes);
+    c.to_dev(d_off, offsets, (size_t)(n + 1) * 8);
+    return value_counts_tail(c, n, rep_rows_out, counts_out, capacity, ndistinct, timing,
+        [&](unsigned long long *slots_keys, unsigned long long *counts, unsigned long long slots, unsigned long long *out, size_t out_n) {
+            const int grid = (int)std::min<int64_t>((n + 255) / 256, (int64_t)ctx->sm_count * 8);
+            lo::k_hash_count_str<<<grid, 256, 0, c.s>>>(d_chars, d_off, n, slots_keys, counts, slots - 1);
+            lo::k_hash_compact_str<<<ctx->sm_count * 8, 256, 0, c.s>>>(slots_keys, counts, slots, (long long *)out, out + out_n,
+                                                                        (unsigned long long)capacity, out + 2 * out_n);
+        });
 }
 
 // text -> number for one column of cells (R-semantics "number" cast).  chars: all cells back to back;
@@ -1491,47 +1524,32 @@ int lo_parse_number_host(lo_ctx *ctx, const uint8_t *chars, const int64_t *offse
     if (nbytes < 0 || (nbytes > 0 && !chars)) return fail(LO_ERR_INVALID, "bad offsets / chars");
     for (int64_t i = 0; i < n; ++i)
         if (offsets[i + 1] < offsets[i]) return fail(LO_ERR_INVALID, "offsets must be non-decreasing (row %lld)", (long long)i);
-    const auto t0 = std::chrono::steady_clock::now();
-    const int64_t launches0 = ctx->launches.load();
+    HostCall c(ctx, "parse_number");
     uint8_t *d_chars = nullptr, *d_status = nullptr;
     long long *d_off = nullptr;
     unsigned long long *d_val = nullptr;
-    cudaStream_t s = ctx->stream;
-    DevTimer kt;
-    cudaError_t e = scratch_alloc(&d_chars, (size_t)nbytes, s);
-    if (e == cudaSuccess) e = scratch_alloc(&d_off, (size_t)(n + 1) * 8, s);
-    if (e == cudaSuccess) e = scratch_alloc(&d_val, (size_t)n * 8, s);
-    if (e == cudaSuccess) e = scratch_alloc(&d_status, (size_t)n, s);
-    if (e == cudaSuccess && nbytes) e = cudaMemcpyAsync(d_chars, chars + offsets[0], (size_t)nbytes, cudaMemcpyHostToDevice, s);
+    c.alloc(&d_chars, (size_t)nbytes);
+    c.alloc(&d_off, (size_t)(n + 1) * 8);
+    c.alloc(&d_val, (size_t)n * 8);
+    c.alloc(&d_status, (size_t)n);
+    c.to_dev(d_chars, chars + offsets[0], (size_t)nbytes);
     std::vector<int64_t> rel;
     const int64_t *off_src = offsets;
-    if (e == cudaSuccess && offsets[0] != 0) {
+    if (offsets[0] != 0) {
         rel.resize(n + 1);
         for (int64_t i = 0; i <= n; ++i) rel[i] = offsets[i] - offsets[0];
         off_src = rel.data();
     }
-    if (e == cudaSuccess) e = cudaMemcpyAsync(d_off, off_src, (size_t)(n + 1) * 8, cudaMemcpyHostToDevice, s);
-    if (e == cudaSuccess) e = kt.start(s);
-    if (e == cudaSuccess) {
+    c.to_dev(d_off, off_src, (size_t)(n + 1) * 8);
+    c.mark();
+    c.launch(1, [&] {
         const int grid = (int)std::min<int64_t>((n + 127) / 128, (int64_t)ctx->sm_count * 16);
-        lo::k_parse_number<<<grid, 128, 0, s>>>(d_chars, d_off, n, d_val, d_status);
-        e = cudaGetLastError();
-        ctx->launches.fetch_add(1, std::memory_order_relaxed);
-    }
-    if (e == cudaSuccess) e = kt.stop(s);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(values, d_val, (size_t)n * 8, cudaMemcpyDeviceToHost, s);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(status, d_status, (size_t)n, cudaMemcpyDeviceToHost, s);
-    scratch_free(d_chars, s); scratch_free(d_off, s); scratch_free(d_val, s); scratch_free(d_status, s);
-    { const cudaError_t e2 = cudaStreamSynchronize(s); if (e == cudaSuccess) e = e2; }
-    if (e != cudaSuccess) return fail(e == cudaErrorMemoryAllocation ? LO_ERR_NOMEM : LO_ERR_CUDA, "parse_number: %s", cudaGetErrorString(e));
-    if (timing) {
-        timing->total_ms  = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
-        timing->h2d_bytes = (double)nbytes + (double)(n + 1) * 8;
-        timing->d2h_bytes = (double)n * 9;
-        timing->launches  = ctx->launches.load() - launches0;
-        timing->kernel_ms = kt.ms();
-    }
-    return LO_OK;
+        lo::k_parse_number<<<grid, 128, 0, c.s>>>(d_chars, d_off, n, d_val, d_status);
+    });
+    c.mark();
+    c.to_host(values, d_val, (size_t)n * 8);
+    c.to_host(status, d_status, (size_t)n);
+    return c.finish(timing);
 }
 
 // number -> text for one column (R-semantics "string" cast): cell lengths, an exclusive scan of them into the Arrow
@@ -1546,62 +1564,40 @@ int lo_format_number_host(lo_ctx *ctx, const double *values, const uint8_t *stat
     offsets[0] = 0;
     if (n == 0) return LO_OK;
     if (!values || !status) return fail(LO_ERR_INVALID, "NULL argument");
-    const auto t0 = std::chrono::steady_clock::now();
-    const int64_t launches0 = ctx->launches.load();
+    HostCall c(ctx, "format_number");
     unsigned long long *d_val = nullptr, *d_bad = nullptr;
     uint8_t *d_status = nullptr, *d_chars = nullptr;
     long long *d_off = nullptr;
     void *d_tmp = nullptr;
     size_t tmp_bytes = 0;
-    cudaStream_t s = ctx->stream;
-    DevTimer kt_len, kt_write;
     const int grid = (int)std::min<int64_t>((n + 127) / 128, (int64_t)ctx->sm_count * 16);
-    cudaError_t e = cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, d_off, n + 1, s);
-    if (e == cudaSuccess) e = scratch_alloc(&d_val, (size_t)n * 8, s);
-    if (e == cudaSuccess) e = scratch_alloc(&d_status, (size_t)n, s);
-    if (e == cudaSuccess) e = scratch_alloc(&d_off, (size_t)(n + 1) * 8, s);
-    if (e == cudaSuccess) e = scratch_alloc(&d_bad, 8, s);
-    if (e == cudaSuccess) e = scratch_alloc((char **)&d_tmp, tmp_bytes, s);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(d_val, values, (size_t)n * 8, cudaMemcpyHostToDevice, s);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(d_status, status, (size_t)n, cudaMemcpyHostToDevice, s);
-    if (e == cudaSuccess) e = cudaMemsetAsync(d_bad, 0xFF, 8, s);
-    if (e == cudaSuccess) e = cudaMemsetAsync(d_off + n, 0, 8, s);           // the scan's last input: offsets[n] = total
-    if (e == cudaSuccess) e = kt_len.start(s);
-    if (e == cudaSuccess) {
-        lo::k_format_number_len<<<grid, 128, 0, s>>>(d_val, d_status, n, d_off, d_bad);
-        e = cudaGetLastError();
-        if (e == cudaSuccess) e = cub::DeviceScan::ExclusiveSum(d_tmp, tmp_bytes, d_off, n + 1, s);
-        ctx->launches.fetch_add(2, std::memory_order_relaxed);
-    }
-    if (e == cudaSuccess) e = kt_len.stop(s);
+    c.run([&] { return cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, d_off, n + 1, c.s); });
+    c.alloc(&d_val, (size_t)n * 8);
+    c.alloc(&d_status, (size_t)n);
+    c.alloc(&d_off, (size_t)(n + 1) * 8);
+    c.alloc(&d_bad, 8);
+    c.alloc(&d_tmp, tmp_bytes);
+    c.to_dev(d_val, values, (size_t)n * 8);
+    c.to_dev(d_status, status, (size_t)n);
+    c.memset(d_bad, 0xFF, 8);
+    c.memset(d_off + n, 0, 8);           // the scan's last input: offsets[n] = total
+    c.mark();
+    c.launch(1, [&] { lo::k_format_number_len<<<grid, 128, 0, c.s>>>(d_val, d_status, n, d_off, d_bad); });
+    c.launch(1, [&] { return cub::DeviceScan::ExclusiveSum(d_tmp, tmp_bytes, d_off, n + 1, c.s); });
+    c.mark();
     unsigned long long bad = ~0ull;
-    if (e == cudaSuccess) e = cudaMemcpyAsync(offsets, d_off, (size_t)(n + 1) * 8, cudaMemcpyDeviceToHost, s);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(&bad, d_bad, 8, cudaMemcpyDeviceToHost, s);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-    const int64_t total = e == cudaSuccess ? offsets[n] : 0;
-    const bool write = e == cudaSuccess && bad >= (unsigned long long)n && chars && total <= chars_capacity && total > 0;
-    if (write) {
-        e = scratch_alloc(&d_chars, (size_t)total, s);
-        if (e == cudaSuccess) e = kt_write.start(s);
-        if (e == cudaSuccess) {
-            lo::k_format_number_write<<<grid, 128, 0, s>>>(d_val, d_status, n, d_off, d_chars);
-            e = cudaGetLastError();
-            ctx->launches.fetch_add(1, std::memory_order_relaxed);
-        }
-        if (e == cudaSuccess) e = kt_write.stop(s);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(chars, d_chars, (size_t)total, cudaMemcpyDeviceToHost, s);
+    c.to_host(offsets, d_off, (size_t)(n + 1) * 8);
+    c.to_host(&bad, d_bad, 8);
+    c.sync();
+    const int64_t total = c.ok() ? offsets[n] : 0;
+    if (bad >= (unsigned long long)n && chars && total <= chars_capacity && total > 0) {
+        c.alloc(&d_chars, (size_t)total);
+        c.mark();
+        c.launch(1, [&] { lo::k_format_number_write<<<grid, 128, 0, c.s>>>(d_val, d_status, n, d_off, d_chars); });
+        c.mark();
+        c.to_host(chars, d_chars, (size_t)total);
     }
-    scratch_free(d_val, s); scratch_free(d_status, s); scratch_free(d_off, s); scratch_free(d_bad, s);
-    scratch_free(d_tmp, s); scratch_free(d_chars, s);
-    { const cudaError_t e2 = cudaStreamSynchronize(s); if (e == cudaSuccess) e = e2; }
-    if (e != cudaSuccess) return fail(e == cudaErrorMemoryAllocation ? LO_ERR_NOMEM : LO_ERR_CUDA, "format_number: %s", cudaGetErrorString(e));
-    if (timing) {
-        timing->total_ms  = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
-        timing->h2d_bytes = (double)n * 9;
-        timing->d2h_bytes = (double)(n + 1) * 8 + 8 + (write ? (double)total : 0.0);
-        timing->launches  = ctx->launches.load() - launches0;
-        timing->kernel_ms = kt_len.ms() + kt_write.ms();
-    }
+    LO_TRY(c.finish(timing));
     if (bad < (unsigned long long)n) {
         const long long row = (long long)bad;
         if (status[row] > LO_NUM_EMPTY)
@@ -1627,20 +1623,11 @@ int lo_minmax_cast_host(lo_ctx *ctx, const double *const *in_cols, int64_t nrows
                                dim3 grid((unsigned)std::min<int64_t>((tin->nrows + 2047) / 2048, ctx->sm_count * 4), (unsigned)k);
                                lo::k_minmax_cast<<<grid, 256, 0, cs>>>(
                                    (const char *)tin->base, tin->pitch, tin->nrows, cdev);
-                               LO_CUDA(cudaGetLastError());
-                               ctx->launches.fetch_add(1, std::memory_order_relaxed);
+                               LO_CUDA(launched(ctx, 1));
                                return LO_OK;
                            });
     LO_TRY(rc);
-    for (int j = 0; j < k; ++j) {
-        nfinite[j] = tmp[(size_t)j * 3 + 2];
-        // the device kept min as ~ordered (so that zero-initialised memory is the identity) and max as ordered
-        uint32_t omin = ~(uint32_t)tmp[(size_t)j * 3 + 0], omax = (uint32_t)tmp[(size_t)j * 3 + 1];
-        auto unorder = [](uint32_t o) { uint32_t b = (o & 0x80000000u) ? (o ^ 0x80000000u) : ~o; float f; memcpy(&f, &b, 4); return f; };
-        mins[j] = nfinite[j] ? unorder(omin) : 0.f;
-        maxs[j] = nfinite[j] ? unorder(omax) : 0.f;
-    }
-    return LO_OK;
+    return lo_minmax_decode(tmp.data(), k, mins, maxs, nfinite);
 }
 
 }  // extern "C"

@@ -43,6 +43,54 @@ def prepare_columns(col_idx: Iterable[int]):
     return _i32(col_idx)[0]
 
 
+def _host_cols(cols, dtype):
+    """(ctypes pointer array, rows) of k equal-length contiguous 1-D host arrays of ``dtype``."""
+    for c in cols:
+        if c.dtype != dtype or not c.flags.c_contiguous or c.ndim != 1 or c.shape[0] != cols[0].shape[0]:
+            raise ValueError(f"cols must be equal-length contiguous 1-D {np.dtype(dtype).name} arrays")
+    return (C.c_void_p * len(cols))(*[c.ctypes.data for c in cols]), (cols[0].shape[0] if len(cols) else 0)
+
+
+def _out_cols(out, k: int, n: int):
+    """ctypes pointer array of k float32 output columns of n rows each, or None.  The library reads k entries: a short
+    ``out`` leaves NULL entries, which it rejects; a longer one raises IndexError here."""
+    if out is None:
+        return None
+    for o in out:
+        if o.dtype != np.float32 or not o.flags.c_contiguous or o.shape != (n,):
+            raise ValueError("out must be contiguous float32 arrays of the input length")
+    return (C.c_void_p * k)(*[o.ctypes.data for o in out])
+
+
+def _timing(t) -> dict:
+    """The lo_host_timing fields the chunked host pipelines report."""
+    return {"total_ms": t.total_ms, "h2d_bytes": t.h2d_bytes, "d2h_bytes": t.d2h_bytes, "launches": t.launches}
+
+
+def _minmax_decode(lib, raw: np.ndarray, k: int):
+    """(min, max, n_finite) of k columns from the raw uint64[3k] of a min/max pre-pass."""
+    mins, maxs, cnt = np.zeros(k, np.float32), np.zeros(k, np.float32), np.zeros(k, np.uint64)
+    N.check(lib.lo_minmax_decode(raw.ctypes.data_as(C.c_void_p), k, mins.ctypes.data_as(C.c_void_p),
+                                 maxs.ctypes.data_as(C.c_void_p), cnt.ctypes.data_as(C.c_void_p)))
+    return mins, maxs, cnt
+
+
+def _value_counts(call, n: int, key_dtype):
+    """(keys, counts) of a lo_value_counts_*_host call ``call(keys_out, counts_out, capacity, ndistinct_ref)``: room
+    for min(n, 65536) groups first, called again with room for every group when they did not fit."""
+    cap = max(min(n, 1 << 16), 1)
+    while True:
+        keys = np.empty(cap, dtype=key_dtype)
+        counts = np.empty(cap, dtype=np.uint64)
+        nd = C.c_int64()
+        rc = call(keys.ctypes.data_as(C.c_void_p), counts.ctypes.data_as(C.c_void_p), cap, C.byref(nd))
+        if rc == N.LO_ERR_INVALID and nd.value > cap:
+            cap = int(nd.value)
+            continue
+        N.check(rc)
+        return keys[:nd.value], counts[:nd.value]
+
+
 class DeviceCounts:
     """uint64[k, nbins] histogram counts resident in HBM (accumulated into by the kernels)."""
 
@@ -296,17 +344,8 @@ class Engine:
         :meth:`pinned_empty` lets copies overlap kernels).  out: k float32 arrays to fill, or None.
         Returns (counts [k, nbins] uint64 | None, timing dict)."""
         k = len(cols)
-        for c in cols:
-            if c.dtype != np.float64 or not c.flags.c_contiguous or c.ndim != 1 or c.shape[0] != cols[0].shape[0]:
-                raise ValueError("cols must be equal-length contiguous 1-D float64 arrays")
-        n = cols[0].shape[0] if k else 0
-        in_p = (C.c_void_p * k)(*[c.ctypes.data for c in cols])
-        out_p = None
-        if out is not None:
-            for o in out:
-                if o.dtype != np.float32 or not o.flags.c_contiguous or o.shape != (n,):
-                    raise ValueError("out must be contiguous float32 arrays of the input length")
-            out_p = (C.c_void_p * k)(*[o.ctypes.data for o in out])
+        in_p, n = _host_cols(cols, np.float64)
+        out_p = _out_cols(out, k, n)
         spec_ref, counts, keep = None, None, None
         if nbins:
             spec, keep = self._spec(k, nbins, lo, hi)
@@ -316,21 +355,15 @@ class Engine:
         N.check(self._lib.lo_project_cast_hist_host(self._ctx, in_p, n, k, out_p, spec_ref,
                                                     counts.ctypes.data_as(C.c_void_p) if counts is not None else None,
                                                     C.byref(timing)))
-        return counts, {"total_ms": timing.total_ms, "h2d_bytes": timing.h2d_bytes, "d2h_bytes": timing.d2h_bytes,
-                        "launches": timing.launches}
+        return counts, _timing(timing)
 
     def hist_u8_cols_host(self, cols: Sequence[np.ndarray]):
         k = len(cols)
-        for c in cols:
-            if c.dtype != np.uint8 or not c.flags.c_contiguous or c.ndim != 1 or c.shape[0] != cols[0].shape[0]:
-                raise ValueError("cols must be equal-length contiguous 1-D uint8 arrays")
-        n = cols[0].shape[0] if k else 0
-        in_p = (C.c_void_p * k)(*[c.ctypes.data for c in cols])
+        in_p, n = _host_cols(cols, np.uint8)
         counts = np.zeros((k, 256), dtype=np.uint64)
         timing = N.HostTiming()
         N.check(self._lib.lo_hist_u8_cols_host(self._ctx, in_p, n, k, counts.ctypes.data_as(C.c_void_p), C.byref(timing)))
-        return counts, {"total_ms": timing.total_ms, "h2d_bytes": timing.h2d_bytes, "d2h_bytes": timing.d2h_bytes,
-                        "launches": timing.launches}
+        return counts, _timing(timing)
 
     def value_counts_u32_host(self, codes: np.ndarray, ncodes: int) -> np.ndarray:
         """counts[c] = number of entries of ``codes`` (uint32, dictionary encoded) equal to c."""
@@ -362,13 +395,7 @@ class Engine:
         """cells: list of ``str`` / ``bytes``.  Returns (values float64[n], status uint8[n]) — values are what
         CPython's ``float(cell)`` returns, status as LO_NUM_* (``_native``)."""
         from .columnar import pack_number_cells
-        n = len(cells)
-        chars, offsets = pack_number_cells(cells)      # non-ASCII digits / whitespace normalised as float(str) does
-        values = np.zeros(n, dtype=np.float64)
-        status = np.zeros(n, dtype=np.uint8)
-        N.check(self._lib.lo_parse_number_host(self._ctx, chars.ctypes.data_as(C.c_void_p), offsets.ctypes.data_as(C.c_void_p),
-                                               n, values.ctypes.data_as(C.c_void_p), status.ctypes.data_as(C.c_void_p), None))
-        return values, status
+        return self.parse_number_packed(*pack_number_cells(cells))   # non-ASCII digits / whitespace normalised as float(str) does
 
     def parse_number_packed(self, chars: np.ndarray, offsets: np.ndarray):
         """The same on an already packed column (chars uint8, offsets int64[n+1]) — e.g. the buffers of an Arrow
@@ -405,8 +432,7 @@ class Engine:
                                                 n, offsets.ctypes.data_as(C.c_void_p), chars.ctypes.data_as(C.c_void_p), cap,
                                                 C.byref(t)))
         if timing is not None:
-            timing.update(total_ms=t.total_ms, kernel_ms=t.kernel_ms, h2d_bytes=t.h2d_bytes, d2h_bytes=t.d2h_bytes,
-                          launches=t.launches)
+            timing.update(_timing(t), kernel_ms=t.kernel_ms)
         return chars[:offsets[n]], offsets
 
     def read_csv_host(self, body, timing: dict | None = None):
@@ -446,38 +472,17 @@ class Engine:
         n = offsets.shape[0] - 1
         if n == 0:
             return np.zeros(0, np.int64), np.zeros(0, np.uint64)
-        cap = max(min(n, 1 << 16), 1)
-        while True:
-            rows = np.empty(cap, dtype=np.int64)
-            counts = np.empty(cap, dtype=np.uint64)
-            nd = C.c_int64()
-            rc = self._lib.lo_value_counts_str_host(self._ctx, chars.ctypes.data_as(C.c_void_p), offsets.ctypes.data_as(C.c_void_p),
-                                                    n, rows.ctypes.data_as(C.c_void_p), counts.ctypes.data_as(C.c_void_p),
-                                                    cap, C.byref(nd), None)
-            if rc == N.LO_ERR_INVALID and nd.value > cap:
-                cap = int(nd.value)
-                continue
-            N.check(rc)
-            return rows[:nd.value], counts[:nd.value]
+        return _value_counts(lambda rows, counts, cap, nd: self._lib.lo_value_counts_str_host(
+            self._ctx, chars.ctypes.data_as(C.c_void_p), offsets.ctypes.data_as(C.c_void_p), n, rows, counts, cap, nd, None),
+            n, np.int64)
 
     def value_counts_f64_host(self, values: np.ndarray):
         """(keys float64[g], counts uint64[g]) — exact value counts of a numeric column (GPU hash group-by),
         -0.0 grouped with 0.0 and all NaNs together; order unspecified."""
         values = np.ascontiguousarray(values, dtype=np.float64)
         n = values.shape[0]
-        cap = max(min(n, 1 << 16), 1)
-        while True:
-            keys = np.empty(cap, dtype=np.float64)
-            counts = np.empty(cap, dtype=np.uint64)
-            nd = C.c_int64()
-            rc = self._lib.lo_value_counts_f64_host(self._ctx, values.ctypes.data_as(C.c_void_p), n,
-                                                    keys.ctypes.data_as(C.c_void_p), counts.ctypes.data_as(C.c_void_p),
-                                                    cap, C.byref(nd), None)
-            if rc == N.LO_ERR_INVALID and nd.value > cap:
-                cap = int(nd.value)
-                continue
-            N.check(rc)
-            return keys[:nd.value], counts[:nd.value]
+        return _value_counts(lambda keys, counts, cap, nd: self._lib.lo_value_counts_f64_host(
+            self._ctx, values.ctypes.data_as(C.c_void_p), n, keys, counts, cap, nd, None), n, np.float64)
 
     def minmax_cast(self, table: DeviceTable, col_idx, stream=None):
         """(min, max, n_finite) of the fp32-cast values of resident columns (range pre-pass on the device)."""
@@ -486,10 +491,7 @@ class Engine:
         N.check(self._lib.lo_minmax_cast_dev(self._ctx, table._h, idx, k, raw._ptr, _stream_ptr(stream)))
         host = raw.to_numpy(stream)
         raw.free()
-        mins, maxs, cnt = np.zeros(k, np.float32), np.zeros(k, np.float32), np.zeros(k, np.uint64)
-        N.check(self._lib.lo_minmax_decode(host.ctypes.data_as(C.c_void_p), k, mins.ctypes.data_as(C.c_void_p),
-                                           maxs.ctypes.data_as(C.c_void_p), cnt.ctypes.data_as(C.c_void_p)))
-        return mins, maxs, cnt
+        return _minmax_decode(self._lib, host, k)
 
     @property
     def resident(self):
@@ -503,18 +505,4 @@ class Engine:
         """cells: list of ``str`` / ``bytes``.  Returns (rep_rows int64[g], counts uint64[g]): one representative row
         per distinct cell and the group sizes (GPU hash group-by on the bytes, exact)."""
         from .columnar import pack_cells
-        n = len(cells)
-        chars, offsets = pack_cells(cells)
-        cap = max(min(n, 1 << 16), 1)
-        while True:
-            rows = np.empty(cap, dtype=np.int64)
-            counts = np.empty(cap, dtype=np.uint64)
-            nd = C.c_int64()
-            rc = self._lib.lo_value_counts_str_host(self._ctx, chars.ctypes.data_as(C.c_void_p), offsets.ctypes.data_as(C.c_void_p),
-                                                    n, rows.ctypes.data_as(C.c_void_p), counts.ctypes.data_as(C.c_void_p),
-                                                    cap, C.byref(nd), None)
-            if rc == N.LO_ERR_INVALID and nd.value > cap:
-                cap = int(nd.value)
-                continue
-            N.check(rc)
-            return rows[:nd.value], counts[:nd.value]
+        return self.value_counts_str_packed(*pack_cells(cells))

@@ -310,15 +310,10 @@ class ShardedEngine:
 
     def minmax_cast(self, table: ShardedTable, col_idx, streams=None):
         """(min, max, n_finite) per column over ALL shards (the range pre-pass of a histogram without ``range``)."""
-        import numpy as np
-        from .engine import _i32
+        from .engine import _i32, _minmax_decode
         idx, k = _i32(col_idx)
         self._N.check(self._lib.lo_group_minmax_cast_dev(self._g, self._tables(table), idx, k, self._streams(streams)))
-        raw = self.result(3 * k)
-        mins, maxs, cnt = np.zeros(k, np.float32), np.zeros(k, np.float32), np.zeros(k, np.uint64)
-        self._N.check(self._lib.lo_minmax_decode(raw.ctypes.data_as(C.c_void_p), k, mins.ctypes.data_as(C.c_void_p),
-                                                 maxs.ctypes.data_as(C.c_void_p), cnt.ctypes.data_as(C.c_void_p)))
-        return mins, maxs, cnt
+        return _minmax_decode(self._lib, self.result(3 * k), k)
 
     def result(self, n: int, member: int = 0):
         """First ``n`` merged counts of the last step as held by local member ``member`` (waits for that step)."""
@@ -345,19 +340,11 @@ class ShardedEngine:
         """Same contract as ``Engine.project_cast_hist_host``; the rows passed are this process's rows, cut across its
         local members by the library.  counts: merged over the whole group (zeros on a rank that holds no result)."""
         import numpy as np
+        from .engine import _host_cols, _out_cols, _timing
         N = self._N
         k = len(cols)
-        n = cols[0].shape[0] if k else 0
-        for c in cols:
-            if c.dtype != np.float64 or not c.flags.c_contiguous or c.ndim != 1 or c.shape[0] != n:
-                raise ValueError("cols must be equal-length contiguous 1-D float64 arrays")
-        in_p = (C.c_void_p * k)(*[c.ctypes.data for c in cols])
-        out_p = None
-        if out is not None:
-            for o in out:
-                if o.dtype != np.float32 or not o.flags.c_contiguous or o.shape != (n,):
-                    raise ValueError("out must be contiguous float32 arrays of the input length")
-            out_p = (C.c_void_p * k)(*[o.ctypes.data for o in out])
+        in_p, n = _host_cols(cols, np.float64)
+        out_p = _out_cols(out, k, n)
         spec_ref, counts, _keep = None, None, None
         if nbins:
             spec, _keep = self.engines[0]._spec(k, nbins, lo, hi)
@@ -367,24 +354,19 @@ class ShardedEngine:
         N.check(self._lib.lo_group_project_cast_hist_host(
             self._g, in_p, n, k, out_p, spec_ref, counts.ctypes.data_as(C.c_void_p) if counts is not None else None,
             N.LO_GROUP_BCAST if bcast else 0, C.byref(timing)))
-        return counts, {"total_ms": timing.total_ms, "h2d_bytes": timing.h2d_bytes, "d2h_bytes": timing.d2h_bytes,
-                        "launches": timing.launches}
+        return counts, _timing(timing)
 
     def hist_u8_cols_host(self, cols, bcast: bool = False):
         import numpy as np
+        from .engine import _host_cols, _timing
         N = self._N
         k = len(cols)
-        n = cols[0].shape[0] if k else 0
-        for c in cols:
-            if c.dtype != np.uint8 or not c.flags.c_contiguous or c.ndim != 1 or c.shape[0] != n:
-                raise ValueError("cols must be equal-length contiguous 1-D uint8 arrays")
-        in_p = (C.c_void_p * k)(*[c.ctypes.data for c in cols])
+        in_p, n = _host_cols(cols, np.uint8)
         counts = np.zeros((k, 256), dtype=np.uint64)
         timing = N.HostTiming()
         N.check(self._lib.lo_group_hist_u8_cols_host(self._g, in_p, n, k, counts.ctypes.data_as(C.c_void_p),
                                                      N.LO_GROUP_BCAST if bcast else 0, C.byref(timing)))
-        return counts, {"total_ms": timing.total_ms, "h2d_bytes": timing.h2d_bytes, "d2h_bytes": timing.d2h_bytes,
-                        "launches": timing.launches}
+        return counts, _timing(timing)
 
     # ---- what the executors expect from an engine ----------------------------------------------------------
     def minmax_cast_host(self, cols):

@@ -137,3 +137,15 @@ def test_ctypes_mirror_matches_the_header_constants_and_struct_layouts(tmp_path)
         assert int(got[f"sizeof.{struct}"]) == ctypes.sizeof(mirror), struct
         for f, _t in mirror._fields_:
             assert int(got[f"offsetof.{struct}.{f}"]) == getattr(mirror, f).offset, f"{struct}.{f}"
+
+
+def test_output_column_array_has_one_entry_per_input_column():
+    """The *project_cast_hist_host calls read k out_cols entries: a short ``out`` list leaves NULL entries, which the
+    library rejects ("out_cols[j] is NULL"); a longer one is refused before any call."""
+    import numpy as np
+    from learningorchestra_b200.engine import _out_cols
+    o = np.zeros(4, np.float32)
+    arr = _out_cols([o], 3, 4)
+    assert len(arr) == 3 and arr[0] == o.ctypes.data and arr[1] is None and arr[2] is None
+    with pytest.raises(IndexError):
+        _out_cols([o, o], 1, 4)
