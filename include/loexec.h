@@ -376,6 +376,52 @@ int lo_csv_read_host(lo_ctx *ctx, const uint8_t *body, int64_t nbytes, lo_csv **
 int lo_csv_columns_host(lo_csv *h, int64_t *offsets, uint8_t *chars, int64_t chars_capacity, lo_host_timing *timing);
 int lo_csv_free(lo_csv *h);
 
+/* The same reader on a body fed in pieces, with device memory bounded by a window instead of the body.
+ *
+ * lo_csv_stream_open: window_bytes = the window's starting capacity W (0 -> LO_CSV_STREAM_WINDOW).
+ * lo_csv_stream_push: hands the stream `n` more bytes of the body; last = 1 says they end it (n may be 0).  Pieces may
+ *   be of any size and cut anywhere (inside "\r\n", a UTF-8 sequence, a "" pair, a quoted multi-line field, a record):
+ *   the result does not depend on the cuts.  The stream copies what fits into its window [tail of the last window |
+ *   new bytes]; when the window is full, or holds the body's last byte, it reads the window up to one past the last
+ *   byte that ended a record (all of it at the end of the body) and keeps the rest as the next window's tail.  A push
+ *   reads at most one window: win->consumed says how many of the n bytes it took, and the caller pushes the others
+ *   again (with the same `last`).  win->records records were read (win->first_record = the absolute index of the
+ *   first; record 0 is the header) with win->ncols columns and win->chars bytes of text; lo_csv_stream_columns copies
+ *   them out in lo_csv_columns_host's layout (offsets int64[ncols][records + 1], absolute in the window's chars), and
+ *   must be called before the next push, which releases them.
+ *   A full window in which no record ends doubles its capacity; only a record the device cannot hold fails, with
+ *   LO_ERR_NOMEM naming its size.
+ *   *info is the body so far as lo_csv_read_host reports it: once win->done, it equals lo_csv_read_host's info on the
+ *   whole body (records, ncols, chars summed over the windows; fail_record and fail_pos absolute in the body).  The
+ *   stream is done after the last byte, or after the first failing record: the rows before it have been delivered,
+ *   and later pushes take their bytes and do nothing.  Any other error (LO_ERR_NOMEM, LO_ERR_CUDA) ends the stream:
+ *   later pushes fail with LO_ERR_INVALID.
+ * Device memory: with W the window's capacity (window_bytes, doubled while a record does not fit in it), the stream
+ *   holds at most 2W (the window and its tail buffer) + 0.47W (segment scratch) + CUB temporary storage + the columns
+ *   of one window: 8 bytes per kept cell + 8 (ncols + 1) + at most W of text; a cell takes at least half a byte of
+ *   the window, so in no case more than 19.5W + CUB storage + 8 (ncols + 1).  It does not grow with the body.
+ *   win->peak_device_bytes reports the most the stream has held so far.
+ * lo_csv_stream_free releases the stream (NULL is fine).  The calls follow the single-pass rules: no device-wide
+ * synchronisation, scratch from the stream-ordered pool, the first error reported, lo_host_timing filled per call. */
+#define LO_CSV_STREAM_WINDOW (64ll << 20)
+typedef struct lo_csv_stream lo_csv_stream;
+typedef struct lo_csv_window {
+    int64_t consumed;            /* bytes of this push taken by the stream */
+    int64_t records;             /* records read by this push (their columns: lo_csv_stream_columns) */
+    int64_t first_record;        /* absolute index of the first of them */
+    int64_t ncols;
+    int64_t chars;               /* their bytes of text */
+    int64_t peak_device_bytes;   /* the most device memory the stream has held so far */
+    int32_t done;                /* 1: the body is read, or a record failed */
+    int32_t pad;
+} lo_csv_window;
+int lo_csv_stream_open(lo_ctx *ctx, int64_t window_bytes, lo_csv_stream **out);
+int lo_csv_stream_push(lo_csv_stream *st, const uint8_t *bytes, int64_t n, int32_t last, lo_csv_window *win,
+                       lo_csv_info *info, lo_host_timing *timing);
+int lo_csv_stream_columns(lo_csv_stream *st, int64_t *offsets, uint8_t *chars, int64_t chars_capacity,
+                          lo_host_timing *timing);
+int lo_csv_stream_free(lo_csv_stream *st);
+
 #ifdef __cplusplus
 }
 #endif

@@ -35,6 +35,7 @@ LO_GROUP_MAX_COUNTS = 262144
 LO_NUM_FLOAT, LO_NUM_INTEGER, LO_NUM_EMPTY, LO_NUM_INVALID, LO_NUM_UNSUPPORTED = 0, 1, 2, 3, 4
 LO_FORMAT_MAX_CELL = 310
 LO_CSV_OK, LO_CSV_SHORT_ROW, LO_CSV_FIELD_LIMIT, LO_CSV_BAD_UTF8, LO_CSV_NUL, LO_CSV_UNSUPPORTED, LO_CSV_EMPTY = range(7)
+LO_CSV_STREAM_WINDOW = 64 << 20
 LO_ABI_VERSION = 3
 
 _ERR_NAMES = {
@@ -66,6 +67,11 @@ class HostTiming(C.Structure):
 class CsvInfo(C.Structure):
     _fields_ = [("records", C.c_int64), ("ncols", C.c_int64), ("chars", C.c_int64), ("fail_record", C.c_int64),
                 ("fail_kind", C.c_int32), ("pad", C.c_int32), ("fail_pos", C.c_int64)]
+
+
+class CsvWindow(C.Structure):
+    _fields_ = [("consumed", C.c_int64), ("records", C.c_int64), ("first_record", C.c_int64), ("ncols", C.c_int64),
+                ("chars", C.c_int64), ("peak_device_bytes", C.c_int64), ("done", C.c_int32), ("pad", C.c_int32)]
 
 
 # every symbol include/loexec.h declares: name -> (restype, argtypes)
@@ -135,6 +141,11 @@ SIGNATURES = {
     "lo_csv_read_host": (C.c_int, [_P, _P, C.c_int64, C.POINTER(_P), C.POINTER(CsvInfo), C.POINTER(HostTiming)]),
     "lo_csv_columns_host": (C.c_int, [_P, _P, _P, C.c_int64, C.POINTER(HostTiming)]),
     "lo_csv_free": (C.c_int, [_P]),
+    "lo_csv_stream_open": (C.c_int, [_P, C.c_int64, C.POINTER(_P)]),
+    "lo_csv_stream_push": (C.c_int, [_P, _P, C.c_int64, C.c_int32, C.POINTER(CsvWindow), C.POINTER(CsvInfo),
+                                     C.POINTER(HostTiming)]),
+    "lo_csv_stream_columns": (C.c_int, [_P, _P, _P, C.c_int64, C.POINTER(HostTiming)]),
+    "lo_csv_stream_free": (C.c_int, [_P]),
 }
 
 _lib = None

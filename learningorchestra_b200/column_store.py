@@ -207,6 +207,16 @@ def _tokenize_device(read_csv, source):
     return header, columns, n, exc
 
 
+def _tokenize_stream(read_stream, source):
+    """(header cells or None, Arrow columns, rows, failure exception or None) by the engine's GPU reader, the source
+    streamed from its path or file object in windows."""
+    header, n, columns, failure = read_stream(source)
+    exc = None if failure is None else _csv_failure(*failure)
+    if header is None:
+        return None, [], 0, exc
+    return header, columns, n, exc
+
+
 class _Table:
     def __init__(self, ids, columns):
         self.ids = np.ascontiguousarray(ids, dtype=np.int64)
@@ -314,15 +324,19 @@ class ColumnarDatabase(Database):
 
         With an engine that has ``read_csv_host`` the body is tokenised on the GPU with the reference's own
         ``csv.reader`` rules: a body the reference fails on keeps the data rows before the failing record, ``finished``
-        stays False and the metadata's ``exception`` says why (a failing header stores no rows).  Without one, pyarrow
-        tokenises it and a malformed body raises."""
+        stays False and the metadata's ``exception`` says why (a failing header stores no rows).  An engine with
+        ``read_csv_stream`` streams the source through the reader in windows, so the body's size is bounded by
+        neither device nor host memory.  Without an engine, pyarrow tokenises it and a malformed body raises."""
         self.insert_one_in_file(filename, {"datasetName": filename, "url": url, "timeCreated": _now(), "_id": 0,
                                            "finished": False, "type": "dataset/csv"})
+        read_stream = getattr(engine, "read_csv_stream", None)
         read_csv = getattr(engine, "read_csv_host", None)
-        if read_csv is None:
-            raw_names, columns, n, failure = _tokenize_pyarrow(source)
-        else:
+        if read_stream is not None:
+            raw_names, columns, n, failure = _tokenize_stream(read_stream, source)
+        elif read_csv is not None:
             raw_names, columns, n, failure = _tokenize_device(read_csv, source)
+        else:
+            raw_names, columns, n, failure = _tokenize_pyarrow(source)
         cols = OrderedDict()
         if raw_names is not None:
             names = [re.sub(r"\W+", "", name) for name in raw_names]

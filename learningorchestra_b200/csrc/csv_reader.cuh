@@ -1,5 +1,5 @@
 // csv_reader.cuh — the CSV rules of the reference's upload reader, byte by byte, for the device reader (csv.inc) and
-// the g++ harness (tests/native/csv_harness.cpp).  __host__ __device__, no CUDA runtime calls.
+// the g++ harnesses (tests/native/csv_harness.cpp, csv_stream_harness.cpp).  __host__ __device__, no CUDA runtime calls.
 //
 // The reference reads an upload with
 //     csv.reader(codecs.iterdecode(response.iter_lines(), "utf-8"), delimiter=",", quotechar='"')
@@ -253,13 +253,15 @@ struct NoVisit {
     LO_CSV_HD void fail(const Carry &, uint64_t) {}
 };
 
-// first record with a parse failure, first data record with fewer than ncols fields
+// first record with a parse failure, first data record with fewer than ncols fields; rec0 = records before the bytes
+// walked (0 for a whole body, so record 0 is the header)
 struct ValidateVisit {
     int64_t ncols;
+    int64_t rec0 = 0;
     int64_t fail_rec = INT64_MAX, short_rec = INT64_MAX;
     LO_CSV_HD void keep(int64_t, const Carry &) {}
     LO_CSV_HD void save(const Carry &) {}
-    LO_CSV_HD void end(const Carry &c) { if (c.rec > 0 && c.col < ncols && c.rec < short_rec) short_rec = c.rec; }
+    LO_CSV_HD void end(const Carry &c) { if (rec0 + c.rec > 0 && c.col < ncols && c.rec < short_rec) short_rec = c.rec; }
     LO_CSV_HD void fail(const Carry &c, uint64_t) { if (c.rec < fail_rec) fail_rec = c.rec; }
 };
 
@@ -286,6 +288,52 @@ struct ScatterVisit {
     LO_CSV_HD void save(const Carry &) {}
     LO_CSV_HD void end(const Carry &) {}
     LO_CSV_HD void fail(const Carry &, uint64_t) {}
+};
+
+// ---- a body fed in pieces: windows ----------------------------------------------------------------------------------
+// Every record ends at a line end or at EOF, and the state after a record end is START_RECORD, so a body can be cut
+// one past any byte that ended a record and the rest read as a body of its own.  Then the bytes before the cut are a
+// complete body to the passes above: the EOF step does nothing there (the last byte is a line break, the state
+// START_RECORD) and UTF-8 look-ahead meets that break before the cut.  The rest starts with a line break only when a
+// run of breaks straddles the cut; it is then classed as a line end instead of skipped, which in START_RECORD is the
+// same step.  What the later part needs from the earlier: the header's field count, and how many records and bytes
+// came before it (record indices and failure positions are absolute in the whole body).
+
+// Position in [b, e) of the last byte that ended a record, walking from state s; -1 if none.
+LO_CSV_HD int64_t segment_last_end(const uint8_t *body, int64_t b, int64_t e, uint32_t s) {
+    int64_t last = -1;
+    int32_t prev = b > 0 ? (int32_t)body[b - 1] : -1;
+    for (int64_t p = b; p < e; ++p) {
+        const uint32_t t = step(s, byte_class(body[p], prev));
+        prev = body[p];
+        s = t & 7u;
+        if ((t >> 4) & kEnd) last = p;
+    }
+    return last;
+}
+
+// The bookkeeping of a window [tail of the previous window | new bytes] of at most cap bytes.  A piece is taken into
+// the window as far as it fits; a full window (or the body's last byte) is read up to its cut: one past the last byte
+// that ended a record, or its whole length at the end of the body.  A full window in which no record ends doubles
+// instead.  [cut, len) is the next window's tail.
+struct StreamWindow {
+    int64_t cap;             // bytes the window holds
+    int64_t len = 0;         // bytes in it
+    int64_t base = 0;        // offset of its first byte in the body
+    int64_t rec0 = 0;        // records before it (absolute index of its first record)
+    int64_t ncols = -1;      // the header's fields once record 0 has been read; -1 before
+    LO_CSV_HD int64_t take(int64_t n) const { return n < cap - len ? n : cap - len; }
+    LO_CSV_HD bool ready(bool final) const { return final || len == cap; }
+    // last_end: the window's last byte that ended a record (-1: none); 0 -> grow the window
+    LO_CSV_HD int64_t cut(int64_t last_end, bool final) const { return final ? len : last_end + 1; }
+    LO_CSV_HD void grow() { cap *= 2; }
+    // the window was read up to cut; nrec records ended in it, the first of them the header when rec0 == 0
+    LO_CSV_HD void advance(int64_t cut, int64_t nrec, int64_t header_cols) {
+        if (rec0 == 0 && nrec > 0) ncols = header_cols;
+        base += cut;
+        len -= cut;
+        rec0 += nrec;
+    }
 };
 
 }  // namespace csv

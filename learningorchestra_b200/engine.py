@@ -11,6 +11,9 @@ dataType services talk to mongod through pymongo (``histogram_image/utils.py:50-
 from __future__ import annotations
 
 import ctypes as C
+import io
+import os
+import threading
 from typing import Iterable, Sequence
 
 import numpy as np
@@ -89,6 +92,77 @@ def _value_counts(call, n: int, key_dtype):
             continue
         N.check(rc)
         return keys[:nd.value], counts[:nd.value]
+
+
+def _pieces(source, buf: np.ndarray):
+    """(n, last) for each piece of ``source`` read into ``buf`` (uint8): full pieces, the rest, then (0, True).
+    source: a path, a binary or text file object, or an iterable of bytes."""
+    if isinstance(source, (str, os.PathLike)):
+        with open(source, "rb", buffering=0) as f:
+            yield from _pieces(f, buf)
+        return
+    view = memoryview(buf)
+    if hasattr(source, "readinto") and not isinstance(source, io.TextIOBase):
+        while True:
+            n = 0
+            while n < buf.size:
+                k = source.readinto(view[n:])
+                if not k:
+                    break
+                n += k
+            if n:
+                yield n, False
+            if n < buf.size:
+                break
+    else:
+        if hasattr(source, "read"):
+            chunks = iter(lambda: source.read(buf.size), source.read(0))
+        else:
+            chunks = iter(source)
+        n = 0
+        for chunk in chunks:
+            data = memoryview(chunk.encode("utf-8") if isinstance(chunk, str) else chunk).cast("B")
+            while len(data):
+                k = min(len(data), buf.size - n)
+                view[n:n + k] = data[:k]
+                n += k
+                data = data[k:]
+                if n == buf.size:
+                    yield n, False
+                    n = 0
+        if n:
+            yield n, False
+    yield 0, True
+
+
+class _TextBuilder:
+    """One text column grown window by window: chars and int64 offsets, doubled as they fill."""
+
+    def __init__(self):
+        self.chars, self.nchars = np.empty(1 << 10, np.uint8), 0
+        self.offsets, self.nrows = np.zeros(1 << 10, np.int64), 0
+
+    @staticmethod
+    def _room(a: np.ndarray, need: int) -> np.ndarray:
+        if need <= a.size:
+            return a
+        b = np.empty(max(need, 2 * a.size), a.dtype)
+        b[:a.size] = a
+        return b
+
+    def append(self, chars: np.ndarray, offsets: np.ndarray):
+        """Cells i of offsets[i]..offsets[i + 1] in chars (absolute offsets, one column of a window)."""
+        k, lo, hi = offsets.size - 1, int(offsets[0]), int(offsets[-1])
+        self.chars = self._room(self.chars, self.nchars + hi - lo)
+        self.chars[self.nchars:self.nchars + hi - lo] = chars[lo:hi]
+        self.offsets = self._room(self.offsets, self.nrows + k + 1)
+        np.add(offsets[1:], self.nchars - lo, out=self.offsets[self.nrows + 1:self.nrows + k + 1])
+        self.nchars += hi - lo
+        self.nrows += k
+
+    def array(self, pa):
+        return pa.LargeStringArray.from_buffers(self.nrows, pa.py_buffer(self.offsets[:self.nrows + 1]),
+                                                pa.py_buffer(self.chars[:self.nchars]))
 
 
 class DeviceCounts:
@@ -216,6 +290,8 @@ class Engine:
         N.check(self._lib.lo_ctx_device(ctx, C.byref(dev), C.byref(sms), C.byref(hbm)))
         self.device, self.sm_count, self.hbm_bytes = dev.value, sms.value, hbm.value
         self._pinned: dict[int, C.c_void_p] = {}
+        self._staged: dict[str, np.ndarray] = {}     # reused pinned buffers (read_csv_stream)
+        self._stream_lock = threading.Lock()          # read_csv_stream's buffers serve one call at a time
 
     # ---- lifetime ---------------------------------------------------------------------------------
     def close(self) -> None:
@@ -225,6 +301,7 @@ class Engine:
             for p in list(self._pinned.values()):
                 self._lib.lo_host_free(self._ctx, p)
             self._pinned.clear()
+            self._staged.clear()
             self._lib.lo_shutdown(self._ctx)
             self._ctx = None
 
@@ -466,6 +543,82 @@ class Engine:
             if info.records else None
         failure = None if info.fail_kind == N.LO_CSV_OK else (int(info.fail_kind), int(info.fail_record), int(info.fail_pos))
         return header, max(int(info.records) - 1, 0), chars, offsets, failure
+
+    def _staging(self, key: str, nbytes: int) -> np.ndarray:
+        """A page-locked uint8 buffer of at least nbytes kept on the engine under ``key``, replaced when too small."""
+        old = self._staged.get(key)
+        if old is not None and old.size >= nbytes:
+            return old
+        if old is not None:
+            self._lib.lo_host_free(self._ctx, self._pinned.pop(old.ctypes.data))
+        buf = self._staged[key] = self.pinned_empty(max(int(nbytes), 1), np.uint8)
+        return buf
+
+    def read_csv_stream(self, source, window_bytes: int | None = None, timing: dict | None = None):
+        """:meth:`read_csv_host` on a body of any size: the source is read in pieces of one window into pinned memory
+        and streamed through the device reader (``lo_csv_stream_*``), whose device memory is bounded by the window, not
+        the body; the whole body is never held on the host either.
+
+        source: a path, a binary (or text) file object, or an iterable of ``bytes``.  window_bytes: the window's
+        starting size (None: LO_CSV_STREAM_WINDOW, 64 MiB); it doubles while a record does not fit.  Returns
+        ``(header_cells, nrows, columns, failure)``: columns are one single-chunk ``pa.LargeStringArray`` per header
+        cell, failure as :meth:`read_csv_host` gives it; the result equals read_csv_host's on the whole body.
+        ``timing``: a dict to receive the calls' lo_host_timing fields summed, the number of windows read and the most
+        device memory the stream held (``peak_device_bytes``)."""
+        window = int(window_bytes) if window_bytes else N.LO_CSV_STREAM_WINDOW
+        if window < 1:
+            raise ValueError("window_bytes must be positive")
+        with self._stream_lock:
+            return self._read_csv_stream(source, window, timing)
+
+    def _read_csv_stream(self, source, window, timing):
+        import pyarrow as pa
+        st, win, info, t = C.c_void_p(), N.CsvWindow(), N.CsvInfo(), N.HostTiming()
+        sums = dict(total_ms=0.0, kernel_ms=0.0, h2d_bytes=0.0, d2h_bytes=0.0, launches=0, windows=0)
+
+        def add(t, kernel=True):
+            for k in ("total_ms", "h2d_bytes", "d2h_bytes", "launches") + (("kernel_ms",) if kernel else ()):
+                sums[k] += getattr(t, k)
+
+        piece = self._staging("csv_piece", window)
+        header, cols = None, []
+        N.check(self._lib.lo_csv_stream_open(self._ctx, window, C.byref(st)))
+        try:
+            for n, last in _pieces(source, piece):
+                off = 0
+                while True:
+                    N.check(self._lib.lo_csv_stream_push(st, C.c_void_p(piece.ctypes.data + off), n - off, int(last),
+                                                         C.byref(win), C.byref(info), C.byref(t)))
+                    add(t)
+                    if win.records:
+                        sums["windows"] += 1
+                        k, nc = int(win.records), int(win.ncols)
+                        offsets = self._staging("csv_offsets", nc * (k + 1) * 8)[:nc * (k + 1) * 8].view(np.int64)
+                        chars = self._staging("csv_chars", win.chars)
+                        N.check(self._lib.lo_csv_stream_columns(st, offsets.ctypes.data_as(C.c_void_p),
+                                                                chars.ctypes.data_as(C.c_void_p), chars.size, C.byref(t)))
+                        add(t, kernel=False)
+                        offsets = offsets.reshape(nc, k + 1)
+                        r0 = 0
+                        if win.first_record == 0:          # record 0: the header
+                            header = [bytes(chars[offsets[c, 0]:offsets[c, 1]]).decode("utf-8") for c in range(nc)]
+                            cols = [_TextBuilder() for _ in range(nc)]
+                            r0 = 1
+                        for c, col in enumerate(cols):
+                            col.append(chars, offsets[c, r0:])
+                    off += win.consumed
+                    if win.done or (off >= n and not last):
+                        break
+                if win.done:
+                    break
+        finally:
+            N.check(self._lib.lo_csv_stream_free(st))
+        if timing is not None:
+            timing.update(sums, peak_device_bytes=int(win.peak_device_bytes))
+        failure = None if info.fail_kind == N.LO_CSV_OK else (int(info.fail_kind), int(info.fail_record), int(info.fail_pos))
+        nrows = max(int(info.records) - 1, 0)
+        columns = [col.array(pa) for col in cols] if header is not None else []
+        return header, nrows, columns, failure
 
     def value_counts_str_packed(self, chars: np.ndarray, offsets: np.ndarray):
         """(rep_rows int64[g], counts uint64[g]) of an already packed text column (offsets[0] == 0)."""

@@ -387,6 +387,9 @@ class ShardedEngine:
     def read_csv_host(self, body, timing=None):
         return self.engines[0].read_csv_host(body, timing)
 
+    def read_csv_stream(self, source, window_bytes=None, timing=None):
+        return self.engines[0].read_csv_stream(source, window_bytes, timing)
+
     def value_counts_str_packed(self, chars, offsets):
         return self.engines[0].value_counts_str_packed(chars, offsets)
 

@@ -1,18 +1,24 @@
 """Device CSV reader (lo_csv_read_host) against pyarrow and the reference's own reader, on bodies generated from a seed.
 
-    python scripts/csv_bench.py [--seed S] [--titanic-mb 1024] [--mnist-mb 256] [--reviews-mb 256] [--out FILE]
+    python scripts/csv_bench.py [--seed S] [--titanic-mb 1024] [--mnist-mb 256] [--reviews-mb 256] [--big-gb N]
+                                [--small-window-mb 16] [--out FILE]
 
 Bodies: Titanic-shaped rows (12 text columns with quoted names), MNIST as CSV (785 integer columns) and review-like
 text (quoted commas, "" pairs, multi-line fields, non-ASCII text).  For each body, in one run: kernel_ms; the whole
 call with pinned and with pageable input and GB/s of body for each; pyarrow.csv.read_csv (its thread count); the oracle
 reader single-threaded on a sample; ingest_csv end to end with and without an engine; a full parity check of the
-columns against the oracle.  The card's name and power limit are printed with the numbers.
+columns against the oracle.  The streaming reader (Engine.read_csv_stream, lo_csv_stream_*) from a file, at the default
+window and at a smaller one: call time, GB/s of body, the peak device bytes it reports and a check that its columns
+equal read_csv_host's; ingest_csv with an engine goes through the stream.  --big-gb N writes a body of N GB to disk,
+records the single-shot reader's LO_ERR_NOMEM on it and streams it (skipped, with the reason, when the host has too
+little RAM for its columns).  The card's name and power limit are printed with the numbers.
 """
 from __future__ import annotations
 
 import argparse
 import io
 import json
+import shutil
 import subprocess
 import sys
 import tempfile
@@ -78,12 +84,82 @@ def timed(fn, reps=3):
     return best, out
 
 
+def same_columns(stream_cols, chars, offsets, first=1):
+    """The stream's Arrow columns == read_csv_host's chars / offsets (data rows from record `first`)."""
+    for c, col in enumerate(stream_cols):
+        off = np.frombuffer(col.buffers()[1], np.int64, count=len(col) + 1, offset=col.offset * 8)
+        data = np.frombuffer(col.buffers()[2], np.uint8, count=int(off[-1]))
+        ref = offsets[c, first:]
+        if len(col) != ref.size - 1 or not np.array_equal(off - off[0], ref - ref[0]):
+            return False
+        if not np.array_equal(data[off[0]:off[-1]], chars[ref[0]:ref[-1]]):
+            return False
+    return True
+
+
+def stream_numbers(eng, path, gb, window):
+    t = {}
+    t0 = time.perf_counter()
+    header, nrows, cols, failure = eng.read_csv_stream(str(path), window, t)
+    dt = time.perf_counter() - t0
+    return {"call_ms": dt * 1e3, "GBps": gb / dt, "kernel_ms": t["kernel_ms"], "windows": t["windows"],
+            "peak_device_bytes": t["peak_device_bytes"]}, (header, nrows, cols, failure)
+
+
+def big_body(eng, a, tmp, results):
+    """A body larger than the single-shot reader's ceiling, written to disk in blocks of the reviews body (long text
+    cells, so the host can hold the columns of a body that large) and streamed."""
+    import os
+    from learningorchestra_b200 import _native as N
+    block = reviews_body(a.seed, 64)
+    header_len = block.index(b"\n") + 1
+    rows = block[header_len:]
+    reps = max(1, int(a.big_gb * 1e9) // len(rows))
+    size = header_len + reps * len(rows)
+    r = {"bytes": size}
+    # the columns need about the body's text plus 8 bytes per cell on the host, twice while they grow
+    cells = rows.count(b"\n") * reps * 3
+    need = 2 * (size + 8 * cells)
+    avail = os.sysconf("SC_AVPHYS_PAGES") * os.sysconf("SC_PAGE_SIZE")
+    disk = shutil.disk_usage(tmp).free
+    if need > avail or size > disk:
+        r["skipped"] = (f"host has {avail / 1e9:.1f} GB of free RAM and {disk / 1e9:.1f} GB of disk; the body takes "
+                        f"{size / 1e9:.1f} GB and its columns about {need / 1e9:.1f} GB")
+        print("big", json.dumps(r), flush=True)
+        results["bodies"]["big"] = r
+        return
+    path = Path(tmp) / "big.csv"
+    with open(path, "wb") as f:
+        f.write(block[:header_len])
+        for _ in range(reps):
+            f.write(rows)
+    del block, rows
+    try:
+        body = np.memmap(path, dtype=np.uint8, mode="r")      # the single-shot call checks HBM before reading it
+        t0 = time.perf_counter()
+        try:
+            eng.read_csv_host(body)
+            r["single_shot"] = "ok"
+        except N.LoexecError as e:
+            r["single_shot"] = f"{e} ({(time.perf_counter() - t0) * 1e3:.0f} ms)"
+        del body
+        num, (header, nrows, cols, failure) = stream_numbers(eng, path, size / 1e9, None)
+        r.update(stream=num, rows=nrows, failure=failure)
+        del cols
+    finally:
+        path.unlink()
+    results["bodies"]["big"] = r
+    print("big", json.dumps(r), flush=True)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--seed", type=int, default=20261016)
     ap.add_argument("--titanic-mb", type=int, default=1024)
     ap.add_argument("--mnist-mb", type=int, default=256)
     ap.add_argument("--reviews-mb", type=int, default=256)
+    ap.add_argument("--big-gb", type=float, default=0)
+    ap.add_argument("--small-window-mb", type=int, default=16)
     ap.add_argument("--out")
     a = ap.parse_args()
     import pyarrow as pa
@@ -127,6 +203,15 @@ def main():
         r["oracle_GBps"] = len(sample) / 1e9 / dt
         path = Path(tmp) / f"{name}.csv"
         path.write_bytes(body)
+        stream_ok = True
+        for label, window in (("stream", None), ("stream_small", a.small_window_mb << 20)):
+            eng.read_csv_stream(str(path), window)                       # warm-up: pinned staging, the pool
+            r[label], (sh, sn, scols, sfail) = stream_numbers(eng, path, gb, window)
+            stream_ok = stream_ok and sh == header and sn == nrows and sfail == failure and \
+                same_columns(scols, chars, offsets)
+            del scols
+        r["stream_equals_single_shot"] = bool(stream_ok)
+        # ingest_csv with an engine streams the file (Engine.read_csv_stream)
         for label, e in (("ingest_engine_ms", eng), ("ingest_pyarrow_ms", None)):
             db = ColumnarDatabase()
             t0 = time.perf_counter()
@@ -141,15 +226,17 @@ def main():
         for c in range(len(header)) if ok else ():
             col = [raw[offsets[c, i]:offsets[c, i + 1]].decode() for i in range(1, nrows + 1)]
             ok = ok and col == [row[c] for row in erows]
-        r["parity"] = bool(ok)
+        r["parity"] = bool(ok and stream_ok)
         del erows, pinned
         results["bodies"][name] = r
         print(name, json.dumps(r), flush=True)
+    if a.big_gb:
+        big_body(eng, a, tmp, results)
     eng.close()
     if a.out:
         Path(a.out).parent.mkdir(parents=True, exist_ok=True)
         Path(a.out).write_text(json.dumps(results, indent=1))
-    if not all(b["parity"] for b in results["bodies"].values()):
+    if not all(b.get("parity", True) for b in results["bodies"].values()):
         sys.exit("parity FAILED")
 
 
