@@ -43,7 +43,7 @@
 extern "C" {
 #endif
 
-#define LO_ABI_VERSION 3
+#define LO_ABI_VERSION 4
 
 #define LO_OK                    0
 #define LO_ERR_INVALID          -1   /* bad argument (message says which)              */
@@ -104,9 +104,6 @@ int         lo_init(int device, lo_ctx **out);
 int         lo_shutdown(lo_ctx *ctx);
 int         lo_ctx_device(const lo_ctx *ctx, int *device, int *sm_count, size_t *hbm_bytes);
 int         lo_sync(lo_ctx *ctx, void *stream);
-/* choose how full tiles of the fused kernel are fed: 0 = register-pipelined LDG.E.256 (default), 1 = TMA bulk
- * copies into a shared-memory ring (cp.async.bulk + mbarrier).  Same results; also set by LOEXEC_TMA=1 at lo_init. */
-int         lo_set_tma(lo_ctx *ctx, int enabled);
 /* number of kernels this context has launched since lo_init (bench "gpu_launches") */
 int         lo_launch_count(const lo_ctx *ctx, int64_t *out);
 

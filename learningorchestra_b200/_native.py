@@ -36,7 +36,7 @@ LO_NUM_FLOAT, LO_NUM_INTEGER, LO_NUM_EMPTY, LO_NUM_INVALID, LO_NUM_UNSUPPORTED =
 LO_FORMAT_MAX_CELL = 310
 LO_CSV_OK, LO_CSV_SHORT_ROW, LO_CSV_FIELD_LIMIT, LO_CSV_BAD_UTF8, LO_CSV_NUL, LO_CSV_UNSUPPORTED, LO_CSV_EMPTY = range(7)
 LO_CSV_STREAM_WINDOW = 64 << 20
-LO_ABI_VERSION = 3
+LO_ABI_VERSION = 4
 
 _ERR_NAMES = {
     LO_ERR_INVALID: "LO_ERR_INVALID", LO_ERR_CUDA: "LO_ERR_CUDA", LO_ERR_NOMEM: "LO_ERR_NOMEM",
@@ -84,7 +84,6 @@ SIGNATURES = {
     "lo_shutdown": (C.c_int, [_P]),
     "lo_ctx_device": (C.c_int, [_P, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_size_t)]),
     "lo_sync": (C.c_int, [_P, _P]),
-    "lo_set_tma": (C.c_int, [_P, C.c_int]),
     "lo_launch_count": (C.c_int, [_P, C.POINTER(C.c_int64)]),
     "lo_host_alloc": (C.c_int, [_P, C.c_size_t, C.POINTER(_P)]),
     "lo_host_alloc_flags": (C.c_int, [_P, C.c_size_t, C.c_int32, C.POINTER(_P)]),

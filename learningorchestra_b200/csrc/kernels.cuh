@@ -7,11 +7,10 @@
 //
 // Design (see DESIGN.md §3):
 //   * table = columnar slabs in HBM; a work tile is (projected column j, kTileRows rows), one tile per CTA
-//     (the grid de-phases itself; a persistent variant runs its CTAs in lock step).
+//     (the grid de-phases itself).
 //   * k_project_cast_hist: every thread streams 32-byte vectors (two LDG.E.128 each) of its column slab with
 //     L1::no_allocate / L2::evict_first through a 2 x 5-vector register pipeline, converts, and streams the
-//     result out with st.cs.  k_project_cast_hist_tma is the same tile fed by cp.async.bulk + mbarriers
-//     (opt-in).
+//     result out with st.cs.
 //   * histogram = PRIVATE PER-THREAD BYTE COUNTERS in shared memory, laid out so that thread t only ever
 //     touches bank (t % 32): word w of thread t lives at smem word w*kThreads + t.  Increment = plain
 //     LDS.U8 / IADD / STS.U8 — no bank conflicts, and the cost is independent of the value distribution (a
@@ -52,17 +51,8 @@ constexpr int kHistSmemBytes = (kHistRows * kThreads + 256) * 4;   // 66560 B ->
 
 // software pipeline of the full-tile path: kPfBuf register buffers of kPfBatch 32-byte vectors;
 // kPfBuf-1 batches are always in flight per thread while one is being converted / binned
-#ifndef LO_PF_BATCH
-#define LO_PF_BATCH 5
-#endif
-#ifndef LO_PF_NBUF
-#define LO_PF_NBUF 2
-#endif
-#ifndef LO_MIN_CTAS
-#define LO_MIN_CTAS 2
-#endif
-constexpr int kPfBatch   = LO_PF_BATCH;
-constexpr int kPfBuf     = LO_PF_NBUF;
+constexpr int kPfBatch   = 5;
+constexpr int kPfBuf     = 2;
 constexpr int kPfBatches = kVecPerThread / kPfBatch;
 static_assert(kVecPerThread % kPfBatch == 0 && kPfBatches % kPfBuf == 0, "pipeline shape must tile the 60 vectors");
 
@@ -123,8 +113,7 @@ struct GroupStep {
 // ---------------------------------------------------------------------------------------------
 // sm_90 loads and stores at most 16 bytes per thread.  A thread's four f64 of a CTA-wide block are therefore two pairs:
 // {p[0], p[1]} and {p[half], p[half + 1]} with p = block + 2 * tid and half = 2 * threads, so each instruction of a warp
-// covers 512 contiguous bytes (the layout the TMA kernel reads from its staging ring).  On sm_90 the L2 evict-first
-// priority of 128-bit loads is an L2::cache_hint policy operand.
+// covers 512 contiguous bytes.  On sm_90 the L2 evict-first priority of 128-bit loads is an L2::cache_hint policy operand.
 __device__ __forceinline__ uint64_t l2_evict_first_policy() {
     uint64_t pol;
     asm("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
@@ -307,11 +296,6 @@ __device__ __forceinline__ void bump_edge(uint8_t *priv, float f, const EdgePara
 // ---------------------------------------------------------------------------------------------
 // CTA-wide fold of the private byte histograms -> RED.64 into counts[]
 // ---------------------------------------------------------------------------------------------
-// per-thread form (no barrier): each thread clears exactly the words it will count in
-__device__ __forceinline__ void zero_private_own(uint32_t *smem, int rows) {
-    for (int w = 0; w < rows; ++w) smem[w * kThreads + (threadIdx.x & (kThreads - 1))] = 0u;
-}
-
 // rows x kThreads words, 16 bytes per store; a thread zeroes OTHER threads' counters too, hence the barrier
 __device__ __forceinline__ void zero_private(uint32_t *smem, int rows) {
     uint4 *p = reinterpret_cast<uint4 *>(smem);
@@ -540,7 +524,7 @@ __device__ __forceinline__ void group_finish_column(const GroupStep &G, unsigned
 // grid.x = k * tiles_per_col ; tile index fastest along rows
 // ---------------------------------------------------------------------------------------------
 template <int OUT, bool HIST, bool ALIGNED, bool EDGES>
-__global__ void __launch_bounds__(kThreads, LO_MIN_CTAS)
+__global__ void __launch_bounds__(kThreads, 2)
 k_project_cast_hist(const char *__restrict__ in_base, long long in_pitch,
                     char *__restrict__ out_base, long long out_pitch,
                     long long nrows, unsigned tiles_per_col, unsigned long long *__restrict__ counts,
@@ -782,174 +766,6 @@ k_project_cast_hist_bins(const char *__restrict__ in_base, long long in_pitch, c
         }
     }
     if (G.mode != 0) group_finish_column(G, j, nb, P.k, chunks_per_col, smem);
-}
-
-// ---------------------------------------------------------------------------------------------
-// K1+K2+K3, TMA form (LOEXEC_TMA=1): the same tile, but the column slab is staged into shared memory by the
-// bulk-copy engine (cp.async.bulk global -> shared, completion on an mbarrier) through a kTmaStages-deep ring
-// driven by one producer thread; the 256 consumer threads read their 32 bytes from the ring instead of
-// issuing the 128-bit loads themselves.  Built to answer "would TMA staging beat the register pipeline?" with a
-// measurement (DESIGN.md §3.8); arithmetic, tile shape, private histograms and results are identical.
-// Full, 32-byte-aligned tiles only — the host routes everything else to k_project_cast_hist.
-// ---------------------------------------------------------------------------------------------
-constexpr int kTmaStages     = 5;
-constexpr int kTmaStageBytes = kThreads * kVec * 8;                    // 8 KiB = one 32-byte vector per consumer
-constexpr int kTmaRounds     = kVecPerThread;                          // 60 rounds per tile
-constexpr int kTmaSmemBytes  = kHistSmemBytes + kTmaStages * kTmaStageBytes + 2 * kTmaStages * 8;
-
-__device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" :: "r"(bar), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" :: "r"(bar) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "LO_WAIT_%=:\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
-        "@p bra LO_DONE_%=;\n\t"
-        "bra LO_WAIT_%=;\n\t"
-        "LO_DONE_%=:\n\t}"
-        :: "r"(bar), "r"(parity) : "memory");
-}
-__device__ __forceinline__ void tma_load_1d(uint32_t dst_smem, const void *src_gmem, uint32_t bytes, uint32_t bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                 :: "r"(dst_smem), "l"(src_gmem), "r"(bytes), "r"(bar) : "memory");
-}
-
-template <int OUT, bool HIST, bool FASTDIV>
-__global__ void __launch_bounds__(kThreads + 32, 2)
-k_project_cast_hist_tma(const char *__restrict__ in_base, long long in_pitch,
-                        char *__restrict__ out_base, long long out_pitch,
-                        long long nrows, unsigned tiles_per_col,
-                        unsigned long long *__restrict__ counts,
-                        const __grid_constant__ ColsF64 P) {
-    extern __shared__ uint32_t smem[];
-    uint8_t *ring = reinterpret_cast<uint8_t *>(smem) + kHistSmemBytes;                 // kTmaStages x 8 KiB
-    const uint32_t bar_full  = smem_u32(ring + kTmaStages * kTmaStageBytes);            // kTmaStages x 8 B
-    const uint32_t bar_empty = bar_full + kTmaStages * 8;
-    const unsigned j    = blockIdx.x / tiles_per_col;
-    const unsigned tile = blockIdx.x - j * tiles_per_col;
-    const long long r0  = (long long)tile * kTileRows;            // host guarantees a full tile
-    const double *in = reinterpret_cast<const double *>(in_base + (long long)P.col[j] * in_pitch) + r0;
-
-    if (threadIdx.x == 0) {
-        for (int s = 0; s < kTmaStages; ++s) {
-            mbar_init(bar_full + 8 * s, 1);                    // the producer's expect_tx arrival
-            mbar_init(bar_empty + 8 * s, kThreads / 32);       // one arrival per consumer warp
-        }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    const bool producer = threadIdx.x >= kThreads;
-    BinParams B = {0.f, 0.f, 1.f, 1.f, 0};
-    int rows = 0;
-    uint8_t *priv = reinterpret_cast<uint8_t *>(smem) + 4 * (threadIdx.x & (kThreads - 1));
-    if (HIST && !producer) {
-        B.lo = P.lo[j]; B.hi = P.hi[j]; B.w = P.w[j];
-        B.r = __frcp_rn(B.w);
-        B.last = P.nbins - 1;
-        rows = (P.nbins + 3) >> 2;
-        zero_private_own(smem, rows);
-    }
-    __syncthreads();
-
-    if (producer) {
-        if (threadIdx.x == kThreads) {                          // one elected thread drives the copy engine
-#pragma unroll 1
-            for (int r = 0; r < kTmaRounds; ++r) {
-                const int s = r % kTmaStages;
-                const uint32_t phase = (uint32_t)(r / kTmaStages) & 1u;
-                mbar_wait(bar_empty + 8 * s, phase ^ 1u);       // slot free (passes at once on the first lap)
-                mbar_expect_tx(bar_full + 8 * s, kTmaStageBytes);
-                tma_load_1d(smem_u32(ring + s * kTmaStageBytes), in + (long long)r * (kThreads * kVec), kTmaStageBytes,
-                            bar_full + 8 * s);
-            }
-        }
-    } else {
-        float  *out32 = (OUT == 1) ? reinterpret_cast<float *>(out_base + (long long)j * out_pitch) + r0 : nullptr;
-        double *out64 = (OUT == 2) ? reinterpret_cast<double *>(out_base + (long long)j * out_pitch) + r0 : nullptr;
-        const int lane = threadIdx.x & 31;
-#ifndef LO_TMA_UNROLL
-#define LO_TMA_UNROLL 1
-#endif
-        static_assert(kTmaRounds % LO_TMA_UNROLL == 0, "rounds per tile must be a multiple of the unroll");
-#pragma unroll 1
-        for (int r0u = 0; r0u < kTmaRounds; r0u += LO_TMA_UNROLL) {
-            double2 a[LO_TMA_UNROLL], b[LO_TMA_UNROLL];
-            // take LO_TMA_UNROLL stages at once: all their shared-memory reads are in flight together, the slots go
-            // back to the copy engine before any arithmetic starts
-#pragma unroll
-            for (int u = 0; u < LO_TMA_UNROLL; ++u) {
-                const int r = r0u + u, s = r % kTmaStages;
-                mbar_wait(bar_full + 8 * s, (uint32_t)(r / kTmaStages) & 1u);
-                // 16-byte accesses at 16-byte lane stride are bank-conflict free: a thread takes doubles
-                // {2t, 2t+1} from the first half of the stage and {512+2t, 513+2t} from the second half
-                a[u] = *reinterpret_cast<const double2 *>(ring + s * kTmaStageBytes + threadIdx.x * 16);
-                b[u] = *reinterpret_cast<const double2 *>(ring + s * kTmaStageBytes + kTmaStageBytes / 2 + threadIdx.x * 16);
-            }
-            __syncwarp();
-            if (lane == 0) {
-#pragma unroll
-                for (int u = 0; u < LO_TMA_UNROLL; ++u) mbar_arrive(bar_empty + 8 * ((r0u + u) % kTmaStages));
-            }
-#pragma unroll
-            for (int u = 0; u < LO_TMA_UNROLL; ++u) {
-                const long long e = (long long)(r0u + u) * (kThreads * kVec) + 2 * threadIdx.x;
-                const float f0 = cast_f64_f32(a[u].x), f1 = cast_f64_f32(a[u].y), f2 = cast_f64_f32(b[u].x), f3 = cast_f64_f32(b[u].y);
-                if (OUT == 1) {
-                    asm volatile("st.global.cs.v2.f32 [%0], {%1,%2};" :: "l"(out32 + e), "f"(f0), "f"(f1) : "memory");
-                    asm volatile("st.global.cs.v2.f32 [%0], {%1,%2};" :: "l"(out32 + e + 512), "f"(f2), "f"(f3) : "memory");
-                }
-                if (OUT == 2) {
-                    asm volatile("st.global.cs.v2.f64 [%0], {%1,%2};" :: "l"(out64 + e), "d"(a[u].x), "d"(a[u].y) : "memory");
-                    asm volatile("st.global.cs.v2.f64 [%0], {%1,%2};" :: "l"(out64 + e + 512), "d"(b[u].x), "d"(b[u].y) : "memory");
-                }
-                if (HIST)
-                    bump4(priv, bin_index_f32<FASTDIV>(f0, B), bin_index_f32<FASTDIV>(f1, B),
-                          bin_index_f32<FASTDIV>(f2, B), bin_index_f32<FASTDIV>(f3, B));
-            }
-        }
-    }
-    if (HIST) {
-        // fold_and_flush is written for exactly kThreads threads; the producer warp only joins its barriers
-        uint32_t *folded = smem + kHistRows * kThreads;
-        const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-        __syncthreads();
-        if (!producer) {
-            for (int w = warp; w < rows; w += kThreads / 32) {
-                const uint32_t *row = smem + w * kThreads;
-                uint32_t even = 0, odd = 0;
-#pragma unroll
-                for (int i = 0; i < kThreads / 32; ++i) {
-                    uint32_t x = row[lane + 32 * i];
-                    even += x & 0x00FF00FFu;
-                    odd  += (x >> 8) & 0x00FF00FFu;
-                }
-#pragma unroll
-                for (int sft = 16; sft > 0; sft >>= 1) {
-                    even += __shfl_xor_sync(0xffffffffu, even, sft);
-                    odd  += __shfl_xor_sync(0xffffffffu, odd, sft);
-                }
-                if (lane == 0) {
-                    folded[4 * w + 0] = even & 0xFFFFu;
-                    folded[4 * w + 1] = odd & 0xFFFFu;
-                    folded[4 * w + 2] = even >> 16;
-                    folded[4 * w + 3] = odd >> 16;
-                }
-            }
-        }
-        __syncthreads();
-        if ((int)threadIdx.x < P.nbins) {
-            const uint32_t c = folded[threadIdx.x];
-            unsigned long long *dst = counts + (long long)j * P.nbins + threadIdx.x;
-            if (c) atomicAdd(dst, (unsigned long long)c);
-        }
-    }
 }
 
 // ---------------------------------------------------------------------------------------------

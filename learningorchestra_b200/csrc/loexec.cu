@@ -114,7 +114,6 @@ struct lo_ctx {
     size_t       hbm_bytes;
     cudaStream_t stream;       // default stream for NULL `stream` arguments
     std::atomic<int64_t> launches{0};
-    std::atomic<bool> use_tma{false};   // LOEXEC_TMA=1 or lo_set_tma(): stage slabs through smem with cp.async.bulk
     // *_host pipelines: each call borrows a StageSet (its own three streams, staging slots, events, count scratch)
     // from this pool, so concurrent calls on one context — the REST services run a thread per job — overlap instead
     // of queueing; at most kMaxStageSets exist, further callers wait for one to come back
@@ -351,18 +350,7 @@ int edge_used(EdgeTable *t, cudaStream_t s) {
     return LO_OK;
 }
 
-template <typename K>
-int allow_smem_tma(K kernel) {
-    LO_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, lo::kTmaSmemBytes));
-    return LO_OK;
-}
-
 int configure_kernels() {
-    LO_TRY(allow_smem_tma(lo::k_project_cast_hist_tma<0, true, true>));
-    LO_TRY(allow_smem_tma(lo::k_project_cast_hist_tma<1, true, true>));
-    LO_TRY(allow_smem_tma(lo::k_project_cast_hist_tma<2, true, true>));
-    LO_TRY(allow_smem_tma(lo::k_project_cast_hist_tma<1, false, false>));
-    LO_TRY(allow_smem_tma(lo::k_project_cast_hist_tma<2, false, false>));
     LO_TRY(allow_smem_hist<0>());
     LO_TRY(allow_smem_hist<1>());
     LO_TRY(allow_smem_hist<2>());
@@ -416,30 +404,6 @@ int launch_f64(lo_ctx *ctx, const lo_table *in, const lo_table *out, int32_t out
     const size_t smem = !HIST ? 0 : edges ? lo::kEdgeSmemBytes : lo::kHistSmemBytes;
     char *out_base = out ? out->base + (int64_t)out_col0 * out->pitch : nullptr;
     const long long out_pitch = out ? out->pitch : 0;
-    bool fast = HIST;     // the TMA kernel's divide
-    for (int j = 0; HIST && j < P.k; ++j) fast = fast && fastdiv_ok(P.w[j]);
-    // LOEXEC_TMA=1: stage the slabs through shared memory with the bulk-copy engine (A/B variant, DESIGN §3.8).
-    // Only full tiles; the ragged last tile of each column (and unaligned / slow-divide / group cases) keep the LDG kernel.
-    if (ctx->use_tma.load(std::memory_order_relaxed) && aligned && fast == HIST && in->nrows >= lo::kTileRows && G.mode == 0) {
-        const unsigned full_tiles = (unsigned)(in->nrows / lo::kTileRows);
-        const unsigned long long tblocks = (unsigned long long)full_tiles * (unsigned)P.k;
-        if (tblocks > 0x7fffffffull) return fail(LO_ERR_INVALID, "table too large for one launch (%llu tiles)", tblocks);
-        lo::k_project_cast_hist_tma<OUT, HIST, HIST><<<(unsigned)tblocks, lo::kThreads + 32, lo::kTmaSmemBytes, s>>>(
-            in->base, in->pitch, out_base, out_pitch, in->nrows, full_tiles, counts, P);
-        LO_CUDA(launched(ctx, 1));
-        const int64_t done = (int64_t)full_tiles * lo::kTileRows;
-        if (done == in->nrows) return LO_OK;
-        // the remaining rows of every column: one ragged tile each, through the regular kernel on a row-offset view
-        const char *ib = in->base + done * 8;
-        char *ob = out ? out->base + done * (int64_t)dtype_size(out->dtype) + (int64_t)out_col0 * out->pitch : nullptr;
-        if (edges) lo::k_project_cast_hist<OUT, HIST, true, true><<<(unsigned)P.k, lo::kThreads, smem, s>>>(
-                       ib, in->pitch, ob, out_pitch, in->nrows - done, 1u, counts, edges, P, kNoGroup);
-        else       lo::k_project_cast_hist<OUT, HIST, true, false><<<(unsigned)P.k, lo::kThreads, smem, s>>>(
-                       ib, in->pitch, ob, out_pitch, in->nrows - done, 1u, counts, edges, P, kNoGroup);
-        LO_CUDA(launched(ctx, 1));
-        if (et) LO_TRY(edge_used(et, s));
-        return LO_OK;
-    }
     // one tile (kTileRows rows of one projected column) per CTA.  A tapered tail — the last wave cut into short
     // tiles — was built and was not faster, and a runtime tile shape slows the uniform case, so tiles are compile-time
     // uniform.
@@ -859,7 +823,6 @@ int lo_init(int device, lo_ctx **out) {
         LO_CUDA(cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &keep));
         return configure_kernels();
     };
-    if (const char *e = getenv("LOEXEC_TMA")) ctx->use_tma.store(e[0] == '1');
     const int rc = setup();
     if (rc != LO_OK) {              // keep the error message, release whatever was created
         const std::string msg = g_err;
@@ -899,12 +862,6 @@ int lo_ctx_device(const lo_ctx *ctx, int *device, int *sm_count, size_t *hbm_byt
 int lo_sync(lo_ctx *ctx, void *stream) {
     LO_TRY(check_ctx(ctx));
     LO_CUDA(cudaStreamSynchronize(pick(ctx, stream)));
-    return LO_OK;
-}
-
-int lo_set_tma(lo_ctx *ctx, int enabled) {
-    if (!ctx) return fail(LO_ERR_INVALID, "ctx is NULL");
-    ctx->use_tma.store(enabled != 0, std::memory_order_relaxed);
     return LO_OK;
 }
 

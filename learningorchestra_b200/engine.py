@@ -311,10 +311,6 @@ class Engine:
     def __exit__(self, *exc):
         self.close()
 
-    def set_tma(self, enabled: bool) -> None:
-        """Feed full tiles of the fused kernel through the TMA-staged variant (same results; DESIGN.md §3.8)."""
-        N.check(self._lib.lo_set_tma(self._ctx, 1 if enabled else 0))
-
     def sync(self, stream=None) -> None:
         N.check(self._lib.lo_sync(self._ctx, _stream_ptr(stream)))
 

@@ -2,7 +2,7 @@
 # compute-sanitizer over the parity subset and the single-rank group path (memcheck, then racecheck on the
 # private-histogram / fold / merge kernels).  Writes gpurun_out/sanitizer_{memcheck,racecheck}.txt
 mkdir -p gpurun_out
-SEL='ragged_sizes or nbins or special_values or constant_column or histogram_only or hist_u8 or unaligned or empty_inputs or tma_staged or memory_arrangement'
+SEL='ragged_sizes or nbins or special_values or constant_column or histogram_only or hist_u8 or unaligned or empty_inputs or memory_arrangement'
 timeout 900 compute-sanitizer --tool memcheck --error-exitcode 1 python -m pytest tests/test_gpu_parity.py -q -k "$SEL" \
     tests/test_gpu_group.py::test_rank_group_one_rank_per_step_launch_count > gpurun_out/sanitizer_memcheck.txt 2>&1
 echo "memcheck rc=$?"; tail -3 gpurun_out/sanitizer_memcheck.txt

@@ -37,7 +37,6 @@ def test_library_is_sm90a_native_code(built):
     assert "STS.U8" in sass and "LDS.U8" in sass                # private byte-counter histogram, no ATOMS
     assert "ATOMS" not in sass
     assert "RED.E.ADD.64.STRONG.SYS" in sass or "REDG.E.ADD.64.STRONG.SYS" in sass    # in-kernel merge: pushes at system scope
-    assert "MUFU.RCP" not in sass.split("BAR.SYNC")[0] or True
 
 
 def test_lane_slot_kernels_issue_one_shared_atomic_per_element(built):
@@ -54,14 +53,6 @@ def test_lane_slot_kernels_issue_one_shared_atomic_per_element(built):
     assert "REDG.E.ADD.64.STRONG.GPU" in lanes or "RED.E.ADD.64.STRONG.GPU" in lanes
     bins = sass.split("Function : _ZN2lo24k_project_cast_hist_binsILi1ELb1EEE")[1].split("Function :")[0]
     assert "ATOMS" in bins and "F2F.F32.F64" in bins and "LDG.E.NA.128" in bins
-
-
-def test_tma_variant_is_compiled_with_bulk_copy_and_mbarriers(built):
-    """The opt-in TMA-staged kernel really uses the bulk-copy engine: UBLKCP (cp.async.bulk) + SYNCS (mbarrier) in SASS."""
-    from learningorchestra_b200 import _native
-    sass = subprocess.run(["cuobjdump", "-sass", str(_native.LIB_PATH)], capture_output=True, text=True).stdout
-    block = sass.split("k_project_cast_hist_tmaILi1ELb1ELb1E")[1].split("Function :")[0]
-    assert "UBLKCP" in block and "SYNCS" in block and "LDS.128" in block
 
 
 def test_no_gpu_means_loud_failure_not_fallback(built):

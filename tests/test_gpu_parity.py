@@ -385,21 +385,6 @@ def test_plain_c_consumer_runs_the_hot_path(engine, tmp_path):
     assert out.returncode == 0 and "abi_smoke ok" in out.stdout, out.stderr
 
 
-def test_tma_staged_variant_has_the_same_results(engine):
-    """LOEXEC_TMA=1 routes full tiles through the cp.async.bulk + mbarrier ring kernel (DESIGN.md §3.8); the switch
-    is read once per process, so the parity subset is re-run in a child process with it set."""
-    import os
-    import subprocess
-    import sys
-    env = dict(os.environ, LOEXEC_TMA="1")
-    out = subprocess.run([sys.executable, "-m", "pytest", __file__, "-m", "gpu", "-q", "-x", "-k",
-                          "ragged_sizes or test_nbins or special_values or constant_column or histogram_only or "
-                          "projection_cast_only or accumulate or host_buffer"],
-                         capture_output=True, text=True, timeout=600, env=env)
-    assert out.returncode == 0, out.stdout[-2000:] + out.stderr[-2000:]
-    assert " passed" in out.stdout
-
-
 def test_more_projected_columns_than_one_launch_holds(engine):
     """k > 128 (f64) and k > 1024 (u8) are split over several launches; counts / outputs line up per column."""
     table = bn.synth_table_f64(1, SEED + 21, 7, 0, 70_000)
