@@ -43,7 +43,7 @@
 extern "C" {
 #endif
 
-#define LO_ABI_VERSION 4
+#define LO_ABI_VERSION 5
 
 #define LO_OK                    0
 #define LO_ERR_INVALID          -1   /* bad argument (message says which)              */
@@ -315,6 +315,34 @@ int lo_value_counts_str_host(lo_ctx *ctx, const uint8_t *chars, const int64_t *o
 #define LO_NUM_UNSUPPORTED 4
 int lo_parse_number_host(lo_ctx *ctx, const uint8_t *chars, const int64_t *offsets, int64_t n,
                          double *values, uint8_t *status, lo_host_timing *timing);
+
+/* The same parse written straight into a device table: cell i (i < n) goes to row row0 + i of column `col` of `out`
+ * (LO_F64) as the bits float() returns; a null cell and "" store the canonical NaN (0x7ff8000000000000), which the
+ * histogram and min/max kernels skip.  chars / offsets are host buffers laid out as for lo_parse_number_host; offsets[0]
+ * need not be 0 (a sliced Arrow array), only chars[offsets[0] .. offsets[n]) is copied.  A cell whose offsets leave that
+ * range counts as unsupported.  validity: NULL (every cell present), or one of
+ *   mask   — n host bytes, 0 = cell i is null;
+ *   bitmap — an Arrow validity bitmap, bit (bit_offset + i), least significant bit first, 0 = cell i is null
+ * (Arrow does not promise that a null slot is empty: its bytes are never parsed).  Instead of a status per row the call
+ * fills *summary: the first invalid row (float() raises ValueError) and the first unsupported row (cell over 1 MiB or a
+ * byte >= 0x80), -1 when there is none, relative to the call's first cell; the null + empty cells; and whether every
+ * other cell is integer valued (the resident column's "int" kind).  Rows of invalid / unsupported cells hold
+ * unspecified values: the caller fails the request. */
+typedef struct lo_validity {
+    const uint8_t *mask;
+    const uint8_t *bitmap;
+    int64_t bit_offset;
+} lo_validity;
+typedef struct lo_parse_summary {
+    int64_t first_invalid;
+    int64_t first_unsupported;
+    int64_t nulls;
+    int32_t all_integer;
+    int32_t pad;
+} lo_parse_summary;
+int lo_parse_number_to_table(lo_ctx *ctx, const uint8_t *chars, const int64_t *offsets, const lo_validity *validity,
+                             int64_t n, lo_table *out, int32_t col, int64_t row0, lo_parse_summary *summary,
+                             lo_host_timing *timing);
 
 /* Number -> text for one column: the reference's "string" cast, str(v) / None -> "" (data_type_handler_image/
  * data_type_update.py:22-28), for every cell at once on the GPU.  The inverse of lo_parse_number_host.

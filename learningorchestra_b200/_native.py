@@ -36,7 +36,7 @@ LO_NUM_FLOAT, LO_NUM_INTEGER, LO_NUM_EMPTY, LO_NUM_INVALID, LO_NUM_UNSUPPORTED =
 LO_FORMAT_MAX_CELL = 310
 LO_CSV_OK, LO_CSV_SHORT_ROW, LO_CSV_FIELD_LIMIT, LO_CSV_BAD_UTF8, LO_CSV_NUL, LO_CSV_UNSUPPORTED, LO_CSV_EMPTY = range(7)
 LO_CSV_STREAM_WINDOW = 64 << 20
-LO_ABI_VERSION = 4
+LO_ABI_VERSION = 5
 
 _ERR_NAMES = {
     LO_ERR_INVALID: "LO_ERR_INVALID", LO_ERR_CUDA: "LO_ERR_CUDA", LO_ERR_NOMEM: "LO_ERR_NOMEM",
@@ -62,6 +62,15 @@ class HistSpec(C.Structure):
 class HostTiming(C.Structure):
     _fields_ = [("total_ms", C.c_double), ("h2d_bytes", C.c_double), ("d2h_bytes", C.c_double),
                 ("launches", C.c_int64), ("kernel_ms", C.c_double)]
+
+
+class Validity(C.Structure):
+    _fields_ = [("mask", C.c_void_p), ("bitmap", C.c_void_p), ("bit_offset", C.c_int64)]
+
+
+class ParseSummary(C.Structure):
+    _fields_ = [("first_invalid", C.c_int64), ("first_unsupported", C.c_int64), ("nulls", C.c_int64),
+                ("all_integer", C.c_int32), ("pad", C.c_int32)]
 
 
 class CsvInfo(C.Structure):
@@ -135,6 +144,8 @@ SIGNATURES = {
     "lo_value_counts_f64_host": (C.c_int, [_P, _P, C.c_int64, _P, _P, C.c_int64, C.POINTER(C.c_int64), C.POINTER(HostTiming)]),
     "lo_value_counts_str_host": (C.c_int, [_P, _P, _P, C.c_int64, _P, _P, C.c_int64, C.POINTER(C.c_int64), C.POINTER(HostTiming)]),
     "lo_parse_number_host": (C.c_int, [_P, _P, _P, C.c_int64, _P, _P, C.POINTER(HostTiming)]),
+    "lo_parse_number_to_table": (C.c_int, [_P, _P, _P, C.POINTER(Validity), C.c_int64, _P, C.c_int32, C.c_int64,
+                                           C.POINTER(ParseSummary), C.POINTER(HostTiming)]),
     "lo_format_number_host": (C.c_int, [_P, _P, _P, C.c_int64, _P, _P, C.c_int64, C.POINTER(HostTiming)]),
     "lo_minmax_cast_host": (C.c_int, [_P, C.POINTER(_P), C.c_int64, C.c_int32, _P, _P, _P, C.POINTER(HostTiming)]),
     "lo_csv_read_host": (C.c_int, [_P, _P, C.c_int64, C.POINTER(_P), C.POINTER(CsvInfo), C.POINTER(HostTiming)]),

@@ -190,22 +190,59 @@ def ascii_number_text(cell: str) -> str:
     return "".join(out)
 
 
+def number_text(cells):
+    """The text the number parser reads: an Arrow ``large_string`` array of ``cells`` (an Arrow string array, or a list
+    of ``str`` / None) in which every cell with a non-ASCII character is :func:`ascii_number_text` of it (rare; found
+    with one vectorised Arrow pass); nulls stay null.  An Arrow array that is all ASCII comes back as it is, same
+    buffers.  Both ``/fieldTypes "number"`` and the text route of binned / cast requests use this one rule."""
+    import pyarrow as pa
+    import pyarrow.compute as pc
+    arr = cells if isinstance(cells, (pa.Array, pa.ChunkedArray)) else pa.array(cells, type=pa.large_string())
+    if isinstance(arr, pa.ChunkedArray):
+        arr = arr.combine_chunks() if arr.num_chunks != 1 else arr.chunk(0)
+    if not pa.types.is_large_string(arr.type):
+        arr = arr.cast(pa.large_string())
+    bad = pc.invert(pc.string_is_ascii(arr)).fill_null(False)
+    if not pc.any(bad).as_py():
+        return arr
+    values = arr.to_pylist()
+    for i in np.flatnonzero(np.asarray(bad.to_numpy(zero_copy_only=False), dtype=bool)):
+        values[i] = ascii_number_text(values[i])
+    return pa.array(values, type=pa.large_string())
+
+
+def text_buffers(arr):
+    """(chars uint8, offsets int64[n+1], validity) of an Arrow ``large_string`` array: views of its buffers, no copy.
+    The offsets are the array's own (offsets[0] != 0 for a slice; cell i is chars[offsets[i]:offsets[i + 1]]);
+    validity is None without nulls, else ``(bitmap uint8, bit_offset)`` — Arrow's validity bitmap and the first cell's
+    bit in it."""
+    n = len(arr)
+    bufs = arr.buffers()
+    offsets = np.frombuffer(bufs[1], dtype=np.int64, count=n + 1 + arr.offset)[arr.offset:] if n else np.zeros(1, np.int64)
+    chars = np.frombuffer(bufs[2], dtype=np.uint8) if bufs[2] is not None and bufs[2].size else np.zeros(1, dtype=np.uint8)
+    validity = (np.frombuffer(bufs[0], dtype=np.uint8), arr.offset) if arr.null_count and bufs[0] is not None else None
+    return chars, offsets, validity
+
+
+def number_text_valid(arr) -> np.ndarray:
+    """bool per cell of an Arrow text array: the cell holds a number after ``float()`` — neither null nor ``""``
+    (``data_type_update.py:37-38`` stores None for both)."""
+    import pyarrow.compute as pc
+    present = pc.greater(pc.binary_length(arr), 0).fill_null(False)
+    return np.asarray(present.to_numpy(zero_copy_only=False), dtype=bool)
+
+
 def pack_number_cells(cells):
-    """:func:`pack_cells` for the number parser: ``str`` cells with non-ASCII characters are normalised first
-    (rare; found with one vectorised Arrow pass)."""
+    """:func:`pack_cells` for the number parser: ``str`` cells go through :func:`number_text` first."""
     if cells and isinstance(cells[0], str):
         try:
-            import pyarrow as pa
-            import pyarrow.compute as pc
-            arr = pa.array(cells, type=pa.large_string())
-            bad = pc.invert(pc.string_is_ascii(arr))
-            if pc.any(bad).as_py():
-                idx = np.flatnonzero(np.asarray(bad.to_numpy(zero_copy_only=False), dtype=bool))
-                cells = list(cells)
-                for i in idx:
-                    cells[i] = ascii_number_text(cells[i])
+            arr = number_text(cells)
         except (ImportError, TypeError, ValueError) as _exc:      # mixed str / bytes columns: cell by cell
             cells = [ascii_number_text(c) if isinstance(c, str) else c for c in cells]
+        else:
+            if not arr.null_count:
+                return text_buffers(arr)[:2]
+            cells = arr.to_pylist()
     return pack_cells(cells)
 
 

@@ -1239,6 +1239,55 @@ __global__ void k_parse_number(const uint8_t *__restrict__ chars, const long lon
     }
 }
 
+// The same parse written straight into one f64 table column (a text field binned or cast without /fieldTypes): cell i
+// is chars[offsets[i] - offsets[0] ..) — the offsets of a sliced Arrow array are rebased here — and lands in col[i] as
+// the bits float() returns; a null cell (mask byte 0, or bitmap bit (bit0 + i) clear) and "" store the canonical NaN.
+// Instead of a status per row the call reduces summary[4] = {first invalid row, first unsupported row (both start at
+// ~0, atomicMin), null + empty cells, cells that are valid but not integer valued} per warp, then one atomic each.
+__device__ __forceinline__ unsigned long long warp_min_u64(unsigned long long v) {
+#pragma unroll
+    for (int s = 16; s > 0; s >>= 1) v = min(v, __shfl_xor_sync(0xffffffffu, v, s));
+    return v;
+}
+
+__global__ void __launch_bounds__(128) k_parse_number_to_col(const uint8_t *__restrict__ chars, const long long *__restrict__ offsets,
+                                                             long long n, const uint8_t *__restrict__ mask,
+                                                             const uint8_t *__restrict__ bitmap, int bit0,
+                                                             unsigned long long *__restrict__ col,
+                                                             unsigned long long *__restrict__ summary) {
+    const long long base = offsets[0], total = offsets[n] - base;
+    unsigned long long first_invalid = ~0ull, first_unsupported = ~0ull;
+    unsigned nulls = 0, non_integer = 0;
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+        const long long b = offsets[i] - base, len = offsets[i + 1] - offsets[i];
+        const bool present = mask ? mask[i] != 0 : bitmap ? ((bitmap[(bit0 + i) >> 3] >> ((bit0 + i) & 7)) & 1) != 0 : true;
+        uint64_t bits = 0x7FF8000000000000ull;
+        uint8_t st = num::kEmpty;
+        if (present)      // a cell outside [offsets[0], offsets[n]) (malformed offsets) is never read: unsupported
+            st = (b < 0 || len < 0 || b + len > total || len > num::kMaxLen) ? (uint8_t)num::kUnsupported
+                                                                             : num::parse_number(chars + b, (int)len, bits);
+        if (st == num::kEmpty) bits = 0x7FF8000000000000ull;
+        col[i] = bits;
+        nulls += st == num::kEmpty;
+        non_integer += st != num::kInteger && st != num::kEmpty;
+        if (st == num::kInvalid) first_invalid = min(first_invalid, (unsigned long long)i);
+        if (st == num::kUnsupported) first_unsupported = min(first_unsupported, (unsigned long long)i);
+    }
+    first_invalid = warp_min_u64(first_invalid);
+    first_unsupported = warp_min_u64(first_unsupported);
+#pragma unroll
+    for (int s = 16; s > 0; s >>= 1) {
+        nulls += __shfl_xor_sync(0xffffffffu, nulls, s);
+        non_integer += __shfl_xor_sync(0xffffffffu, non_integer, s);
+    }
+    if ((threadIdx.x & 31) == 0) {
+        if (first_invalid != ~0ull) atomicMin(summary + 0, first_invalid);
+        if (first_unsupported != ~0ull) atomicMin(summary + 1, first_unsupported);
+        if (nulls) atomicAdd(summary + 2, (unsigned long long)nulls);
+        if (non_integer) atomicAdd(summary + 3, (unsigned long long)non_integer);
+    }
+}
+
 // R-semantics cast "string" (data_type_update.py:22-28): str(v) / None -> "" of one cell per thread
 // (format_number.cuh).  Pass 1 writes each cell's length (the input of the offsets scan) and the first row whose status
 // or value cannot be formatted; pass 2 writes each cell's text at its scanned offset.  Both run the same format_cell.

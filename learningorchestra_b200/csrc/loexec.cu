@@ -1509,6 +1509,63 @@ int lo_parse_number_host(lo_ctx *ctx, const uint8_t *chars, const int64_t *offse
     return c.finish(timing);
 }
 
+// text -> number straight into rows [row0, row0 + n) of one f64 table column: the same parse, no per-row status; the
+// call's summary instead (first invalid / unsupported row, null + empty cells, all valid cells integer valued).
+int lo_parse_number_to_table(lo_ctx *ctx, const uint8_t *chars, const int64_t *offsets, const lo_validity *validity,
+                             int64_t n, lo_table *out, int32_t col, int64_t row0, lo_parse_summary *summary,
+                             lo_host_timing *timing) {
+    LO_TRY(check_ctx(ctx));
+    if (!summary) return fail(LO_ERR_INVALID, "summary is NULL");
+    *summary = lo_parse_summary{-1, -1, 0, 1, 0};
+    if (!out || out->dtype != LO_F64) return fail(LO_ERR_INVALID, "output table must be LO_F64");
+    LO_TRY(check_range(out, col, row0, n));
+    if (n == 0) return LO_OK;
+    if (!offsets) return fail(LO_ERR_INVALID, "offsets is NULL");
+    const int64_t nbytes = offsets[n] - offsets[0];
+    if (nbytes < 0 || (nbytes > 0 && !chars)) return fail(LO_ERR_INVALID, "bad offsets / chars");
+    if (validity && validity->mask && validity->bitmap) return fail(LO_ERR_INVALID, "validity: mask or bitmap, not both");
+    if (validity && validity->bitmap && validity->bit_offset < 0) return fail(LO_ERR_INVALID, "validity: bit_offset < 0");
+    HostCall c(ctx, "parse_number_to_table");
+    uint8_t *d_chars = nullptr, *d_valid = nullptr;
+    long long *d_off = nullptr;
+    unsigned long long *d_sum = nullptr;
+    c.alloc(&d_chars, (size_t)nbytes);
+    c.alloc(&d_off, (size_t)(n + 1) * 8);
+    c.alloc(&d_sum, 4 * 8);
+    c.to_dev(d_chars, chars + offsets[0], (size_t)nbytes);
+    c.to_dev(d_off, offsets, (size_t)(n + 1) * 8);
+    const uint8_t *d_mask = nullptr, *d_bitmap = nullptr;
+    int bit0 = 0;
+    if (validity && validity->mask) {
+        c.alloc(&d_valid, (size_t)n);
+        c.to_dev(d_valid, validity->mask, (size_t)n);
+        d_mask = d_valid;
+    } else if (validity && validity->bitmap) {
+        const int64_t first = validity->bit_offset >> 3, last = (validity->bit_offset + n - 1) >> 3;
+        c.alloc(&d_valid, (size_t)(last - first + 1));
+        c.to_dev(d_valid, validity->bitmap + first, (size_t)(last - first + 1));
+        d_bitmap = d_valid;
+        bit0 = (int)(validity->bit_offset & 7);
+    }
+    c.memset(d_sum, 0xFF, 2 * 8);
+    c.memset(d_sum + 2, 0, 2 * 8);
+    unsigned long long *dst = (unsigned long long *)(out->base + (int64_t)col * out->pitch) + row0;
+    c.mark();
+    c.launch(1, [&] {
+        const int grid = (int)std::min<int64_t>((n + 127) / 128, (int64_t)ctx->sm_count * 16);
+        lo::k_parse_number_to_col<<<grid, 128, 0, c.s>>>(d_chars, d_off, n, d_mask, d_bitmap, bit0, dst, d_sum);
+    });
+    c.mark();
+    unsigned long long sum[4] = {~0ull, ~0ull, 0, 0};
+    c.to_host(sum, d_sum, sizeof(sum));
+    LO_TRY(c.finish(timing));
+    summary->first_invalid = sum[0] < (unsigned long long)n ? (int64_t)sum[0] : -1;
+    summary->first_unsupported = sum[1] < (unsigned long long)n ? (int64_t)sum[1] : -1;
+    summary->nulls = (int64_t)sum[2];
+    summary->all_integer = sum[3] == 0;
+    return LO_OK;
+}
+
 // number -> text for one column (R-semantics "string" cast): cell lengths, an exclusive scan of them into the Arrow
 // offsets, then every cell's text at its offset.  The offsets come back before the text is made, so the caller's
 // capacity is checked against the exact size and the device text buffer is allocated at that size.

@@ -106,11 +106,7 @@ class DataType:
                 integral = col.valid & np.isfinite(v) & (v == np.floor(v))
                 db.set_column(filename, field, NumberColumn(v, col.valid, integral))
                 return
-            import pyarrow.compute as pc
-            arr = col.arr
-            if not pc.all(pc.string_is_ascii(arr.fill_null(""))).as_py():      # Unicode digits / spaces, as float(str)
-                import pyarrow as pa
-                arr = pa.array([None if c is None else columnar.ascii_number_text(c) for c in arr.to_pylist()], type=pa.large_string())
+            arr = columnar.number_text(col.arr)                 # Unicode digits / spaces, as float(str)
             chars, offsets, nulls = TextColumn(arr).packed()
             values, status = self.engine.parse_number_packed(chars, offsets)
             bad = np.flatnonzero((status == N.LO_NUM_INVALID) | (status == N.LO_NUM_UNSUPPORTED))

@@ -481,6 +481,32 @@ class Engine:
                                                    n, values.ctypes.data_as(C.c_void_p), status.ctypes.data_as(C.c_void_p), None))
         return values, status
 
+    def parse_number_into(self, table: DeviceTable, col: int, chars: np.ndarray, offsets: np.ndarray, nulls=None) -> dict:
+        """``float(cell)`` of every cell of a packed text column (chars uint8, offsets int64[n+1], offsets[0] may be
+        non-zero) written on the device into f64 column ``col`` of ``table``, one row per cell; null and empty cells
+        become NaN.  The text must be ASCII-normalised (:func:`columnar.number_text`).  nulls: None, a bool array
+        (True = null), or ``(bitmap, bit_offset)`` — an Arrow validity bitmap as uint8.  Returns the call's summary:
+        ``first_invalid`` / ``first_unsupported`` (row relative to the first cell, or None), ``nulls`` (null + empty
+        cells), ``integer`` (every other cell integer valued) and the lo_host_timing fields."""
+        n = offsets.shape[0] - 1
+        keep = None                 # the validity buffer handed to the call
+        v = N.Validity()
+        if isinstance(nulls, tuple):
+            keep = np.ascontiguousarray(nulls[0], dtype=np.uint8)
+            v.bitmap, v.bit_offset = keep.ctypes.data, int(nulls[1])
+        elif nulls is not None:
+            keep = np.ascontiguousarray(~np.asarray(nulls, dtype=bool)).view(np.uint8)
+            if keep.shape != (n,):
+                raise ValueError("nulls must have one entry per cell")
+            v.mask = keep.ctypes.data
+        offsets = np.ascontiguousarray(offsets, dtype=np.int64)
+        s, t = N.ParseSummary(), N.HostTiming()
+        N.check(self._lib.lo_parse_number_to_table(self._ctx, chars.ctypes.data_as(C.c_void_p), offsets.ctypes.data_as(C.c_void_p),
+                                                   C.byref(v), n, table._h, int(col), 0, C.byref(s), C.byref(t)))
+        return {"first_invalid": s.first_invalid if s.first_invalid >= 0 else None,
+                "first_unsupported": s.first_unsupported if s.first_unsupported >= 0 else None,
+                "nulls": int(s.nulls), "integer": bool(s.all_integer), **_timing(t), "kernel_ms": t.kernel_ms}
+
     def format_number_host(self, values: np.ndarray, status: np.ndarray, timing: dict | None = None):
         """The inverse of :meth:`parse_number_packed`: values float64[n] and status uint8[n] (LO_NUM_FLOAT ->
         ``repr(float)``, LO_NUM_INTEGER -> ``str(int)``, LO_NUM_EMPTY -> ``""``) become one packed text column

@@ -14,8 +14,9 @@ Here the counting runs on the GPU with no host dictionary:
   when MongoDB groups them (:func:`columnar.tagged_cell`: 1 == 1.0, ``True`` != 1, ``"1"`` != 1).
 
 ``None`` / missing values (the metadata document among them) are counted while packing.  With ``bins`` (optional
-extension, REST keys ``bins`` / ``range``) the fields must be numeric and get the fixed-width B-semantics histogram
-of SURVEY.md §8c from the fused kernel, run on the HBM-resident copy of the dataset (``table_cache``).
+extension, REST keys ``bins`` / ``range``) the fields must be numeric or text (text is parsed with ``float()`` on the
+device into the resident slab; the dataset stays text) and get the fixed-width B-semantics histogram of SURVEY.md §8c
+from the fused kernel, run on the HBM-resident copy of the dataset (``table_cache``).
 The dictionary-code kernels (``hist_u8_cols_host`` / ``value_counts_u32_host``) remain available on the engine for
 columns that arrive already encoded (e.g. the uint8 tables of config M).
 """

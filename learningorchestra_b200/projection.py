@@ -8,7 +8,8 @@ Reference job (``projection.py:32-48``): Spark loads the input collection, drops
   adapter — there is no arithmetic to put on a GPU, and the values must come back untouched (strings
   included).
 * ``cast_to="float32"`` (this build's optional extension, REST key ``castTo``): the selected columns must
-  be numeric; they go through the fused sm_90a kernel (projection + fp64->fp32 RNE cast, and with
+  be numeric or text (text is ``float(cell)`` parsed on the device; None / ``""`` stay None); they go through
+  the fused sm_90a kernel (projection + fp64->fp32 RNE cast, and with
   ``bins`` a fixed-width histogram in the same pass) via ``lo_project_cast_hist_host``.
 """
 from __future__ import annotations
@@ -115,7 +116,8 @@ class Projection:
                 cols = {}
                 for j, f in enumerate(selected):
                     src = database.column(source, f)
-                    cols[f] = NumberColumn(np.where(src.valid, out.to_numpy(j).astype(np.float64), np.nan), src.valid)
+                    valid = columnar.number_text_valid(src.arr) if src.kind == "text" else src.valid
+                    cols[f] = NumberColumn(np.where(valid, out.to_numpy(j).astype(np.float64), np.nan), valid)
             finally:
                 if out is not None:
                     out.free()
@@ -125,9 +127,13 @@ class Projection:
     def __gpu_cast(self, database, target, rows, ids, selected, bins, value_range):
         if self.__engine is None:
             raise RuntimeError("cast_to needs an Engine in the spark_session slot (there is no CPU fallback)")
+        from .table_cache import is_text_field
         cols, masks = [], []
         for f in selected:
-            packed = columnar.numeric_column([d.get(f) for d in rows])
+            values = [d.get(f) for d in rows]
+            packed = columnar.numeric_column(values)
+            if packed is None and is_text_field(values):
+                packed = self.__parse_text(values)
             if packed is None:
                 raise ValueError(f"field {f!r} is not numeric; run /fieldTypes first")
             cols.append(packed[0])
@@ -153,3 +159,15 @@ class Projection:
             o[self.__DOCUMENT_ID] = ids[i]
             docs.append(o)
         return docs
+
+    def __parse_text(self, values):
+        """(float64 values, valid mask) of a text field: the cells parsed on the device by the same call the resident
+        tables use (:func:`table_cache.parse_text_column`), then read back for the host pipeline."""
+        from .table_cache import parse_text_column
+        table = self.__engine.table("f64", len(values), 1)
+        try:
+            parse_text_column(self.__engine, table, 0, values)
+            parsed = table.to_numpy(0)
+        finally:
+            table.free()
+        return parsed, np.array([v is not None and v != "" for v in values], dtype=bool)

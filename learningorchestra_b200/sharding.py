@@ -13,6 +13,7 @@ pages by ``_id`` range, ``database_api_image/utils.py:17-23``).
 from __future__ import annotations
 
 import ctypes as C
+import threading
 
 ROW_ALIGN = 32
 
@@ -48,6 +49,25 @@ def allreduce_counts(counts_tensor, group=None):
     if dist.is_available() and dist.is_initialized() and dist.get_world_size(group) > 1:
         dist.all_reduce(counts_tensor, op=dist.ReduceOp.SUM, group=group)
     return counts_tensor
+
+
+def combine_parse_summaries(parts, row_offsets) -> dict:
+    """One ``parse_number_into`` summary from those of several shards: the first bad rows are the minimum over the
+    shards after adding each shard's first global row, counts and bytes add up, ``integer`` holds on every shard, and
+    the times are the longest shard's (the shards run at once)."""
+    out = {"first_invalid": None, "first_unsupported": None, "nulls": 0, "integer": True, "total_ms": 0.0,
+           "kernel_ms": 0.0, "h2d_bytes": 0.0, "d2h_bytes": 0.0, "launches": 0}
+    for part, off in zip(parts, row_offsets):
+        for key in ("first_invalid", "first_unsupported"):
+            if part[key] is not None and (out[key] is None or off + part[key] < out[key]):
+                out[key] = off + part[key]
+        out["nulls"] += part["nulls"]
+        out["integer"] = out["integer"] and part["integer"]
+        for key in ("total_ms", "kernel_ms"):
+            out[key] = max(out[key], part[key])
+        for key in ("h2d_bytes", "d2h_bytes", "launches"):
+            out[key] += part[key]
+    return out
 
 
 class ShardedTable:
@@ -334,6 +354,38 @@ class ShardedEngine:
         out = C.c_uint64()
         self._N.check(self._lib.lo_group_timeouts(self._g, C.byref(out)))
         return int(out.value)
+
+    def parse_number_into(self, table: ShardedTable, col: int, chars, offsets, nulls=None) -> dict:
+        """``Engine.parse_number_into`` over a sharded table: ``chars`` / ``offsets`` / ``nulls`` describe ALL
+        ``table.nrows`` rows, and every local member parses the slice of its own shard into it, each on a host thread
+        of its own.  The summary is over this process's shards, rows global: with a rank group each rank holds its own
+        and the global first bad row is the minimum over the ranks."""
+        def shard_nulls(off, nr):
+            if nulls is None:
+                return None
+            if isinstance(nulls, tuple):
+                return nulls[0], int(nulls[1]) + off
+            return nulls[off:off + nr]
+
+        parts = [None] * self.nlocal
+
+        def run(i):
+            t, off = table.shards[i], table.offsets[i]
+            try:
+                parts[i] = self.engines[i].parse_number_into(t, col, chars, offsets[off:off + t.nrows + 1],
+                                                             shard_nulls(off, t.nrows))
+            except BaseException as exc:       # re-raised on the calling thread
+                parts[i] = exc
+
+        threads = [threading.Thread(target=run, args=(i,)) for i in range(self.nlocal)]
+        for th in threads:
+            th.start()
+        for th in threads:
+            th.join()
+        for p in parts:
+            if isinstance(p, BaseException):
+                raise p
+        return combine_parse_summaries(parts, table.offsets)
 
     # ---- host buffers -------------------------------------------------------------------------------------
     def project_cast_hist_host(self, cols, nbins: int | None = None, lo=None, hi=None, out=None, bcast: bool = False):

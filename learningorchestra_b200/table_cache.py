@@ -7,6 +7,11 @@ columnar :class:`~learningorchestra_b200.engine.DeviceTable` and stay on the GPU
 projection requests on the same dataset run on the resident slabs (``lo_project_cast_hist_dev``) with no
 document scan and no host->device copy, which is the regime ``bench.py``'s ``value`` measures.
 
+Text fields (every dataset arrives as text) are parsed on the device straight into their slabs with CPython's
+``float()`` (``lo_parse_number_to_table``): a binned histogram or a ``castTo`` projection of a freshly uploaded CSV
+needs no ``/fieldTypes`` job first, and the dataset is never modified.  The slab equals the one ``/fieldTypes
+"number"`` would have led to, bit for bit.
+
 Staleness: the in-process :class:`~learningorchestra_b200.utils.Database` bumps ``version(filename)`` on every
 write to data rows; a cached table is used only while its version matches.  A ``Database`` without
 ``version`` (foreign object) is never cached.  Eviction: least recently used beyond ``max_bytes``.
@@ -40,6 +45,34 @@ def device_number_column(values: np.ndarray, valid: np.ndarray, is_int: np.ndarr
     if valid.all():
         return values, valid, "int" if is_int.all() else "float"
     return np.where(valid, values, np.nan), valid, "int" if bool((is_int | ~valid).all()) else "float"
+
+
+def _number_source(packed):
+    return None if packed is None else ("number", packed)
+
+
+def is_text_field(values) -> bool:
+    """A document field the text route takes: at least one value, and every value that is not None a ``str``."""
+    return any(v is not None for v in values) and all(v is None or type(v) is str for v in values)
+
+
+def parse_text_column(engine, table, col: int, cells):
+    """``float(cell)`` of every cell of a text field — an Arrow string array, or a list of ``str`` / None — parsed on
+    the device straight into f64 column ``col`` of ``table`` (a ``DeviceTable`` or ``ShardedTable``): None and ``""``
+    become NaN, every other cell the binary64 ``/fieldTypes "number"`` stores.  Returns (kind "int" | "float", null
+    count).  The first bad cell in row order fails the call: ValueError with ``float()``'s message for text it rejects,
+    RuntimeError for a cell over the parser's 1 MiB limit (there is no host fallback)."""
+    chars, offsets, validity = columnar.text_buffers(columnar.number_text(cells))
+    summary = engine.parse_number_into(table, col, chars, offsets, validity)
+    bad = [r for r in (summary["first_invalid"], summary["first_unsupported"]) if r is not None]
+    if bad:
+        row = min(bad)
+        cell = cells[row].as_py() if hasattr(cells, "to_pylist") else cells[row]
+        if row == summary["first_unsupported"]:
+            raise RuntimeError(f"cell of {len(cell)} characters exceeds the device parser's 1 MiB limit "
+                               "and there is no CPU fallback")
+        raise ValueError(f"could not convert string to float: {cell!r}")
+    return ("int" if summary["integer"] else "float"), summary["nulls"]
 
 
 class ResidentTables:
@@ -77,8 +110,10 @@ class ResidentTables:
 
     def ensure(self, database, filename: str, fields) -> ResidentDataset:
         """Resident table holding (at least) ``fields`` of ``filename``; built from the documents on a miss.
-        Raises ValueError if a requested field is not numeric.  The returned entry is LEASED: pair every call with
-        :meth:`release` (or use :meth:`lease`)."""
+        A field may be numeric or text (a column-store text column, or document values that are all ``str`` / None):
+        text is parsed on the device into its slab, the dataset itself stays text.  Raises ValueError if a requested
+        field is neither, or names the first cell ``float()`` rejects; on any failure nothing is cached.  The returned
+        entry is LEASED: pair every call with :meth:`release` (or use :meth:`lease`)."""
         version = database.version(filename) if hasattr(database, "version") else None
         with self._lock:
             entry = self._entries.get(filename)
@@ -98,25 +133,43 @@ class ResidentTables:
                 rows = columnar.data_rows(database.find(filename, {}))
                 rows.sort(key=lambda d: d["_id"])
                 row_ids = np.array([d["_id"] for d in rows], dtype=np.int64)
-            cols, kinds, nulls, names = [], [], [], []
+            sources, names = [], []          # per resident column: ("number", packed) or ("text", cells)
             for f in wanted:
                 if columnar_rows:
                     c = database.column(filename, f)
                     if c is not None and c.kind == "object":
-                        packed = columnar.numeric_column(c.to_pylist())
+                        src = _number_source(columnar.numeric_column(c.to_pylist()))
                     elif c is not None and c.kind == "number":
-                        packed = device_number_column(c.values, c.valid, c.is_int)
+                        src = ("number", device_number_column(c.values, c.valid, c.is_int))
+                    elif c is not None and c.kind == "text":
+                        src = ("text", c.arr)
                     else:
-                        packed = None
+                        src = None
                 else:
-                    packed = columnar.numeric_column([d.get(f) for d in rows])
-                if packed is None:
+                    values = [d.get(f) for d in rows]
+                    src = _number_source(columnar.numeric_column(values))
+                    if src is None and is_text_field(values):
+                        src = ("text", values)
+                if src is None:
                     if f in fields:
                         raise ValueError(f"field {f!r} is not numeric; run /fieldTypes first")
                     continue                 # a previously resident column that stopped being numeric: drop it
-                names.append(f); cols.append(packed[0]); kinds.append(packed[2])
-                nulls.append(int(packed[1].size - np.count_nonzero(packed[1])))
-            table = self.engine.table_from_numpy(cols) if len(rows) and cols else self.engine.table("f64", 0, max(len(cols), 1))
+                names.append(f); sources.append(src)
+            table = self.engine.table("f64", len(rows) if sources else 0, max(len(sources), 1))
+            kinds, nulls = [], []
+            try:
+                for j, (how, src) in enumerate(sources):
+                    if how == "number":
+                        values, valid, kind = src
+                        if len(rows):
+                            table.upload(j, values)
+                        kinds.append(kind); nulls.append(int(valid.size - np.count_nonzero(valid)))
+                    else:
+                        kind, n_null = parse_text_column(self.engine, table, j, src)
+                        kinds.append(kind); nulls.append(n_null)
+            except BaseException:
+                table.free()                 # a bad cell: nothing of the partly built table stays, nothing is cached
+                raise
             new = ResidentDataset(version, row_ids, names, kinds, nulls, table)
             new.users = 1
             if entry is not None:
