@@ -14,6 +14,7 @@ import numpy as np
 import pytest
 
 from oracle import bsem_numpy as bn
+from test_gpu_hist_routes import EDGE_RANGES
 
 ROOT = Path(__file__).resolve().parent.parent
 KAT = json.loads((ROOT / "tests" / "golden" / "bin_kat.json").read_text())["cases"]
@@ -71,8 +72,10 @@ def test_edges_bin_the_kat_vectors_like_the_oracle(built, case):
     np.testing.assert_array_equal(got, np.asarray(c["bin"]))
 
 
-@pytest.mark.parametrize("lo,hi,nbins", TRIPLES)
+@pytest.mark.parametrize("lo,hi,nbins", TRIPLES + [r for r in EDGE_RANGES if r not in TRIPLES])
 def test_edges_of_the_self_test_ranges(built, lo, hi, nbins):
+    """The ranges of the exhaustive self-tests and of the GPU route tests (up to 65 536 bins), whose values are placed
+    on and around these edges."""
     rng = np.random.default_rng(nbins)
     _check_edges(lo, hi, nbins, extra=rng.uniform(lo, hi, 20_000))
 
