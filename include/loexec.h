@@ -246,7 +246,9 @@ int lo_group_shard(const lo_group *g, int64_t total_rows, int32_t index, int64_t
 /* The hot path over the group.  in[i] / out[i] / streams[i]: the shard, output table (or out == NULL) and stream
  * (or streams == NULL: each context's own) of LOCAL member i.  Asynchronous.  The merged k x nbins matrix of the
  * step lands in the group's result buffer on the root (on every member with LO_GROUP_BCAST or LO_MERGE_NCCL);
- * read it with lo_group_result.  k <= 128 (f64) / 1024 (u8) per call. */
+ * read it with lo_group_result.  k <= 128 (f64) / 1024 (u8) per call, and k * nbins <= LO_GROUP_MAX_COUNTS: the
+ * group's matrices hold that many counts, so the f64 entry points (_dev and _host) return LO_ERR_INVALID for a larger
+ * step before launching anything; split its columns over several steps. */
 int lo_group_project_cast_hist_dev(lo_group *g, const lo_table *const *in, const int32_t *col_idx, int32_t k,
                                    lo_table *const *out, const lo_hist_spec *spec, int32_t flags,
                                    void *const *streams);

@@ -51,6 +51,26 @@ def allreduce_counts(counts_tensor, group=None):
     return counts_tensor
 
 
+def column_batches(k: int, nbins: int, cap: int | None = None) -> list[tuple[int, int]]:
+    """Column ranges [begin, end) of the group steps one ``k x nbins`` histogram request takes.  A group merges at most
+    ``cap`` (LO_GROUP_MAX_COUNTS) counts per step: a request within that is one step, a larger one runs of
+    ``max(1, cap // nbins)`` columns, in column order.  Depends on (k, nbins) only, so every rank issues the same steps."""
+    if cap is None:
+        from ._native import LO_GROUP_MAX_COUNTS as cap
+    if k * nbins <= cap:
+        return [(0, k)]
+    per = max(1, cap // nbins)
+    return [(c0, min(k, c0 + per)) for c0 in range(0, k, per)]
+
+
+def _combine_timings(parts) -> dict:
+    out = dict(parts[0])
+    for t in parts[1:]:
+        for key in out:
+            out[key] += t[key]
+    return out
+
+
 def combine_parse_summaries(parts, row_offsets) -> dict:
     """One ``parse_number_into`` summary from those of several shards: the first bad rows are the minimum over the
     shards after adding each shard's first global row, counts and bytes add up, ``integer`` holds on every shard, and
@@ -122,12 +142,20 @@ class ShardedTable:
 
 
 class GroupCounts:
-    """Merged counts of the step that produced it, in the group's result buffer (valid until the next group call)."""
+    """Merged counts of the step that produced it, in the group's result buffer (valid until the next group call).
+    A request split over several steps (:func:`column_batches`) has read each step's counts out already: ``host``
+    holds them, or is None on a rank that receives no result."""
 
-    def __init__(self, sharded: "ShardedEngine", k: int, nbins: int):
+    def __init__(self, sharded: "ShardedEngine", k: int, nbins: int, host=None, batched: bool = False):
         self.engine, self.k, self.nbins = sharded, int(k), int(nbins)
+        self._host, self._batched = host, batched
 
     def to_numpy(self, stream=None):
+        if self._host is not None:
+            return self._host.copy()
+        if self._batched:
+            N = self.engine._N
+            raise N.LoexecError(N.LO_ERR_INVALID, "this rank received no merged counts (pass bcast=True to receive them everywhere)")
         return self.engine.result(self.k * self.nbins).reshape(self.k, self.nbins)
 
     def free(self) -> None:
@@ -303,14 +331,45 @@ class ShardedEngine:
         """One step over all shards: fused projection + cast + histogram on every member, partial histograms merged
         inside the kernels.  Asynchronous; the merged counts are read with ``.to_numpy()`` / :meth:`result`.
         ``independent``: this step reads nothing the previous group step wrote (another job, or the same inputs
-        again), so it may start while that step's last wave is still draining."""
+        again), so it may start while that step's last wave is still draining.
+        A request of more than LO_GROUP_MAX_COUNTS counts is split into column batches (:func:`column_batches`), one
+        step each, whose merged counts are read out before the next step; the call then returns after the last."""
         from .engine import _i32
         idx, k = _i32(col_idx)
-        spec, _keep = self.engines[0]._spec(k, nbins, lo, hi)
-        self._N.check(self._lib.lo_group_project_cast_hist_dev(
-            self._g, self._tables(table), idx, k, self._tables(out), C.byref(spec),
-            self._flags(bcast, independent), self._streams(streams)))
-        return GroupCounts(self, k, nbins)
+        batches = column_batches(k, nbins)
+        if len(batches) == 1:
+            spec, _keep = self.engines[0]._spec(k, nbins, lo, hi)
+            self._N.check(self._lib.lo_group_project_cast_hist_dev(
+                self._g, self._tables(table), idx, k, self._tables(out), C.byref(spec),
+                self._flags(bcast, independent), self._streams(streams)))
+            return GroupCounts(self, k, nbins)
+        import numpy as np
+        lo = np.broadcast_to(np.asarray(lo, np.float32), (k,))
+        hi = np.broadcast_to(np.asarray(hi, np.float32), (k,))
+        host = np.zeros((k, nbins), np.uint64) if bcast or self.has_result or self.merge == "nccl" else None
+        for c0, c1 in batches:
+            spec, _keep = self.engines[0]._spec(c1 - c0, nbins, lo[c0:c1], hi[c0:c1])
+            views = self._column_views(out, c0, c1)
+            try:
+                self._N.check(self._lib.lo_group_project_cast_hist_dev(
+                    self._g, self._tables(table), _i32(idx[c0:c1])[0], c1 - c0, self._tables(views), C.byref(spec),
+                    self._flags(bcast, independent), self._streams(streams)))
+            finally:
+                if views is not None:
+                    views.free()           # descriptors only: the kernels took base and pitch by value
+            if host is not None:
+                host[c0:c1] = self.result((c1 - c0) * nbins).reshape(c1 - c0, nbins)
+        return GroupCounts(self, k, nbins, host=host, batched=True)
+
+    def _column_views(self, t: ShardedTable | None, c0: int, c1: int) -> ShardedTable | None:
+        """Columns [c0, c1) of every shard of ``t``, as tables over the same memory."""
+        if t is None:
+            return None
+        from .engine import _DTYPES
+        name = {code: n for n, code in _DTYPES.items()}[t.shards[0].dtype_code]
+        shards = [e.wrap(name, s.nrows, c1 - c0, s.base_ptr + c0 * s.pitch_bytes, s.pitch_bytes, keepalive=s)
+                  for e, s in zip(self.engines, t.shards)]
+        return ShardedTable(self, shards, t.offsets, t.nrows)
 
     def project_cast(self, table: ShardedTable, col_idx, out: ShardedTable | None = None, out_dtype: str = "f32",
                      streams=None) -> ShardedTable:
@@ -390,11 +449,20 @@ class ShardedEngine:
     # ---- host buffers -------------------------------------------------------------------------------------
     def project_cast_hist_host(self, cols, nbins: int | None = None, lo=None, hi=None, out=None, bcast: bool = False):
         """Same contract as ``Engine.project_cast_hist_host``; the rows passed are this process's rows, cut across its
-        local members by the library.  counts: merged over the whole group (zeros on a rank that holds no result)."""
+        local members by the library.  counts: merged over the whole group (zeros on a rank that holds no result).
+        More than LO_GROUP_MAX_COUNTS counts: one call per column batch (:func:`column_batches`), timings added up."""
         import numpy as np
         from .engine import _host_cols, _out_cols, _timing
         N = self._N
         k = len(cols)
+        batches = column_batches(k, nbins) if nbins else [(0, k)]
+        if len(batches) > 1:
+            lo = np.broadcast_to(np.asarray(lo, np.float32), (k,))
+            hi = np.broadcast_to(np.asarray(hi, np.float32), (k,))
+            parts = [self.project_cast_hist_host(cols[c0:c1], nbins, lo[c0:c1], hi[c0:c1],
+                                                 out=out[c0:c1] if out is not None else None, bcast=bcast)
+                     for c0, c1 in batches]
+            return np.concatenate([c for c, _ in parts]), _combine_timings([t for _, t in parts])
         in_p, n = _host_cols(cols, np.float64)
         out_p = _out_cols(out, k, n)
         spec_ref, counts, _keep = None, None, None

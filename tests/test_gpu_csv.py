@@ -104,7 +104,7 @@ def test_ingest_matches_the_pyarrow_path_on_titanic(engine, tmp_path):
     for name in a.column_names("t"):
         assert a.column("t", name).arr.to_pylist() == b.column("t", name).arr.to_pylist()
         b.column("t", name).arr.validate(full=True)
-    by_id = lambda db: sorted(db.find("t", {}), key=lambda d: d["_id"])
+    by_id = lambda db: sorted((strip(d) for d in db.find("t", {})), key=lambda d: d["_id"])   # the two ingests may straddle a second
     assert by_id(a) == by_id(b)
 
 

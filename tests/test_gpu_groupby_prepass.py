@@ -19,6 +19,10 @@ import numpy as np
 import pytest
 from werkzeug.test import Client
 
+from edge_values import F32_MAX, NAN_BITS
+from edge_values import f64 as _f64
+from edge_values import prepass_columns as _prepass_columns
+from edge_values import ref_minmax as _ref_minmax
 from learningorchestra_b200 import _native as N
 from learningorchestra_b200 import server, utils
 from oracle import bsem_numpy as bn
@@ -26,11 +30,6 @@ from oracle import rsem
 
 pytestmark = pytest.mark.gpu
 GOLD = Path(__file__).resolve().parent / "golden"
-F32_MAX = 3.4028234663852886e38
-
-
-def _f64(bits):
-    return np.array(bits, dtype=np.uint64).view(np.float64)
 
 
 def _table_slots(n: int) -> int:
@@ -42,8 +41,6 @@ def _table_slots(n: int) -> int:
 
 
 # ---- numeric $group ---------------------------------------------------------------------------------------------
-NAN_BITS = [0x7FF8000000000000, 0xFFF8000000000000, 0x7FF0000000000001, 0xFFF0000000000001, 0x7FF4000000000000,
-            0x7FFFFFFFFFFFFFFF, 0xFFFFFFFFFFFFFFFF, 0x7FF8DEADBEEF0001, 0xFFF00000DEADBEEF, 0x7FFC000000000123]
 ZERO_BITS = [0x0000000000000000, 0x8000000000000000]
 
 
@@ -243,41 +240,6 @@ def test_value_counts_str_packed_on_a_sliced_arrow_column(engine):
 
 
 # ---- range pre-pass -----------------------------------------------------------------------------------------------
-def _prepass_columns(n):
-    rng = np.random.default_rng(31)
-    cols = []
-    cols.append(_f64(np.array(NAN_BITS, np.uint64)[rng.integers(0, len(NAN_BITS), n)]))            # all NaN
-    cols.append(np.where(rng.random(n) < 0.5, np.inf, -np.inf))                                     # all +-inf
-    c = np.array([3.4028235677973366e38, 1e39, -1e39, F32_MAX])[rng.integers(0, 4, n)]               # only FLT_MAX
-    cols.append(c)                                                                                   # survives the cast
-    cols.append(-rng.uniform(1.0, 1e6, n))                                                          # negatives only
-    cols.append(np.where(rng.random(n) < 0.5, 0.0, -0.0))                                           # +0.0 and -0.0
-    tiny = np.array([1e-46, -1e-46, 1e-40, -1e-40, 2.0 ** -149, 2.0 ** -150, 2.0 ** -150 + 2.0 ** -200, -(2.0 ** -150)])
-    c = np.concatenate([tiny, rng.uniform(-1.2e-38, 1.2e-38, n - tiny.size)])                       # -> +-0 / subnormal
-    cols.append(c)
-    for where in (0, n - 1, n // 2 + 7):                                                            # one finite value
-        c = np.full(n, np.nan)
-        c[where] = -12.375
-        cols.append(c)
-    cols.append(rng.normal(0.0, 1e4, n))
-    return cols
-
-
-def _ref_minmax(col):
-    """(min, max, nfinite) of the finite fp32-cast values; -0.0 orders below +0.0; no finite value -> (0, 0, 0)."""
-    f = bn.cast_f64_f32(col)
-    fin = f[np.isfinite(f)]
-    if fin.size == 0:
-        return np.float32(0.0), np.float32(0.0), 0
-    mn, mx = fin.min(), fin.max()
-    zeros = fin[fin == 0]
-    if mn == 0:
-        mn = np.float32(-0.0) if np.signbit(zeros).any() else np.float32(0.0)
-    if mx == 0:
-        mx = np.float32(0.0) if (~np.signbit(zeros)).any() else np.float32(-0.0)
-    return mn, mx, fin.size
-
-
 def _check_minmax(got, cols, col_idx):
     mins, maxs, cnt = got
     for j, c in enumerate(col_idx):

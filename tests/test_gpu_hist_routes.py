@@ -9,12 +9,12 @@ context's count of divide launches, the wide-bin kernel through ``selftest_fastd
 launcher tests.  Counts must equal the oracle's, fp32 outputs must be bit-equal to its cast and fp64 copies bit-equal to
 the input, NaN payloads included.
 """
-import ctypes
 from typing import NamedTuple
 
 import numpy as np
 import pytest
 
+from edge_values import edge_column
 from oracle import bsem_numpy as bn
 
 pytestmark = pytest.mark.gpu
@@ -89,58 +89,9 @@ def _bits(a):
     return a.view({4: np.uint32, 8: np.uint64}[a.dtype.itemsize])
 
 
-def _f64(*bits):
-    return np.array(bits, np.uint64).view(np.float64)
-
-
-F32_MAX_TIE = float(np.float64(np.finfo(np.float32).max) + 2.0 ** 103)    # halfway to 2^128: rounds to +inf
-SPECIALS = np.concatenate([
-    [0.0, -0.0],
-    np.array([1, 3, 0x7FFFFF, 0x80000001, 0x80400000], np.uint32).view(np.float32).astype(np.float64),   # fp32 subnormals
-    # overflow in fp32 (the tie at FLT_MAX rounds to inf, one ulp below it to FLT_MAX) and underflow (2^-150 is the tie
-    # with 0, 3 * 2^-150 the tie between the two smallest subnormals)
-    [F32_MAX_TIE, -F32_MAX_TIE, np.nextafter(F32_MAX_TIE, 0.0), 1e39, -1e300, 2.0 ** -150, -(2.0 ** -150), 3 * 2.0 ** -150,
-     1e-46, -1e-300, np.inf, -np.inf],
-    _f64(0x7FF8000000000000, 0xFFF4000000000001),      # quiet NaN; negative signalling NaN with a payload
-])
-
-
-def _edges(lo, hi, nbins):
-    from learningorchestra_b200 import _native
-    E = np.zeros(nbins + 1, np.float32)
-    assert _native.load().lo_hist_edges(ctypes.c_float(lo), ctypes.c_float(hi), nbins,
-                                        E.ctypes.data_as(ctypes.c_void_p)) == _native.LO_OK
-    return E
-
-
-_columns_cache = {}
-
-
-def _edge_column(lo, hi, nbins):
-    """fp64 values on every edge of (lo, hi, nbins) and on both fp32 neighbours, the exact midpoints between an edge and
-    each neighbour (round-to-nearest-even ties of the cast) and one fp64 ulp either side of them, the range ends and
-    their outer neighbours, special values and a uniform fill; shuffled with a fixed seed."""
-    key = (lo, hi, nbins)
-    if key not in _columns_cache:
-        E = _edges(lo, hi, nbins)
-        e = E.astype(np.float64)
-        up = np.nextafter(E, np.float32(np.inf)).astype(np.float64)
-        down = np.nextafter(E, np.float32(-np.inf)).astype(np.float64)
-        mids = np.concatenate([(e + up) / 2, (e + down) / 2])       # exact: 25 significant bits
-        mids = mids[np.isfinite(mids)]
-        lo32, hi32 = np.float32(lo), np.float32(hi)
-        ends = np.array([lo32, hi32, np.nextafter(lo32, np.float32(-np.inf)), np.nextafter(hi32, np.float32(np.inf))],
-                        np.float64)
-        rng = np.random.default_rng(nbins)
-        x = np.concatenate([e, up, down, mids, np.nextafter(mids, -np.inf), np.nextafter(mids, np.inf), ends, SPECIALS,
-                            rng.uniform(lo, hi, 4096 + nbins)])
-        _columns_cache[key] = x[rng.permutation(x.size)]
-    return _columns_cache[key]
-
-
 def _table(lo, hi, nbins, rows):
     """[k, rows] fp64: the edge column tiled over k <= MAX_K columns (all of it once there are enough rows)."""
-    x = _edge_column(lo, hi, nbins)
+    x = edge_column(lo, hi, nbins)
     k = min(MAX_K, -(-x.size // rows))
     return np.resize(x, k * rows).reshape(k, rows)
 
@@ -338,7 +289,7 @@ def test_host_pipeline_chunks_through_the_wide_bin_routes(engine, monkeypatch, n
     """1 MiB chunks: two columns go through five chunks of 61 440 rows (the last one short), one launch each."""
     monkeypatch.setenv("LOEXEC_CHUNK_MB", "1")
     rows = 4 * TILE + 1234
-    x = np.stack([np.resize(_edge_column(lo, hi, nbins), rows) for lo, hi in ranges])
+    x = np.stack([np.resize(edge_column(lo, hi, nbins), rows) for lo, hi in ranges])
     lo = np.array([r[0] for r in ranges], np.float32)
     hi = np.array([r[1] for r in ranges], np.float32)
     outs = [np.empty(rows, np.float32) for _ in ranges]

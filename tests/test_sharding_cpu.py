@@ -10,9 +10,32 @@ import torch
 import torch.distributed as dist
 import torch.multiprocessing as mp
 
-from learningorchestra_b200.sharding import all_shard_bounds, allreduce_counts, shard_bounds
+from learningorchestra_b200.sharding import all_shard_bounds, allreduce_counts, column_batches, shard_bounds
 
 SEED = 20260921
+GROUP_CAP = 262144          # LO_GROUP_MAX_COUNTS
+
+
+def test_column_batches_fit_the_group_cap():
+    from learningorchestra_b200 import _native as N
+    assert N.LO_GROUP_MAX_COUNTS == GROUP_CAP
+    # within the cap: one step, today's single asynchronous call
+    assert column_batches(4, 65536) == [(0, 4)]
+    assert column_batches(1024, 256) == [(0, 1024)]
+    assert column_batches(64, 4096) == [(0, 64)]
+    # over it: runs of cap // nbins columns in column order, the last one short
+    assert column_batches(5, 65536) == [(0, 4), (4, 5)]
+    assert column_batches(128, 4096) == [(0, 64), (64, 128)]
+    assert column_batches(65, 4096) == [(0, 64), (64, 65)]
+    assert column_batches(3, 200_000, cap=150_000) == [(0, 1), (1, 2), (2, 3)]     # wider than the cap: one column each
+    for k in (1, 2, 5, 17, 64, 65, 127, 128):
+        for nbins in (1, 7, 256, 1000, 2048, 2049, 4096, 16384, 16385, 52429, 57345, 65536):
+            b = column_batches(k, nbins)
+            assert b[0][0] == 0 and b[-1][1] == k
+            assert all(e0 == b1 for (_, e0), (b1, _) in zip(b[:-1], b[1:]))          # contiguous, in order
+            assert all((e - s) * nbins <= GROUP_CAP for s, e in b)
+            assert len(b) == (1 if k * nbins <= GROUP_CAP else -(-k // (GROUP_CAP // nbins)))
+            assert b == column_batches(k, nbins)                                     # the same on every rank
 
 
 def test_shard_bounds_cover_and_align():
