@@ -43,7 +43,7 @@
 extern "C" {
 #endif
 
-#define LO_ABI_VERSION 5
+#define LO_ABI_VERSION 6
 
 #define LO_OK                    0
 #define LO_ERR_INVALID          -1   /* bad argument (message says which)              */
@@ -345,6 +345,27 @@ typedef struct lo_parse_summary {
 int lo_parse_number_to_table(lo_ctx *ctx, const uint8_t *chars, const int64_t *offsets, const lo_validity *validity,
                              int64_t n, lo_table *out, int32_t col, int64_t row0, lo_parse_summary *summary,
                              lo_host_timing *timing);
+
+/* One text column resident in HBM, for `$group` requests that come back to the same dataset: the cells cross PCIe once.
+ * lo_text_upload takes what lo_parse_number_to_table takes — offsets[0] need not be 0 (only chars[offsets[0] ..
+ * offsets[n]) is copied, the device offsets are rebased to 0), validity NULL / mask / bitmap with any bit_offset — and
+ * n < 2^31.  It checks free device memory first: too little -> LO_ERR_NOMEM naming the size.  lo_text_info: cells,
+ * bytes of text, null cells, device bytes held (any pointer may be NULL).  lo_text_free: NULL is fine.
+ * lo_value_counts_text: lo_value_counts_str_host's contract (rep_rows_out / counts_out / capacity / *ndistinct, more
+ * groups than capacity -> LO_ERR_INVALID with *ndistinct set) on the resident column: no cell crosses PCIe
+ * (h2d_bytes 0), null rows are not counted, representative rows index the whole column, nulls included.  Not `_dev`: it
+ * synchronises and writes host arrays.
+ * The text group-by kernel stages keys in a per-CTA shared-memory table of LO_TEXT_STAGE_SLOTS slots before the global
+ * one, with at most 8 CTAs per SM: a column with more than LO_TEXT_STAGE_SLOTS distinct cells per CTA overflows it,
+ * those keys go straight to the global table, and after a few such spills the CTA stops probing its stage. */
+#define LO_TEXT_STAGE_SLOTS 512
+typedef struct lo_text lo_text;
+int lo_text_upload(lo_ctx *ctx, const uint8_t *chars, const int64_t *offsets, const lo_validity *validity,
+                   int64_t n, lo_text **out, lo_host_timing *timing);
+int lo_text_info(const lo_text *t, int64_t *n, int64_t *nbytes, int64_t *nulls, size_t *device_bytes);
+int lo_text_free(lo_ctx *ctx, lo_text *t);
+int lo_value_counts_text(lo_ctx *ctx, const lo_text *t, int64_t *rep_rows_out, uint64_t *counts_out,
+                         int64_t capacity, int64_t *ndistinct, lo_host_timing *timing);
 
 /* Number -> text for one column: the reference's "string" cast, str(v) / None -> "" (data_type_handler_image/
  * data_type_update.py:22-28), for every cell at once on the GPU.  The inverse of lo_parse_number_host.

@@ -36,7 +36,8 @@ LO_NUM_FLOAT, LO_NUM_INTEGER, LO_NUM_EMPTY, LO_NUM_INVALID, LO_NUM_UNSUPPORTED =
 LO_FORMAT_MAX_CELL = 310
 LO_CSV_OK, LO_CSV_SHORT_ROW, LO_CSV_FIELD_LIMIT, LO_CSV_BAD_UTF8, LO_CSV_NUL, LO_CSV_UNSUPPORTED, LO_CSV_EMPTY = range(7)
 LO_CSV_STREAM_WINDOW = 64 << 20
-LO_ABI_VERSION = 5
+LO_TEXT_STAGE_SLOTS = 512
+LO_ABI_VERSION = 6
 
 _ERR_NAMES = {
     LO_ERR_INVALID: "LO_ERR_INVALID", LO_ERR_CUDA: "LO_ERR_CUDA", LO_ERR_NOMEM: "LO_ERR_NOMEM",
@@ -146,6 +147,10 @@ SIGNATURES = {
     "lo_parse_number_host": (C.c_int, [_P, _P, _P, C.c_int64, _P, _P, C.POINTER(HostTiming)]),
     "lo_parse_number_to_table": (C.c_int, [_P, _P, _P, C.POINTER(Validity), C.c_int64, _P, C.c_int32, C.c_int64,
                                            C.POINTER(ParseSummary), C.POINTER(HostTiming)]),
+    "lo_text_upload": (C.c_int, [_P, _P, _P, C.POINTER(Validity), C.c_int64, C.POINTER(_P), C.POINTER(HostTiming)]),
+    "lo_text_info": (C.c_int, [_P, C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(C.c_size_t)]),
+    "lo_text_free": (C.c_int, [_P, _P]),
+    "lo_value_counts_text": (C.c_int, [_P, _P, _P, _P, C.c_int64, C.POINTER(C.c_int64), C.POINTER(HostTiming)]),
     "lo_format_number_host": (C.c_int, [_P, _P, _P, C.c_int64, _P, _P, C.c_int64, C.POINTER(HostTiming)]),
     "lo_minmax_cast_host": (C.c_int, [_P, C.POINTER(_P), C.c_int64, C.c_int32, _P, _P, _P, C.POINTER(HostTiming)]),
     "lo_csv_read_host": (C.c_int, [_P, _P, C.c_int64, C.POINTER(_P), C.POINTER(CsvInfo), C.POINTER(HostTiming)]),

@@ -1177,12 +1177,52 @@ __device__ __forceinline__ bool same_cell(const uint8_t *chars, const long long 
     return true;
 }
 
-__global__ void k_hash_count_str(const uint8_t *__restrict__ chars, const long long *__restrict__ offsets, long long n,
-                                 unsigned long long *__restrict__ slots, unsigned long long *__restrict__ counts,
-                                 unsigned long long mask) {
+// Add `add` rows to the group of slot word `mine` (tag | representative row) whose cell hashes to h, in the global table.
+__device__ __forceinline__ void str_table_add(const uint8_t *chars, const long long *offsets, unsigned long long *slots,
+                                              unsigned long long *counts, unsigned long long mask, unsigned long long h,
+                                              unsigned long long mine, unsigned long long add) {
+    const long long row = (long long)(mine & 0x7FFFFFFFull);
+    unsigned long long s = splitmix64(h) & mask;
+    for (;;) {
+        const unsigned long long cur = atomicCAS(slots + s, kEmptyKey, mine);
+        if (cur == kEmptyKey || ((cur >> 31) == (mine >> 31) && same_cell(chars, offsets, row, (long long)(cur & 0x7FFFFFFFull)))) {
+            atomicAdd(counts + s, add);
+            return;
+        }
+        s = (s + 1) & mask;
+    }
+}
+
+// Per-CTA shared-memory stage of k_hash_count_str: kStrStageSlots slots of (slot word, cell hash, 32-bit count), probed
+// at most kStrStageProbe slots deep.  A low-cardinality column then costs one shared atomic per warp-merged key and one
+// global insert per group per CTA at the end, instead of a global CAS + RED.64 per key on the same few L2 lines; a key
+// that finds no room goes straight to the global table.  A column with more distinct cells than the stage holds would
+// pay the probes for nothing: once kStrStageBypass keys of a CTA have spilled, that CTA stops probing its stage (the
+// groups already staged are still flushed).  Sized from scripts/value_counts_bench.py (DESIGN §3.6).
+constexpr int kStrStageSlots = 512;
+constexpr int kStrStageProbe = 8;
+constexpr unsigned kStrStageBypass = 64;
+static_assert((kStrStageSlots & (kStrStageSlots - 1)) == 0, "the stage is indexed with a mask");
+
+// Cells are chars[offsets[i] .. offsets[i+1]) with offsets[0] == 0.  Validity: mask (one byte per cell, 0 = null),
+// bitmap (Arrow bitmap, bit bit0 + i, 0 = null) or neither; a null row is skipped and its bytes are never read.
+// Representative rows index the whole column, nulls included.
+__global__ void __launch_bounds__(256) k_hash_count_str(const uint8_t *__restrict__ chars, const long long *__restrict__ offsets,
+                                                        long long n, const uint8_t *__restrict__ valid_mask,
+                                                        const uint8_t *__restrict__ valid_bitmap, int bit0,
+                                                        unsigned long long *__restrict__ slots,
+                                                        unsigned long long *__restrict__ counts, unsigned long long mask) {
+    __shared__ unsigned long long st_word[kStrStageSlots];
+    __shared__ unsigned long long st_hash[kStrStageSlots];
+    __shared__ unsigned st_count[kStrStageSlots];
+    __shared__ unsigned st_spills;
+    for (int s = threadIdx.x; s < kStrStageSlots; s += blockDim.x) { st_word[s] = kEmptyKey; st_count[s] = 0; }
+    if (threadIdx.x == 0) st_spills = 0;
+    __syncthreads();
     for (long long i0 = blockIdx.x * (long long)blockDim.x; i0 < n; i0 += (long long)gridDim.x * blockDim.x) {
         const long long i = i0 + threadIdx.x;
-        const bool live = i < n;
+        const bool live = i < n && (valid_mask ? valid_mask[i] != 0
+                                    : valid_bitmap ? ((valid_bitmap[(bit0 + i) >> 3] >> ((bit0 + i) & 7)) & 1) != 0 : true);
         const unsigned active = __ballot_sync(0xffffffffu, live);
         if (!live) continue;
         const unsigned long long h = hash_bytes(chars + offsets[i], offsets[i + 1] - offsets[i]);
@@ -1191,22 +1231,37 @@ __global__ void k_hash_count_str(const uint8_t *__restrict__ chars, const long l
         const long long leader_row = __shfl_sync(active, i, leader);
         const bool same = ((int)(threadIdx.x & 31) == leader) || same_cell(chars, offsets, i, leader_row);
         const unsigned eq = __ballot_sync(active, same);
-        unsigned long long add;
-        if ((int)(threadIdx.x & 31) == leader) add = (unsigned long long)__popc(peers & eq);
-        else if (!same) add = 1ull;               // hash collision inside the warp: insert on its own
+        unsigned add;
+        if ((int)(threadIdx.x & 31) == leader) add = (unsigned)__popc(peers & eq);
+        else if (!same) add = 1u;                 // hash collision inside the warp: insert on its own
         else continue;                            // counted by the leader
         const unsigned long long tag = (h >> 31) << 31;                     // top 33 bits
         const unsigned long long mine = tag | (unsigned long long)i;        // i < 2^31
-        unsigned long long s = splitmix64(h) & mask;
-        for (;;) {
-            unsigned long long cur = atomicCAS(slots + s, kEmptyKey, mine);
-            if (cur == kEmptyKey) { atomicAdd(counts + s, add); break; }
-            if ((cur >> 31) == (tag >> 31) && same_cell(chars, offsets, i, (long long)(cur & 0x7FFFFFFFull))) {
-                atomicAdd(counts + s, add);
-                break;
+        const unsigned start = (unsigned)splitmix64(h);
+        bool staged = false;
+        if (*(volatile unsigned *)&st_spills < kStrStageBypass) {
+            for (int p = 0; p < kStrStageProbe; ++p) {
+                const int s = (int)((start + p) & (kStrStageSlots - 1));
+                // a slot only ever goes from empty to taken: a plain read skips taken slots without an atomic
+                unsigned long long cur = *(volatile unsigned long long *)(st_word + s);
+                if (cur == kEmptyKey) {
+                    cur = atomicCAS(st_word + s, kEmptyKey, mine);
+                    if (cur == kEmptyKey) st_hash[s] = h;                // read only after the loop's barrier
+                }
+                if (cur == kEmptyKey || ((cur >> 31) == (tag >> 31) && same_cell(chars, offsets, i, (long long)(cur & 0x7FFFFFFFull)))) {
+                    atomicAdd(st_count + s, add);
+                    staged = true;
+                    break;
+                }
             }
-            s = (s + 1) & mask;
+            if (!staged) atomicAdd(&st_spills, 1u);
         }
+        if (!staged) str_table_add(chars, offsets, slots, counts, mask, h, mine, add);   // spill
+    }
+    __syncthreads();
+    for (int s = threadIdx.x; s < kStrStageSlots; s += blockDim.x) {
+        const unsigned long long w = st_word[s];
+        if (w != kEmptyKey) str_table_add(chars, offsets, slots, counts, mask, st_hash[s], w, st_count[s]);
     }
 }
 

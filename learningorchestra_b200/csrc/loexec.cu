@@ -1359,7 +1359,36 @@ int value_counts_tail(HostCall &c, int64_t n, void *keys_out, uint64_t *counts_o
     return LO_OK;
 }
 
+// value_counts_tail of a text column already on the device (offsets[0] == 0; validity as k_hash_count_str reads it):
+// the call of lo_value_counts_str_host after its copies, and all of lo_value_counts_text.
+int value_counts_str_tail(HostCall &c, const uint8_t *d_chars, const long long *d_off, const uint8_t *d_mask,
+                          const uint8_t *d_bitmap, int bit0, int64_t n, int64_t *rep_rows_out, uint64_t *counts_out,
+                          int64_t capacity, int64_t *ndistinct, lo_host_timing *timing) {
+    return value_counts_tail(c, n, rep_rows_out, counts_out, capacity, ndistinct, timing,
+        [&](unsigned long long *slots_keys, unsigned long long *counts, unsigned long long slots, unsigned long long *out, size_t out_n) {
+            const int grid = (int)std::min<int64_t>((n + 255) / 256, (int64_t)c.ctx->sm_count * 8);
+            lo::k_hash_count_str<<<grid, 256, 0, c.s>>>(d_chars, d_off, n, d_mask, d_bitmap, bit0, slots_keys, counts, slots - 1);
+            lo::k_hash_compact_str<<<c.ctx->sm_count * 8, 256, 0, c.s>>>(slots_keys, counts, slots, (long long *)out, out + out_n,
+                                                                          (unsigned long long)capacity, out + 2 * out_n);
+        });
+}
+
 }  // namespace
+
+static_assert(lo::kStrStageSlots == LO_TEXT_STAGE_SLOTS, "loexec.h documents the text group-by's stage size");
+
+// one text column resident in HBM (lo_text_upload): chars, offsets rebased to 0, the validity as it was given (n mask
+// bytes, or the bitmap bytes covering the column with the first cell at bit bit0), all from the stream-ordered pool
+struct lo_text {
+    lo_ctx *ctx;
+    uint8_t *chars;
+    long long *offsets;
+    uint8_t *valid;
+    bool mask;
+    int bit0;
+    int64_t n, nbytes, nulls;
+    size_t device_bytes;
+};
 
 extern "C" {
 
@@ -1459,13 +1488,101 @@ int lo_value_counts_str_host(lo_ctx *ctx, const uint8_t *chars, const int64_t *o
     c.alloc(&d_off, (size_t)(n + 1) * 8);
     c.to_dev(d_chars, chars, (size_t)nbytes);
     c.to_dev(d_off, offsets, (size_t)(n + 1) * 8);
-    return value_counts_tail(c, n, rep_rows_out, counts_out, capacity, ndistinct, timing,
-        [&](unsigned long long *slots_keys, unsigned long long *counts, unsigned long long slots, unsigned long long *out, size_t out_n) {
-            const int grid = (int)std::min<int64_t>((n + 255) / 256, (int64_t)ctx->sm_count * 8);
-            lo::k_hash_count_str<<<grid, 256, 0, c.s>>>(d_chars, d_off, n, slots_keys, counts, slots - 1);
-            lo::k_hash_compact_str<<<ctx->sm_count * 8, 256, 0, c.s>>>(slots_keys, counts, slots, (long long *)out, out + out_n,
-                                                                        (unsigned long long)capacity, out + 2 * out_n);
-        });
+    return value_counts_str_tail(c, d_chars, d_off, nullptr, nullptr, 0, n, rep_rows_out, counts_out, capacity, ndistinct,
+                                 timing);
+}
+
+// ---- text columns resident in HBM ---------------------------------------------------------------------------------
+int lo_text_upload(lo_ctx *ctx, const uint8_t *chars, const int64_t *offsets, const lo_validity *validity, int64_t n,
+                   lo_text **out, lo_host_timing *timing) {
+    LO_TRY(check_ctx(ctx));
+    if (!out) return fail(LO_ERR_INVALID, "out is NULL");
+    *out = nullptr;
+    if (n < 0) return fail(LO_ERR_INVALID, "n < 0");
+    if (n > 0x7fffffffll) return fail(LO_ERR_INVALID, "at most 2^31-1 rows per column");
+    if (!offsets) return fail(LO_ERR_INVALID, "offsets is NULL");
+    const int64_t nbytes = offsets[n] - offsets[0];
+    if (nbytes < 0 || (nbytes > 0 && !chars)) return fail(LO_ERR_INVALID, "bad offsets / chars");
+    for (int64_t i = 0; i < n; ++i)
+        if (offsets[i + 1] < offsets[i]) return fail(LO_ERR_INVALID, "offsets must be non-decreasing (row %lld)", (long long)i);
+    if (validity && validity->mask && validity->bitmap) return fail(LO_ERR_INVALID, "validity: mask or bitmap, not both");
+    if (validity && validity->bitmap && validity->bit_offset < 0) return fail(LO_ERR_INVALID, "validity: bit_offset < 0");
+    const bool has_mask = validity && validity->mask && n > 0, has_bitmap = validity && validity->bitmap && n > 0;
+    const int64_t first = has_bitmap ? validity->bit_offset >> 3 : 0;
+    const size_t valid_bytes = has_mask ? (size_t)n : has_bitmap ? (size_t)(((validity->bit_offset + n - 1) >> 3) - first + 1) : 0;
+    const size_t need = (size_t)std::max<int64_t>(nbytes, 1) + (size_t)(n + 1) * 8 + valid_bytes;
+    size_t free_b = 0, total_b = 0;
+    const cudaError_t e = cudaMemGetInfo(&free_b, &total_b);
+    if (e != cudaSuccess) return fail(LO_ERR_CUDA, "cudaMemGetInfo: %s", cudaGetErrorString(e));
+    if (need > free_b)
+        return fail(LO_ERR_NOMEM, "text_upload: the column needs %zu bytes of device memory, %zu are free", need, free_b);
+    int64_t nulls = 0;                       // counted here: the host holds the validity already
+    if (has_mask) {
+        for (int64_t i = 0; i < n; ++i) nulls += validity->mask[i] == 0;
+    } else if (has_bitmap) {
+        for (int64_t i = 0; i < n; ++i) {
+            const int64_t b = validity->bit_offset + i;
+            nulls += ((validity->bitmap[b >> 3] >> (b & 7)) & 1) == 0;
+        }
+    }
+    std::unique_ptr<lo_text> t(new (std::nothrow) lo_text);
+    if (!t) return fail(LO_ERR_NOMEM, "out of host memory");
+    *t = lo_text{ctx, nullptr, nullptr, nullptr, has_mask, has_bitmap ? (int)(validity->bit_offset & 7) : 0, n, nbytes, nulls, need};
+    HostCall c(ctx, "text_upload");
+    c.alloc(&t->chars, (size_t)nbytes);
+    c.alloc(&t->offsets, (size_t)(n + 1) * 8);
+    if (valid_bytes) c.alloc(&t->valid, valid_bytes);
+    c.to_dev(t->chars, chars + offsets[0], (size_t)nbytes);
+    std::vector<int64_t> rel;                // the offsets of a sliced Arrow array, rebased to 0
+    const int64_t *off_src = offsets;
+    if (offsets[0] != 0) {
+        rel.resize(n + 1);
+        for (int64_t i = 0; i <= n; ++i) rel[i] = offsets[i] - offsets[0];
+        off_src = rel.data();
+    }
+    c.to_dev(t->offsets, off_src, (size_t)(n + 1) * 8);
+    if (has_mask) c.to_dev(t->valid, validity->mask, valid_bytes);
+    if (has_bitmap) c.to_dev(t->valid, validity->bitmap + first, valid_bytes);
+    c.keep(t->chars);
+    c.keep(t->offsets);
+    if (t->valid) c.keep(t->valid);
+    LO_TRY(c.finish(timing));                // synchronises: the host buffers (and `rel`) may go
+    *out = t.release();
+    return LO_OK;
+}
+
+int lo_text_info(const lo_text *t, int64_t *n, int64_t *nbytes, int64_t *nulls, size_t *device_bytes) {
+    if (!t) return fail(LO_ERR_INVALID, "text is NULL");
+    if (n) *n = t->n;
+    if (nbytes) *nbytes = t->nbytes;
+    if (nulls) *nulls = t->nulls;
+    if (device_bytes) *device_bytes = t->device_bytes;
+    return LO_OK;
+}
+
+int lo_text_free(lo_ctx *ctx, lo_text *t) {
+    if (!t) return LO_OK;
+    LO_TRY(check_ctx(ctx));
+    if (t->ctx != ctx) return fail(LO_ERR_INVALID, "text belongs to another context");
+    for (void *p : {(void *)t->chars, (void *)t->offsets, (void *)t->valid})
+        if (p) cudaFreeAsync(p, ctx->stream);
+    delete t;
+    return LO_OK;
+}
+
+int lo_value_counts_text(lo_ctx *ctx, const lo_text *t, int64_t *rep_rows_out, uint64_t *counts_out, int64_t capacity,
+                         int64_t *ndistinct, lo_host_timing *timing) {
+    LO_TRY(check_ctx(ctx));
+    if (!t) return fail(LO_ERR_INVALID, "text is NULL");
+    if (t->ctx != ctx) return fail(LO_ERR_INVALID, "text belongs to another context");
+    if (capacity < 0) return fail(LO_ERR_INVALID, "negative size");
+    if (!ndistinct) return fail(LO_ERR_INVALID, "ndistinct is NULL");
+    *ndistinct = 0;
+    if (t->n == t->nulls) return LO_OK;      // no cell to count (n == 0 included)
+    if (capacity > 0 && (!rep_rows_out || !counts_out)) return fail(LO_ERR_INVALID, "NULL argument");
+    HostCall c(ctx, "value_counts_text");
+    return value_counts_str_tail(c, t->chars, t->offsets, t->mask ? t->valid : nullptr, t->mask ? nullptr : t->valid,
+                                 t->bit0, t->n, rep_rows_out, counts_out, capacity, ndistinct, timing);
 }
 
 // text -> number for one column of cells (R-semantics "number" cast).  chars: all cells back to back;

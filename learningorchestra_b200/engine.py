@@ -278,6 +278,29 @@ class DeviceTable:
             pass
 
 
+class DeviceText:
+    """One text column resident in HBM (``lo_text_upload``): chars, offsets and validity on the device, and ``arr``, the
+    Arrow ``large_string`` array it was made from, which the group keys are read from (``arr.take(rep_rows)``).
+    ``n`` cells, ``nulls`` of them null, ``nbytes`` device bytes held."""
+
+    def __init__(self, engine: "Engine", handle: C.c_void_p, arr):
+        self.engine, self._h, self.arr = engine, handle, arr
+        n, chars, nulls, dev = C.c_int64(), C.c_int64(), C.c_int64(), C.c_size_t()
+        N.check(engine._lib.lo_text_info(handle, C.byref(n), C.byref(chars), C.byref(nulls), C.byref(dev)))
+        self.n, self.chars, self.nulls, self.nbytes = n.value, chars.value, nulls.value, dev.value
+
+    def free(self) -> None:
+        if self._h is not None and self.engine._ctx is not None:
+            N.check(self.engine._lib.lo_text_free(self.engine._ctx, self._h))
+        self._h = None
+
+    def __del__(self):
+        try:
+            self.free()
+        except Exception:
+            pass
+
+
 class Engine:
     """One libloexec context = one H100.  ``Engine(device)`` raises LoexecError without a GPU."""
 
@@ -650,6 +673,45 @@ class Engine:
         return _value_counts(lambda rows, counts, cap, nd: self._lib.lo_value_counts_str_host(
             self._ctx, chars.ctypes.data_as(C.c_void_p), offsets.ctypes.data_as(C.c_void_p), n, rows, counts, cap, nd, None),
             n, np.int64)
+
+    def text(self, cells, timing: dict | None = None) -> DeviceText:
+        """A text column uploaded to HBM once for repeated counting: ``cells`` is an Arrow string array (its buffers go
+        up as they are: a slice, nulls and any bit offset included) or a list of ``str`` / None (None = null).  Raises
+        LoexecError LO_ERR_NOMEM when the device has too little free memory.  ``timing``: a dict to receive the call's
+        lo_host_timing fields."""
+        import pyarrow as pa
+        from .columnar import text_buffers
+        arr = cells if isinstance(cells, (pa.Array, pa.ChunkedArray)) else pa.array(cells, type=pa.large_string())
+        if isinstance(arr, pa.ChunkedArray):
+            arr = arr.combine_chunks() if arr.num_chunks != 1 else arr.chunk(0)
+        if not pa.types.is_large_string(arr.type):
+            arr = arr.cast(pa.large_string())
+        chars, offsets, validity = text_buffers(arr)
+        v = N.Validity()
+        if validity is not None:
+            v.bitmap, v.bit_offset = validity[0].ctypes.data, int(validity[1])
+        h, t = C.c_void_p(), N.HostTiming()
+        N.check(self._lib.lo_text_upload(self._ctx, chars.ctypes.data_as(C.c_void_p), offsets.ctypes.data_as(C.c_void_p),
+                                         C.byref(v), len(arr), C.byref(h), C.byref(t)))
+        if timing is not None:
+            timing.update(_timing(t), kernel_ms=t.kernel_ms)
+        return DeviceText(self, h, arr)
+
+    def value_counts_text(self, text: DeviceText, timing: dict | None = None):
+        """(rep_rows int64[g], counts uint64[g]) of a resident text column (``lo_value_counts_text``): one
+        representative row per distinct non-null cell, indexing the whole column, and the group sizes; null cells are
+        not counted and no cell crosses PCIe.  ``timing``: a dict to receive the (last) call's lo_host_timing fields."""
+        if text._h is None:
+            raise ValueError("the text column has been freed")
+        n = text.n - text.nulls
+        if n == 0:
+            return np.zeros(0, np.int64), np.zeros(0, np.uint64)
+        t = N.HostTiming()
+        out = _value_counts(lambda rows, counts, cap, nd: self._lib.lo_value_counts_text(
+            self._ctx, text._h, rows, counts, cap, nd, C.byref(t)), n, np.int64)
+        if timing is not None:
+            timing.update(_timing(t), kernel_ms=t.kernel_ms)
+        return out
 
     def value_counts_f64_host(self, values: np.ndarray):
         """(keys float64[g], counts uint64[g]) — exact value counts of a numeric column (GPU hash group-by),

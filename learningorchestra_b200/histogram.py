@@ -9,11 +9,16 @@ Here the counting runs on the GPU with no host dictionary:
 
 * number fields (every value an int / float / None): GPU hash group-by on the binary64 keys
   (``lo_value_counts_f64_host``; -0.0 == 0.0, NaN == NaN as in MongoDB);
-* text fields (every value a ``str`` / None): GPU hash group-by on the cells' bytes (``lo_value_counts_str_host``);
-* mixed-type fields: the same byte-wise group-by over a tagged encoding under which two cells are equal exactly
-  when MongoDB groups them (:func:`columnar.tagged_cell`: 1 == 1.0, ``True`` != 1, ``"1"`` != 1).
+* text fields (every value a ``str`` / None — every field of a fresh ``POST /files`` upload): GPU hash group-by on the
+  cells' bytes over the field's text column kept resident in HBM (``table_cache``, ``lo_value_counts_text``), leased
+  for the request.  The first request uploads the column; later ones copy no cell to the device and read no document.
+  Group keys are read from the host's Arrow array at the representative rows; the ``null`` group is the column's null
+  cells plus the documents that are not data rows (the metadata document);
+* mixed-type fields: the byte-wise group-by over a tagged encoding under which two cells are equal exactly
+  when MongoDB groups them (:func:`columnar.tagged_cell`: 1 == 1.0, ``True`` != 1, ``"1"`` != 1), packed per request
+  (``lo_value_counts_str_host``).
 
-``None`` / missing values (the metadata document among them) are counted while packing.  With ``bins`` (optional
+``None`` / missing values of number and mixed fields are counted while packing.  With ``bins`` (optional
 extension, REST keys ``bins`` / ``range``) the fields must be numeric or text (text is parsed with ``float()`` on the
 device into the resident slab; the dataset stays text) and get the fixed-width B-semantics histogram of SURVEY.md §8c
 from the fused kernel, run on the HBM-resident copy of the dataset (``table_cache``).
@@ -29,6 +34,17 @@ import numpy as np
 
 from . import columnar
 from .utils import record_exception
+
+
+def text_groups(arr, rep, counts, none_count):
+    """Result groups of a text field counted on the device: the key of each group is the cell at its representative row
+    of ``arr`` (the whole column, nulls included), then the ``null`` group of ``none_count`` null / missing cells."""
+    import pyarrow as pa
+    keys = arr.take(pa.array(np.asarray(rep, dtype=np.int64))).to_pylist() if len(rep) else []
+    groups = [{"_id": k, "count": int(c)} for k, c in zip(keys, counts)]
+    if none_count:
+        groups.append({"_id": None, "count": int(none_count)})
+    return groups
 
 
 class Histogram:
@@ -57,12 +73,15 @@ class Histogram:
                 raise RuntimeError("Histogram needs an Engine: the counting has no CPU fallback")
             if bins:
                 results = self.__binned(parent_filename, fields, int(bins), value_range)
-            elif getattr(self.database_connector, "has_columns", lambda _f: False)(parent_filename):
-                results = self.__value_counts_columnar(parent_filename, fields)
             else:
-                # unfiltered, like $group; materialised once (a pymongo Cursor can be walked only once)
-                documents = list(self.database_connector.find(parent_filename, {}))
-                results = self.__value_counts(documents, fields)
+                results = self.__value_counts_resident_text(parent_filename, fields)
+                rest = [f for f in fields if f not in results]
+                if rest and getattr(self.database_connector, "has_columns", lambda _f: False)(parent_filename):
+                    results.update(self.__value_counts_columnar(parent_filename, rest))
+                elif rest:
+                    # unfiltered, like $group; materialised once (a pymongo Cursor can be walked only once)
+                    documents = list(self.database_connector.find(parent_filename, {}))
+                    results.update(self.__value_counts(documents, rest))
             document_id = 1
             for field in fields:
                 self.database_connector.insert_one_in_file(
@@ -74,6 +93,22 @@ class Histogram:
             raise
 
     # ---- R-semantics: exact value counts -------------------------------------------------------------
+    def __value_counts_resident_text(self, parent_filename, fields):
+        """``$group`` of the fields that are text in the store, from their columns resident in HBM (``table_cache``),
+        under a lease: the cells cross PCIe when the column is first made resident, not on every request.  Returns the
+        groups of those fields only; the others (number, mixed-type, all null) are left to the host-packing routes."""
+        resident = getattr(self.engine, "resident", None)
+        if resident is None or getattr(self.engine, "value_counts_text", None) is None:
+            return {}
+        results = {}
+        with resident.lease(self.database_connector, parent_filename, (), text=fields) as data:
+            for f in fields:
+                text = data.texts.get(f)
+                if text is not None and f not in results:
+                    rep, counts = self.engine.value_counts_text(text)
+                    results[f] = text_groups(text.arr, rep, counts, text.nulls + data.absent[f])
+        return results
+
     def __value_counts(self, documents, fields):
         results = {}
         for f in fields:

@@ -519,6 +519,12 @@ class ShardedEngine:
     def value_counts_str_host(self, cells):
         return self.engines[0].value_counts_str_host(cells)
 
+    def text(self, cells, timing=None):
+        return self.engines[0].text(cells, timing)
+
+    def value_counts_text(self, text, timing=None):
+        return self.engines[0].value_counts_text(text, timing)
+
     @property
     def resident(self):
         """Datasets kept in HBM between requests, rows sharded over the group (:mod:`table_cache`)."""

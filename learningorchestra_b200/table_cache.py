@@ -12,9 +12,16 @@ Text fields (every dataset arrives as text) are parsed on the device straight in
 needs no ``/fieldTypes`` job first, and the dataset is never modified.  The slab equals the one ``/fieldTypes
 "number"`` would have led to, bit for bit.
 
+Text columns are kept as text too, next to the slabs in the same :class:`ResidentDataset`, for the ``$group`` of
+``/histograms`` without ``bins`` (``Engine.text`` / ``lo_text_upload``): a column-store text column's Arrow buffers go
+up as they are, a document-store text field's cells with None as null.  Such a column is never parsed, so a field of
+words (``Sex``) is kept and counted like any other; the host keeps the Arrow array to read the group keys from, and the
+entry records how many documents that are not data rows (the metadata document) lack the field — the ``null`` group.
+
 Staleness: the in-process :class:`~learningorchestra_b200.utils.Database` bumps ``version(filename)`` on every
-write to data rows; a cached table is used only while its version matches.  A ``Database`` without
-``version`` (foreign object) is never cached.  Eviction: least recently used beyond ``max_bytes``.
+write to data rows (a ``/fieldTypes`` job included); a cached entry is used only while its version matches, and the
+next request rebuilds it.  A ``Database`` without ``version`` (foreign object) is never cached: its entry is freed when
+the request's lease ends.  Eviction: least recently used beyond ``max_bytes``, slabs and text columns counted together.
 """
 from __future__ import annotations
 
@@ -27,15 +34,34 @@ from . import columnar
 
 
 class ResidentDataset:
-    def __init__(self, version, ids, fields, kinds, nulls, table):
+    """One dataset's resident device objects.  An entry rebuilt at the same version shares the objects it does not
+    change with its predecessor (each object counts the entries holding it, ``holders``) and a device object is freed
+    with the last entry that holds it, so a lease on either entry keeps everything it reads alive."""
+
+    def __init__(self, version, ids, fields, kinds, nulls, table, texts=None, absent=None):
         self.version, self.ids, self.fields, self.kinds, self.nulls, self.table = version, ids, fields, kinds, nulls, table
         self.column = {f: i for i, f in enumerate(fields)}
+        # text columns kept as text for $group: field -> DeviceText, or None for a field that was checked and is not a
+        # text field (number, mixed, all null, or set on a document that is not a data row)
+        self.texts = dict(texts or {})
+        self.absent = dict(absent or {})   # text field -> documents that are not data rows and lack it (null group)
         self.users = 0          # leases handed out and not yet released (guarded by ResidentTables._lock)
         self.retired = False    # dropped from the cache: freed when the last user releases it
+        for obj in self._objects():
+            obj.holders = getattr(obj, "holders", 0) + 1
+
+    def _objects(self):
+        return [o for o in [self.table, *self.texts.values()] if o is not None]
 
     @property
     def nbytes(self) -> int:
-        return self.table.pitch_bytes * self.table.ncols
+        return self.table.pitch_bytes * self.table.ncols + sum(t.nbytes for t in self.texts.values() if t is not None)
+
+    def free(self) -> None:
+        for obj in self._objects():
+            obj.holders -= 1
+            if obj.holders <= 0:
+                obj.free()
 
 
 def device_number_column(values: np.ndarray, valid: np.ndarray, is_int: np.ndarray):
@@ -82,14 +108,14 @@ class ResidentTables:
         self._lock = threading.RLock()
         self.hits = self.misses = 0
 
-    def lease(self, database, filename: str, fields):
-        """``with resident.lease(db, name, fields) as data:`` — the table cannot be freed (version bump, eviction,
-        invalidate, another job's rebuild) while the block runs GPU work on it."""
+    def lease(self, database, filename: str, fields, text=()):
+        """``with resident.lease(db, name, fields, text) as data:`` — the table and the text columns cannot be freed
+        (version bump, eviction, invalidate, another job's rebuild) while the block runs GPU work on them."""
         cache = self
 
         class _Lease:
             def __enter__(self_inner):
-                self_inner.data = cache.ensure(database, filename, fields)
+                self_inner.data = cache.ensure(database, filename, fields, text)
                 return self_inner.data
 
             def __exit__(self_inner, *exc):
@@ -100,39 +126,67 @@ class ResidentTables:
         with self._lock:
             entry.users -= 1
             if entry.retired and entry.users <= 0:
-                entry.table.free()
+                entry.free()
 
     def _retire(self, entry: ResidentDataset) -> None:
         """Called with the lock held: free now if nobody uses the table, else when the last lease ends."""
         entry.retired = True
         if entry.users <= 0:
-            entry.table.free()
+            entry.free()
 
-    def ensure(self, database, filename: str, fields) -> ResidentDataset:
+    def ensure(self, database, filename: str, fields, text=()) -> ResidentDataset:
         """Resident table holding (at least) ``fields`` of ``filename``; built from the documents on a miss.
         A field may be numeric or text (a column-store text column, or document values that are all ``str`` / None):
         text is parsed on the device into its slab, the dataset itself stays text.  Raises ValueError if a requested
-        field is neither, or names the first cell ``float()`` rejects; on any failure nothing is cached.  The returned
-        entry is LEASED: pair every call with :meth:`release` (or use :meth:`lease`)."""
+        field is neither, or names the first cell ``float()`` rejects; on any failure nothing is cached.
+
+        ``text``: fields to keep as text columns for counting (``entry.texts``), never parsed.  A field that is not a
+        text field there is recorded as None and raises nothing: its caller takes another route.  The returned entry is
+        LEASED: pair every call with :meth:`release` (or use :meth:`lease`)."""
         version = database.version(filename) if hasattr(database, "version") else None
         with self._lock:
             entry = self._entries.get(filename)
-            if entry is not None and version is not None and entry.version == version and all(f in entry.column for f in fields):
+            if entry is not None and version is not None and entry.version == version and \
+                    all(f in entry.column for f in fields) and all(f in entry.texts for f in text):
                 self._entries.move_to_end(filename)
                 self.hits += 1
                 entry.users += 1
                 return entry
             self.misses += 1
-            keep = [f for f in (entry.fields if entry is not None and entry.version == version else []) if f not in fields]
-            wanted = list(fields) + keep
+            # the same version: what the entry already holds is shared with its successor, not built again — the
+            # slabs when no new number field is asked for, the text columns always
+            same = entry is not None and entry.version == version
+            share_table = same and all(f in entry.column for f in fields)
+            keep = [f for f in (entry.fields if same else []) if f not in fields]
+            wanted = [] if share_table else list(fields) + keep
+            texts = dict(entry.texts) if same else {}
+            absent = dict(entry.absent) if same else {}
+            wanted_text = [f for f in dict.fromkeys(text) if f not in texts]
             columnar_rows = getattr(database, "has_columns", lambda _f: False)(filename)
-            if columnar_rows:            # rows already stored as columns (column_store): no document is touched
+            if share_table and not wanted_text:
+                rows = row_ids = entry.ids
+            elif columnar_rows:          # rows already stored as columns (column_store): no document is touched
                 row_ids = database.row_ids(filename)
                 rows = row_ids
+                others = database.other_documents(filename) if wanted_text else []
             else:
-                rows = columnar.data_rows(database.find(filename, {}))
+                documents = list(database.find(filename, {}))
+                rows = columnar.data_rows(documents)
+                others = [d for d in documents if d.get("_id") == columnar.METADATA_DOCUMENT_ID]
                 rows.sort(key=lambda d: d["_id"])
                 row_ids = np.array([d["_id"] for d in rows], dtype=np.int64)
+            text_sources = {}
+            for f in wanted_text:
+                src = None
+                if not any(d.get(f) is not None for d in others):
+                    if columnar_rows:
+                        c = database.column(filename, f)
+                        src = c.arr if c is not None and c.kind == "text" else None
+                    else:
+                        values = [d.get(f) for d in rows]
+                        src = values if is_text_field(values) else None
+                text_sources[f] = src
+                absent[f] = sum(1 for d in others if d.get(f) is None)
             sources, names = [], []          # per resident column: ("number", packed) or ("text", cells)
             for f in wanted:
                 if columnar_rows:
@@ -155,8 +209,11 @@ class ResidentTables:
                         raise ValueError(f"field {f!r} is not numeric; run /fieldTypes first")
                     continue                 # a previously resident column that stopped being numeric: drop it
                 names.append(f); sources.append(src)
-            table = self.engine.table("f64", len(rows) if sources else 0, max(len(sources), 1))
-            kinds, nulls = [], []
+            if share_table:
+                table, names, kinds, nulls = entry.table, entry.fields, entry.kinds, entry.nulls
+            else:
+                table, kinds, nulls = self.engine.table("f64", len(rows) if sources else 0, max(len(sources), 1)), [], []
+            made = {}
             try:
                 for j, (how, src) in enumerate(sources):
                     if how == "number":
@@ -167,10 +224,13 @@ class ResidentTables:
                     else:
                         kind, n_null = parse_text_column(self.engine, table, j, src)
                         kinds.append(kind); nulls.append(n_null)
+                for f, src in text_sources.items():
+                    made[f] = self.engine.text(src) if src is not None else None
             except BaseException:
-                table.free()                 # a bad cell: nothing of the partly built table stays, nothing is cached
+                # a bad cell: nothing built by this call stays, nothing is cached
+                ResidentDataset(version, row_ids, [], [], [], None if share_table else table, made).free()
                 raise
-            new = ResidentDataset(version, row_ids, names, kinds, nulls, table)
+            new = ResidentDataset(version, row_ids, names, kinds, nulls, table, {**texts, **made}, absent)
             new.users = 1
             if entry is not None:
                 self._entries.pop(filename, None)
