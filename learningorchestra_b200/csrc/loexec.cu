@@ -457,24 +457,21 @@ int launch_f64_bins(lo_ctx *ctx, const lo_table *in, const lo_table *out, int32_
     return LO_OK;
 }
 
-int project_cast_hist_impl(lo_ctx *ctx, const lo_table *in, const int32_t *col_idx, int32_t k,
-                           lo_table *out, const lo_hist_spec *spec, uint64_t *counts_dev, cudaStream_t s,
-                           const lo::GroupStep *group = nullptr) {
+// the argument checks of project_cast_hist_impl, which enqueue nothing; w receives the bin widths when there is a spec
+int check_project_cast_hist(const lo_table *in, const int32_t *col_idx, int32_t k, const lo_table *out,
+                            const lo_hist_spec *spec, const uint64_t *counts_dev, bool group, std::vector<float> &w) {
     if (!in) return fail(LO_ERR_INVALID, "input table is NULL");
     if (in->dtype != LO_F64) return fail(LO_ERR_INVALID, "input table must be LO_F64 (got dtype %d)", in->dtype);
     LO_TRY(check_cols(in, col_idx, k));
-    int out_mode = 0;
     if (out) {
-        if (out->dtype == LO_F32) out_mode = 1;
-        else if (out->dtype == LO_F64) out_mode = 2;
-        else return fail(LO_ERR_INVALID, "output table must be LO_F32 or LO_F64 (got dtype %d)", out->dtype);
+        if (out->dtype != LO_F32 && out->dtype != LO_F64)
+            return fail(LO_ERR_INVALID, "output table must be LO_F32 or LO_F64 (got dtype %d)", out->dtype);
         if (out->nrows != in->nrows) return fail(LO_ERR_INVALID, "output rows %lld != input rows %lld",
                                                   (long long)out->nrows, (long long)in->nrows);
         if (out->ncols < k) return fail(LO_ERR_INVALID, "output has %d columns, need %d", out->ncols, k);
         if (out->device != in->device) return fail(LO_ERR_INVALID, "tables live on different devices");
     }
     if (!out && !spec) return fail(LO_ERR_INVALID, "nothing to do: no output table and no histogram spec");
-    std::vector<float> w;
     if (spec) {
         if (!counts_dev) return fail(LO_ERR_INVALID, "counts_dev is NULL");
         w.resize(k);
@@ -482,7 +479,16 @@ int project_cast_hist_impl(lo_ctx *ctx, const lo_table *in, const int32_t *col_i
     }
     if (group && (!spec || k > lo::kMaxColsF64))
         return fail(LO_ERR_INVALID, "a group step needs a histogram spec and k <= %d (got %d)", lo::kMaxColsF64, k);
+    return LO_OK;
+}
+
+int project_cast_hist_impl(lo_ctx *ctx, const lo_table *in, const int32_t *col_idx, int32_t k,
+                           lo_table *out, const lo_hist_spec *spec, uint64_t *counts_dev, cudaStream_t s,
+                           const lo::GroupStep *group = nullptr) {
+    std::vector<float> w;
+    LO_TRY(check_project_cast_hist(in, col_idx, k, out, spec, counts_dev, group != nullptr, w));
     if (in->nrows == 0 && !group) return LO_OK;
+    const int out_mode = !out ? 0 : out->dtype == LO_F32 ? 1 : 2;
     const bool aligned = aligned32(in) && (!out || aligned32(out));
     const lo::GroupStep &G = group ? *group : kNoGroup;
 
@@ -515,13 +521,19 @@ int project_cast_hist_impl(lo_ctx *ctx, const lo_table *in, const int32_t *col_i
     return LO_OK;
 }
 
-int hist_u8_impl(lo_ctx *ctx, const lo_table *in, const int32_t *col_idx, int32_t k,
-                 uint64_t *counts_dev, cudaStream_t s, const lo::GroupStep *group = nullptr) {
+// the argument checks of hist_u8_impl, which enqueue nothing
+int check_hist_u8(const lo_table *in, const int32_t *col_idx, int32_t k, const uint64_t *counts_dev, bool group) {
     if (!in) return fail(LO_ERR_INVALID, "input table is NULL");
     if (in->dtype != LO_U8) return fail(LO_ERR_INVALID, "input table must be LO_U8 (got dtype %d)", in->dtype);
     LO_TRY(check_cols(in, col_idx, k));
     if (!counts_dev && !group) return fail(LO_ERR_INVALID, "counts_dev is NULL");
     if (group && k > lo::kMaxColsU8) return fail(LO_ERR_INVALID, "a group step takes k <= %d byte columns (got %d)", lo::kMaxColsU8, k);
+    return LO_OK;
+}
+
+int hist_u8_impl(lo_ctx *ctx, const lo_table *in, const int32_t *col_idx, int32_t k,
+                 uint64_t *counts_dev, cudaStream_t s, const lo::GroupStep *group = nullptr) {
+    LO_TRY(check_hist_u8(in, col_idx, k, counts_dev, group != nullptr));
     if (in->nrows == 0 && !group) return LO_OK;
     const lo::GroupStep &G = group ? *group : kNoGroup;
     const bool aligned = ((uintptr_t)in->base % 16 == 0) && (in->pitch % 16 == 0);
