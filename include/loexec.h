@@ -43,7 +43,7 @@
 extern "C" {
 #endif
 
-#define LO_ABI_VERSION 6
+#define LO_ABI_VERSION 7
 
 #define LO_OK                    0
 #define LO_ERR_INVALID          -1   /* bad argument (message says which)              */
@@ -294,6 +294,17 @@ int lo_value_counts_u32_host(lo_ctx *ctx, const uint32_t *codes, int64_t nrows, 
 int lo_value_counts_f64_host(lo_ctx *ctx, const double *values, int64_t n, double *keys_out,
                              uint64_t *counts_out, int64_t capacity, int64_t *ndistinct,
                              lo_host_timing *timing);
+/* The same on rows [0, nrows) of column `col` of a device table (LO_F64), e.g. a dataset's slab kept in HBM for
+ * repeated `$group` requests: nothing crosses PCIe but the groups (h2d_bytes 0), two kernel launches.  A null stored as
+ * NaN in the slab counts under the NaN key: the caller, which knows its nulls, separates them from real NaNs.
+ * LO_ERR_INVALID before anything is enqueued for a NULL table, a table that is not LO_F64 or lives on another
+ * context's device, `col` outside [0, ncols), or NULL outputs with capacity > 0.  Not `_dev`: it synchronises and
+ * writes host arrays.  Both calls run one binary64 group-by kernel: warp-merged keys are staged in a per-CTA
+ * shared-memory table before the global one (16-byte loads when the column is 16-byte aligned, as every slab of
+ * lo_table_alloc is). */
+int lo_value_counts_f64_table(lo_ctx *ctx, const lo_table *t, int32_t col, double *keys_out,
+                              uint64_t *counts_out, int64_t capacity, int64_t *ndistinct,
+                              lo_host_timing *timing);
 
 /* The same for one TEXT column: cell i = chars[offsets[i] .. offsets[i+1]) (offsets[0] == 0, n < 2^31).  Keys are
  * compared byte for byte on the device (exact whatever the hash does).  rep_rows_out[g] = row index of one member

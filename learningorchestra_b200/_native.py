@@ -37,7 +37,7 @@ LO_FORMAT_MAX_CELL = 310
 LO_CSV_OK, LO_CSV_SHORT_ROW, LO_CSV_FIELD_LIMIT, LO_CSV_BAD_UTF8, LO_CSV_NUL, LO_CSV_UNSUPPORTED, LO_CSV_EMPTY = range(7)
 LO_CSV_STREAM_WINDOW = 64 << 20
 LO_TEXT_STAGE_SLOTS = 512
-LO_ABI_VERSION = 6
+LO_ABI_VERSION = 7
 
 _ERR_NAMES = {
     LO_ERR_INVALID: "LO_ERR_INVALID", LO_ERR_CUDA: "LO_ERR_CUDA", LO_ERR_NOMEM: "LO_ERR_NOMEM",
@@ -143,6 +143,7 @@ SIGNATURES = {
     "lo_ctx_bind_numa": (C.c_int, [_P, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
     "lo_value_counts_u32_host": (C.c_int, [_P, _P, C.c_int64, C.c_uint32, _P, C.POINTER(HostTiming)]),
     "lo_value_counts_f64_host": (C.c_int, [_P, _P, C.c_int64, _P, _P, C.c_int64, C.POINTER(C.c_int64), C.POINTER(HostTiming)]),
+    "lo_value_counts_f64_table": (C.c_int, [_P, _P, C.c_int32, _P, _P, C.c_int64, C.POINTER(C.c_int64), C.POINTER(HostTiming)]),
     "lo_value_counts_str_host": (C.c_int, [_P, _P, _P, C.c_int64, _P, _P, C.c_int64, C.POINTER(C.c_int64), C.POINTER(HostTiming)]),
     "lo_parse_number_host": (C.c_int, [_P, _P, _P, C.c_int64, _P, _P, C.POINTER(HostTiming)]),
     "lo_parse_number_to_table": (C.c_int, [_P, _P, _P, C.POINTER(Validity), C.c_int64, _P, C.c_int32, C.c_int64,

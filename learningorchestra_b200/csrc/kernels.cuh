@@ -28,7 +28,7 @@
 //     LDS.128, one comparison; edge_counter_offset), elsewhere without a divide (hoisted reciprocal + two FMA
 //     corrections; bin_index_f32) — both proven and exhaustively self-tested equal to the IEEE quotient.
 //   * also here: k_parse_number (CPython float() on the GPU, parse_number.cuh), k_format_number_len / _write (its
-//     inverse, CPython str(), format_number.cuh), k_hash_count_f64 / _str
+//     inverse, CPython str(), format_number.cuh), k_group_f64 / k_hash_count_str
 //     (exact group-by), k_minmax_cast, the group's small kernels (push, big-matrix merge, barrier), generators, checksum.
 #pragma once
 #include <cstdint>
@@ -1112,7 +1112,8 @@ __global__ void k_minmax_cast(const char *__restrict__ base, long long pitch, lo
 // ($group / $sum:1 of histogram_image/histogram.py:31-36 on number fields).  Keys are binary64 bit patterns
 // canonicalised to MongoDB's grouping equality for numbers (-0.0 == 0.0, NaN == NaN); open addressing with
 // linear probing in HBM, 64-bit CAS to claim a slot, RED.64 to count; equal keys inside a warp are merged
-// first (match.any) so a two-valued column does not serialise on two L2 addresses.
+// first (match.any) and then per CTA in a shared-memory stage, so a two-valued column does not serialise on two L2
+// addresses.
 // ---------------------------------------------------------------------------------------------
 constexpr unsigned long long kEmptyKey = 0xFFFFFFFFFFFFFFFFull;      // a NaN payload no canonical key can have
 
@@ -1122,23 +1123,107 @@ __device__ __forceinline__ unsigned long long canonical_key(double x) {
     return (unsigned long long)__double_as_longlong(x);
 }
 
-__global__ void k_hash_count_f64(const double *__restrict__ values, long long n, unsigned long long *__restrict__ keys,
-                                 unsigned long long *__restrict__ counts, unsigned long long mask) {
-    for (long long i0 = blockIdx.x * (long long)blockDim.x; i0 < n; i0 += (long long)gridDim.x * blockDim.x) {
-        const long long i = i0 + threadIdx.x;
-        const bool live = i < n;
-        const unsigned active = __ballot_sync(0xffffffffu, live);
-        if (!live) continue;
-        const unsigned long long key = canonical_key(values[i]);
-        const unsigned peers = __match_any_sync(active, key);
-        if ((int)(threadIdx.x & 31) != __ffs(peers) - 1) continue;      // one lane per distinct key in the warp
-        const unsigned long long add = (unsigned long long)__popc(peers);
-        unsigned long long h = splitmix64(key) & mask;
-        for (;;) {
-            const unsigned long long old = atomicCAS(keys + h, kEmptyKey, key);
-            if (old == kEmptyKey || old == key) { atomicAdd(counts + h, add); break; }
-            h = (h + 1) & mask;
+// Add `add` rows to the group of canonical key `key` in the global table.
+__device__ __forceinline__ void f64_table_add(unsigned long long *keys, unsigned long long *counts, unsigned long long mask,
+                                              unsigned long long key, unsigned long long add) {
+    unsigned long long h = splitmix64(key) & mask;
+    for (;;) {
+        const unsigned long long old = atomicCAS(keys + h, kEmptyKey, key);
+        if (old == kEmptyKey || old == key) { atomicAdd(counts + h, add); return; }
+        h = (h + 1) & mask;
+    }
+}
+
+// Per-CTA shared-memory stage of k_group_f64: kF64StageSlots slots of (canonical key, 32-bit count), probed at most
+// kF64StageProbe slots deep.  A key is its own identity, so a slot is claimed with one 64-bit shared CAS and counted with
+// a shared add; a key that finds no room goes straight to the global table with its warp count, and once
+// kF64StageBypass keys of a CTA have spilled that CTA stops probing (the groups already staged are still flushed, one
+// global insert each).  A 32-bit stage count holds a CTA's rows: the launch uses min(ceil(n / 512), 8 sm_count) CTAs,
+// so a CTA sees at most max(512, n / (8 sm_count)) rows, far below 2^32 for any column that fits in HBM.  Sized from
+// scripts/value_counts_bench.py (DESIGN §3.6).
+constexpr int kF64StageSlots = 1024;
+constexpr int kF64StageProbe = 8;
+constexpr unsigned kF64StageBypass = 64;
+static_assert((kF64StageSlots & (kF64StageSlots - 1)) == 0, "the stage is indexed with a mask");
+
+__device__ __forceinline__ void f64_stage_add(unsigned long long *st_key, unsigned *st_count, unsigned *st_spills,
+                                              unsigned long long *keys, unsigned long long *counts, unsigned long long mask,
+                                              unsigned long long key, unsigned add) {
+    bool staged = false;
+    if (*(volatile unsigned *)st_spills < kF64StageBypass) {
+        const unsigned start = (unsigned)splitmix64(key);
+        for (int p = 0; p < kF64StageProbe; ++p) {
+            const int s = (int)((start + p) & (kF64StageSlots - 1));
+            // a slot only ever goes from empty to taken: a plain read skips taken slots without an atomic
+            unsigned long long cur = *(volatile unsigned long long *)(st_key + s);
+            if (cur == kEmptyKey) cur = atomicCAS(st_key + s, kEmptyKey, key);
+            if (cur == kEmptyKey || cur == key) {
+                atomicAdd(st_count + s, add);
+                staged = true;
+                break;
+            }
         }
+        if (!staged) atomicAdd(st_spills, 1u);
+    }
+    if (!staged) f64_table_add(keys, counts, mask, key, add);   // spill
+}
+
+// The binary64 group-by of rows [0, n) of one column, shared by lo_value_counts_f64_host and lo_value_counts_f64_table.
+// kVec16: values is 16-byte aligned and every thread loads two doubles per ld.global.nc.v2 (row n - 1 of an odd n is
+// the scalar tail); otherwise one double per load (a wrapped table whose column starts at an 8-byte offset).  Lanes of a
+// warp holding the same key are merged with match.any; with kVec16 a thread whose two keys are equal counts them in the
+// first round (`dup`), and only the lanes whose second key differs take a second round.
+template <bool kVec16>
+__global__ void __launch_bounds__(256) k_group_f64(const double *__restrict__ values, long long n,
+                                                   unsigned long long *__restrict__ keys,
+                                                   unsigned long long *__restrict__ counts, unsigned long long mask) {
+    __shared__ unsigned long long st_key[kF64StageSlots];
+    __shared__ unsigned st_count[kF64StageSlots];
+    __shared__ unsigned st_spills;
+    for (int s = threadIdx.x; s < kF64StageSlots; s += blockDim.x) { st_key[s] = kEmptyKey; st_count[s] = 0; }
+    if (threadIdx.x == 0) st_spills = 0;
+    __syncthreads();
+    const int lane = (int)(threadIdx.x & 31);
+    const long long stride = (long long)gridDim.x * blockDim.x;
+    if constexpr (kVec16) {
+        const long long npairs = n >> 1;
+        const double2 *v2 = reinterpret_cast<const double2 *>(values);
+        for (long long p0 = blockIdx.x * (long long)blockDim.x; p0 < npairs; p0 += stride) {
+            const long long p = p0 + threadIdx.x;
+            const bool live = p < npairs;
+            double2 v = make_double2(0.0, 0.0);
+            if (live) v = __ldg(v2 + p);
+            const unsigned long long a = canonical_key(v.x), b = canonical_key(v.y);
+            const unsigned active = __ballot_sync(0xffffffffu, live);
+            const unsigned dup = __ballot_sync(0xffffffffu, live && a == b);
+            if (!live) continue;
+            unsigned peers = __match_any_sync(active, a);
+            if (lane == __ffs(peers) - 1)
+                f64_stage_add(st_key, st_count, &st_spills, keys, counts, mask, a,
+                              (unsigned)(__popc(peers) + __popc(peers & dup)));
+            if (a == b) continue;
+            peers = __match_any_sync(active & ~dup, b);
+            if (lane == __ffs(peers) - 1)
+                f64_stage_add(st_key, st_count, &st_spills, keys, counts, mask, b, (unsigned)__popc(peers));
+        }
+        if ((n & 1) && blockIdx.x == 0 && threadIdx.x == 0)
+            f64_stage_add(st_key, st_count, &st_spills, keys, counts, mask, canonical_key(__ldg(values + n - 1)), 1u);
+    } else {
+        for (long long i0 = blockIdx.x * (long long)blockDim.x; i0 < n; i0 += stride) {
+            const long long i = i0 + threadIdx.x;
+            const bool live = i < n;
+            const unsigned active = __ballot_sync(0xffffffffu, live);
+            if (!live) continue;
+            const unsigned long long key = canonical_key(__ldg(values + i));
+            const unsigned peers = __match_any_sync(active, key);
+            if (lane == __ffs(peers) - 1)                              // one lane per distinct key in the warp
+                f64_stage_add(st_key, st_count, &st_spills, keys, counts, mask, key, (unsigned)__popc(peers));
+        }
+    }
+    __syncthreads();
+    for (int s = threadIdx.x; s < kF64StageSlots; s += blockDim.x) {
+        const unsigned long long k = st_key[s];
+        if (k != kEmptyKey) f64_table_add(keys, counts, mask, k, st_count[s]);
     }
 }
 

@@ -1385,6 +1385,22 @@ int value_counts_str_tail(HostCall &c, const uint8_t *d_chars, const long long *
         });
 }
 
+// value_counts_tail of rows [0, n) of a number column already on the device: the call of lo_value_counts_f64_host after
+// its copy, and all of lo_value_counts_f64_table.  A 16-byte aligned column takes k_group_f64's 16-byte loads.
+int value_counts_f64_tail(HostCall &c, const double *d_val, int64_t n, double *keys_out, uint64_t *counts_out,
+                          int64_t capacity, int64_t *ndistinct, lo_host_timing *timing) {
+    return value_counts_tail(c, n, keys_out, counts_out, capacity, ndistinct, timing,
+        [&](unsigned long long *keys, unsigned long long *counts, unsigned long long slots, unsigned long long *out, size_t out_n) {
+            const int grid = (int)std::min<int64_t>((n + 511) / 512, (int64_t)c.ctx->sm_count * 8);
+            if ((uintptr_t)d_val % 16 == 0)
+                lo::k_group_f64<true><<<grid, 256, 0, c.s>>>(d_val, n, keys, counts, slots - 1);
+            else
+                lo::k_group_f64<false><<<grid, 256, 0, c.s>>>(d_val, n, keys, counts, slots - 1);
+            lo::k_hash_compact<<<c.ctx->sm_count * 8, 256, 0, c.s>>>(keys, counts, slots, out, out + out_n,
+                                                                      (unsigned long long)capacity, out + 2 * out_n);
+        });
+}
+
 }  // namespace
 
 static_assert(lo::kStrStageSlots == LO_TEXT_STAGE_SLOTS, "loexec.h documents the text group-by's stage size");
@@ -1469,13 +1485,25 @@ int lo_value_counts_f64_host(lo_ctx *ctx, const double *values, int64_t n, doubl
     double *d_val = nullptr;
     c.alloc(&d_val, (size_t)n * 8);
     c.to_dev(d_val, values, (size_t)n * 8);
-    return value_counts_tail(c, n, keys_out, counts_out, capacity, ndistinct, timing,
-        [&](unsigned long long *keys, unsigned long long *counts, unsigned long long slots, unsigned long long *out, size_t out_n) {
-            const int grid = (int)std::min<int64_t>((n + 255) / 256, (int64_t)ctx->sm_count * 8);
-            lo::k_hash_count_f64<<<grid, 256, 0, c.s>>>(d_val, n, keys, counts, slots - 1);
-            lo::k_hash_compact<<<ctx->sm_count * 8, 256, 0, c.s>>>(keys, counts, slots, out, out + out_n,
-                                                                    (unsigned long long)capacity, out + 2 * out_n);
-        });
+    return value_counts_f64_tail(c, d_val, n, keys_out, counts_out, capacity, ndistinct, timing);
+}
+
+// the same on rows [0, nrows) of column `col` of a device table: nothing crosses PCIe but the groups
+int lo_value_counts_f64_table(lo_ctx *ctx, const lo_table *t, int32_t col, double *keys_out, uint64_t *counts_out,
+                              int64_t capacity, int64_t *ndistinct, lo_host_timing *timing) {
+    LO_TRY(check_ctx(ctx));
+    if (!t) return fail(LO_ERR_INVALID, "table is NULL");
+    if (t->device != ctx->device) return fail(LO_ERR_INVALID, "table lives on device %d, the context on %d", t->device, ctx->device);
+    if (t->dtype != LO_F64) return fail(LO_ERR_INVALID, "table dtype %d is not LO_F64", t->dtype);
+    if (col < 0 || col >= t->ncols) return fail(LO_ERR_INVALID, "column %d outside [0, %d)", col, t->ncols);
+    if (capacity < 0) return fail(LO_ERR_INVALID, "negative size");
+    if (!ndistinct) return fail(LO_ERR_INVALID, "ndistinct is NULL");
+    *ndistinct = 0;
+    if (t->nrows == 0) return LO_OK;
+    if (capacity > 0 && (!keys_out || !counts_out)) return fail(LO_ERR_INVALID, "NULL argument");
+    HostCall c(ctx, "value_counts_f64_table");
+    return value_counts_f64_tail(c, (const double *)(t->base + (int64_t)col * t->pitch), t->nrows, keys_out, counts_out,
+                                 capacity, ndistinct, timing);
 }
 
 // exact value counts of one TEXT column (cells = chars[offsets[i] .. offsets[i+1])): GPU hash group-by on the bytes.

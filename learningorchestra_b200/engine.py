@@ -721,6 +721,18 @@ class Engine:
         return _value_counts(lambda keys, counts, cap, nd: self._lib.lo_value_counts_f64_host(
             self._ctx, values.ctypes.data_as(C.c_void_p), n, keys, counts, cap, nd, None), n, np.float64)
 
+    def value_counts_column(self, table: DeviceTable, col: int, timing: dict | None = None):
+        """(keys float64[g], counts uint64[g]) of rows [0, nrows) of f64 column ``col`` of a device table
+        (``lo_value_counts_f64_table``): the same groups as :meth:`value_counts_f64_host` with nothing copied to the
+        device.  A null stored as NaN in the slab counts under the NaN key.  ``timing``: a dict to receive the (last)
+        call's lo_host_timing fields."""
+        t = N.HostTiming()
+        out = _value_counts(lambda keys, counts, cap, nd: self._lib.lo_value_counts_f64_table(
+            self._ctx, table._h, int(col), keys, counts, cap, nd, C.byref(t)), table.nrows, np.float64)
+        if timing is not None:
+            timing.update(_timing(t), kernel_ms=t.kernel_ms)
+        return out
+
     def minmax_cast(self, table: DeviceTable, col_idx, stream=None):
         """(min, max, n_finite) of the fp32-cast values of resident columns (range pre-pass on the device)."""
         idx, k = _i32(col_idx)

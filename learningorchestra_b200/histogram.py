@@ -7,8 +7,14 @@ document ``{field: [{"_id": value, "count": n}, ...], "_id": k}`` per field, the
 
 Here the counting runs on the GPU with no host dictionary:
 
-* number fields (every value an int / float / None): GPU hash group-by on the binary64 keys
-  (``lo_value_counts_f64_host``; -0.0 == 0.0, NaN == NaN as in MongoDB);
+* number fields (every value an int / float / None): GPU hash group-by on the binary64 keys (-0.0 == 0.0, NaN == NaN
+  as in MongoDB) over the field's slab kept resident in HBM (``table_cache``, ``lo_value_counts_f64_table``; a slab
+  already made resident by a binned or ``castTo`` request is counted as it is), leased with the text columns.  Nulls
+  are NaN in the slab: the NaN key's count less the null rows is the group of real NaNs, and the ``null`` group is the
+  null rows plus the documents that are not data rows.  Keys are typed by the host route's rule (a column store's
+  ``integers_collapsed``, a document store's ``numeric_column`` kind).  A rank group's process holds only its own
+  rows, and a field set on a document that is not a data row is not in the slab: both pack the values per request
+  (``lo_value_counts_f64_host``);
 * text fields (every value a ``str`` / None — every field of a fresh ``POST /files`` upload): GPU hash group-by on the
   cells' bytes over the field's text column kept resident in HBM (``table_cache``, ``lo_value_counts_text``), leased
   for the request.  The first request uploads the column; later ones copy no cell to the device and read no document.
@@ -18,7 +24,7 @@ Here the counting runs on the GPU with no host dictionary:
   when MongoDB groups them (:func:`columnar.tagged_cell`: 1 == 1.0, ``True`` != 1, ``"1"`` != 1), packed per request
   (``lo_value_counts_str_host``).
 
-``None`` / missing values of number and mixed fields are counted while packing.  With ``bins`` (optional
+``None`` / missing values of packed number and mixed fields are counted while packing.  With ``bins`` (optional
 extension, REST keys ``bins`` / ``range``) the fields must be numeric or text (text is parsed with ``float()`` on the
 device into the resident slab; the dataset stays text) and get the fixed-width B-semantics histogram of SURVEY.md §8c
 from the fused kernel, run on the HBM-resident copy of the dataset (``table_cache``).
@@ -44,6 +50,25 @@ def text_groups(arr, rep, counts, none_count):
     groups = [{"_id": k, "count": int(c)} for k, c in zip(keys, counts)]
     if none_count:
         groups.append({"_id": None, "count": int(none_count)})
+    return groups
+
+
+def number_groups(keys, counts, as_int, nulls, absent):
+    """Result groups of a number field counted from its slab, where a null row is NaN: the NaN key's count less the
+    ``nulls`` null rows is the group of real NaNs (emitted when there are any), and the ``null`` group is those null rows
+    plus the ``absent`` documents that are not data rows and lack the field.  ``as_int``: a finite integral key is an
+    ``int`` (the host route's rule for the store, ``ResidentDataset.numbers``)."""
+    groups = []
+    for k, c in zip(np.asarray(keys, np.float64).tolist(), np.asarray(counts, np.uint64).tolist()):
+        if math.isnan(k):
+            c -= nulls
+            if c <= 0:
+                continue
+        elif as_int and math.isfinite(k) and k.is_integer():
+            k = int(k)
+        groups.append({"_id": k, "count": int(c)})
+    if nulls + absent:
+        groups.append({"_id": None, "count": int(nulls + absent)})
     return groups
 
 
@@ -74,7 +99,7 @@ class Histogram:
             if bins:
                 results = self.__binned(parent_filename, fields, int(bins), value_range)
             else:
-                results = self.__value_counts_resident_text(parent_filename, fields)
+                results = self.__value_counts_resident(parent_filename, fields)
                 rest = [f for f in fields if f not in results]
                 if rest and getattr(self.database_connector, "has_columns", lambda _f: False)(parent_filename):
                     results.update(self.__value_counts_columnar(parent_filename, rest))
@@ -93,20 +118,33 @@ class Histogram:
             raise
 
     # ---- R-semantics: exact value counts -------------------------------------------------------------
-    def __value_counts_resident_text(self, parent_filename, fields):
-        """``$group`` of the fields that are text in the store, from their columns resident in HBM (``table_cache``),
-        under a lease: the cells cross PCIe when the column is first made resident, not on every request.  Returns the
-        groups of those fields only; the others (number, mixed-type, all null) are left to the host-packing routes."""
+    def __value_counts_resident(self, parent_filename, fields):
+        """``$group`` of the fields that are text or number in the store, from their columns resident in HBM
+        (``table_cache``), under one lease: the values cross PCIe when the column is first made resident, not on every
+        request.  Returns the groups of those fields only; the others (mixed-type, set on a document that is not a data
+        row) are left to the host-packing routes, and so is every number field of a rank group, whose process holds
+        only its own rows."""
         resident = getattr(self.engine, "resident", None)
-        if resident is None or getattr(self.engine, "value_counts_text", None) is None:
+        if resident is None:
+            return {}
+        text = fields if getattr(self.engine, "value_counts_text", None) is not None else ()
+        all_rows = getattr(self.engine, "world", 1) == getattr(self.engine, "nlocal", 1)
+        numbers = fields if all_rows and getattr(self.engine, "value_counts_column", None) is not None else ()
+        if not text and not numbers:
             return {}
         results = {}
-        with resident.lease(self.database_connector, parent_filename, (), text=fields) as data:
+        with resident.lease(self.database_connector, parent_filename, (), text=text, numbers=numbers) as data:
             for f in fields:
-                text = data.texts.get(f)
-                if text is not None and f not in results:
-                    rep, counts = self.engine.value_counts_text(text)
-                    results[f] = text_groups(text.arr, rep, counts, text.nulls + data.absent[f])
+                if f in results:
+                    continue
+                txt, as_int = data.texts.get(f), data.numbers.get(f)
+                if txt is not None:
+                    rep, counts = self.engine.value_counts_text(txt)
+                    results[f] = text_groups(txt.arr, rep, counts, txt.nulls + data.absent[f])
+                elif as_int is not None and f in data.column:
+                    j = data.column[f]
+                    keys, counts = self.engine.value_counts_column(data.table, j)
+                    results[f] = number_groups(keys, counts, as_int, data.nulls[j], data.absent[f])
         return results
 
     def __value_counts(self, documents, fields):

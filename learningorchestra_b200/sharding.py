@@ -90,6 +90,21 @@ def combine_parse_summaries(parts, row_offsets) -> dict:
     return out
 
 
+def merge_value_counts(parts):
+    """One ``$group`` of a number column from the (keys float64, counts uint64) of its shards.  Keys are canonical on
+    the device (one NaN pattern, no -0.0), so equal bits are the same group: the bit patterns are merged with
+    ``np.unique`` and the counts summed in uint64, exactly."""
+    import numpy as np
+    if not parts:
+        return np.zeros(0, np.float64), np.zeros(0, np.uint64)
+    bits = np.concatenate([np.asarray(k, np.float64).view(np.uint64) for k, _ in parts])
+    counts = np.concatenate([np.asarray(c, np.uint64) for _, c in parts])
+    keys, inverse = np.unique(bits, return_inverse=True)
+    sums = np.zeros(keys.size, np.uint64)
+    np.add.at(sums, inverse.ravel(), counts)
+    return keys.view(np.float64), sums
+
+
 class ShardedTable:
     """A columnar table whose rows are range-sharded over the local members of a :class:`ShardedEngine`.
     ``shards[i]`` is the :class:`~learningorchestra_b200.engine.DeviceTable` on local member i and holds global
@@ -445,6 +460,31 @@ class ShardedEngine:
             if isinstance(p, BaseException):
                 raise p
         return combine_parse_summaries(parts, table.offsets)
+
+    def value_counts_column(self, table: ShardedTable, col: int):
+        """``Engine.value_counts_column`` over a sharded table: every local shard is counted on its own device from a
+        host thread of its own, and the groups are merged on the host (:func:`merge_value_counts`).  A rank group's
+        process holds only its own rows, so it refuses rather than return a partial count."""
+        if self.world > self.nlocal:
+            raise self._N.LoexecError(self._N.LO_ERR_INVALID, f"value_counts_column needs every row: this process holds "
+                                      f"{self.nlocal} of the group's {self.world} shards")
+        parts = [None] * self.nlocal
+
+        def run(i):
+            try:
+                parts[i] = self.engines[i].value_counts_column(table.shards[i], col)
+            except BaseException as exc:       # re-raised on the calling thread
+                parts[i] = exc
+
+        threads = [threading.Thread(target=run, args=(i,)) for i in range(self.nlocal)]
+        for th in threads:
+            th.start()
+        for th in threads:
+            th.join()
+        for p in parts:
+            if isinstance(p, BaseException):
+                raise p
+        return merge_value_counts(parts)
 
     # ---- host buffers -------------------------------------------------------------------------------------
     def project_cast_hist_host(self, cols, nbins: int | None = None, lo=None, hi=None, out=None, bcast: bool = False):

@@ -18,6 +18,12 @@ up as they are, a document-store text field's cells with None as null.  Such a c
 words (``Sex``) is kept and counted like any other; the host keeps the Arrow array to read the group keys from, and the
 entry records how many documents that are not data rows (the metadata document) lack the field — the ``null`` group.
 
+Number fields are counted from their slabs (``Engine.value_counts_column``).  For each such field the entry records,
+when it is built, whether the slab came from a number column of the store (a text field parsed for a binned request is
+still counted as text), the documents that are not data rows lacking it, and how the host route types its keys: a
+column store's ``integers_collapsed``, a document store's ``numeric_column`` kind.  A slab already resident for a
+binned or ``castTo`` request is counted as it is.
+
 Staleness: the in-process :class:`~learningorchestra_b200.utils.Database` bumps ``version(filename)`` on every
 write to data rows (a ``/fieldTypes`` job included); a cached entry is used only while its version matches, and the
 next request rebuilds it.  A ``Database`` without ``version`` (foreign object) is never cached: its entry is freed when
@@ -38,13 +44,17 @@ class ResidentDataset:
     change with its predecessor (each object counts the entries holding it, ``holders``) and a device object is freed
     with the last entry that holds it, so a lease on either entry keeps everything it reads alive."""
 
-    def __init__(self, version, ids, fields, kinds, nulls, table, texts=None, absent=None):
+    def __init__(self, version, ids, fields, kinds, nulls, table, texts=None, absent=None, numbers=None):
         self.version, self.ids, self.fields, self.kinds, self.nulls, self.table = version, ids, fields, kinds, nulls, table
         self.column = {f: i for i, f in enumerate(fields)}
         # text columns kept as text for $group: field -> DeviceText, or None for a field that was checked and is not a
         # text field (number, mixed, all null, or set on a document that is not a data row)
         self.texts = dict(texts or {})
-        self.absent = dict(absent or {})   # text field -> documents that are not data rows and lack it (null group)
+        # number fields whose $group is counted from their slab: field -> whether a finite integral key is an int (the
+        # host route's rule for that store), or None for a field that was checked and takes another route (text, even
+        # when parsed into a slab for a binned request; mixed; set on a document that is not a data row)
+        self.numbers = dict(numbers or {})
+        self.absent = dict(absent or {})   # counted field -> documents that are not data rows and lack it (null group)
         self.users = 0          # leases handed out and not yet released (guarded by ResidentTables._lock)
         self.retired = False    # dropped from the cache: freed when the last user releases it
         for obj in self._objects():
@@ -108,14 +118,14 @@ class ResidentTables:
         self._lock = threading.RLock()
         self.hits = self.misses = 0
 
-    def lease(self, database, filename: str, fields, text=()):
-        """``with resident.lease(db, name, fields, text) as data:`` — the table and the text columns cannot be freed
-        (version bump, eviction, invalidate, another job's rebuild) while the block runs GPU work on them."""
+    def lease(self, database, filename: str, fields, text=(), numbers=()):
+        """``with resident.lease(db, name, fields, text, numbers) as data:`` — the table and the text columns cannot be
+        freed (version bump, eviction, invalidate, another job's rebuild) while the block runs GPU work on them."""
         cache = self
 
         class _Lease:
             def __enter__(self_inner):
-                self_inner.data = cache.ensure(database, filename, fields, text)
+                self_inner.data = cache.ensure(database, filename, fields, text, numbers)
                 return self_inner.data
 
             def __exit__(self_inner, *exc):
@@ -134,20 +144,24 @@ class ResidentTables:
         if entry.users <= 0:
             entry.free()
 
-    def ensure(self, database, filename: str, fields, text=()) -> ResidentDataset:
+    def ensure(self, database, filename: str, fields, text=(), numbers=()) -> ResidentDataset:
         """Resident table holding (at least) ``fields`` of ``filename``; built from the documents on a miss.
         A field may be numeric or text (a column-store text column, or document values that are all ``str`` / None):
         text is parsed on the device into its slab, the dataset itself stays text.  Raises ValueError if a requested
         field is neither, or names the first cell ``float()`` rejects; on any failure nothing is cached.
 
         ``text``: fields to keep as text columns for counting (``entry.texts``), never parsed.  A field that is not a
-        text field there is recorded as None and raises nothing: its caller takes another route.  The returned entry is
-        LEASED: pair every call with :meth:`release` (or use :meth:`lease`)."""
+        text field there is recorded as None and raises nothing: its caller takes another route.
+        ``numbers``: fields to count from their slabs (``entry.numbers``): a number field of the store is made resident
+        if it is not already (a slab of a binned or ``castTo`` request is used as it is); any other field is recorded
+        as None and raises nothing.  The returned entry is LEASED: pair every call with :meth:`release` (or use
+        :meth:`lease`)."""
         version = database.version(filename) if hasattr(database, "version") else None
         with self._lock:
             entry = self._entries.get(filename)
             if entry is not None and version is not None and entry.version == version and \
-                    all(f in entry.column for f in fields) and all(f in entry.texts for f in text):
+                    all(f in entry.column for f in fields) and all(f in entry.texts for f in text) and \
+                    all(f in entry.numbers for f in numbers):
                 self._entries.move_to_end(filename)
                 self.hits += 1
                 entry.users += 1
@@ -158,17 +172,18 @@ class ResidentTables:
             same = entry is not None and entry.version == version
             share_table = same and all(f in entry.column for f in fields)
             keep = [f for f in (entry.fields if same else []) if f not in fields]
-            wanted = [] if share_table else list(fields) + keep
             texts = dict(entry.texts) if same else {}
+            counted = dict(entry.numbers) if same else {}
             absent = dict(entry.absent) if same else {}
             wanted_text = [f for f in dict.fromkeys(text) if f not in texts]
+            wanted_num = [f for f in dict.fromkeys(numbers) if f not in counted]
             columnar_rows = getattr(database, "has_columns", lambda _f: False)(filename)
-            if share_table and not wanted_text:
+            if share_table and not wanted_text and not wanted_num:
                 rows = row_ids = entry.ids
             elif columnar_rows:          # rows already stored as columns (column_store): no document is touched
                 row_ids = database.row_ids(filename)
                 rows = row_ids
-                others = database.other_documents(filename) if wanted_text else []
+                others = database.other_documents(filename)
             else:
                 documents = list(database.find(filename, {}))
                 rows = columnar.data_rows(documents)
@@ -187,23 +202,51 @@ class ResidentTables:
                         src = values if is_text_field(values) else None
                 text_sources[f] = src
                 absent[f] = sum(1 for d in others if d.get(f) is None)
+            classified = {}
+
+            def source(f):
+                """(("number", packed) | ("text", cells) | None, key rule): the key rule is entry.numbers' value for
+                a field whose groups come from its slab — a number column of the store that no other document sets."""
+                if f not in classified:
+                    as_int = None
+                    if columnar_rows:
+                        c = database.column(filename, f)
+                        if c is not None and c.kind == "object":
+                            src = _number_source(columnar.numeric_column(c.to_pylist()))
+                        elif c is not None and c.kind == "number":
+                            src = ("number", device_number_column(c.values, c.valid, c.is_int))
+                            as_int = c.integers_collapsed
+                        elif c is not None and c.kind == "text":
+                            src = ("text", c.arr)
+                        else:
+                            src = None
+                    else:
+                        values = [d.get(f) for d in rows]
+                        src = _number_source(columnar.numeric_column(values))
+                        if src is not None:
+                            as_int = src[1][2] == "int"
+                        elif is_text_field(values):
+                            src = ("text", values)
+                    if any(d.get(f) is not None for d in others):
+                        as_int = None
+                    classified[f] = src, as_int
+                return classified[f]
+
+            for f in wanted_num:
+                src, counted[f] = source(f)
+                absent[f] = sum(1 for d in others if d.get(f) is None)
+                if counted[f] is not None and f not in (entry.column if same else {}):
+                    share_table = False      # a number field to make resident: the slabs are built again
+            new_num = [f for f in wanted_num if counted[f] is not None and f not in fields and f not in keep]
+            wanted = [] if share_table else list(fields) + keep + new_num
             sources, names = [], []          # per resident column: ("number", packed) or ("text", cells)
             for f in wanted:
-                if columnar_rows:
-                    c = database.column(filename, f)
-                    if c is not None and c.kind == "object":
-                        src = _number_source(columnar.numeric_column(c.to_pylist()))
-                    elif c is not None and c.kind == "number":
-                        src = ("number", device_number_column(c.values, c.valid, c.is_int))
-                    elif c is not None and c.kind == "text":
-                        src = ("text", c.arr)
-                    else:
-                        src = None
-                else:
-                    values = [d.get(f) for d in rows]
-                    src = _number_source(columnar.numeric_column(values))
-                    if src is None and is_text_field(values):
-                        src = ("text", values)
+                src, as_int = source(f)
+                counted[f] = as_int
+                if as_int is not None:
+                    absent[f] = sum(1 for d in others if d.get(f) is None)
+                if src is not None and src[0] == "number":
+                    texts.setdefault(f, None)    # checked: not a text field, so a count request on it is a hit
                 if src is None:
                     if f in fields:
                         raise ValueError(f"field {f!r} is not numeric; run /fieldTypes first")
@@ -230,7 +273,7 @@ class ResidentTables:
                 # a bad cell: nothing built by this call stays, nothing is cached
                 ResidentDataset(version, row_ids, [], [], [], None if share_table else table, made).free()
                 raise
-            new = ResidentDataset(version, row_ids, names, kinds, nulls, table, {**texts, **made}, absent)
+            new = ResidentDataset(version, row_ids, names, kinds, nulls, table, {**texts, **made}, absent, counted)
             new.users = 1
             if entry is not None:
                 self._entries.pop(filename, None)
