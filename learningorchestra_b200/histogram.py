@@ -44,7 +44,8 @@ from .utils import record_exception
 
 def text_groups(arr, rep, counts, none_count):
     """Result groups of a text field counted on the device: the key of each group is the cell at its representative row
-    of ``arr`` (the whole column, nulls included), then the ``null`` group of ``none_count`` null / missing cells."""
+    of ``arr`` (the array that was counted, nulls included or not), then the ``null`` group of ``none_count`` null /
+    missing cells when there are any."""
     import pyarrow as pa
     keys = arr.take(pa.array(np.asarray(rep, dtype=np.int64))).to_pylist() if len(rep) else []
     groups = [{"_id": k, "count": int(c)} for k, c in zip(keys, counts)]
@@ -54,10 +55,11 @@ def text_groups(arr, rep, counts, none_count):
 
 
 def number_groups(keys, counts, as_int, nulls, absent):
-    """Result groups of a number field counted from its slab, where a null row is NaN: the NaN key's count less the
-    ``nulls`` null rows is the group of real NaNs (emitted when there are any), and the ``null`` group is those null rows
-    plus the ``absent`` documents that are not data rows and lack the field.  ``as_int``: a finite integral key is an
-    ``int`` (the host route's rule for the store, ``ResidentDataset.numbers``)."""
+    """Result groups of a number field counted on the device.  Counted from its slab, where a null row is NaN: the NaN
+    key's count less the ``nulls`` null rows is the group of real NaNs (emitted when there are any), and the ``null``
+    group is those null rows plus the ``absent`` documents that are not data rows and lack the field.  The host routes
+    count only the values that are not null and pass 0 for both.  ``as_int``: a finite integral key is an ``int`` (the
+    store's rule: a column store's ``integers_collapsed``, a document store's ``numeric_column`` kind)."""
     groups = []
     for k, c in zip(np.asarray(keys, np.float64).tolist(), np.asarray(counts, np.uint64).tolist()):
         if math.isnan(k):
@@ -157,8 +159,7 @@ class Histogram:
                 groups = []
             elif packed is not None:                                     # number field: group-by on binary64 keys
                 col, valid, kind = packed
-                keys, counts = self.engine.value_counts_f64_host(col[valid])
-                groups = [{"_id": (int(k) if kind == "int" else float(k)), "count": int(c)} for k, c in zip(keys, counts)]
+                groups = number_groups(*self.engine.value_counts_f64_host(col[valid]), kind == "int", 0, 0)
             else:                                                        # text or mixed: group-by on the cells' bytes
                 if all(isinstance(values[i], str) for i in present):
                     cells = [values[i] for i in present]
@@ -188,18 +189,14 @@ class Histogram:
                 groups, none_count = [], none_count + nrows
             elif col.kind == "number":
                 keys, counts = self.engine.value_counts_f64_host(col.values[col.valid]) if col.valid.any() else ([], [])
-                as_int = col.integers_collapsed
-                groups = [{"_id": (int(k) if as_int and math.isfinite(k) and float(k).is_integer() else float(k)), "count": int(c)}
-                          for k, c in zip(keys, counts)]
+                groups = number_groups(keys, counts, col.integers_collapsed, 0, 0)
                 none_count += int((~col.valid).sum())
             elif col.kind == "text":
                 arr = col.arr.drop_null() if col.arr.null_count else col.arr
                 none_count += col.arr.null_count
                 from .column_store import TextColumn
                 chars, offsets, _ = TextColumn(arr).packed()
-                rep, counts = self.engine.value_counts_str_packed(chars, offsets)
-                keys = arr.take(__import__("pyarrow").array(rep, type=__import__("pyarrow").int64())).to_pylist() if len(rep) else []
-                groups = [{"_id": k, "count": int(c)} for k, c in zip(keys, counts)]
+                groups = text_groups(arr, *self.engine.value_counts_str_packed(chars, offsets), 0)
             else:                                    # mixed-type column: the document path's tagged byte-wise group-by
                 sub = self.__value_counts([{f: v} for v in col.to_pylist()], [f])[f]
                 none_count += sum(g["count"] for g in sub if g["_id"] is None)

@@ -33,6 +33,7 @@ from __future__ import annotations
 
 import threading
 from collections import OrderedDict
+from typing import NamedTuple
 
 import numpy as np
 
@@ -83,13 +84,111 @@ def device_number_column(values: np.ndarray, valid: np.ndarray, is_int: np.ndarr
     return np.where(valid, values, np.nan), valid, "int" if bool((is_int | ~valid).all()) else "float"
 
 
-def _number_source(packed):
-    return None if packed is None else ("number", packed)
-
-
 def is_text_field(values) -> bool:
     """A document field the text route takes: at least one value, and every value that is not None a ``str``."""
     return any(v is not None for v in values) and all(v is None or type(v) is str for v in values)
+
+
+class _Field(NamedTuple):
+    """What one field of a dataset is for the resident copy.  ``slab``: what its resident column is made from —
+    ``("number", (values, valid, kind))`` to upload, ``("text", cells)`` to parse, or None (not numeric).  ``text``: the
+    cells to keep as text for counting, or None.  ``as_int``: the key rule ``ResidentDataset.numbers`` records when its
+    groups come from its slab, else None.  ``absent``: the documents that are not data rows and lack it."""
+    slab: tuple | None
+    text: object
+    as_int: bool | None
+    absent: int
+
+
+class _Snapshot:
+    """The dataset as one build reads it: the data rows (or the column store's handle), their ids and the documents
+    that are not data rows.  A field is read on first use and remembered, so nothing reads a field nobody asked for and
+    nothing reads a field twice."""
+
+    def __init__(self, database, filename: str):
+        self.database, self.filename = database, filename
+        self.columnar = getattr(database, "has_columns", lambda _f: False)(filename)
+        if self.columnar:        # rows already stored as columns (column_store): no document is touched
+            self.row_ids = database.row_ids(filename)
+            self.others = database.other_documents(filename)
+        else:
+            documents = list(database.find(filename, {}))
+            self.rows = sorted(columnar.data_rows(documents), key=lambda d: d["_id"])
+            self.others = [d for d in documents if d.get("_id") == columnar.METADATA_DOCUMENT_ID]
+            self.row_ids = np.array([d["_id"] for d in self.rows], dtype=np.int64)
+        self._fields = {}
+
+    def field(self, f) -> _Field:
+        if f not in self._fields:
+            slab = text = as_int = None
+            if self.columnar:
+                c = self.database.column(self.filename, f)
+                kind = c.kind if c is not None else None
+                if kind == "number":
+                    slab, as_int = ("number", device_number_column(c.values, c.valid, c.is_int)), c.integers_collapsed
+                elif kind == "object":
+                    packed = columnar.numeric_column(c.to_pylist())
+                    slab = ("number", packed) if packed is not None else None
+                elif kind == "text":
+                    slab, text = ("text", c.arr), c.arr
+            else:
+                values = [d.get(f) for d in self.rows]
+                if is_text_field(values):
+                    slab, text = ("text", values), values
+                else:
+                    packed = columnar.numeric_column(values)
+                    if packed is not None:
+                        slab, as_int = ("number", packed), packed[2] == "int"
+            if any(d.get(f) is not None for d in self.others):
+                text = as_int = None     # its groups are not the data rows' alone: the host routes count it
+            self._fields[f] = _Field(slab, text, as_int, sum(1 for d in self.others if d.get(f) is None))
+        return self._fields[f]
+
+
+class _Plan(NamedTuple):
+    """What a miss builds: ``columns`` (field, slab) in table order, or None when the predecessor's table is shared;
+    ``uploads`` the text columns to make, field -> cells (None: recorded as not text); the rest as in ResidentDataset."""
+    columns: list | None
+    uploads: dict
+    texts: dict
+    numbers: dict
+    absent: dict
+
+
+def _plan(base, fields, text, numbers, snap: _Snapshot) -> _Plan:
+    """The entry a miss builds from ``snap``, given ``base``, the cached entry at the same version (or None): what
+    ``base`` holds is shared, not built again — its text columns always, its table when no requested or counted number
+    field is missing from it.  Raises ValueError for the first requested field that is neither number nor text."""
+    texts = dict(base.texts) if base else {}
+    counted = dict(base.numbers) if base else {}
+    absent = dict(base.absent) if base else {}
+    resident = base.fields if base else []
+    uploads = {}
+    for f in dict.fromkeys(text):
+        if f not in texts:
+            uploads[f], absent[f] = snap.field(f).text, snap.field(f).absent
+    grow = []                    # number fields to count that are not resident (every resident field is in counted)
+    for f in dict.fromkeys(numbers):
+        if f not in counted:
+            counted[f], absent[f] = snap.field(f).as_int, snap.field(f).absent
+            if counted[f] is not None:
+                grow.append(f)
+    if base and not grow and all(f in base.column for f in fields):
+        return _Plan(None, uploads, texts, counted, absent)
+    columns = []
+    for f in [*fields, *(f for f in resident if f not in fields), *(f for f in grow if f not in fields)]:
+        info = snap.field(f)
+        counted[f] = info.as_int
+        if info.as_int is not None:
+            absent[f] = info.absent
+        if info.slab is None:
+            if f in fields:
+                raise ValueError(f"field {f!r} is not numeric; run /fieldTypes first")
+            continue                 # a previously resident column that stopped being numeric: drop it
+        if info.slab[0] == "number":
+            texts.setdefault(f, None)    # checked: not a text field, so a count request on it is a hit
+        columns.append((f, info.slab))
+    return _Plan(columns, uploads, texts, counted, absent)
 
 
 def parse_text_column(engine, table, col: int, cells):
@@ -167,113 +266,9 @@ class ResidentTables:
                 entry.users += 1
                 return entry
             self.misses += 1
-            # the same version: what the entry already holds is shared with its successor, not built again — the
-            # slabs when no new number field is asked for, the text columns always
-            same = entry is not None and entry.version == version
-            share_table = same and all(f in entry.column for f in fields)
-            keep = [f for f in (entry.fields if same else []) if f not in fields]
-            texts = dict(entry.texts) if same else {}
-            counted = dict(entry.numbers) if same else {}
-            absent = dict(entry.absent) if same else {}
-            wanted_text = [f for f in dict.fromkeys(text) if f not in texts]
-            wanted_num = [f for f in dict.fromkeys(numbers) if f not in counted]
-            columnar_rows = getattr(database, "has_columns", lambda _f: False)(filename)
-            if share_table and not wanted_text and not wanted_num:
-                rows = row_ids = entry.ids
-            elif columnar_rows:          # rows already stored as columns (column_store): no document is touched
-                row_ids = database.row_ids(filename)
-                rows = row_ids
-                others = database.other_documents(filename)
-            else:
-                documents = list(database.find(filename, {}))
-                rows = columnar.data_rows(documents)
-                others = [d for d in documents if d.get("_id") == columnar.METADATA_DOCUMENT_ID]
-                rows.sort(key=lambda d: d["_id"])
-                row_ids = np.array([d["_id"] for d in rows], dtype=np.int64)
-            text_sources = {}
-            for f in wanted_text:
-                src = None
-                if not any(d.get(f) is not None for d in others):
-                    if columnar_rows:
-                        c = database.column(filename, f)
-                        src = c.arr if c is not None and c.kind == "text" else None
-                    else:
-                        values = [d.get(f) for d in rows]
-                        src = values if is_text_field(values) else None
-                text_sources[f] = src
-                absent[f] = sum(1 for d in others if d.get(f) is None)
-            classified = {}
-
-            def source(f):
-                """(("number", packed) | ("text", cells) | None, key rule): the key rule is entry.numbers' value for
-                a field whose groups come from its slab — a number column of the store that no other document sets."""
-                if f not in classified:
-                    as_int = None
-                    if columnar_rows:
-                        c = database.column(filename, f)
-                        if c is not None and c.kind == "object":
-                            src = _number_source(columnar.numeric_column(c.to_pylist()))
-                        elif c is not None and c.kind == "number":
-                            src = ("number", device_number_column(c.values, c.valid, c.is_int))
-                            as_int = c.integers_collapsed
-                        elif c is not None and c.kind == "text":
-                            src = ("text", c.arr)
-                        else:
-                            src = None
-                    else:
-                        values = [d.get(f) for d in rows]
-                        src = _number_source(columnar.numeric_column(values))
-                        if src is not None:
-                            as_int = src[1][2] == "int"
-                        elif is_text_field(values):
-                            src = ("text", values)
-                    if any(d.get(f) is not None for d in others):
-                        as_int = None
-                    classified[f] = src, as_int
-                return classified[f]
-
-            for f in wanted_num:
-                src, counted[f] = source(f)
-                absent[f] = sum(1 for d in others if d.get(f) is None)
-                if counted[f] is not None and f not in (entry.column if same else {}):
-                    share_table = False      # a number field to make resident: the slabs are built again
-            new_num = [f for f in wanted_num if counted[f] is not None and f not in fields and f not in keep]
-            wanted = [] if share_table else list(fields) + keep + new_num
-            sources, names = [], []          # per resident column: ("number", packed) or ("text", cells)
-            for f in wanted:
-                src, as_int = source(f)
-                counted[f] = as_int
-                if as_int is not None:
-                    absent[f] = sum(1 for d in others if d.get(f) is None)
-                if src is not None and src[0] == "number":
-                    texts.setdefault(f, None)    # checked: not a text field, so a count request on it is a hit
-                if src is None:
-                    if f in fields:
-                        raise ValueError(f"field {f!r} is not numeric; run /fieldTypes first")
-                    continue                 # a previously resident column that stopped being numeric: drop it
-                names.append(f); sources.append(src)
-            if share_table:
-                table, names, kinds, nulls = entry.table, entry.fields, entry.kinds, entry.nulls
-            else:
-                table, kinds, nulls = self.engine.table("f64", len(rows) if sources else 0, max(len(sources), 1)), [], []
-            made = {}
-            try:
-                for j, (how, src) in enumerate(sources):
-                    if how == "number":
-                        values, valid, kind = src
-                        if len(rows):
-                            table.upload(j, values)
-                        kinds.append(kind); nulls.append(int(valid.size - np.count_nonzero(valid)))
-                    else:
-                        kind, n_null = parse_text_column(self.engine, table, j, src)
-                        kinds.append(kind); nulls.append(n_null)
-                for f, src in text_sources.items():
-                    made[f] = self.engine.text(src) if src is not None else None
-            except BaseException:
-                # a bad cell: nothing built by this call stays, nothing is cached
-                ResidentDataset(version, row_ids, [], [], [], None if share_table else table, made).free()
-                raise
-            new = ResidentDataset(version, row_ids, names, kinds, nulls, table, {**texts, **made}, absent, counted)
+            base = entry if entry is not None and entry.version == version else None
+            snap = _Snapshot(database, filename)
+            new = self._build(version, base, snap, _plan(base, fields, text, numbers, snap))
             new.users = 1
             if entry is not None:
                 self._entries.pop(filename, None)
@@ -285,6 +280,33 @@ class ResidentTables:
             else:
                 new.retired = True         # never cached (foreign Database without version()): freed on release
             return new
+
+    def _build(self, version, base, snap: _Snapshot, plan: _Plan) -> ResidentDataset:
+        """The entry ``plan`` describes: its columns uploaded or parsed in table order, then its text columns.  On any
+        failure (a bad cell: the first in table order, so in request order) what this call made is freed and re-raised."""
+        if plan.columns is None:
+            table, names, kinds, nulls = base.table, base.fields, base.kinds, base.nulls
+        else:
+            names, kinds, nulls = [f for f, _slab in plan.columns], [], []
+            table = self.engine.table("f64", len(snap.row_ids) if names else 0, max(len(names), 1))
+        made = {}
+        try:
+            for j, (_f, (how, src)) in enumerate(plan.columns or ()):
+                if how == "number":
+                    values, valid, kind = src
+                    if len(snap.row_ids):
+                        table.upload(j, values)
+                    kinds.append(kind); nulls.append(int(valid.size - np.count_nonzero(valid)))
+                else:
+                    kind, n_null = parse_text_column(self.engine, table, j, src)
+                    kinds.append(kind); nulls.append(n_null)
+            for f, cells in plan.uploads.items():
+                made[f] = self.engine.text(cells) if cells is not None else None
+        except BaseException:
+            ResidentDataset(version, snap.row_ids, [], [], [], None if plan.columns is None else table, made).free()
+            raise
+        return ResidentDataset(version, snap.row_ids, names, kinds, nulls, table, {**plan.texts, **made}, plan.absent,
+                               plan.numbers)
 
     def _evict(self):
         total = sum(e.nbytes for e in self._entries.values())
