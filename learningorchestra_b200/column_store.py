@@ -62,17 +62,22 @@ class NumberColumn:
         return bool(np.array_equal(integral, self.is_int[self.valid]))
 
 
+def large_text(cells):
+    """One single-chunk Arrow ``large_string`` array of ``cells``: a list of ``str`` / None, a ``ChunkedArray`` or any
+    Arrow string array.  A ``large_string`` array comes back as it is, same buffers."""
+    import pyarrow as pa
+    arr = cells if isinstance(cells, (pa.Array, pa.ChunkedArray)) else pa.array(cells, type=pa.large_string())
+    if isinstance(arr, pa.ChunkedArray):
+        arr = arr.combine_chunks() if arr.num_chunks != 1 else arr.chunk(0)
+    return arr if pa.types.is_large_string(arr.type) else arr.cast(pa.large_string())
+
+
 class TextColumn:
     """arr: ``pyarrow.LargeStringArray`` (null = ``None``)."""
     kind = "text"
 
     def __init__(self, arr):
-        import pyarrow as pa
-        if isinstance(arr, pa.ChunkedArray):
-            arr = arr.combine_chunks() if arr.num_chunks != 1 else arr.chunk(0)
-        if not pa.types.is_large_string(arr.type):
-            arr = arr.cast(pa.large_string())
-        self.arr = arr
+        self.arr = large_text(arr)
 
     def __len__(self):
         return len(self.arr)
@@ -86,18 +91,11 @@ class TextColumn:
         return TextColumn(self.arr.take(pa.array(np.asarray(index, dtype=np.int64))))
 
     def packed(self):
-        """(chars uint8, offsets int64[n+1] starting at 0, null mask or None) — views of the Arrow buffers."""
-        a = self.arr
-        n = len(a)
-        bufs = a.buffers()
-        offsets = np.frombuffer(bufs[1], dtype=np.int64, count=n + 1 + a.offset)[a.offset:]
-        chars = np.frombuffer(bufs[2], dtype=np.uint8) if bufs[2] is not None and bufs[2].size else np.zeros(1, dtype=np.uint8)
-        if n and offsets[0] != 0:
-            chars, offsets = chars[offsets[0]:], offsets - offsets[0]
-        nulls = None
-        if a.null_count:
-            nulls = np.asarray(a.is_null().to_numpy(zero_copy_only=False), dtype=bool)
-        return (chars if chars.size else np.zeros(1, dtype=np.uint8)), np.ascontiguousarray(offsets), nulls
+        """(chars uint8, offsets int64[n+1] starting at 0, null mask or None): the column's
+        :func:`columnar.text_buffers`, rebased by :func:`columnar.zero_based`, and its nulls as a bool array."""
+        from .columnar import text_buffers, zero_based
+        nulls = np.asarray(self.arr.is_null().to_numpy(zero_copy_only=False), dtype=bool) if self.arr.null_count else None
+        return (*zero_based(*text_buffers(self.arr)[:2]), nulls)
 
 
 class ObjectColumn:

@@ -197,11 +197,8 @@ def number_text(cells):
     buffers.  Both ``/fieldTypes "number"`` and the text route of binned / cast requests use this one rule."""
     import pyarrow as pa
     import pyarrow.compute as pc
-    arr = cells if isinstance(cells, (pa.Array, pa.ChunkedArray)) else pa.array(cells, type=pa.large_string())
-    if isinstance(arr, pa.ChunkedArray):
-        arr = arr.combine_chunks() if arr.num_chunks != 1 else arr.chunk(0)
-    if not pa.types.is_large_string(arr.type):
-        arr = arr.cast(pa.large_string())
+    from .column_store import large_text
+    arr = large_text(cells)
     bad = pc.invert(pc.string_is_ascii(arr)).fill_null(False)
     if not pc.any(bad).as_py():
         return arr
@@ -222,6 +219,13 @@ def text_buffers(arr):
     chars = np.frombuffer(bufs[2], dtype=np.uint8) if bufs[2] is not None and bufs[2].size else np.zeros(1, dtype=np.uint8)
     validity = (np.frombuffer(bufs[0], dtype=np.uint8), arr.offset) if arr.null_count and bufs[0] is not None else None
     return chars, offsets, validity
+
+
+def zero_based(chars, offsets):
+    """(chars, offsets) of :func:`text_buffers` with offsets[0] == 0, the layout ``lo_value_counts_str_host`` takes:
+    chars from the first cell's first byte on (a view) and the offsets less offsets[0] (a copy, for a slice only)."""
+    first = int(offsets[0])
+    return (chars, offsets) if first == 0 else (chars[first:], offsets - first)
 
 
 def number_text_valid(arr) -> np.ndarray:
@@ -258,12 +262,7 @@ def pack_cells(cells):
         arr = pa.array(cells, type=pa.large_string() if is_text else pa.large_binary())
         if arr.null_count:
             raise ValueError("null cell")
-        bufs = arr.buffers()
-        offsets = np.frombuffer(bufs[1], dtype=np.int64, count=n + 1 + arr.offset)[arr.offset:]
-        data = np.frombuffer(bufs[2], dtype=np.uint8) if bufs[2] is not None and bufs[2].size else np.zeros(1, dtype=np.uint8)
-        if offsets[0] != 0:
-            data, offsets = data[offsets[0]:], offsets - offsets[0]
-        return np.ascontiguousarray(data) if data.size else np.zeros(1, dtype=np.uint8), np.ascontiguousarray(offsets)
+        return text_buffers(arr)[:2]           # a new array: offsets[0] == 0
     except Exception:                          # mixed str / bytes, exotic objects: encode one by one
         enc = [c.encode("utf-8") if isinstance(c, str) else bytes(c) for c in cells]
         offsets = np.zeros(n + 1, dtype=np.int64)

@@ -772,6 +772,67 @@ struct HostCall {
     }
 };
 
+// ---- text columns from the host: the Arrow large_string layout of lo_parse_number_to_table (loexec.h) -------------
+constexpr int kGroupRowBits = 31;            // the text group-by keeps a row index beside a 33-bit tag in one slot
+constexpr int kAnyRowBits = 63;
+
+// Refuses, in this order: n outside [0, 2^row_bits) before offsets is read, NULL offsets, offsets[n] < offsets[0], NULL
+// chars with bytes to copy, both forms of validity, a negative bit offset.  check_ascending walks the offsets between.
+int check_text_in(const uint8_t *chars, const int64_t *offsets, const lo_validity *validity, int64_t n, int row_bits) {
+    if (n < 0 || n >> row_bits) return fail(LO_ERR_INVALID, "n = %lld: 0 to 2^%d-1 rows per call", (long long)n, row_bits);
+    if (!offsets) return fail(LO_ERR_INVALID, "offsets is NULL");
+    const int64_t nbytes = offsets[n] - offsets[0];
+    if (nbytes < 0 || (nbytes > 0 && !chars)) return fail(LO_ERR_INVALID, "bad offsets / chars");
+    if (validity && validity->mask && validity->bitmap) return fail(LO_ERR_INVALID, "validity: mask or bitmap, not both");
+    if (validity && validity->bitmap && validity->bit_offset < 0) return fail(LO_ERR_INVALID, "validity: bit_offset < 0");
+    return LO_OK;
+}
+
+int check_ascending(const int64_t *offsets, int64_t n) {
+    for (int64_t i = 0; i < n; ++i)
+        if (offsets[i + 1] < offsets[i]) return fail(LO_ERR_INVALID, "offsets must be non-decreasing (row %lld)", (long long)i);
+    return LO_OK;
+}
+
+// the host bytes of a checked validity that cover n cells: the n mask bytes, or the bitmap bytes holding bits
+// bit_offset .. bit_offset + n - 1; none without validity
+const uint8_t *validity_span(const lo_validity *v, int64_t n, size_t *bytes) {
+    const bool mask = v && v->mask && n > 0, bitmap = v && v->bitmap && n > 0;
+    *bytes = mask ? (size_t)n : bitmap ? (size_t)(((v->bit_offset + n - 1) >> 3) - (v->bit_offset >> 3) + 1) : 0;
+    return mask ? v->mask : bitmap ? v->bitmap + (v->bit_offset >> 3) : nullptr;
+}
+
+// a checked text column in c's scratch (stage_text), as the text kernels take it
+struct TextDev {
+    uint8_t *chars = nullptr;                // chars[offsets[0] .. offsets[n])
+    long long *offsets = nullptr;
+    uint8_t *mask = nullptr, *bitmap = nullptr;   // at most one: validity_span's bytes
+    int bit0 = 0;                            // cell 0's bit in bitmap[0]
+    std::vector<int64_t> rebased;            // what the offsets were copied from: kept until the call synchronises
+};
+
+// rebase: the device offsets start at 0 (rebased on the host when offsets[0] != 0), else they are copied as given
+TextDev stage_text(HostCall &c, const uint8_t *chars, const int64_t *offsets, const lo_validity *validity, int64_t n,
+                   bool rebase) {
+    TextDev d;
+    const size_t nbytes = (size_t)(offsets[n] - offsets[0]);
+    size_t vbytes = 0;
+    const uint8_t *valid = validity_span(validity, n, &vbytes);
+    uint8_t **d_valid = vbytes && validity->mask ? &d.mask : &d.bitmap;
+    c.alloc(&d.chars, nbytes);
+    c.alloc(&d.offsets, (size_t)(n + 1) * 8);
+    if (vbytes) c.alloc(d_valid, vbytes);
+    c.to_dev(d.chars, chars + offsets[0], nbytes);
+    if (rebase && offsets[0] != 0) {
+        d.rebased.resize(n + 1);
+        for (int64_t i = 0; i <= n; ++i) d.rebased[i] = offsets[i] - offsets[0];
+    }
+    c.to_dev(d.offsets, d.rebased.empty() ? offsets : d.rebased.data(), (size_t)(n + 1) * 8);
+    c.to_dev(*d_valid, valid, vbytes);
+    if (d.bitmap) d.bit0 = (int)(validity->bit_offset & 7);
+    return d;
+}
+
 }  // namespace
 
 // =================================================================================================
@@ -1411,8 +1472,7 @@ struct lo_text {
     lo_ctx *ctx;
     uint8_t *chars;
     long long *offsets;
-    uint8_t *valid;
-    bool mask;
+    uint8_t *mask, *bitmap;
     int bit0;
     int64_t n, nbytes, nulls;
     size_t device_bytes;
@@ -1512,24 +1572,17 @@ int lo_value_counts_str_host(lo_ctx *ctx, const uint8_t *chars, const int64_t *o
                              uint64_t *counts_out, int64_t capacity, int64_t *ndistinct, lo_host_timing *timing) {
     LO_TRY(check_ctx(ctx));
     if (n < 0 || capacity < 0) return fail(LO_ERR_INVALID, "negative size");
-    if (n > 0x7fffffffll) return fail(LO_ERR_INVALID, "at most 2^31-1 rows per call");
     if (!ndistinct) return fail(LO_ERR_INVALID, "ndistinct is NULL");
     *ndistinct = 0;
     if (n == 0) return LO_OK;
-    if (!offsets || (capacity > 0 && (!rep_rows_out || !counts_out))) return fail(LO_ERR_INVALID, "NULL argument");
-    const int64_t nbytes = offsets[n] - offsets[0];
-    if (offsets[0] != 0 || nbytes < 0 || (nbytes > 0 && !chars)) return fail(LO_ERR_INVALID, "offsets must start at 0 and be non-decreasing");
-    for (int64_t i = 0; i < n; ++i)
-        if (offsets[i + 1] < offsets[i]) return fail(LO_ERR_INVALID, "offsets must be non-decreasing (row %lld)", (long long)i);
+    if (capacity > 0 && (!rep_rows_out || !counts_out)) return fail(LO_ERR_INVALID, "NULL argument");
+    LO_TRY(check_text_in(chars, offsets, nullptr, n, kGroupRowBits));
+    if (offsets[0] != 0) return fail(LO_ERR_INVALID, "offsets[0] must be 0");
+    LO_TRY(check_ascending(offsets, n));
     HostCall c(ctx, "value_counts_str");
-    uint8_t *d_chars = nullptr;
-    long long *d_off = nullptr;
-    c.alloc(&d_chars, (size_t)nbytes);
-    c.alloc(&d_off, (size_t)(n + 1) * 8);
-    c.to_dev(d_chars, chars, (size_t)nbytes);
-    c.to_dev(d_off, offsets, (size_t)(n + 1) * 8);
-    return value_counts_str_tail(c, d_chars, d_off, nullptr, nullptr, 0, n, rep_rows_out, counts_out, capacity, ndistinct,
-                                 timing);
+    const TextDev d = stage_text(c, chars, offsets, nullptr, n, true);
+    return value_counts_str_tail(c, d.chars, d.offsets, nullptr, nullptr, 0, n, rep_rows_out, counts_out, capacity,
+                                 ndistinct, timing);
 }
 
 // ---- text columns resident in HBM ---------------------------------------------------------------------------------
@@ -1538,18 +1591,11 @@ int lo_text_upload(lo_ctx *ctx, const uint8_t *chars, const int64_t *offsets, co
     LO_TRY(check_ctx(ctx));
     if (!out) return fail(LO_ERR_INVALID, "out is NULL");
     *out = nullptr;
-    if (n < 0) return fail(LO_ERR_INVALID, "n < 0");
-    if (n > 0x7fffffffll) return fail(LO_ERR_INVALID, "at most 2^31-1 rows per column");
-    if (!offsets) return fail(LO_ERR_INVALID, "offsets is NULL");
+    LO_TRY(check_text_in(chars, offsets, validity, n, kGroupRowBits));
+    LO_TRY(check_ascending(offsets, n));
     const int64_t nbytes = offsets[n] - offsets[0];
-    if (nbytes < 0 || (nbytes > 0 && !chars)) return fail(LO_ERR_INVALID, "bad offsets / chars");
-    for (int64_t i = 0; i < n; ++i)
-        if (offsets[i + 1] < offsets[i]) return fail(LO_ERR_INVALID, "offsets must be non-decreasing (row %lld)", (long long)i);
-    if (validity && validity->mask && validity->bitmap) return fail(LO_ERR_INVALID, "validity: mask or bitmap, not both");
-    if (validity && validity->bitmap && validity->bit_offset < 0) return fail(LO_ERR_INVALID, "validity: bit_offset < 0");
-    const bool has_mask = validity && validity->mask && n > 0, has_bitmap = validity && validity->bitmap && n > 0;
-    const int64_t first = has_bitmap ? validity->bit_offset >> 3 : 0;
-    const size_t valid_bytes = has_mask ? (size_t)n : has_bitmap ? (size_t)(((validity->bit_offset + n - 1) >> 3) - first + 1) : 0;
+    size_t valid_bytes = 0;
+    validity_span(validity, n, &valid_bytes);
     const size_t need = (size_t)std::max<int64_t>(nbytes, 1) + (size_t)(n + 1) * 8 + valid_bytes;
     size_t free_b = 0, total_b = 0;
     const cudaError_t e = cudaMemGetInfo(&free_b, &total_b);
@@ -1557,9 +1603,9 @@ int lo_text_upload(lo_ctx *ctx, const uint8_t *chars, const int64_t *offsets, co
     if (need > free_b)
         return fail(LO_ERR_NOMEM, "text_upload: the column needs %zu bytes of device memory, %zu are free", need, free_b);
     int64_t nulls = 0;                       // counted here: the host holds the validity already
-    if (has_mask) {
+    if (validity && validity->mask) {
         for (int64_t i = 0; i < n; ++i) nulls += validity->mask[i] == 0;
-    } else if (has_bitmap) {
+    } else if (validity && validity->bitmap) {
         for (int64_t i = 0; i < n; ++i) {
             const int64_t b = validity->bit_offset + i;
             nulls += ((validity->bitmap[b >> 3] >> (b & 7)) & 1) == 0;
@@ -1567,26 +1613,12 @@ int lo_text_upload(lo_ctx *ctx, const uint8_t *chars, const int64_t *offsets, co
     }
     std::unique_ptr<lo_text> t(new (std::nothrow) lo_text);
     if (!t) return fail(LO_ERR_NOMEM, "out of host memory");
-    *t = lo_text{ctx, nullptr, nullptr, nullptr, has_mask, has_bitmap ? (int)(validity->bit_offset & 7) : 0, n, nbytes, nulls, need};
     HostCall c(ctx, "text_upload");
-    c.alloc(&t->chars, (size_t)nbytes);
-    c.alloc(&t->offsets, (size_t)(n + 1) * 8);
-    if (valid_bytes) c.alloc(&t->valid, valid_bytes);
-    c.to_dev(t->chars, chars + offsets[0], (size_t)nbytes);
-    std::vector<int64_t> rel;                // the offsets of a sliced Arrow array, rebased to 0
-    const int64_t *off_src = offsets;
-    if (offsets[0] != 0) {
-        rel.resize(n + 1);
-        for (int64_t i = 0; i <= n; ++i) rel[i] = offsets[i] - offsets[0];
-        off_src = rel.data();
-    }
-    c.to_dev(t->offsets, off_src, (size_t)(n + 1) * 8);
-    if (has_mask) c.to_dev(t->valid, validity->mask, valid_bytes);
-    if (has_bitmap) c.to_dev(t->valid, validity->bitmap + first, valid_bytes);
-    c.keep(t->chars);
-    c.keep(t->offsets);
-    if (t->valid) c.keep(t->valid);
-    LO_TRY(c.finish(timing));                // synchronises: the host buffers (and `rel`) may go
+    const TextDev d = stage_text(c, chars, offsets, validity, n, true);
+    for (const void *p : {(const void *)d.chars, (const void *)d.offsets, (const void *)d.mask, (const void *)d.bitmap})
+        c.keep(p);
+    LO_TRY(c.finish(timing));                // synchronises: the host buffers may go
+    *t = lo_text{ctx, d.chars, d.offsets, d.mask, d.bitmap, d.bit0, n, nbytes, nulls, need};
     *out = t.release();
     return LO_OK;
 }
@@ -1604,7 +1636,7 @@ int lo_text_free(lo_ctx *ctx, lo_text *t) {
     if (!t) return LO_OK;
     LO_TRY(check_ctx(ctx));
     if (t->ctx != ctx) return fail(LO_ERR_INVALID, "text belongs to another context");
-    for (void *p : {(void *)t->chars, (void *)t->offsets, (void *)t->valid})
+    for (void *p : {(void *)t->chars, (void *)t->offsets, (void *)t->mask, (void *)t->bitmap})
         if (p) cudaFreeAsync(p, ctx->stream);
     delete t;
     return LO_OK;
@@ -1621,8 +1653,8 @@ int lo_value_counts_text(lo_ctx *ctx, const lo_text *t, int64_t *rep_rows_out, u
     if (t->n == t->nulls) return LO_OK;      // no cell to count (n == 0 included)
     if (capacity > 0 && (!rep_rows_out || !counts_out)) return fail(LO_ERR_INVALID, "NULL argument");
     HostCall c(ctx, "value_counts_text");
-    return value_counts_str_tail(c, t->chars, t->offsets, t->mask ? t->valid : nullptr, t->mask ? nullptr : t->valid,
-                                 t->bit0, t->n, rep_rows_out, counts_out, capacity, ndistinct, timing);
+    return value_counts_str_tail(c, t->chars, t->offsets, t->mask, t->bitmap, t->bit0, t->n, rep_rows_out, counts_out,
+                                 capacity, ndistinct, timing);
 }
 
 // text -> number for one column of cells (R-semantics "number" cast).  chars: all cells back to back;
@@ -1631,34 +1663,20 @@ int lo_value_counts_text(lo_ctx *ctx, const lo_text *t, int64_t *rep_rows_out, u
 int lo_parse_number_host(lo_ctx *ctx, const uint8_t *chars, const int64_t *offsets, int64_t n, double *values,
                          uint8_t *status, lo_host_timing *timing) {
     LO_TRY(check_ctx(ctx));
-    if (n < 0) return fail(LO_ERR_INVALID, "n < 0");
     if (n == 0) return LO_OK;
-    if (!offsets || !values || !status) return fail(LO_ERR_INVALID, "NULL argument");
-    const int64_t nbytes = offsets[n] - offsets[0];
-    if (nbytes < 0 || (nbytes > 0 && !chars)) return fail(LO_ERR_INVALID, "bad offsets / chars");
-    for (int64_t i = 0; i < n; ++i)
-        if (offsets[i + 1] < offsets[i]) return fail(LO_ERR_INVALID, "offsets must be non-decreasing (row %lld)", (long long)i);
+    if (!values || !status) return fail(LO_ERR_INVALID, "NULL argument");
+    LO_TRY(check_text_in(chars, offsets, nullptr, n, kAnyRowBits));
+    LO_TRY(check_ascending(offsets, n));
     HostCall c(ctx, "parse_number");
-    uint8_t *d_chars = nullptr, *d_status = nullptr;
-    long long *d_off = nullptr;
+    const TextDev d = stage_text(c, chars, offsets, nullptr, n, true);
+    uint8_t *d_status = nullptr;
     unsigned long long *d_val = nullptr;
-    c.alloc(&d_chars, (size_t)nbytes);
-    c.alloc(&d_off, (size_t)(n + 1) * 8);
     c.alloc(&d_val, (size_t)n * 8);
     c.alloc(&d_status, (size_t)n);
-    c.to_dev(d_chars, chars + offsets[0], (size_t)nbytes);
-    std::vector<int64_t> rel;
-    const int64_t *off_src = offsets;
-    if (offsets[0] != 0) {
-        rel.resize(n + 1);
-        for (int64_t i = 0; i <= n; ++i) rel[i] = offsets[i] - offsets[0];
-        off_src = rel.data();
-    }
-    c.to_dev(d_off, off_src, (size_t)(n + 1) * 8);
     c.mark();
     c.launch(1, [&] {
         const int grid = (int)std::min<int64_t>((n + 127) / 128, (int64_t)ctx->sm_count * 16);
-        lo::k_parse_number<<<grid, 128, 0, c.s>>>(d_chars, d_off, n, d_val, d_status);
+        lo::k_parse_number<<<grid, 128, 0, c.s>>>(d.chars, d.offsets, n, d_val, d_status);
     });
     c.mark();
     c.to_host(values, d_val, (size_t)n * 8);
@@ -1677,40 +1695,21 @@ int lo_parse_number_to_table(lo_ctx *ctx, const uint8_t *chars, const int64_t *o
     if (!out || out->dtype != LO_F64) return fail(LO_ERR_INVALID, "output table must be LO_F64");
     LO_TRY(check_range(out, col, row0, n));
     if (n == 0) return LO_OK;
-    if (!offsets) return fail(LO_ERR_INVALID, "offsets is NULL");
-    const int64_t nbytes = offsets[n] - offsets[0];
-    if (nbytes < 0 || (nbytes > 0 && !chars)) return fail(LO_ERR_INVALID, "bad offsets / chars");
-    if (validity && validity->mask && validity->bitmap) return fail(LO_ERR_INVALID, "validity: mask or bitmap, not both");
-    if (validity && validity->bitmap && validity->bit_offset < 0) return fail(LO_ERR_INVALID, "validity: bit_offset < 0");
+    LO_TRY(check_text_in(chars, offsets, validity, n, kAnyRowBits));
+    // No check_ascending and no host rebase: a sharded parse hands every shard a slice of one offsets array, and either
+    // would be one more host pass over it per shard.  The kernel rebases the offsets and reports a cell whose offsets
+    // leave [offsets[0], offsets[n]] or run backwards as unsupported.
     HostCall c(ctx, "parse_number_to_table");
-    uint8_t *d_chars = nullptr, *d_valid = nullptr;
-    long long *d_off = nullptr;
+    const TextDev d = stage_text(c, chars, offsets, validity, n, false);
     unsigned long long *d_sum = nullptr;
-    c.alloc(&d_chars, (size_t)nbytes);
-    c.alloc(&d_off, (size_t)(n + 1) * 8);
     c.alloc(&d_sum, 4 * 8);
-    c.to_dev(d_chars, chars + offsets[0], (size_t)nbytes);
-    c.to_dev(d_off, offsets, (size_t)(n + 1) * 8);
-    const uint8_t *d_mask = nullptr, *d_bitmap = nullptr;
-    int bit0 = 0;
-    if (validity && validity->mask) {
-        c.alloc(&d_valid, (size_t)n);
-        c.to_dev(d_valid, validity->mask, (size_t)n);
-        d_mask = d_valid;
-    } else if (validity && validity->bitmap) {
-        const int64_t first = validity->bit_offset >> 3, last = (validity->bit_offset + n - 1) >> 3;
-        c.alloc(&d_valid, (size_t)(last - first + 1));
-        c.to_dev(d_valid, validity->bitmap + first, (size_t)(last - first + 1));
-        d_bitmap = d_valid;
-        bit0 = (int)(validity->bit_offset & 7);
-    }
     c.memset(d_sum, 0xFF, 2 * 8);
     c.memset(d_sum + 2, 0, 2 * 8);
     unsigned long long *dst = (unsigned long long *)(out->base + (int64_t)col * out->pitch) + row0;
     c.mark();
     c.launch(1, [&] {
         const int grid = (int)std::min<int64_t>((n + 127) / 128, (int64_t)ctx->sm_count * 16);
-        lo::k_parse_number_to_col<<<grid, 128, 0, c.s>>>(d_chars, d_off, n, d_mask, d_bitmap, bit0, dst, d_sum);
+        lo::k_parse_number_to_col<<<grid, 128, 0, c.s>>>(d.chars, d.offsets, n, d.mask, d.bitmap, d.bit0, dst, d_sum);
     });
     c.mark();
     unsigned long long sum[4] = {~0ull, ~0ull, 0, 0};

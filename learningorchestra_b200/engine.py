@@ -70,6 +70,20 @@ def _timing(t) -> dict:
     return {"total_ms": t.total_ms, "h2d_bytes": t.h2d_bytes, "d2h_bytes": t.d2h_bytes, "launches": t.launches}
 
 
+def _validity(nulls, n: int):
+    """(lo_validity, the array it points into) of ``nulls`` as :meth:`Engine.parse_number_into` takes it."""
+    v, keep = N.Validity(), None
+    if isinstance(nulls, tuple):
+        keep = np.ascontiguousarray(nulls[0], dtype=np.uint8)
+        v.bitmap, v.bit_offset = keep.ctypes.data, int(nulls[1])
+    elif nulls is not None:
+        keep = np.ascontiguousarray(~np.asarray(nulls, dtype=bool)).view(np.uint8)
+        if keep.shape != (n,):
+            raise ValueError("nulls must have one entry per cell")
+        v.mask = keep.ctypes.data
+    return v, keep
+
+
 def _minmax_decode(lib, raw: np.ndarray, k: int):
     """(min, max, n_finite) of k columns from the raw uint64[3k] of a min/max pre-pass."""
     mins, maxs, cnt = np.zeros(k, np.float32), np.zeros(k, np.float32), np.zeros(k, np.uint64)
@@ -512,16 +526,7 @@ class Engine:
         ``first_invalid`` / ``first_unsupported`` (row relative to the first cell, or None), ``nulls`` (null + empty
         cells), ``integer`` (every other cell integer valued) and the lo_host_timing fields."""
         n = offsets.shape[0] - 1
-        keep = None                 # the validity buffer handed to the call
-        v = N.Validity()
-        if isinstance(nulls, tuple):
-            keep = np.ascontiguousarray(nulls[0], dtype=np.uint8)
-            v.bitmap, v.bit_offset = keep.ctypes.data, int(nulls[1])
-        elif nulls is not None:
-            keep = np.ascontiguousarray(~np.asarray(nulls, dtype=bool)).view(np.uint8)
-            if keep.shape != (n,):
-                raise ValueError("nulls must have one entry per cell")
-            v.mask = keep.ctypes.data
+        v, _keep = _validity(nulls, n)
         offsets = np.ascontiguousarray(offsets, dtype=np.int64)
         s, t = N.ParseSummary(), N.HostTiming()
         N.check(self._lib.lo_parse_number_to_table(self._ctx, chars.ctypes.data_as(C.c_void_p), offsets.ctypes.data_as(C.c_void_p),
@@ -679,17 +684,11 @@ class Engine:
         up as they are: a slice, nulls and any bit offset included) or a list of ``str`` / None (None = null).  Raises
         LoexecError LO_ERR_NOMEM when the device has too little free memory.  ``timing``: a dict to receive the call's
         lo_host_timing fields."""
-        import pyarrow as pa
+        from .column_store import large_text
         from .columnar import text_buffers
-        arr = cells if isinstance(cells, (pa.Array, pa.ChunkedArray)) else pa.array(cells, type=pa.large_string())
-        if isinstance(arr, pa.ChunkedArray):
-            arr = arr.combine_chunks() if arr.num_chunks != 1 else arr.chunk(0)
-        if not pa.types.is_large_string(arr.type):
-            arr = arr.cast(pa.large_string())
+        arr = large_text(cells)
         chars, offsets, validity = text_buffers(arr)
-        v = N.Validity()
-        if validity is not None:
-            v.bitmap, v.bit_offset = validity[0].ctypes.data, int(validity[1])
+        v, _keep = _validity(validity, len(arr))
         h, t = C.c_void_p(), N.HostTiming()
         N.check(self._lib.lo_text_upload(self._ctx, chars.ctypes.data_as(C.c_void_p), offsets.ctypes.data_as(C.c_void_p),
                                          C.byref(v), len(arr), C.byref(h), C.byref(t)))

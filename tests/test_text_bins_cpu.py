@@ -11,7 +11,7 @@ import pyarrow as pa
 import pytest
 
 from learningorchestra_b200 import columnar, utils
-from learningorchestra_b200.column_store import ColumnarDatabase
+from learningorchestra_b200.column_store import ColumnarDatabase, TextColumn, large_text
 from learningorchestra_b200.sharding import combine_parse_summaries
 from learningorchestra_b200.table_cache import ResidentTables, is_text_field
 
@@ -40,6 +40,55 @@ def test_text_buffers_of_a_sliced_array_with_nulls():
     assert columnar.text_buffers(pa.array(["a"], type=pa.large_string()))[2] is None
     np.testing.assert_array_equal(columnar.number_text_valid(pa.array(["1", None, "", "x"], type=pa.large_string())),
                                   [True, False, False, True])
+
+
+def _text_inputs():
+    cells = [None if i % 5 == 2 else "é" * (i % 3) + str(i) for i in range(40)]
+    large = pa.array(cells, type=pa.large_string())
+    return {
+        "list": cells[:17],
+        "large": large,
+        "sliced": large.slice(11, 20),
+        "sliced_without_nulls": pa.array([c or "" for c in cells], type=pa.large_string()).slice(3, 30),
+        "string": pa.array(cells, type=pa.string()).slice(7, 25),
+        "chunked": pa.chunked_array([large.slice(0, 9), pa.array(cells[9:], type=pa.large_string())]),
+        "one_chunk": pa.chunked_array([large.slice(5, 10)]),
+        "empty": pa.array([], type=pa.large_string()),
+        "sliced_empty_tail": pa.array(["ab", "", None, ""], type=pa.large_string()).slice(1),
+    }
+
+
+@pytest.mark.parametrize("name", list(_text_inputs()))
+def test_every_text_input_reads_as_one_large_string_array(name):
+    src = _text_inputs()[name]
+    cells = src if isinstance(src, list) else src.to_pylist()
+    n = len(cells)
+    arr = large_text(src)
+    assert isinstance(arr, pa.Array) and pa.types.is_large_string(arr.type) and arr.to_pylist() == cells
+    if isinstance(src, pa.Array) and pa.types.is_large_string(src.type):
+        assert arr is src
+    chars, offsets, validity = columnar.text_buffers(arr)
+    assert chars.dtype == np.uint8 and chars.size >= 1 and offsets.dtype == np.int64 and offsets.shape == (n + 1,)
+    if n and arr.buffers()[2] is not None:          # views of the Arrow buffers, the slice's offsets as they are
+        assert chars.ctypes.data == arr.buffers()[2].address
+        assert offsets.ctypes.data == arr.buffers()[1].address + 8 * arr.offset
+    cell_bytes = [chars[offsets[i]:offsets[i + 1]].tobytes() for i in range(n)]
+    assert [b.decode() for b, c in zip(cell_bytes, cells) if c is not None] == [c for c in cells if c is not None]
+    if None in cells:
+        bitmap, bit0 = validity
+        assert [not (bitmap[(bit0 + i) >> 3] >> ((bit0 + i) & 7)) & 1 for i in range(n)] == [c is None for c in cells]
+    else:
+        assert validity is None
+    zchars, zoffsets = columnar.zero_based(chars, offsets)
+    assert zoffsets[0] == 0 and zoffsets.shape == (n + 1,)
+    assert [zchars[zoffsets[i]:zoffsets[i + 1]].tobytes() for i in range(n)] == cell_bytes
+    pchars, poffsets, nulls = TextColumn(arr).packed()
+    np.testing.assert_array_equal(poffsets, zoffsets)
+    assert [pchars[poffsets[i]:poffsets[i + 1]].tobytes() for i in range(n)] == cell_bytes
+    assert (nulls is None) if None not in cells else nulls.tolist() == [c is None for c in cells]
+    present = [c for c in cells if c is not None]
+    pchars, poffsets = columnar.pack_cells(present)
+    assert poffsets[0] == 0 and [pchars[poffsets[i]:poffsets[i + 1]].tobytes().decode() for i in range(len(present))] == present
 
 
 def test_shard_summaries_merge_to_the_global_first_row():
