@@ -378,6 +378,23 @@ int lo_text_free(lo_ctx *ctx, lo_text *t);
 int lo_value_counts_text(lo_ctx *ctx, const lo_text *t, int64_t *rep_rows_out, uint64_t *counts_out,
                          int64_t capacity, int64_t *ndistinct, lo_host_timing *timing);
 
+/* lo_value_counts_text of one text column cut into nshards row-range shards, each a lo_text on any context (several
+ * may share one): shards[i] holds the column's rows [row0[i], row0[i] + n_i), disjoint and in row order.  Each shard is
+ * counted on its own context's device and stream; its groups are packed into a key column there (cells, global rows,
+ * counts), copied to root's device with cudaMemcpyPeerAsync (peer access need not be enabled) and merged there by a
+ * second hash pass over the distinct keys only, with 64-bit counts.  The contract is lo_value_counts_text's, with
+ * rep_rows_out holding GLOBAL rows (row0[i] + the shard's row); nshards == 1 is lo_value_counts_text plus row0[0].
+ * Refused with LO_ERR_INVALID before anything is launched: a NULL root, shards, row0 or shard; nshards outside
+ * [1, LO_GROUP_MAX_DEVICES]; a negative, decreasing or overlapping row0; NULL outputs with capacity > 0.  The merge
+ * keeps a 31-bit key index: more than 2^31-1 groups summed over the shards -> LO_ERR_INVALID.
+ * Launches: 5 on the context of every shard with a non-null cell (count, compact, key lengths, scan, key gather) and
+ * 3 on root (merge, compact, global rows).  timing: total_ms is the whole call, kernel_ms the root's merge (between two
+ * events on root's stream), launches those on root's context during the call, h2d_bytes 0 and d2h_bytes the groups
+ * read back.  The bytes that cross between devices are in neither byte count. */
+int lo_value_counts_text_shards(lo_ctx *root, const lo_text *const *shards, const int64_t *row0, int32_t nshards,
+                                int64_t *rep_rows_out, uint64_t *counts_out, int64_t capacity, int64_t *ndistinct,
+                                lo_host_timing *timing);
+
 /* Number -> text for one column: the reference's "string" cast, str(v) / None -> "" (data_type_handler_image/
  * data_type_update.py:22-28), for every cell at once on the GPU.  The inverse of lo_parse_number_host.
  * status[i] uses the LO_NUM_* codes above: FLOAT -> repr(float) (shortest round-trip digits, CPython's notation),

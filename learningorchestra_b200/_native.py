@@ -152,6 +152,8 @@ SIGNATURES = {
     "lo_text_info": (C.c_int, [_P, C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(C.c_size_t)]),
     "lo_text_free": (C.c_int, [_P, _P]),
     "lo_value_counts_text": (C.c_int, [_P, _P, _P, _P, C.c_int64, C.POINTER(C.c_int64), C.POINTER(HostTiming)]),
+    "lo_value_counts_text_shards": (C.c_int, [_P, C.POINTER(_P), C.POINTER(C.c_int64), C.c_int32, _P, _P, C.c_int64,
+                                              C.POINTER(C.c_int64), C.POINTER(HostTiming)]),
     "lo_format_number_host": (C.c_int, [_P, _P, _P, C.c_int64, _P, _P, C.c_int64, C.POINTER(HostTiming)]),
     "lo_minmax_cast_host": (C.c_int, [_P, C.POINTER(_P), C.c_int64, C.c_int32, _P, _P, _P, C.POINTER(HostTiming)]),
     "lo_csv_read_host": (C.c_int, [_P, _P, C.c_int64, C.POINTER(_P), C.POINTER(CsvInfo), C.POINTER(HostTiming)]),

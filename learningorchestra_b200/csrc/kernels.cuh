@@ -1364,6 +1364,59 @@ __global__ void k_hash_compact_str(const unsigned long long *__restrict__ slots,
     }
 }
 
+// ---------------------------------------------------------------------------------------------
+// value counts of a text column cut into row-range shards (lo_value_counts_text_shards): each shard is counted on its
+// own device by the two kernels above, its groups are gathered into a packed key column (k_gather_lens, an exclusive
+// scan, k_gather_cells), the packed pieces are copied to the root device, and k_hash_sum_str merges them there.
+// ---------------------------------------------------------------------------------------------
+// lens[g] = the byte length of group g's representative cell (rows: the compacted representative rows of one shard)
+__global__ void k_gather_lens(const long long *__restrict__ offsets, const long long *__restrict__ rows, long long ngroups,
+                              long long *__restrict__ lens) {
+    for (long long g = blockIdx.x * (long long)blockDim.x + threadIdx.x; g < ngroups; g += (long long)gridDim.x * blockDim.x) {
+        const long long r = rows[g];
+        lens[g] = offsets[r + 1] - offsets[r];
+    }
+}
+
+// Copies group g's cell to key_chars[key_off[g] ..) and turns the shard's arrays into their pieces of the concatenated
+// key column: rows[g] += row0 (a global row), key_off[g] += byte0 for g in [0, ngroups] (each entry is read and
+// rewritten by its own thread only; the copy's length comes from the cell's offsets).
+__global__ void k_gather_cells(const uint8_t *__restrict__ chars, const long long *__restrict__ offsets,
+                               long long *__restrict__ rows, long long ngroups, long long *__restrict__ key_off,
+                               uint8_t *__restrict__ key_chars, long long row0, long long byte0) {
+    for (long long g = blockIdx.x * (long long)blockDim.x + threadIdx.x; g <= ngroups; g += (long long)gridDim.x * blockDim.x) {
+        const long long dst = key_off[g];
+        key_off[g] = dst + byte0;
+        if (g == ngroups) break;
+        const long long r = rows[g], b = offsets[r], len = offsets[r + 1] - b;
+        for (long long i = 0; i < len; ++i) key_chars[dst + i] = chars[b + i];
+        rows[g] = r + row0;
+    }
+}
+
+// The merge: key i of the concatenated key column (chars / offsets) carries weight[i] rows, its shard's count.  A key
+// occurs at most once per shard, so there is nothing for a warp match or a shared-memory stage to merge: each thread
+// inserts its key into the global table (k_hash_count_str's slot format, row = the key's index) with a 64-bit add.
+__global__ void __launch_bounds__(256) k_hash_sum_str(const uint8_t *__restrict__ chars, const long long *__restrict__ offsets,
+                                                      const unsigned long long *__restrict__ weight, long long n,
+                                                      unsigned long long *__restrict__ slots,
+                                                      unsigned long long *__restrict__ counts, unsigned long long mask) {
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+        const unsigned long long h = hash_bytes(chars + offsets[i], offsets[i + 1] - offsets[i]);
+        str_table_add(chars, offsets, slots, counts, mask, h, ((h >> 31) << 31) | (unsigned long long)i, weight[i]);
+    }
+}
+
+// rows[g] = global_rows[rows[g]] for the first min(*ngroups, capacity) groups: k_hash_compact_str's key indices become
+// the global rows the shards gathered
+__global__ void k_take_rows(long long *__restrict__ rows, const long long *__restrict__ global_rows,
+                            const unsigned long long *__restrict__ ngroups, unsigned long long capacity) {
+    const unsigned long long n = min(*ngroups, capacity);
+    for (unsigned long long g = blockIdx.x * (unsigned long long)blockDim.x + threadIdx.x; g < n;
+         g += (unsigned long long)gridDim.x * blockDim.x)
+        rows[g] = global_rows[rows[g]];
+}
+
 // R-semantics cast "number" (data_type_update.py:40-43): one cell per thread, CPython float() grammar,
 // correctly rounded binary64 (parse_number.cuh) + the is_integer() flag the adapter turns into int(v)
 __global__ void k_parse_number(const uint8_t *__restrict__ chars, const long long *__restrict__ offsets, long long n,

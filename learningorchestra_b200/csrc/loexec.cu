@@ -1402,10 +1402,11 @@ int check_project_host(const double *const *in_cols, int64_t nrows, int32_t k, f
 // The rest of lo_value_counts_*_host once the input is on the device.  count_and_compact(keys, counts, slots, out,
 // out_n) launches the two kernels of the hash group-by: count into a table of `slots` slots (keys all ones, counts
 // zero), then compact the groups into out[0 .. out_n) (keys) and out[out_n .. 2 out_n) (counts), at most `capacity`
-// of them, and their number into out[2 out_n].  The first min(groups, capacity) of them are copied out.
+// of them, and their number into out[2 out_n].  The first min(groups, capacity) of them are copied out.  nlaunch: the
+// kernels count_and_compact launches.
 template <typename CountAndCompact>
 int value_counts_tail(HostCall &c, int64_t n, void *keys_out, uint64_t *counts_out, int64_t capacity, int64_t *ndistinct,
-                      lo_host_timing *timing, CountAndCompact count_and_compact) {
+                      lo_host_timing *timing, CountAndCompact count_and_compact, int nlaunch = 2) {
     unsigned long long slots = 1024;
     while (slots < 2ull * (unsigned long long)n) slots <<= 1;
     const size_t out_n = (size_t)std::max<int64_t>(capacity, 1);
@@ -1417,7 +1418,7 @@ int value_counts_tail(HostCall &c, int64_t n, void *keys_out, uint64_t *counts_o
     c.memset(d_keys, 0xFF, slots * 8);
     c.memset(d_counts, 0, slots * 8);
     c.memset(d_out + 2 * out_n, 0, 8);
-    c.launch(2, [&] { count_and_compact(d_keys, d_counts, slots, d_out, out_n); });
+    c.launch(nlaunch, [&] { count_and_compact(d_keys, d_counts, slots, d_out, out_n); });
     c.mark();
     unsigned long long nd = 0;
     c.to_host(&nd, d_out + 2 * out_n, 8);
@@ -1655,6 +1656,189 @@ int lo_value_counts_text(lo_ctx *ctx, const lo_text *t, int64_t *rep_rows_out, u
     HostCall c(ctx, "value_counts_text");
     return value_counts_str_tail(c, t->chars, t->offsets, t->mask, t->bitmap, t->bit0, t->n, rep_rows_out, counts_out,
                                  capacity, ndistinct, timing);
+}
+
+}  // extern "C"
+
+namespace {
+
+// one shard of lo_value_counts_text_shards, worked on its own context's call frame and stream
+struct TextShard {
+    const lo_text *t;
+    int64_t row0;
+    int64_t cap;                             // n - nulls: at most this many groups
+    std::unique_ptr<HostCall> c;
+    unsigned long long *grp = nullptr;       // compacted groups: rows [0, cap), counts [cap, 2 cap), their number [2 cap]
+    long long *key_off = nullptr;            // the packed key column of its groups: nd + 1 offsets, then the bytes
+    uint8_t *key_chars = nullptr;
+    cudaEvent_t gathered = nullptr;          // the packed pieces are ready to copy
+    unsigned long long nd = 0;
+    long long bytes = 0, group0 = 0, byte0 = 0;   // its bytes, and where its pieces start in the concatenated column
+};
+
+}  // namespace
+
+extern "C" {
+
+// Value counts of one text column cut into row-range shards, each resident on its own context (loexec.h).  Four steps,
+// each enqueued on every shard before the host waits on any, so shards on different devices run at once:
+//   1. count and compact each shard on its device (k_hash_count_str, k_hash_compact_str); the host reads its group count;
+//   2. the byte lengths of its groups' cells and their exclusive scan; the host reads its key bytes;
+//   3. k_gather_cells packs the keys, rebases their offsets into the concatenated column and makes the rows global;
+//   4. the root waits on each shard's event, copies the packed pieces over with cudaMemcpyPeerAsync, and merges them
+//      (k_hash_sum_str, k_hash_compact_str, k_take_rows).  Each shard's stream waits on the root's copies before its
+//      scratch is freed.
+int lo_value_counts_text_shards(lo_ctx *root, const lo_text *const *shards, const int64_t *row0, int32_t nshards,
+                                int64_t *rep_rows_out, uint64_t *counts_out, int64_t capacity, int64_t *ndistinct,
+                                lo_host_timing *timing) {
+    if (!root) return fail(LO_ERR_INVALID, "root is NULL");
+    static_assert(lo::kMaxPeers + 1 == LO_GROUP_MAX_DEVICES, "a group's devices: the root and its peers");
+    if (nshards < 1 || nshards > LO_GROUP_MAX_DEVICES)
+        return fail(LO_ERR_INVALID, "nshards = %d: 1 to %d shards", nshards, LO_GROUP_MAX_DEVICES);
+    if (!shards || !row0) return fail(LO_ERR_INVALID, "shards or row0 is NULL");
+    int64_t cells = 0;
+    for (int i = 0; i < nshards; ++i) {
+        if (!shards[i]) return fail(LO_ERR_INVALID, "shards[%d] is NULL", i);
+        if (row0[i] < 0) return fail(LO_ERR_INVALID, "row0[%d] = %lld is negative", i, (long long)row0[i]);
+        if (i > 0 && row0[i] < row0[i - 1] + shards[i - 1]->n)
+            return fail(LO_ERR_INVALID, "row0[%d] = %lld: shard %d ends at row %lld (shards are disjoint and in row order)",
+                        i, (long long)row0[i], i - 1, (long long)(row0[i - 1] + shards[i - 1]->n));
+        cells += shards[i]->n - shards[i]->nulls;
+    }
+    if (capacity < 0) return fail(LO_ERR_INVALID, "negative size");
+    if (!ndistinct) return fail(LO_ERR_INVALID, "ndistinct is NULL");
+    *ndistinct = 0;
+    if (cells == 0) return LO_OK;            // no cell to count
+    if (capacity > 0 && (!rep_rows_out || !counts_out)) return fail(LO_ERR_INVALID, "NULL argument");
+    LO_TRY(check_ctx(root));
+    HostCall c(root, "value_counts_text_shards");
+    std::vector<TextShard> sh;
+    for (int i = 0; i < nshards; ++i)
+        if (shards[i]->n > shards[i]->nulls) sh.push_back(TextShard{shards[i], row0[i], shards[i]->n - shards[i]->nulls});
+    auto all_ok = [&] {
+        for (const TextShard &s : sh)
+            if (!s.c->ok()) return false;
+        return true;
+    };
+    auto grid_for = [](lo_ctx *ctx, int64_t n) { return (int)std::min<int64_t>((n + 255) / 256, (int64_t)ctx->sm_count * 8); };
+
+    for (TextShard &s : sh) {                // 1. count and compact
+        lo_ctx *ctx = s.t->ctx;
+        s.c = std::make_unique<HostCall>(ctx, "value_counts_text_shards");
+        HostCall &sc = *s.c;
+        sc.run([&] { return cudaSetDevice(ctx->device); });
+        unsigned long long slots = 1024;
+        while (slots < 2ull * (unsigned long long)s.t->n) slots <<= 1;
+        unsigned long long *table = nullptr, *counts = nullptr;
+        sc.alloc(&table, slots * 8);
+        sc.alloc(&counts, slots * 8);
+        sc.alloc(&s.grp, (2 * (size_t)s.cap + 1) * 8);
+        sc.memset(table, 0xFF, slots * 8);
+        sc.memset(counts, 0, slots * 8);
+        sc.memset(s.grp + 2 * s.cap, 0, 8);
+        sc.launch(2, [&] {
+            lo::k_hash_count_str<<<grid_for(ctx, s.t->n), 256, 0, sc.s>>>(s.t->chars, s.t->offsets, s.t->n, s.t->mask,
+                                                                           s.t->bitmap, s.t->bit0, table, counts, slots - 1);
+            lo::k_hash_compact_str<<<ctx->sm_count * 8, 256, 0, sc.s>>>(table, counts, slots, (long long *)s.grp,
+                                                                         s.grp + s.cap, (unsigned long long)s.cap,
+                                                                         s.grp + 2 * s.cap);
+        });
+        sc.drop(table);
+        sc.drop(counts);
+    }
+    for (TextShard &s : sh) {
+        s.c->to_host(&s.nd, s.grp + 2 * s.cap, 8);
+        s.c->sync();
+    }
+    std::vector<size_t> scan_bytes(sh.size(), 0);
+    for (size_t i = 0; i < sh.size() && all_ok(); ++i) {   // 2. key lengths and their scan
+        TextShard &s = sh[i];
+        HostCall &sc = *s.c;
+        lo_ctx *ctx = s.t->ctx;
+        const int64_t nd = (int64_t)s.nd;
+        void *tmp = nullptr;
+        sc.run([&] { return cudaSetDevice(ctx->device); });
+        sc.alloc(&s.key_off, (size_t)(nd + 1) * 8);
+        sc.run([&] { return cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes[i], s.key_off, nd + 1, sc.s); });
+        sc.alloc(&tmp, scan_bytes[i]);
+        sc.memset(s.key_off + nd, 0, 8);     // the scan's last input: key_off[nd] = the key bytes
+        sc.launch(1, [&] { lo::k_gather_lens<<<grid_for(ctx, nd), 256, 0, sc.s>>>(s.t->offsets, (const long long *)s.grp, nd, s.key_off); });
+        sc.launch(1, [&] { return cub::DeviceScan::ExclusiveSum(tmp, scan_bytes[i], s.key_off, nd + 1, sc.s); });
+        sc.drop(tmp);
+    }
+    long long groups = 0, bytes = 0;
+    for (TextShard &s : sh) {
+        if (!all_ok()) break;
+        s.c->to_host(&s.bytes, s.key_off + s.nd, 8);
+        s.c->sync();
+        s.group0 = groups;
+        s.byte0 = bytes;
+        groups += (long long)s.nd;
+        bytes += s.bytes;
+    }
+    if (all_ok() && groups >> 31)            // the merge's slot word keeps a 31-bit key index
+        c.check([&] { return fail(LO_ERR_INVALID, "the shards hold %lld groups: at most 2^31-1 can be merged", groups); });
+    for (TextShard &s : sh) {                // 3. pack the keys
+        if (!all_ok() || !c.ok()) break;
+        HostCall &sc = *s.c;
+        lo_ctx *ctx = s.t->ctx;
+        sc.run([&] { return cudaSetDevice(ctx->device); });
+        sc.alloc(&s.key_chars, (size_t)s.bytes);
+        sc.launch(1, [&] {
+            lo::k_gather_cells<<<grid_for(ctx, (int64_t)s.nd + 1), 256, 0, sc.s>>>(
+                s.t->chars, s.t->offsets, (long long *)s.grp, (long long)s.nd, s.key_off, s.key_chars, s.row0, s.byte0);
+        });
+        sc.run([&] { return cudaEventCreateWithFlags(&s.gathered, cudaEventDisableTiming); });
+        sc.run([&] { return cudaEventRecord(s.gathered, sc.s); });
+    }
+    int rc = LO_OK;
+    cudaEvent_t copied = nullptr;
+    if (all_ok() && c.ok()) {                // 4. copy the pieces to the root and merge them there
+        c.run([&] { return cudaSetDevice(root->device); });
+        uint8_t *chars = nullptr;
+        long long *offsets = nullptr, *rows = nullptr;
+        unsigned long long *weight = nullptr;
+        c.alloc(&chars, (size_t)bytes);
+        c.alloc(&offsets, (size_t)(groups + 1) * 8);
+        c.alloc(&rows, (size_t)groups * 8);
+        c.alloc(&weight, (size_t)groups * 8);
+        for (TextShard &s : sh) {
+            const int dev = s.t->ctx->device;
+            c.run([&] { return cudaStreamWaitEvent(c.s, s.gathered, 0); });
+            // nd + 1 offsets: the last is the next shard's first (the same value), or offsets[groups]
+            c.run([&] { return cudaMemcpyPeerAsync(offsets + s.group0, root->device, s.key_off, dev, (s.nd + 1) * 8, c.s); });
+            c.run([&] { return cudaMemcpyPeerAsync(rows + s.group0, root->device, s.grp, dev, s.nd * 8, c.s); });
+            c.run([&] { return cudaMemcpyPeerAsync(weight + s.group0, root->device, s.grp + s.cap, dev, s.nd * 8, c.s); });
+            if (s.bytes) c.run([&] { return cudaMemcpyPeerAsync(chars + s.byte0, root->device, s.key_chars, dev, s.bytes, c.s); });
+        }
+        c.run([&] { return cudaEventCreateWithFlags(&copied, cudaEventDisableTiming); });
+        c.run([&] { return cudaEventRecord(copied, c.s); });
+        for (TextShard &s : sh)              // a shard's scratch is freed after the root has read it
+            if (c.ok()) s.c->run([&] { return cudaStreamWaitEvent(s.c->s, copied, 0); });
+        rc = value_counts_tail(c, groups, rep_rows_out, counts_out, capacity, ndistinct, timing,
+            [&](unsigned long long *slots_keys, unsigned long long *counts, unsigned long long slots, unsigned long long *out, size_t out_n) {
+                lo::k_hash_sum_str<<<grid_for(root, groups), 256, 0, c.s>>>(chars, offsets, weight, groups, slots_keys,
+                                                                             counts, slots - 1);
+                lo::k_hash_compact_str<<<root->sm_count * 8, 256, 0, c.s>>>(slots_keys, counts, slots, (long long *)out,
+                                                                             out + out_n, (unsigned long long)capacity,
+                                                                             out + 2 * out_n);
+                lo::k_take_rows<<<root->sm_count * 8, 256, 0, c.s>>>((long long *)out, rows, out + 2 * out_n,
+                                                                      (unsigned long long)capacity);
+            }, 3);
+    } else {
+        rc = c.finish(nullptr);              // synchronises the root: nothing of it reads a shard any more
+    }
+    std::string msg = g_err;
+    for (TextShard &s : sh) {                // free every shard's scratch; the first error is the call's
+        cudaSetDevice(s.t->ctx->device);
+        const int r = s.c->finish(nullptr);
+        if (rc == LO_OK && r != LO_OK) { rc = r; msg = g_err; }
+        if (s.gathered) cudaEventDestroy(s.gathered);
+    }
+    if (copied) cudaEventDestroy(copied);
+    cudaSetDevice(root->device);
+    g_err = msg;
+    return rc;
 }
 
 // text -> number for one column of cells (R-semantics "number" cast).  chars: all cells back to back;

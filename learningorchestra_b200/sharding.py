@@ -156,6 +156,55 @@ class ShardedTable:
         self.shards = []
 
 
+class ShardedText:
+    """One text column cut into row-range pieces over the local members of a :class:`ShardedEngine`, at the slab shards'
+    row split (:meth:`ShardedEngine.bounds`).  ``pieces[i]`` is the
+    :class:`~learningorchestra_b200.engine.DeviceText` on local member i and holds global rows
+    ``[offsets[i], offsets[i] + pieces[i].n)``.  ``arr`` is the whole Arrow array the group keys are read from (the
+    representative rows are global); ``n``, ``nulls`` and ``nbytes`` sum over the pieces."""
+
+    def __init__(self, pieces, offsets, arr):
+        self.pieces, self.offsets, self.arr = list(pieces), list(offsets), arr
+        self.n = sum(p.n for p in self.pieces)
+        self.nulls = sum(p.nulls for p in self.pieces)
+        self.nbytes = sum(p.nbytes for p in self.pieces)
+
+    @classmethod
+    def upload(cls, engines, bounds, arr, timing: dict | None = None) -> "ShardedText":
+        """Rows ``[b, e)`` of ``arr`` (a ``large_string`` array) uploaded with ``engines[i].text`` for the i-th of
+        ``bounds``, each from a host thread of its own.  When any upload fails (LO_ERR_NOMEM on a full device, say) the
+        pieces already made are freed and the first error is raised.  ``timing``: the longest piece's times, the
+        pieces' bytes and launches added up."""
+        parts, times = [None] * len(engines), [{} for _ in engines]
+
+        def run(i):
+            b, e = bounds[i]
+            try:
+                parts[i] = engines[i].text(arr.slice(b, e - b), timing=times[i])
+            except BaseException as exc:       # re-raised on the calling thread
+                parts[i] = exc
+
+        threads = [threading.Thread(target=run, args=(i,)) for i in range(len(engines))]
+        for th in threads:
+            th.start()
+        for th in threads:
+            th.join()
+        failed = [p for p in parts if isinstance(p, BaseException)]
+        if failed:
+            for p in parts:
+                if p is not None and not isinstance(p, BaseException):
+                    p.free()
+            raise failed[0]
+        if timing is not None:
+            timing.update({k: max(t[k] for t in times) for k in ("total_ms", "kernel_ms")},
+                          **{k: sum(t[k] for t in times) for k in ("h2d_bytes", "d2h_bytes", "launches")})
+        return cls(parts, [b for b, _ in bounds], arr)
+
+    def free(self) -> None:
+        for p in self.pieces:
+            p.free()
+
+
 class GroupCounts:
     """Merged counts of the step that produced it, in the group's result buffer (valid until the next group call).
     A request split over several steps (:func:`column_batches`) has read each step's counts out already: ``host``
@@ -560,10 +609,37 @@ class ShardedEngine:
         return self.engines[0].value_counts_str_host(cells)
 
     def text(self, cells, timing=None):
-        return self.engines[0].text(cells, timing)
+        """``Engine.text`` over the group: a :class:`ShardedText` whose pieces follow :meth:`bounds`, one per local
+        member, uploaded at once.  A rank group's process holds only its own rows of a table but every cell of a text
+        column it is given, so it keeps the whole column on its own device (a ``DeviceText``)."""
+        if self.world > self.nlocal:
+            return self.engines[0].text(cells, timing)
+        from .column_store import large_text
+        arr = large_text(cells)
+        return ShardedText.upload(self.engines, self.bounds(len(arr)), arr, timing)
 
     def value_counts_text(self, text, timing=None):
-        return self.engines[0].value_counts_text(text, timing)
+        """``Engine.value_counts_text`` of a :class:`ShardedText` (``lo_value_counts_text_shards``): every piece is
+        counted on its own device, and the groups are merged on the first local member's device.  Representative rows
+        index the whole column.  A ``DeviceText`` (a rank group's) is counted on its own device."""
+        if not isinstance(text, ShardedText):
+            return self.engines[0].value_counts_text(text, timing)
+        import numpy as np
+        from .engine import _timing, _value_counts
+        if any(p._h is None for p in text.pieces):
+            raise ValueError("the text column has been freed")
+        n = text.n - text.nulls
+        if n == 0:
+            return np.zeros(0, np.int64), np.zeros(0, np.uint64)
+        N, k = self._N, len(text.pieces)
+        handles = (C.c_void_p * k)(*[p._h for p in text.pieces])
+        row0 = (C.c_int64 * k)(*text.offsets)
+        t = N.HostTiming()
+        out = _value_counts(lambda rows, counts, cap, nd: self._lib.lo_value_counts_text_shards(
+            self.engines[0]._ctx, handles, row0, k, rows, counts, cap, nd, C.byref(t)), n, np.int64)
+        if timing is not None:
+            timing.update(_timing(t), kernel_ms=t.kernel_ms)
+        return out
 
     @property
     def resident(self):
