@@ -691,8 +691,10 @@ struct HostCall {
     double h2d = 0, d2h = 0;
     const std::chrono::steady_clock::time_point t0 = std::chrono::steady_clock::now();
     const int64_t launches0;
+    const bool timed;                        // false: nobody reads the frame's lo_host_timing, so mark() records nothing
 
-    HostCall(lo_ctx *c, const char *call) : ctx(c), name(call), s(c->stream), launches0(c->launches.load()) {}
+    HostCall(lo_ctx *c, const char *call, bool timed = true)
+        : ctx(c), name(call), s(c->stream), launches0(c->launches.load()), timed(timed) {}
     ~HostCall() {
         release(scratch);
         for (cudaEvent_t ev : marks) cudaEventDestroy(ev);
@@ -737,7 +739,7 @@ struct HostCall {
     void memset(void *d, int v, size_t bytes) { run([&] { return cudaMemsetAsync(d, v, bytes, s); }); }
     void sync() { run([&] { return cudaStreamSynchronize(s); }); }
     void mark() {                            // start or end of a timed section
-        run([&] {
+        if (timed) run([&] {
             cudaEvent_t ev = nullptr;
             const cudaError_t e = cudaEventCreate(&ev);
             if (e != cudaSuccess) return e;
@@ -802,19 +804,19 @@ const uint8_t *validity_span(const lo_validity *v, int64_t n, size_t *bytes) {
     return mask ? v->mask : bitmap ? v->bitmap + (v->bit_offset >> 3) : nullptr;
 }
 
-// a checked text column in c's scratch (stage_text), as the text kernels take it
-struct TextDev {
+// a text column on the device, as the text kernels take it: staged for one call (stage_text) or resident (lo_text)
+struct TextCols {
     uint8_t *chars = nullptr;                // chars[offsets[0] .. offsets[n])
     long long *offsets = nullptr;
     uint8_t *mask = nullptr, *bitmap = nullptr;   // at most one: validity_span's bytes
     int bit0 = 0;                            // cell 0's bit in bitmap[0]
-    std::vector<int64_t> rebased;            // what the offsets were copied from: kept until the call synchronises
 };
 
-// rebase: the device offsets start at 0 (rebased on the host when offsets[0] != 0), else they are copied as given
-TextDev stage_text(HostCall &c, const uint8_t *chars, const int64_t *offsets, const lo_validity *validity, int64_t n,
-                   bool rebase) {
-    TextDev d;
+// A checked text column copied into c's scratch.  rebased NULL: the offsets are copied as given; else they start at 0
+// on the device, rebased on the host into *rebased when offsets[0] != 0 (kept by the caller until the call synchronises).
+TextCols stage_text(HostCall &c, const uint8_t *chars, const int64_t *offsets, const lo_validity *validity, int64_t n,
+                    std::vector<int64_t> *rebased) {
+    TextCols d;
     const size_t nbytes = (size_t)(offsets[n] - offsets[0]);
     size_t vbytes = 0;
     const uint8_t *valid = validity_span(validity, n, &vbytes);
@@ -823,11 +825,11 @@ TextDev stage_text(HostCall &c, const uint8_t *chars, const int64_t *offsets, co
     c.alloc(&d.offsets, (size_t)(n + 1) * 8);
     if (vbytes) c.alloc(d_valid, vbytes);
     c.to_dev(d.chars, chars + offsets[0], nbytes);
-    if (rebase && offsets[0] != 0) {
-        d.rebased.resize(n + 1);
-        for (int64_t i = 0; i <= n; ++i) d.rebased[i] = offsets[i] - offsets[0];
+    if (rebased && offsets[0] != 0) {
+        rebased->resize(n + 1);
+        for (int64_t i = 0; i <= n; ++i) (*rebased)[i] = offsets[i] - offsets[0];
     }
-    c.to_dev(d.offsets, d.rebased.empty() ? offsets : d.rebased.data(), (size_t)(n + 1) * 8);
+    c.to_dev(d.offsets, rebased && !rebased->empty() ? rebased->data() : offsets, (size_t)(n + 1) * 8);
     c.to_dev(*d_valid, valid, vbytes);
     if (d.bitmap) d.bit0 = (int)(validity->bit_offset & 7);
     return d;
@@ -1399,17 +1401,29 @@ int check_project_host(const double *const *in_cols, int64_t nrows, int32_t k, f
     return LO_OK;
 }
 
-// The rest of lo_value_counts_*_host once the input is on the device.  count_and_compact(keys, counts, slots, out,
-// out_n) launches the two kernels of the hash group-by: count into a table of `slots` slots (keys all ones, counts
-// zero), then compact the groups into out[0 .. out_n) (keys) and out[out_n .. 2 out_n) (counts), at most `capacity`
-// of them, and their number into out[2 out_n].  The first min(groups, capacity) of them are copied out.  nlaunch: the
-// kernels count_and_compact launches.
-template <typename CountAndCompact>
-int value_counts_tail(HostCall &c, int64_t n, void *keys_out, uint64_t *counts_out, int64_t capacity, int64_t *ndistinct,
-                      lo_host_timing *timing, CountAndCompact count_and_compact, int nlaunch = 2) {
+// The output checks of every lo_value_counts_* call that returns groups, in the order they refuse: a negative capacity
+// and a NULL ndistinct, after which *ndistinct is 0 until the groups are counted ...
+int check_ndistinct(int64_t capacity, int64_t *ndistinct) {
+    if (capacity < 0) return fail(LO_ERR_INVALID, "negative size");
+    if (!ndistinct) return fail(LO_ERR_INVALID, "ndistinct is NULL");
+    *ndistinct = 0;
+    return LO_OK;
+}
+
+// ... then, once there is something to count, NULL outputs with room for groups
+int check_groups_out(int64_t capacity, const void *keys_out, const uint64_t *counts_out) {
+    if (capacity > 0 && (!keys_out || !counts_out)) return fail(LO_ERR_INVALID, "NULL argument");
+    return LO_OK;
+}
+
+// The device half of the hash group-by of n rows.  launch(keys, counts, slots, out, out_n) enqueues the nlaunch kernels
+// that count into a table of `slots` slots (keys all ones, counts zero), then compact at most out_n groups into
+// out[0 .. out_n) (keys) and out[out_n .. 2 out_n) (counts) and the number of groups into out[2 out_n].  Returns out,
+// in c's scratch; the table goes back to the pool in stream order.
+template <typename Launch>
+unsigned long long *count_groups(HostCall &c, int64_t n, size_t out_n, Launch launch, int nlaunch = 2) {
     unsigned long long slots = 1024;
     while (slots < 2ull * (unsigned long long)n) slots <<= 1;
-    const size_t out_n = (size_t)std::max<int64_t>(capacity, 1);
     unsigned long long *d_keys = nullptr, *d_counts = nullptr, *d_out = nullptr;
     c.alloc(&d_keys, slots * 8);
     c.alloc(&d_counts, slots * 8);
@@ -1418,14 +1432,23 @@ int value_counts_tail(HostCall &c, int64_t n, void *keys_out, uint64_t *counts_o
     c.memset(d_keys, 0xFF, slots * 8);
     c.memset(d_counts, 0, slots * 8);
     c.memset(d_out + 2 * out_n, 0, 8);
-    c.launch(nlaunch, [&] { count_and_compact(d_keys, d_counts, slots, d_out, out_n); });
+    c.launch(nlaunch, [&] { launch(d_keys, d_counts, slots, d_out, out_n); });
     c.mark();
+    c.drop(d_keys);
+    c.drop(d_counts);
+    return d_out;
+}
+
+// The host half: the first min(groups, capacity) groups of count_groups' out (out_n = capacity) copied out and the call
+// finished.  More groups than capacity is refused after *ndistinct is set, so the caller can retry larger.
+int copy_groups(HostCall &c, const unsigned long long *out, int64_t capacity, void *keys_out, uint64_t *counts_out,
+                int64_t *ndistinct, lo_host_timing *timing) {
     unsigned long long nd = 0;
-    c.to_host(&nd, d_out + 2 * out_n, 8);
+    c.to_host(&nd, out + 2 * capacity, 8);
     c.sync();
     const size_t take = (size_t)std::min<unsigned long long>(nd, (unsigned long long)capacity);
-    c.to_host(keys_out, d_out, take * 8);
-    c.to_host(counts_out, d_out + out_n, take * 8);
+    c.to_host(keys_out, out, take * 8);
+    c.to_host(counts_out, out + capacity, take * 8);
     LO_TRY(c.finish(timing));
     *ndistinct = (int64_t)nd;
     if ((int64_t)nd > capacity)
@@ -1433,18 +1456,35 @@ int value_counts_tail(HostCall &c, int64_t n, void *keys_out, uint64_t *counts_o
     return LO_OK;
 }
 
-// value_counts_tail of a text column already on the device (offsets[0] == 0; validity as k_hash_count_str reads it):
-// the call of lo_value_counts_str_host after its copies, and all of lo_value_counts_text.
-int value_counts_str_tail(HostCall &c, const uint8_t *d_chars, const long long *d_off, const uint8_t *d_mask,
-                          const uint8_t *d_bitmap, int bit0, int64_t n, int64_t *rep_rows_out, uint64_t *counts_out,
-                          int64_t capacity, int64_t *ndistinct, lo_host_timing *timing) {
-    return value_counts_tail(c, n, rep_rows_out, counts_out, capacity, ndistinct, timing,
-        [&](unsigned long long *slots_keys, unsigned long long *counts, unsigned long long slots, unsigned long long *out, size_t out_n) {
-            const int grid = (int)std::min<int64_t>((n + 255) / 256, (int64_t)c.ctx->sm_count * 8);
-            lo::k_hash_count_str<<<grid, 256, 0, c.s>>>(d_chars, d_off, n, d_mask, d_bitmap, bit0, slots_keys, counts, slots - 1);
-            lo::k_hash_compact_str<<<c.ctx->sm_count * 8, 256, 0, c.s>>>(slots_keys, counts, slots, (long long *)out, out + out_n,
-                                                                          (unsigned long long)capacity, out + 2 * out_n);
+// The rest of a lo_value_counts_* call once its input is on the device: at most `capacity` groups, copied out.
+template <typename Launch>
+int value_counts_tail(HostCall &c, int64_t n, void *keys_out, uint64_t *counts_out, int64_t capacity, int64_t *ndistinct,
+                      lo_host_timing *timing, Launch launch, int nlaunch = 2) {
+    const unsigned long long *out = count_groups(c, n, (size_t)capacity, launch, nlaunch);
+    return copy_groups(c, out, capacity, keys_out, counts_out, ndistinct, timing);
+}
+
+// blocks of 256 threads for n items, at most 8 per SM
+int grid_for(const lo_ctx *ctx, int64_t n) { return (int)std::min<int64_t>((n + 255) / 256, (int64_t)ctx->sm_count * 8); }
+
+// count_groups of the n cells of a text column on the device (offsets[0] == 0; validity as k_hash_count_str reads
+// it): the keys are the groups' representative rows
+unsigned long long *count_text_groups(HostCall &c, const TextCols &t, int64_t n, size_t out_n) {
+    return count_groups(c, n, out_n,
+        [&](unsigned long long *slots_keys, unsigned long long *counts, unsigned long long slots, unsigned long long *out, size_t) {
+            lo::k_hash_count_str<<<grid_for(c.ctx, n), 256, 0, c.s>>>(t.chars, t.offsets, n, t.mask, t.bitmap, t.bit0,
+                                                                       slots_keys, counts, slots - 1);
+            lo::k_hash_compact_str<<<c.ctx->sm_count * 8, 256, 0, c.s>>>(slots_keys, counts, slots, (long long *)out,
+                                                                          out + out_n, (unsigned long long)out_n, out + 2 * out_n);
         });
+}
+
+// the groups of a text column already on the device: the call of lo_value_counts_str_host after its copies, and all of
+// lo_value_counts_text
+int value_counts_str_tail(HostCall &c, const TextCols &t, int64_t n, int64_t *rep_rows_out, uint64_t *counts_out,
+                          int64_t capacity, int64_t *ndistinct, lo_host_timing *timing) {
+    const unsigned long long *out = count_text_groups(c, t, n, (size_t)capacity);
+    return copy_groups(c, out, capacity, rep_rows_out, counts_out, ndistinct, timing);
 }
 
 // value_counts_tail of rows [0, n) of a number column already on the device: the call of lo_value_counts_f64_host after
@@ -1459,7 +1499,7 @@ int value_counts_f64_tail(HostCall &c, const double *d_val, int64_t n, double *k
             else
                 lo::k_group_f64<false><<<grid, 256, 0, c.s>>>(d_val, n, keys, counts, slots - 1);
             lo::k_hash_compact<<<c.ctx->sm_count * 8, 256, 0, c.s>>>(keys, counts, slots, out, out + out_n,
-                                                                      (unsigned long long)capacity, out + 2 * out_n);
+                                                                      (unsigned long long)out_n, out + 2 * out_n);
         });
 }
 
@@ -1471,10 +1511,7 @@ static_assert(lo::kStrStageSlots == LO_TEXT_STAGE_SLOTS, "loexec.h documents the
 // bytes, or the bitmap bytes covering the column with the first cell at bit bit0), all from the stream-ordered pool
 struct lo_text {
     lo_ctx *ctx;
-    uint8_t *chars;
-    long long *offsets;
-    uint8_t *mask, *bitmap;
-    int bit0;
+    TextCols cols;
     int64_t n, nbytes, nulls;
     size_t device_bytes;
 };
@@ -1537,11 +1574,11 @@ int lo_value_counts_u32_host(lo_ctx *ctx, const uint32_t *codes, int64_t nrows, 
 int lo_value_counts_f64_host(lo_ctx *ctx, const double *values, int64_t n, double *keys_out, uint64_t *counts_out,
                              int64_t capacity, int64_t *ndistinct, lo_host_timing *timing) {
     LO_TRY(check_ctx(ctx));
-    if (n < 0 || capacity < 0) return fail(LO_ERR_INVALID, "negative size");
-    if (!ndistinct) return fail(LO_ERR_INVALID, "ndistinct is NULL");
-    *ndistinct = 0;
+    if (n < 0) return fail(LO_ERR_INVALID, "negative size");
+    LO_TRY(check_ndistinct(capacity, ndistinct));
     if (n == 0) return LO_OK;
-    if (!values || (capacity > 0 && (!keys_out || !counts_out))) return fail(LO_ERR_INVALID, "NULL argument");
+    if (!values) return fail(LO_ERR_INVALID, "NULL argument");
+    LO_TRY(check_groups_out(capacity, keys_out, counts_out));
     HostCall c(ctx, "value_counts_f64");
     double *d_val = nullptr;
     c.alloc(&d_val, (size_t)n * 8);
@@ -1557,11 +1594,9 @@ int lo_value_counts_f64_table(lo_ctx *ctx, const lo_table *t, int32_t col, doubl
     if (t->device != ctx->device) return fail(LO_ERR_INVALID, "table lives on device %d, the context on %d", t->device, ctx->device);
     if (t->dtype != LO_F64) return fail(LO_ERR_INVALID, "table dtype %d is not LO_F64", t->dtype);
     if (col < 0 || col >= t->ncols) return fail(LO_ERR_INVALID, "column %d outside [0, %d)", col, t->ncols);
-    if (capacity < 0) return fail(LO_ERR_INVALID, "negative size");
-    if (!ndistinct) return fail(LO_ERR_INVALID, "ndistinct is NULL");
-    *ndistinct = 0;
+    LO_TRY(check_ndistinct(capacity, ndistinct));
     if (t->nrows == 0) return LO_OK;
-    if (capacity > 0 && (!keys_out || !counts_out)) return fail(LO_ERR_INVALID, "NULL argument");
+    LO_TRY(check_groups_out(capacity, keys_out, counts_out));
     HostCall c(ctx, "value_counts_f64_table");
     return value_counts_f64_tail(c, (const double *)(t->base + (int64_t)col * t->pitch), t->nrows, keys_out, counts_out,
                                  capacity, ndistinct, timing);
@@ -1572,18 +1607,16 @@ int lo_value_counts_f64_table(lo_ctx *ctx, const lo_table *t, int32_t col, doubl
 int lo_value_counts_str_host(lo_ctx *ctx, const uint8_t *chars, const int64_t *offsets, int64_t n, int64_t *rep_rows_out,
                              uint64_t *counts_out, int64_t capacity, int64_t *ndistinct, lo_host_timing *timing) {
     LO_TRY(check_ctx(ctx));
-    if (n < 0 || capacity < 0) return fail(LO_ERR_INVALID, "negative size");
-    if (!ndistinct) return fail(LO_ERR_INVALID, "ndistinct is NULL");
-    *ndistinct = 0;
+    if (n < 0) return fail(LO_ERR_INVALID, "negative size");
+    LO_TRY(check_ndistinct(capacity, ndistinct));
     if (n == 0) return LO_OK;
-    if (capacity > 0 && (!rep_rows_out || !counts_out)) return fail(LO_ERR_INVALID, "NULL argument");
+    LO_TRY(check_groups_out(capacity, rep_rows_out, counts_out));
     LO_TRY(check_text_in(chars, offsets, nullptr, n, kGroupRowBits));
     if (offsets[0] != 0) return fail(LO_ERR_INVALID, "offsets[0] must be 0");
     LO_TRY(check_ascending(offsets, n));
     HostCall c(ctx, "value_counts_str");
-    const TextDev d = stage_text(c, chars, offsets, nullptr, n, true);
-    return value_counts_str_tail(c, d.chars, d.offsets, nullptr, nullptr, 0, n, rep_rows_out, counts_out, capacity,
-                                 ndistinct, timing);
+    const TextCols d = stage_text(c, chars, offsets, nullptr, n, nullptr);    // offsets[0] is 0: copied as given
+    return value_counts_str_tail(c, d, n, rep_rows_out, counts_out, capacity, ndistinct, timing);
 }
 
 // ---- text columns resident in HBM ---------------------------------------------------------------------------------
@@ -1615,11 +1648,12 @@ int lo_text_upload(lo_ctx *ctx, const uint8_t *chars, const int64_t *offsets, co
     std::unique_ptr<lo_text> t(new (std::nothrow) lo_text);
     if (!t) return fail(LO_ERR_NOMEM, "out of host memory");
     HostCall c(ctx, "text_upload");
-    const TextDev d = stage_text(c, chars, offsets, validity, n, true);
+    std::vector<int64_t> rebased;
+    const TextCols d = stage_text(c, chars, offsets, validity, n, &rebased);
     for (const void *p : {(const void *)d.chars, (const void *)d.offsets, (const void *)d.mask, (const void *)d.bitmap})
         c.keep(p);
     LO_TRY(c.finish(timing));                // synchronises: the host buffers may go
-    *t = lo_text{ctx, d.chars, d.offsets, d.mask, d.bitmap, d.bit0, n, nbytes, nulls, need};
+    *t = lo_text{ctx, d, n, nbytes, nulls, need};
     *out = t.release();
     return LO_OK;
 }
@@ -1637,7 +1671,7 @@ int lo_text_free(lo_ctx *ctx, lo_text *t) {
     if (!t) return LO_OK;
     LO_TRY(check_ctx(ctx));
     if (t->ctx != ctx) return fail(LO_ERR_INVALID, "text belongs to another context");
-    for (void *p : {(void *)t->chars, (void *)t->offsets, (void *)t->mask, (void *)t->bitmap})
+    for (void *p : {(void *)t->cols.chars, (void *)t->cols.offsets, (void *)t->cols.mask, (void *)t->cols.bitmap})
         if (p) cudaFreeAsync(p, ctx->stream);
     delete t;
     return LO_OK;
@@ -1648,14 +1682,11 @@ int lo_value_counts_text(lo_ctx *ctx, const lo_text *t, int64_t *rep_rows_out, u
     LO_TRY(check_ctx(ctx));
     if (!t) return fail(LO_ERR_INVALID, "text is NULL");
     if (t->ctx != ctx) return fail(LO_ERR_INVALID, "text belongs to another context");
-    if (capacity < 0) return fail(LO_ERR_INVALID, "negative size");
-    if (!ndistinct) return fail(LO_ERR_INVALID, "ndistinct is NULL");
-    *ndistinct = 0;
+    LO_TRY(check_ndistinct(capacity, ndistinct));
     if (t->n == t->nulls) return LO_OK;      // no cell to count (n == 0 included)
-    if (capacity > 0 && (!rep_rows_out || !counts_out)) return fail(LO_ERR_INVALID, "NULL argument");
+    LO_TRY(check_groups_out(capacity, rep_rows_out, counts_out));
     HostCall c(ctx, "value_counts_text");
-    return value_counts_str_tail(c, t->chars, t->offsets, t->mask, t->bitmap, t->bit0, t->n, rep_rows_out, counts_out,
-                                 capacity, ndistinct, timing);
+    return value_counts_str_tail(c, t->cols, t->n, rep_rows_out, counts_out, capacity, ndistinct, timing);
 }
 
 }  // extern "C"
@@ -1668,7 +1699,7 @@ struct TextShard {
     int64_t row0;
     int64_t cap;                             // n - nulls: at most this many groups
     std::unique_ptr<HostCall> c;
-    unsigned long long *grp = nullptr;       // compacted groups: rows [0, cap), counts [cap, 2 cap), their number [2 cap]
+    unsigned long long *grp = nullptr;       // count_text_groups' out: rows [0, cap), counts [cap, 2 cap), their number [2 cap]
     long long *key_off = nullptr;            // the packed key column of its groups: nd + 1 offsets, then the bytes
     uint8_t *key_chars = nullptr;
     cudaEvent_t gathered = nullptr;          // the packed pieces are ready to copy
@@ -1682,7 +1713,7 @@ extern "C" {
 
 // Value counts of one text column cut into row-range shards, each resident on its own context (loexec.h).  Four steps,
 // each enqueued on every shard before the host waits on any, so shards on different devices run at once:
-//   1. count and compact each shard on its device (k_hash_count_str, k_hash_compact_str); the host reads its group count;
+//   1. count and compact each shard on its device (count_text_groups); the host reads its group count;
 //   2. the byte lengths of its groups' cells and their exclusive scan; the host reads its key bytes;
 //   3. k_gather_cells packs the keys, rebases their offsets into the concatenated column and makes the rows global;
 //   4. the root waits on each shard's event, copies the packed pieces over with cudaMemcpyPeerAsync, and merges them
@@ -1696,104 +1727,68 @@ int lo_value_counts_text_shards(lo_ctx *root, const lo_text *const *shards, cons
     if (nshards < 1 || nshards > LO_GROUP_MAX_DEVICES)
         return fail(LO_ERR_INVALID, "nshards = %d: 1 to %d shards", nshards, LO_GROUP_MAX_DEVICES);
     if (!shards || !row0) return fail(LO_ERR_INVALID, "shards or row0 is NULL");
-    int64_t cells = 0;
+    std::vector<TextShard> sh;               // the shards with a cell to count
     for (int i = 0; i < nshards; ++i) {
         if (!shards[i]) return fail(LO_ERR_INVALID, "shards[%d] is NULL", i);
         if (row0[i] < 0) return fail(LO_ERR_INVALID, "row0[%d] = %lld is negative", i, (long long)row0[i]);
         if (i > 0 && row0[i] < row0[i - 1] + shards[i - 1]->n)
             return fail(LO_ERR_INVALID, "row0[%d] = %lld: shard %d ends at row %lld (shards are disjoint and in row order)",
                         i, (long long)row0[i], i - 1, (long long)(row0[i - 1] + shards[i - 1]->n));
-        cells += shards[i]->n - shards[i]->nulls;
+        if (shards[i]->n > shards[i]->nulls) sh.push_back(TextShard{shards[i], row0[i], shards[i]->n - shards[i]->nulls});
     }
-    if (capacity < 0) return fail(LO_ERR_INVALID, "negative size");
-    if (!ndistinct) return fail(LO_ERR_INVALID, "ndistinct is NULL");
-    *ndistinct = 0;
-    if (cells == 0) return LO_OK;            // no cell to count
-    if (capacity > 0 && (!rep_rows_out || !counts_out)) return fail(LO_ERR_INVALID, "NULL argument");
+    LO_TRY(check_ndistinct(capacity, ndistinct));
+    if (sh.empty()) return LO_OK;
+    LO_TRY(check_groups_out(capacity, rep_rows_out, counts_out));
     LO_TRY(check_ctx(root));
     HostCall c(root, "value_counts_text_shards");
-    std::vector<TextShard> sh;
-    for (int i = 0; i < nshards; ++i)
-        if (shards[i]->n > shards[i]->nulls) sh.push_back(TextShard{shards[i], row0[i], shards[i]->n - shards[i]->nulls});
-    auto all_ok = [&] {
-        for (const TextShard &s : sh)
-            if (!s.c->ok()) return false;
-        return true;
+    for (TextShard &s : sh) s.c = std::make_unique<HostCall>(s.t->ctx, "value_counts_text_shards", false);
+    auto ok = [&] { return c.ok() && std::all_of(sh.begin(), sh.end(), [](const TextShard &s) { return s.c->ok(); }); };
+    // step(s, its call frame) for every shard in row order, on the shard's device, until the root or a shard fails
+    auto each_shard = [&](auto step) {
+        for (TextShard &s : sh) {
+            if (!ok()) return;
+            s.c->run([&] { return cudaSetDevice(s.t->ctx->device); });
+            step(s, *s.c);
+        }
     };
-    auto grid_for = [](lo_ctx *ctx, int64_t n) { return (int)std::min<int64_t>((n + 255) / 256, (int64_t)ctx->sm_count * 8); };
-
-    for (TextShard &s : sh) {                // 1. count and compact
-        lo_ctx *ctx = s.t->ctx;
-        s.c = std::make_unique<HostCall>(ctx, "value_counts_text_shards");
-        HostCall &sc = *s.c;
-        sc.run([&] { return cudaSetDevice(ctx->device); });
-        unsigned long long slots = 1024;
-        while (slots < 2ull * (unsigned long long)s.t->n) slots <<= 1;
-        unsigned long long *table = nullptr, *counts = nullptr;
-        sc.alloc(&table, slots * 8);
-        sc.alloc(&counts, slots * 8);
-        sc.alloc(&s.grp, (2 * (size_t)s.cap + 1) * 8);
-        sc.memset(table, 0xFF, slots * 8);
-        sc.memset(counts, 0, slots * 8);
-        sc.memset(s.grp + 2 * s.cap, 0, 8);
-        sc.launch(2, [&] {
-            lo::k_hash_count_str<<<grid_for(ctx, s.t->n), 256, 0, sc.s>>>(s.t->chars, s.t->offsets, s.t->n, s.t->mask,
-                                                                           s.t->bitmap, s.t->bit0, table, counts, slots - 1);
-            lo::k_hash_compact_str<<<ctx->sm_count * 8, 256, 0, sc.s>>>(table, counts, slots, (long long *)s.grp,
-                                                                         s.grp + s.cap, (unsigned long long)s.cap,
-                                                                         s.grp + 2 * s.cap);
-        });
-        sc.drop(table);
-        sc.drop(counts);
-    }
-    for (TextShard &s : sh) {
-        s.c->to_host(&s.nd, s.grp + 2 * s.cap, 8);
-        s.c->sync();
-    }
-    std::vector<size_t> scan_bytes(sh.size(), 0);
-    for (size_t i = 0; i < sh.size() && all_ok(); ++i) {   // 2. key lengths and their scan
-        TextShard &s = sh[i];
-        HostCall &sc = *s.c;
-        lo_ctx *ctx = s.t->ctx;
+    // 1. count and compact
+    each_shard([](TextShard &s, HostCall &sc) { s.grp = count_text_groups(sc, s.t->cols, s.t->n, (size_t)s.cap); });
+    each_shard([](TextShard &s, HostCall &sc) { sc.to_host(&s.nd, s.grp + 2 * s.cap, 8); sc.sync(); });
+    each_shard([](TextShard &s, HostCall &sc) {   // 2. key lengths and their scan
         const int64_t nd = (int64_t)s.nd;
+        size_t scan_bytes = 0;
         void *tmp = nullptr;
-        sc.run([&] { return cudaSetDevice(ctx->device); });
         sc.alloc(&s.key_off, (size_t)(nd + 1) * 8);
-        sc.run([&] { return cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes[i], s.key_off, nd + 1, sc.s); });
-        sc.alloc(&tmp, scan_bytes[i]);
+        sc.run([&] { return cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, s.key_off, nd + 1, sc.s); });
+        sc.alloc(&tmp, scan_bytes);
         sc.memset(s.key_off + nd, 0, 8);     // the scan's last input: key_off[nd] = the key bytes
-        sc.launch(1, [&] { lo::k_gather_lens<<<grid_for(ctx, nd), 256, 0, sc.s>>>(s.t->offsets, (const long long *)s.grp, nd, s.key_off); });
-        sc.launch(1, [&] { return cub::DeviceScan::ExclusiveSum(tmp, scan_bytes[i], s.key_off, nd + 1, sc.s); });
+        sc.launch(1, [&] { lo::k_gather_lens<<<grid_for(sc.ctx, nd), 256, 0, sc.s>>>(s.t->cols.offsets, (const long long *)s.grp, nd, s.key_off); });
+        sc.launch(1, [&] { return cub::DeviceScan::ExclusiveSum(tmp, scan_bytes, s.key_off, nd + 1, sc.s); });
         sc.drop(tmp);
-    }
+    });
     long long groups = 0, bytes = 0;
-    for (TextShard &s : sh) {
-        if (!all_ok()) break;
-        s.c->to_host(&s.bytes, s.key_off + s.nd, 8);
-        s.c->sync();
+    each_shard([&](TextShard &s, HostCall &sc) {
+        sc.to_host(&s.bytes, s.key_off + s.nd, 8);
+        sc.sync();
         s.group0 = groups;
         s.byte0 = bytes;
         groups += (long long)s.nd;
         bytes += s.bytes;
-    }
-    if (all_ok() && groups >> 31)            // the merge's slot word keeps a 31-bit key index
+    });
+    if (ok() && groups >> 31)                // the merge's slot word keeps a 31-bit key index
         c.check([&] { return fail(LO_ERR_INVALID, "the shards hold %lld groups: at most 2^31-1 can be merged", groups); });
-    for (TextShard &s : sh) {                // 3. pack the keys
-        if (!all_ok() || !c.ok()) break;
-        HostCall &sc = *s.c;
-        lo_ctx *ctx = s.t->ctx;
-        sc.run([&] { return cudaSetDevice(ctx->device); });
+    each_shard([](TextShard &s, HostCall &sc) {   // 3. pack the keys
         sc.alloc(&s.key_chars, (size_t)s.bytes);
         sc.launch(1, [&] {
-            lo::k_gather_cells<<<grid_for(ctx, (int64_t)s.nd + 1), 256, 0, sc.s>>>(
-                s.t->chars, s.t->offsets, (long long *)s.grp, (long long)s.nd, s.key_off, s.key_chars, s.row0, s.byte0);
+            lo::k_gather_cells<<<grid_for(sc.ctx, (int64_t)s.nd + 1), 256, 0, sc.s>>>(s.t->cols.chars, s.t->cols.offsets,
+                (long long *)s.grp, (long long)s.nd, s.key_off, s.key_chars, s.row0, s.byte0);
         });
         sc.run([&] { return cudaEventCreateWithFlags(&s.gathered, cudaEventDisableTiming); });
         sc.run([&] { return cudaEventRecord(s.gathered, sc.s); });
-    }
+    });
     int rc = LO_OK;
     cudaEvent_t copied = nullptr;
-    if (all_ok() && c.ok()) {                // 4. copy the pieces to the root and merge them there
+    if (ok()) {                              // 4. copy the pieces to the root and merge them there
         c.run([&] { return cudaSetDevice(root->device); });
         uint8_t *chars = nullptr;
         long long *offsets = nullptr, *rows = nullptr;
@@ -1820,10 +1815,10 @@ int lo_value_counts_text_shards(lo_ctx *root, const lo_text *const *shards, cons
                 lo::k_hash_sum_str<<<grid_for(root, groups), 256, 0, c.s>>>(chars, offsets, weight, groups, slots_keys,
                                                                              counts, slots - 1);
                 lo::k_hash_compact_str<<<root->sm_count * 8, 256, 0, c.s>>>(slots_keys, counts, slots, (long long *)out,
-                                                                             out + out_n, (unsigned long long)capacity,
+                                                                             out + out_n, (unsigned long long)out_n,
                                                                              out + 2 * out_n);
                 lo::k_take_rows<<<root->sm_count * 8, 256, 0, c.s>>>((long long *)out, rows, out + 2 * out_n,
-                                                                      (unsigned long long)capacity);
+                                                                      (unsigned long long)out_n);
             }, 3);
     } else {
         rc = c.finish(nullptr);              // synchronises the root: nothing of it reads a shard any more
@@ -1852,7 +1847,8 @@ int lo_parse_number_host(lo_ctx *ctx, const uint8_t *chars, const int64_t *offse
     LO_TRY(check_text_in(chars, offsets, nullptr, n, kAnyRowBits));
     LO_TRY(check_ascending(offsets, n));
     HostCall c(ctx, "parse_number");
-    const TextDev d = stage_text(c, chars, offsets, nullptr, n, true);
+    std::vector<int64_t> rebased;
+    const TextCols d = stage_text(c, chars, offsets, nullptr, n, &rebased);
     uint8_t *d_status = nullptr;
     unsigned long long *d_val = nullptr;
     c.alloc(&d_val, (size_t)n * 8);
@@ -1884,7 +1880,7 @@ int lo_parse_number_to_table(lo_ctx *ctx, const uint8_t *chars, const int64_t *o
     // would be one more host pass over it per shard.  The kernel rebases the offsets and reports a cell whose offsets
     // leave [offsets[0], offsets[n]] or run backwards as unsupported.
     HostCall c(ctx, "parse_number_to_table");
-    const TextDev d = stage_text(c, chars, offsets, validity, n, false);
+    const TextCols d = stage_text(c, chars, offsets, validity, n, nullptr);
     unsigned long long *d_sum = nullptr;
     c.alloc(&d_sum, 4 * 8);
     c.memset(d_sum, 0xFF, 2 * 8);

@@ -92,19 +92,24 @@ def _minmax_decode(lib, raw: np.ndarray, k: int):
     return mins, maxs, cnt
 
 
-def _value_counts(call, n: int, key_dtype):
-    """(keys, counts) of a lo_value_counts_*_host call ``call(keys_out, counts_out, capacity, ndistinct_ref)``: room
-    for min(n, 65536) groups first, called again with room for every group when they did not fit."""
+def _value_counts(call, n: int, key_dtype, timing: dict | None = None):
+    """(keys, counts) of a lo_value_counts_* call ``call(keys_out, counts_out, capacity, ndistinct_ref, timing_ref)``:
+    room for min(n, 65536) groups first, called again with room for every group when they did not fit.  ``timing``: a
+    dict to receive the last call's lo_host_timing fields; None passes no lo_host_timing."""
+    t = N.HostTiming() if timing is not None else None
     cap = max(min(n, 1 << 16), 1)
     while True:
         keys = np.empty(cap, dtype=key_dtype)
         counts = np.empty(cap, dtype=np.uint64)
         nd = C.c_int64()
-        rc = call(keys.ctypes.data_as(C.c_void_p), counts.ctypes.data_as(C.c_void_p), cap, C.byref(nd))
+        rc = call(keys.ctypes.data_as(C.c_void_p), counts.ctypes.data_as(C.c_void_p), cap, C.byref(nd),
+                  C.byref(t) if t is not None else None)
         if rc == N.LO_ERR_INVALID and nd.value > cap:
             cap = int(nd.value)
             continue
         N.check(rc)
+        if t is not None:
+            timing.update(_timing(t), kernel_ms=t.kernel_ms)
         return keys[:nd.value], counts[:nd.value]
 
 
@@ -675,8 +680,8 @@ class Engine:
         n = offsets.shape[0] - 1
         if n == 0:
             return np.zeros(0, np.int64), np.zeros(0, np.uint64)
-        return _value_counts(lambda rows, counts, cap, nd: self._lib.lo_value_counts_str_host(
-            self._ctx, chars.ctypes.data_as(C.c_void_p), offsets.ctypes.data_as(C.c_void_p), n, rows, counts, cap, nd, None),
+        return _value_counts(lambda rows, counts, cap, nd, t: self._lib.lo_value_counts_str_host(
+            self._ctx, chars.ctypes.data_as(C.c_void_p), offsets.ctypes.data_as(C.c_void_p), n, rows, counts, cap, nd, t),
             n, np.int64)
 
     def text(self, cells, timing: dict | None = None) -> DeviceText:
@@ -705,32 +710,24 @@ class Engine:
         n = text.n - text.nulls
         if n == 0:
             return np.zeros(0, np.int64), np.zeros(0, np.uint64)
-        t = N.HostTiming()
-        out = _value_counts(lambda rows, counts, cap, nd: self._lib.lo_value_counts_text(
-            self._ctx, text._h, rows, counts, cap, nd, C.byref(t)), n, np.int64)
-        if timing is not None:
-            timing.update(_timing(t), kernel_ms=t.kernel_ms)
-        return out
+        return _value_counts(lambda rows, counts, cap, nd, t: self._lib.lo_value_counts_text(
+            self._ctx, text._h, rows, counts, cap, nd, t), n, np.int64, timing)
 
     def value_counts_f64_host(self, values: np.ndarray):
         """(keys float64[g], counts uint64[g]) — exact value counts of a numeric column (GPU hash group-by),
         -0.0 grouped with 0.0 and all NaNs together; order unspecified."""
         values = np.ascontiguousarray(values, dtype=np.float64)
         n = values.shape[0]
-        return _value_counts(lambda keys, counts, cap, nd: self._lib.lo_value_counts_f64_host(
-            self._ctx, values.ctypes.data_as(C.c_void_p), n, keys, counts, cap, nd, None), n, np.float64)
+        return _value_counts(lambda keys, counts, cap, nd, t: self._lib.lo_value_counts_f64_host(
+            self._ctx, values.ctypes.data_as(C.c_void_p), n, keys, counts, cap, nd, t), n, np.float64)
 
     def value_counts_column(self, table: DeviceTable, col: int, timing: dict | None = None):
         """(keys float64[g], counts uint64[g]) of rows [0, nrows) of f64 column ``col`` of a device table
         (``lo_value_counts_f64_table``): the same groups as :meth:`value_counts_f64_host` with nothing copied to the
         device.  A null stored as NaN in the slab counts under the NaN key.  ``timing``: a dict to receive the (last)
         call's lo_host_timing fields."""
-        t = N.HostTiming()
-        out = _value_counts(lambda keys, counts, cap, nd: self._lib.lo_value_counts_f64_table(
-            self._ctx, table._h, int(col), keys, counts, cap, nd, C.byref(t)), table.nrows, np.float64)
-        if timing is not None:
-            timing.update(_timing(t), kernel_ms=t.kernel_ms)
-        return out
+        return _value_counts(lambda keys, counts, cap, nd, t: self._lib.lo_value_counts_f64_table(
+            self._ctx, table._h, int(col), keys, counts, cap, nd, t), table.nrows, np.float64, timing)
 
     def minmax_cast(self, table: DeviceTable, col_idx, stream=None):
         """(min, max, n_finite) of the fp32-cast values of resident columns (range pre-pass on the device)."""

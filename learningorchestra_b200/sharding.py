@@ -63,6 +63,33 @@ def column_batches(k: int, nbins: int, cap: int | None = None) -> list[tuple[int
     return [(c0, min(k, c0 + per)) for c0 in range(0, k, per)]
 
 
+def on_each(n: int, fn, undo=None) -> list:
+    """``[fn(0), ..., fn(n - 1)]``, each member's call on a host thread of its own so the devices work at once.  Every
+    call runs to its end; when any raised, ``undo`` (if given) is called on each result the others returned and the
+    first exception in member order is raised."""
+    results, errors = [None] * n, [None] * n
+
+    def run(i):
+        try:
+            results[i] = fn(i)
+        except BaseException as exc:       # re-raised on the calling thread
+            errors[i] = exc
+
+    threads = [threading.Thread(target=run, args=(i,)) for i in range(n)]
+    for th in threads:
+        th.start()
+    for th in threads:
+        th.join()
+    failed = [e for e in errors if e is not None]
+    if failed:
+        if undo is not None:
+            for r, e in zip(results, errors):
+                if e is None:
+                    undo(r)
+        raise failed[0]
+    return results
+
+
 def _combine_timings(parts) -> dict:
     out = dict(parts[0])
     for t in parts[1:]:
@@ -175,26 +202,13 @@ class ShardedText:
         ``bounds``, each from a host thread of its own.  When any upload fails (LO_ERR_NOMEM on a full device, say) the
         pieces already made are freed and the first error is raised.  ``timing``: the longest piece's times, the
         pieces' bytes and launches added up."""
-        parts, times = [None] * len(engines), [{} for _ in engines]
+        times = [{} for _ in engines]
 
         def run(i):
             b, e = bounds[i]
-            try:
-                parts[i] = engines[i].text(arr.slice(b, e - b), timing=times[i])
-            except BaseException as exc:       # re-raised on the calling thread
-                parts[i] = exc
+            return engines[i].text(arr.slice(b, e - b), timing=times[i])
 
-        threads = [threading.Thread(target=run, args=(i,)) for i in range(len(engines))]
-        for th in threads:
-            th.start()
-        for th in threads:
-            th.join()
-        failed = [p for p in parts if isinstance(p, BaseException)]
-        if failed:
-            for p in parts:
-                if p is not None and not isinstance(p, BaseException):
-                    p.free()
-            raise failed[0]
+        parts = on_each(len(engines), run, undo=lambda p: p.free())
         if timing is not None:
             timing.update({k: max(t[k] for t in times) for k in ("total_ms", "kernel_ms")},
                           **{k: sum(t[k] for t in times) for k in ("h2d_bytes", "d2h_bytes", "launches")})
@@ -490,25 +504,12 @@ class ShardedEngine:
                 return nulls[0], int(nulls[1]) + off
             return nulls[off:off + nr]
 
-        parts = [None] * self.nlocal
-
         def run(i):
             t, off = table.shards[i], table.offsets[i]
-            try:
-                parts[i] = self.engines[i].parse_number_into(t, col, chars, offsets[off:off + t.nrows + 1],
-                                                             shard_nulls(off, t.nrows))
-            except BaseException as exc:       # re-raised on the calling thread
-                parts[i] = exc
+            return self.engines[i].parse_number_into(t, col, chars, offsets[off:off + t.nrows + 1],
+                                                     shard_nulls(off, t.nrows))
 
-        threads = [threading.Thread(target=run, args=(i,)) for i in range(self.nlocal)]
-        for th in threads:
-            th.start()
-        for th in threads:
-            th.join()
-        for p in parts:
-            if isinstance(p, BaseException):
-                raise p
-        return combine_parse_summaries(parts, table.offsets)
+        return combine_parse_summaries(on_each(self.nlocal, run), table.offsets)
 
     def value_counts_column(self, table: ShardedTable, col: int):
         """``Engine.value_counts_column`` over a sharded table: every local shard is counted on its own device from a
@@ -517,23 +518,7 @@ class ShardedEngine:
         if self.world > self.nlocal:
             raise self._N.LoexecError(self._N.LO_ERR_INVALID, f"value_counts_column needs every row: this process holds "
                                       f"{self.nlocal} of the group's {self.world} shards")
-        parts = [None] * self.nlocal
-
-        def run(i):
-            try:
-                parts[i] = self.engines[i].value_counts_column(table.shards[i], col)
-            except BaseException as exc:       # re-raised on the calling thread
-                parts[i] = exc
-
-        threads = [threading.Thread(target=run, args=(i,)) for i in range(self.nlocal)]
-        for th in threads:
-            th.start()
-        for th in threads:
-            th.join()
-        for p in parts:
-            if isinstance(p, BaseException):
-                raise p
-        return merge_value_counts(parts)
+        return merge_value_counts(on_each(self.nlocal, lambda i: self.engines[i].value_counts_column(table.shards[i], col)))
 
     # ---- host buffers -------------------------------------------------------------------------------------
     def project_cast_hist_host(self, cols, nbins: int | None = None, lo=None, hi=None, out=None, bcast: bool = False):
@@ -625,21 +610,17 @@ class ShardedEngine:
         if not isinstance(text, ShardedText):
             return self.engines[0].value_counts_text(text, timing)
         import numpy as np
-        from .engine import _timing, _value_counts
+        from .engine import _value_counts
         if any(p._h is None for p in text.pieces):
             raise ValueError("the text column has been freed")
         n = text.n - text.nulls
         if n == 0:
             return np.zeros(0, np.int64), np.zeros(0, np.uint64)
-        N, k = self._N, len(text.pieces)
+        k = len(text.pieces)
         handles = (C.c_void_p * k)(*[p._h for p in text.pieces])
         row0 = (C.c_int64 * k)(*text.offsets)
-        t = N.HostTiming()
-        out = _value_counts(lambda rows, counts, cap, nd: self._lib.lo_value_counts_text_shards(
-            self.engines[0]._ctx, handles, row0, k, rows, counts, cap, nd, C.byref(t)), n, np.int64)
-        if timing is not None:
-            timing.update(_timing(t), kernel_ms=t.kernel_ms)
-        return out
+        return _value_counts(lambda rows, counts, cap, nd, t: self._lib.lo_value_counts_text_shards(
+            self.engines[0]._ctx, handles, row0, k, rows, counts, cap, nd, t), n, np.int64, timing)
 
     @property
     def resident(self):

@@ -55,16 +55,12 @@ def timed(call, reps):
 
 
 def shards_call(eng, pieces, row0, n, timing):
-    from learningorchestra_b200 import _native as N
-    from learningorchestra_b200.engine import _timing, _value_counts
+    from learningorchestra_b200.engine import _value_counts
     k = len(pieces)
     handles = (C.c_void_p * k)(*[p._h for p in pieces])
     r0 = (C.c_int64 * k)(*row0)
-    t = N.HostTiming()
-    out = _value_counts(lambda rows, counts, cap, nd: eng._lib.lo_value_counts_text_shards(
-        eng._ctx, handles, r0, k, rows, counts, cap, nd, C.byref(t)), n, np.int64)
-    timing.update(_timing(t), kernel_ms=t.kernel_ms)
-    return out
+    return _value_counts(lambda rows, counts, cap, nd, t: eng._lib.lo_value_counts_text_shards(
+        eng._ctx, handles, r0, k, rows, counts, cap, nd, t), n, np.int64, timing)
 
 
 def column_numbers(eng, arr, cuts, reps):

@@ -3,6 +3,8 @@ Each rank computes its shard's partial histogram with the ORACLE (there is no GP
 test is the sharding arithmetic and the reduction plumbing that bench.py / the executors use on NCCL."""
 import os
 import socket
+import threading
+import time
 
 import numpy as np
 import pytest
@@ -10,7 +12,7 @@ import torch
 import torch.distributed as dist
 import torch.multiprocessing as mp
 
-from learningorchestra_b200.sharding import all_shard_bounds, allreduce_counts, column_batches, shard_bounds
+from learningorchestra_b200.sharding import all_shard_bounds, allreduce_counts, column_batches, on_each, shard_bounds
 
 SEED = 20260921
 GROUP_CAP = 262144          # LO_GROUP_MAX_COUNTS
@@ -50,6 +52,36 @@ def test_shard_bounds_cover_and_align():
     assert shard_bounds(100_000_000, 8, 3) == (37_500_000, 50_000_000)
     with pytest.raises(ValueError):
         shard_bounds(10, 2, 2)
+
+
+def test_on_each_runs_every_member_at_once_and_undoes_the_results_of_a_failed_fan_out():
+    n = 5
+    together = threading.Barrier(n, timeout=30)      # breaks unless all members are running at the same time
+
+    def square(i):
+        together.wait()
+        time.sleep(0.01 * (n - i))                   # the last member finishes first
+        return i * i
+
+    assert on_each(n, square) == [i * i for i in range(n)]
+    assert on_each(0, square) == []
+
+    ran, undone, lock = [], [], threading.Lock()
+
+    def some_fail(i):
+        time.sleep(0.01 * (n - i))
+        with lock:
+            ran.append(i)
+        if i in (1, 3):                              # member 3 raises first, member 1 comes first in member order
+            raise ValueError(f"member {i}")
+        return {"member": i}
+
+    with pytest.raises(ValueError, match="member 1"):
+        on_each(n, some_fail, undo=undone.append)
+    assert sorted(ran) == list(range(n))
+    assert sorted(r["member"] for r in undone) == [0, 2, 4]
+    with pytest.raises(ValueError, match="member 1"):
+        on_each(n, some_fail)                        # no undo: the first failure still comes back
 
 
 def _free_port():
