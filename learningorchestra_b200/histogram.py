@@ -11,20 +11,21 @@ Here the counting runs on the GPU with no host dictionary:
   as in MongoDB) over the field's slab kept resident in HBM (``table_cache``, ``lo_value_counts_f64_table``; a slab
   already made resident by a binned or ``castTo`` request is counted as it is), leased with the text columns.  Nulls
   are NaN in the slab: the NaN key's count less the null rows is the group of real NaNs, and the ``null`` group is the
-  null rows plus the documents that are not data rows.  Keys are typed by the host route's rule (a column store's
-  ``integers_collapsed``, a document store's ``numeric_column`` kind).  A rank group's process holds only its own
-  rows, and a field set on a document that is not a data row is not in the slab: both pack the values per request
-  (``lo_value_counts_f64_host``);
+  null rows plus the documents that are not data rows.  Keys are typed by the store's rule, which ``table_cache``
+  applies.  A rank group's process holds only its own rows, and a field set on a document that is not a data row is
+  not in the slab: both take the host route;
 * text fields (every value a ``str`` / None — every field of a fresh ``POST /files`` upload): GPU hash group-by on the
   cells' bytes over the field's text column kept resident in HBM (``table_cache``, ``lo_value_counts_text``), leased
   for the request.  The first request uploads the column; later ones copy no cell to the device and read no document.
   Group keys are read from the host's Arrow array at the representative rows; the ``null`` group is the column's null
   cells plus the documents that are not data rows (the metadata document);
 * mixed-type fields: the byte-wise group-by over a tagged encoding under which two cells are equal exactly
-  when MongoDB groups them (:func:`columnar.tagged_cell`: 1 == 1.0, ``True`` != 1, ``"1"`` != 1), packed per request
-  (``lo_value_counts_str_host``).
+  when MongoDB groups them (:func:`columnar.tagged_cell`: 1 == 1.0, ``True`` != 1, ``"1"`` != 1).
 
-``None`` / missing values of packed number and mixed fields are counted while packing.  With ``bins`` (optional
+What HBM does not count takes the one host route, on either store: one :class:`~table_cache.Snapshot` reads the
+dataset and says what each field is (``Snapshot.values``), and its values are packed per request — a number field's
+valid values to ``lo_value_counts_f64_host``, a text field's non-null cells or a mixed field's tagged cells to
+``lo_value_counts_str_host``.  ``None`` / missing values are counted by the reader.  With ``bins`` (optional
 extension, REST keys ``bins`` / ``range``) the fields must be numeric or text (text is parsed with ``float()`` on the
 device into the resident slab; the dataset stays text) and get the fixed-width B-semantics histogram of SURVEY.md §8c
 from the fused kernel, run on the HBM-resident copy of the dataset (``table_cache``).
@@ -39,6 +40,8 @@ from concurrent.futures import ThreadPoolExecutor
 import numpy as np
 
 from . import columnar
+from .column_store import TextColumn, large_text
+from .table_cache import Snapshot
 from .utils import record_exception
 
 
@@ -57,9 +60,9 @@ def text_groups(arr, rep, counts, none_count):
 def number_groups(keys, counts, as_int, nulls, absent):
     """Result groups of a number field counted on the device.  Counted from its slab, where a null row is NaN: the NaN
     key's count less the ``nulls`` null rows is the group of real NaNs (emitted when there are any), and the ``null``
-    group is those null rows plus the ``absent`` documents that are not data rows and lack the field.  The host routes
-    count only the values that are not null and pass 0 for both.  ``as_int``: a finite integral key is an ``int`` (the
-    store's rule: a column store's ``integers_collapsed``, a document store's ``numeric_column`` kind)."""
+    group is those null rows plus the ``absent`` documents that are not data rows and lack the field.  The host route
+    counts only the values that are not null and passes 0 for both.  ``as_int``: a finite integral key is an ``int``
+    (the store's rule, which :class:`~table_cache.Snapshot` applies)."""
     groups = []
     for k, c in zip(np.asarray(keys, np.float64).tolist(), np.asarray(counts, np.uint64).tolist()):
         if math.isnan(k):
@@ -103,12 +106,8 @@ class Histogram:
             else:
                 results = self.__value_counts_resident(parent_filename, fields)
                 rest = [f for f in fields if f not in results]
-                if rest and getattr(self.database_connector, "has_columns", lambda _f: False)(parent_filename):
-                    results.update(self.__value_counts_columnar(parent_filename, rest))
-                elif rest:
-                    # unfiltered, like $group; materialised once (a pymongo Cursor can be walked only once)
-                    documents = list(self.database_connector.find(parent_filename, {}))
-                    results.update(self.__value_counts(documents, rest))
+                if rest:
+                    results.update(self.__value_counts_host(parent_filename, rest))
             document_id = 1
             for field in fields:
                 self.database_connector.insert_one_in_file(
@@ -124,8 +123,8 @@ class Histogram:
         """``$group`` of the fields that are text or number in the store, from their columns resident in HBM
         (``table_cache``), under one lease: the values cross PCIe when the column is first made resident, not on every
         request.  Returns the groups of those fields only; the others (mixed-type, set on a document that is not a data
-        row) are left to the host-packing routes, and so is every number field of a rank group, whose process holds
-        only its own rows."""
+        row) are left to the host route (``__value_counts_host``), and so is every number field of a rank group, whose
+        process holds only its own rows."""
         resident = getattr(self.engine, "resident", None)
         if resident is None:
             return {}
@@ -149,71 +148,35 @@ class Histogram:
                     results[f] = number_groups(keys, counts, as_int, data.nulls[j], data.absent[f])
         return results
 
-    def __value_counts(self, documents, fields):
+    def __value_counts_host(self, parent_filename, fields):
+        """The same ``$group`` read from one :class:`~table_cache.Snapshot`, packed per request.  What documents that are
+        not data rows set is counted the same way and merged by :func:`columnar.group_key`; the ``null`` group is last."""
+        snap = Snapshot(self.database_connector, parent_filename)
         results = {}
         for f in fields:
-            values = [d.get(f) for d in documents]
-            present = [i for i, v in enumerate(values) if v is not None]
-            packed = columnar.numeric_column(values) if documents else None
-            if not present:
-                groups = []
-            elif packed is not None:                                     # number field: group-by on binary64 keys
-                col, valid, kind = packed
-                groups = number_groups(*self.engine.value_counts_f64_host(col[valid]), kind == "int", 0, 0)
-            else:                                                        # text or mixed: group-by on the cells' bytes
-                if all(isinstance(values[i], str) for i in present):
-                    cells = [values[i] for i in present]
-                else:
-                    cells = [columnar.tagged_cell(values[i]) for i in present]
-                rep, counts = self.engine.value_counts_str_host(cells)
-                groups = [{"_id": values[present[int(r)]], "count": int(c)} for r, c in zip(rep, counts)]
-            if len(present) != len(values):                              # None / missing (metadata document included)
-                groups.append({"_id": None, "count": len(values) - len(present)})
-            results[f] = groups
+            values, groups = snap.values(f), {}
+            for g in self.__groups(values) + (self.__groups(values.extra) if values.extra else []):
+                hit = groups.setdefault(columnar.group_key(g["_id"]), g)
+                if hit is not g:
+                    hit["count"] += g["count"]
+            results[f] = list(groups.values()) + ([{"_id": None, "count": values.nulls}] if values.nulls else [])
         return results
 
-    def __value_counts_columnar(self, parent_filename, fields):
-        """The same ``$group`` on a collection whose rows are stored as columns (:mod:`column_store`): a text field's
-        Arrow buffers (chars + offsets) go to the byte-wise GPU group-by untouched, a number field's float64 array to
-        the binary64 group-by — no document is materialised.  Documents that are not data rows (the metadata document)
-        have none of the fields and count under ``null``, as in the reference."""
-        db = self.database_connector
-        others = db.other_documents(parent_filename)
-        nrows = db.nrows(parent_filename)
-        results = {}
-        for f in fields:
-            col = db.column(parent_filename, f)
-            none_count = sum(1 for d in others if d.get(f) is None)
-            extra = [d[f] for d in others if d.get(f) is not None]
-            if col is None:
-                groups, none_count = [], none_count + nrows
-            elif col.kind == "number":
-                keys, counts = self.engine.value_counts_f64_host(col.values[col.valid]) if col.valid.any() else ([], [])
-                groups = number_groups(keys, counts, col.integers_collapsed, 0, 0)
-                none_count += int((~col.valid).sum())
-            elif col.kind == "text":
-                arr = col.arr.drop_null() if col.arr.null_count else col.arr
-                none_count += col.arr.null_count
-                from .column_store import TextColumn
-                chars, offsets, _ = TextColumn(arr).packed()
-                groups = text_groups(arr, *self.engine.value_counts_str_packed(chars, offsets), 0)
-            else:                                    # mixed-type column: the document path's tagged byte-wise group-by
-                sub = self.__value_counts([{f: v} for v in col.to_pylist()], [f])[f]
-                none_count += sum(g["count"] for g in sub if g["_id"] is None)
-                groups = [g for g in sub if g["_id"] is not None]
-            if extra:                                # (result documents with the field: not produced by this stack)
-                merged = self.__value_counts([{f: v} for v in extra], [f])[f]
-                index = {columnar.group_key(g["_id"]): g for g in groups}
-                for g in merged:
-                    hit = index.get(columnar.group_key(g["_id"]))
-                    if hit:
-                        hit["count"] += g["count"]
-                    else:
-                        groups.append(g)
-            if none_count:
-                groups.append({"_id": None, "count": none_count})
-            results[f] = groups
-        return results
+    def __groups(self, values):
+        """The groups of the values of a :class:`~table_cache.Values` that are not null."""
+        if values.kind == "number":
+            col, valid, kind = values.data
+            return number_groups(*self.engine.value_counts_f64_host(col[valid]), kind == "int", 0, 0)
+        if values.kind == "text":
+            arr = large_text(values.data)
+            arr = arr.drop_null() if arr.null_count else arr
+            chars, offsets, _ = TextColumn(arr).packed()
+            return text_groups(arr, *self.engine.value_counts_str_packed(chars, offsets), 0)
+        if values.kind == "mixed":
+            present = [v for v in values.data if v is not None]
+            rep, counts = self.engine.value_counts_str_host([columnar.tagged_cell(v) for v in present])
+            return [{"_id": present[int(r)], "count": int(c)} for r, c in zip(rep, counts)]
+        return []
 
     # ---- B-semantics: fixed-width bins of the fp32-cast value -----------------------------------------
     def __binned(self, parent_filename, fields, bins, value_range):

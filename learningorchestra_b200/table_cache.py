@@ -20,9 +20,10 @@ entry records how many documents that are not data rows (the metadata document) 
 
 Number fields are counted from their slabs (``Engine.value_counts_column``).  For each such field the entry records,
 when it is built, whether the slab came from a number column of the store (a text field parsed for a binned request is
-still counted as text), the documents that are not data rows lacking it, and how the host route types its keys: a
-column store's ``integers_collapsed``, a document store's ``numeric_column`` kind.  A slab already resident for a
-binned or ``castTo`` request is counted as it is.
+still counted as text), the documents that are not data rows lacking it, and how its keys are typed: a column store's
+``integers_collapsed``, a document store's ``numeric_column`` kind.  A slab already resident for a binned or ``castTo``
+request is counted as it is.  :class:`Snapshot` is the one reader of a dataset's fields, for this build and for
+``Histogram``'s host route.
 
 Staleness: the in-process :class:`~learningorchestra_b200.utils.Database` bumps ``version(filename)`` on every
 write to data rows (a ``/fieldTypes`` job included); a cached entry is used only while its version matches, and the
@@ -33,6 +34,7 @@ from __future__ import annotations
 
 import threading
 from collections import OrderedDict
+from functools import cached_property
 from typing import NamedTuple
 
 import numpy as np
@@ -85,7 +87,8 @@ def device_number_column(values: np.ndarray, valid: np.ndarray, is_int: np.ndarr
 
 
 def is_text_field(values) -> bool:
-    """A document field the text route takes: at least one value, and every value that is not None a ``str``."""
+    """A document field the text route takes: at least one value, and every value that is not None exactly a ``str``
+    (no store holds a ``str`` subclass such as ``numpy.str_``; a field of them would count as mixed)."""
     return any(v is not None for v in values) and all(v is None or type(v) is str for v in values)
 
 
@@ -100,10 +103,33 @@ class _Field(NamedTuple):
     absent: int
 
 
-class _Snapshot:
-    """The dataset as one build reads it: the data rows (or the column store's handle), their ids and the documents
-    that are not data rows.  A field is read on first use and remembered, so nothing reads a field nobody asked for and
-    nothing reads a field twice."""
+class Values(NamedTuple):
+    """A field as the host route counts it, ``data`` as the store has it: ``kind`` "number" (``numeric_column``'s values,
+    valid mask and key kind), "text" (the cells, an Arrow array or a list), "mixed" (a list) or None (no value set).
+    ``extra``: the Values of what documents that are not data rows set, or None.  ``nulls``: the null cells of ``data``
+    and the documents that are not data rows and lack the field."""
+    kind: str | None
+    data: object
+    extra: "Values | None"
+    nulls: int
+
+
+def classify(values) -> Values:
+    """A list of document values by the document store's rule: text when every value that is not None is a ``str``,
+    number when :func:`columnar.numeric_column` packs them, else mixed."""
+    if is_text_field(values):
+        return Values("text", values, None, sum(1 for v in values if v is None))
+    packed = columnar.numeric_column(values)
+    if packed is None:
+        return Values("mixed", values, None, sum(1 for v in values if v is None))
+    n = int(np.count_nonzero(packed[1]))
+    return Values("number" if n else None, packed, None, len(values) - n)
+
+
+class Snapshot:
+    """The dataset as one request reads it: the data rows (or the column store's handle), their ids and the documents
+    that are not data rows.  The one place that says what kind a stored field is, for the resident build
+    (:meth:`field`) and for the host route (:meth:`values`)."""
 
     def __init__(self, database, filename: str):
         self.database, self.filename = database, filename
@@ -111,14 +137,46 @@ class _Snapshot:
         if self.columnar:        # rows already stored as columns (column_store): no document is touched
             self.row_ids = database.row_ids(filename)
             self.others = database.other_documents(filename)
-        else:
-            documents = list(database.find(filename, {}))
-            self.rows = sorted(columnar.data_rows(documents), key=lambda d: d["_id"])
-            self.others = [d for d in documents if d.get("_id") == columnar.METADATA_DOCUMENT_ID]
-            self.row_ids = np.array([d["_id"] for d in self.rows], dtype=np.int64)
+        else:                    # split into rows and others on first use: the host route reads neither
+            self.documents = list(database.find(filename, {}))
         self._fields = {}
 
+    @cached_property
+    def rows(self):
+        return sorted(columnar.data_rows(self.documents), key=lambda d: d["_id"])
+
+    @cached_property
+    def others(self):
+        return [d for d in self.documents if d.get("_id") == columnar.METADATA_DOCUMENT_ID]
+
+    @cached_property
+    def row_ids(self):
+        return np.array([d["_id"] for d in self.rows], dtype=np.int64)
+
+    def _absent(self, f) -> int:
+        """The documents that are not data rows and lack ``f``: they count under ``null``."""
+        return sum(1 for d in self.others if d.get(f) is None)
+
+    def values(self, f) -> Values:
+        """``f`` as the host route counts it: a document store's documents in store order, the other documents among
+        them; a column store's column by its kind (an object column by :func:`classify`), with ``extra``."""
+        if not self.columnar:
+            return classify([d.get(f) for d in self.documents])
+        c, n = self.database.column(self.filename, f), len(self.row_ids)
+        kind = c.kind if c is not None else None
+        if kind == "number":
+            key_kind = "int" if c.integers_collapsed else "float"
+            v = Values("number", (c.values, c.valid, key_kind), None, n - int(np.count_nonzero(c.valid)))
+        elif kind == "text":
+            v = Values("text", c.arr, None, c.arr.null_count)
+        else:
+            v = classify(c.to_pylist()) if kind == "object" else Values(None, None, None, n)
+        extra = [d[f] for d in self.others if d.get(f) is not None]
+        return Values(v.kind if v.nulls < n else None, v.data, classify(extra) if extra else None,
+                      v.nulls + self._absent(f))
+
     def field(self, f) -> _Field:
+        """``f`` for the resident copy, from the data rows alone."""
         if f not in self._fields:
             slab = text = as_int = None
             if self.columnar:
@@ -126,22 +184,21 @@ class _Snapshot:
                 kind = c.kind if c is not None else None
                 if kind == "number":
                     slab, as_int = ("number", device_number_column(c.values, c.valid, c.is_int)), c.integers_collapsed
-                elif kind == "object":
-                    packed = columnar.numeric_column(c.to_pylist())
-                    slab = ("number", packed) if packed is not None else None
+                elif kind == "object":               # its groups are counted by the host route
+                    v = classify(c.to_pylist())
+                    slab = ("number", v.data) if v.kind not in ("text", "mixed") else None
                 elif kind == "text":
                     slab, text = ("text", c.arr), c.arr
             else:
-                values = [d.get(f) for d in self.rows]
-                if is_text_field(values):
-                    slab, text = ("text", values), values
-                else:
-                    packed = columnar.numeric_column(values)
-                    if packed is not None:
-                        slab, as_int = ("number", packed), packed[2] == "int"
-            if any(d.get(f) is not None for d in self.others):
-                text = as_int = None     # its groups are not the data rows' alone: the host routes count it
-            self._fields[f] = _Field(slab, text, as_int, sum(1 for d in self.others if d.get(f) is None))
+                v = classify([d.get(f) for d in self.rows])
+                if v.kind == "text":
+                    slab, text = ("text", v.data), v.data
+                elif v.kind != "mixed":              # a number field, or one that no row sets
+                    slab, as_int = ("number", v.data), v.data[2] == "int"
+            absent = self._absent(f)
+            if absent < len(self.others):
+                text = as_int = None     # its groups are not the data rows' alone: the host route counts it
+            self._fields[f] = _Field(slab, text, as_int, absent)
         return self._fields[f]
 
 
@@ -155,7 +212,7 @@ class _Plan(NamedTuple):
     absent: dict
 
 
-def _plan(base, fields, text, numbers, snap: _Snapshot) -> _Plan:
+def _plan(base, fields, text, numbers, snap: Snapshot) -> _Plan:
     """The entry a miss builds from ``snap``, given ``base``, the cached entry at the same version (or None): what
     ``base`` holds is shared, not built again — its text columns always, its table when no requested or counted number
     field is missing from it.  Raises ValueError for the first requested field that is neither number nor text."""
@@ -267,7 +324,7 @@ class ResidentTables:
                 return entry
             self.misses += 1
             base = entry if entry is not None and entry.version == version else None
-            snap = _Snapshot(database, filename)
+            snap = Snapshot(database, filename)
             new = self._build(version, base, snap, _plan(base, fields, text, numbers, snap))
             new.users = 1
             if entry is not None:
@@ -281,7 +338,7 @@ class ResidentTables:
                 new.retired = True         # never cached (foreign Database without version()): freed on release
             return new
 
-    def _build(self, version, base, snap: _Snapshot, plan: _Plan) -> ResidentDataset:
+    def _build(self, version, base, snap: Snapshot, plan: _Plan) -> ResidentDataset:
         """The entry ``plan`` describes: its columns uploaded or parsed in table order, then its text columns.  On any
         failure (a bad cell: the first in table order, so in request order) what this call made is freed and re-raised."""
         if plan.columns is None:
