@@ -77,6 +77,26 @@ def number_groups(keys, counts, as_int, nulls, absent):
     return groups
 
 
+def binned(engine, table, cols, bins, value_range, out=None):
+    """The fixed-width histogram of columns ``cols`` of a leased resident ``table``: (lo, hi, counts [k, bins]).  The
+    range is ``value_range`` or, without one, the device min / max pre-pass's (constant and empty columns included);
+    nulls are NaN in the slabs and skipped.  ``out``: an f32 table the fused kernel also writes the cast columns to."""
+    if value_range is None:
+        lo, hi = columnar.auto_range(*engine.minmax_cast(table, cols), bins)
+    else:
+        lo = np.full(len(cols), value_range[0], np.float32)
+        hi = np.full(len(cols), value_range[1], np.float32)
+    dev = engine.project_cast_hist(table, cols, bins, lo, hi, out=out)
+    counts = dev.to_numpy()
+    dev.free()
+    return lo, hi, counts
+
+
+def bins_result(bins, lo, hi, counts):
+    """The result of one field's fixed-width histogram."""
+    return {"bins": int(bins), "range": [float(lo), float(hi)], "counts": [int(c) for c in counts]}
+
+
 class Histogram:
     METADATA_DOCUMENT_ID = 0
     DOCUMENT_ID_NAME = "_id"
@@ -101,13 +121,14 @@ class Histogram:
         try:
             if self.engine is None:
                 raise RuntimeError("Histogram needs an Engine: the counting has no CPU fallback")
+            snap = Snapshot(self.database_connector, parent_filename)     # one read of the dataset for every route
             if bins:
-                results = self.__binned(parent_filename, fields, int(bins), value_range)
+                results = self.__binned(snap, fields, int(bins), value_range)
             else:
-                results = self.__value_counts_resident(parent_filename, fields)
+                results = self.__value_counts_resident(snap, fields)
                 rest = [f for f in fields if f not in results]
                 if rest:
-                    results.update(self.__value_counts_host(parent_filename, rest))
+                    results.update(self.__value_counts_host(snap, rest))
             document_id = 1
             for field in fields:
                 self.database_connector.insert_one_in_file(
@@ -119,7 +140,7 @@ class Histogram:
             raise
 
     # ---- R-semantics: exact value counts -------------------------------------------------------------
-    def __value_counts_resident(self, parent_filename, fields):
+    def __value_counts_resident(self, snap, fields):
         """``$group`` of the fields that are text or number in the store, from their columns resident in HBM
         (``table_cache``), under one lease: the values cross PCIe when the column is first made resident, not on every
         request.  Returns the groups of those fields only; the others (mixed-type, set on a document that is not a data
@@ -134,7 +155,8 @@ class Histogram:
         if not text and not numbers:
             return {}
         results = {}
-        with resident.lease(self.database_connector, parent_filename, (), text=text, numbers=numbers) as data:
+        with resident.lease(self.database_connector, snap.filename, (), text=text, numbers=numbers,
+                            snapshot=snap) as data:
             for f in fields:
                 if f in results:
                     continue
@@ -148,10 +170,10 @@ class Histogram:
                     results[f] = number_groups(keys, counts, as_int, data.nulls[j], data.absent[f])
         return results
 
-    def __value_counts_host(self, parent_filename, fields):
-        """The same ``$group`` read from one :class:`~table_cache.Snapshot`, packed per request.  What documents that are
-        not data rows set is counted the same way and merged by :func:`columnar.group_key`; the ``null`` group is last."""
-        snap = Snapshot(self.database_connector, parent_filename)
+    def __value_counts_host(self, snap, fields):
+        """The same ``$group`` read from the request's :class:`~table_cache.Snapshot`, packed per request.  What documents
+        that are not data rows set is counted the same way and merged by :func:`columnar.group_key`; the ``null`` group
+        is last."""
         results = {}
         for f in fields:
             values, groups = snap.values(f), {}
@@ -179,18 +201,9 @@ class Histogram:
         return []
 
     # ---- B-semantics: fixed-width bins of the fp32-cast value -----------------------------------------
-    def __binned(self, parent_filename, fields, bins, value_range):
+    def __binned(self, snap, fields, bins, value_range):
         """Columns come from the GPU-resident copy of the dataset (built from the documents on first use,
         reused until the collection is written to): no document scan, no H2D on a repeat request."""
-        with self.engine.resident.lease(self.database_connector, parent_filename, fields) as data:
-            cols = [data.column[f] for f in fields]            # nulls are NaN in the slabs: skipped by the kernel
-            if value_range is None:
-                lo, hi = columnar.auto_range(*self.engine.minmax_cast(data.table, cols), bins)   # constant / empty columns included
-            else:
-                lo = np.full(len(fields), value_range[0], np.float32)
-                hi = np.full(len(fields), value_range[1], np.float32)
-            dev_counts = self.engine.project_cast_hist(data.table, cols, bins, lo, hi)
-            counts = dev_counts.to_numpy()
-            dev_counts.free()
-        return {f: {"bins": bins, "range": [float(lo[j]), float(hi[j])], "counts": [int(c) for c in counts[j]]}
-                for j, f in enumerate(fields)}
+        with self.engine.resident.lease(self.database_connector, snap.filename, fields, snapshot=snap) as data:
+            lo, hi, counts = binned(self.engine, data.table, [data.column[f] for f in fields], bins, value_range)
+        return {f: bins_result(bins, lo[j], hi[j], counts[j]) for j, f in enumerate(fields)}

@@ -40,6 +40,7 @@ from typing import NamedTuple
 import numpy as np
 
 from . import columnar
+from .column_store import large_text
 
 
 class ResidentDataset:
@@ -127,30 +128,42 @@ def classify(values) -> Values:
 
 
 class Snapshot:
-    """The dataset as one request reads it: the data rows (or the column store's handle), their ids and the documents
-    that are not data rows.  The one place that says what kind a stored field is, for the resident build
-    (:meth:`field`) and for the host route (:meth:`values`)."""
+    """The dataset as one request reads it: its version, the data rows (or the column store's handle), their ids and
+    the documents that are not data rows.  The one place that says what kind a stored field is, for the resident build
+    (:meth:`field`), for the host route (:meth:`values`) and for the cells a cast writes (:meth:`valid`).
+
+    Only ``version`` is read up front, before any data, so an entry built from the snapshot is never newer than the
+    version it records.  The rest is read on first use: a request the resident copy answers reads no document."""
 
     def __init__(self, database, filename: str):
         self.database, self.filename = database, filename
+        self.version = database.version(filename) if hasattr(database, "version") else None
         self.columnar = getattr(database, "has_columns", lambda _f: False)(filename)
-        if self.columnar:        # rows already stored as columns (column_store): no document is touched
-            self.row_ids = database.row_ids(filename)
-            self.others = database.other_documents(filename)
-        else:                    # split into rows and others on first use: the host route reads neither
-            self.documents = list(database.find(filename, {}))
         self._fields = {}
 
     @cached_property
+    def documents(self):
+        return list(self.database.find(self.filename, {}))
+
+    @cached_property
+    def data(self):
+        """A document store's data rows in the order the store holds them."""
+        return columnar.data_rows(self.documents)
+
+    @cached_property
     def rows(self):
-        return sorted(columnar.data_rows(self.documents), key=lambda d: d["_id"])
+        return sorted(self.data, key=lambda d: d["_id"])
 
     @cached_property
     def others(self):
+        if self.columnar:        # rows stored as columns (column_store): no data row is materialised
+            return self.database.other_documents(self.filename)
         return [d for d in self.documents if d.get("_id") == columnar.METADATA_DOCUMENT_ID]
 
     @cached_property
     def row_ids(self):
+        if self.columnar:
+            return self.database.row_ids(self.filename)
         return np.array([d["_id"] for d in self.rows], dtype=np.int64)
 
     def _absent(self, f) -> int:
@@ -200,6 +213,18 @@ class Snapshot:
                 text = as_int = None     # its groups are not the data rows' alone: the host route counts it
             self._fields[f] = _Field(slab, text, as_int, absent)
         return self._fields[f]
+
+    def valid(self, f) -> np.ndarray:
+        """One bool per data row, in :attr:`rows` order, of a field the resident copy holds: the cell holds a number
+        after ``float()`` (not null, not ``""``).  A column store's number or text column is read as it is stored; the
+        slab's copy of its values is never made here."""
+        c = self.database.column(self.filename, f) if self.columnar else None
+        if c is not None and c.kind == "number":
+            return c.valid
+        if c is not None and c.kind == "text":
+            return columnar.number_text_valid(c.arr)
+        how, src = self.field(f).slab            # a document field or an object column: what the slab is made from
+        return src[1] if how == "number" else columnar.number_text_valid(large_text(src))
 
 
 class _Plan(NamedTuple):
@@ -274,14 +299,14 @@ class ResidentTables:
         self._lock = threading.RLock()
         self.hits = self.misses = 0
 
-    def lease(self, database, filename: str, fields, text=(), numbers=()):
+    def lease(self, database, filename: str, fields, text=(), numbers=(), snapshot=None):
         """``with resident.lease(db, name, fields, text, numbers) as data:`` — the table and the text columns cannot be
         freed (version bump, eviction, invalidate, another job's rebuild) while the block runs GPU work on them."""
         cache = self
 
         class _Lease:
             def __enter__(self_inner):
-                self_inner.data = cache.ensure(database, filename, fields, text, numbers)
+                self_inner.data = cache.ensure(database, filename, fields, text, numbers, snapshot)
                 return self_inner.data
 
             def __exit__(self_inner, *exc):
@@ -300,7 +325,7 @@ class ResidentTables:
         if entry.users <= 0:
             entry.free()
 
-    def ensure(self, database, filename: str, fields, text=(), numbers=()) -> ResidentDataset:
+    def ensure(self, database, filename: str, fields, text=(), numbers=(), snapshot=None) -> ResidentDataset:
         """Resident table holding (at least) ``fields`` of ``filename``; built from the documents on a miss.
         A field may be numeric or text (a column-store text column, or document values that are all ``str`` / None):
         text is parsed on the device into its slab, the dataset itself stays text.  Raises ValueError if a requested
@@ -311,8 +336,11 @@ class ResidentTables:
         ``numbers``: fields to count from their slabs (``entry.numbers``): a number field of the store is made resident
         if it is not already (a slab of a binned or ``castTo`` request is used as it is); any other field is recorded
         as None and raises nothing.  The returned entry is LEASED: pair every call with :meth:`release` (or use
-        :meth:`lease`)."""
-        version = database.version(filename) if hasattr(database, "version") else None
+        :meth:`lease`).
+        ``snapshot``: the caller's :class:`Snapshot` of ``filename``, so that what it reads besides the entry comes from
+        the same read of the store; the entry is checked against, or built at, its version."""
+        snap = snapshot if snapshot is not None else Snapshot(database, filename)
+        version = snap.version
         with self._lock:
             entry = self._entries.get(filename)
             if entry is not None and version is not None and entry.version == version and \
@@ -324,7 +352,6 @@ class ResidentTables:
                 return entry
             self.misses += 1
             base = entry if entry is not None and entry.version == version else None
-            snap = Snapshot(database, filename)
             new = self._build(version, base, snap, _plan(base, fields, text, numbers, snap))
             new.users = 1
             if entry is not None:

@@ -118,6 +118,16 @@ def test_titanic_text_fields_equal_fieldtypes_then_request(engine, tmp_path):
             got = [d[f] for d in pdocs]
             assert [(_f32_bits(v)) for v in got] == [None if r[f] in (None, "") else int(b) for r, b in
                                                      zip(rows, x.view(np.uint32))], (kind, f)
+        # a repeat castTo reads the resident slabs: a hit that parses nothing, with the same output
+        hits, misses = engine.resident.hits, engine.resident.misses
+        r = c.post("/projections", json={"inputDatasetName": "t", "outputDatasetName": "a_p2", "names": FIELDS4,
+                                         "castTo": "float32", "bins": 10})
+        assert r.status_code == 201
+        assert (engine.resident.hits, engine.resident.misses) == (hits + 1, misses), kind
+        rdocs, rmeta = _outputs(db, "a_p2")
+        assert rmeta["finished"] is True and rmeta["histogram"] == pmeta["histogram"], kind
+        assert [[_f32_bits(d[f]) for f in FIELDS4] for d in sorted(rdocs, key=lambda d: d["_id"])] == \
+            [[_f32_bits(d[f]) for f in FIELDS4] for d in pdocs], kind
         # oracle 2: the same requests after /fieldTypes "number" on a copy of the dataset
         _, db2, path2 = [s for s in _stores("n", g["headers"], g["rows"], tmp_path) if s[0] == kind][0]
         c2 = _client(db2, engine, "n", path2)

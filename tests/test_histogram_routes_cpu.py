@@ -269,3 +269,17 @@ def test_a_long_number_field_with_nan_and_none(store, engine):
     assert _typed(groups, False) == [(("null",), "NoneType", 11), ((_NUM, "nan"), "float", 10),
                                      ((_NUM, 0), "float", 20), ((_NUM, 1.5), "float", 20), ((_NUM, 2), "float", 10)]
     assert groups[-1]["_id"] is None and eng.calls == LONG_CALLS[engine]
+
+
+def test_a_document_store_is_read_once_per_request(monkeypatch):
+    """A cold request that needs the resident route and the host route reads the documents once; a warm request that
+    the resident route answers alone reads none."""
+    db, eng, reads = _documents(), _Engine(), []
+    find = db.find
+    monkeypatch.setattr(db, "find", lambda name, query: reads.append(name) or find(name, query))
+    Histogram(db, utils.HistogramMetadata(db), eng).file_processing("d", "cold", FIELDS)
+    assert reads.count("d") == 1
+    Histogram(db, utils.HistogramMetadata(db), eng).file_processing("d", "warm", ["I", "T"])
+    assert reads.count("d") == 1 and eng.resident.hits == 1
+    eng.resident.clear()
+    assert not eng.live
