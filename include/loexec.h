@@ -131,6 +131,9 @@ int lo_table_upload_col(lo_ctx *ctx, lo_table *t, int32_t col, int64_t row0,
 /* ordered after everything already enqueued on `stream` (NULL = the context's stream); waits for that stream only */
 int lo_table_download_col(lo_ctx *ctx, const lo_table *t, int32_t col, int64_t row0,
                           void *host, int64_t nrows, void *stream);
+/* device -> device: column src_col of src into column dst_col of dst, both on ctx's device, same dtype and rows
+ * (else LO_ERR_INVALID); on the context's stream, waited for */
+int lo_table_copy_col(lo_ctx *ctx, const lo_table *src, int32_t src_col, lo_table *dst, int32_t dst_col);
 /* fill every column on the device with the counter-based generator; row r of this table is
  * global row (row_offset + r), so any shard regenerates its own range. */
 int lo_table_fill_synthetic_dev(lo_ctx *ctx, lo_table *t, int kind, uint64_t seed,
@@ -407,6 +410,31 @@ int lo_value_counts_text_shards(lo_ctx *root, const lo_text *const *shards, cons
 #define LO_FORMAT_MAX_CELL 310
 int lo_format_number_host(lo_ctx *ctx, const double *values, const uint8_t *status, int64_t n,
                           int64_t *offsets, uint8_t *chars, int64_t chars_capacity, lo_host_timing *timing);
+
+/* The two casts of a stored column between resident objects, so that a column already in HBM converts there.
+ *
+ * lo_parse_text_to_table: lo_parse_number_to_table (same kernel, same summary, same canonical NaN for null and "") with
+ * the resident text column `src` as the input: its device chars, offsets and validity are read in place, no cell
+ * crosses PCIe (h2d_bytes 0).  Cell i goes to row i of column `col` of `out`.  Refused with LO_ERR_INVALID before
+ * anything is launched: a NULL src / out / summary, src made on another context, `out` not LO_F64 or on another
+ * device, `col` outside [0, ncols), src->n != out's rows.
+ *
+ * lo_format_table_to_text: lo_format_number_host of column `col` of the f64 table `in` into a NEW resident text column
+ * *out (no nulls: an empty cell is "").  Cell i's status is LO_NUM_EMPTY where `valid` says 0, else LO_NUM_INTEGER
+ * where `is_int` says 1, else LO_NUM_FLOAT; each is a lo_validity (mask or Arrow bitmap as for lo_text_upload; NULL:
+ * every cell valid / no cell integer), and only its bytes cross PCIe.  lo_format_number_host's rules hold: an is_int
+ * cell that is not finite and integral -> LO_ERR_INVALID naming the first such row (nothing is made), a cell takes at
+ * most LO_FORMAT_MAX_CELL bytes.  The table must have fewer than 2^31 rows (a text column's limit).
+ *
+ * lo_text_download: a resident text column back into host Arrow large_string buffers: offsets int64[n + 1] from 0 and
+ * the chars (chars_capacity at least the text's bytes, lo_text_info's nbytes; else LO_ERR_INVALID).  The validity is
+ * not copied: lo_text_info says how many cells are null. */
+int lo_parse_text_to_table(lo_ctx *ctx, const lo_text *src, lo_table *out, int32_t col, lo_parse_summary *summary,
+                           lo_host_timing *timing);
+int lo_format_table_to_text(lo_ctx *ctx, const lo_table *in, int32_t col, const lo_validity *valid,
+                            const lo_validity *is_int, lo_text **out, lo_host_timing *timing);
+int lo_text_download(lo_ctx *ctx, const lo_text *t, int64_t *offsets, uint8_t *chars, int64_t chars_capacity,
+                     lo_host_timing *timing);
 
 /* Per-column min and max of the CAST fp32 values over finite entries (NaN / +-inf ignored): the
  * range pre-pass for a histogram request that carries no range (SURVEY.md §2.1 C2).

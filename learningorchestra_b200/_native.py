@@ -105,6 +105,7 @@ SIGNATURES = {
                                 C.POINTER(C.c_int64), C.POINTER(_P)]),
     "lo_table_upload_col": (C.c_int, [_P, _P, C.c_int32, C.c_int64, _P, C.c_int64]),
     "lo_table_download_col": (C.c_int, [_P, _P, C.c_int32, C.c_int64, _P, C.c_int64, _P]),
+    "lo_table_copy_col": (C.c_int, [_P, _P, C.c_int32, _P, C.c_int32]),
     "lo_table_fill_synthetic_dev": (C.c_int, [_P, _P, C.c_int, C.c_uint64, C.c_int64, C.c_double, C.c_double, _P]),
     "lo_table_checksum": (C.c_int, [_P, _P, C.c_int32, C.c_int64, C.POINTER(C.c_uint64)]),
     "lo_selftest_fastdiv": (C.c_int, [_P, C.c_float, C.c_float, C.c_int32, C.POINTER(C.c_int), C.POINTER(C.c_uint64)]),
@@ -155,6 +156,10 @@ SIGNATURES = {
     "lo_value_counts_text_shards": (C.c_int, [_P, C.POINTER(_P), C.POINTER(C.c_int64), C.c_int32, _P, _P, C.c_int64,
                                               C.POINTER(C.c_int64), C.POINTER(HostTiming)]),
     "lo_format_number_host": (C.c_int, [_P, _P, _P, C.c_int64, _P, _P, C.c_int64, C.POINTER(HostTiming)]),
+    "lo_parse_text_to_table": (C.c_int, [_P, _P, _P, C.c_int32, C.POINTER(ParseSummary), C.POINTER(HostTiming)]),
+    "lo_format_table_to_text": (C.c_int, [_P, _P, C.c_int32, C.POINTER(Validity), C.POINTER(Validity), C.POINTER(_P),
+                                          C.POINTER(HostTiming)]),
+    "lo_text_download": (C.c_int, [_P, _P, _P, _P, C.c_int64, C.POINTER(HostTiming)]),
     "lo_minmax_cast_host": (C.c_int, [_P, C.POINTER(_P), C.c_int64, C.c_int32, _P, _P, _P, C.POINTER(HostTiming)]),
     "lo_csv_read_host": (C.c_int, [_P, _P, C.c_int64, C.POINTER(_P), C.POINTER(CsvInfo), C.POINTER(HostTiming)]),
     "lo_csv_columns_host": (C.c_int, [_P, _P, _P, C.c_int64, C.POINTER(HostTiming)]),

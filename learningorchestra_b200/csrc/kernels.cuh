@@ -1502,6 +1502,44 @@ __global__ void k_format_number_write(const unsigned long long *__restrict__ val
         fmt::format_cell(value_bits[i], status[i], chars + offsets[i]);
 }
 
+// One flag per cell of a resident column: mask byte i (0 = clear), or bit (bit0 + i) of an Arrow bitmap; neither ->
+// every cell reads `none`.
+struct CellFlags {
+    const uint8_t *mask, *bitmap;
+    int bit0;
+    __device__ __forceinline__ bool at(long long i, bool none) const {
+        return mask ? mask[i] != 0 : bitmap ? ((bitmap[(bit0 + i) >> 3] >> ((bit0 + i) & 7)) & 1) != 0 : none;
+    }
+};
+
+// The status lo_format_number_host takes, derived from the stored column's flags: not valid -> "", is_int -> str(int),
+// else repr(float)
+__device__ __forceinline__ uint8_t column_status(const CellFlags &valid, const CellFlags &is_int, long long i) {
+    return !valid.at(i, true) ? (uint8_t)num::kEmpty : is_int.at(i, false) ? (uint8_t)num::kInteger : (uint8_t)num::kFloat;
+}
+
+// k_format_number_len / _write reading one f64 table column and the column's valid / is_int flags instead of host
+// values and statuses
+__global__ void __launch_bounds__(128) k_format_col_len(const unsigned long long *__restrict__ col, CellFlags valid,
+                                                        CellFlags is_int, long long n, long long *__restrict__ lengths,
+                                                        unsigned long long *__restrict__ first_bad) {
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+        int len = fmt::format_cell(col[i], column_status(valid, is_int, i), nullptr);
+        if (len < 0) {
+            atomicMin(first_bad, (unsigned long long)i);
+            len = 0;
+        }
+        lengths[i] = len;
+    }
+}
+
+__global__ void __launch_bounds__(128) k_format_col_write(const unsigned long long *__restrict__ col, CellFlags valid,
+                                                          CellFlags is_int, long long n,
+                                                          const long long *__restrict__ offsets, uint8_t *__restrict__ chars) {
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+        fmt::format_cell(col[i], column_status(valid, is_int, i), chars + offsets[i]);
+}
+
 // exhaustive self-test: every one of the 2^32 fp32 bit patterns through both divide variants
 __global__ void k_selftest_fastdiv(float lo, float hi, float w, int nbins, unsigned long long *mismatches) {
     BinParams B = {lo, hi, w, __frcp_rn(w), nbins - 1};

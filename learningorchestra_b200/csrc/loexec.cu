@@ -1074,6 +1074,23 @@ int lo_table_download_col(lo_ctx *ctx, const lo_table *t, int32_t col, int64_t r
     return LO_OK;
 }
 
+int lo_table_copy_col(lo_ctx *ctx, const lo_table *src, int32_t src_col, lo_table *dst, int32_t dst_col) {
+    LO_TRY(check_ctx(ctx));
+    LO_TRY(check_range(src, src_col, 0, 0));
+    LO_TRY(check_range(dst, dst_col, 0, 0));
+    if (src->device != ctx->device || dst->device != ctx->device)
+        return fail(LO_ERR_INVALID, "tables live on devices %d and %d, the context on %d", src->device, dst->device, ctx->device);
+    if (src->dtype != dst->dtype || src->nrows != dst->nrows)
+        return fail(LO_ERR_INVALID, "tables differ: dtype %d / %d, rows %lld / %lld", src->dtype, dst->dtype,
+                    (long long)src->nrows, (long long)dst->nrows);
+    if (src->nrows == 0) return LO_OK;
+    const int64_t bytes = src->nrows * (int64_t)dtype_size(src->dtype);
+    LO_CUDA(cudaMemcpyAsync(dst->base + (int64_t)dst_col * dst->pitch, src->base + (int64_t)src_col * src->pitch,
+                            (size_t)bytes, cudaMemcpyDeviceToDevice, ctx->stream));
+    LO_CUDA(cudaStreamSynchronize(ctx->stream));
+    return LO_OK;
+}
+
 int lo_table_fill_synthetic_dev(lo_ctx *ctx, lo_table *t, int kind, uint64_t seed, int64_t row_offset,
                                 double lo_v, double hi_v, void *stream) {
     LO_TRY(check_ctx(ctx));
@@ -1957,6 +1974,136 @@ int lo_format_number_host(lo_ctx *ctx, const double *values, const uint8_t *stat
     if (chars && total > chars_capacity)
         return fail(LO_ERR_INVALID, "the text takes %lld bytes, chars_capacity is %lld", (long long)total, (long long)chars_capacity);
     return LO_OK;
+}
+
+// lo_parse_number_to_table with a resident text column as the input: the same kernel over the column's device chars,
+// offsets (rebased to 0 when it was made) and validity, so no cell crosses PCIe
+int lo_parse_text_to_table(lo_ctx *ctx, const lo_text *src, lo_table *out, int32_t col, lo_parse_summary *summary,
+                           lo_host_timing *timing) {
+    LO_TRY(check_ctx(ctx));
+    if (!summary) return fail(LO_ERR_INVALID, "summary is NULL");
+    *summary = lo_parse_summary{-1, -1, 0, 1, 0};
+    if (!src) return fail(LO_ERR_INVALID, "text is NULL");
+    if (src->ctx != ctx) return fail(LO_ERR_INVALID, "text belongs to another context");
+    if (!out || out->dtype != LO_F64) return fail(LO_ERR_INVALID, "output table must be LO_F64");
+    if (out->device != ctx->device) return fail(LO_ERR_INVALID, "table lives on device %d, the context on %d", out->device, ctx->device);
+    LO_TRY(check_range(out, col, 0, 0));
+    if (src->n != out->nrows)
+        return fail(LO_ERR_INVALID, "text of %lld cells for a table of %lld rows", (long long)src->n, (long long)out->nrows);
+    const int64_t n = src->n;
+    if (n == 0) return LO_OK;
+    HostCall c(ctx, "parse_text_to_table");
+    const TextCols &d = src->cols;
+    unsigned long long *d_sum = nullptr;
+    c.alloc(&d_sum, 4 * 8);
+    c.memset(d_sum, 0xFF, 2 * 8);
+    c.memset(d_sum + 2, 0, 2 * 8);
+    unsigned long long *dst = (unsigned long long *)(out->base + (int64_t)col * out->pitch);
+    c.mark();
+    c.launch(1, [&] {
+        const int grid = (int)std::min<int64_t>((n + 127) / 128, (int64_t)ctx->sm_count * 16);
+        lo::k_parse_number_to_col<<<grid, 128, 0, c.s>>>(d.chars, d.offsets, n, d.mask, d.bitmap, d.bit0, dst, d_sum);
+    });
+    c.mark();
+    unsigned long long sum[4] = {~0ull, ~0ull, 0, 0};
+    c.to_host(sum, d_sum, sizeof(sum));
+    LO_TRY(c.finish(timing));
+    summary->first_invalid = sum[0] < (unsigned long long)n ? (int64_t)sum[0] : -1;
+    summary->first_unsupported = sum[1] < (unsigned long long)n ? (int64_t)sum[1] : -1;
+    summary->nulls = (int64_t)sum[2];
+    summary->all_integer = sum[3] == 0;
+    return LO_OK;
+}
+
+// lo_format_number_host of one resident f64 column into a new resident text column: the statuses come from the two
+// flag arrays on the device, the lengths, their scan and the text stay there; only the flags and the total cross PCIe
+int lo_format_table_to_text(lo_ctx *ctx, const lo_table *in, int32_t col, const lo_validity *valid,
+                            const lo_validity *is_int, lo_text **out, lo_host_timing *timing) {
+    LO_TRY(check_ctx(ctx));
+    if (!out) return fail(LO_ERR_INVALID, "out is NULL");
+    *out = nullptr;
+    if (!in || in->dtype != LO_F64) return fail(LO_ERR_INVALID, "input table must be LO_F64");
+    if (in->device != ctx->device) return fail(LO_ERR_INVALID, "table lives on device %d, the context on %d", in->device, ctx->device);
+    LO_TRY(check_range(in, col, 0, 0));
+    const int64_t n = in->nrows;
+    if (n >> kGroupRowBits) return fail(LO_ERR_INVALID, "n = %lld: 0 to 2^%d-1 rows per text column", (long long)n, kGroupRowBits);
+    for (const lo_validity *v : {valid, is_int}) {
+        if (v && v->mask && v->bitmap) return fail(LO_ERR_INVALID, "validity: mask or bitmap, not both");
+        if (v && v->bitmap && v->bit_offset < 0) return fail(LO_ERR_INVALID, "validity: bit_offset < 0");
+    }
+    std::unique_ptr<lo_text> t(new (std::nothrow) lo_text);
+    if (!t) return fail(LO_ERR_NOMEM, "out of host memory");
+    HostCall c(ctx, "format_table_to_text");
+    const unsigned long long *d_val = (const unsigned long long *)(in->base + (int64_t)col * in->pitch);
+    lo::CellFlags flags[2] = {{nullptr, nullptr, 0}, {nullptr, nullptr, 0}};
+    const lo_validity *src[2] = {valid, is_int};
+    for (int k = 0; k < 2; ++k) {            // the flags' host bytes, staged as stage_text stages a validity
+        size_t bytes = 0;
+        const uint8_t *h = validity_span(src[k], n, &bytes);
+        if (!bytes) continue;
+        uint8_t *d = nullptr;
+        c.alloc(&d, bytes);
+        c.to_dev(d, h, bytes);
+        if (src[k]->mask) flags[k].mask = d;
+        else flags[k] = lo::CellFlags{nullptr, d, (int)(src[k]->bit_offset & 7)};
+    }
+    long long *d_off = nullptr;
+    unsigned long long *d_bad = nullptr;
+    uint8_t *d_chars = nullptr;
+    void *d_tmp = nullptr;
+    size_t tmp_bytes = 0;
+    const int grid = (int)std::min<int64_t>(std::max<int64_t>((n + 127) / 128, 1), (int64_t)ctx->sm_count * 16);
+    c.run([&] { return cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, d_off, n + 1, c.s); });
+    c.alloc(&d_off, (size_t)(n + 1) * 8);
+    c.alloc(&d_bad, 8);
+    c.alloc(&d_tmp, tmp_bytes);
+    c.memset(d_bad, 0xFF, 8);
+    c.memset(d_off + n, 0, 8);           // the scan's last input: offsets[n] = total
+    c.mark();
+    if (n) c.launch(1, [&] { lo::k_format_col_len<<<grid, 128, 0, c.s>>>(d_val, flags[0], flags[1], n, d_off, d_bad); });
+    c.launch(1, [&] { return cub::DeviceScan::ExclusiveSum(d_tmp, tmp_bytes, d_off, n + 1, c.s); });
+    c.mark();
+    unsigned long long bad = ~0ull;
+    long long total = 0;
+    c.to_host(&total, d_off + n, 8);
+    c.to_host(&bad, d_bad, 8);
+    c.sync();
+    if (bad < (unsigned long long)n) {
+        double v = 0;
+        c.to_host(&v, d_val + bad, 8);
+        LO_TRY(c.finish(nullptr));
+        return fail(LO_ERR_INVALID, "row %lld: an is_int value %.17g is not finite and integral", (long long)bad, v);
+    }
+    c.alloc(&d_chars, (size_t)total);
+    c.mark();
+    if (total > 0)
+        c.launch(1, [&] { lo::k_format_col_write<<<grid, 128, 0, c.s>>>(d_val, flags[0], flags[1], n, d_off, d_chars); });
+    c.mark();
+    c.keep(d_off);
+    c.keep(d_chars);
+    LO_TRY(c.finish(timing));
+    TextCols cols;
+    cols.chars = d_chars;
+    cols.offsets = d_off;
+    *t = lo_text{ctx, cols, n, (int64_t)total, 0, (size_t)std::max<long long>(total, 1) + (size_t)(n + 1) * 8};
+    *out = t.release();
+    return LO_OK;
+}
+
+// a resident text column's cells back into host Arrow large_string buffers: offsets (n + 1, from 0) and the chars
+int lo_text_download(lo_ctx *ctx, const lo_text *t, int64_t *offsets, uint8_t *chars, int64_t chars_capacity,
+                     lo_host_timing *timing) {
+    LO_TRY(check_ctx(ctx));
+    if (!t) return fail(LO_ERR_INVALID, "text is NULL");
+    if (t->ctx != ctx) return fail(LO_ERR_INVALID, "text belongs to another context");
+    if (!offsets) return fail(LO_ERR_INVALID, "offsets is NULL");
+    if (chars_capacity < t->nbytes || (t->nbytes && !chars))
+        return fail(LO_ERR_INVALID, "the text takes %lld bytes, chars_capacity is %lld", (long long)t->nbytes,
+                    (long long)chars_capacity);
+    HostCall c(ctx, "text_download");
+    c.to_host(offsets, t->cols.offsets, (size_t)(t->n + 1) * 8);
+    c.to_host(chars, t->cols.chars, (size_t)t->nbytes);
+    return c.finish(timing);
 }
 
 // per-column min / max of the CAST fp32 values, ignoring NaN and +-inf (the range pre-pass when a

@@ -86,9 +86,13 @@ class DataType:
         if col.kind == "object":                       # mixed cells: the per-document definition decides
             db.to_documents(filename)
             return self.field_converter(filename, field, field_type)
+        resident = self.__resident()
         if field_type == self.STRING_TYPE:
             if col.kind == "text":                     # str(v) of a str is itself; None -> ""
                 new = TextColumn(col.arr.fill_null("")) if col.arr.null_count else col
+            elif resident is not None:                 # from the resident slab into a resident text column
+                self.__format_resident(resident, filename, field)
+                return
             elif getattr(self.engine, "format_number_host", None) is not None:     # str(int) / repr(float) on the GPU
                 import pyarrow as pa
                 status = np.where(~col.valid, N.LO_NUM_EMPTY, np.where(col.is_int, N.LO_NUM_INTEGER, N.LO_NUM_FLOAT))
@@ -107,6 +111,8 @@ class DataType:
                 db.set_column(filename, field, NumberColumn(v, col.valid, integral))
                 return
             arr = columnar.number_text(col.arr)                 # Unicode digits / spaces, as float(str)
+            if resident is not None and arr is col.arr and self.__parse_resident(resident, filename, field, col):
+                return
             chars, offsets, nulls = TextColumn(arr).packed()
             values, status = self.engine.parse_number_packed(chars, offsets)
             bad = np.flatnonzero((status == N.LO_NUM_INVALID) | (status == N.LO_NUM_UNSUPPORTED))
@@ -134,6 +140,84 @@ class DataType:
             self.engine.project_cast_hist_host([np.ascontiguousarray(col.values)], None, out=[out])
             db.set_column(filename, field, NumberColumn(np.where(col.valid, out.astype(np.float64), np.nan), col.valid))
         # unknown type: the reference issues an empty $set
+
+    def __resident(self):
+        """The engine's resident datasets (:mod:`table_cache`) when it holds every row of a table, else None (an engine
+        without them, a rank group's process, which holds its own rows only)."""
+        resident = getattr(self.engine, "resident", None)
+        if resident is None or getattr(self.engine, "world", 1) != getattr(self.engine, "nlocal", 1):
+            return None
+        return resident
+
+    def __parse_resident(self, resident, filename, field, col) -> bool:
+        """``"number"`` of an ASCII text column from its resident copy (uploaded once if it is not resident yet): parsed
+        on every device into a fresh f64 column, read back, and that column handed to the cache with the new
+        NumberColumn.  A slab already parsed from this text (a binned or ``castTo`` request) is the result as it is.
+        The NumberColumn equals the packed route's: ``valid`` from the text, ``is_int`` = valid and integral.  False
+        when the field is not kept as text (set on a document that is not a data row): the packed route takes it."""
+        from .column_store import ObjectColumn
+        from .table_cache import Snapshot
+        db = self.database_connector
+        snap = Snapshot(db, filename)
+        entry = resident.holding(db, filename, field, snap)
+        if entry is not None:
+            try:
+                values = entry.table.to_numpy(entry.column[field])
+            finally:
+                resident.release(entry)
+            db.set_column(filename, field, new := self.__number_column(values, col.arr))
+            resident.adopt(filename, field, new, same_as=col)
+            return True
+        with resident.lease(db, filename, (), text=[field], snapshot=snap) as data:
+            text = data.texts.get(field)
+            if text is None:
+                return False
+            table = self.engine.table("f64", len(col), 1)
+            try:
+                summary = self.engine.parse_text_into(table, 0, text)
+                values = table.to_numpy(0)
+            except BaseException:
+                table.free()
+                raise
+        bad = [r for r in (summary["first_invalid"], summary["first_unsupported"]) if r is not None]
+        if bad:
+            # as the packed route: earlier rows converted, the rest untouched, finished stays False
+            table.free()
+            first = min(bad)
+            cells = col.to_pylist()
+            head = self.__number_column(values[:first], col.arr.slice(0, first)).to_pylist()
+            db.set_column(filename, field, ObjectColumn(head + cells[first:]))
+            if first == summary["first_unsupported"]:
+                raise RuntimeError(f"cell of {len(cells[first])} characters exceeds the device parser's 1 MiB limit "
+                                   "and there is no CPU fallback")
+            raise ValueError(f"could not convert string to float: {cells[first]!r}")
+        new = self.__number_column(values, col.arr)
+        db.set_column(filename, field, new)
+        resident.adopt(filename, field, new, table, slab=("int" if summary["integer"] else "float", summary["nulls"]))
+        return True
+
+    @staticmethod
+    def __number_column(values, arr):
+        """The NumberColumn ``"number"`` leaves of the text cells ``arr`` (an Arrow array) whose parsed values (NaN for
+        null and "") are ``values``."""
+        from .column_store import NumberColumn
+        valid = columnar.number_text_valid(arr)
+        return NumberColumn(values, valid, valid & np.isfinite(values) & (values == np.floor(values)))
+
+    def __format_resident(self, resident, filename, field):
+        """``"string"`` of a number column from its resident slab into a new resident text column, on every device; the
+        text column is read back once for the store and handed to the cache with it, so a later ``$group`` of the field
+        counts it with no upload."""
+        from .column_store import TextColumn
+        from .table_cache import Snapshot
+        db = self.database_connector
+        snap = Snapshot(db, filename)
+        col = snap.column(field)
+        with resident.lease(db, filename, [field], snapshot=snap) as data:
+            text = self.engine.format_column(data.table, data.column[field], col.valid, col.is_int)
+        new = TextColumn(text.arr)
+        db.set_column(filename, field, new)
+        resident.adopt(filename, field, new, text)
 
     def __to_text(self, rows, field):
         """``data_type_update.py:22-28``: ``None -> ""``, anything else ``str(v)``; the reference's guard

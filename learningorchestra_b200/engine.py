@@ -84,6 +84,13 @@ def _validity(nulls, n: int):
     return v, keep
 
 
+def _summary(s, t) -> dict:
+    """The dict :meth:`Engine.parse_number_into` returns from a lo_parse_summary and its lo_host_timing."""
+    return {"first_invalid": s.first_invalid if s.first_invalid >= 0 else None,
+            "first_unsupported": s.first_unsupported if s.first_unsupported >= 0 else None,
+            "nulls": int(s.nulls), "integer": bool(s.all_integer), **_timing(t), "kernel_ms": t.kernel_ms}
+
+
 def _minmax_decode(lib, raw: np.ndarray, k: int):
     """(min, max, n_finite) of k columns from the raw uint64[3k] of a min/max pre-pass."""
     mins, maxs, cnt = np.zeros(k, np.float32), np.zeros(k, np.float32), np.zeros(k, np.uint64)
@@ -536,9 +543,61 @@ class Engine:
         s, t = N.ParseSummary(), N.HostTiming()
         N.check(self._lib.lo_parse_number_to_table(self._ctx, chars.ctypes.data_as(C.c_void_p), offsets.ctypes.data_as(C.c_void_p),
                                                    C.byref(v), n, table._h, int(col), 0, C.byref(s), C.byref(t)))
-        return {"first_invalid": s.first_invalid if s.first_invalid >= 0 else None,
-                "first_unsupported": s.first_unsupported if s.first_unsupported >= 0 else None,
-                "nulls": int(s.nulls), "integer": bool(s.all_integer), **_timing(t), "kernel_ms": t.kernel_ms}
+        return _summary(s, t)
+
+    def parse_text_into(self, table: DeviceTable, col: int, text: DeviceText) -> dict:
+        """:meth:`parse_number_into` with a resident text column as the input (``lo_parse_text_to_table``): cell i of
+        ``text`` goes to row i of f64 column ``col`` of ``table``, which has one row per cell, and no cell crosses PCIe.
+        The text must be ASCII (:func:`columnar.number_text` returns it as it is).  Returns the same summary."""
+        if text._h is None:
+            raise ValueError("the text column has been freed")
+        s, t = N.ParseSummary(), N.HostTiming()
+        N.check(self._lib.lo_parse_text_to_table(self._ctx, text._h, table._h, int(col), C.byref(s), C.byref(t)))
+        return _summary(s, t)
+
+    def format_text(self, table: DeviceTable, col: int, valid: np.ndarray, is_int: np.ndarray) -> DeviceText:
+        """The ``"string"`` cast of f64 column ``col`` of ``table`` into a new resident text column
+        (``lo_format_table_to_text``), without reading it back (``arr`` None): row i is ``""`` where ``valid[i]`` is
+        False, ``str(int)`` where ``is_int[i]``, else ``repr(float)``.  ``valid`` / ``is_int``: one bool per row; they
+        cross PCIe as bitmaps.  An ``is_int`` row that is not finite and integral raises LoexecError naming it."""
+        n = table.nrows
+        flags = [np.asarray(a, dtype=bool) for a in (valid, is_int)]
+        if any(a.shape != (n,) for a in flags):
+            raise ValueError("valid and is_int must have one entry per row")
+        (v, _kv), (i, _ki) = [_validity((np.packbits(a, bitorder="little"), 0), n) for a in flags]
+        h, t = C.c_void_p(), N.HostTiming()
+        N.check(self._lib.lo_format_table_to_text(self._ctx, table._h, int(col), C.byref(v), C.byref(i), C.byref(h),
+                                                  C.byref(t)))
+        return DeviceText(self, h, None)
+
+    def download_text(self, text: DeviceText, offsets: np.ndarray | None = None, chars: np.ndarray | None = None):
+        """(offsets int64[n + 1] from 0, chars uint8) of a resident text column (``lo_text_download``), written into
+        ``offsets`` / ``chars`` when given (contiguous, of at least those sizes)."""
+        offsets = np.empty(text.n + 1, np.int64) if offsets is None else offsets
+        chars = np.empty(max(text.chars, 1), np.uint8) if chars is None else chars
+        if offsets.dtype != np.int64 or offsets.shape != (text.n + 1,) or not offsets.flags.c_contiguous or \
+                chars.dtype != np.uint8 or not chars.flags.c_contiguous:
+            raise ValueError("offsets must be int64[n + 1] and chars uint8, both contiguous")
+        N.check(self._lib.lo_text_download(self._ctx, text._h, offsets.ctypes.data_as(C.c_void_p),
+                                           chars.ctypes.data_as(C.c_void_p), chars.size, None))
+        return offsets, chars
+
+    def format_column(self, table: DeviceTable, col: int, valid: np.ndarray, is_int: np.ndarray) -> DeviceText:
+        """:meth:`format_text`, its ``arr`` the Arrow ``large_string`` array read back: the buffers
+        :meth:`format_number_host` returns for the same column."""
+        import pyarrow as pa
+        text = self.format_text(table, col, valid, is_int)
+        try:
+            offsets, chars = self.download_text(text)
+        except BaseException:
+            text.free()
+            raise
+        text.arr = pa.LargeStringArray.from_buffers(text.n, pa.py_buffer(offsets), pa.py_buffer(chars[:text.chars]))
+        return text
+
+    def copy_column(self, src: DeviceTable, src_col: int, dst: DeviceTable, dst_col: int) -> None:
+        """Column ``src_col`` of ``src`` into column ``dst_col`` of ``dst`` (same dtype and rows), device to device."""
+        N.check(self._lib.lo_table_copy_col(self._ctx, src._h, int(src_col), dst._h, int(dst_col)))
 
     def format_number_host(self, values: np.ndarray, status: np.ndarray, timing: dict | None = None):
         """The inverse of :meth:`parse_number_packed`: values float64[n] and status uint8[n] (LO_NUM_FLOAT ->

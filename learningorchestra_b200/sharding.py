@@ -511,6 +511,57 @@ class ShardedEngine:
 
         return combine_parse_summaries(on_each(self.nlocal, run), table.offsets)
 
+    def _every_row(self, what: str) -> None:
+        if self.world > self.nlocal:
+            raise self._N.LoexecError(self._N.LO_ERR_INVALID, f"{what} needs every row: this process holds "
+                                      f"{self.nlocal} of the group's {self.world} shards")
+
+    def parse_text_into(self, table: ShardedTable, col: int, text: ShardedText) -> dict:
+        """``Engine.parse_text_into`` over a sharded table: piece i of ``text`` and shard i of ``table`` hold the same rows
+        (both cut at :meth:`bounds`), so every member parses its piece into its shard on its own device, from a host
+        thread of its own, and nothing crosses devices.  The summary's rows are global."""
+        self._every_row("parse_text_into")
+        if text.offsets != table.offsets or [p.n for p in text.pieces] != [t.nrows for t in table.shards]:
+            raise ValueError("the text column and the table are not cut at the same rows")
+        return combine_parse_summaries(on_each(self.nlocal, lambda i: self.engines[i].parse_text_into(
+            table.shards[i], col, text.pieces[i])), table.offsets)
+
+    def format_column(self, table: ShardedTable, col: int, valid, is_int) -> ShardedText:
+        """``Engine.format_column`` over a sharded table: every member formats its shard into a text piece on its own
+        device, and each piece is read straight into its slice of one host buffer, its offsets moved by the bytes of the
+        pieces before it.  ``valid`` / ``is_int`` describe every row; the result's ``arr`` is one Arrow array."""
+        import numpy as np
+        import pyarrow as pa
+        self._every_row("format_column")
+        bounds = [(off, off + t.nrows) for t, off in zip(table.shards, table.offsets)]
+        pieces = on_each(self.nlocal, lambda i: self.engines[i].format_text(
+            table.shards[i], col, valid[bounds[i][0]:bounds[i][1]], is_int[bounds[i][0]:bounds[i][1]]),
+            undo=lambda p: p.free())
+        try:
+            base = np.concatenate([[0], np.cumsum([p.chars for p in pieces])]).astype(np.int64)
+            offsets = np.empty(table.nrows + 1, np.int64)
+            chars = np.empty(max(int(base[-1]), 1), np.uint8)
+
+            def fetch(i):
+                (b, e), p = bounds[i], pieces[i]
+                self.engines[i].download_text(p, offsets[b:e + 1], chars[base[i]:base[i] + p.chars])
+                offsets[b + 1:e] += base[i]        # the piece's inner offsets; its two ends are shared with neighbours
+
+            on_each(self.nlocal, fetch)
+            for (b, e), lo, hi in zip(bounds, base[:-1], base[1:]):
+                offsets[b], offsets[e] = lo, hi
+        except BaseException:
+            for p in pieces:
+                p.free()
+            raise
+        arr = pa.LargeStringArray.from_buffers(table.nrows, pa.py_buffer(offsets), pa.py_buffer(chars[:base[-1]]))
+        return ShardedText(pieces, table.offsets, arr)
+
+    def copy_column(self, src: ShardedTable, src_col: int, dst: ShardedTable, dst_col: int) -> None:
+        """``Engine.copy_column`` shard by shard: both tables are cut at the same rows, so each copy stays on its device."""
+        for e, s, d in zip(self.engines, src.shards, dst.shards):
+            e.copy_column(s, src_col, d, dst_col)
+
     def value_counts_column(self, table: ShardedTable, col: int):
         """``Engine.value_counts_column`` over a sharded table: every local shard is counted on its own device from a
         host thread of its own, and the groups are merged on the host (:func:`merge_value_counts`).  A rank group's

@@ -48,7 +48,7 @@ class ResidentDataset:
     change with its predecessor (each object counts the entries holding it, ``holders``) and a device object is freed
     with the last entry that holds it, so a lease on either entry keeps everything it reads alive."""
 
-    def __init__(self, version, ids, fields, kinds, nulls, table, texts=None, absent=None, numbers=None):
+    def __init__(self, version, ids, fields, kinds, nulls, table, texts=None, absent=None, numbers=None, sources=None):
         self.version, self.ids, self.fields, self.kinds, self.nulls, self.table = version, ids, fields, kinds, nulls, table
         self.column = {f: i for i, f in enumerate(fields)}
         # text columns kept as text for $group: field -> DeviceText, or None for a field that was checked and is not a
@@ -59,17 +59,23 @@ class ResidentDataset:
         # when parsed into a slab for a binned request; mixed; set on a document that is not a data row)
         self.numbers = dict(numbers or {})
         self.absent = dict(absent or {})   # counted field -> documents that are not data rows and lack it (null group)
+        # a column store's entry: ("slab" | "text", field) -> the store columns that object serves (the one it was made
+        # from, and any that replaced it with the same values); None for a document store, whose entries serve one version
+        self.sources = sources
+        # objects handed over for store columns written after this entry was built: ("slab" | "text", field) ->
+        # (column, object, kind, nulls) — a slab is a one-column table, kind and nulls as in ``kinds`` / ``nulls``
+        self.adopted = {}
         self.users = 0          # leases handed out and not yet released (guarded by ResidentTables._lock)
         self.retired = False    # dropped from the cache: freed when the last user releases it
         for obj in self._objects():
             obj.holders = getattr(obj, "holders", 0) + 1
 
     def _objects(self):
-        return [o for o in [self.table, *self.texts.values()] if o is not None]
+        return [o for o in [self.table, *self.texts.values(), *(a[1] for a in self.adopted.values())] if o is not None]
 
     @property
     def nbytes(self) -> int:
-        return self.table.pitch_bytes * self.table.ncols + sum(t.nbytes for t in self.texts.values() if t is not None)
+        return sum(o.pitch_bytes * o.ncols if hasattr(o, "ncols") else o.nbytes for o in self._objects())
 
     def free(self) -> None:
         for obj in self._objects():
@@ -139,7 +145,7 @@ class Snapshot:
         self.database, self.filename = database, filename
         self.version = database.version(filename) if hasattr(database, "version") else None
         self.columnar = getattr(database, "has_columns", lambda _f: False)(filename)
-        self._fields = {}
+        self._fields, self._columns = {}, {}
 
     @cached_property
     def documents(self):
@@ -166,6 +172,12 @@ class Snapshot:
             return self.database.row_ids(self.filename)
         return np.array([d["_id"] for d in self.rows], dtype=np.int64)
 
+    def column(self, f):
+        """A column store's column of ``f`` as this snapshot first read it (None when no data row has the field)."""
+        if f not in self._columns:
+            self._columns[f] = self.database.column(self.filename, f)
+        return self._columns[f]
+
     def _absent(self, f) -> int:
         """The documents that are not data rows and lack ``f``: they count under ``null``."""
         return sum(1 for d in self.others if d.get(f) is None)
@@ -175,7 +187,7 @@ class Snapshot:
         them; a column store's column by its kind (an object column by :func:`classify`), with ``extra``."""
         if not self.columnar:
             return classify([d.get(f) for d in self.documents])
-        c, n = self.database.column(self.filename, f), len(self.row_ids)
+        c, n = self.column(f), len(self.row_ids)
         kind = c.kind if c is not None else None
         if kind == "number":
             key_kind = "int" if c.integers_collapsed else "float"
@@ -193,7 +205,7 @@ class Snapshot:
         if f not in self._fields:
             slab = text = as_int = None
             if self.columnar:
-                c = self.database.column(self.filename, f)
+                c = self.column(f)
                 kind = c.kind if c is not None else None
                 if kind == "number":
                     slab, as_int = ("number", device_number_column(c.values, c.valid, c.is_int)), c.integers_collapsed
@@ -218,7 +230,7 @@ class Snapshot:
         """One bool per data row, in :attr:`rows` order, of a field the resident copy holds: the cell holds a number
         after ``float()`` (not null, not ``""``).  A column store's number or text column is read as it is stored; the
         slab's copy of its values is never made here."""
-        c = self.database.column(self.filename, f) if self.columnar else None
+        c = self.column(f) if self.columnar else None
         if c is not None and c.kind == "number":
             return c.valid
         if c is not None and c.kind == "text":
@@ -228,23 +240,57 @@ class Snapshot:
 
 
 class _Plan(NamedTuple):
-    """What a miss builds: ``columns`` (field, slab) in table order, or None when the predecessor's table is shared;
-    ``uploads`` the text columns to make, field -> cells (None: recorded as not text); the rest as in ResidentDataset."""
+    """What a miss builds: ``columns`` (field, slab) in table order, a slab as :class:`_Field` has it or ``("copy",
+    (table, column, kind, nulls))`` for a resident slab copied device to device; or None when ``shared``'s table is used
+    as it is.  ``uploads`` the text columns to make, field -> cells (None: recorded as not text); the rest as in
+    ResidentDataset."""
     columns: list | None
     uploads: dict
     texts: dict
     numbers: dict
     absent: dict
+    shared: "ResidentDataset | None" = None
 
 
-def _plan(base, fields, text, numbers, snap: Snapshot) -> _Plan:
+def _carried(prev, snap: Snapshot):
+    """What ``prev``, the cached entry of an older version, still holds for ``snap``: (texts field -> text column, slabs
+    field -> (table, column, kind, nulls)).  A stored column is immutable (``set_column`` replaces the object), so an
+    object made from store column ``c`` with row ids ``ids`` serves every later version whose snapshot still holds the
+    same ``c`` and ``ids`` objects.  Nothing for a document store: its writes are per document and its fields may hold
+    mixed cells, so its entries serve their own version only."""
+    if prev is None or prev.sources is None or not snap.columnar or prev.ids is not snap.row_ids:
+        return {}, {}
+
+    def serves(role, f, made_from):
+        return any(c is snap.column(f) for c in made_from.get((role, f), ()))
+
+    texts = {f: t for f, t in prev.texts.items() if t is not None and serves("text", f, prev.sources)}
+    slabs = {f: (prev.table, j, prev.kinds[j], prev.nulls[j]) for j, f in enumerate(prev.fields)
+             if serves("slab", f, prev.sources)}
+    for (role, f), (column, obj, kind, nulls) in prev.adopted.items():
+        if column is snap.column(f):
+            if role == "text":
+                texts.setdefault(f, obj)
+            else:
+                slabs.setdefault(f, (obj, 0, kind, nulls))
+    return texts, slabs
+
+
+def _plan(base, prev, fields, text, numbers, snap: Snapshot) -> _Plan:
     """The entry a miss builds from ``snap``, given ``base``, the cached entry at the same version (or None): what
     ``base`` holds is shared, not built again — its text columns always, its table when no requested or counted number
-    field is missing from it.  Raises ValueError for the first requested field that is neither number nor text."""
+    field is missing from it.  Without a base, ``prev`` (the stale entry, or None) gives what it still holds
+    (:func:`_carried`): those text columns are taken as they are, those slabs copied device to device, or its whole
+    table shared when it holds exactly the columns the entry needs.  Raises ValueError for the first requested field
+    that is neither number nor text."""
     texts = dict(base.texts) if base else {}
     counted = dict(base.numbers) if base else {}
     absent = dict(base.absent) if base else {}
-    resident = base.fields if base else []
+    kept_texts, kept_slabs = _carried(prev, snap) if base is None else ({}, {})
+    resident = base.fields if base else list(kept_slabs)
+    for f, t in kept_texts.items():
+        if snap.field(f).text is not None:
+            texts[f], absent[f] = t, snap.field(f).absent
     uploads = {}
     for f in dict.fromkeys(text):
         if f not in texts:
@@ -253,10 +299,10 @@ def _plan(base, fields, text, numbers, snap: Snapshot) -> _Plan:
     for f in dict.fromkeys(numbers):
         if f not in counted:
             counted[f], absent[f] = snap.field(f).as_int, snap.field(f).absent
-            if counted[f] is not None:
+            if counted[f] is not None and f not in resident:
                 grow.append(f)
     if base and not grow and all(f in base.column for f in fields):
-        return _Plan(None, uploads, texts, counted, absent)
+        return _Plan(None, uploads, texts, counted, absent, base)
     columns = []
     for f in [*fields, *(f for f in resident if f not in fields), *(f for f in grow if f not in fields)]:
         info = snap.field(f)
@@ -269,7 +315,10 @@ def _plan(base, fields, text, numbers, snap: Snapshot) -> _Plan:
             continue                 # a previously resident column that stopped being numeric: drop it
         if info.slab[0] == "number":
             texts.setdefault(f, None)    # checked: not a text field, so a count request on it is a hit
-        columns.append((f, info.slab))
+        columns.append((f, ("copy", kept_slabs[f]) if f in kept_slabs else info.slab))
+    if prev is not None and kept_slabs and [f for f, _ in columns] == prev.fields and \
+            all(how == "copy" and src[:2] == (prev.table, j) for j, (_f, (how, src)) in enumerate(columns)):
+        return _Plan(None, uploads, texts, counted, absent, prev)
     return _Plan(columns, uploads, texts, counted, absent)
 
 
@@ -352,7 +401,7 @@ class ResidentTables:
                 return entry
             self.misses += 1
             base = entry if entry is not None and entry.version == version else None
-            new = self._build(version, base, snap, _plan(base, fields, text, numbers, snap))
+            new = self._build(version, snap, _plan(base, entry, fields, text, numbers, snap))
             new.users = 1
             if entry is not None:
                 self._entries.pop(filename, None)
@@ -365,11 +414,12 @@ class ResidentTables:
                 new.retired = True         # never cached (foreign Database without version()): freed on release
             return new
 
-    def _build(self, version, base, snap: Snapshot, plan: _Plan) -> ResidentDataset:
-        """The entry ``plan`` describes: its columns uploaded or parsed in table order, then its text columns.  On any
-        failure (a bad cell: the first in table order, so in request order) what this call made is freed and re-raised."""
+    def _build(self, version, snap: Snapshot, plan: _Plan) -> ResidentDataset:
+        """The entry ``plan`` describes: its columns uploaded, parsed or copied in table order, then its text columns.  On
+        any failure (a bad cell: the first in table order, so in request order) what this call made is freed and
+        re-raised."""
         if plan.columns is None:
-            table, names, kinds, nulls = base.table, base.fields, base.kinds, base.nulls
+            table, names, kinds, nulls = plan.shared.table, plan.shared.fields, plan.shared.kinds, plan.shared.nulls
         else:
             names, kinds, nulls = [f for f, _slab in plan.columns], [], []
             table = self.engine.table("f64", len(snap.row_ids) if names else 0, max(len(names), 1))
@@ -381,6 +431,11 @@ class ResidentTables:
                     if len(snap.row_ids):
                         table.upload(j, values)
                     kinds.append(kind); nulls.append(int(valid.size - np.count_nonzero(valid)))
+                elif how == "copy":
+                    from_table, from_col, kind, n_null = src
+                    if len(snap.row_ids):
+                        self.engine.copy_column(from_table, from_col, table, j)
+                    kinds.append(kind); nulls.append(n_null)
                 else:
                     kind, n_null = parse_text_column(self.engine, table, j, src)
                     kinds.append(kind); nulls.append(n_null)
@@ -389,8 +444,53 @@ class ResidentTables:
         except BaseException:
             ResidentDataset(version, snap.row_ids, [], [], [], None if plan.columns is None else table, made).free()
             raise
-        return ResidentDataset(version, snap.row_ids, names, kinds, nulls, table, {**plan.texts, **made}, plan.absent,
-                               plan.numbers)
+        texts = {**plan.texts, **made}
+        sources = None
+        if snap.columnar:
+            sources = {("slab", f): (snap.column(f),) for f in names}
+            sources.update({("text", f): (snap.column(f),) for f, t in texts.items() if t is not None})
+        return ResidentDataset(version, snap.row_ids, names, kinds, nulls, table, texts, plan.absent, plan.numbers,
+                               sources)
+
+    def adopt(self, filename: str, field: str, column, obj=None, slab=None, same_as=None) -> None:
+        """Hand the cache the device result of a conversion that replaced column ``field`` of a column store by
+        ``column``, so that the next miss takes it instead of building it from the host (:func:`_carried`).  ``obj``: a
+        text column made from ``column``, or with ``slab`` = (kind, nulls) a one-column f64 table holding its values;
+        None: the slab the cached entry made from column ``same_as`` (the one ``column`` replaced) holds them.  The cache owns ``obj`` from here on:
+        it counts toward ``max_bytes`` and is freed with the entry it joins (invalidate, clear, eviction, the next
+        version), or at once when there is no column-store entry to join."""
+        with self._lock:
+            entry = self._entries.get(filename)
+            if entry is None or entry.sources is None:
+                if obj is not None:
+                    obj.free()
+                return
+            if obj is None:
+                key = ("slab", field)
+                if any(c is same_as for c in entry.sources.get(key, ())):
+                    entry.sources[key] += (column,)
+                return
+            key = ("slab" if slab is not None else "text", field)
+            obj.holders = getattr(obj, "holders", 0) + 1
+            old = entry.adopted.pop(key, None)
+            entry.adopted[key] = (column, obj, *(slab or (None, None)))
+            if old is not None:
+                old[1].holders -= 1
+                if old[1].holders <= 0:
+                    old[1].free()
+            self._evict()
+
+    def holding(self, database, filename: str, field: str, snapshot: "Snapshot") -> ResidentDataset | None:
+        """The cached entry at ``snapshot``'s version when its table holds a slab of ``field``, LEASED (a hit: pair it
+        with :meth:`release`); else None, and nothing is built."""
+        with self._lock:
+            entry = self._entries.get(filename)
+            if entry is None or snapshot.version is None or entry.version != snapshot.version or field not in entry.column:
+                return None
+            self._entries.move_to_end(filename)
+            self.hits += 1
+            entry.users += 1
+            return entry
 
     def _evict(self):
         total = sum(e.nbytes for e in self._entries.values())
