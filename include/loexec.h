@@ -58,6 +58,7 @@ extern "C" {
 #define LO_F32 2   /* IEEE binary32 */
 #define LO_U8  3   /* unsigned byte */
 #define LO_U32 4   /* dictionary codes (host entry points only) */
+#define LO_I32 5   /* dictionary codes of a text column (lo_text_codes): tables only, no compute entry reads them */
 
 /* synthetic generators (oracle/bsem.c and oracle/bsem_numpy.py hold the bit-identical CPU twins) */
 #define LO_SYNTH_UNIFORM   0  /* f64: lo + (hi-lo) * (splitmix64(...)>>11) * 2^-53            */
@@ -397,6 +398,40 @@ int lo_value_counts_text(lo_ctx *ctx, const lo_text *t, int64_t *rep_rows_out, u
 int lo_value_counts_text_shards(lo_ctx *root, const lo_text *const *shards, const int64_t *row0, int32_t nshards,
                                 int64_t *rep_rows_out, uint64_t *counts_out, int64_t capacity, int64_t *ndistinct,
                                 lo_host_timing *timing);
+
+/* Dictionary codes of one resident text column, for a GPU consumer that indexes words itself (a model's categorical
+ * inputs).  Row i of column `col` of `out` (LO_I32, nrows == the text's n, on the text's device) receives -1 for a null
+ * row, else the code of its cell: the distinct non-null cells are numbered 0, 1, ... in the order of their FIRST ROWS
+ * (the order of Arrow's dictionary_encode).  Cells compare byte for byte; "" is a cell, not a null.
+ * first_rows_out[c] = the first row of code c (ascending): the dictionary is the cells at those rows.  capacity /
+ * *ndistinct as in lo_value_counts_text: more distinct cells than capacity -> LO_ERR_INVALID with *ndistinct set and the
+ * first `capacity` first rows copied (the codes are written all the same).  Codes do not depend on the hash table's
+ * layout, nor on how the column is cut into shards.
+ * Refused with LO_ERR_INVALID before anything is launched: a NULL text or out, text made on another context, `out` not
+ * LO_I32 or of other rows than the text or on another device, `col` outside [0, ncols), a negative capacity, a NULL
+ * ndistinct, a NULL first_rows_out with capacity > 0.
+ * Launches: 6 (count, slot pass, compact, radix sort, rank, remap) when a cell is not null, else none (the column is set
+ * to -1).  timing: kernel_ms the call's kernels (between events on the context's stream, the group count read between
+ * them left out), h2d_bytes 0, d2h_bytes the group count and the first rows read back. */
+int lo_text_codes(lo_ctx *ctx, const lo_text *t, lo_table *out, int32_t col, int64_t *first_rows_out,
+                  int64_t capacity, int64_t *ndistinct, lo_host_timing *timing);
+/* lo_text_codes of one text column cut into nshards row-range shards, laid out as for lo_value_counts_text_shards:
+ * shards[i] holds rows [row0[i], row0[i] + n_i), and its codes land in column `col` of out[i], a table on shards[i]'s
+ * device.  first_rows_out holds GLOBAL rows; codes and first rows equal lo_text_codes' on the whole column for any cut.
+ * Each shard numbers its own cells on its device and packs its distinct cells with their first global rows (the key
+ * column of lo_value_counts_text_shards); the keys are copied to root's device, merged there by the lowest first row
+ * of each cell and ordered, and each shard copies its keys' codes back and remaps its rows.
+ * Refused with LO_ERR_INVALID before anything is launched: a NULL root, shards, row0, out, shard or out[i]; nshards
+ * outside [1, LO_GROUP_MAX_DEVICES]; a negative, decreasing or overlapping row0; out[i] failing lo_text_codes' checks
+ * against shards[i]; a negative capacity, NULL ndistinct, NULL first_rows_out with capacity > 0.  More than 2^31-1
+ * distinct cells summed over the shards -> LO_ERR_INVALID before the root merges.
+ * Launches: 8 on the context of every shard with a non-null cell (count, slot pass, compact, key lengths, scan, key
+ * gather, rank, remap), none on a shard without one, and 5 on root (merge, compact, radix sort, rank, key remap).
+ * timing: total_ms the whole call, kernel_ms the root's merge and ordering, launches those on root's context during the
+ * call, h2d_bytes 0, d2h_bytes the group count and first rows read back on root. */
+int lo_text_codes_shards(lo_ctx *root, const lo_text *const *shards, const int64_t *row0, int32_t nshards,
+                         lo_table *const *out, int32_t col, int64_t *first_rows_out, int64_t capacity,
+                         int64_t *ndistinct, lo_host_timing *timing);
 
 /* Number -> text for one column: the reference's "string" cast, str(v) / None -> "" (data_type_handler_image/
  * data_type_update.py:22-28), for every cell at once on the GPU.  The inverse of lo_parse_number_host.

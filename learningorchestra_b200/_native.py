@@ -23,7 +23,7 @@ LO_ERR_NOT_IMPLEMENTED = -4
 LO_ERR_NO_DEVICE = -5
 LO_ERR_ALIGNMENT = -6
 
-LO_F64, LO_F32, LO_U8, LO_U32 = 1, 2, 3, 4
+LO_F64, LO_F32, LO_U8, LO_U32, LO_I32 = 1, 2, 3, 4, 5
 LO_SYNTH_UNIFORM, LO_SYNTH_EDGES, LO_SYNTH_CONSTCOL, LO_SYNTH_MNIST_U8 = 0, 1, 2, 3
 LO_MAX_BINS = 65536
 LO_MERGE_AUTO, LO_MERGE_PEER, LO_MERGE_NCCL = 0, 1, 2
@@ -155,6 +155,9 @@ SIGNATURES = {
     "lo_value_counts_text": (C.c_int, [_P, _P, _P, _P, C.c_int64, C.POINTER(C.c_int64), C.POINTER(HostTiming)]),
     "lo_value_counts_text_shards": (C.c_int, [_P, C.POINTER(_P), C.POINTER(C.c_int64), C.c_int32, _P, _P, C.c_int64,
                                               C.POINTER(C.c_int64), C.POINTER(HostTiming)]),
+    "lo_text_codes": (C.c_int, [_P, _P, _P, C.c_int32, _P, C.c_int64, C.POINTER(C.c_int64), C.POINTER(HostTiming)]),
+    "lo_text_codes_shards": (C.c_int, [_P, C.POINTER(_P), C.POINTER(C.c_int64), C.c_int32, C.POINTER(_P), C.c_int32, _P,
+                                       C.c_int64, C.POINTER(C.c_int64), C.POINTER(HostTiming)]),
     "lo_format_number_host": (C.c_int, [_P, _P, _P, C.c_int64, _P, _P, C.c_int64, C.POINTER(HostTiming)]),
     "lo_parse_text_to_table": (C.c_int, [_P, _P, _P, C.c_int32, C.POINTER(ParseSummary), C.POINTER(HostTiming)]),
     "lo_format_table_to_text": (C.c_int, [_P, _P, C.c_int32, C.POINTER(Validity), C.POINTER(Validity), C.POINTER(_P),

@@ -51,18 +51,33 @@ class DeviceFrame:
     """The processed frame for a GPU consumer: the HBM-resident slabs themselves, no device->host copy.
     ``columns[name]`` is a list of :class:`~learningorchestra_b200.engine.DeviceColumn` (one per shard: one element on a
     single GPU) exposing ``__cuda_array_interface__`` — nulls are NaN in the slab; ``nulls[name]`` counts them.
-    Holds a lease on the resident dataset: call :meth:`release` (or use ``with``) when the consumer is done."""
+    A text field (``device_frame(..., text=True)``) is a column of int32 dictionary codes instead, ``kinds[name] ==
+    "text"``: -1 for a null row, else the index of its cell in ``dictionaries[name]``, the Arrow array of the distinct
+    cells in the order of their first rows.  The frame owns those code tables (they are not cached) and frees them in
+    :meth:`release`.  Holds a lease on the resident dataset: call :meth:`release` (or use ``with``) when the consumer is
+    done."""
 
-    def __init__(self, cache, data, fields):
+    def __init__(self, cache, data, fields, codes=None):
         self._cache, self._data = cache, data
+        self._codes = dict(codes or {})          # text field -> (code table, dictionary)
         self.fields = list(fields)
         self.ids = data.ids
         shards = getattr(data.table, "shards", [data.table])
-        self.columns = {f: [t.column_view(data.column[f], keepalive=self) for t in shards] for f in self.fields}
-        self.kinds = {f: data.kinds[data.column[f]] for f in self.fields}
-        self.nulls = {f: data.nulls[data.column[f]] for f in self.fields}
+        self.columns, self.kinds, self.nulls, self.dictionaries = {}, {}, {}, {}
+        for f in self.fields:
+            if f in self._codes:
+                table, dictionary = self._codes[f]
+                self.columns[f] = [t.column_view(0, keepalive=self) for t in getattr(table, "shards", [table])]
+                self.kinds[f], self.nulls[f], self.dictionaries[f] = "text", data.texts[f].nulls, dictionary
+            else:
+                self.columns[f] = [t.column_view(data.column[f], keepalive=self) for t in shards]
+                self.kinds[f] = data.kinds[data.column[f]]
+                self.nulls[f] = data.nulls[data.column[f]]
 
     def release(self):
+        codes, self._codes = self._codes, {}
+        for table, _dictionary in codes.values():
+            table.free()
         if self._data is not None:
             self._cache.release(self._data)
             self._data = None
@@ -74,18 +89,40 @@ class DeviceFrame:
         self.release()
 
 
-def device_frame(database, filename, engine) -> DeviceFrame:
+def device_frame(database, filename, engine, text: bool = False) -> DeviceFrame:
     """``Builder.__file_processor``'s frame (data rows, metadata columns dropped) handed over ON THE DEVICE: the
     numeric fields of the dataset as zero-copy views of the resident slabs (``builder_image/builder.py:172-194`` loads
-    the same frame into Spark).  Text fields are not part of it — use :func:`file_processor` for the host form."""
+    the same frame into Spark).  ``text``: the fields of the store that are text (:class:`~table_cache.Snapshot`'s rule;
+    mixed fields stay out) join it as int32 dictionary codes made on the device from the resident text columns — the
+    same columns ``/histograms`` counts, uploaded only when none is resident yet; the fields keep the store's order.
+    Without ``text`` the frame holds the number fields alone — use :func:`file_processor` for the host form."""
     if getattr(database, "has_columns", lambda _f: False)(filename):
         names = [f for f in database.column_names(filename) if f not in METADATA_FIELDS]
         numeric = [f for f in names if getattr(database.column(filename, f), "kind", "") == "number"]
     else:
         names, rows = frame_fields(database, filename)
         numeric = [f for f in names if rows and columnar.numeric_column([d.get(f) for d in rows]) is not None]
-    data = engine.resident.ensure(database, filename, numeric)
-    return DeviceFrame(engine.resident, data, numeric)
+    if not text:
+        data = engine.resident.ensure(database, filename, numeric)
+        return DeviceFrame(engine.resident, data, numeric)
+    from .engine import text_dictionary
+    from .table_cache import Snapshot
+    snap = Snapshot(database, filename)
+    words = [f for f in names if f not in numeric and snap.field(f).text is not None]
+    data = engine.resident.ensure(database, filename, numeric, text=words, snapshot=snap)
+    codes = {}
+    try:
+        for f in words:
+            cells = data.texts[f]
+            table = engine.table("i32", cells.n, 1)
+            codes[f] = (table, None)             # freed below if its codes fail
+            codes[f] = (table, text_dictionary(cells.arr, engine.text_codes(cells, table, 0)))
+    except BaseException:
+        for table, _dictionary in codes.values():
+            table.free()
+        engine.resident.release(data)
+        raise
+    return DeviceFrame(engine.resident, data, [f for f in names if f in numeric or f in codes], codes)
 
 
 def _frame(fields, rows, packed, resident):

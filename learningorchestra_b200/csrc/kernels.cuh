@@ -1262,18 +1262,40 @@ __device__ __forceinline__ bool same_cell(const uint8_t *chars, const long long 
     return true;
 }
 
-// Add `add` rows to the group of slot word `mine` (tag | representative row) whose cell hashes to h, in the global table.
-__device__ __forceinline__ void str_table_add(const uint8_t *chars, const long long *offsets, unsigned long long *slots,
-                                              unsigned long long *counts, unsigned long long mask, unsigned long long h,
-                                              unsigned long long mine, unsigned long long add) {
+// The slot of the group of slot word `mine` (tag | representative row) whose cell hashes to h, in the global table;
+// claimed for it when the group is new.
+__device__ __forceinline__ unsigned long long str_table_slot(const uint8_t *chars, const long long *offsets,
+                                                             unsigned long long *slots, unsigned long long mask,
+                                                             unsigned long long h, unsigned long long mine) {
     const long long row = (long long)(mine & 0x7FFFFFFFull);
     unsigned long long s = splitmix64(h) & mask;
     for (;;) {
         const unsigned long long cur = atomicCAS(slots + s, kEmptyKey, mine);
-        if (cur == kEmptyKey || ((cur >> 31) == (mine >> 31) && same_cell(chars, offsets, row, (long long)(cur & 0x7FFFFFFFull)))) {
-            atomicAdd(counts + s, add);
-            return;
-        }
+        if (cur == kEmptyKey || ((cur >> 31) == (mine >> 31) && same_cell(chars, offsets, row, (long long)(cur & 0x7FFFFFFFull))))
+            return s;
+        s = (s + 1) & mask;
+    }
+}
+
+// Add `add` rows to the group of slot word `mine` whose cell hashes to h, in the global table.
+__device__ __forceinline__ void str_table_add(const uint8_t *chars, const long long *offsets, unsigned long long *slots,
+                                              unsigned long long *counts, unsigned long long mask, unsigned long long h,
+                                              unsigned long long mine, unsigned long long add) {
+    atomicAdd(counts + str_table_slot(chars, offsets, slots, mask, h, mine), add);
+}
+
+// The slot of the group of row `row`, whose cell hashes to h, in a finished table that holds that cell: a lookup with
+// the probe order and compare of str_table_slot, never an insert.  An empty slot ends the probe (the cell was never
+// inserted, which a table built from the same column cannot produce) instead of reading past it.
+__device__ __forceinline__ unsigned long long str_table_find(const uint8_t *chars, const long long *offsets,
+                                                             const unsigned long long *__restrict__ slots,
+                                                             unsigned long long mask, unsigned long long h, long long row) {
+    unsigned long long s = splitmix64(h) & mask;
+    for (;;) {
+        const unsigned long long cur = slots[s];
+        if (cur == kEmptyKey ||
+            ((cur >> 31) == (h >> 31) && same_cell(chars, offsets, row, (long long)(cur & 0x7FFFFFFFull))))
+            return s;
         s = (s + 1) & mask;
     }
 }
@@ -1415,6 +1437,89 @@ __global__ void k_take_rows(long long *__restrict__ rows, const long long *__res
     for (unsigned long long g = blockIdx.x * (unsigned long long)blockDim.x + threadIdx.x; g < n;
          g += (unsigned long long)gridDim.x * blockDim.x)
         rows[g] = global_rows[rows[g]];
+}
+
+// ---------------------------------------------------------------------------------------------
+// dictionary codes of a TEXT column (lo_text_codes, lo_text_codes_shards): an int32 code per row, -1 for a null row,
+// the distinct cells numbered 0, 1, ... in the order of their first rows.  After k_hash_count_str has built the table,
+// k_text_slots writes each live row's slot into the code column and keeps each slot's lowest row; k_compact_first lists
+// the occupied slots with those rows; a radix sort of (first row, slot) orders them and k_rank_slots gives every slot
+// its code; k_remap_codes turns each row's slot into its code.  The table's compaction order is not deterministic, the
+// first rows are: the codes do not depend on it, nor on how the column is cut into shards.
+// ---------------------------------------------------------------------------------------------
+__device__ __forceinline__ bool text_row_live(const uint8_t *valid_mask, const uint8_t *valid_bitmap, int bit0, long long i) {
+    return valid_mask ? valid_mask[i] != 0
+                      : valid_bitmap ? ((valid_bitmap[(bit0 + i) >> 3] >> ((bit0 + i) & 7)) & 1) != 0 : true;
+}
+
+// The slot pass: codes[i] = the slot of row i's group (its bit pattern as an int32; a table has at most 2^32 slots),
+// -1 for a null row; first[slot] = min over the group's rows.  The lowest lane of a warp holding a group has its lowest
+// row there, so only that lane moves first[] and only while its row is below what first[] already holds.
+__global__ void __launch_bounds__(256) k_text_slots(const uint8_t *__restrict__ chars, const long long *__restrict__ offsets,
+                                                    long long n, const uint8_t *__restrict__ valid_mask,
+                                                    const uint8_t *__restrict__ valid_bitmap, int bit0,
+                                                    const unsigned long long *__restrict__ slots, unsigned long long mask,
+                                                    unsigned long long *first, int *__restrict__ codes) {
+    for (long long i0 = blockIdx.x * (long long)blockDim.x; i0 < n; i0 += (long long)gridDim.x * blockDim.x) {
+        const long long i = i0 + threadIdx.x;
+        const bool live = i < n && text_row_live(valid_mask, valid_bitmap, bit0, i);
+        const unsigned active = __ballot_sync(0xffffffffu, live);
+        if (!live) {
+            if (i < n) codes[i] = -1;
+            continue;
+        }
+        const unsigned long long h = hash_bytes(chars + offsets[i], offsets[i + 1] - offsets[i]);
+        const unsigned long long s = str_table_find(chars, offsets, slots, mask, h, i);
+        codes[i] = (int)(unsigned)s;
+        const unsigned peers = __match_any_sync(active, s);
+        if ((int)(threadIdx.x & 31) == __ffs(peers) - 1 && *(volatile unsigned long long *)(first + s) > (unsigned long long)i)
+            atomicMin(first + s, (unsigned long long)i);
+    }
+}
+
+// The merge of lo_text_codes_shards: key i of the concatenated key column (chars / offsets) is a shard's group, its
+// weight the group's first GLOBAL row.  The table keeps each group's lowest first row in first[] (all ones before) and
+// key_slot[i] receives the slot key i landed in.
+__global__ void __launch_bounds__(256) k_hash_min_str(const uint8_t *__restrict__ chars, const long long *__restrict__ offsets,
+                                                      const unsigned long long *__restrict__ weight, long long n,
+                                                      unsigned long long *__restrict__ slots,
+                                                      unsigned long long *__restrict__ first, unsigned long long mask,
+                                                      unsigned *__restrict__ key_slot) {
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+        const unsigned long long h = hash_bytes(chars + offsets[i], offsets[i + 1] - offsets[i]);
+        const unsigned long long s = str_table_slot(chars, offsets, slots, mask, h, ((h >> 31) << 31) | (unsigned long long)i);
+        atomicMin(first + s, weight[i]);
+        key_slot[i] = (unsigned)s;
+    }
+}
+
+// k_hash_compact_str for the codes: the occupied slots and their first rows, at most `capacity` of them
+__global__ void k_compact_first(const unsigned long long *__restrict__ slots, const unsigned long long *__restrict__ first,
+                                unsigned long long nslots, unsigned long long *__restrict__ out_first,
+                                unsigned *__restrict__ out_slot, unsigned long long capacity,
+                                unsigned long long *__restrict__ n_out) {
+    for (unsigned long long i = blockIdx.x * (unsigned long long)blockDim.x + threadIdx.x; i < nslots;
+         i += (unsigned long long)gridDim.x * blockDim.x) {
+        if (slots[i] != kEmptyKey) {
+            const unsigned long long pos = atomicAdd(n_out, 1ull);
+            if (pos < capacity) { out_first[pos] = first[i]; out_slot[pos] = (unsigned)i; }
+        }
+    }
+}
+
+// slot_code[slot[g]] = code[g] (code == nullptr: g, the group's rank in first-row order) for g < n
+__global__ void k_rank_slots(const unsigned *__restrict__ slot, const int *__restrict__ code, long long n,
+                             unsigned long long *__restrict__ slot_code) {
+    for (long long g = blockIdx.x * (long long)blockDim.x + threadIdx.x; g < n; g += (long long)gridDim.x * blockDim.x)
+        slot_code[slot[g]] = code ? (unsigned long long)(unsigned)code[g] : (unsigned long long)g;
+}
+
+// codes[i] = slot_code[codes[i]] for every live row (validity as k_text_slots reads it; none: every row)
+__global__ void k_remap_codes(int *__restrict__ codes, long long n, const uint8_t *__restrict__ valid_mask,
+                              const uint8_t *__restrict__ valid_bitmap, int bit0,
+                              const unsigned long long *__restrict__ slot_code) {
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+        if (text_row_live(valid_mask, valid_bitmap, bit0, i)) codes[i] = (int)slot_code[(unsigned)codes[i]];
 }
 
 // R-semantics cast "number" (data_type_update.py:40-43): one cell per thread, CPython float() grammar,

@@ -6,6 +6,7 @@
 #include "loexec.h"
 #include "kernels.cuh"
 
+#include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
 
 #include <algorithm>
@@ -65,6 +66,7 @@ size_t dtype_size(int dtype) {
         case LO_F32: return 4;
         case LO_U8:  return 1;
         case LO_U32: return 4;
+        case LO_I32: return 4;
         default:     return 0;
     }
 }
@@ -1118,6 +1120,7 @@ int lo_table_checksum(lo_ctx *ctx, const lo_table *t, int32_t col, int64_t row_o
     LO_TRY(check_ctx(ctx));
     LO_TRY(check_range(t, col, 0, 0));
     if (!out) return fail(LO_ERR_INVALID, "out is NULL");
+    if (t->dtype == LO_I32) return fail(LO_ERR_INVALID, "table dtype LO_I32: the checksum reads LO_F64, LO_F32 and LO_U8 slabs");
     HostCall c(ctx, "checksum");
     unsigned long long *d = nullptr, h = 0;
     c.alloc(&d, 8);
@@ -1848,6 +1851,335 @@ int lo_value_counts_text_shards(lo_ctx *root, const lo_text *const *shards, cons
         if (s.gathered) cudaEventDestroy(s.gathered);
     }
     if (copied) cudaEventDestroy(copied);
+    cudaSetDevice(root->device);
+    g_err = msg;
+    return rc;
+}
+
+}  // extern "C"
+
+// ---- dictionary codes of resident text columns (lo_text_codes, lo_text_codes_shards) ------------------------------
+namespace {
+
+// The output of a codes call on text column t: column `col` of an LO_I32 table of t->n rows on t's device.
+int check_codes_out(const lo_text *t, const lo_table *out, int32_t col, const char *name) {
+    if (!out) return fail(LO_ERR_INVALID, "%s is NULL", name);
+    if (out->dtype != LO_I32) return fail(LO_ERR_INVALID, "%s: dtype %d is not LO_I32", name, out->dtype);
+    if (col < 0 || col >= out->ncols) return fail(LO_ERR_INVALID, "%s: column %d outside [0, %d)", name, col, out->ncols);
+    if (out->nrows != t->n)
+        return fail(LO_ERR_INVALID, "%s has %lld rows, its text column %lld", name, (long long)out->nrows, (long long)t->n);
+    if (out->device != t->ctx->device)
+        return fail(LO_ERR_INVALID, "%s lives on device %d, its text column on %d", name, out->device, t->ctx->device);
+    return LO_OK;
+}
+
+int *codes_col(const lo_table *out, int32_t col) { return (int *)(out->base + (int64_t)col * out->pitch); }
+
+// the bits a radix sort of rows up to max_row orders (at least 1)
+int row_bits(int64_t max_row) {
+    int b = 1;
+    while (b < 63 && (max_row >> b)) ++b;
+    return b;
+}
+
+// a table of at least twice as many slots as groups, 1024 or more (count_groups' sizing)
+unsigned long long slots_for(int64_t groups) {
+    unsigned long long s = 1024;
+    while (s < 2ull * (unsigned long long)groups) s <<= 1;
+    return s;
+}
+
+// One column's table of a codes call and the groups listed from it
+struct CodesTable {
+    unsigned long long *keys = nullptr;       // the slot words
+    unsigned long long *first = nullptr;      // per slot: k_hash_count_str's counts, then the first row, then the code
+    unsigned long long nslots = 0;
+    unsigned long long *grp_first = nullptr;  // k_compact_first: the groups' first rows [0, cap), their number at [cap]
+    unsigned *grp_slot = nullptr;             // and their slots
+};
+
+// The column's half of a codes call on c's stream, for a text column of n rows, `live` of them not null: the table
+// k_hash_count_str builds, the slot pass into `codes` and the compaction of the occupied slots with their first rows.
+// Three launches.
+void codes_slots(HostCall &c, const TextCols &t, int64_t n, int64_t live, int *codes, CodesTable &T) {
+    T.nslots = slots_for(live);
+    const unsigned long long mask = T.nslots - 1;
+    c.alloc(&T.keys, T.nslots * 8);
+    c.alloc(&T.first, T.nslots * 8);
+    c.alloc(&T.grp_first, (size_t)(live + 1) * 8);
+    c.alloc(&T.grp_slot, (size_t)live * 4);
+    c.memset(T.keys, 0xFF, T.nslots * 8);
+    c.memset(T.first, 0, T.nslots * 8);
+    c.memset(T.grp_first + live, 0, 8);
+    c.launch(1, [&] {
+        lo::k_hash_count_str<<<grid_for(c.ctx, n), 256, 0, c.s>>>(t.chars, t.offsets, n, t.mask, t.bitmap, t.bit0, T.keys,
+                                                                   T.first, mask);
+    });
+    c.memset(T.first, 0xFF, T.nslots * 8);    // the counts are not needed: the same words keep the first rows
+    c.launch(1, [&] {
+        lo::k_text_slots<<<grid_for(c.ctx, n), 256, 0, c.s>>>(t.chars, t.offsets, n, t.mask, t.bitmap, t.bit0, T.keys, mask,
+                                                               T.first, codes);
+    });
+    c.launch(1, [&] {
+        lo::k_compact_first<<<c.ctx->sm_count * 8, 256, 0, c.s>>>(T.keys, T.first, T.nslots, T.grp_first, T.grp_slot,
+                                                                   (unsigned long long)live, T.grp_first + live);
+    });
+}
+
+// Orders nd groups (first rows and slots as k_compact_first lists them) by first row: sorted_first receives the first
+// rows in code order and slot_code[slot] each group's code.  Two launches: the radix sort over the rows' low `bits`
+// bits (first rows are unique per group, so no tie is left to the sort) and k_rank_slots.
+void order_groups(HostCall &c, const unsigned long long *first, const unsigned *slot, int64_t nd, int bits,
+                  unsigned long long *sorted_first, unsigned long long *slot_code) {
+    unsigned *sorted_slot = nullptr;
+    void *tmp = nullptr;
+    size_t tmp_bytes = 0;
+    c.alloc(&sorted_slot, (size_t)nd * 4);
+    c.run([&] { return cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, first, sorted_first, slot, sorted_slot, nd, 0, bits, c.s); });
+    c.alloc(&tmp, tmp_bytes);
+    c.launch(1, [&] { return cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, first, sorted_first, slot, sorted_slot, nd, 0, bits, c.s); });
+    c.launch(1, [&] { lo::k_rank_slots<<<grid_for(c.ctx, nd), 256, 0, c.s>>>(sorted_slot, nullptr, nd, slot_code); });
+    c.drop(tmp);
+    c.drop(sorted_slot);
+}
+
+// The end of a codes call: the first min(nd, capacity) first rows copied out and the call finished.  More groups than
+// capacity is refused after *ndistinct is set, as copy_groups does; the codes are written all the same.
+int copy_first_rows(HostCall &c, const unsigned long long *sorted_first, unsigned long long nd, int64_t capacity,
+                    int64_t *first_rows_out, int64_t *ndistinct, lo_host_timing *timing) {
+    const size_t take = (size_t)std::min<unsigned long long>(nd, (unsigned long long)capacity);
+    c.to_host(first_rows_out, sorted_first, take * 8);
+    LO_TRY(c.finish(timing));
+    *ndistinct = (int64_t)nd;
+    if ((int64_t)nd > capacity)
+        return fail(LO_ERR_INVALID, "%llu distinct cells do not fit the caller's capacity %lld", nd, (long long)capacity);
+    return LO_OK;
+}
+
+// one shard of lo_text_codes_shards, worked on its own context's call frame and stream
+struct CodesShard {
+    const lo_text *t;
+    int *codes;
+    int64_t row0;
+    int64_t live;                            // n - nulls: at most this many groups
+    std::unique_ptr<HostCall> c;
+    CodesTable T;
+    long long *key_off = nullptr;            // the packed key column of its groups: nd + 1 offsets, then the bytes
+    uint8_t *key_chars = nullptr;
+    int *key_code = nullptr;                 // the global codes of its groups, copied back from the root
+    cudaEvent_t gathered = nullptr;          // the packed pieces are ready to copy
+    cudaEvent_t taken = nullptr;             // the shard has copied its codes from the root
+    unsigned long long nd = 0;
+    long long bytes = 0, group0 = 0, byte0 = 0;   // its bytes, and where its pieces start in the concatenated column
+};
+
+}  // namespace
+
+extern "C" {
+
+int lo_text_codes(lo_ctx *ctx, const lo_text *t, lo_table *out, int32_t col, int64_t *first_rows_out, int64_t capacity,
+                  int64_t *ndistinct, lo_host_timing *timing) {
+    LO_TRY(check_ctx(ctx));
+    if (!t) return fail(LO_ERR_INVALID, "text is NULL");
+    if (t->ctx != ctx) return fail(LO_ERR_INVALID, "text belongs to another context");
+    LO_TRY(check_codes_out(t, out, col, "out"));
+    LO_TRY(check_ndistinct(capacity, ndistinct));
+    if (capacity > 0 && !first_rows_out) return fail(LO_ERR_INVALID, "NULL argument: first_rows_out with capacity > 0");
+    HostCall c(ctx, "text_codes");
+    int *codes = codes_col(out, col);
+    const int64_t live = t->n - t->nulls;
+    if (live == 0) {                         // no cell to number (n == 0 included): every row is -1
+        c.memset(codes, 0xFF, (size_t)t->n * 4);
+        return c.finish(timing);
+    }
+    CodesTable T;
+    c.mark();
+    codes_slots(c, t->cols, t->n, live, codes, T);
+    c.mark();
+    unsigned long long nd = 0, *sorted = nullptr;
+    c.to_host(&nd, T.grp_first + live, 8);
+    c.sync();
+    c.alloc(&sorted, nd * 8);
+    c.mark();
+    order_groups(c, T.grp_first, T.grp_slot, (int64_t)nd, row_bits(t->n - 1), sorted, T.first);
+    c.launch(1, [&] {
+        lo::k_remap_codes<<<grid_for(ctx, t->n), 256, 0, c.s>>>(codes, t->n, t->cols.mask, t->cols.bitmap, t->cols.bit0, T.first);
+    });
+    c.mark();
+    return copy_first_rows(c, sorted, nd, capacity, first_rows_out, ndistinct, timing);
+}
+
+// Codes of one text column cut into row-range shards, each resident on its own context (loexec.h).  Each step is
+// enqueued on every shard before the host waits on any, so shards on different devices run at once:
+//   1. each shard's table, slot pass and compaction (codes_slots); the host reads its group count;
+//   2. the byte lengths of its groups' cells (at their first rows) and their exclusive scan; the host reads its key bytes;
+//   3. k_gather_cells packs the keys and turns the first rows global: they are the keys' weights;
+//   4. the root copies the packed pieces over with cudaMemcpyPeerAsync, merges them with k_hash_min_str (each group's
+//      lowest global first row, each key's slot), compacts and orders the groups, and remaps its key slots to codes;
+//   5. each shard copies its keys' codes back, writes them to its own slots (k_rank_slots) and remaps its rows.
+// The root's scratch is freed after every shard has taken its codes; a shard's after the root's step 4, which it waits on.
+int lo_text_codes_shards(lo_ctx *root, const lo_text *const *shards, const int64_t *row0, int32_t nshards,
+                         lo_table *const *out, int32_t col, int64_t *first_rows_out, int64_t capacity, int64_t *ndistinct,
+                         lo_host_timing *timing) {
+    if (!root) return fail(LO_ERR_INVALID, "root is NULL");
+    if (nshards < 1 || nshards > LO_GROUP_MAX_DEVICES)
+        return fail(LO_ERR_INVALID, "nshards = %d: 1 to %d shards", nshards, LO_GROUP_MAX_DEVICES);
+    if (!shards || !row0 || !out) return fail(LO_ERR_INVALID, "shards, row0 or out is NULL");
+    std::vector<CodesShard> sh;              // the shards with a row
+    for (int i = 0; i < nshards; ++i) {
+        if (!shards[i]) return fail(LO_ERR_INVALID, "shards[%d] is NULL", i);
+        if (row0[i] < 0) return fail(LO_ERR_INVALID, "row0[%d] = %lld is negative", i, (long long)row0[i]);
+        if (i > 0 && row0[i] < row0[i - 1] + shards[i - 1]->n)
+            return fail(LO_ERR_INVALID, "row0[%d] = %lld: shard %d ends at row %lld (shards are disjoint and in row order)",
+                        i, (long long)row0[i], i - 1, (long long)(row0[i - 1] + shards[i - 1]->n));
+        char name[16];
+        snprintf(name, sizeof name, "out[%d]", i);
+        LO_TRY(check_codes_out(shards[i], out[i], col, name));
+        if (shards[i]->n > 0)
+            sh.push_back(CodesShard{shards[i], codes_col(out[i], col), row0[i], shards[i]->n - shards[i]->nulls});
+    }
+    LO_TRY(check_ndistinct(capacity, ndistinct));
+    if (capacity > 0 && !first_rows_out) return fail(LO_ERR_INVALID, "NULL argument: first_rows_out with capacity > 0");
+    LO_TRY(check_ctx(root));
+    HostCall c(root, "text_codes_shards");
+    for (CodesShard &s : sh) s.c = std::make_unique<HostCall>(s.t->ctx, "text_codes_shards", false);
+    auto ok = [&] { return c.ok() && std::all_of(sh.begin(), sh.end(), [](const CodesShard &s) { return s.c->ok(); }); };
+    // step(s, its call frame) for every shard with a cell to number, in row order, on the shard's device, until the
+    // root or a shard fails
+    auto each_shard = [&](auto step) {
+        for (CodesShard &s : sh) {
+            if (!ok()) return;
+            if (!s.live) continue;
+            s.c->run([&] { return cudaSetDevice(s.t->ctx->device); });
+            step(s, *s.c);
+        }
+    };
+    for (CodesShard &s : sh)                 // a shard without a cell: every row is -1, no launch
+        if (!s.live && ok()) {
+            s.c->run([&] { return cudaSetDevice(s.t->ctx->device); });
+            s.c->memset(s.codes, 0xFF, (size_t)s.t->n * 4);
+        }
+    // 1. table, slot pass, compaction
+    each_shard([](CodesShard &s, HostCall &sc) { codes_slots(sc, s.t->cols, s.t->n, s.live, s.codes, s.T); });
+    each_shard([](CodesShard &s, HostCall &sc) { sc.to_host(&s.nd, s.T.grp_first + s.live, 8); sc.sync(); });
+    each_shard([](CodesShard &s, HostCall &sc) {  // 2. key lengths and their scan
+        const int64_t nd = (int64_t)s.nd;
+        size_t scan_bytes = 0;
+        void *tmp = nullptr;
+        sc.alloc(&s.key_off, (size_t)(nd + 1) * 8);
+        sc.run([&] { return cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, s.key_off, nd + 1, sc.s); });
+        sc.alloc(&tmp, scan_bytes);
+        sc.memset(s.key_off + nd, 0, 8);     // the scan's last input: key_off[nd] = the key bytes
+        sc.launch(1, [&] {
+            lo::k_gather_lens<<<grid_for(sc.ctx, nd), 256, 0, sc.s>>>(s.t->cols.offsets, (const long long *)s.T.grp_first, nd,
+                                                                        s.key_off);
+        });
+        sc.launch(1, [&] { return cub::DeviceScan::ExclusiveSum(tmp, scan_bytes, s.key_off, nd + 1, sc.s); });
+        sc.drop(tmp);
+    });
+    long long groups = 0, bytes = 0;
+    int64_t max_row = 0;
+    each_shard([&](CodesShard &s, HostCall &sc) {
+        sc.to_host(&s.bytes, s.key_off + s.nd, 8);
+        sc.sync();
+        s.group0 = groups;
+        s.byte0 = bytes;
+        groups += (long long)s.nd;
+        bytes += s.bytes;
+        max_row = s.row0 + s.t->n - 1;
+    });
+    if (ok() && groups >> 31)                // the merge's slot word keeps a 31-bit key index, and codes are int32
+        c.check([&] { return fail(LO_ERR_INVALID, "the shards hold %lld distinct cells: at most 2^31-1 can be numbered", groups); });
+    each_shard([](CodesShard &s, HostCall &sc) {  // 3. pack the keys; their first rows become global
+        sc.alloc(&s.key_chars, (size_t)s.bytes);
+        sc.launch(1, [&] {
+            lo::k_gather_cells<<<grid_for(sc.ctx, (int64_t)s.nd + 1), 256, 0, sc.s>>>(s.t->cols.chars, s.t->cols.offsets,
+                (long long *)s.T.grp_first, (long long)s.nd, s.key_off, s.key_chars, s.row0, s.byte0);
+        });
+        sc.run([&] { return cudaEventCreateWithFlags(&s.gathered, cudaEventDisableTiming); });
+        sc.run([&] { return cudaEventRecord(s.gathered, sc.s); });
+    });
+    unsigned long long nd = 0, *sorted = nullptr;
+    cudaEvent_t remapped = nullptr;
+    if (ok() && groups > 0) {                // 4. copy the pieces to the root, merge and order them there
+        c.run([&] { return cudaSetDevice(root->device); });
+        uint8_t *chars = nullptr;
+        long long *offsets = nullptr;
+        unsigned long long *weight = nullptr;
+        unsigned *key_slot = nullptr;
+        c.alloc(&chars, (size_t)bytes);
+        c.alloc(&offsets, (size_t)(groups + 1) * 8);
+        c.alloc(&weight, (size_t)groups * 8);
+        c.alloc(&key_slot, (size_t)groups * 4);
+        for (CodesShard &s : sh) {
+            if (!s.live) continue;
+            const int dev = s.t->ctx->device;
+            c.run([&] { return cudaStreamWaitEvent(c.s, s.gathered, 0); });
+            // nd + 1 offsets: the last is the next shard's first (the same value), or offsets[groups]
+            c.run([&] { return cudaMemcpyPeerAsync(offsets + s.group0, root->device, s.key_off, dev, (s.nd + 1) * 8, c.s); });
+            c.run([&] { return cudaMemcpyPeerAsync(weight + s.group0, root->device, s.T.grp_first, dev, s.nd * 8, c.s); });
+            if (s.bytes) c.run([&] { return cudaMemcpyPeerAsync(chars + s.byte0, root->device, s.key_chars, dev, s.bytes, c.s); });
+        }
+        CodesTable R;
+        R.nslots = slots_for(groups);
+        c.alloc(&R.keys, R.nslots * 8);
+        c.alloc(&R.first, R.nslots * 8);
+        c.alloc(&R.grp_first, (size_t)(groups + 1) * 8);
+        c.alloc(&R.grp_slot, (size_t)groups * 4);
+        c.mark();
+        c.memset(R.keys, 0xFF, R.nslots * 8);
+        c.memset(R.first, 0xFF, R.nslots * 8);
+        c.memset(R.grp_first + groups, 0, 8);
+        c.launch(1, [&] {
+            lo::k_hash_min_str<<<grid_for(root, groups), 256, 0, c.s>>>(chars, offsets, weight, groups, R.keys, R.first,
+                                                                         R.nslots - 1, key_slot);
+        });
+        c.launch(1, [&] {
+            lo::k_compact_first<<<root->sm_count * 8, 256, 0, c.s>>>(R.keys, R.first, R.nslots, R.grp_first, R.grp_slot,
+                                                                      (unsigned long long)groups, R.grp_first + groups);
+        });
+        c.mark();
+        c.to_host(&nd, R.grp_first + groups, 8);
+        c.sync();
+        c.alloc(&sorted, nd * 8);
+        c.mark();
+        order_groups(c, R.grp_first, R.grp_slot, (int64_t)nd, row_bits(max_row), sorted, R.first);
+        c.launch(1, [&] {   // key i's slot -> its code, in place
+            lo::k_remap_codes<<<grid_for(root, groups), 256, 0, c.s>>>((int *)key_slot, groups, nullptr, nullptr, 0, R.first);
+        });
+        c.mark();
+        c.run([&] { return cudaEventCreateWithFlags(&remapped, cudaEventDisableTiming); });
+        c.run([&] { return cudaEventRecord(remapped, c.s); });
+        each_shard([&](CodesShard &s, HostCall &sc) {   // 5. each shard's codes back, onto its slots and rows
+            const int64_t snd = (int64_t)s.nd;
+            sc.run([&] { return cudaStreamWaitEvent(sc.s, remapped, 0); });
+            sc.alloc(&s.key_code, (size_t)snd * 4);
+            sc.run([&] {
+                return cudaMemcpyPeerAsync(s.key_code, s.t->ctx->device, key_slot + s.group0, root->device, (size_t)snd * 4, sc.s);
+            });
+            sc.run([&] { return cudaEventCreateWithFlags(&s.taken, cudaEventDisableTiming); });
+            sc.run([&] { return cudaEventRecord(s.taken, sc.s); });
+            sc.launch(1, [&] { lo::k_rank_slots<<<grid_for(sc.ctx, snd), 256, 0, sc.s>>>(s.T.grp_slot, s.key_code, snd, s.T.first); });
+            sc.launch(1, [&] {
+                lo::k_remap_codes<<<grid_for(sc.ctx, s.t->n), 256, 0, sc.s>>>(s.codes, s.t->n, s.t->cols.mask, s.t->cols.bitmap,
+                                                                                s.t->cols.bit0, s.T.first);
+            });
+        });
+        c.run([&] { return cudaSetDevice(root->device); });
+        for (CodesShard &s : sh)             // the root's scratch is freed after every shard has read its codes
+            if (s.taken) c.run([&] { return cudaStreamWaitEvent(c.s, s.taken, 0); });
+    }
+    int rc = ok() ? copy_first_rows(c, sorted, nd, capacity, first_rows_out, ndistinct, timing)
+                  : c.finish(nullptr);       // synchronises the root: nothing of it reads a shard any more
+    std::string msg = g_err;
+    for (CodesShard &s : sh) {               // free every shard's scratch; the first error is the call's
+        cudaSetDevice(s.t->ctx->device);
+        const int r = s.c->finish(nullptr);
+        if (rc == LO_OK && r != LO_OK) { rc = r; msg = g_err; }
+        if (s.gathered) cudaEventDestroy(s.gathered);
+        if (s.taken) cudaEventDestroy(s.taken);
+    }
+    if (remapped) cudaEventDestroy(remapped);
     cudaSetDevice(root->device);
     g_err = msg;
     return rc;

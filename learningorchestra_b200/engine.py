@@ -20,8 +20,8 @@ import numpy as np
 
 from . import _native as N
 
-_DTYPES = {"f64": N.LO_F64, "f32": N.LO_F32, "u8": N.LO_U8}
-_NP = {N.LO_F64: np.float64, N.LO_F32: np.float32, N.LO_U8: np.uint8}
+_DTYPES = {"f64": N.LO_F64, "f32": N.LO_F32, "u8": N.LO_U8, "i32": N.LO_I32}
+_NP = {N.LO_F64: np.float64, N.LO_F32: np.float32, N.LO_U8: np.uint8, N.LO_I32: np.int32}
 
 
 def _stream_ptr(stream) -> C.c_void_p:
@@ -118,6 +118,32 @@ def _value_counts(call, n: int, key_dtype, timing: dict | None = None):
         if t is not None:
             timing.update(_timing(t), kernel_ms=t.kernel_ms)
         return keys[:nd.value], counts[:nd.value]
+
+
+def _first_rows(call, n: int, timing: dict | None = None) -> np.ndarray:
+    """The first rows (int64[ndistinct], ascending) of a lo_text_codes* call ``call(first_rows_out, capacity,
+    ndistinct_ref, timing_ref)`` on a column of ``n`` non-null cells: room for min(n, 65536) first rows, called again with
+    room for every one when they did not fit (as :func:`_value_counts`)."""
+    t = N.HostTiming() if timing is not None else None
+    cap = max(min(n, 1 << 16), 1)
+    while True:
+        rows = np.empty(cap, dtype=np.int64)
+        nd = C.c_int64()
+        rc = call(rows.ctypes.data_as(C.c_void_p), cap, C.byref(nd), C.byref(t) if t is not None else None)
+        if rc == N.LO_ERR_INVALID and nd.value > cap:
+            cap = int(nd.value)
+            continue
+        N.check(rc)
+        if t is not None:
+            timing.update(_timing(t), kernel_ms=t.kernel_ms)
+        return rows[:nd.value]
+
+
+def text_dictionary(arr, first_rows):
+    """The dictionary of a text column's codes: the cells of ``arr`` (the Arrow array that was uploaded) at
+    ``first_rows``, in code order — read the way ``histogram.text_groups`` reads group keys."""
+    import pyarrow as pa
+    return arr.take(pa.array(np.asarray(first_rows, dtype=np.int64)))
 
 
 def _pieces(source, buf: np.ndarray):
@@ -236,7 +262,7 @@ class DeviceColumn:
     ``torch.as_tensor(col, device="cuda")``, ``cupy.asarray(col)`` or Numba see the slab in place.  Keeps its table
     (and whatever the table keeps) alive."""
 
-    _TYPESTR = {N.LO_F64: "<f8", N.LO_F32: "<f4", N.LO_U8: "|u1"}
+    _TYPESTR = {N.LO_F64: "<f8", N.LO_F32: "<f4", N.LO_U8: "|u1", N.LO_I32: "<i4"}
 
     def __init__(self, table: "DeviceTable", col: int, keepalive=None):
         if not 0 <= col < table.ncols:
@@ -771,6 +797,17 @@ class Engine:
             return np.zeros(0, np.int64), np.zeros(0, np.uint64)
         return _value_counts(lambda rows, counts, cap, nd, t: self._lib.lo_value_counts_text(
             self._ctx, text._h, rows, counts, cap, nd, t), n, np.int64, timing)
+
+    def text_codes(self, text: DeviceText, table: DeviceTable, col: int, timing: dict | None = None) -> np.ndarray:
+        """Dictionary codes of a resident text column (``lo_text_codes``) into int32 column ``col`` of ``table`` (an
+        ``"i32"`` table with one row per cell): -1 for a null row, else the code of the cell, the distinct cells numbered
+        in the order of their first rows (``pyarrow.compute.dictionary_encode``'s order).  Returns those first rows
+        (int64, ascending): the dictionary is ``text.arr.take(first_rows)`` (:func:`text_dictionary`).  No cell crosses
+        PCIe.  ``timing``: a dict to receive the (last) call's lo_host_timing fields."""
+        if text._h is None:
+            raise ValueError("the text column has been freed")
+        return _first_rows(lambda rows, cap, nd, t: self._lib.lo_text_codes(
+            self._ctx, text._h, table._h, int(col), rows, cap, nd, t), text.n - text.nulls, timing)
 
     def value_counts_f64_host(self, values: np.ndarray):
         """(keys float64[g], counts uint64[g]) — exact value counts of a numeric column (GPU hash group-by),

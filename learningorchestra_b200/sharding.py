@@ -673,6 +673,26 @@ class ShardedEngine:
         return _value_counts(lambda rows, counts, cap, nd, t: self._lib.lo_value_counts_text_shards(
             self.engines[0]._ctx, handles, row0, k, rows, counts, cap, nd, t), n, np.int64, timing)
 
+    def text_codes(self, text: ShardedText, table: ShardedTable, col: int, timing=None):
+        """``Engine.text_codes`` of a :class:`ShardedText` into int32 column ``col`` of ``table`` (``lo_text_codes_shards``),
+        both cut at the same rows: every piece is numbered on its own device, the distinct cells are merged and ordered
+        on the first local member's device, and each shard's rows receive the global codes.  Returns the GLOBAL first rows
+        of the codes.  A rank group's process holds only its own rows, so it refuses rather than number a part."""
+        from .engine import _first_rows
+        self._every_row("text_codes")
+        if not isinstance(text, ShardedText):
+            raise TypeError("text_codes takes a ShardedText (ShardedEngine.text)")
+        if text.offsets != table.offsets or [p.n for p in text.pieces] != [t.nrows for t in table.shards]:
+            raise ValueError("the text column and the table are not cut at the same rows")
+        if any(p._h is None for p in text.pieces):
+            raise ValueError("the text column has been freed")
+        k = len(text.pieces)
+        handles = (C.c_void_p * k)(*[p._h for p in text.pieces])
+        row0 = (C.c_int64 * k)(*text.offsets)
+        return _first_rows(lambda rows, cap, nd, t: self._lib.lo_text_codes_shards(
+            self.engines[0]._ctx, handles, row0, k, self._tables(table), int(col), rows, cap, nd, t),
+            text.n - text.nulls, timing)
+
     @property
     def resident(self):
         """Datasets kept in HBM between requests, rows sharded over the group (:mod:`table_cache`)."""

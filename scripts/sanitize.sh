@@ -6,6 +6,11 @@ SEL='ragged_sizes or nbins or special_values or constant_column or histogram_onl
 timeout 900 compute-sanitizer --tool memcheck --error-exitcode 1 python -m pytest tests/test_gpu_parity.py -q -k "$SEL" \
     tests/test_gpu_group.py::test_rank_group_one_rank_per_step_launch_count > gpurun_out/sanitizer_memcheck.txt 2>&1
 echo "memcheck rc=$?"; tail -3 gpurun_out/sanitizer_memcheck.txt
+# memcheck of the text dictionary codes (slot pass, shard merge, remap); its log goes to a temporary directory
+codes_log="$(mktemp -d)/sanitizer_memcheck_text_codes.txt"
+timeout 900 compute-sanitizer --tool memcheck --error-exitcode 1 python -m pytest tests/test_gpu_text_codes.py -q \
+    > "$codes_log" 2>&1
+echo "memcheck (text codes) rc=$? log=$codes_log"; tail -3 "$codes_log"
 timeout 900 compute-sanitizer --tool racecheck --error-exitcode 1 python -m pytest tests/test_gpu_parity.py -q -k "ragged_sizes or nbins or hist_u8 or constant_column" \
     > gpurun_out/sanitizer_racecheck.txt 2>&1
 echo "racecheck rc=$?"; tail -3 gpurun_out/sanitizer_racecheck.txt
