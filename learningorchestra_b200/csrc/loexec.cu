@@ -10,6 +10,7 @@
 #include <cub/device/device_scan.cuh>
 
 #include <algorithm>
+#include <array>
 #include <atomic>
 #include <condition_variable>
 #include <cctype>
@@ -1459,21 +1460,27 @@ unsigned long long *count_groups(HostCall &c, int64_t n, size_t out_n, Launch la
     return d_out;
 }
 
-// The host half: the first min(groups, capacity) groups of count_groups' out (out_n = capacity) copied out and the call
-// finished.  More groups than capacity is refused after *ndistinct is set, so the caller can retry larger.
-int copy_groups(HostCall &c, const unsigned long long *out, int64_t capacity, void *keys_out, uint64_t *counts_out,
-                int64_t *ndistinct, lo_host_timing *timing) {
-    unsigned long long nd = 0;
-    c.to_host(&nd, out + 2 * capacity, 8);
-    c.sync();
+// The end of every call that returns at most `capacity` of the nd groups it found: the first min(nd, capacity) 8-byte
+// words of each {host output, device column} pair copied out and the call finished.  More groups than capacity is
+// refused after *ndistinct is set, so the caller can retry larger.
+int finish_groups(HostCall &c, unsigned long long nd, int64_t capacity,
+                  std::initializer_list<std::pair<void *, const void *>> outs, int64_t *ndistinct, lo_host_timing *timing) {
     const size_t take = (size_t)std::min<unsigned long long>(nd, (unsigned long long)capacity);
-    c.to_host(keys_out, out, take * 8);
-    c.to_host(counts_out, out + capacity, take * 8);
+    for (const auto &[host, dev] : outs) c.to_host(host, dev, take * 8);
     LO_TRY(c.finish(timing));
     *ndistinct = (int64_t)nd;
     if ((int64_t)nd > capacity)
         return fail(LO_ERR_INVALID, "%llu distinct keys do not fit the caller's capacity %lld", nd, (long long)capacity);
     return LO_OK;
+}
+
+// The host half: the groups of count_groups' out (out_n = capacity), their number read first.
+int copy_groups(HostCall &c, const unsigned long long *out, int64_t capacity, void *keys_out, uint64_t *counts_out,
+                int64_t *ndistinct, lo_host_timing *timing) {
+    unsigned long long nd = 0;
+    c.to_host(&nd, out + 2 * capacity, 8);
+    c.sync();
+    return finish_groups(c, nd, capacity, {{keys_out, out}, {counts_out, out + capacity}}, ndistinct, timing);
 }
 
 // The rest of a lo_value_counts_* call once its input is on the device: at most `capacity` groups, copied out.
@@ -1713,147 +1720,213 @@ int lo_value_counts_text(lo_ctx *ctx, const lo_text *t, int64_t *rep_rows_out, u
 
 namespace {
 
-// one shard of lo_value_counts_text_shards, worked on its own context's call frame and stream
-struct TextShard {
-    const lo_text *t;
-    int64_t row0;
-    int64_t cap;                             // n - nulls: at most this many groups
-    std::unique_ptr<HostCall> c;
-    unsigned long long *grp = nullptr;       // count_text_groups' out: rows [0, cap), counts [cap, 2 cap), their number [2 cap]
-    long long *key_off = nullptr;            // the packed key column of its groups: nd + 1 offsets, then the bytes
-    uint8_t *key_chars = nullptr;
-    cudaEvent_t gathered = nullptr;          // the packed pieces are ready to copy
-    unsigned long long nd = 0;
-    long long bytes = 0, group0 = 0, byte0 = 0;   // its bytes, and where its pieces start in the concatenated column
-};
-
-}  // namespace
-
-extern "C" {
-
-// Value counts of one text column cut into row-range shards, each resident on its own context (loexec.h).  Four steps,
-// each enqueued on every shard before the host waits on any, so shards on different devices run at once:
-//   1. count and compact each shard on its device (count_text_groups); the host reads its group count;
-//   2. the byte lengths of its groups' cells and their exclusive scan; the host reads its key bytes;
-//   3. k_gather_cells packs the keys, rebases their offsets into the concatenated column and makes the rows global;
-//   4. the root waits on each shard's event, copies the packed pieces over with cudaMemcpyPeerAsync, and merges them
-//      (k_hash_sum_str, k_hash_compact_str, k_take_rows).  Each shard's stream waits on the root's copies before its
-//      scratch is freed.
-int lo_value_counts_text_shards(lo_ctx *root, const lo_text *const *shards, const int64_t *row0, int32_t nshards,
-                                int64_t *rep_rows_out, uint64_t *counts_out, int64_t capacity, int64_t *ndistinct,
-                                lo_host_timing *timing) {
+// The refusals of every call on a text column cut into row-range shards, in this order: a NULL root, nshards outside
+// [1, LO_GROUP_MAX_DEVICES], NULL shards or row0, then shard by shard a NULL shard and a row0 that is negative or inside
+// the shard before.
+int check_shards(const lo_ctx *root, const lo_text *const *shards, const int64_t *row0, int32_t nshards) {
     if (!root) return fail(LO_ERR_INVALID, "root is NULL");
     static_assert(lo::kMaxPeers + 1 == LO_GROUP_MAX_DEVICES, "a group's devices: the root and its peers");
     if (nshards < 1 || nshards > LO_GROUP_MAX_DEVICES)
         return fail(LO_ERR_INVALID, "nshards = %d: 1 to %d shards", nshards, LO_GROUP_MAX_DEVICES);
     if (!shards || !row0) return fail(LO_ERR_INVALID, "shards or row0 is NULL");
-    std::vector<TextShard> sh;               // the shards with a cell to count
     for (int i = 0; i < nshards; ++i) {
         if (!shards[i]) return fail(LO_ERR_INVALID, "shards[%d] is NULL", i);
         if (row0[i] < 0) return fail(LO_ERR_INVALID, "row0[%d] = %lld is negative", i, (long long)row0[i]);
         if (i > 0 && row0[i] < row0[i - 1] + shards[i - 1]->n)
             return fail(LO_ERR_INVALID, "row0[%d] = %lld: shard %d ends at row %lld (shards are disjoint and in row order)",
                         i, (long long)row0[i], i - 1, (long long)(row0[i - 1] + shards[i - 1]->n));
-        if (shards[i]->n > shards[i]->nulls) sh.push_back(TextShard{shards[i], row0[i], shards[i]->n - shards[i]->nulls});
     }
-    LO_TRY(check_ndistinct(capacity, ndistinct));
-    if (sh.empty()) return LO_OK;
-    LO_TRY(check_groups_out(capacity, rep_rows_out, counts_out));
-    LO_TRY(check_ctx(root));
-    HostCall c(root, "value_counts_text_shards");
-    for (TextShard &s : sh) s.c = std::make_unique<HostCall>(s.t->ctx, "value_counts_text_shards", false);
-    auto ok = [&] { return c.ok() && std::all_of(sh.begin(), sh.end(), [](const TextShard &s) { return s.c->ok(); }); };
-    // step(s, its call frame) for every shard in row order, on the shard's device, until the root or a shard fails
-    auto each_shard = [&](auto step) {
-        for (TextShard &s : sh) {
+    return LO_OK;
+}
+
+// The offsets of a key column of the cells at nd rows of a text column on c's device: the exclusive scan of their byte
+// lengths, nd + 1 of them (the last is their bytes).  Two launches.
+long long *key_offsets(HostCall &c, const TextCols &t, const unsigned long long *rows, int64_t nd) {
+    long long *key_off = nullptr;
+    size_t scan_bytes = 0;
+    void *tmp = nullptr;
+    c.alloc(&key_off, (size_t)(nd + 1) * 8);
+    c.run([&] { return cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, key_off, nd + 1, c.s); });
+    c.alloc(&tmp, scan_bytes);
+    c.memset(key_off + nd, 0, 8);            // the scan's last input
+    c.launch(1, [&] { lo::k_gather_lens<<<grid_for(c.ctx, nd), 256, 0, c.s>>>(t.offsets, (const long long *)rows, nd, key_off); });
+    c.launch(1, [&] { return cub::DeviceScan::ExclusiveSum(tmp, scan_bytes, key_off, nd + 1, c.s); });
+    c.drop(tmp);
+    return key_off;
+}
+
+// A call on one text column cut into checked row-range shards, each resident on its own context, whose groups are
+// merged on root's context.  Each shard works on an untimed call frame of its own, on its context's stream; the root's
+// frame `c` times the call.  Each step is enqueued on every shard before the host waits on any, so shards on different
+// devices run at once:
+//   1. each: the caller lists every shard's groups on its device, one row of each group;
+//   2. pack_keys: the host reads each shard's group count; the byte lengths of its groups' cells and their exclusive
+//      scan; the host reads its key bytes; k_gather_cells packs the keys, rebases their offsets into the concatenated
+//      column and makes the rows global;
+//   3. send_keys: the root waits on each shard's event and copies the packed pieces over with cudaMemcpyPeerAsync;
+//   4. wait_root: once the root has read the pieces, each shard's stream waits on the root's, so a shard's scratch is
+//      freed after the root has read it;
+//   5. finish: the root's frame first, then every shard's.
+// X is the caller's own state of a shard.
+template <typename X>
+struct ShardFrame {
+    struct Shard : X {
+        const lo_text *t;
+        int64_t row0;
+        int64_t live;                                // n - nulls: at most this many groups
+        std::unique_ptr<HostCall> c;
+        unsigned long long nd = 0;                   // its groups
+        long long *key_off = nullptr;                // the packed key column of its groups: nd + 1 offsets, then the bytes
+        uint8_t *key_chars = nullptr;
+        cudaEvent_t gathered = nullptr;              // the packed pieces are ready to copy
+        long long bytes = 0, group0 = 0, byte0 = 0;  // its bytes, and where its pieces start in the concatenated column
+    };
+    lo_ctx *root;
+    HostCall c;
+    std::vector<Shard> sh;                           // the shards with a row, in row order
+    long long groups = 0, bytes = 0;                 // summed over the shards
+    cudaEvent_t root_read = nullptr;                 // wait_root's event on root's stream
+
+    // own(i): the caller's state of shards[i]
+    template <typename Own>
+    ShardFrame(lo_ctx *root_, const char *name, const lo_text *const *shards, const int64_t *row0, int32_t nshards, Own own)
+        : root(root_), c(root_, name) {
+        for (int i = 0; i < nshards; ++i)
+            if (shards[i]->n > 0)
+                sh.push_back(Shard{own(i), shards[i], row0[i], shards[i]->n - shards[i]->nulls,
+                                   std::make_unique<HostCall>(shards[i]->ctx, name, false)});
+    }
+
+    bool ok() const { return c.ok() && std::all_of(sh.begin(), sh.end(), [](const Shard &s) { return s.c->ok(); }); }
+
+    // step(s, its call frame) for every shard with a cell, in row order, on the shard's device, until the root or a
+    // shard fails
+    template <typename Step> void each(Step step) {
+        for (Shard &s : sh) {
             if (!ok()) return;
+            if (!s.live) continue;
             s.c->run([&] { return cudaSetDevice(s.t->ctx->device); });
             step(s, *s.c);
         }
-    };
-    // 1. count and compact
-    each_shard([](TextShard &s, HostCall &sc) { s.grp = count_text_groups(sc, s.t->cols, s.t->n, (size_t)s.cap); });
-    each_shard([](TextShard &s, HostCall &sc) { sc.to_host(&s.nd, s.grp + 2 * s.cap, 8); sc.sync(); });
-    each_shard([](TextShard &s, HostCall &sc) {   // 2. key lengths and their scan
-        const int64_t nd = (int64_t)s.nd;
-        size_t scan_bytes = 0;
-        void *tmp = nullptr;
-        sc.alloc(&s.key_off, (size_t)(nd + 1) * 8);
-        sc.run([&] { return cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, s.key_off, nd + 1, sc.s); });
-        sc.alloc(&tmp, scan_bytes);
-        sc.memset(s.key_off + nd, 0, 8);     // the scan's last input: key_off[nd] = the key bytes
-        sc.launch(1, [&] { lo::k_gather_lens<<<grid_for(sc.ctx, nd), 256, 0, sc.s>>>(s.t->cols.offsets, (const long long *)s.grp, nd, s.key_off); });
-        sc.launch(1, [&] { return cub::DeviceScan::ExclusiveSum(tmp, scan_bytes, s.key_off, nd + 1, sc.s); });
-        sc.drop(tmp);
-    });
-    long long groups = 0, bytes = 0;
-    each_shard([&](TextShard &s, HostCall &sc) {
-        sc.to_host(&s.bytes, s.key_off + s.nd, 8);
-        sc.sync();
-        s.group0 = groups;
-        s.byte0 = bytes;
-        groups += (long long)s.nd;
-        bytes += s.bytes;
-    });
-    if (ok() && groups >> 31)                // the merge's slot word keeps a 31-bit key index
-        c.check([&] { return fail(LO_ERR_INVALID, "the shards hold %lld groups: at most 2^31-1 can be merged", groups); });
-    each_shard([](TextShard &s, HostCall &sc) {   // 3. pack the keys
-        sc.alloc(&s.key_chars, (size_t)s.bytes);
-        sc.launch(1, [&] {
-            lo::k_gather_cells<<<grid_for(sc.ctx, (int64_t)s.nd + 1), 256, 0, sc.s>>>(s.t->cols.chars, s.t->cols.offsets,
-                (long long *)s.grp, (long long)s.nd, s.key_off, s.key_chars, s.row0, s.byte0);
+    }
+
+    // listed(s) = {the rows in s of its groups, on its device; the word there that holds their number}
+    template <typename Listed> void pack_keys(Listed listed) {
+        each([&](Shard &s, HostCall &sc) { sc.to_host(&s.nd, listed(s).second, 8); sc.sync(); });
+        each([&](Shard &s, HostCall &sc) { s.key_off = key_offsets(sc, s.t->cols, listed(s).first, (int64_t)s.nd); });
+        each([&](Shard &s, HostCall &sc) {
+            sc.to_host(&s.bytes, s.key_off + s.nd, 8);
+            sc.sync();
+            s.group0 = groups;
+            s.byte0 = bytes;
+            groups += (long long)s.nd;
+            bytes += s.bytes;
         });
-        sc.run([&] { return cudaEventCreateWithFlags(&s.gathered, cudaEventDisableTiming); });
-        sc.run([&] { return cudaEventRecord(s.gathered, sc.s); });
-    });
-    int rc = LO_OK;
-    cudaEvent_t copied = nullptr;
-    if (ok()) {                              // 4. copy the pieces to the root and merge them there
+        if (ok() && groups >> 31)            // the merge's slot word keeps a 31-bit key index, and codes are int32
+            c.check([&] { return fail(LO_ERR_INVALID, "the shards hold %lld groups: at most 2^31-1 can be merged", groups); });
+        each([&](Shard &s, HostCall &sc) {   // pack the keys
+            sc.alloc(&s.key_chars, (size_t)s.bytes);
+            sc.launch(1, [&] {
+                lo::k_gather_cells<<<grid_for(sc.ctx, (int64_t)s.nd + 1), 256, 0, sc.s>>>(s.t->cols.chars, s.t->cols.offsets,
+                    (long long *)listed(s).first, (long long)s.nd, s.key_off, s.key_chars, s.row0, s.byte0);
+            });
+            sc.run([&] { return cudaEventCreateWithFlags(&s.gathered, cudaEventDisableTiming); });
+            sc.run([&] { return cudaEventRecord(s.gathered, sc.s); });
+        });
+    }
+
+    // On root's device: chars and offsets receive the concatenated key column (offsets[groups] = bytes), and each of
+    // `cols` one 8-byte word per group, cols[j] taking words(s)[j] .. + nd of every shard s.
+    template <size_t N, typename Words>
+    void send_keys(uint8_t *&chars, long long *&offsets, std::array<unsigned long long *, N> &cols, Words words) {
         c.run([&] { return cudaSetDevice(root->device); });
-        uint8_t *chars = nullptr;
-        long long *offsets = nullptr, *rows = nullptr;
-        unsigned long long *weight = nullptr;
         c.alloc(&chars, (size_t)bytes);
         c.alloc(&offsets, (size_t)(groups + 1) * 8);
-        c.alloc(&rows, (size_t)groups * 8);
-        c.alloc(&weight, (size_t)groups * 8);
-        for (TextShard &s : sh) {
+        for (unsigned long long *&col : cols) c.alloc(&col, (size_t)groups * 8);
+        for (Shard &s : sh) {
+            if (!s.live) continue;
             const int dev = s.t->ctx->device;
             c.run([&] { return cudaStreamWaitEvent(c.s, s.gathered, 0); });
             // nd + 1 offsets: the last is the next shard's first (the same value), or offsets[groups]
             c.run([&] { return cudaMemcpyPeerAsync(offsets + s.group0, root->device, s.key_off, dev, (s.nd + 1) * 8, c.s); });
-            c.run([&] { return cudaMemcpyPeerAsync(rows + s.group0, root->device, s.grp, dev, s.nd * 8, c.s); });
-            c.run([&] { return cudaMemcpyPeerAsync(weight + s.group0, root->device, s.grp + s.cap, dev, s.nd * 8, c.s); });
+            for (size_t j = 0; j < N; ++j)
+                c.run([&] { return cudaMemcpyPeerAsync(cols[j] + s.group0, root->device, words(s)[j], dev, s.nd * 8, c.s); });
             if (s.bytes) c.run([&] { return cudaMemcpyPeerAsync(chars + s.byte0, root->device, s.key_chars, dev, s.bytes, c.s); });
         }
-        c.run([&] { return cudaEventCreateWithFlags(&copied, cudaEventDisableTiming); });
-        c.run([&] { return cudaEventRecord(copied, c.s); });
-        for (TextShard &s : sh)              // a shard's scratch is freed after the root has read it
-            if (c.ok()) s.c->run([&] { return cudaStreamWaitEvent(s.c->s, copied, 0); });
-        rc = value_counts_tail(c, groups, rep_rows_out, counts_out, capacity, ndistinct, timing,
-            [&](unsigned long long *slots_keys, unsigned long long *counts, unsigned long long slots, unsigned long long *out, size_t out_n) {
-                lo::k_hash_sum_str<<<grid_for(root, groups), 256, 0, c.s>>>(chars, offsets, weight, groups, slots_keys,
-                                                                             counts, slots - 1);
-                lo::k_hash_compact_str<<<root->sm_count * 8, 256, 0, c.s>>>(slots_keys, counts, slots, (long long *)out,
-                                                                             out + out_n, (unsigned long long)out_n,
-                                                                             out + 2 * out_n);
-                lo::k_take_rows<<<root->sm_count * 8, 256, 0, c.s>>>((long long *)out, rows, out + 2 * out_n,
-                                                                      (unsigned long long)out_n);
-            }, 3);
-    } else {
-        rc = c.finish(nullptr);              // synchronises the root: nothing of it reads a shard any more
     }
-    std::string msg = g_err;
-    for (TextShard &s : sh) {                // free every shard's scratch; the first error is the call's
-        cudaSetDevice(s.t->ctx->device);
-        const int r = s.c->finish(nullptr);
-        if (rc == LO_OK && r != LO_OK) { rc = r; msg = g_err; }
-        if (s.gathered) cudaEventDestroy(s.gathered);
+
+    // every shard's stream waits on what root's stream has enqueued so far: its reads of the pieces, and what the shards
+    // read back from it
+    void wait_root() {
+        c.run([&] { return cudaEventCreateWithFlags(&root_read, cudaEventDisableTiming); });
+        c.run([&] { return cudaEventRecord(root_read, c.s); });
+        for (Shard &s : sh)
+            if (s.live && c.ok()) s.c->run([&] { return cudaStreamWaitEvent(s.c->s, root_read, 0); });
     }
-    if (copied) cudaEventDestroy(copied);
-    cudaSetDevice(root->device);
-    g_err = msg;
-    return rc;
+
+    // After the root's frame has finished with `rc` (it has synchronised: nothing of it reads a shard any more): frees
+    // every shard's scratch.  The root's error is the call's, else the first shard's in row order; root's device is
+    // current again.
+    int finish(int rc) {
+        std::string msg = g_err;
+        for (Shard &s : sh) {
+            cudaSetDevice(s.t->ctx->device);
+            const int r = s.c->finish(nullptr);
+            if (rc == LO_OK && r != LO_OK) { rc = r; msg = g_err; }
+            if (s.gathered) cudaEventDestroy(s.gathered);
+        }
+        if (root_read) cudaEventDestroy(root_read);
+        cudaSetDevice(root->device);
+        g_err = msg;
+        return rc;
+    }
+};
+
+// lo_value_counts_text_shards' own state of a shard: count_text_groups' out, rows [0, live), counts [live, 2 live),
+// their number [2 live]
+struct CountShard {
+    unsigned long long *grp = nullptr;
+};
+
+}  // namespace
+
+extern "C" {
+
+// Value counts of one text column cut into row-range shards, each resident on its own context (loexec.h), in the steps
+// of ShardFrame: each shard counts and compacts its cells (count_text_groups) and packs its groups' keys; the root
+// copies the keys with their rows and counts over and merges them (k_hash_sum_str, k_hash_compact_str, k_take_rows).
+int lo_value_counts_text_shards(lo_ctx *root, const lo_text *const *shards, const int64_t *row0, int32_t nshards,
+                                int64_t *rep_rows_out, uint64_t *counts_out, int64_t capacity, int64_t *ndistinct,
+                                lo_host_timing *timing) {
+    LO_TRY(check_shards(root, shards, row0, nshards));
+    LO_TRY(check_ndistinct(capacity, ndistinct));
+    if (std::none_of(shards, shards + nshards, [](const lo_text *t) { return t->n > t->nulls; })) return LO_OK;
+    LO_TRY(check_groups_out(capacity, rep_rows_out, counts_out));
+    LO_TRY(check_ctx(root));
+    ShardFrame<CountShard> f(root, "value_counts_text_shards", shards, row0, nshards, [](int) { return CountShard{}; });
+    f.each([](auto &s, HostCall &sc) { s.grp = count_text_groups(sc, s.t->cols, s.t->n, (size_t)s.live); });
+    f.pack_keys([](auto &s) { return std::pair(s.grp, s.grp + 2 * s.live); });
+    if (!f.ok()) return f.finish(f.c.finish(nullptr));
+    HostCall &c = f.c;
+    const long long groups = f.groups;
+    uint8_t *chars = nullptr;
+    long long *offsets = nullptr;
+    std::array<unsigned long long *, 2> cols{};     // the groups' global rows and their counts
+    f.send_keys(chars, offsets, cols, [](auto &s) { return std::array{s.grp, s.grp + s.live}; });
+    f.wait_root();
+    const long long *rows = (const long long *)cols[0];
+    const unsigned long long *weight = cols[1];
+    const int rc = value_counts_tail(c, groups, rep_rows_out, counts_out, capacity, ndistinct, timing,
+        [&](unsigned long long *slots_keys, unsigned long long *counts, unsigned long long slots, unsigned long long *out, size_t out_n) {
+            lo::k_hash_sum_str<<<grid_for(root, groups), 256, 0, c.s>>>(chars, offsets, weight, groups, slots_keys,
+                                                                         counts, slots - 1);
+            lo::k_hash_compact_str<<<root->sm_count * 8, 256, 0, c.s>>>(slots_keys, counts, slots, (long long *)out,
+                                                                         out + out_n, (unsigned long long)out_n,
+                                                                         out + 2 * out_n);
+            lo::k_take_rows<<<root->sm_count * 8, 256, 0, c.s>>>((long long *)out, rows, out + 2 * out_n,
+                                                                  (unsigned long long)out_n);
+        }, 3);
+    return f.finish(rc);
 }
 
 }  // extern "C"
@@ -1943,34 +2016,12 @@ void order_groups(HostCall &c, const unsigned long long *first, const unsigned *
     c.drop(sorted_slot);
 }
 
-// The end of a codes call: the first min(nd, capacity) first rows copied out and the call finished.  More groups than
-// capacity is refused after *ndistinct is set, as copy_groups does; the codes are written all the same.
-int copy_first_rows(HostCall &c, const unsigned long long *sorted_first, unsigned long long nd, int64_t capacity,
-                    int64_t *first_rows_out, int64_t *ndistinct, lo_host_timing *timing) {
-    const size_t take = (size_t)std::min<unsigned long long>(nd, (unsigned long long)capacity);
-    c.to_host(first_rows_out, sorted_first, take * 8);
-    LO_TRY(c.finish(timing));
-    *ndistinct = (int64_t)nd;
-    if ((int64_t)nd > capacity)
-        return fail(LO_ERR_INVALID, "%llu distinct cells do not fit the caller's capacity %lld", nd, (long long)capacity);
-    return LO_OK;
-}
-
-// one shard of lo_text_codes_shards, worked on its own context's call frame and stream
+// lo_text_codes_shards' own state of a shard
 struct CodesShard {
-    const lo_text *t;
-    int *codes;
-    int64_t row0;
-    int64_t live;                            // n - nulls: at most this many groups
-    std::unique_ptr<HostCall> c;
+    int *codes;                              // its column of out[i]
     CodesTable T;
-    long long *key_off = nullptr;            // the packed key column of its groups: nd + 1 offsets, then the bytes
-    uint8_t *key_chars = nullptr;
     int *key_code = nullptr;                 // the global codes of its groups, copied back from the root
-    cudaEvent_t gathered = nullptr;          // the packed pieces are ready to copy
     cudaEvent_t taken = nullptr;             // the shard has copied its codes from the root
-    unsigned long long nd = 0;
-    long long bytes = 0, group0 = 0, byte0 = 0;   // its bytes, and where its pieces start in the concatenated column
 };
 
 }  // namespace
@@ -2006,120 +2057,52 @@ int lo_text_codes(lo_ctx *ctx, const lo_text *t, lo_table *out, int32_t col, int
         lo::k_remap_codes<<<grid_for(ctx, t->n), 256, 0, c.s>>>(codes, t->n, t->cols.mask, t->cols.bitmap, t->cols.bit0, T.first);
     });
     c.mark();
-    return copy_first_rows(c, sorted, nd, capacity, first_rows_out, ndistinct, timing);
+    return finish_groups(c, nd, capacity, {{first_rows_out, sorted}}, ndistinct, timing);   // codes written all the same
 }
 
-// Codes of one text column cut into row-range shards, each resident on its own context (loexec.h).  Each step is
-// enqueued on every shard before the host waits on any, so shards on different devices run at once:
-//   1. each shard's table, slot pass and compaction (codes_slots); the host reads its group count;
-//   2. the byte lengths of its groups' cells (at their first rows) and their exclusive scan; the host reads its key bytes;
-//   3. k_gather_cells packs the keys and turns the first rows global: they are the keys' weights;
-//   4. the root copies the packed pieces over with cudaMemcpyPeerAsync, merges them with k_hash_min_str (each group's
-//      lowest global first row, each key's slot), compacts and orders the groups, and remaps its key slots to codes;
-//   5. each shard copies its keys' codes back, writes them to its own slots (k_rank_slots) and remaps its rows.
-// The root's scratch is freed after every shard has taken its codes; a shard's after the root's step 4, which it waits on.
+// Codes of one text column cut into row-range shards, each resident on its own context (loexec.h), in the steps of
+// ShardFrame, the keys' first rows made global being their weights:
+//   1. each shard's table, slot pass and compaction (codes_slots); each shard packs its groups' keys;
+//   2. the root copies the keys with their first rows over, merges them with k_hash_min_str (each group's lowest
+//      global first row, each key's slot), compacts and orders the groups, and remaps its key slots to codes;
+//   3. each shard copies its keys' codes back, writes them to its own slots (k_rank_slots) and remaps its rows.
+// The root's scratch is freed after every shard has taken its codes; a shard's after the root's step 2.
 int lo_text_codes_shards(lo_ctx *root, const lo_text *const *shards, const int64_t *row0, int32_t nshards,
                          lo_table *const *out, int32_t col, int64_t *first_rows_out, int64_t capacity, int64_t *ndistinct,
                          lo_host_timing *timing) {
-    if (!root) return fail(LO_ERR_INVALID, "root is NULL");
-    if (nshards < 1 || nshards > LO_GROUP_MAX_DEVICES)
-        return fail(LO_ERR_INVALID, "nshards = %d: 1 to %d shards", nshards, LO_GROUP_MAX_DEVICES);
-    if (!shards || !row0 || !out) return fail(LO_ERR_INVALID, "shards, row0 or out is NULL");
-    std::vector<CodesShard> sh;              // the shards with a row
+    LO_TRY(check_shards(root, shards, row0, nshards));
+    if (!out) return fail(LO_ERR_INVALID, "out is NULL");
     for (int i = 0; i < nshards; ++i) {
-        if (!shards[i]) return fail(LO_ERR_INVALID, "shards[%d] is NULL", i);
-        if (row0[i] < 0) return fail(LO_ERR_INVALID, "row0[%d] = %lld is negative", i, (long long)row0[i]);
-        if (i > 0 && row0[i] < row0[i - 1] + shards[i - 1]->n)
-            return fail(LO_ERR_INVALID, "row0[%d] = %lld: shard %d ends at row %lld (shards are disjoint and in row order)",
-                        i, (long long)row0[i], i - 1, (long long)(row0[i - 1] + shards[i - 1]->n));
         char name[16];
         snprintf(name, sizeof name, "out[%d]", i);
         LO_TRY(check_codes_out(shards[i], out[i], col, name));
-        if (shards[i]->n > 0)
-            sh.push_back(CodesShard{shards[i], codes_col(out[i], col), row0[i], shards[i]->n - shards[i]->nulls});
     }
     LO_TRY(check_ndistinct(capacity, ndistinct));
     if (capacity > 0 && !first_rows_out) return fail(LO_ERR_INVALID, "NULL argument: first_rows_out with capacity > 0");
     LO_TRY(check_ctx(root));
-    HostCall c(root, "text_codes_shards");
-    for (CodesShard &s : sh) s.c = std::make_unique<HostCall>(s.t->ctx, "text_codes_shards", false);
-    auto ok = [&] { return c.ok() && std::all_of(sh.begin(), sh.end(), [](const CodesShard &s) { return s.c->ok(); }); };
-    // step(s, its call frame) for every shard with a cell to number, in row order, on the shard's device, until the
-    // root or a shard fails
-    auto each_shard = [&](auto step) {
-        for (CodesShard &s : sh) {
-            if (!ok()) return;
-            if (!s.live) continue;
-            s.c->run([&] { return cudaSetDevice(s.t->ctx->device); });
-            step(s, *s.c);
-        }
-    };
-    for (CodesShard &s : sh)                 // a shard without a cell: every row is -1, no launch
-        if (!s.live && ok()) {
+    ShardFrame<CodesShard> f(root, "text_codes_shards", shards, row0, nshards,
+                             [&](int i) { return CodesShard{codes_col(out[i], col)}; });
+    for (auto &s : f.sh)                     // a shard without a cell: every row is -1, no launch
+        if (!s.live && f.ok()) {
             s.c->run([&] { return cudaSetDevice(s.t->ctx->device); });
             s.c->memset(s.codes, 0xFF, (size_t)s.t->n * 4);
         }
-    // 1. table, slot pass, compaction
-    each_shard([](CodesShard &s, HostCall &sc) { codes_slots(sc, s.t->cols, s.t->n, s.live, s.codes, s.T); });
-    each_shard([](CodesShard &s, HostCall &sc) { sc.to_host(&s.nd, s.T.grp_first + s.live, 8); sc.sync(); });
-    each_shard([](CodesShard &s, HostCall &sc) {  // 2. key lengths and their scan
-        const int64_t nd = (int64_t)s.nd;
-        size_t scan_bytes = 0;
-        void *tmp = nullptr;
-        sc.alloc(&s.key_off, (size_t)(nd + 1) * 8);
-        sc.run([&] { return cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, s.key_off, nd + 1, sc.s); });
-        sc.alloc(&tmp, scan_bytes);
-        sc.memset(s.key_off + nd, 0, 8);     // the scan's last input: key_off[nd] = the key bytes
-        sc.launch(1, [&] {
-            lo::k_gather_lens<<<grid_for(sc.ctx, nd), 256, 0, sc.s>>>(s.t->cols.offsets, (const long long *)s.T.grp_first, nd,
-                                                                        s.key_off);
-        });
-        sc.launch(1, [&] { return cub::DeviceScan::ExclusiveSum(tmp, scan_bytes, s.key_off, nd + 1, sc.s); });
-        sc.drop(tmp);
-    });
-    long long groups = 0, bytes = 0;
+    f.each([](auto &s, HostCall &sc) { codes_slots(sc, s.t->cols, s.t->n, s.live, s.codes, s.T); });
+    f.pack_keys([](auto &s) { return std::pair(s.T.grp_first, s.T.grp_first + s.live); });
+    HostCall &c = f.c;
+    const long long groups = f.groups;
     int64_t max_row = 0;
-    each_shard([&](CodesShard &s, HostCall &sc) {
-        sc.to_host(&s.bytes, s.key_off + s.nd, 8);
-        sc.sync();
-        s.group0 = groups;
-        s.byte0 = bytes;
-        groups += (long long)s.nd;
-        bytes += s.bytes;
-        max_row = s.row0 + s.t->n - 1;
-    });
-    if (ok() && groups >> 31)                // the merge's slot word keeps a 31-bit key index, and codes are int32
-        c.check([&] { return fail(LO_ERR_INVALID, "the shards hold %lld distinct cells: at most 2^31-1 can be numbered", groups); });
-    each_shard([](CodesShard &s, HostCall &sc) {  // 3. pack the keys; their first rows become global
-        sc.alloc(&s.key_chars, (size_t)s.bytes);
-        sc.launch(1, [&] {
-            lo::k_gather_cells<<<grid_for(sc.ctx, (int64_t)s.nd + 1), 256, 0, sc.s>>>(s.t->cols.chars, s.t->cols.offsets,
-                (long long *)s.T.grp_first, (long long)s.nd, s.key_off, s.key_chars, s.row0, s.byte0);
-        });
-        sc.run([&] { return cudaEventCreateWithFlags(&s.gathered, cudaEventDisableTiming); });
-        sc.run([&] { return cudaEventRecord(s.gathered, sc.s); });
-    });
+    for (const auto &s : f.sh)
+        if (s.live) max_row = s.row0 + s.t->n - 1;
     unsigned long long nd = 0, *sorted = nullptr;
-    cudaEvent_t remapped = nullptr;
-    if (ok() && groups > 0) {                // 4. copy the pieces to the root, merge and order them there
-        c.run([&] { return cudaSetDevice(root->device); });
+    if (f.ok() && groups > 0) {              // 2. merge and order the keys on the root
         uint8_t *chars = nullptr;
         long long *offsets = nullptr;
-        unsigned long long *weight = nullptr;
+        std::array<unsigned long long *, 1> cols{};     // the keys' global first rows
+        f.send_keys(chars, offsets, cols, [](auto &s) { return std::array{s.T.grp_first}; });
+        const unsigned long long *weight = cols[0];
         unsigned *key_slot = nullptr;
-        c.alloc(&chars, (size_t)bytes);
-        c.alloc(&offsets, (size_t)(groups + 1) * 8);
-        c.alloc(&weight, (size_t)groups * 8);
         c.alloc(&key_slot, (size_t)groups * 4);
-        for (CodesShard &s : sh) {
-            if (!s.live) continue;
-            const int dev = s.t->ctx->device;
-            c.run([&] { return cudaStreamWaitEvent(c.s, s.gathered, 0); });
-            // nd + 1 offsets: the last is the next shard's first (the same value), or offsets[groups]
-            c.run([&] { return cudaMemcpyPeerAsync(offsets + s.group0, root->device, s.key_off, dev, (s.nd + 1) * 8, c.s); });
-            c.run([&] { return cudaMemcpyPeerAsync(weight + s.group0, root->device, s.T.grp_first, dev, s.nd * 8, c.s); });
-            if (s.bytes) c.run([&] { return cudaMemcpyPeerAsync(chars + s.byte0, root->device, s.key_chars, dev, s.bytes, c.s); });
-        }
         CodesTable R;
         R.nslots = slots_for(groups);
         c.alloc(&R.keys, R.nslots * 8);
@@ -2148,11 +2131,9 @@ int lo_text_codes_shards(lo_ctx *root, const lo_text *const *shards, const int64
             lo::k_remap_codes<<<grid_for(root, groups), 256, 0, c.s>>>((int *)key_slot, groups, nullptr, nullptr, 0, R.first);
         });
         c.mark();
-        c.run([&] { return cudaEventCreateWithFlags(&remapped, cudaEventDisableTiming); });
-        c.run([&] { return cudaEventRecord(remapped, c.s); });
-        each_shard([&](CodesShard &s, HostCall &sc) {   // 5. each shard's codes back, onto its slots and rows
+        f.wait_root();
+        f.each([&](auto &s, HostCall &sc) {  // 3. each shard's codes back, onto its slots and rows
             const int64_t snd = (int64_t)s.nd;
-            sc.run([&] { return cudaStreamWaitEvent(sc.s, remapped, 0); });
             sc.alloc(&s.key_code, (size_t)snd * 4);
             sc.run([&] {
                 return cudaMemcpyPeerAsync(s.key_code, s.t->ctx->device, key_slot + s.group0, root->device, (size_t)snd * 4, sc.s);
@@ -2166,22 +2147,13 @@ int lo_text_codes_shards(lo_ctx *root, const lo_text *const *shards, const int64
             });
         });
         c.run([&] { return cudaSetDevice(root->device); });
-        for (CodesShard &s : sh)             // the root's scratch is freed after every shard has read its codes
+        for (auto &s : f.sh)                 // the root's scratch is freed after every shard has read its codes
             if (s.taken) c.run([&] { return cudaStreamWaitEvent(c.s, s.taken, 0); });
     }
-    int rc = ok() ? copy_first_rows(c, sorted, nd, capacity, first_rows_out, ndistinct, timing)
-                  : c.finish(nullptr);       // synchronises the root: nothing of it reads a shard any more
-    std::string msg = g_err;
-    for (CodesShard &s : sh) {               // free every shard's scratch; the first error is the call's
-        cudaSetDevice(s.t->ctx->device);
-        const int r = s.c->finish(nullptr);
-        if (rc == LO_OK && r != LO_OK) { rc = r; msg = g_err; }
-        if (s.gathered) cudaEventDestroy(s.gathered);
+    const int rc = f.finish(f.ok() ? finish_groups(c, nd, capacity, {{first_rows_out, sorted}}, ndistinct, timing)
+                                   : c.finish(nullptr));
+    for (auto &s : f.sh)
         if (s.taken) cudaEventDestroy(s.taken);
-    }
-    if (remapped) cudaEventDestroy(remapped);
-    cudaSetDevice(root->device);
-    g_err = msg;
     return rc;
 }
 

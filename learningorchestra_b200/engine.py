@@ -99,44 +99,36 @@ def _minmax_decode(lib, raw: np.ndarray, k: int):
     return mins, maxs, cnt
 
 
-def _value_counts(call, n: int, key_dtype, timing: dict | None = None):
-    """(keys, counts) of a lo_value_counts_* call ``call(keys_out, counts_out, capacity, ndistinct_ref, timing_ref)``:
-    room for min(n, 65536) groups first, called again with room for every group when they did not fit.  ``timing``: a
-    dict to receive the last call's lo_host_timing fields; None passes no lo_host_timing."""
+def _groups(call, n: int, dtypes, timing: dict | None = None) -> tuple:
+    """The outputs of a call that returns at most ``capacity`` of the groups of ``n`` cells, ``call(*outs, capacity,
+    ndistinct_ref, timing_ref)`` with one output array per dtype of ``dtypes``: room for min(n, 65536) groups first,
+    called again with room for every group when they did not fit.  ``timing``: a dict to receive the last call's
+    lo_host_timing fields; None passes no lo_host_timing."""
     t = N.HostTiming() if timing is not None else None
     cap = max(min(n, 1 << 16), 1)
     while True:
-        keys = np.empty(cap, dtype=key_dtype)
-        counts = np.empty(cap, dtype=np.uint64)
+        outs = [np.empty(cap, dtype=d) for d in dtypes]
         nd = C.c_int64()
-        rc = call(keys.ctypes.data_as(C.c_void_p), counts.ctypes.data_as(C.c_void_p), cap, C.byref(nd),
-                  C.byref(t) if t is not None else None)
+        rc = call(*[o.ctypes.data_as(C.c_void_p) for o in outs], cap, C.byref(nd), C.byref(t) if t is not None else None)
         if rc == N.LO_ERR_INVALID and nd.value > cap:
             cap = int(nd.value)
             continue
         N.check(rc)
         if t is not None:
             timing.update(_timing(t), kernel_ms=t.kernel_ms)
-        return keys[:nd.value], counts[:nd.value]
+        return tuple(o[:nd.value] for o in outs)
+
+
+def _value_counts(call, n: int, key_dtype, timing: dict | None = None):
+    """(keys, counts) of a lo_value_counts_* call ``call(keys_out, counts_out, capacity, ndistinct_ref, timing_ref)``
+    (:func:`_groups`)."""
+    return _groups(call, n, (key_dtype, np.uint64), timing)
 
 
 def _first_rows(call, n: int, timing: dict | None = None) -> np.ndarray:
     """The first rows (int64[ndistinct], ascending) of a lo_text_codes* call ``call(first_rows_out, capacity,
-    ndistinct_ref, timing_ref)`` on a column of ``n`` non-null cells: room for min(n, 65536) first rows, called again with
-    room for every one when they did not fit (as :func:`_value_counts`)."""
-    t = N.HostTiming() if timing is not None else None
-    cap = max(min(n, 1 << 16), 1)
-    while True:
-        rows = np.empty(cap, dtype=np.int64)
-        nd = C.c_int64()
-        rc = call(rows.ctypes.data_as(C.c_void_p), cap, C.byref(nd), C.byref(t) if t is not None else None)
-        if rc == N.LO_ERR_INVALID and nd.value > cap:
-            cap = int(nd.value)
-            continue
-        N.check(rc)
-        if t is not None:
-            timing.update(_timing(t), kernel_ms=t.kernel_ms)
-        return rows[:nd.value]
+    ndistinct_ref, timing_ref)`` on a column of ``n`` non-null cells (:func:`_groups`)."""
+    return _groups(call, n, (np.int64,), timing)[0]
 
 
 def text_dictionary(arr, first_rows):

@@ -214,6 +214,18 @@ class ShardedText:
                           **{k: sum(t[k] for t in times) for k in ("h2d_bytes", "d2h_bytes", "launches")})
         return cls(parts, [b for b, _ in bounds], arr)
 
+    def args(self):
+        """The ``shards`` and ``row0`` arguments of a ``lo_*_shards`` call on this column (ctypes arrays)."""
+        if any(p._h is None for p in self.pieces):
+            raise ValueError("the text column has been freed")
+        k = len(self.pieces)
+        return (C.c_void_p * k)(*[p._h for p in self.pieces]), (C.c_int64 * k)(*self.offsets)
+
+    def check_cut(self, table) -> None:
+        """Refuses a :class:`ShardedTable` whose shards do not hold the same rows as this column's pieces."""
+        if self.offsets != table.offsets or [p.n for p in self.pieces] != [t.nrows for t in table.shards]:
+            raise ValueError("the text column and the table are not cut at the same rows")
+
     def free(self) -> None:
         for p in self.pieces:
             p.free()
@@ -521,8 +533,7 @@ class ShardedEngine:
         (both cut at :meth:`bounds`), so every member parses its piece into its shard on its own device, from a host
         thread of its own, and nothing crosses devices.  The summary's rows are global."""
         self._every_row("parse_text_into")
-        if text.offsets != table.offsets or [p.n for p in text.pieces] != [t.nrows for t in table.shards]:
-            raise ValueError("the text column and the table are not cut at the same rows")
+        text.check_cut(table)
         return combine_parse_summaries(on_each(self.nlocal, lambda i: self.engines[i].parse_text_into(
             table.shards[i], col, text.pieces[i])), table.offsets)
 
@@ -566,9 +577,7 @@ class ShardedEngine:
         """``Engine.value_counts_column`` over a sharded table: every local shard is counted on its own device from a
         host thread of its own, and the groups are merged on the host (:func:`merge_value_counts`).  A rank group's
         process holds only its own rows, so it refuses rather than return a partial count."""
-        if self.world > self.nlocal:
-            raise self._N.LoexecError(self._N.LO_ERR_INVALID, f"value_counts_column needs every row: this process holds "
-                                      f"{self.nlocal} of the group's {self.world} shards")
+        self._every_row("value_counts_column")
         return merge_value_counts(on_each(self.nlocal, lambda i: self.engines[i].value_counts_column(table.shards[i], col)))
 
     # ---- host buffers -------------------------------------------------------------------------------------
@@ -662,16 +671,12 @@ class ShardedEngine:
             return self.engines[0].value_counts_text(text, timing)
         import numpy as np
         from .engine import _value_counts
-        if any(p._h is None for p in text.pieces):
-            raise ValueError("the text column has been freed")
+        shards, row0 = text.args()
         n = text.n - text.nulls
         if n == 0:
             return np.zeros(0, np.int64), np.zeros(0, np.uint64)
-        k = len(text.pieces)
-        handles = (C.c_void_p * k)(*[p._h for p in text.pieces])
-        row0 = (C.c_int64 * k)(*text.offsets)
         return _value_counts(lambda rows, counts, cap, nd, t: self._lib.lo_value_counts_text_shards(
-            self.engines[0]._ctx, handles, row0, k, rows, counts, cap, nd, t), n, np.int64, timing)
+            self.engines[0]._ctx, shards, row0, len(shards), rows, counts, cap, nd, t), n, np.int64, timing)
 
     def text_codes(self, text: ShardedText, table: ShardedTable, col: int, timing=None):
         """``Engine.text_codes`` of a :class:`ShardedText` into int32 column ``col`` of ``table`` (``lo_text_codes_shards``),
@@ -682,15 +687,10 @@ class ShardedEngine:
         self._every_row("text_codes")
         if not isinstance(text, ShardedText):
             raise TypeError("text_codes takes a ShardedText (ShardedEngine.text)")
-        if text.offsets != table.offsets or [p.n for p in text.pieces] != [t.nrows for t in table.shards]:
-            raise ValueError("the text column and the table are not cut at the same rows")
-        if any(p._h is None for p in text.pieces):
-            raise ValueError("the text column has been freed")
-        k = len(text.pieces)
-        handles = (C.c_void_p * k)(*[p._h for p in text.pieces])
-        row0 = (C.c_int64 * k)(*text.offsets)
+        text.check_cut(table)
+        shards, row0 = text.args()
         return _first_rows(lambda rows, cap, nd, t: self._lib.lo_text_codes_shards(
-            self.engines[0]._ctx, handles, row0, k, self._tables(table), int(col), rows, cap, nd, t),
+            self.engines[0]._ctx, shards, row0, len(shards), self._tables(table), int(col), rows, cap, nd, t),
             text.n - text.nulls, timing)
 
     @property
