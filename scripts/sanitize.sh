@@ -11,6 +11,12 @@ codes_log="$(mktemp -d)/sanitizer_memcheck_text_codes.txt"
 timeout 900 compute-sanitizer --tool memcheck --error-exitcode 1 python -m pytest tests/test_gpu_text_codes.py -q \
     > "$codes_log" 2>&1
 echo "memcheck (text codes) rc=$? log=$codes_log"; tail -3 "$codes_log"
+# memcheck of the number parser and the resident formatter on every entry point, without the million-row cases: a read
+# past the last staged cell shows here (the CPU harness puts a NUL after it)
+parse_log="$(mktemp -d)/sanitizer_memcheck_parse.txt"
+timeout 900 compute-sanitizer --tool memcheck --error-exitcode 1 python -m pytest tests/test_gpu_parse.py -q -k "not million" \
+    > "$parse_log" 2>&1
+echo "memcheck (parse) rc=$? log=$parse_log"; tail -3 "$parse_log"
 timeout 900 compute-sanitizer --tool racecheck --error-exitcode 1 python -m pytest tests/test_gpu_parity.py -q -k "ragged_sizes or nbins or hist_u8 or constant_column" \
     > gpurun_out/sanitizer_racecheck.txt 2>&1
 echo "racecheck rc=$?"; tail -3 gpurun_out/sanitizer_racecheck.txt

@@ -66,7 +66,10 @@ def check(parse, strings):
                 assert int(b) == eb, (s, hex(int(b)), hex(eb))
 
 
-def test_grammar_and_reference_cast_vectors(parse):
+# ---- the corpus: one builder per family of cells, shared with the device tests (test_gpu_parse.py) ----------------
+def grammar_cases():
+    """The reference's cast vectors and the grammar's cases: signs, points, exponents, whitespace, underscores,
+    inf / nan spellings, zeros, round-trip and overflow / underflow edges, and a few non-ASCII cells."""
     import json
     vec = json.loads((ROOT / "tests" / "golden" / "reference_cast_vectors.json").read_text())
     cases = [s for s in vec["in"] if s is not None]
@@ -82,20 +85,12 @@ def test_grammar_and_reference_cast_vectors(parse):
               "0.1", "0.2", "0.3", "0.30000000000000004", "123456789012345678", "1234567890123456789", "12345678901234567890",
               "123456789012345678901234567890", "0.000000000000000000000000000001", "1" + "0" * 400, "0." + "0" * 400 + "1",
               "1e99999999999999999999", "1e-99999999999999999999", "１２", "٣", "1 ", "é"]
-    from learningorchestra_b200.columnar import ascii_number_text
-    bits, st = parse(cases)
-    for s, b, t in zip(cases, bits, st):
-        assert t == UNSUPPORTED if any(ord(ch) >= 0x80 for ch in s) else t != UNSUPPORTED, s   # raw UTF-8 is reported, not guessed
-    # ... and through the packer's normalisation (what float(str) does first) every case is decided as CPython decides it
-    bits, st = parse([ascii_number_text(c) for c in cases])
-    for s, b, t in zip(cases, bits, st):
-        es, eb = expected(s)
-        assert t == es, (repr(s), int(t), es)
-        if es in (FLOAT, INTEGER) and not math.isnan(struct.unpack("<d", struct.pack("<Q", eb))[0]):
-            assert int(b) == eb, (s, hex(int(b)), hex(eb))
+    return cases
 
 
-def test_random_short_decimals(parse):
+def random_short_decimals():
+    """300 000 cells of at most 19 significant digits: repr of random doubles, integers with exponents, fixed-point
+    decimals, digit strings with a point anywhere, and small mantissas at the ends of the exponent range."""
     rng = random.Random(20260921)
     cases = []
     for _ in range(300_000):
@@ -116,12 +111,13 @@ def test_random_short_decimals(parse):
         else:
             s = f"{rng.randint(1, 999)}e{rng.randint(-345, 310)}"
         cases.append(s)
-    check(parse, cases)
+    return cases
 
 
-def test_halfway_and_long_digit_strings(parse):
+def halfway_and_long_digits():
     """> 19 significant digits: exact midpoints between adjacent doubles (ties-to-even), and midpoints nudged by
-    one unit hundreds of digits further right (must go up / down) — the big-integer slow path."""
+    one unit hundreds of digits further right (must go up / down) — the big-integer slow path — then 20 000 random
+    strings of 20 to 60 digits."""
     rng = random.Random(7)
     cases = []
     for _ in range(3000):
@@ -152,18 +148,52 @@ def test_halfway_and_long_digit_strings(parse):
         digits = "".join(rng.choice("0123456789") for _ in range(d))
         pos = rng.randint(0, d)
         cases.append(digits[:pos] + "." + digits[pos:] + rng.choice(["", f"e{rng.randint(-340, 300)}"]))
-    check(parse, cases)
+    return cases
+
+
+def long_cells():
+    """Cells of thousands of bytes: digits past the 800th only matter as a sticky bit."""
+    return ["1" * 1025, "0" * 5000 + "7", "1" * 400 + "." + "9" * 3000, "0." + "0" * 2000 + "123", "9" * 309, "9" * 308 + "." + "5" * 2000,
+            "2.4703282292062327208051355972538996e-324" + "0" * 1500 + "1", " " * 1500 + "1e5" + "\t" * 900,
+            "1" + "_0" * 700, "4.9e-324" + "0" * 2000, "1" + "0" * 1100 + "e-1100", "0" * 3000, "." + "0" * 3000 + "e5"]
+
+
+def unicode_cells():
+    """Unicode decimal digits and whitespace, which float(str) maps to ASCII first, and characters it refuses."""
+    return ["１２", "٣.٥", "\u2003 5\u00a0", "１_０", "-１e２", "é1", "1é", "１٣.５e-１", "\u30001\u3000", "१२३", "1\u00b2", "½", "\x1c5", "5\x85"]
+
+
+def test_grammar_and_reference_cast_vectors(parse):
+    cases = grammar_cases()
+    from learningorchestra_b200.columnar import ascii_number_text
+    bits, st = parse(cases)
+    for s, b, t in zip(cases, bits, st):
+        assert t == UNSUPPORTED if any(ord(ch) >= 0x80 for ch in s) else t != UNSUPPORTED, s   # raw UTF-8 is reported, not guessed
+    # ... and through the packer's normalisation (what float(str) does first) every case is decided as CPython decides it
+    bits, st = parse([ascii_number_text(c) for c in cases])
+    for s, b, t in zip(cases, bits, st):
+        es, eb = expected(s)
+        assert t == es, (repr(s), int(t), es)
+        if es in (FLOAT, INTEGER) and not math.isnan(struct.unpack("<d", struct.pack("<Q", eb))[0]):
+            assert int(b) == eb, (s, hex(int(b)), hex(eb))
+
+
+def test_random_short_decimals(parse):
+    check(parse, random_short_decimals())
+
+
+def test_halfway_and_long_digit_strings(parse):
+    """> 19 significant digits: exact midpoints between adjacent doubles (ties-to-even), and midpoints nudged by
+    one unit hundreds of digits further right (must go up / down) — the big-integer slow path."""
+    check(parse, halfway_and_long_digits())
 
 
 def test_long_cells_and_unicode_text(parse):
     """No length limit short of 1 MiB: digits past the 800th only matter as a sticky bit.  Unicode decimal digits and
     whitespace go through the packer's float(str) normalisation."""
     from learningorchestra_b200.columnar import ascii_number_text
-    long_cases = ["1" * 1025, "0" * 5000 + "7", "1" * 400 + "." + "9" * 3000, "0." + "0" * 2000 + "123", "9" * 309, "9" * 308 + "." + "5" * 2000,
-                  "2.4703282292062327208051355972538996e-324" + "0" * 1500 + "1", " " * 1500 + "1e5" + "\t" * 900,
-                  "1" + "_0" * 700, "4.9e-324" + "0" * 2000, "1" + "0" * 1100 + "e-1100", "0" * 3000, "." + "0" * 3000 + "e5"]
-    check(parse, long_cases)
-    uni = ["１２", "٣.٥", "\u2003 5\u00a0", "１_０", "-１e２", "é1", "1é", "１٣.５e-１", "\u30001\u3000", "१२३", "1\u00b2", "½", "\x1c5", "5\x85"]
+    check(parse, long_cells())
+    uni = unicode_cells()
     bits, st = parse([ascii_number_text(c) for c in uni])
     for s, b, t in zip(uni, bits, st):
         es, eb = expected(s)
