@@ -58,7 +58,7 @@ extern "C" {
 #define LO_F32 2   /* IEEE binary32 */
 #define LO_U8  3   /* unsigned byte */
 #define LO_U32 4   /* dictionary codes (host entry points only) */
-#define LO_I32 5   /* dictionary codes of a text column (lo_text_codes): tables only, no compute entry reads them */
+#define LO_I32 5   /* dictionary codes of a text column (lo_text_codes): read by lo_assemble_rows only, refused elsewhere */
 
 /* synthetic generators (oracle/bsem.c and oracle/bsem_numpy.py hold the bit-identical CPU twins) */
 #define LO_SYNTH_UNIFORM   0  /* f64: lo + (hi-lo) * (splitmix64(...)>>11) * 2^-53            */
@@ -432,6 +432,40 @@ int lo_text_codes(lo_ctx *ctx, const lo_text *t, lo_table *out, int32_t col, int
 int lo_text_codes_shards(lo_ctx *root, const lo_text *const *shards, const int64_t *row0, int32_t nshards,
                          lo_table *const *out, int32_t col, int64_t *first_rows_out, int64_t capacity,
                          int64_t *ndistinct, lo_host_timing *timing);
+
+/* The feature matrix of a model's training step: Spark 2.4's VectorAssembler(inputCols, outputCol="features") plus its
+ * "label" column (builder_image/builder.py:99-134), from k source columns in HBM into one row-major matrix, on the GPU.
+ * Source j is column src_col[j] of src[j], an LO_F64 slab (NaN is invalid: a null or a real NaN) or an LO_I32 column of
+ * dictionary codes (lo_text_codes; -1 is invalid).  The tables may differ; all live on ctx's device with the same nrows
+ * n.  Row i of x (x's column 0, row stride ld >= k elements) is [value(j, i) for j < k]; y[i] (optional, with label /
+ * label_col: one more source) is the label's value.  x and y are both LO_F32 (fp64->fp32 RNE, NaN -> 0x7fc00000, codes
+ * int->fp32 RNE) or both LO_F64 (exact).  An invalid cell, by mode:
+ *   LO_INVALID_ERROR — the call fails with LO_ERR_INVALID; info->bad_row / bad_col name the lowest invalid row and its
+ *                      lowest invalid source in that row (k: the label); x and y hold nothing to read;
+ *   LO_INVALID_SKIP  — rows with an invalid cell in any source or the label are left out; the kept rows stay in order;
+ *   LO_INVALID_KEEP  — written as NaN of the output dtype (a -1 code too; an f64 NaN keeps its bits in LO_F64).
+ * info->nkept = the rows written to x and y; kept_rows (host int64[n] or NULL) receives their source rows in output order.
+ * x must hold n * ld elements in column 0, y n (the rows skip leaves out stay unwritten).
+ * Refused with LO_ERR_INVALID before anything is enqueued: NULL src, src_col, x or info; k outside [1, 2097120]; ld < k; a
+ * NULL source, a source that is not LO_F64 / LO_I32, on another device, with src_col outside [0, ncols) or rows other
+ * than src[0]'s (the label likewise); an unknown mode; x not LO_F32 / LO_F64 or on another device or too small; y
+ * without a label or a label without y; y of another dtype than x, on another device or too small.
+ * Launches: none when n == 0; 1 (ERROR, KEEP: the write pass); 3 (SKIP: validity pass, scan of the tiles' kept counts,
+ * write pass).  Bytes moved: ERROR / KEEP read every source once and write n rows; SKIP reads every source twice and
+ * writes the kept rows (DESIGN.md §3.6.1).  timing: kernel_ms the call's kernels, d2h_bytes the kept rows and the counts
+ * read back, h2d_bytes the k source descriptors. */
+#define LO_INVALID_ERROR 0
+#define LO_INVALID_SKIP  1
+#define LO_INVALID_KEEP  2
+typedef struct lo_assemble_info {
+    int64_t nkept;
+    int64_t bad_row;     /* LO_INVALID_ERROR: the lowest row holding an invalid cell, else -1 */
+    int32_t bad_col;     /* its lowest invalid source (k: the label), else -1 */
+    int32_t pad;
+} lo_assemble_info;
+int lo_assemble_rows(lo_ctx *ctx, const lo_table *const *src, const int32_t *src_col, int32_t k, const lo_table *label,
+                     int32_t label_col, int32_t mode, lo_table *x, int64_t ld, lo_table *y, int64_t *kept_rows,
+                     lo_assemble_info *info, lo_host_timing *timing);
 
 /* Number -> text for one column: the reference's "string" cast, str(v) / None -> "" (data_type_handler_image/
  * data_type_update.py:22-28), for every cell at once on the GPU.  The inverse of lo_parse_number_host.

@@ -37,6 +37,7 @@ LO_FORMAT_MAX_CELL = 310
 LO_CSV_OK, LO_CSV_SHORT_ROW, LO_CSV_FIELD_LIMIT, LO_CSV_BAD_UTF8, LO_CSV_NUL, LO_CSV_UNSUPPORTED, LO_CSV_EMPTY = range(7)
 LO_CSV_STREAM_WINDOW = 64 << 20
 LO_TEXT_STAGE_SLOTS = 512
+LO_INVALID_ERROR, LO_INVALID_SKIP, LO_INVALID_KEEP = 0, 1, 2
 LO_ABI_VERSION = 7
 
 _ERR_NAMES = {
@@ -82,6 +83,10 @@ class CsvInfo(C.Structure):
 class CsvWindow(C.Structure):
     _fields_ = [("consumed", C.c_int64), ("records", C.c_int64), ("first_record", C.c_int64), ("ncols", C.c_int64),
                 ("chars", C.c_int64), ("peak_device_bytes", C.c_int64), ("done", C.c_int32), ("pad", C.c_int32)]
+
+
+class AssembleInfo(C.Structure):
+    _fields_ = [("nkept", C.c_int64), ("bad_row", C.c_int64), ("bad_col", C.c_int32), ("pad", C.c_int32)]
 
 
 # every symbol include/loexec.h declares: name -> (restype, argtypes)
@@ -158,6 +163,8 @@ SIGNATURES = {
     "lo_text_codes": (C.c_int, [_P, _P, _P, C.c_int32, _P, C.c_int64, C.POINTER(C.c_int64), C.POINTER(HostTiming)]),
     "lo_text_codes_shards": (C.c_int, [_P, C.POINTER(_P), C.POINTER(C.c_int64), C.c_int32, C.POINTER(_P), C.c_int32, _P,
                                        C.c_int64, C.POINTER(C.c_int64), C.POINTER(HostTiming)]),
+    "lo_assemble_rows": (C.c_int, [_P, C.POINTER(_P), C.POINTER(C.c_int32), C.c_int32, _P, C.c_int32, C.c_int32, _P,
+                                   C.c_int64, _P, _P, C.POINTER(AssembleInfo), C.POINTER(HostTiming)]),
     "lo_format_number_host": (C.c_int, [_P, _P, _P, C.c_int64, _P, _P, C.c_int64, C.POINTER(HostTiming)]),
     "lo_parse_text_to_table": (C.c_int, [_P, _P, _P, C.c_int32, C.POINTER(ParseSummary), C.POINTER(HostTiming)]),
     "lo_format_table_to_text": (C.c_int, [_P, _P, C.c_int32, C.POINTER(Validity), C.POINTER(Validity), C.POINTER(_P),

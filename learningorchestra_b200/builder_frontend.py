@@ -74,6 +74,42 @@ class DeviceFrame:
                 self.kinds[f] = data.kinds[data.column[f]]
                 self.nulls[f] = data.nulls[data.column[f]]
 
+    def features(self, fields=None, label=None, dtype: str = "float32", handle_invalid: str = "error") -> "Features":
+        """The step the reference's modelingCode ends in before ``classifier.fit``: Spark 2.4's
+        ``VectorAssembler(inputCols=fields, outputCol="features")`` and its ``label`` column, assembled in HBM on every
+        shard's device (``Engine.assemble_rows``).  Row i is ``[value(f, i) for f in fields]``: a number field's slab
+        value, a text field's dictionary code, as ``dtype`` ("float32": round-to-nearest-even; "float64": exact).
+        ``fields=None``: every field of the frame but ``label``, in frame order.  A cell is invalid when it is NaN (a null
+        or a real NaN) or a null text cell (code -1); ``handle_invalid``: "error" raises LoexecError LO_ERR_INVALID naming
+        the ``_id`` and field of the lowest one, "skip" drops every row with one in ``fields`` or ``label``, "keep" writes
+        NaN.  A field not in the frame raises KeyError before anything runs."""
+        from .engine import InvalidCellError, assemble_args
+        assemble_args(handle_invalid, dtype)
+        fields = [f for f in self.fields if f != label] if fields is None else list(fields)
+        for f in fields + ([label] if label is not None else []):
+            if f not in self.columns:
+                raise KeyError(f)
+        if not fields:
+            raise ValueError("features needs at least one field")
+        if self._data is None:
+            raise ValueError("the frame has been released")
+        engine = self._cache.engine
+        try:
+            parts = engine.assemble_rows([self._source(f) for f in fields],
+                                         self._source(label) if label is not None else None, dtype, handle_invalid)
+        except InvalidCellError as e:
+            name = label if e.position == len(fields) else fields[e.position]
+            raise InvalidCellError(e.row, e.position,
+                                   f"features: field {name!r} of the row with _id {self.ids[e.row]} is null or NaN "
+                                   f"(handle_invalid='error')") from None
+        return Features(self, parts if isinstance(parts, list) else [parts], fields, label, dtype)
+
+    def _source(self, f):
+        """(table, column) of field f as ``assemble_rows`` reads it: its code table, or the dataset's slab table."""
+        if f in self._codes:
+            return self._codes[f][0], 0
+        return self._data.table, self._data.column[f]
+
     def release(self):
         codes, self._codes = self._codes, {}
         for table, _dictionary in codes.values():
@@ -81,6 +117,36 @@ class DeviceFrame:
         if self._data is not None:
             self._cache.release(self._data)
             self._data = None
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.release()
+
+
+class Features:
+    """What :meth:`DeviceFrame.features` made: ``x[i]`` the feature matrix of shard i (one on a single GPU) as a
+    zero-copy ``__cuda_array_interface__`` view of shape ``(n_i, len(fields))``, row-major, on ``devices[i]``
+    (``torch.as_tensor(features.x[i], device=f"cuda:{features.devices[i]}")`` reads it in place); ``y[i]`` the label's
+    vector of n_i values, or ``y`` None; ``row_ids`` the ``_id`` of every row, shards concatenated in order; ``fields``
+    the column order.  Owns its tables and frees them in :meth:`release` (or with ``with``); keeps its frame alive."""
+
+    def __init__(self, frame: DeviceFrame, parts, fields, label, dtype):
+        import numpy as np
+        self._frame, self._parts = frame, list(parts)
+        self.fields, self.label, self.dtype = list(fields), label, dtype
+        self.devices = [p.x.engine.device for p in self._parts]
+        self.x = [p.matrix(keepalive=self) for p in self._parts]
+        self.y = [p.vector(keepalive=self) for p in self._parts] if label is not None else None
+        ids = np.asarray(frame.ids)
+        self.row_ids = np.concatenate([ids[p.first:p.first + p.nkept] if p.kept is None else ids[p.rows]
+                                       for p in self._parts]) if self._parts else np.zeros(0, np.int64)
+
+    def release(self):
+        parts, self._parts = self._parts, []
+        for p in parts:
+            p.free()
 
     def __enter__(self):
         return self

@@ -1680,6 +1680,245 @@ __global__ void __launch_bounds__(256) k_selftest_edges(float lo, float hi, floa
     if ((threadIdx.x & 31) == 0 && bad) atomicAdd(mismatches, bad);
 }
 
+// ---------------------------------------------------------------------------------------------
+// the feature matrix (lo_assemble_rows): Spark's VectorAssembler over k source columns, row-major.  A CTA takes a tile of
+// kAsmRows rows x a chunk of kAsmCols source columns: each warp reads 4 of the chunk's columns (16-byte read-once loads of
+// a full, aligned tile), converts in registers, transposes through shared memory and stores whole rows (one contiguous
+// span when the row is the chunk) or the chunk's row segments, with 16-byte streaming stores where aligned.  Invalid
+// cells (f64 NaN, code -1) are found in the same pass.
+// ---------------------------------------------------------------------------------------------
+constexpr int kAsmRows = 128;
+constexpr int kAsmCols = 32;
+constexpr int kAsmThreads = 256;          // 8 warps x 4 columns = one chunk
+constexpr int kAsmWords = kAsmRows / 32;  // keep-bit words per tile (the skip mode's validity pass)
+
+struct AsmSrc {
+    const char *p;      // the column's row 0
+    int i32;            // 1: int32 dictionary codes (-1 invalid), 0: f64 (NaN invalid)
+    int vec;            // 1: 16-byte aligned, full tiles take vector loads
+};
+
+__device__ __forceinline__ void ldg_v2u64_stream(const void *p, uint64_t pol, unsigned long long &a, unsigned long long &b) {
+    asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.v2.u64 {%0,%1}, [%2], %3;" : "=l"(a), "=l"(b) : "l"(p), "l"(pol));
+}
+__device__ __forceinline__ unsigned long long ldg_u64_stream(const void *p, uint64_t pol) {
+    unsigned long long v;
+    asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.u64 %0, [%1], %2;" : "=l"(v) : "l"(p), "l"(pol));
+    return v;
+}
+__device__ __forceinline__ unsigned ldg_u32_stream(const void *p, uint64_t pol) {
+    unsigned v;
+    asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.u32 %0, [%1], %2;" : "=r"(v) : "l"(p), "l"(pol));
+    return v;
+}
+__device__ __forceinline__ void stg_v16_stream(float *p, const float (&v)[4]) {
+    asm volatile("st.global.cs.v4.f32 [%0], {%1,%2,%3,%4};" :: "l"(p), "f"(v[0]), "f"(v[1]), "f"(v[2]), "f"(v[3]) : "memory");
+}
+__device__ __forceinline__ void stg_v16_stream(double *p, const double (&v)[2]) {
+    asm volatile("st.global.cs.v2.f64 [%0], {%1,%2};" :: "l"(p), "d"(v[0]), "d"(v[1]) : "memory");
+}
+
+// One warp's loads of one source column over a tile of nr rows from row0: four words per lane.  Vector loads (full tile,
+// aligned column): an f64 lane holds rows {2l, 2l+1, 64+2l, 65+2l}, an i32 lane rows 4l .. 4l+3 packed in w[0..1]; else
+// w[q] holds row l + 32q (rows < nr only).
+__device__ __forceinline__ void asm_load(const AsmSrc &s, long long row0, int nr, bool vec, int lane, uint64_t pol,
+                                         unsigned long long (&w)[4]) {
+    if (vec && !s.i32) {
+        const unsigned long long *p = reinterpret_cast<const unsigned long long *>(s.p) + row0 + 2 * lane;
+        ldg_v2u64_stream(p, pol, w[0], w[1]);
+        ldg_v2u64_stream(p + 64, pol, w[2], w[3]);
+    } else if (vec) {
+        ldg_v2u64_stream(reinterpret_cast<const unsigned *>(s.p) + row0 + 4 * lane, pol, w[0], w[1]);
+    } else {
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+            const int r = lane + 32 * q;
+            if (r < nr)
+                w[q] = s.i32 ? ldg_u32_stream(reinterpret_cast<const unsigned *>(s.p) + row0 + r, pol)
+                             : ldg_u64_stream(reinterpret_cast<const unsigned long long *>(s.p) + row0 + r, pol);
+        }
+    }
+}
+__device__ __forceinline__ int asm_row(bool vec, bool i32, int lane, int q) {
+    return !vec ? lane + 32 * q : i32 ? 4 * lane + q : (q & 2) * 32 + 2 * lane + (q & 1);
+}
+__device__ __forceinline__ unsigned long long asm_word(const unsigned long long (&w)[4], bool vec, bool i32, int q) {
+    return vec && i32 ? (w[q >> 1] >> (32 * (q & 1))) & 0xFFFFFFFFull : w[q];
+}
+__device__ __forceinline__ bool asm_bad(unsigned long long word, bool i32) {
+    return i32 ? (int)(unsigned)word == -1 : __longlong_as_double((long long)word) != __longlong_as_double((long long)word);
+}
+// the cell as the output dtype: f32 by fp64->fp32 RNE (cast_f64_f32) or from the code by int->fp32 RNE; f64 the slab's
+// bits or the exact code; a code of -1 becomes the canonical quiet NaN of the dtype
+__device__ __forceinline__ float asm_value(unsigned long long word, bool i32, float) {
+    if (!i32) return cast_f64_f32(__longlong_as_double((long long)word));
+    const int c = (int)(unsigned)word;
+    return c == -1 ? __int_as_float(0x7fc00000) : __int2float_rn(c);
+}
+__device__ __forceinline__ double asm_value(unsigned long long word, bool i32, double) {
+    if (!i32) return __longlong_as_double((long long)word);
+    const int c = (int)(unsigned)word;
+    return c == -1 ? __longlong_as_double(0x7FF8000000000000ll) : (double)c;
+}
+
+// The skip mode's validity pass: keep_bits[4 t .. 4 t + 3] = the rows of tile t whose cells in every source and the
+// label are valid (bit r of word r / 32), tile_count[t] = their number.
+__global__ void __launch_bounds__(kAsmThreads) k_assemble_valid(const AsmSrc *__restrict__ src, int k, AsmSrc label,
+                                                                long long n, unsigned *__restrict__ keep_bits,
+                                                                unsigned long long *__restrict__ tile_count) {
+    __shared__ unsigned bad[kAsmWords];
+    if (threadIdx.x < kAsmWords) bad[threadIdx.x] = 0;
+    __syncthreads();
+    const long long row0 = (long long)blockIdx.x * kAsmRows;
+    const int nr = (int)min((long long)kAsmRows, n - row0);
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const uint64_t pol = l2_evict_first_policy();
+    for (int c = warp; c < k; c += kAsmThreads / 32) {
+        const AsmSrc s = src[c];
+        const bool vec = nr == kAsmRows && s.vec;
+        unsigned long long w[4];
+        asm_load(s, row0, nr, vec, lane, pol, w);
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+            const int r = asm_row(vec, s.i32, lane, q);
+            if (r < nr && asm_bad(asm_word(w, vec, s.i32, q), s.i32)) atomicOr(&bad[r >> 5], 1u << (r & 31));
+        }
+    }
+    if (label.p && (int)threadIdx.x < nr) {
+        const int r = threadIdx.x;
+        const unsigned long long word = label.i32 ? ldg_u32_stream(reinterpret_cast<const unsigned *>(label.p) + row0 + r, pol)
+                                                  : ldg_u64_stream(reinterpret_cast<const unsigned long long *>(label.p) + row0 + r, pol);
+        if (asm_bad(word, label.i32)) atomicOr(&bad[r >> 5], 1u << (r & 31));
+    }
+    __syncthreads();
+    if (threadIdx.x < 32) {
+        const int i = threadIdx.x;
+        const int live = min(max(nr - 32 * i, 0), 32);
+        const unsigned keep = i < kAsmWords ? ~bad[i] & (live == 32 ? ~0u : (1u << live) - 1) : 0u;
+        if (i < kAsmWords) keep_bits[(long long)blockIdx.x * kAsmWords + i] = keep;
+        unsigned cnt = __popc(keep);
+#pragma unroll
+        for (int s = 16; s > 0; s >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, s);
+        if (i == 0) tile_count[blockIdx.x] = cnt;
+    }
+}
+
+// The write pass: the rows of tile blockIdx.x, columns [32 blockIdx.y, + 32) of the k sources, into x (row stride ld),
+// the label into y and (SKIP) the kept rows' source rows into kept_rows, by chunk 0.  !SKIP: row r goes to row r and, with
+// err, the lowest invalid cell's key row * (k + 1) + source (k: the label) is kept in *err.  SKIP: the tile's kept rows
+// (keep_bits) go to rows tile_off[t] .. tile_off[t + 1] in order.
+template <typename T, bool SKIP>
+__global__ void __launch_bounds__(kAsmThreads) k_assemble_rows(const AsmSrc *__restrict__ src, int k, AsmSrc label,
+                                                               long long n, T *__restrict__ x, long long ld,
+                                                               T *__restrict__ y, long long *__restrict__ kept_rows,
+                                                               const unsigned *__restrict__ keep_bits,
+                                                               const unsigned long long *__restrict__ tile_off,
+                                                               unsigned long long *__restrict__ err) {
+    constexpr int kVW = 16 / (int)sizeof(T);
+    __shared__ T tile[kAsmRows][kAsmCols + 1];
+    __shared__ int dst[SKIP ? kAsmRows : 1];      // SKIP: a row's place among the tile's kept rows, -1 dropped
+    const long long row0 = (long long)blockIdx.x * kAsmRows;
+    const int nr = (int)min((long long)kAsmRows, n - row0);
+    const int c0 = blockIdx.y * kAsmCols, kc = min(kAsmCols, k - c0);
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const uint64_t pol = l2_evict_first_policy();
+    long long out0 = row0;
+    int nout = nr;
+    if (SKIP) {
+        if (threadIdx.x < kAsmRows) {
+            const int r = threadIdx.x;
+            const unsigned *bits = keep_bits + (long long)blockIdx.x * kAsmWords;
+            int before = 0;
+            for (int i = 0; i < (r >> 5); ++i) before += __popc(bits[i]);
+            const unsigned word = bits[r >> 5];
+            dst[r] = (word >> (r & 31)) & 1 ? before + __popc(word & ((1u << (r & 31)) - 1)) : -1;
+        }
+        out0 = (long long)tile_off[blockIdx.x];
+        nout = (int)((long long)tile_off[blockIdx.x + 1] - out0);
+        __syncthreads();
+    }
+    AsmSrc s[4];
+    bool vec[4];
+    unsigned long long w[4][4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {                 // every load of the warp in flight before the first is used
+        const int cc = warp + 8 * i;
+        if (cc < kc) {
+            s[i] = src[c0 + cc];
+            vec[i] = nr == kAsmRows && s[i].vec;
+            asm_load(s[i], row0, nr, vec[i], lane, pol, w[i]);
+        }
+    }
+    unsigned long long bad_key = ~0ull;
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+        const int cc = warp + 8 * i;
+        if (cc >= kc) continue;
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+            const int r = asm_row(vec[i], s[i].i32, lane, q);
+            if (r >= nr) continue;
+            const unsigned long long word = asm_word(w[i], vec[i], s[i].i32, q);
+            const T v = asm_value(word, s[i].i32, T());
+            if (SKIP) {
+                if (dst[r] >= 0) tile[dst[r]][cc] = v;
+            } else {
+                tile[r][cc] = v;
+                if (err && asm_bad(word, s[i].i32))
+                    bad_key = min(bad_key, (unsigned long long)(row0 + r) * (unsigned long long)(k + 1) + (unsigned)(c0 + cc));
+            }
+        }
+    }
+    if (blockIdx.y == 0 && (int)threadIdx.x < nr) {
+        const int r = threadIdx.x;
+        const long long o = SKIP ? (dst[r] >= 0 ? out0 + dst[r] : -1) : row0 + r;
+        if (label.p) {
+            const unsigned long long word = label.i32 ? ldg_u32_stream(reinterpret_cast<const unsigned *>(label.p) + row0 + r, pol)
+                                                      : ldg_u64_stream(reinterpret_cast<const unsigned long long *>(label.p) + row0 + r, pol);
+            if (o >= 0) y[o] = asm_value(word, label.i32, T());
+            if (!SKIP && err && asm_bad(word, label.i32))
+                bad_key = min(bad_key, (unsigned long long)(row0 + r) * (unsigned long long)(k + 1) + (unsigned)k);
+        }
+        if (SKIP && kept_rows && o >= 0) kept_rows[o] = row0 + r;
+    }
+    if (!SKIP && err) {
+        bad_key = warp_min_u64(bad_key);
+        if (lane == 0 && bad_key != ~0ull) atomicMin(err, bad_key);
+    }
+    __syncthreads();
+    T *base = x + out0 * ld + c0;
+    if (kc == ld) {                               // whole rows: the tile's output is one span of nout * kc elements
+        const int len = nout * kc;
+        const int head = min(len, (int)(((16 - ((uintptr_t)base & 15)) & 15) / sizeof(T)));
+        const int nvec = (len - head) / kVW;
+        for (int e = threadIdx.x; e < head; e += kAsmThreads) base[e] = tile[e / kc][e % kc];
+        for (int e = head + nvec * kVW + threadIdx.x; e < len; e += kAsmThreads) base[e] = tile[e / kc][e % kc];
+        for (int v = threadIdx.x; v < nvec; v += kAsmThreads) {
+            const int e = head + v * kVW;
+            int r = e / kc, c = e - r * kc;
+            T vals[kVW];
+#pragma unroll
+            for (int j = 0; j < kVW; ++j) {
+                vals[j] = tile[r][c];
+                if (++c == kc) { c = 0; ++r; }
+            }
+            stg_v16_stream(base + e, vals);
+        }
+    } else if (kc % kVW == 0 && ((uintptr_t)base & 15) == 0 && (ld * (long long)sizeof(T)) % 16 == 0) {
+        const int vpr = kc / kVW;                 // row segments of whole 16-byte vectors
+        for (int v = threadIdx.x; v < nout * vpr; v += kAsmThreads) {
+            const int r = v / vpr, c = (v - r * vpr) * kVW;
+            T vals[kVW];
+#pragma unroll
+            for (int j = 0; j < kVW; ++j) vals[j] = tile[r][c + j];
+            stg_v16_stream(base + (long long)r * ld + c, vals);
+        }
+    } else {
+        for (int r = warp; r < nout; r += kAsmThreads / 32)
+            if (lane < kc) base[(long long)r * ld + lane] = tile[r][lane];
+    }
+}
+
 template <typename T>
 __global__ void k_checksum(const T *col, long long nrows, long long row_offset, unsigned long long *out) {
     unsigned long long acc = 0;

@@ -2433,5 +2433,131 @@ int lo_minmax_cast_host(lo_ctx *ctx, const double *const *in_cols, int64_t nrows
 
 }  // extern "C"
 
+namespace {
+
+// a source column of lo_assemble_rows: NULL, dtype, device, column and rows checked; *p receives its descriptor
+int check_assemble_src(const lo_ctx *ctx, const lo_table *t, int32_t col, int64_t n, const char *name, lo::AsmSrc *p) {
+    if (!t) return fail(LO_ERR_INVALID, "%s is NULL", name);
+    if (t->dtype != LO_F64 && t->dtype != LO_I32) return fail(LO_ERR_INVALID, "%s must be LO_F64 or LO_I32 (dtype %d)", name, t->dtype);
+    if (t->device != ctx->device) return fail(LO_ERR_INVALID, "%s lives on device %d, the context on %d", name, t->device, ctx->device);
+    if (col < 0 || col >= t->ncols) return fail(LO_ERR_INVALID, "%s: column %d outside [0, %d)", name, col, t->ncols);
+    if (t->nrows != n)
+        return fail(LO_ERR_INVALID, "%s has %lld rows, the first source %lld", name, (long long)t->nrows, (long long)n);
+    p->p = t->base + (int64_t)col * t->pitch;
+    p->i32 = t->dtype == LO_I32;
+    p->vec = (uintptr_t)p->p % 16 == 0;
+    return LO_OK;
+}
+
+int check_assemble_out(const lo_ctx *ctx, const lo_table *t, int dtype, int64_t need, const char *name) {
+    if (t->dtype != dtype) return fail(LO_ERR_INVALID, "%s must be %s", name, dtype == LO_F32 ? "LO_F32" : "LO_F64");
+    if (t->device != ctx->device) return fail(LO_ERR_INVALID, "%s lives on device %d, the context on %d", name, t->device, ctx->device);
+    if (t->nrows < need)
+        return fail(LO_ERR_INVALID, "%s holds %lld elements, %lld needed", name, (long long)t->nrows, (long long)need);
+    return LO_OK;
+}
+
+constexpr int64_t kAsmMaxK = 65535ll * lo::kAsmCols;    // chunks on the grid's y dimension
+
+template <typename T>
+void launch_assemble(HostCall &c, bool skip, const lo::AsmSrc *src, int k, const lo::AsmSrc &label, int64_t n, T *x,
+                     int64_t ld, T *y, long long *kept, const unsigned *bits, const unsigned long long *off,
+                     unsigned long long *err) {
+    const dim3 grid((unsigned)((n + lo::kAsmRows - 1) / lo::kAsmRows), (unsigned)((k + lo::kAsmCols - 1) / lo::kAsmCols));
+    c.launch(1, [&] {
+        if (skip) lo::k_assemble_rows<T, true><<<grid, lo::kAsmThreads, 0, c.s>>>(src, k, label, n, x, ld, y, kept, bits, off, nullptr);
+        else      lo::k_assemble_rows<T, false><<<grid, lo::kAsmThreads, 0, c.s>>>(src, k, label, n, x, ld, y, nullptr, nullptr, nullptr, err);
+    });
+}
+
+}  // namespace
+
+extern "C" {
+
+int lo_assemble_rows(lo_ctx *ctx, const lo_table *const *src, const int32_t *src_col, int32_t k, const lo_table *label,
+                     int32_t label_col, int32_t mode, lo_table *x, int64_t ld, lo_table *y, int64_t *kept_rows,
+                     lo_assemble_info *info, lo_host_timing *timing) {
+    LO_TRY(check_ctx(ctx));
+    if (!info) return fail(LO_ERR_INVALID, "info is NULL");
+    *info = lo_assemble_info{0, -1, -1, 0};
+    if (!src || !src_col) return fail(LO_ERR_INVALID, "src or src_col is NULL");
+    if (k < 1 || k > kAsmMaxK) return fail(LO_ERR_INVALID, "k = %d outside [1, %lld]", k, (long long)kAsmMaxK);
+    if (mode != LO_INVALID_ERROR && mode != LO_INVALID_SKIP && mode != LO_INVALID_KEEP)
+        return fail(LO_ERR_INVALID, "unknown mode %d", mode);
+    if (!src[0]) return fail(LO_ERR_INVALID, "src[0] is NULL");
+    const int64_t n = src[0]->nrows;
+    std::vector<lo::AsmSrc> desc((size_t)k);
+    for (int j = 0; j < k; ++j) {
+        char name[24];
+        snprintf(name, sizeof name, "src[%d]", j);
+        LO_TRY(check_assemble_src(ctx, src[j], src_col[j], n, name, &desc[j]));
+    }
+    lo::AsmSrc lab = {nullptr, 0, 0};
+    if (label) LO_TRY(check_assemble_src(ctx, label, label_col, n, "label", &lab));
+    if (!x) return fail(LO_ERR_INVALID, "x is NULL");
+    if (x->dtype != LO_F32 && x->dtype != LO_F64) return fail(LO_ERR_INVALID, "x must be LO_F32 or LO_F64 (dtype %d)", x->dtype);
+    if (ld < k) return fail(LO_ERR_INVALID, "ld = %lld is less than k = %d", (long long)ld, k);
+    if (n > 0 && ld > (INT64_MAX / 2) / n) return fail(LO_ERR_INVALID, "n * ld overflows (ld = %lld)", (long long)ld);
+    LO_TRY(check_assemble_out(ctx, x, x->dtype, n * ld, "x"));
+    if (!label != !y) return fail(LO_ERR_INVALID, "y and label go together");
+    if (y) LO_TRY(check_assemble_out(ctx, y, x->dtype, n, "y"));
+    HostCall c(ctx, "assemble_rows");
+    if (n == 0) return c.finish(timing);
+    const bool skip = mode == LO_INVALID_SKIP, err_mode = mode == LO_INVALID_ERROR;
+    const int64_t ntiles = (n + lo::kAsmRows - 1) / lo::kAsmRows;
+    lo::AsmSrc *d_src = nullptr;
+    unsigned long long *err = nullptr, *off = nullptr;
+    unsigned *bits = nullptr;
+    long long *kept = nullptr;
+    c.alloc(&d_src, (size_t)k * sizeof(lo::AsmSrc));
+    c.to_dev(d_src, desc.data(), (size_t)k * sizeof(lo::AsmSrc));
+    if (err_mode) {
+        c.alloc(&err, 8);
+        c.memset(err, 0xFF, 8);
+    }
+    void *tmp = nullptr;
+    size_t tmp_bytes = 0;
+    if (skip) {
+        c.alloc(&bits, (size_t)ntiles * lo::kAsmWords * 4);
+        c.alloc(&off, (size_t)(ntiles + 1) * 8);
+        if (kept_rows) c.alloc(&kept, (size_t)n * 8);
+        c.memset(off + ntiles, 0, 8);
+        c.run([&] { return cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, off, ntiles + 1, c.s); });
+        c.alloc(&tmp, tmp_bytes);
+    }
+    c.mark();
+    if (skip) {
+        c.launch(1, [&] {
+            lo::k_assemble_valid<<<(unsigned)ntiles, lo::kAsmThreads, 0, c.s>>>(d_src, k, lab, n, bits, off);
+        });
+        c.launch(1, [&] { return cub::DeviceScan::ExclusiveSum(tmp, tmp_bytes, off, ntiles + 1, c.s); });
+    }
+    if (x->dtype == LO_F32)
+        launch_assemble(c, skip, d_src, k, lab, n, (float *)x->base, ld, y ? (float *)y->base : nullptr, kept, bits, off, err);
+    else
+        launch_assemble(c, skip, d_src, k, lab, n, (double *)x->base, ld, y ? (double *)y->base : nullptr, kept, bits, off, err);
+    c.mark();
+    unsigned long long nkept = (unsigned long long)n, key = ~0ull;
+    if (skip) {
+        c.to_host(&nkept, off + ntiles, 8);
+        c.sync();
+        if (kept_rows) c.to_host(kept_rows, kept, nkept * 8);
+    }
+    if (err_mode) c.to_host(&key, err, 8);
+    LO_TRY(c.finish(timing));
+    if (key != ~0ull) {
+        info->bad_row = (int64_t)(key / (unsigned long long)(k + 1));
+        info->bad_col = (int32_t)(key % (unsigned long long)(k + 1));
+        return fail(LO_ERR_INVALID, "invalid cell (NaN or code -1) in row %lld, %s %d", (long long)info->bad_row,
+                    info->bad_col == k ? "the label, source" : "source", info->bad_col);
+    }
+    info->nkept = (int64_t)nkept;
+    if (kept_rows && !skip)
+        for (int64_t i = 0; i < n; ++i) kept_rows[i] = i;
+    return LO_OK;
+}
+
+}  // extern "C"
+
 #include "group.inc"
 #include "csv.inc"

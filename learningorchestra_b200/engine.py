@@ -269,6 +269,71 @@ class DeviceColumn:
                 "version": 3, "strides": None}
 
 
+class DeviceArray:
+    """Zero-copy ``__cuda_array_interface__`` view of the first ``prod(shape)`` elements of a table's column 0, C order:
+    a row-major matrix or a vector of :meth:`Engine.assemble_rows`.  Keeps its table (and ``keepalive``) alive."""
+
+    def __init__(self, table: "DeviceTable", shape: tuple, keepalive=None):
+        self.table, self.shape, self._keepalive = table, tuple(int(d) for d in shape), keepalive
+        self.data_ptr = table.base_ptr
+
+    @property
+    def __cuda_array_interface__(self):
+        return {"shape": self.shape, "typestr": DeviceColumn._TYPESTR[self.table.dtype_code], "data": (self.data_ptr, False),
+                "version": 3, "strides": None}
+
+
+class InvalidCellError(N.LoexecError):
+    """:meth:`Engine.assemble_rows` with ``handle_invalid="error"`` met an invalid cell: ``row`` is the lowest such row
+    (a source row; global over the shards of a :class:`~sharding.ShardedEngine`) and ``position`` its lowest invalid
+    source (an index into ``sources``; ``len(sources)``: the label)."""
+
+    def __init__(self, row: int, position: int, message: str):
+        super().__init__(N.LO_ERR_INVALID, message)
+        self.row, self.position = int(row), int(position)
+
+
+class AssembledRows:
+    """The feature matrix one device made (:meth:`Engine.assemble_rows`): ``x`` a flat table holding ``nkept`` rows of
+    ``k`` values, row-major; ``y`` the label's flat table or None; ``rows`` the kept source rows (int64, output order)
+    plus ``first``, the shard's first row.  ``kept`` None: every row was kept, and ``rows`` is made only when read.
+    :meth:`matrix` / :meth:`vector` view them in place.  :meth:`free` frees both tables; it may be called again."""
+
+    def __init__(self, x: "DeviceTable", y: "DeviceTable | None", kept: np.ndarray | None, k: int, nkept: int):
+        self.x, self.y, self.kept, self.k, self.nkept = x, y, kept, int(k), int(nkept)
+        self.first = 0
+
+    @property
+    def rows(self) -> np.ndarray:
+        if self.kept is None:
+            return np.arange(self.first, self.first + self.nkept, dtype=np.int64)
+        return self.kept + self.first
+
+    def matrix(self, keepalive=None) -> DeviceArray:
+        return DeviceArray(self.x, (self.nkept, self.k), keepalive)
+
+    def vector(self, keepalive=None) -> DeviceArray | None:
+        return None if self.y is None else DeviceArray(self.y, (self.nkept,), keepalive)
+
+    def free(self) -> None:
+        for t in (self.x, self.y):
+            if t is not None:
+                t.free()
+
+
+ASSEMBLE_MODES = {"error": N.LO_INVALID_ERROR, "skip": N.LO_INVALID_SKIP, "keep": N.LO_INVALID_KEEP}
+ASSEMBLE_DTYPES = {"float32": "f32", "float64": "f64"}
+
+
+def assemble_args(handle_invalid: str, dtype: str) -> tuple[int, str]:
+    """(lo_assemble_rows mode, table dtype) of the Python names; ValueError for any other."""
+    if handle_invalid not in ASSEMBLE_MODES:
+        raise ValueError(f"handle_invalid must be one of {sorted(ASSEMBLE_MODES)}, not {handle_invalid!r}")
+    if dtype not in ASSEMBLE_DTYPES:
+        raise ValueError(f"dtype must be one of {sorted(ASSEMBLE_DTYPES)}, not {dtype!r}")
+    return ASSEMBLE_MODES[handle_invalid], ASSEMBLE_DTYPES[dtype]
+
+
 class DeviceTable:
     """Columnar table in HBM: ``ncols`` slabs of ``nrows`` elements of one dtype."""
 
@@ -800,6 +865,58 @@ class Engine:
             raise ValueError("the text column has been freed")
         return _first_rows(lambda rows, cap, nd, t: self._lib.lo_text_codes(
             self._ctx, text._h, table._h, int(col), rows, cap, nd, t), text.n - text.nulls, timing)
+
+    def assemble_rows(self, sources, label=None, dtype: str = "float32", handle_invalid: str = "error",
+                      timing: dict | None = None) -> AssembledRows:
+        """Spark's ``VectorAssembler`` on the device (``lo_assemble_rows``): row i of the result is the value of every
+        ``(table, col)`` of ``sources`` at row i — an f64 slab's value, an int32 code column's code — as ``dtype``
+        (``"float32"``: fp64->fp32 round-to-nearest-even; ``"float64"``: exact), and ``label`` (one more ``(table,
+        col)`` or None) fills ``y``.  A NaN cell or a -1 code is invalid: ``handle_invalid="error"`` raises
+        :class:`InvalidCellError` naming the lowest one, ``"skip"`` leaves its row out, ``"keep"`` writes NaN.
+        ``timing``: a dict to receive the call's lo_host_timing fields."""
+        rows, bad = self._assemble_rows(sources, label, dtype, handle_invalid, timing)
+        if bad is not None:
+            raise InvalidCellError(*bad)
+        return rows
+
+    def _assemble_rows(self, sources, label, dtype, handle_invalid, timing=None):
+        """(AssembledRows, None), or (None, (row, position, message)) when ``"error"`` met an invalid cell (the tables
+        freed): :meth:`assemble_rows` without raising, for :meth:`ShardedEngine.assemble_rows` to compare shards."""
+        mode, out = assemble_args(handle_invalid, dtype)
+        k = len(sources)
+        if k == 0:
+            raise ValueError("assemble_rows needs at least one source column")
+        if any(t._h is None for t, _c in sources) or (label is not None and label[0]._h is None):
+            raise ValueError("a source table has been freed")
+        n = sources[0][0].nrows
+        tabs = (C.c_void_p * k)(*[t._h for t, _c in sources])
+        cols = (C.c_int32 * k)(*[int(c) for _t, c in sources])
+        x = self.table(out, n * k, 1)
+        y = rows = None
+        try:
+            y = self.table(out, n, 1) if label is not None else None
+            rows = np.empty(n, np.int64) if mode == N.LO_INVALID_SKIP else None    # else every row is kept, in order
+            info, t = N.AssembleInfo(), N.HostTiming()
+            rc = self._lib.lo_assemble_rows(self._ctx, tabs, cols, k, label[0]._h if label is not None else None,
+                                            int(label[1]) if label is not None else 0, mode, x._h, k,
+                                            y._h if y is not None else None,
+                                            rows.ctypes.data_as(C.c_void_p) if rows is not None else None,
+                                            C.byref(info), C.byref(t))
+            if rc == N.LO_ERR_INVALID and info.bad_row >= 0:
+                msg = self._lib.lo_last_error().decode("utf-8", "replace")
+                x.free()
+                if y is not None:
+                    y.free()
+                return None, (int(info.bad_row), int(info.bad_col), msg)
+            N.check(rc)
+        except BaseException:
+            x.free()
+            if y is not None:
+                y.free()
+            raise
+        if timing is not None:
+            timing.update(_timing(t), kernel_ms=t.kernel_ms)
+        return AssembledRows(x, y, rows[:info.nkept] if rows is not None else None, k, info.nkept), None
 
     def value_counts_f64_host(self, values: np.ndarray):
         """(keys float64[g], counts uint64[g]) — exact value counts of a numeric column (GPU hash group-by),

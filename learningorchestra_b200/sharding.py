@@ -693,6 +693,38 @@ class ShardedEngine:
             self.engines[0]._ctx, shards, row0, len(shards), self._tables(table), int(col), rows, cap, nd, t),
             text.n - text.nulls, timing)
 
+    def assemble_rows(self, sources, label=None, dtype: str = "float32", handle_invalid: str = "error") -> list:
+        """``Engine.assemble_rows`` over sharded tables: ``sources`` / ``label`` are ``(ShardedTable, col)`` pairs cut at
+        the same rows, and every member assembles its own shard's rows on its own device, from a host thread of its own;
+        nothing crosses devices.  Returns one ``AssembledRows`` per local member, its ``rows`` global (the shard's first
+        row added).  ``"error"``: the lowest invalid row over all shards is raised (``InvalidCellError``).  A rank group's
+        process holds only its own rows, so it refuses rather than assemble a part."""
+        from .engine import InvalidCellError, assemble_args
+        self._every_row("assemble_rows")
+        assemble_args(handle_invalid, dtype)
+        tables = [t for t, _c in sources] + ([label[0]] if label is not None else [])
+        offsets = tables[0].offsets if tables else []
+        if any(t.offsets != offsets or [s.nrows for s in t.shards] != [s.nrows for s in tables[0].shards] for t in tables):
+            raise ValueError("the source tables are not cut at the same rows")
+
+        def run(i):
+            return self.engines[i]._assemble_rows([(t.shards[i], c) for t, c in sources],
+                                                  (label[0].shards[i], label[1]) if label is not None else None,
+                                                  dtype, handle_invalid)
+
+        parts = on_each(self.nlocal, run, undo=lambda p: p[0] is not None and p[0].free())
+        bad = [(off + b[0], b[1]) for (_r, b), off in zip(parts, offsets) if b is not None]
+        if bad:
+            for rows, _b in parts:
+                if rows is not None:
+                    rows.free()
+            row, position = min(bad)
+            raise InvalidCellError(row, position, f"invalid cell (NaN or code -1) in row {row}, "
+                                   f"{'the label' if position == len(sources) else 'source %d' % position}")
+        for (rows, _b), off in zip(parts, offsets):
+            rows.first = off
+        return [rows for rows, _b in parts]
+
     @property
     def resident(self):
         """Datasets kept in HBM between requests, rows sharded over the group (:mod:`table_cache`)."""

@@ -11,6 +11,11 @@ codes_log="$(mktemp -d)/sanitizer_memcheck_text_codes.txt"
 timeout 900 compute-sanitizer --tool memcheck --error-exitcode 1 python -m pytest tests/test_gpu_text_codes.py -q \
     > "$codes_log" 2>&1
 echo "memcheck (text codes) rc=$? log=$codes_log"; tail -3 "$codes_log"
+# memcheck of the feature matrix (validity pass, scan, write pass; every shape and refusal); its log goes to a temporary directory
+features_log="$(mktemp -d)/sanitizer_memcheck_features.txt"
+timeout 900 compute-sanitizer --tool memcheck --error-exitcode 1 python -m pytest tests/test_gpu_features.py -q \
+    > "$features_log" 2>&1
+echo "memcheck (features) rc=$? log=$features_log"; tail -3 "$features_log"
 # memcheck of the number parser and the resident formatter on every entry point, without the million-row cases: a read
 # past the last staged cell shows here (the CPU harness puts a NUL after it)
 parse_log="$(mktemp -d)/sanitizer_memcheck_parse.txt"
