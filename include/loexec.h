@@ -467,6 +467,63 @@ int lo_assemble_rows(lo_ctx *ctx, const lo_table *const *src, const int32_t *src
                      int32_t label_col, int32_t mode, lo_table *x, int64_t ld, lo_table *y, int64_t *kept_rows,
                      lo_assemble_info *info, lo_host_timing *timing);
 
+/* Spark 2.4's multinomial NaiveBayes (ml.classification.NaiveBayes with smoothing, no weightCol, no thresholds;
+ * builder_image/builder.py:55-61's "NB") over a feature matrix of lo_assemble_rows: x holds n rows of k features
+ * (column 0, row stride ld >= k elements), y their labels, both LO_F32 or both LO_F64 on ctx's device; every value is
+ * widened to f64 exactly.  Classes are label values, ascending; C = their number.  DESIGN.md §3.6.2.
+ *
+ * lo_nb_labels: the distinct values of y[0 .. n), ascending, into labels_out (host double[capacity]); -0.0 is 0.0.  The
+ * f64 hash group-by of lo_value_counts_f64_table (an LO_F32 y is widened on the way in).  *nlabels = their number; more
+ * than capacity fails with LO_ERR_INVALID after *nlabels is set, and so does a NaN label (*nlabels set, labels_out
+ * unwritten).  Launches: none when n == 0; 2 (LO_F64) or 3 (LO_F32: the widening).  Bytes: y read once (LO_F32: read,
+ * written as f64 and read again).  timing: d2h_bytes the groups read back.
+ *
+ * lo_nb_fit: counts_out[c] (host int64[C]) = the rows whose label is classes[c]; sums_out[c * k + j] (host double[C * k])
+ * = the f64 sum of x[i][j] over those rows, reduced in a fixed order without floating-point atomics: the same input gives
+ * the same bits on every run, and exact partial sums (integer-valued features below 2^53) give the exact sum.  No sum
+ * is a sequential run of more than 256 adds (a tree above that), so |sum - exact| <= 1e-13 * sum.  Every
+ * feature must be >= 0.0 (Spark's requireNonnegativeValues: NaN fails it, +inf passes); else the call fails with
+ * LO_ERR_INVALID and info->bad_row / bad_col name the lowest such row and its lowest such column.  A label that is none
+ * of classes fails the same way with bad_col = k.  classes: nclasses values, strictly ascending, not NaN.
+ * Launches: none when n == 0; per window of rows whose CTAs' C x k partials fit 256 MiB, one k_nb_sums (one read of x
+ * and y) and the k_nb_reduce levels of its partials (32 to 1 each); then the levels over the windows' sums.  timing:
+ * h2d_bytes the classes, d2h_bytes the sums, counts and the error word.
+ *
+ * lo_nb_predict: the model (pi host double[C], theta host double[C * k], row-major) applied to every row:
+ *   raw_c = (sum_j theta[c * k + j] * x_j, from 0.0 in ascending j) + pi[c], every product and add rounded on its own
+ *   (F2J dgemv, no FMA); then Spark's raw2probabilityInPlace: m the left-fold max, e_c = exp(raw_c - m), summed in c
+ *   order, p_c = e_c / sum; prediction = Vector.argmax(p) (index 0, then a later index only when strictly greater) as
+ *   the f64 class INDEX.
+ * Transform (confusion_out NULL): prob (LO_F64, n * C elements, row-major) and pred (LO_F64, n) are written, and raw
+ * (LO_F64, n * C, or NULL) receives the raw values; y and eval_labels must be NULL.  Evaluate (confusion_out a host
+ * int64[neval * C]): nothing per row is written (prob, raw and pred must be NULL); confusion_out[a * C + p] = the rows
+ * whose label is eval_labels[a] (neval values, strictly ascending, not NaN) and whose prediction is p.  A label that is
+ * none of eval_labels fails with LO_ERR_INVALID, info->bad_row its lowest row, bad_col = k.
+ * Launches: none when n == 0; 1 (k_nb_predict).  Bytes: x read once; transform writes n * 8 * (C + 1) (+ n * 8 * C with
+ * raw); evaluate reads y once more and writes nothing per row.  timing: h2d_bytes the model (and labels), d2h_bytes the
+ * confusion counts and the error word.
+ *
+ * Refused with LO_ERR_INVALID before anything is enqueued (all three, as they apply): a NULL x, y, classes, model,
+ * output or info; x or y not LO_F32 / LO_F64, of different dtypes or on another device; k < 1; ld < k; n < 0; x holding
+ * fewer than n * ld elements, y fewer than n; C or neval outside [1, LO_NB_MAX_CLASSES]; C * k > LO_NB_MAX_THETA;
+ * classes or eval_labels not strictly ascending or holding NaN; an output table of the wrong dtype, device or size;
+ * the transform / evaluate arguments mixed. */
+#define LO_NB_MAX_CLASSES 1024
+#define LO_NB_MAX_THETA   16384   /* C * k: theta in f64 in 128 KiB of shared memory */
+typedef struct lo_nb_info {
+    int64_t bad_row;     /* the lowest row holding a refused value, else -1 */
+    int32_t bad_col;     /* its lowest refused feature column (k: the label), else -1 */
+    int32_t pad;
+} lo_nb_info;
+int lo_nb_labels(lo_ctx *ctx, const lo_table *y, int64_t n, double *labels_out, int64_t capacity, int64_t *nlabels,
+                 lo_host_timing *timing);
+int lo_nb_fit(lo_ctx *ctx, const lo_table *x, int64_t ld, int32_t k, const lo_table *y, int64_t n, const double *classes,
+              int32_t nclasses, double *sums_out, int64_t *counts_out, lo_nb_info *info, lo_host_timing *timing);
+int lo_nb_predict(lo_ctx *ctx, const lo_table *x, int64_t ld, int32_t k, int64_t n, const double *pi, const double *theta,
+                  int32_t nclasses, lo_table *prob, lo_table *raw, lo_table *pred, const lo_table *y,
+                  const double *eval_labels, int32_t neval, int64_t *confusion_out, lo_nb_info *info,
+                  lo_host_timing *timing);
+
 /* Number -> text for one column: the reference's "string" cast, str(v) / None -> "" (data_type_handler_image/
  * data_type_update.py:22-28), for every cell at once on the GPU.  The inverse of lo_parse_number_host.
  * status[i] uses the LO_NUM_* codes above: FLOAT -> repr(float) (shortest round-trip digits, CPython's notation),

@@ -38,6 +38,8 @@ LO_CSV_OK, LO_CSV_SHORT_ROW, LO_CSV_FIELD_LIMIT, LO_CSV_BAD_UTF8, LO_CSV_NUL, LO
 LO_CSV_STREAM_WINDOW = 64 << 20
 LO_TEXT_STAGE_SLOTS = 512
 LO_INVALID_ERROR, LO_INVALID_SKIP, LO_INVALID_KEEP = 0, 1, 2
+LO_NB_MAX_CLASSES = 1024
+LO_NB_MAX_THETA = 16384
 LO_ABI_VERSION = 7
 
 _ERR_NAMES = {
@@ -87,6 +89,10 @@ class CsvWindow(C.Structure):
 
 class AssembleInfo(C.Structure):
     _fields_ = [("nkept", C.c_int64), ("bad_row", C.c_int64), ("bad_col", C.c_int32), ("pad", C.c_int32)]
+
+
+class NbInfo(C.Structure):
+    _fields_ = [("bad_row", C.c_int64), ("bad_col", C.c_int32), ("pad", C.c_int32)]
 
 
 # every symbol include/loexec.h declares: name -> (restype, argtypes)
@@ -165,6 +171,11 @@ SIGNATURES = {
                                        C.c_int64, C.POINTER(C.c_int64), C.POINTER(HostTiming)]),
     "lo_assemble_rows": (C.c_int, [_P, C.POINTER(_P), C.POINTER(C.c_int32), C.c_int32, _P, C.c_int32, C.c_int32, _P,
                                    C.c_int64, _P, _P, C.POINTER(AssembleInfo), C.POINTER(HostTiming)]),
+    "lo_nb_labels": (C.c_int, [_P, _P, C.c_int64, _P, C.c_int64, C.POINTER(C.c_int64), C.POINTER(HostTiming)]),
+    "lo_nb_fit": (C.c_int, [_P, _P, C.c_int64, C.c_int32, _P, C.c_int64, _P, C.c_int32, _P, _P, C.POINTER(NbInfo),
+                            C.POINTER(HostTiming)]),
+    "lo_nb_predict": (C.c_int, [_P, _P, C.c_int64, C.c_int32, C.c_int64, _P, _P, C.c_int32, _P, _P, _P, _P, _P,
+                                C.c_int32, _P, C.POINTER(NbInfo), C.POINTER(HostTiming)]),
     "lo_format_number_host": (C.c_int, [_P, _P, _P, C.c_int64, _P, _P, C.c_int64, C.POINTER(HostTiming)]),
     "lo_parse_text_to_table": (C.c_int, [_P, _P, _P, C.c_int32, C.POINTER(ParseSummary), C.POINTER(HostTiming)]),
     "lo_format_table_to_text": (C.c_int, [_P, _P, C.c_int32, C.POINTER(Validity), C.POINTER(Validity), C.POINTER(_P),

@@ -5,6 +5,7 @@
 // lo_init() fails and nothing else is callable.
 #include "loexec.h"
 #include "kernels.cuh"
+#include "naive_bayes.cuh"
 
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
@@ -2554,6 +2555,283 @@ int lo_assemble_rows(lo_ctx *ctx, const lo_table *const *src, const int32_t *src
     info->nkept = (int64_t)nkept;
     if (kept_rows && !skip)
         for (int64_t i = 0; i < n; ++i) kept_rows[i] = i;
+    return LO_OK;
+}
+
+}  // extern "C"
+
+static_assert(lo::kNbMaxClasses == LO_NB_MAX_CLASSES && lo::kNbMaxTheta == LO_NB_MAX_THETA, "loexec.h documents the caps");
+
+namespace {
+
+// an LO_F32 / LO_F64 table of lo_nb_*: NULL, dtype (dtype 0: either float dtype), device and size checked
+int check_nb_table(const lo_ctx *ctx, const lo_table *t, int dtype, int64_t need, const char *name) {
+    if (!t) return fail(LO_ERR_INVALID, "%s is NULL", name);
+    if (dtype ? t->dtype != dtype : t->dtype != LO_F32 && t->dtype != LO_F64)
+        return fail(LO_ERR_INVALID, "%s must be %s (dtype %d)", name, dtype == LO_F64 ? "LO_F64" : "LO_F32 or LO_F64", t->dtype);
+    if (t->device != ctx->device) return fail(LO_ERR_INVALID, "%s lives on device %d, the context on %d", name, t->device, ctx->device);
+    if (t->nrows < need)
+        return fail(LO_ERR_INVALID, "%s holds %lld elements, %lld needed", name, (long long)t->nrows, (long long)need);
+    return LO_OK;
+}
+
+// the matrix x (n rows of k, stride ld) and, when given, its labels y of the same dtype
+int check_nb_matrix(const lo_ctx *ctx, const lo_table *x, int64_t ld, int32_t k, int64_t n, const lo_table *y) {
+    if (k < 1) return fail(LO_ERR_INVALID, "k = %d: at least one feature", k);
+    if (ld < k) return fail(LO_ERR_INVALID, "ld = %lld is less than k = %d", (long long)ld, k);
+    if (n < 0) return fail(LO_ERR_INVALID, "n = %lld is negative", (long long)n);
+    if (n > 0 && ld > (INT64_MAX / 2) / n) return fail(LO_ERR_INVALID, "n * ld overflows (ld = %lld)", (long long)ld);
+    LO_TRY(check_nb_table(ctx, x, 0, n * ld, "x"));
+    if (y) LO_TRY(check_nb_table(ctx, y, x->dtype, n, "y"));
+    return LO_OK;
+}
+
+// a class or label table: count in [1, LO_NB_MAX_CLASSES], strictly ascending, no NaN; *direct: exactly 0 .. m-1
+int check_nb_classes(const double *v, int32_t m, const char *name, int *direct) {
+    if (!v) return fail(LO_ERR_INVALID, "%s is NULL", name);
+    if (m < 1 || m > LO_NB_MAX_CLASSES) return fail(LO_ERR_INVALID, "%d %s outside [1, %d]", m, name, LO_NB_MAX_CLASSES);
+    *direct = 1;
+    for (int32_t i = 0; i < m; ++i) {
+        if (v[i] != v[i] || (i > 0 && !(v[i] > v[i - 1])))
+            return fail(LO_ERR_INVALID, "%s must be strictly ascending and not NaN (entry %d)", name, i);
+        if (v[i] != (double)i) *direct = 0;
+    }
+    return LO_OK;
+}
+
+int check_nb_caps(int32_t nclasses, int32_t k) {
+    if (nclasses < 1 || nclasses > LO_NB_MAX_CLASSES)
+        return fail(LO_ERR_INVALID, "%d classes outside [1, %d]", nclasses, LO_NB_MAX_CLASSES);
+    if ((int64_t)nclasses * k > LO_NB_MAX_THETA)
+        return fail(LO_ERR_INVALID, "%d classes x %d features exceed LO_NB_MAX_THETA = %d", nclasses, k, LO_NB_MAX_THETA);
+    return LO_OK;
+}
+
+// *info and the message of a refused row (key = row * (k + 1) + column)
+int nb_bad_row(lo_nb_info *info, unsigned long long key, int32_t k, const char *what) {
+    info->bad_row = (int64_t)(key / (unsigned long long)(k + 1));
+    info->bad_col = (int32_t)(key % (unsigned long long)(k + 1));
+    if (info->bad_col == k) return fail(LO_ERR_INVALID, "row %lld: its label is not one of the %s", (long long)info->bad_row, what);
+    return fail(LO_ERR_INVALID, "row %lld, feature %d: negative or NaN (NaiveBayes needs values >= 0)",
+                (long long)info->bad_row, info->bad_col);
+}
+
+// k_nb_sums over rows [row0, row1): one CTA per G * kNbRun rows, shape = {G, Q, kp, stride, vw}
+template <typename T>
+void launch_nb_sums(HostCall &c, const lo_table *x, int64_t ld, int32_t k, const lo_table *y, int64_t row0, int64_t row1,
+                    const double *cls, int32_t C, int direct, double *partial, unsigned long long *counts,
+                    unsigned long long *err, const int (&shape)[5], int smem) {
+    const int G = shape[0], Q = shape[1], kp = shape[2], stride = shape[3], vw = shape[4];
+    const int64_t per_cta = (int64_t)G * lo::kNbRun, nct = (row1 - row0 + per_cta - 1) / per_cta;
+    auto go = [&](auto kernel) {
+        c.run([&] { return cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem); });
+        c.launch(1, [&] {
+            kernel<<<(unsigned)nct, lo::kNbThreads, smem, c.s>>>((const T *)x->base, ld, k, (const T *)y->base, row0, row1,
+                                                               cls, C, direct, G, Q, kp, stride, partial, counts, err);
+        });
+    };
+    if (vw > 1) go(lo::k_nb_sums<T, 16 / (int)sizeof(T)>);
+    else        go(lo::k_nb_sums<T, 1>);
+}
+
+// The m rows of `slots` partials at src added into dst (slots doubles) by k_nb_reduce levels of kNbFan, ping-ponging
+// through buf[0] / buf[1] (each ceil(m / kNbFan) rows).
+void nb_tree(HostCall &c, const double *src, int64_t m, size_t slots, double *dst, double *const (&buf)[2]) {
+    for (int which = 0;; which ^= 1) {
+        const int64_t m2 = (m + lo::kNbFan - 1) / lo::kNbFan;
+        double *out = m2 == 1 ? dst : buf[which];
+        const dim3 grid((unsigned)((slots + lo::kNbThreads - 1) / lo::kNbThreads), (unsigned)m2);
+        c.launch(1, [&] { lo::k_nb_reduce<<<grid, lo::kNbThreads, 0, c.s>>>(src, m, (int)slots, out); });
+        if (m2 == 1) return;
+        src = out;
+        m = m2;
+    }
+}
+
+}  // namespace
+
+extern "C" {
+
+int lo_nb_labels(lo_ctx *ctx, const lo_table *y, int64_t n, double *labels_out, int64_t capacity, int64_t *nlabels,
+                 lo_host_timing *timing) {
+    LO_TRY(check_ctx(ctx));
+    if (n < 0) return fail(LO_ERR_INVALID, "n = %lld is negative", (long long)n);
+    LO_TRY(check_nb_table(ctx, y, 0, n, "y"));
+    LO_TRY(check_ndistinct(capacity, nlabels));
+    if (n == 0) return LO_OK;
+    if (capacity > 0 && !labels_out) return fail(LO_ERR_INVALID, "labels_out is NULL");
+    HostCall c(ctx, "nb_labels");
+    const double *d_val = (const double *)y->base;
+    if (y->dtype == LO_F32) {
+        double *wide = nullptr;
+        c.alloc(&wide, (size_t)n * 8);
+        c.launch(1, [&] { lo::k_nb_widen<<<grid_for(ctx, n), 256, 0, c.s>>>((const float *)y->base, n, wide); });
+        d_val = wide;
+    }
+    std::vector<uint64_t> counts((size_t)capacity);
+    LO_TRY(value_counts_f64_tail(c, d_val, n, labels_out, counts.data(), capacity, nlabels, timing));
+    std::sort(labels_out, labels_out + *nlabels, [](double a, double b) { return a < b || (b != b && a == a); });
+    if (*nlabels > 0 && labels_out[*nlabels - 1] != labels_out[*nlabels - 1])
+        return fail(LO_ERR_INVALID, "a label is NaN");
+    return LO_OK;
+}
+
+int lo_nb_fit(lo_ctx *ctx, const lo_table *x, int64_t ld, int32_t k, const lo_table *y, int64_t n, const double *classes,
+              int32_t nclasses, double *sums_out, int64_t *counts_out, lo_nb_info *info, lo_host_timing *timing) {
+    LO_TRY(check_ctx(ctx));
+    if (!info) return fail(LO_ERR_INVALID, "info is NULL");
+    *info = lo_nb_info{-1, -1, 0};
+    if (!y) return fail(LO_ERR_INVALID, "y is NULL");
+    LO_TRY(check_nb_matrix(ctx, x, ld, k, n, y));
+    LO_TRY(check_nb_caps(nclasses, k));
+    int direct = 0;
+    LO_TRY(check_nb_classes(classes, nclasses, "classes", &direct));
+    if (!sums_out || !counts_out) return fail(LO_ERR_INVALID, "sums_out or counts_out is NULL");
+    const int32_t C = nclasses;
+    const size_t slots = (size_t)C * k;
+    std::fill(sums_out, sums_out + slots, 0.0);
+    std::fill(counts_out, counts_out + C, (int64_t)0);
+    HostCall c(ctx, "nb_fit");
+    if (n == 0) return c.finish(timing);
+    // a 16-byte load per row and column group when every row starts 16-byte aligned; row groups as many as fit 256
+    // threads and the copies' budget.  Column j of a class row at nb_col(j) (kp per row); the copy stride = 2 mod 16
+    // doubles, so a warp's row groups and column groups use different banks.
+    const size_t esz = x->dtype == LO_F32 ? 4 : 8;
+    const int vw = (uintptr_t)x->base % 16 == 0 && (ld * (int64_t)esz) % 16 == 0 ? (int)(16 / esz) : 1;
+    const int Q = (k + vw - 1) / vw, kp = lo::nb_col(Q * vw - 1) + 1;
+    const int stride = C * kp + (int)(((2 - (int64_t)C * kp) % 16 + 16) % 16);
+    int G = Q >= lo::kNbThreads ? 1 : lo::kNbThreads / Q;
+    G = std::max(1, std::min<int>(G, lo::kNbSumsSmem / (stride * 8)));
+    const int smem = G * stride * 8 + C * 8 + C * 4;
+    const int shape[5] = {G, Q, kp, stride, vw};
+    // Rows go in windows whose CTAs' partials fit kNbPartialBytes; each window's partials, then the windows' sums, are
+    // added by the k_nb_reduce tree.  A sum thus takes at most kNbRun adds in a thread, 16 + G / 16 over the row groups
+    // and kNbFan per tree level.
+    const int64_t per_cta = (int64_t)G * lo::kNbRun;
+    const int64_t wct = std::max<int64_t>(1, std::min<int64_t>(1 << 20, lo::kNbPartialBytes / (int64_t)(slots * 8)));
+    const int64_t wrows = wct * per_cta, nw = (n + wrows - 1) / wrows;
+    const int64_t nct = std::min(wct, (n + per_cta - 1) / per_cta);
+    const int64_t level1 = (std::max(nct, nw) + lo::kNbFan - 1) / lo::kNbFan;
+    double *d_cls = nullptr, *partial = nullptr, *wins = nullptr, *sums = nullptr, *buf[2] = {nullptr, nullptr};
+    unsigned long long *counts = nullptr, *err = nullptr;
+    c.alloc(&d_cls, (size_t)C * 8);
+    c.alloc(&partial, (size_t)nct * slots * 8);
+    c.alloc(&wins, (size_t)nw * slots * 8);
+    c.alloc(&buf[0], (size_t)level1 * slots * 8);
+    c.alloc(&buf[1], (size_t)level1 * slots * 8);
+    c.alloc(&sums, slots * 8);
+    c.alloc(&counts, (size_t)C * 8);
+    c.alloc(&err, 8);
+    c.to_dev(d_cls, classes, (size_t)C * 8);
+    c.memset(counts, 0, (size_t)C * 8);
+    c.memset(err, 0xFF, 8);
+    c.mark();
+    for (int64_t w = 0; w < nw; ++w) {
+        const int64_t r0 = w * wrows, r1 = std::min(n, r0 + wrows);
+        if (x->dtype == LO_F32)
+            launch_nb_sums<float>(c, x, ld, k, y, r0, r1, d_cls, C, direct, partial, counts, err, shape, smem);
+        else
+            launch_nb_sums<double>(c, x, ld, k, y, r0, r1, d_cls, C, direct, partial, counts, err, shape, smem);
+        nb_tree(c, partial, (r1 - r0 + per_cta - 1) / per_cta, slots, wins + (size_t)w * slots, buf);
+    }
+    nb_tree(c, wins, nw, slots, sums, buf);
+    c.mark();
+    unsigned long long key = ~0ull;
+    c.to_host(sums_out, sums, slots * 8);
+    c.to_host(counts_out, counts, (size_t)C * 8);
+    c.to_host(&key, err, 8);
+    LO_TRY(c.finish(timing));
+    if (key != ~0ull) {
+        std::fill(sums_out, sums_out + slots, 0.0);
+        std::fill(counts_out, counts_out + C, (int64_t)0);
+        return nb_bad_row(info, key, k, "classes");
+    }
+    return LO_OK;
+}
+
+int lo_nb_predict(lo_ctx *ctx, const lo_table *x, int64_t ld, int32_t k, int64_t n, const double *pi, const double *theta,
+                  int32_t nclasses, lo_table *prob, lo_table *raw, lo_table *pred, const lo_table *y,
+                  const double *eval_labels, int32_t neval, int64_t *confusion_out, lo_nb_info *info,
+                  lo_host_timing *timing) {
+    LO_TRY(check_ctx(ctx));
+    if (!info) return fail(LO_ERR_INVALID, "info is NULL");
+    *info = lo_nb_info{-1, -1, 0};
+    const bool eval = confusion_out != nullptr;
+    if (eval && !y) return fail(LO_ERR_INVALID, "evaluate needs y");
+    LO_TRY(check_nb_matrix(ctx, x, ld, k, n, eval ? y : nullptr));
+    LO_TRY(check_nb_caps(nclasses, k));
+    if (!pi || !theta) return fail(LO_ERR_INVALID, "pi or theta is NULL");
+    const int32_t C = nclasses;
+    int direct = 0;
+    if (eval) {
+        if (prob || raw || pred) return fail(LO_ERR_INVALID, "evaluate writes no rows: prob, raw and pred must be NULL");
+        LO_TRY(check_nb_classes(eval_labels, neval, "eval_labels", &direct));
+        std::fill(confusion_out, confusion_out + (size_t)neval * C, (int64_t)0);
+    } else {
+        if (y || eval_labels) return fail(LO_ERR_INVALID, "y and eval_labels go with confusion_out");
+        if (n > 0 && C > INT64_MAX / 8 / n) return fail(LO_ERR_INVALID, "n * C overflows");
+        LO_TRY(check_nb_table(ctx, prob, LO_F64, n * C, "prob"));
+        LO_TRY(check_nb_table(ctx, pred, LO_F64, n, "pred"));
+        if (raw) LO_TRY(check_nb_table(ctx, raw, LO_F64, n * C, "raw"));
+    }
+    HostCall c(ctx, eval ? "nb_evaluate" : "nb_predict");
+    if (n == 0) return c.finish(timing);
+    // theta j-major for the blocks of classes; raws and the histogram in shared memory when they fit beside the tables
+    std::vector<double> theta_t((size_t)k * C);
+    for (int32_t cc = 0; cc < C; ++cc)
+        for (int32_t j = 0; j < k; ++j) theta_t[(size_t)j * C + cc] = theta[(size_t)cc * k + j];
+    const int64_t base = ((int64_t)k * C + C + lo::kNbTile * (lo::kNbChunk + 1) + (eval ? neval : 0)) * 8;
+    const int64_t raws_bytes = (int64_t)C * lo::kNbTile * 8, hist_bytes = eval ? (int64_t)neval * C * 4 : 0;
+    const bool raws_smem = base + raws_bytes <= lo::kNbSmemMax;
+    const int64_t with_raws = base + (raws_smem ? raws_bytes : 0);
+    const bool hist_smem = eval && with_raws + hist_bytes <= lo::kNbSmemMax;
+    const int smem = (int)(with_raws + (hist_smem ? hist_bytes : 0));
+    double *d_theta = nullptr, *d_pi = nullptr, *d_evl = nullptr, *raws = nullptr;
+    unsigned long long *conf = nullptr, *err = nullptr;
+    c.alloc(&d_theta, theta_t.size() * 8);
+    c.alloc(&d_pi, (size_t)C * 8);
+    c.to_dev(d_theta, theta_t.data(), theta_t.size() * 8);
+    c.to_dev(d_pi, pi, (size_t)C * 8);
+    if (eval) {
+        c.alloc(&d_evl, (size_t)neval * 8);
+        c.alloc(&conf, (size_t)neval * C * 8);
+        c.alloc(&err, 8);
+        c.to_dev(d_evl, eval_labels, (size_t)neval * 8);
+        c.memset(conf, 0, (size_t)neval * C * 8);
+        c.memset(err, 0xFF, 8);
+    }
+    auto go = [&](auto kernel, auto tag) {
+        using T = decltype(tag);
+        int per_sm = 0;
+        c.run([&] { return cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem); });
+        c.run([&] { return cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, lo::kNbTile, smem); });
+        const int64_t ntiles = (n + lo::kNbTile - 1) / lo::kNbTile;
+        const int grid = (int)std::min<int64_t>(ntiles, (int64_t)ctx->sm_count * std::max(1, per_sm));
+        if (!raws_smem) c.alloc(&raws, (size_t)grid * raws_bytes);
+        c.mark();
+        c.launch(1, [&] {
+            kernel<<<grid, lo::kNbTile, smem, c.s>>>((const T *)x->base, ld, k, n, d_theta, d_pi, C,
+                                                     prob ? (double *)prob->base : nullptr, raw ? (double *)raw->base : nullptr,
+                                                     pred ? (double *)pred->base : nullptr, y ? (const T *)y->base : nullptr,
+                                                     d_evl, neval, direct, conf, raws, hist_smem ? 1 : 0, err);
+        });
+        c.mark();
+    };
+    if (x->dtype == LO_F32) {
+        if (eval) go(lo::k_nb_predict<float, true>, 0.0f); else go(lo::k_nb_predict<float, false>, 0.0f);
+    } else {
+        if (eval) go(lo::k_nb_predict<double, true>, 0.0); else go(lo::k_nb_predict<double, false>, 0.0);
+    }
+    unsigned long long key = ~0ull;
+    if (eval) {
+        c.to_host(confusion_out, conf, (size_t)neval * C * 8);
+        c.to_host(&key, err, 8);
+    }
+    LO_TRY(c.finish(timing));
+    if (key != ~0ull) {
+        std::fill(confusion_out, confusion_out + (size_t)neval * C, (int64_t)0);
+        return nb_bad_row(info, key, k, "evaluated labels");
+    }
     return LO_OK;
 }
 

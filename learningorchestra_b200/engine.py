@@ -321,6 +321,29 @@ class AssembledRows:
                 t.free()
 
 
+class PredictedRows:
+    """What :meth:`Engine.nb_predict` wrote for one device's rows: ``prob`` (n x C f64, row-major), ``pred`` (n f64 class
+    indices) and ``raw`` (n x C f64, or None).  :meth:`probability` / :meth:`prediction` / :meth:`raw_view` view them in
+    place; :meth:`free` frees every table and may be called again."""
+
+    def __init__(self, prob: "DeviceTable", raw: "DeviceTable | None", pred: "DeviceTable", n: int, nclasses: int):
+        self.prob, self.raw, self.pred, self.n, self.nclasses = prob, raw, pred, int(n), int(nclasses)
+
+    def probability(self, keepalive=None) -> DeviceArray:
+        return DeviceArray(self.prob, (self.n, self.nclasses), keepalive)
+
+    def prediction(self, keepalive=None) -> DeviceArray:
+        return DeviceArray(self.pred, (self.n,), keepalive)
+
+    def raw_view(self, keepalive=None) -> DeviceArray | None:
+        return None if self.raw is None else DeviceArray(self.raw, (self.n, self.nclasses), keepalive)
+
+    def free(self) -> None:
+        for t in (self.prob, self.raw, self.pred):
+            if t is not None:
+                t.free()
+
+
 ASSEMBLE_MODES = {"error": N.LO_INVALID_ERROR, "skip": N.LO_INVALID_SKIP, "keep": N.LO_INVALID_KEEP}
 ASSEMBLE_DTYPES = {"float32": "f32", "float64": "f64"}
 
@@ -917,6 +940,97 @@ class Engine:
         if timing is not None:
             timing.update(_timing(t), kernel_ms=t.kernel_ms)
         return AssembledRows(x, y, rows[:info.nkept] if rows is not None else None, k, info.nkept), None
+
+    def nb_labels(self, part: AssembledRows) -> np.ndarray:
+        """The distinct label values of ``part`` (an :class:`AssembledRows` with ``y``), ascending, -0.0 as 0.0
+        (``lo_nb_labels``: the f64 group-by on the device).  A NaN label, or more than LO_NB_MAX_CLASSES values, raise
+        LoexecError LO_ERR_INVALID."""
+        if part.y is None:
+            raise ValueError("the rows have no label")
+        out = np.empty(N.LO_NB_MAX_CLASSES, np.float64)
+        nd, t = C.c_int64(), N.HostTiming()
+        N.check(self._lib.lo_nb_labels(self._ctx, part.y._h, part.nkept, out.ctypes.data_as(C.c_void_p), len(out),
+                                       C.byref(nd), C.byref(t)))
+        return out[:nd.value].copy()
+
+    def nb_fit(self, part: AssembledRows, classes, timing: dict | None = None) -> tuple[np.ndarray, np.ndarray]:
+        """(sums float64[C, k], counts int64[C]) of multinomial NaiveBayes over ``part`` (``lo_nb_fit``): counts[c] the
+        rows labelled classes[c], sums[c, j] the f64 sum of feature j over them, in a fixed order.  A negative or NaN
+        feature, or a label that is no class, raises :class:`InvalidCellError` naming the lowest row (``position`` the
+        feature; k: the label).  ``timing``: a dict to receive the call's lo_host_timing fields."""
+        res, bad = self._nb_fit(part, classes, timing)
+        if bad is not None:
+            raise InvalidCellError(*bad)
+        return res
+
+    def _nb_fit(self, part, classes, timing=None):
+        """(result, None), or (None, (row, position, message)): :meth:`nb_fit` without raising, for the shards."""
+        if part.y is None:
+            raise ValueError("the rows have no label")
+        cls = np.ascontiguousarray(classes, dtype=np.float64)
+        sums = np.zeros((len(cls), part.k), np.float64)
+        counts = np.zeros(len(cls), np.int64)
+        info, t = N.NbInfo(), N.HostTiming()
+        rc = self._lib.lo_nb_fit(self._ctx, part.x._h, part.k, part.k, part.y._h, part.nkept, cls.ctypes.data_as(C.c_void_p),
+                                 len(cls), sums.ctypes.data_as(C.c_void_p), counts.ctypes.data_as(C.c_void_p),
+                                 C.byref(info), C.byref(t))
+        if rc == N.LO_ERR_INVALID and info.bad_row >= 0:
+            return None, (int(info.bad_row), int(info.bad_col), self._lib.lo_last_error().decode("utf-8", "replace"))
+        N.check(rc)
+        if timing is not None:
+            timing.update(_timing(t), kernel_ms=t.kernel_ms)
+        return (sums, counts), None
+
+    def nb_predict(self, part: AssembledRows, pi, theta, raw: bool = False, labels=None, timing: dict | None = None):
+        """A NaiveBayes model (``pi`` float64[C], ``theta`` float64[C, k]) over ``part`` (``lo_nb_predict``).
+        ``labels`` None: transform — a :class:`PredictedRows` with every row's probability and prediction (and raw
+        values with ``raw``).  ``labels`` the ascending label values to count: evaluate — the int64[len(labels), C]
+        confusion counts of (label, prediction index), nothing written per row; a label not in ``labels`` raises
+        :class:`InvalidCellError`.  ``timing``: a dict to receive the call's lo_host_timing fields."""
+        res, bad = self._nb_predict(part, pi, theta, raw, labels, timing)
+        if bad is not None:
+            raise InvalidCellError(*bad)
+        return res
+
+    def _nb_predict(self, part, pi, theta, raw=False, labels=None, timing=None):
+        pi = np.ascontiguousarray(pi, dtype=np.float64)
+        theta = np.ascontiguousarray(theta, dtype=np.float64)
+        nc, n = len(pi), part.nkept
+        if theta.shape != (nc, part.k):
+            raise ValueError(f"theta has shape {theta.shape}, ({nc}, {part.k}) expected")
+        info, t = N.NbInfo(), N.HostTiming()
+        args = (self._ctx, part.x._h, part.k, part.k, n, pi.ctypes.data_as(C.c_void_p), theta.ctypes.data_as(C.c_void_p), nc)
+        if labels is not None:
+            if part.y is None:
+                raise ValueError("the rows have no label")
+            lab = np.ascontiguousarray(labels, dtype=np.float64)
+            conf = np.zeros((len(lab), nc), np.int64)
+            rc = self._lib.lo_nb_predict(*args, None, None, None, part.y._h, lab.ctypes.data_as(C.c_void_p), len(lab),
+                                         conf.ctypes.data_as(C.c_void_p), C.byref(info), C.byref(t))
+            if rc == N.LO_ERR_INVALID and info.bad_row >= 0:
+                return None, (int(info.bad_row), int(info.bad_col), self._lib.lo_last_error().decode("utf-8", "replace"))
+            N.check(rc)
+            if timing is not None:
+                timing.update(_timing(t), kernel_ms=t.kernel_ms)
+            return conf, None
+        tables = []
+        try:
+            prob = self.table("f64", n * nc, 1)
+            tables.append(prob)
+            pred = self.table("f64", n, 1)
+            tables.append(pred)
+            rawt = self.table("f64", n * nc, 1) if raw else None
+            if rawt is not None:
+                tables.append(rawt)
+            N.check(self._lib.lo_nb_predict(*args, prob._h, rawt._h if rawt is not None else None, pred._h, None, None, 0,
+                                            None, C.byref(info), C.byref(t)))
+        except BaseException:
+            for tb in tables:
+                tb.free()
+            raise
+        if timing is not None:
+            timing.update(_timing(t), kernel_ms=t.kernel_ms)
+        return PredictedRows(prob, rawt, pred, n, nc), None
 
     def value_counts_f64_host(self, values: np.ndarray):
         """(keys float64[g], counts uint64[g]) — exact value counts of a numeric column (GPU hash group-by),

@@ -725,6 +725,63 @@ class ShardedEngine:
             rows.first = off
         return [rows for rows, _b in parts]
 
+    def nb_labels(self, parts) -> "np.ndarray":
+        """``Engine.nb_labels`` over the shards' ``AssembledRows`` (one per local member, as :meth:`assemble_rows` made
+        them): every member groups its own labels on its own device, from a host thread of its own; the union, ascending."""
+        import numpy as np
+        self._every_row("nb_labels")
+        got = on_each(self.nlocal, lambda i: self.engines[i].nb_labels(parts[i]))
+        labels = np.unique(np.concatenate(got)) if got else np.zeros(0)
+        if len(labels) > self._N.LO_NB_MAX_CLASSES:
+            raise self._N.LoexecError(self._N.LO_ERR_INVALID, f"{len(labels)} distinct labels: at most "
+                                      f"{self._N.LO_NB_MAX_CLASSES} classes")
+        return labels
+
+    def nb_fit(self, parts, classes):
+        """``Engine.nb_fit`` over the shards: each member sums its own rows over the same ``classes`` on its own device;
+        the sums and counts are added on the host in shard order, so integer-valued features give the single-GPU sums
+        bit for bit.  A refused row is raised as the lowest over all shards, its row global (rows of the earlier shards
+        counted first)."""
+        self._every_row("nb_fit")
+        got = on_each(self.nlocal, lambda i: self.engines[i]._nb_fit(parts[i], classes))
+        self._raise_lowest(parts, [b for _r, b in got])
+        sums, counts = got[0][0]
+        for (s, c), _b in got[1:]:
+            sums, counts = sums + s, counts + c
+        return sums, counts
+
+    def nb_predict(self, parts, pi, theta, raw: bool = False, labels=None):
+        """``Engine.nb_predict`` over the shards, each on its own device from a host thread of its own.  Transform: one
+        ``PredictedRows`` per member.  Evaluate (``labels``): the members' confusion counts summed."""
+        self._every_row("nb_predict")
+        got = on_each(self.nlocal, lambda i: self.engines[i]._nb_predict(parts[i], pi, theta, raw, labels),
+                      undo=lambda r: r[0] is not None and labels is None and r[0].free())
+        try:
+            self._raise_lowest(parts, [b for _r, b in got])
+        except BaseException:
+            for r, _b in got:
+                if r is not None and labels is None:
+                    r.free()
+            raise
+        if labels is not None:
+            confusion = got[0][0]
+            for r, _b in got[1:]:
+                confusion = confusion + r
+            return confusion
+        return [r for r, _b in got]
+
+    @staticmethod
+    def _raise_lowest(parts, bad) -> None:
+        """InvalidCellError for the lowest of the shards' refused rows (each shard's row made global), if any."""
+        from .engine import InvalidCellError
+        first, hits = 0, []
+        for p, b in zip(parts, bad):
+            if b is not None:
+                hits.append((first + b[0], b[1], b[2]))
+            first += p.nkept
+        if hits:
+            raise InvalidCellError(*min(hits))
+
     @property
     def resident(self):
         """Datasets kept in HBM between requests, rows sharded over the group (:mod:`table_cache`)."""

@@ -16,6 +16,11 @@ features_log="$(mktemp -d)/sanitizer_memcheck_features.txt"
 timeout 900 compute-sanitizer --tool memcheck --error-exitcode 1 python -m pytest tests/test_gpu_features.py -q \
     > "$features_log" 2>&1
 echo "memcheck (features) rc=$? log=$features_log"; tail -3 "$features_log"
+# memcheck of the NaiveBayes kernels (fit, transform, evaluate; every shape, cap and refusal); its log goes to a temporary directory
+nb_log="$(mktemp -d)/sanitizer_memcheck_naive_bayes.txt"
+timeout 1800 compute-sanitizer --tool memcheck --error-exitcode 1 python -m pytest tests/test_gpu_naive_bayes.py -q \
+    > "$nb_log" 2>&1
+echo "memcheck (naive bayes) rc=$? log=$nb_log"; tail -3 "$nb_log"
 # memcheck of the number parser and the resident formatter on every entry point, without the million-row cases: a read
 # past the last staged cell shows here (the CPU harness puts a NUL after it)
 parse_log="$(mktemp -d)/sanitizer_memcheck_parse.txt"
