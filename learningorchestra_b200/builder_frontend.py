@@ -84,6 +84,7 @@ class DeviceFrame:
         the ``_id`` and field of the lowest one, "skip" drops every row with one in ``fields`` or ``label``, "keep" writes
         NaN.  A field not in the frame raises KeyError before anything runs."""
         from .engine import InvalidCellError, assemble_args
+        from .sharding import ShardedEngine
         assemble_args(handle_invalid, dtype)
         fields = [f for f in self.fields if f != label] if fields is None else list(fields)
         for f in fields + ([label] if label is not None else []):
@@ -98,11 +99,8 @@ class DeviceFrame:
             parts = engine.assemble_rows([self._source(f) for f in fields],
                                          self._source(label) if label is not None else None, dtype, handle_invalid)
         except InvalidCellError as e:
-            name = label if e.position == len(fields) else fields[e.position]
-            raise InvalidCellError(e.row, e.position,
-                                   f"features: field {name!r} of the row with _id {self.ids[e.row]} is null or NaN "
-                                   f"(handle_invalid='error')") from None
-        return Features(self, parts if isinstance(parts, list) else [parts], fields, label, dtype)
+            raise named_cell(e, fields, label, self.ids, "features", ("is null or NaN (handle_invalid='error')",) * 2) from None
+        return Features(self, parts if isinstance(engine, ShardedEngine) else [parts], fields, label, dtype)
 
     def _source(self, f):
         """(table, column) of field f as ``assemble_rows`` reads it: its code table, or the dataset's slab table."""
@@ -123,6 +121,16 @@ class DeviceFrame:
 
     def __exit__(self, *exc):
         self.release()
+
+
+def named_cell(e, fields, label, ids, call: str, reasons: tuple[str, str]):
+    """A refused cell ``e`` (an :class:`~engine.InvalidCellError` whose row indexes ``ids`` and whose position indexes
+    ``fields``, ``len(fields)`` the label) restated for the user: "<call>: field F of the row with _id I <reason>",
+    ``reasons[0]`` for a feature, ``reasons[1]`` for the label.  ``row`` and ``position`` stay."""
+    from .engine import InvalidCellError
+    is_label = e.position == len(fields)
+    name = label if is_label else fields[e.position]
+    return InvalidCellError(e.row, e.position, f"{call}: field {name!r} of the row with _id {ids[e.row]} {reasons[is_label]}")
 
 
 class Features:

@@ -12,22 +12,22 @@ import numpy as np
 from . import _native as N
 
 
-def _engine(features):
-    return features._frame._cache.engine
-
-
-def _sharded(engine) -> bool:
-    from .sharding import ShardedEngine
-    return isinstance(engine, ShardedEngine)
-
-
-def _raise_named(features, e):
-    """The device's refused row (a row of the features, shards concatenated) as the ``_id`` and field it holds."""
+def _on_device(features, call, per_part: bool = False):
+    """``call(engine, rows)`` on the features' engine: a ShardedEngine takes every shard's rows and gives one result per
+    shard where it gives one per row (``per_part``); an Engine takes its one part, and its result is made a list of one
+    where ``per_part``.  A refused cell (its row a row of the features, shards concatenated) is raised as the ``_id``
+    and field it holds."""
+    from .builder_frontend import named_cell
     from .engine import InvalidCellError
-    name = features.label if e.position == len(features.fields) else features.fields[e.position]
-    what = "is not a class of the model" if e.position == len(features.fields) else "is negative or NaN"
-    raise InvalidCellError(e.row, e.position, f"NaiveBayes: field {name!r} of the row with _id "
-                           f"{features.row_ids[e.row]} {what}") from None
+    from .sharding import ShardedEngine
+    engine = features._frame._cache.engine
+    sharded = isinstance(engine, ShardedEngine)
+    try:
+        out = call(engine, features._parts if sharded else features._parts[0])
+    except InvalidCellError as e:
+        raise named_cell(e, features.fields, features.label, features.row_ids, "NaiveBayes",
+                         ("is negative or NaN", "is not a class of the model")) from None
+    return [out] if per_part and not sharded else out
 
 
 def _usable(features) -> None:
@@ -41,10 +41,7 @@ def _labels(features) -> np.ndarray:
     _usable(features)
     if features.label is None:
         raise ValueError("NaiveBayes needs features with a label")
-    engine = _engine(features)
-    if _sharded(engine):
-        return engine.nb_labels(features._parts)
-    return engine.nb_labels(features._parts[0])
+    return _on_device(features, lambda engine, rows: engine.nb_labels(rows))
 
 
 def model_arrays(sums: np.ndarray, counts: np.ndarray, smoothing: float) -> tuple[np.ndarray, np.ndarray]:
@@ -76,7 +73,6 @@ class NaiveBayes:
         classes are the distinct label values, ascending; a NaN label, more than LO_NB_MAX_CLASSES of them, C x k above
         LO_NB_MAX_THETA or no row at all are refused, and so is a negative or NaN feature (InvalidCellError naming the
         ``_id`` and field of the lowest such row)."""
-        from .engine import InvalidCellError
         classes = _labels(features)
         if len(features.row_ids) == 0:
             raise N.LoexecError(N.LO_ERR_INVALID, "NaiveBayes needs at least one row")
@@ -84,14 +80,7 @@ class NaiveBayes:
         if len(classes) * k > N.LO_NB_MAX_THETA:
             raise N.LoexecError(N.LO_ERR_INVALID, f"{len(classes)} classes x {k} features exceed LO_NB_MAX_THETA = "
                                 f"{N.LO_NB_MAX_THETA}")
-        engine = _engine(features)
-        try:
-            if _sharded(engine):
-                sums, counts = engine.nb_fit(features._parts, classes)
-            else:
-                sums, counts = engine.nb_fit(features._parts[0], classes)
-        except InvalidCellError as e:
-            _raise_named(features, e)
+        sums, counts = _on_device(features, lambda engine, rows: engine.nb_fit(rows, classes))
         pi, theta = model_arrays(sums, counts, self.smoothing)
         return NaiveBayesModel(classes, pi, theta, features.fields, sums, counts)
 
@@ -114,31 +103,20 @@ class NaiveBayesModel:
         with ``raw`` its ``rawPrediction``, written in HBM on the rows' own devices."""
         _usable(features)
         self._check(features)
-        engine = _engine(features)
-        if _sharded(engine):
-            parts = engine.nb_predict(features._parts, self.pi, self.theta, raw=raw)
-        else:
-            parts = [engine.nb_predict(features._parts[0], self.pi, self.theta, raw=raw)]
+        parts = _on_device(features, lambda engine, rows: engine.nb_predict(rows, self.pi, self.theta, raw=raw),
+                           per_part=True)
         return Predictions(features, parts)
 
     def evaluate(self, features) -> dict:
         """``MulticlassClassificationEvaluator`` f1 and accuracy over ``transform(features)`` (builder.py:124-142), as one
         fused pass per device that writes nothing per row: ``{"f1", "accuracy", "labels", "confusion"}`` where
         ``confusion[a, p]`` counts the rows labelled ``labels[a]`` predicted as class index p."""
-        from .engine import InvalidCellError
         _usable(features)
         self._check(features)
         labels = _labels(features)
         if len(features.row_ids) == 0:
             raise N.LoexecError(N.LO_ERR_INVALID, "evaluate needs at least one row")
-        engine = _engine(features)
-        try:
-            if _sharded(engine):
-                confusion = engine.nb_predict(features._parts, self.pi, self.theta, labels=labels)
-            else:
-                confusion = engine.nb_predict(features._parts[0], self.pi, self.theta, labels=labels)
-        except InvalidCellError as e:
-            _raise_named(features, e)
+        confusion = _on_device(features, lambda engine, rows: engine.nb_predict(rows, self.pi, self.theta, labels=labels))
         f1, accuracy = metrics(labels, confusion)
         return {"f1": f1, "accuracy": accuracy, "labels": labels, "confusion": confusion}
 

@@ -1537,17 +1537,36 @@ __global__ void k_parse_number(const uint8_t *__restrict__ chars, const long lon
     }
 }
 
-// The same parse written straight into one f64 table column (a text field binned or cast without /fieldTypes): cell i
-// is chars[offsets[i] - offsets[0] ..) — the offsets of a sliced Arrow array are rebased here — and lands in col[i] as
-// the bits float() returns; a null cell (mask byte 0, or bitmap bit (bit0 + i) clear) and "" store the canonical NaN.
-// Instead of a status per row the call reduces summary[4] = {first invalid row, first unsupported row (both start at
-// ~0, atomicMin), null + empty cells, cells that are valid but not integer valued} per warp, then one atomic each.
+// The least of a warp's 64-bit values, in every lane.
 __device__ __forceinline__ unsigned long long warp_min_u64(unsigned long long v) {
 #pragma unroll
     for (int s = 16; s > 0; s >>= 1) v = min(v, __shfl_xor_sync(0xffffffffu, v, s));
     return v;
 }
 
+// A refused cell of the feature matrix (k_assemble_rows, k_nb_sums, k_nb_predict): cell (row, col) of k features and
+// the label (col k) has key row * (k + 1) + col, so the lowest key is the lowest row's lowest column.  A kernel keeps
+// the least key a thread met, starting at ~0, and report_cell gives the warp's least to *err with one atomicMin;
+// cell_of_key gives the host the cell back.
+__device__ __forceinline__ unsigned long long cell_key(long long row, int k, int col) {
+    return (unsigned long long)row * (unsigned long long)(k + 1) + (unsigned)col;
+}
+
+__device__ __forceinline__ void report_cell(unsigned long long key, unsigned long long *err) {
+    key = warp_min_u64(key);
+    if ((threadIdx.x & 31) == 0 && key != ~0ull) atomicMin(err, key);
+}
+
+inline void cell_of_key(unsigned long long key, int k, int64_t *row, int32_t *col) {
+    *row = (int64_t)(key / (unsigned long long)(k + 1));
+    *col = (int32_t)(key % (unsigned long long)(k + 1));
+}
+
+// The same parse written straight into one f64 table column (a text field binned or cast without /fieldTypes): cell i
+// is chars[offsets[i] - offsets[0] ..) — the offsets of a sliced Arrow array are rebased here — and lands in col[i] as
+// the bits float() returns; a null cell (mask byte 0, or bitmap bit (bit0 + i) clear) and "" store the canonical NaN.
+// Instead of a status per row the call reduces summary[4] = {first invalid row, first unsupported row (both start at
+// ~0, atomicMin), null + empty cells, cells that are valid but not integer valued} per warp, then one atomic each.
 __global__ void __launch_bounds__(128) k_parse_number_to_col(const uint8_t *__restrict__ chars, const long long *__restrict__ offsets,
                                                              long long n, const uint8_t *__restrict__ mask,
                                                              const uint8_t *__restrict__ bitmap, int bit0,
@@ -1805,7 +1824,7 @@ __global__ void __launch_bounds__(kAsmThreads) k_assemble_valid(const AsmSrc *__
 
 // The write pass: the rows of tile blockIdx.x, columns [32 blockIdx.y, + 32) of the k sources, into x (row stride ld),
 // the label into y and (SKIP) the kept rows' source rows into kept_rows, by chunk 0.  !SKIP: row r goes to row r and, with
-// err, the lowest invalid cell's key row * (k + 1) + source (k: the label) is kept in *err.  SKIP: the tile's kept rows
+// err, the lowest invalid cell's key cell_key(row, k, source) (source k: the label) is kept in *err.  SKIP: the tile's kept rows
 // (keep_bits) go to rows tile_off[t] .. tile_off[t + 1] in order.
 template <typename T, bool SKIP>
 __global__ void __launch_bounds__(kAsmThreads) k_assemble_rows(const AsmSrc *__restrict__ src, int k, AsmSrc label,
@@ -1865,7 +1884,7 @@ __global__ void __launch_bounds__(kAsmThreads) k_assemble_rows(const AsmSrc *__r
             } else {
                 tile[r][cc] = v;
                 if (err && asm_bad(word, s[i].i32))
-                    bad_key = min(bad_key, (unsigned long long)(row0 + r) * (unsigned long long)(k + 1) + (unsigned)(c0 + cc));
+                    bad_key = min(bad_key, cell_key(row0 + r, k, c0 + cc));
             }
         }
     }
@@ -1877,14 +1896,11 @@ __global__ void __launch_bounds__(kAsmThreads) k_assemble_rows(const AsmSrc *__r
                                                       : ldg_u64_stream(reinterpret_cast<const unsigned long long *>(label.p) + row0 + r, pol);
             if (o >= 0) y[o] = asm_value(word, label.i32, T());
             if (!SKIP && err && asm_bad(word, label.i32))
-                bad_key = min(bad_key, (unsigned long long)(row0 + r) * (unsigned long long)(k + 1) + (unsigned)k);
+                bad_key = min(bad_key, cell_key(row0 + r, k, k));
         }
         if (SKIP && kept_rows && o >= 0) kept_rows[o] = row0 + r;
     }
-    if (!SKIP && err) {
-        bad_key = warp_min_u64(bad_key);
-        if (lane == 0 && bad_key != ~0ull) atomicMin(err, bad_key);
-    }
+    if (!SKIP && err) report_cell(bad_key, err);
     __syncthreads();
     T *base = x + out0 * ld + c0;
     if (kc == ld) {                               // whole rows: the tile's output is one span of nout * kc elements

@@ -2450,13 +2450,41 @@ int check_assemble_src(const lo_ctx *ctx, const lo_table *t, int32_t col, int64_
     return LO_OK;
 }
 
-int check_assemble_out(const lo_ctx *ctx, const lo_table *t, int dtype, int64_t need, const char *name) {
-    if (t->dtype != dtype) return fail(LO_ERR_INVALID, "%s must be %s", name, dtype == LO_F32 ? "LO_F32" : "LO_F64");
+// an LO_F32 / LO_F64 table of the feature-matrix calls: NULL, dtype (0: either float dtype), device and size checked
+int check_float_table(const lo_ctx *ctx, const lo_table *t, int dtype, int64_t need, const char *name) {
+    if (!t) return fail(LO_ERR_INVALID, "%s is NULL", name);
+    if (dtype ? t->dtype != dtype : t->dtype != LO_F32 && t->dtype != LO_F64)
+        return fail(LO_ERR_INVALID, "%s must be %s (dtype %d)", name,
+                    dtype == LO_F32 ? "LO_F32" : dtype == LO_F64 ? "LO_F64" : "LO_F32 or LO_F64", t->dtype);
     if (t->device != ctx->device) return fail(LO_ERR_INVALID, "%s lives on device %d, the context on %d", name, t->device, ctx->device);
     if (t->nrows < need)
         return fail(LO_ERR_INVALID, "%s holds %lld elements, %lld needed", name, (long long)t->nrows, (long long)need);
     return LO_OK;
 }
+
+// n rows of k values at stride ld: ld >= k, n >= 0 and n * ld representable
+int check_matrix_shape(int64_t ld, int32_t k, int64_t n) {
+    if (ld < k) return fail(LO_ERR_INVALID, "ld = %lld is less than k = %d", (long long)ld, k);
+    if (n < 0) return fail(LO_ERR_INVALID, "n = %lld is negative", (long long)n);
+    if (n > 0 && ld > (INT64_MAX / 2) / n) return fail(LO_ERR_INVALID, "n * ld overflows (ld = %lld)", (long long)ld);
+    return LO_OK;
+}
+
+// The lowest refused cell of a call (lo::cell_key): a word armed to ~0 on the call's stream that the kernels lower, read
+// back with the call's outputs.  After c.finish, found() fills info's bad_row / bad_col when a cell was refused.
+struct RefusedCell {
+    unsigned long long *word = nullptr, key = ~0ull;
+    void arm(HostCall &c) {
+        c.alloc(&word, 8);
+        c.memset(word, 0xFF, 8);
+    }
+    void read(HostCall &c) { if (word) c.to_host(&key, word, 8); }
+    template <typename Info> bool found(int32_t k, Info *info) const {
+        if (key == ~0ull) return false;
+        lo::cell_of_key(key, k, &info->bad_row, &info->bad_col);
+        return true;
+    }
+};
 
 constexpr int64_t kAsmMaxK = 65535ll * lo::kAsmCols;    // chunks on the grid's y dimension
 
@@ -2497,25 +2525,22 @@ int lo_assemble_rows(lo_ctx *ctx, const lo_table *const *src, const int32_t *src
     if (label) LO_TRY(check_assemble_src(ctx, label, label_col, n, "label", &lab));
     if (!x) return fail(LO_ERR_INVALID, "x is NULL");
     if (x->dtype != LO_F32 && x->dtype != LO_F64) return fail(LO_ERR_INVALID, "x must be LO_F32 or LO_F64 (dtype %d)", x->dtype);
-    if (ld < k) return fail(LO_ERR_INVALID, "ld = %lld is less than k = %d", (long long)ld, k);
-    if (n > 0 && ld > (INT64_MAX / 2) / n) return fail(LO_ERR_INVALID, "n * ld overflows (ld = %lld)", (long long)ld);
-    LO_TRY(check_assemble_out(ctx, x, x->dtype, n * ld, "x"));
+    LO_TRY(check_matrix_shape(ld, k, n));
+    LO_TRY(check_float_table(ctx, x, x->dtype, n * ld, "x"));
     if (!label != !y) return fail(LO_ERR_INVALID, "y and label go together");
-    if (y) LO_TRY(check_assemble_out(ctx, y, x->dtype, n, "y"));
+    if (y) LO_TRY(check_float_table(ctx, y, x->dtype, n, "y"));
     HostCall c(ctx, "assemble_rows");
     if (n == 0) return c.finish(timing);
     const bool skip = mode == LO_INVALID_SKIP, err_mode = mode == LO_INVALID_ERROR;
     const int64_t ntiles = (n + lo::kAsmRows - 1) / lo::kAsmRows;
     lo::AsmSrc *d_src = nullptr;
-    unsigned long long *err = nullptr, *off = nullptr;
+    unsigned long long *off = nullptr;
     unsigned *bits = nullptr;
     long long *kept = nullptr;
+    RefusedCell bad;
     c.alloc(&d_src, (size_t)k * sizeof(lo::AsmSrc));
     c.to_dev(d_src, desc.data(), (size_t)k * sizeof(lo::AsmSrc));
-    if (err_mode) {
-        c.alloc(&err, 8);
-        c.memset(err, 0xFF, 8);
-    }
+    if (err_mode) bad.arm(c);
     void *tmp = nullptr;
     size_t tmp_bytes = 0;
     if (skip) {
@@ -2534,24 +2559,21 @@ int lo_assemble_rows(lo_ctx *ctx, const lo_table *const *src, const int32_t *src
         c.launch(1, [&] { return cub::DeviceScan::ExclusiveSum(tmp, tmp_bytes, off, ntiles + 1, c.s); });
     }
     if (x->dtype == LO_F32)
-        launch_assemble(c, skip, d_src, k, lab, n, (float *)x->base, ld, y ? (float *)y->base : nullptr, kept, bits, off, err);
+        launch_assemble(c, skip, d_src, k, lab, n, (float *)x->base, ld, y ? (float *)y->base : nullptr, kept, bits, off, bad.word);
     else
-        launch_assemble(c, skip, d_src, k, lab, n, (double *)x->base, ld, y ? (double *)y->base : nullptr, kept, bits, off, err);
+        launch_assemble(c, skip, d_src, k, lab, n, (double *)x->base, ld, y ? (double *)y->base : nullptr, kept, bits, off, bad.word);
     c.mark();
-    unsigned long long nkept = (unsigned long long)n, key = ~0ull;
+    unsigned long long nkept = (unsigned long long)n;
     if (skip) {
         c.to_host(&nkept, off + ntiles, 8);
         c.sync();
         if (kept_rows) c.to_host(kept_rows, kept, nkept * 8);
     }
-    if (err_mode) c.to_host(&key, err, 8);
+    bad.read(c);
     LO_TRY(c.finish(timing));
-    if (key != ~0ull) {
-        info->bad_row = (int64_t)(key / (unsigned long long)(k + 1));
-        info->bad_col = (int32_t)(key % (unsigned long long)(k + 1));
+    if (bad.found(k, info))
         return fail(LO_ERR_INVALID, "invalid cell (NaN or code -1) in row %lld, %s %d", (long long)info->bad_row,
                     info->bad_col == k ? "the label, source" : "source", info->bad_col);
-    }
     info->nkept = (int64_t)nkept;
     if (kept_rows && !skip)
         for (int64_t i = 0; i < n; ++i) kept_rows[i] = i;
@@ -2564,25 +2586,12 @@ static_assert(lo::kNbMaxClasses == LO_NB_MAX_CLASSES && lo::kNbMaxTheta == LO_NB
 
 namespace {
 
-// an LO_F32 / LO_F64 table of lo_nb_*: NULL, dtype (dtype 0: either float dtype), device and size checked
-int check_nb_table(const lo_ctx *ctx, const lo_table *t, int dtype, int64_t need, const char *name) {
-    if (!t) return fail(LO_ERR_INVALID, "%s is NULL", name);
-    if (dtype ? t->dtype != dtype : t->dtype != LO_F32 && t->dtype != LO_F64)
-        return fail(LO_ERR_INVALID, "%s must be %s (dtype %d)", name, dtype == LO_F64 ? "LO_F64" : "LO_F32 or LO_F64", t->dtype);
-    if (t->device != ctx->device) return fail(LO_ERR_INVALID, "%s lives on device %d, the context on %d", name, t->device, ctx->device);
-    if (t->nrows < need)
-        return fail(LO_ERR_INVALID, "%s holds %lld elements, %lld needed", name, (long long)t->nrows, (long long)need);
-    return LO_OK;
-}
-
 // the matrix x (n rows of k, stride ld) and, when given, its labels y of the same dtype
 int check_nb_matrix(const lo_ctx *ctx, const lo_table *x, int64_t ld, int32_t k, int64_t n, const lo_table *y) {
     if (k < 1) return fail(LO_ERR_INVALID, "k = %d: at least one feature", k);
-    if (ld < k) return fail(LO_ERR_INVALID, "ld = %lld is less than k = %d", (long long)ld, k);
-    if (n < 0) return fail(LO_ERR_INVALID, "n = %lld is negative", (long long)n);
-    if (n > 0 && ld > (INT64_MAX / 2) / n) return fail(LO_ERR_INVALID, "n * ld overflows (ld = %lld)", (long long)ld);
-    LO_TRY(check_nb_table(ctx, x, 0, n * ld, "x"));
-    if (y) LO_TRY(check_nb_table(ctx, y, x->dtype, n, "y"));
+    LO_TRY(check_matrix_shape(ld, k, n));
+    LO_TRY(check_float_table(ctx, x, 0, n * ld, "x"));
+    if (y) LO_TRY(check_float_table(ctx, y, x->dtype, n, "y"));
     return LO_OK;
 }
 
@@ -2605,15 +2614,6 @@ int check_nb_caps(int32_t nclasses, int32_t k) {
     if ((int64_t)nclasses * k > LO_NB_MAX_THETA)
         return fail(LO_ERR_INVALID, "%d classes x %d features exceed LO_NB_MAX_THETA = %d", nclasses, k, LO_NB_MAX_THETA);
     return LO_OK;
-}
-
-// *info and the message of a refused row (key = row * (k + 1) + column)
-int nb_bad_row(lo_nb_info *info, unsigned long long key, int32_t k, const char *what) {
-    info->bad_row = (int64_t)(key / (unsigned long long)(k + 1));
-    info->bad_col = (int32_t)(key % (unsigned long long)(k + 1));
-    if (info->bad_col == k) return fail(LO_ERR_INVALID, "row %lld: its label is not one of the %s", (long long)info->bad_row, what);
-    return fail(LO_ERR_INVALID, "row %lld, feature %d: negative or NaN (NaiveBayes needs values >= 0)",
-                (long long)info->bad_row, info->bad_col);
 }
 
 // k_nb_sums over rows [row0, row1): one CTA per G * kNbRun rows, shape = {G, Q, kp, stride, vw}
@@ -2656,7 +2656,7 @@ int lo_nb_labels(lo_ctx *ctx, const lo_table *y, int64_t n, double *labels_out, 
                  lo_host_timing *timing) {
     LO_TRY(check_ctx(ctx));
     if (n < 0) return fail(LO_ERR_INVALID, "n = %lld is negative", (long long)n);
-    LO_TRY(check_nb_table(ctx, y, 0, n, "y"));
+    LO_TRY(check_float_table(ctx, y, 0, n, "y"));
     LO_TRY(check_ndistinct(capacity, nlabels));
     if (n == 0) return LO_OK;
     if (capacity > 0 && !labels_out) return fail(LO_ERR_INVALID, "labels_out is NULL");
@@ -2713,7 +2713,8 @@ int lo_nb_fit(lo_ctx *ctx, const lo_table *x, int64_t ld, int32_t k, const lo_ta
     const int64_t nct = std::min(wct, (n + per_cta - 1) / per_cta);
     const int64_t level1 = (std::max(nct, nw) + lo::kNbFan - 1) / lo::kNbFan;
     double *d_cls = nullptr, *partial = nullptr, *wins = nullptr, *sums = nullptr, *buf[2] = {nullptr, nullptr};
-    unsigned long long *counts = nullptr, *err = nullptr;
+    unsigned long long *counts = nullptr;
+    RefusedCell bad;
     c.alloc(&d_cls, (size_t)C * 8);
     c.alloc(&partial, (size_t)nct * slots * 8);
     c.alloc(&wins, (size_t)nw * slots * 8);
@@ -2721,32 +2722,30 @@ int lo_nb_fit(lo_ctx *ctx, const lo_table *x, int64_t ld, int32_t k, const lo_ta
     c.alloc(&buf[1], (size_t)level1 * slots * 8);
     c.alloc(&sums, slots * 8);
     c.alloc(&counts, (size_t)C * 8);
-    c.alloc(&err, 8);
     c.to_dev(d_cls, classes, (size_t)C * 8);
     c.memset(counts, 0, (size_t)C * 8);
-    c.memset(err, 0xFF, 8);
+    bad.arm(c);
     c.mark();
     for (int64_t w = 0; w < nw; ++w) {
         const int64_t r0 = w * wrows, r1 = std::min(n, r0 + wrows);
         if (x->dtype == LO_F32)
-            launch_nb_sums<float>(c, x, ld, k, y, r0, r1, d_cls, C, direct, partial, counts, err, shape, smem);
+            launch_nb_sums<float>(c, x, ld, k, y, r0, r1, d_cls, C, direct, partial, counts, bad.word, shape, smem);
         else
-            launch_nb_sums<double>(c, x, ld, k, y, r0, r1, d_cls, C, direct, partial, counts, err, shape, smem);
+            launch_nb_sums<double>(c, x, ld, k, y, r0, r1, d_cls, C, direct, partial, counts, bad.word, shape, smem);
         nb_tree(c, partial, (r1 - r0 + per_cta - 1) / per_cta, slots, wins + (size_t)w * slots, buf);
     }
     nb_tree(c, wins, nw, slots, sums, buf);
     c.mark();
-    unsigned long long key = ~0ull;
     c.to_host(sums_out, sums, slots * 8);
     c.to_host(counts_out, counts, (size_t)C * 8);
-    c.to_host(&key, err, 8);
+    bad.read(c);
     LO_TRY(c.finish(timing));
-    if (key != ~0ull) {
-        std::fill(sums_out, sums_out + slots, 0.0);
-        std::fill(counts_out, counts_out + C, (int64_t)0);
-        return nb_bad_row(info, key, k, "classes");
-    }
-    return LO_OK;
+    if (!bad.found(k, info)) return LO_OK;
+    std::fill(sums_out, sums_out + slots, 0.0);
+    std::fill(counts_out, counts_out + C, (int64_t)0);
+    if (info->bad_col == k) return fail(LO_ERR_INVALID, "row %lld: its label is not one of the classes", (long long)info->bad_row);
+    return fail(LO_ERR_INVALID, "row %lld, feature %d: negative or NaN (NaiveBayes needs values >= 0)",
+                (long long)info->bad_row, info->bad_col);
 }
 
 int lo_nb_predict(lo_ctx *ctx, const lo_table *x, int64_t ld, int32_t k, int64_t n, const double *pi, const double *theta,
@@ -2770,9 +2769,9 @@ int lo_nb_predict(lo_ctx *ctx, const lo_table *x, int64_t ld, int32_t k, int64_t
     } else {
         if (y || eval_labels) return fail(LO_ERR_INVALID, "y and eval_labels go with confusion_out");
         if (n > 0 && C > INT64_MAX / 8 / n) return fail(LO_ERR_INVALID, "n * C overflows");
-        LO_TRY(check_nb_table(ctx, prob, LO_F64, n * C, "prob"));
-        LO_TRY(check_nb_table(ctx, pred, LO_F64, n, "pred"));
-        if (raw) LO_TRY(check_nb_table(ctx, raw, LO_F64, n * C, "raw"));
+        LO_TRY(check_float_table(ctx, prob, LO_F64, n * C, "prob"));
+        LO_TRY(check_float_table(ctx, pred, LO_F64, n, "pred"));
+        if (raw) LO_TRY(check_float_table(ctx, raw, LO_F64, n * C, "raw"));
     }
     HostCall c(ctx, eval ? "nb_evaluate" : "nb_predict");
     if (n == 0) return c.finish(timing);
@@ -2787,7 +2786,8 @@ int lo_nb_predict(lo_ctx *ctx, const lo_table *x, int64_t ld, int32_t k, int64_t
     const bool hist_smem = eval && with_raws + hist_bytes <= lo::kNbSmemMax;
     const int smem = (int)(with_raws + (hist_smem ? hist_bytes : 0));
     double *d_theta = nullptr, *d_pi = nullptr, *d_evl = nullptr, *raws = nullptr;
-    unsigned long long *conf = nullptr, *err = nullptr;
+    unsigned long long *conf = nullptr;
+    RefusedCell bad;
     c.alloc(&d_theta, theta_t.size() * 8);
     c.alloc(&d_pi, (size_t)C * 8);
     c.to_dev(d_theta, theta_t.data(), theta_t.size() * 8);
@@ -2795,10 +2795,9 @@ int lo_nb_predict(lo_ctx *ctx, const lo_table *x, int64_t ld, int32_t k, int64_t
     if (eval) {
         c.alloc(&d_evl, (size_t)neval * 8);
         c.alloc(&conf, (size_t)neval * C * 8);
-        c.alloc(&err, 8);
         c.to_dev(d_evl, eval_labels, (size_t)neval * 8);
         c.memset(conf, 0, (size_t)neval * C * 8);
-        c.memset(err, 0xFF, 8);
+        bad.arm(c);
     }
     auto go = [&](auto kernel, auto tag) {
         using T = decltype(tag);
@@ -2813,7 +2812,7 @@ int lo_nb_predict(lo_ctx *ctx, const lo_table *x, int64_t ld, int32_t k, int64_t
             kernel<<<grid, lo::kNbTile, smem, c.s>>>((const T *)x->base, ld, k, n, d_theta, d_pi, C,
                                                      prob ? (double *)prob->base : nullptr, raw ? (double *)raw->base : nullptr,
                                                      pred ? (double *)pred->base : nullptr, y ? (const T *)y->base : nullptr,
-                                                     d_evl, neval, direct, conf, raws, hist_smem ? 1 : 0, err);
+                                                     d_evl, neval, direct, conf, raws, hist_smem ? 1 : 0, bad.word);
         });
         c.mark();
     };
@@ -2822,17 +2821,12 @@ int lo_nb_predict(lo_ctx *ctx, const lo_table *x, int64_t ld, int32_t k, int64_t
     } else {
         if (eval) go(lo::k_nb_predict<double, true>, 0.0); else go(lo::k_nb_predict<double, false>, 0.0);
     }
-    unsigned long long key = ~0ull;
-    if (eval) {
-        c.to_host(confusion_out, conf, (size_t)neval * C * 8);
-        c.to_host(&key, err, 8);
-    }
+    if (eval) c.to_host(confusion_out, conf, (size_t)neval * C * 8);
+    bad.read(c);
     LO_TRY(c.finish(timing));
-    if (key != ~0ull) {
-        std::fill(confusion_out, confusion_out + (size_t)neval * C, (int64_t)0);
-        return nb_bad_row(info, key, k, "evaluated labels");
-    }
-    return LO_OK;
+    if (!bad.found(k, info)) return LO_OK;
+    std::fill(confusion_out, confusion_out + (size_t)neval * C, (int64_t)0);
+    return fail(LO_ERR_INVALID, "row %lld: its label is not one of the evaluated labels", (long long)info->bad_row);
 }
 
 }  // extern "C"

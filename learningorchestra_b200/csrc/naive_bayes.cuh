@@ -1,5 +1,5 @@
 // naive_bayes.cuh — Spark 2.4's multinomial NaiveBayes over the feature matrix in HBM (lo_nb_fit, lo_nb_predict;
-// DESIGN.md §3.6.2).  Included by loexec.cu after kernels.cuh, whose streaming loads and warp_min_u64 it uses.
+// DESIGN.md §3.6.2).  Included by loexec.cu after kernels.cuh, whose streaming loads and refused-cell keys it uses.
 //   * k_nb_sums + k_nb_reduce (fit): per-class row counts and f64 column sums of a row-major f32 / f64 matrix, reduced
 //     in a fixed order and in bounded runs (no floating-point atomics), and the lowest row holding a negative or NaN
 //     feature.
@@ -79,8 +79,8 @@ __device__ __forceinline__ void nb_load(const T *p, uint64_t pol, double (&v)[VW
 // and no sum takes more than kNbRun adds here.  Column j of class c sits at c * kp + nb_col(j) of a copy: the one-double
 // skew per 16 columns puts a warp's column groups on different banks, and the copy stride (= 2 mod 16 doubles) its row
 // groups.  At the end the copies are added into partial[b][c * k + j] in runs of 16 (g order), the class counts go to
-// counts[] by integer atomics, and the lowest key row * (k + 1) + j of a feature that is not >= 0 (negative or NaN) or
-// of a label that is no class (j = k) to *err.
+// counts[] by integer atomics, and the lowest key cell_key(row, k, j) of a feature that is not >= 0 (negative or NaN)
+// or of a label that is no class (j = k) to *err.
 __host__ __device__ __forceinline__ int nb_col(int j) { return j + (j >> 4); }
 
 template <typename T, int VW>
@@ -118,7 +118,7 @@ __global__ void __launch_bounds__(kNbThreads) k_nb_sums(const T *__restrict__ x,
                 if (rr >= r1) continue;
                 const int c = nb_class(lab[i], cls, C, direct);
                 if (c < 0) {
-                    bad = min(bad, (unsigned long long)rr * (unsigned long long)(k + 1) + (unsigned)k);
+                    bad = min(bad, cell_key(rr, k, k));
                     continue;
                 }
                 if (q == 0) atomicAdd(&cnt[c], 1u);
@@ -127,14 +127,13 @@ __global__ void __launch_bounds__(kNbThreads) k_nb_sums(const T *__restrict__ x,
                 for (int w = 0; w < VW; ++w) {
                     const int j = q * VW + w;
                     if (j >= k) continue;
-                    if (!(v[i][w] >= 0.0)) bad = min(bad, (unsigned long long)rr * (unsigned long long)(k + 1) + (unsigned)j);
+                    if (!(v[i][w] >= 0.0)) bad = min(bad, cell_key(rr, k, j));
                     row[w] += v[i][w];
                 }
             }
         }
     }
-    bad = warp_min_u64(bad);
-    if ((threadIdx.x & 31) == 0 && bad != ~0ull) atomicMin(err, bad);
+    report_cell(bad, err);
     __syncthreads();
     double *out = partial + (size_t)blockIdx.x * C * k;
     for (int s = threadIdx.x; s < C * k; s += kNbThreads) {
@@ -209,7 +208,7 @@ __device__ __noinline__ int nb_softmax(double *raw, int C) {
 // !EVAL: raw (optional), probability and prediction of every row, with streaming stores.  EVAL: nothing per row; the
 // row's label slot a in eval_labels (direct or binary search) and its prediction p count in hist[a * C + p] (shared
 // memory when it fits, flushed once per CTA with integer atomics; else straight into confusion); a label that is not in
-// eval_labels gives the key row * (k + 1) + k to *err.
+// eval_labels gives the key cell_key(row, k, k) to *err.
 template <typename T, bool EVAL>
 __global__ void __launch_bounds__(kNbTile) k_nb_predict(const T *__restrict__ x, long long ld, int k, long long n,
                                                         const double *__restrict__ theta_t, const double *__restrict__ pi,
@@ -278,14 +277,13 @@ __global__ void __launch_bounds__(kNbTile) k_nb_predict(const T *__restrict__ x,
             __stcs(pred + row, (double)p);
         } else {
             const int a = nb_class((double)y[row], evl, neval, direct);
-            if (a < 0) bad = min(bad, (unsigned long long)row * (unsigned long long)(k + 1) + (unsigned)k);
+            if (a < 0) bad = min(bad, cell_key(row, k, k));
             else if (hist_in_smem) atomicAdd(&hist[a * C + p], 1u);
             else atomicAdd(&confusion[(size_t)a * C + p], 1ull);
         }
     }
     if (EVAL) {
-        bad = warp_min_u64(bad);
-        if (lane == 0 && bad != ~0ull) atomicMin(err, bad);
+        report_cell(bad, err);
         if (hist_in_smem) {
             __syncthreads();
             for (int i = threadIdx.x; i < neval * C; i += kNbTile)

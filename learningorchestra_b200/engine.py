@@ -10,6 +10,7 @@ dataType services talk to mongod through pymongo (``histogram_image/utils.py:50-
 """
 from __future__ import annotations
 
+import contextlib
 import ctypes as C
 import io
 import os
@@ -70,6 +71,12 @@ def _timing(t) -> dict:
     return {"total_ms": t.total_ms, "h2d_bytes": t.h2d_bytes, "d2h_bytes": t.d2h_bytes, "launches": t.launches}
 
 
+def _report(timing: dict | None, t) -> None:
+    """A call's lo_host_timing ``t`` into the caller's ``timing`` dict, when it passed one."""
+    if timing is not None:
+        timing.update(_timing(t), kernel_ms=t.kernel_ms)
+
+
 def _validity(nulls, n: int):
     """(lo_validity, the array it points into) of ``nulls`` as :meth:`Engine.parse_number_into` takes it."""
     v, keep = N.Validity(), None
@@ -114,8 +121,7 @@ def _groups(call, n: int, dtypes, timing: dict | None = None) -> tuple:
             cap = int(nd.value)
             continue
         N.check(rc)
-        if t is not None:
-            timing.update(_timing(t), kernel_ms=t.kernel_ms)
+        _report(timing, t)
         return tuple(o[:nd.value] for o in outs)
 
 
@@ -284,13 +290,51 @@ class DeviceArray:
 
 
 class InvalidCellError(N.LoexecError):
-    """:meth:`Engine.assemble_rows` with ``handle_invalid="error"`` met an invalid cell: ``row`` is the lowest such row
-    (a source row; global over the shards of a :class:`~sharding.ShardedEngine`) and ``position`` its lowest invalid
-    source (an index into ``sources``; ``len(sources)``: the label)."""
+    """A call refused a cell of the feature matrix: :meth:`Engine.assemble_rows` with ``handle_invalid="error"`` met an
+    invalid cell, :meth:`Engine.nb_fit` / :meth:`Engine.nb_predict` a negative or NaN feature or an unknown label.
+    ``row`` is the lowest such row (a source row for assemble_rows, a row of the matrix for the others; global over the
+    shards of a :class:`~sharding.ShardedEngine`) and ``position`` its lowest refused column (an index into the sources
+    or features; their count: the label).  ``reason``, when given, is the message as a format of ``row`` and
+    ``position``, so that :meth:`moved` moves the row the message names too; else the message is ``message``."""
 
-    def __init__(self, row: int, position: int, message: str):
-        super().__init__(N.LO_ERR_INVALID, message)
-        self.row, self.position = int(row), int(position)
+    def __init__(self, row: int, position: int, message: str | None = None, reason: str | None = None):
+        self.row, self.position, self.reason = int(row), int(position), reason
+        super().__init__(N.LO_ERR_INVALID, message if reason is None else reason.format(row=self.row, position=self.position))
+
+    def moved(self, first: int) -> "InvalidCellError":
+        """The same refusal ``first`` rows further on: a shard's row made global."""
+        return InvalidCellError(self.row + first, self.position, self.message, self.reason)
+
+
+# The messages of a refused cell, (a feature's, the label's), in lo_last_error()'s words
+_ASSEMBLE_REFUSED = ("invalid cell (NaN or code -1) in row {row}, source {position}",
+                     "invalid cell (NaN or code -1) in row {row}, the label, source {position}")
+_NB_FEATURE_REFUSED = "row {row}, feature {position}: negative or NaN (NaiveBayes needs values >= 0)"
+_FIT_REFUSED = (_NB_FEATURE_REFUSED, "row {row}: its label is not one of the classes")
+_EVALUATE_REFUSED = (_NB_FEATURE_REFUSED, "row {row}: its label is not one of the evaluated labels")
+
+
+def _check_cells(rc: int, info, k: int, reasons: tuple[str, str]) -> None:
+    """``N.check(rc)``, except that a refused cell (LO_ERR_INVALID with ``info.bad_row`` set) raises
+    :class:`InvalidCellError` with ``reasons[0]`` for a feature's cell and ``reasons[1]`` for the label's (column k)."""
+    if rc == N.LO_ERR_INVALID and info.bad_row >= 0:
+        raise InvalidCellError(info.bad_row, info.bad_col, reason=reasons[info.bad_col == k])
+    N.check(rc)
+
+
+class _Owned(contextlib.ExitStack):
+    """The tables a call makes for its result: :meth:`own` frees them when the call raises; a call that returns keeps
+    them."""
+
+    def own(self, table):
+        if table is not None:
+            self.callback(table.free)
+        return table
+
+    def __exit__(self, exc_type, *rest):
+        if exc_type is None:
+            self.pop_all()
+        return super().__exit__(exc_type, *rest)
 
 
 class AssembledRows:
@@ -728,8 +772,7 @@ class Engine:
         N.check(self._lib.lo_format_number_host(self._ctx, values.ctypes.data_as(C.c_void_p), status.ctypes.data_as(C.c_void_p),
                                                 n, offsets.ctypes.data_as(C.c_void_p), chars.ctypes.data_as(C.c_void_p), cap,
                                                 C.byref(t)))
-        if timing is not None:
-            timing.update(_timing(t), kernel_ms=t.kernel_ms)
+        _report(timing, t)
         return chars[:offsets[n]], offsets
 
     def read_csv_host(self, body, timing: dict | None = None):
@@ -862,8 +905,7 @@ class Engine:
         h, t = C.c_void_p(), N.HostTiming()
         N.check(self._lib.lo_text_upload(self._ctx, chars.ctypes.data_as(C.c_void_p), offsets.ctypes.data_as(C.c_void_p),
                                          C.byref(v), len(arr), C.byref(h), C.byref(t)))
-        if timing is not None:
-            timing.update(_timing(t), kernel_ms=t.kernel_ms)
+        _report(timing, t)
         return DeviceText(self, h, arr)
 
     def value_counts_text(self, text: DeviceText, timing: dict | None = None):
@@ -897,14 +939,6 @@ class Engine:
         col)`` or None) fills ``y``.  A NaN cell or a -1 code is invalid: ``handle_invalid="error"`` raises
         :class:`InvalidCellError` naming the lowest one, ``"skip"`` leaves its row out, ``"keep"`` writes NaN.
         ``timing``: a dict to receive the call's lo_host_timing fields."""
-        rows, bad = self._assemble_rows(sources, label, dtype, handle_invalid, timing)
-        if bad is not None:
-            raise InvalidCellError(*bad)
-        return rows
-
-    def _assemble_rows(self, sources, label, dtype, handle_invalid, timing=None):
-        """(AssembledRows, None), or (None, (row, position, message)) when ``"error"`` met an invalid cell (the tables
-        freed): :meth:`assemble_rows` without raising, for :meth:`ShardedEngine.assemble_rows` to compare shards."""
         mode, out = assemble_args(handle_invalid, dtype)
         k = len(sources)
         if k == 0:
@@ -914,32 +948,19 @@ class Engine:
         n = sources[0][0].nrows
         tabs = (C.c_void_p * k)(*[t._h for t, _c in sources])
         cols = (C.c_int32 * k)(*[int(c) for _t, c in sources])
-        x = self.table(out, n * k, 1)
-        y = rows = None
-        try:
-            y = self.table(out, n, 1) if label is not None else None
-            rows = np.empty(n, np.int64) if mode == N.LO_INVALID_SKIP else None    # else every row is kept, in order
-            info, t = N.AssembleInfo(), N.HostTiming()
+        rows = np.empty(n, np.int64) if mode == N.LO_INVALID_SKIP else None    # else every row is kept, in order
+        info, t = N.AssembleInfo(), N.HostTiming()
+        with _Owned() as owned:
+            x = owned.own(self.table(out, n * k, 1))
+            y = owned.own(self.table(out, n, 1) if label is not None else None)
             rc = self._lib.lo_assemble_rows(self._ctx, tabs, cols, k, label[0]._h if label is not None else None,
                                             int(label[1]) if label is not None else 0, mode, x._h, k,
                                             y._h if y is not None else None,
                                             rows.ctypes.data_as(C.c_void_p) if rows is not None else None,
                                             C.byref(info), C.byref(t))
-            if rc == N.LO_ERR_INVALID and info.bad_row >= 0:
-                msg = self._lib.lo_last_error().decode("utf-8", "replace")
-                x.free()
-                if y is not None:
-                    y.free()
-                return None, (int(info.bad_row), int(info.bad_col), msg)
-            N.check(rc)
-        except BaseException:
-            x.free()
-            if y is not None:
-                y.free()
-            raise
-        if timing is not None:
-            timing.update(_timing(t), kernel_ms=t.kernel_ms)
-        return AssembledRows(x, y, rows[:info.nkept] if rows is not None else None, k, info.nkept), None
+            _check_cells(rc, info, k, _ASSEMBLE_REFUSED)
+        _report(timing, t)
+        return AssembledRows(x, y, rows[:info.nkept] if rows is not None else None, k, info.nkept)
 
     def nb_labels(self, part: AssembledRows) -> np.ndarray:
         """The distinct label values of ``part`` (an :class:`AssembledRows` with ``y``), ascending, -0.0 as 0.0
@@ -958,13 +979,6 @@ class Engine:
         rows labelled classes[c], sums[c, j] the f64 sum of feature j over them, in a fixed order.  A negative or NaN
         feature, or a label that is no class, raises :class:`InvalidCellError` naming the lowest row (``position`` the
         feature; k: the label).  ``timing``: a dict to receive the call's lo_host_timing fields."""
-        res, bad = self._nb_fit(part, classes, timing)
-        if bad is not None:
-            raise InvalidCellError(*bad)
-        return res
-
-    def _nb_fit(self, part, classes, timing=None):
-        """(result, None), or (None, (row, position, message)): :meth:`nb_fit` without raising, for the shards."""
         if part.y is None:
             raise ValueError("the rows have no label")
         cls = np.ascontiguousarray(classes, dtype=np.float64)
@@ -974,12 +988,9 @@ class Engine:
         rc = self._lib.lo_nb_fit(self._ctx, part.x._h, part.k, part.k, part.y._h, part.nkept, cls.ctypes.data_as(C.c_void_p),
                                  len(cls), sums.ctypes.data_as(C.c_void_p), counts.ctypes.data_as(C.c_void_p),
                                  C.byref(info), C.byref(t))
-        if rc == N.LO_ERR_INVALID and info.bad_row >= 0:
-            return None, (int(info.bad_row), int(info.bad_col), self._lib.lo_last_error().decode("utf-8", "replace"))
-        N.check(rc)
-        if timing is not None:
-            timing.update(_timing(t), kernel_ms=t.kernel_ms)
-        return (sums, counts), None
+        _check_cells(rc, info, part.k, _FIT_REFUSED)
+        _report(timing, t)
+        return sums, counts
 
     def nb_predict(self, part: AssembledRows, pi, theta, raw: bool = False, labels=None, timing: dict | None = None):
         """A NaiveBayes model (``pi`` float64[C], ``theta`` float64[C, k]) over ``part`` (``lo_nb_predict``).
@@ -987,12 +998,6 @@ class Engine:
         values with ``raw``).  ``labels`` the ascending label values to count: evaluate — the int64[len(labels), C]
         confusion counts of (label, prediction index), nothing written per row; a label not in ``labels`` raises
         :class:`InvalidCellError`.  ``timing``: a dict to receive the call's lo_host_timing fields."""
-        res, bad = self._nb_predict(part, pi, theta, raw, labels, timing)
-        if bad is not None:
-            raise InvalidCellError(*bad)
-        return res
-
-    def _nb_predict(self, part, pi, theta, raw=False, labels=None, timing=None):
         pi = np.ascontiguousarray(pi, dtype=np.float64)
         theta = np.ascontiguousarray(theta, dtype=np.float64)
         nc, n = len(pi), part.nkept
@@ -1007,30 +1012,17 @@ class Engine:
             conf = np.zeros((len(lab), nc), np.int64)
             rc = self._lib.lo_nb_predict(*args, None, None, None, part.y._h, lab.ctypes.data_as(C.c_void_p), len(lab),
                                          conf.ctypes.data_as(C.c_void_p), C.byref(info), C.byref(t))
-            if rc == N.LO_ERR_INVALID and info.bad_row >= 0:
-                return None, (int(info.bad_row), int(info.bad_col), self._lib.lo_last_error().decode("utf-8", "replace"))
-            N.check(rc)
-            if timing is not None:
-                timing.update(_timing(t), kernel_ms=t.kernel_ms)
-            return conf, None
-        tables = []
-        try:
-            prob = self.table("f64", n * nc, 1)
-            tables.append(prob)
-            pred = self.table("f64", n, 1)
-            tables.append(pred)
-            rawt = self.table("f64", n * nc, 1) if raw else None
-            if rawt is not None:
-                tables.append(rawt)
+            _check_cells(rc, info, part.k, _EVALUATE_REFUSED)
+            _report(timing, t)
+            return conf
+        with _Owned() as owned:
+            prob = owned.own(self.table("f64", n * nc, 1))
+            pred = owned.own(self.table("f64", n, 1))
+            rawt = owned.own(self.table("f64", n * nc, 1) if raw else None)
             N.check(self._lib.lo_nb_predict(*args, prob._h, rawt._h if rawt is not None else None, pred._h, None, None, 0,
                                             None, C.byref(info), C.byref(t)))
-        except BaseException:
-            for tb in tables:
-                tb.free()
-            raise
-        if timing is not None:
-            timing.update(_timing(t), kernel_ms=t.kernel_ms)
-        return PredictedRows(prob, rawt, pred, n, nc), None
+        _report(timing, t)
+        return PredictedRows(prob, rawt, pred, n, nc)
 
     def value_counts_f64_host(self, values: np.ndarray):
         """(keys float64[g], counts uint64[g]) — exact value counts of a numeric column (GPU hash group-by),

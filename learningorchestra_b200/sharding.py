@@ -13,6 +13,7 @@ pages by ``_id`` range, ``database_api_image/utils.py:17-23``).
 from __future__ import annotations
 
 import ctypes as C
+import itertools
 import threading
 
 ROW_ALIGN = 32
@@ -88,6 +89,11 @@ def on_each(n: int, fn, undo=None) -> list:
                     undo(r)
         raise failed[0]
     return results
+
+
+def _firsts(parts) -> list:
+    """The first row of each of the shards' ``AssembledRows`` in the rows of all of them, shards in order."""
+    return list(itertools.accumulate((p.nkept for p in parts[:-1]), initial=0))
 
 
 def _combine_timings(parts) -> dict:
@@ -528,13 +534,38 @@ class ShardedEngine:
             raise self._N.LoexecError(self._N.LO_ERR_INVALID, f"{what} needs every row: this process holds "
                                       f"{self.nlocal} of the group's {self.world} shards")
 
+    def _each(self, what: str, fn, undo=None, first_rows=None) -> list:
+        """``[fn(0), ..., fn(nlocal - 1)]`` through :func:`on_each`, for a call ``what`` that needs every row (a rank
+        group refuses it).  When any member raised, ``undo`` runs on the others' results.  An error that is not a
+        refused cell wins, the first in member order; else the lowest refused cell is raised, each member's
+        ``InvalidCellError`` moved by ``first_rows[i]`` (member i's first row in the numbering the caller reports)."""
+        from .engine import InvalidCellError
+        self._every_row(what)
+        errors = [None] * self.nlocal
+
+        def run(i):
+            try:
+                return fn(i)
+            except BaseException as exc:
+                errors[i] = exc
+                raise
+
+        try:
+            return on_each(self.nlocal, run, undo)
+        except InvalidCellError:
+            pass
+        failed = [(i, e) for i, e in enumerate(errors) if e is not None]
+        other = [e for _i, e in failed if not isinstance(e, InvalidCellError)]
+        if other:
+            raise other[0]
+        raise min((e.moved(first_rows[i]) for i, e in failed), key=lambda e: (e.row, e.position))
+
     def parse_text_into(self, table: ShardedTable, col: int, text: ShardedText) -> dict:
         """``Engine.parse_text_into`` over a sharded table: piece i of ``text`` and shard i of ``table`` hold the same rows
         (both cut at :meth:`bounds`), so every member parses its piece into its shard on its own device, from a host
         thread of its own, and nothing crosses devices.  The summary's rows are global."""
-        self._every_row("parse_text_into")
         text.check_cut(table)
-        return combine_parse_summaries(on_each(self.nlocal, lambda i: self.engines[i].parse_text_into(
+        return combine_parse_summaries(self._each("parse_text_into", lambda i: self.engines[i].parse_text_into(
             table.shards[i], col, text.pieces[i])), table.offsets)
 
     def format_column(self, table: ShardedTable, col: int, valid, is_int) -> ShardedText:
@@ -543,9 +574,8 @@ class ShardedEngine:
         pieces before it.  ``valid`` / ``is_int`` describe every row; the result's ``arr`` is one Arrow array."""
         import numpy as np
         import pyarrow as pa
-        self._every_row("format_column")
         bounds = [(off, off + t.nrows) for t, off in zip(table.shards, table.offsets)]
-        pieces = on_each(self.nlocal, lambda i: self.engines[i].format_text(
+        pieces = self._each("format_column", lambda i: self.engines[i].format_text(
             table.shards[i], col, valid[bounds[i][0]:bounds[i][1]], is_int[bounds[i][0]:bounds[i][1]]),
             undo=lambda p: p.free())
         try:
@@ -577,8 +607,8 @@ class ShardedEngine:
         """``Engine.value_counts_column`` over a sharded table: every local shard is counted on its own device from a
         host thread of its own, and the groups are merged on the host (:func:`merge_value_counts`).  A rank group's
         process holds only its own rows, so it refuses rather than return a partial count."""
-        self._every_row("value_counts_column")
-        return merge_value_counts(on_each(self.nlocal, lambda i: self.engines[i].value_counts_column(table.shards[i], col)))
+        return merge_value_counts(self._each("value_counts_column",
+                                             lambda i: self.engines[i].value_counts_column(table.shards[i], col)))
 
     # ---- host buffers -------------------------------------------------------------------------------------
     def project_cast_hist_host(self, cols, nbins: int | None = None, lo=None, hi=None, out=None, bcast: bool = False):
@@ -699,38 +729,24 @@ class ShardedEngine:
         nothing crosses devices.  Returns one ``AssembledRows`` per local member, its ``rows`` global (the shard's first
         row added).  ``"error"``: the lowest invalid row over all shards is raised (``InvalidCellError``).  A rank group's
         process holds only its own rows, so it refuses rather than assemble a part."""
-        from .engine import InvalidCellError, assemble_args
-        self._every_row("assemble_rows")
+        from .engine import assemble_args
         assemble_args(handle_invalid, dtype)
         tables = [t for t, _c in sources] + ([label[0]] if label is not None else [])
         offsets = tables[0].offsets if tables else []
         if any(t.offsets != offsets or [s.nrows for s in t.shards] != [s.nrows for s in tables[0].shards] for t in tables):
             raise ValueError("the source tables are not cut at the same rows")
-
-        def run(i):
-            return self.engines[i]._assemble_rows([(t.shards[i], c) for t, c in sources],
-                                                  (label[0].shards[i], label[1]) if label is not None else None,
-                                                  dtype, handle_invalid)
-
-        parts = on_each(self.nlocal, run, undo=lambda p: p[0] is not None and p[0].free())
-        bad = [(off + b[0], b[1]) for (_r, b), off in zip(parts, offsets) if b is not None]
-        if bad:
-            for rows, _b in parts:
-                if rows is not None:
-                    rows.free()
-            row, position = min(bad)
-            raise InvalidCellError(row, position, f"invalid cell (NaN or code -1) in row {row}, "
-                                   f"{'the label' if position == len(sources) else 'source %d' % position}")
-        for (rows, _b), off in zip(parts, offsets):
-            rows.first = off
-        return [rows for rows, _b in parts]
+        parts = self._each("assemble_rows", lambda i: self.engines[i].assemble_rows(
+            [(t.shards[i], c) for t, c in sources], (label[0].shards[i], label[1]) if label is not None else None,
+            dtype, handle_invalid), undo=lambda p: p.free(), first_rows=offsets)
+        for p, off in zip(parts, offsets):
+            p.first = off
+        return parts
 
     def nb_labels(self, parts) -> "np.ndarray":
         """``Engine.nb_labels`` over the shards' ``AssembledRows`` (one per local member, as :meth:`assemble_rows` made
         them): every member groups its own labels on its own device, from a host thread of its own; the union, ascending."""
         import numpy as np
-        self._every_row("nb_labels")
-        got = on_each(self.nlocal, lambda i: self.engines[i].nb_labels(parts[i]))
+        got = self._each("nb_labels", lambda i: self.engines[i].nb_labels(parts[i]))
         labels = np.unique(np.concatenate(got)) if got else np.zeros(0)
         if len(labels) > self._N.LO_NB_MAX_CLASSES:
             raise self._N.LoexecError(self._N.LO_ERR_INVALID, f"{len(labels)} distinct labels: at most "
@@ -742,45 +758,24 @@ class ShardedEngine:
         the sums and counts are added on the host in shard order, so integer-valued features give the single-GPU sums
         bit for bit.  A refused row is raised as the lowest over all shards, its row global (rows of the earlier shards
         counted first)."""
-        self._every_row("nb_fit")
-        got = on_each(self.nlocal, lambda i: self.engines[i]._nb_fit(parts[i], classes))
-        self._raise_lowest(parts, [b for _r, b in got])
-        sums, counts = got[0][0]
-        for (s, c), _b in got[1:]:
+        got = self._each("nb_fit", lambda i: self.engines[i].nb_fit(parts[i], classes), first_rows=_firsts(parts))
+        sums, counts = got[0]
+        for s, c in got[1:]:
             sums, counts = sums + s, counts + c
         return sums, counts
 
     def nb_predict(self, parts, pi, theta, raw: bool = False, labels=None):
         """``Engine.nb_predict`` over the shards, each on its own device from a host thread of its own.  Transform: one
-        ``PredictedRows`` per member.  Evaluate (``labels``): the members' confusion counts summed."""
-        self._every_row("nb_predict")
-        got = on_each(self.nlocal, lambda i: self.engines[i]._nb_predict(parts[i], pi, theta, raw, labels),
-                      undo=lambda r: r[0] is not None and labels is None and r[0].free())
-        try:
-            self._raise_lowest(parts, [b for _r, b in got])
-        except BaseException:
-            for r, _b in got:
-                if r is not None and labels is None:
-                    r.free()
-            raise
-        if labels is not None:
-            confusion = got[0][0]
-            for r, _b in got[1:]:
-                confusion = confusion + r
-            return confusion
-        return [r for r, _b in got]
-
-    @staticmethod
-    def _raise_lowest(parts, bad) -> None:
-        """InvalidCellError for the lowest of the shards' refused rows (each shard's row made global), if any."""
-        from .engine import InvalidCellError
-        first, hits = 0, []
-        for p, b in zip(parts, bad):
-            if b is not None:
-                hits.append((first + b[0], b[1], b[2]))
-            first += p.nkept
-        if hits:
-            raise InvalidCellError(*min(hits))
+        ``PredictedRows`` per member.  Evaluate (``labels``): the members' confusion counts summed; a refused row is
+        raised as the lowest over all shards, its row global."""
+        got = self._each("nb_predict", lambda i: self.engines[i].nb_predict(parts[i], pi, theta, raw, labels),
+                         undo=(lambda p: p.free()) if labels is None else None, first_rows=_firsts(parts))
+        if labels is None:
+            return got
+        confusion = got[0]
+        for c in got[1:]:
+            confusion = confusion + c
+        return confusion
 
     @property
     def resident(self):

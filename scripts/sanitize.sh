@@ -21,6 +21,11 @@ nb_log="$(mktemp -d)/sanitizer_memcheck_naive_bayes.txt"
 timeout 1800 compute-sanitizer --tool memcheck --error-exitcode 1 python -m pytest tests/test_gpu_naive_bayes.py -q \
     > "$nb_log" 2>&1
 echo "memcheck (naive bayes) rc=$? log=$nb_log"; tail -3 "$nb_log"
+# memcheck of the refused cells over one GPU and every cut (the key's report and read-back); its log goes to a temporary directory
+refused_log="$(mktemp -d)/sanitizer_memcheck_refused_cells.txt"
+timeout 900 compute-sanitizer --tool memcheck --error-exitcode 1 python -m pytest tests/test_gpu_refused_cells.py -q \
+    > "$refused_log" 2>&1
+echo "memcheck (refused cells) rc=$? log=$refused_log"; tail -3 "$refused_log"
 # memcheck of the number parser and the resident formatter on every entry point, without the million-row cases: a read
 # past the last staged cell shows here (the CPU harness puts a NUL after it)
 parse_log="$(mktemp -d)/sanitizer_memcheck_parse.txt"

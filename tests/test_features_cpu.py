@@ -66,22 +66,16 @@ class _Engine:
     def __init__(self, log, device=0, bad=None):
         self.log, self.device, self.bad = log, device, bad
 
-    def _assemble_rows(self, sources, label, dtype, handle_invalid, timing=None):
+    def assemble_rows(self, sources, label=None, dtype="float32", handle_invalid="error"):
         self.log["calls"].append(([c for _t, c in sources], label and label[1], dtype, handle_invalid))
         n = sources[0][0].nrows
         if handle_invalid == "error" and self.bad is not None:
-            return None, (*self.bad, "invalid")
+            raise InvalidCellError(*self.bad, "invalid")
         rows = np.arange(n, dtype=np.int64)[::2] if handle_invalid == "skip" else None
         out = {"float32": "f32", "float64": "f64"}[dtype]
         y = _Table(self.log, out, n, self.device) if label is not None else None
         nkept = n if rows is None else len(rows)
-        return AssembledRows(_Table(self.log, out, n * len(sources), self.device), y, rows, len(sources), nkept), None
-
-    def assemble_rows(self, sources, label=None, dtype="float32", handle_invalid="error"):
-        rows, bad = self._assemble_rows(sources, label, dtype, handle_invalid)
-        if bad is not None:
-            raise InvalidCellError(*bad)
-        return rows
+        return AssembledRows(_Table(self.log, out, n * len(sources), self.device), y, rows, len(sources), nkept)
 
 
 def _log():

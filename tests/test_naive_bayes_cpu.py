@@ -137,27 +137,18 @@ class _Engine:
         self.log.append("labels")
         return nb.classes_of(part.y)
 
-    def _nb_fit(self, part, classes):
+    def nb_fit(self, part, classes):
         self.log.append("fit")
         bad = np.argwhere(~(part.hx >= 0))
         if len(bad):
-            return None, (int(bad[0][0]), int(bad[0][1]), "bad")
+            raise InvalidCellError(int(bad[0][0]), int(bad[0][1]), "bad")
         y = np.asarray(part.y) + 0.0
         return (np.array([part.hx[y == c].sum(0) for c in classes]).reshape(len(classes), part.k),
-                np.array([(y == c).sum() for c in classes], np.int64)), None
-
-    def nb_fit(self, part, classes):
-        res, bad = self._nb_fit(part, classes)
-        if bad is not None:
-            raise InvalidCellError(*bad)
-        return res
-
-    def _nb_predict(self, part, pi, theta, raw=False, labels=None):
-        pred = nb.prediction(nb.probability(nb.raw(part.hx, pi, theta)))
-        return nb.confusion(part.y, pred, labels, len(pi)), None
+                np.array([(y == c).sum() for c in classes], np.int64))
 
     def nb_predict(self, part, pi, theta, raw=False, labels=None):
-        return self._nb_predict(part, pi, theta, raw, labels)[0]
+        pred = nb.prediction(nb.probability(nb.raw(part.hx, pi, theta)))
+        return nb.confusion(part.y, pred, labels, len(pi))
 
 
 def _feats(engine, parts, label="y"):
