@@ -524,6 +524,60 @@ int lo_nb_predict(lo_ctx *ctx, const lo_table *x, int64_t ld, int32_t k, int64_t
                   const double *eval_labels, int32_t neval, int64_t *confusion_out, lo_nb_info *info,
                   lo_host_timing *timing);
 
+/* Spark 2.4's LogisticRegression (ml.classification.LogisticRegression with elasticNetParam 0, fitIntercept,
+ * standardization, no weightCol, no bounds; builder_image/builder.py:55-61's "LR") over the same feature matrix as the
+ * NaiveBayes calls: x holds n rows of k features (column 0, row stride ld >= k elements), y their labels, both LO_F32 or
+ * both LO_F64 on ctx's device, every value widened to f64 exactly.  The optimizer runs on the host; these calls are its
+ * device passes.  DESIGN.md §3.6.3.
+ *
+ * lo_lr_stats: sum_out[j] (host double[k]) = the f64 sum of column j; m2_out[j] (host double[k]) = the f64 sum of
+ * (x_j - sum_out[j] / n)^2 (a second pass, after the first is read back); label_counts_out[c] (host
+ * int64[LO_NB_MAX_CLASSES]) = the rows labelled c.  Every label must be an integer >= 0 (NaN, +-inf, negative and
+ * fractional labels are refused) and every feature finite; else the call fails with LO_ERR_INVALID and info->bad_row /
+ * bad_col name the lowest refused row and its lowest refused column (k: the label).  A label >= LO_NB_MAX_CLASSES fails
+ * with LO_ERR_INVALID and info->bad_row = -1.  A failed call leaves the outputs zero.  Sums as lo_lr_loss_grad's.
+ * Launches: none when n == 0; per pass and window of rows, one k_lr_stats and its k_nb_reduce levels, then the levels over
+ * the windows (pass 2 only when pass 1 refused nothing).  Bytes: x read twice, y once.  timing: h2d_bytes the means,
+ * d2h_bytes the sums, the label counts and the error word.
+ *
+ * lo_lr_loss_grad: LogisticAggregator at one point.  The model is nclasses rows c of k effective coefficients coef[c * k +
+ * j] (host; Spark's coefficient over the column's std, 0 where the std is 0) and intercept[c] (host double[nclasses]).
+ * multinomial = 0: binomial, nclasses must be 1 and the labels 0 or 1; per row margin = -(sum_j coef_j x_j +
+ * intercept), multiplier = 1 / (1 + exp(margin)) - y, loss = log1pExp(margin) (y > 0) or log1pExp(margin) - margin.
+ * multinomial = 1: the labels in [0, nclasses); margins m_c = sum_j coef[c][j] x_j + intercept[c], shifted by their max
+ * when that is > 0, multiplier_c = exp(m_c) / sum_c exp(m_c) - [y == c], loss = log(sum) - m_y (+ the max when shifted).
+ * out (host double[1 + nclasses * (k + 1)]) = [sum of the losses, sum of multiplier_c * x_j at 1 + c * k + j, sum of
+ * multiplier_c at 1 + nclasses * k + c], over every row.  Labels must have passed lo_lr_stats; others give unspecified
+ * sums.  No floating-point atomics: the same input on the same shard layout gives the same bits on every run.  No sum is
+ * a sequential run of more than 2048 adds (a fixed-order tree of 32-wide levels above that), so |sum - exact| <= 1e-12 *
+ * the sum of |terms|.  Launches: none when n == 0; per window of rows whose CTAs' partials fit 256 MiB, one
+ * k_lr_loss_grad (one read of x and y) and its k_nb_reduce levels, then the levels over the windows.  timing: h2d_bytes
+ * the model, d2h_bytes out.
+ *
+ * lo_lr_predict: lo_nb_predict's transform and evaluate (same arguments, outputs and refusals) for a LogisticRegression
+ * model.  multinomial = 1: theta = coef (nclasses x k), pi = intercept, raw as lo_nb_predict's; then
+ * LogisticRegressionModel's raw2probabilityInPlace: m = the first greatest raw value; m == +inf (a constant-label model)
+ * gives probability 1 at its index and 0 elsewhere; else e_c = exp(raw_c - m) when m > 0, exp(raw_c) otherwise, summed
+ * in c order, p_c = e_c * (1 / sum); prediction = Vector.argmax(p).  multinomial = 0: nclasses = 1, coef the k
+ * coefficients and intercept[0] the intercept; per row m = (sum_j coef_j * x_j, from 0.0 in ascending j, every product
+ * and add rounded on its own) + intercept, raw = [-m, m], probability = [1 - p1, p1] with p1 = 1 / (1 + exp(-m)),
+ * prediction = (p1 > threshold ? 1 : 0), two columns in prob, raw and confusion_out; threshold must lie in [0, 1].
+ * Launches, bytes and timing as lo_nb_predict's (C = 2 outputs when binomial).
+ *
+ * Refused with LO_ERR_INVALID before anything is enqueued (as they apply): lo_nb_fit's and lo_nb_predict's refusals of
+ * x, y, ld, k, n and the outputs; k > LO_NB_MAX_THETA (stats); multinomial other than 0 or 1; a binomial model with
+ * nclasses != 1; a multinomial one with nclasses outside [1, LO_NB_MAX_CLASSES] (lo_lr_loss_grad: [2, ...], a one-class
+ * model has nothing to train); (multinomial ? nclasses : 2) * k > LO_NB_MAX_THETA; a NULL model or output.  Every model
+ * within these caps fits lo_lr_loss_grad's tile in shared memory; a shape that did not would be refused the same way. */
+int lo_lr_stats(lo_ctx *ctx, const lo_table *x, int64_t ld, int32_t k, const lo_table *y, int64_t n, double *sum_out,
+                double *m2_out, int64_t *label_counts_out, lo_nb_info *info, lo_host_timing *timing);
+int lo_lr_loss_grad(lo_ctx *ctx, const lo_table *x, int64_t ld, int32_t k, const lo_table *y, int64_t n, const double *coef,
+                    const double *intercept, int32_t nclasses, int32_t multinomial, double *out, lo_host_timing *timing);
+int lo_lr_predict(lo_ctx *ctx, const lo_table *x, int64_t ld, int32_t k, int64_t n, const double *coef,
+                  const double *intercept, int32_t nclasses, int32_t multinomial, double threshold, lo_table *prob,
+                  lo_table *raw, lo_table *pred, const lo_table *y, const double *eval_labels, int32_t neval,
+                  int64_t *confusion_out, lo_nb_info *info, lo_host_timing *timing);
+
 /* Number -> text for one column: the reference's "string" cast, str(v) / None -> "" (data_type_handler_image/
  * data_type_update.py:22-28), for every cell at once on the GPU.  The inverse of lo_parse_number_host.
  * status[i] uses the LO_NUM_* codes above: FLOAT -> repr(float) (shortest round-trip digits, CPython's notation),

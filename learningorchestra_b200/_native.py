@@ -176,6 +176,12 @@ SIGNATURES = {
                             C.POINTER(HostTiming)]),
     "lo_nb_predict": (C.c_int, [_P, _P, C.c_int64, C.c_int32, C.c_int64, _P, _P, C.c_int32, _P, _P, _P, _P, _P,
                                 C.c_int32, _P, C.POINTER(NbInfo), C.POINTER(HostTiming)]),
+    "lo_lr_stats": (C.c_int, [_P, _P, C.c_int64, C.c_int32, _P, C.c_int64, _P, _P, _P, C.POINTER(NbInfo),
+                              C.POINTER(HostTiming)]),
+    "lo_lr_loss_grad": (C.c_int, [_P, _P, C.c_int64, C.c_int32, _P, C.c_int64, _P, _P, C.c_int32, C.c_int32, _P,
+                                  C.POINTER(HostTiming)]),
+    "lo_lr_predict": (C.c_int, [_P, _P, C.c_int64, C.c_int32, C.c_int64, _P, _P, C.c_int32, C.c_int32, C.c_double, _P,
+                                _P, _P, _P, _P, C.c_int32, _P, C.POINTER(NbInfo), C.POINTER(HostTiming)]),
     "lo_format_number_host": (C.c_int, [_P, _P, _P, C.c_int64, _P, _P, C.c_int64, C.POINTER(HostTiming)]),
     "lo_parse_text_to_table": (C.c_int, [_P, _P, _P, C.c_int32, C.POINTER(ParseSummary), C.POINTER(HostTiming)]),
     "lo_format_table_to_text": (C.c_int, [_P, _P, C.c_int32, C.POINTER(Validity), C.POINTER(Validity), C.POINTER(_P),

@@ -1,22 +1,32 @@
-"""The builder's "NB" classifier on the GPU: Spark 2.4's multinomial ``NaiveBayes`` (``builder_image/builder.py:55-61``)
-fitted on, applied to and evaluated over the feature matrix in HBM (:meth:`DeviceFrame.features`), on one GPU or on
-every shard of a local :class:`~sharding.ShardedEngine`.  DESIGN.md §3.6.2 states the semantics.
+"""The builder's "NB" and "LR" classifiers on the GPU: Spark 2.4's multinomial ``NaiveBayes`` and ``LogisticRegression``
+(``builder_image/builder.py:55-61``) fitted on, applied to and evaluated over the feature matrix in HBM
+(:meth:`DeviceFrame.features`), on one GPU or on every shard of a local :class:`~sharding.ShardedEngine`.  DESIGN.md
+§3.6.2 and §3.6.3 state the semantics.
 
-The device computes the class counts and per-class feature sums (``lo_nb_fit``), every row's raw values, probabilities
-and prediction (``lo_nb_predict``) and the confusion counts of an evaluation; the model's logs (C x k values) and the
-evaluator's metrics are computed here, on the host, from those."""
+NaiveBayes: the device computes the class counts and per-class feature sums (``lo_nb_fit``); LogisticRegression: the
+column statistics and label counts (``lo_lr_stats``) and one pass of loss and gradient sums per function evaluation of
+the host's L-BFGS (``lo_lr_loss_grad``, :mod:`lbfgs`).  Both compute every row's raw values, probabilities and prediction
+(``lo_nb_predict`` / ``lo_lr_predict``) and the confusion counts of an evaluation on the device; the models' arrays and
+the evaluator's metrics are computed here, on the host, from those."""
 from __future__ import annotations
+
+import math
 
 import numpy as np
 
 from . import _native as N
 
 
-def _on_device(features, call, per_part: bool = False):
+_NB_REASONS = ("is negative or NaN", "is not a class of the model")
+_LR_REASONS = ("is NaN or infinite", "is not an integer label >= 0")
+
+
+def _on_device(features, call, per_part: bool = False, name: str = "NaiveBayes",
+               reasons: tuple[str, str] = _NB_REASONS):
     """``call(engine, rows)`` on the features' engine: a ShardedEngine takes every shard's rows and gives one result per
     shard where it gives one per row (``per_part``); an Engine takes its one part, and its result is made a list of one
     where ``per_part``.  A refused cell (its row a row of the features, shards concatenated) is raised as the ``_id``
-    and field it holds."""
+    and field it holds: "<name>: field F of the row with _id I <reason>", ``reasons`` (a feature's, the label's)."""
     from .builder_frontend import named_cell
     from .engine import InvalidCellError
     from .sharding import ShardedEngine
@@ -25,8 +35,7 @@ def _on_device(features, call, per_part: bool = False):
     try:
         out = call(engine, features._parts if sharded else features._parts[0])
     except InvalidCellError as e:
-        raise named_cell(e, features.fields, features.label, features.row_ids, "NaiveBayes",
-                         ("is negative or NaN", "is not a class of the model")) from None
+        raise named_cell(e, features.fields, features.label, features.row_ids, name, reasons) from None
     return [out] if per_part and not sharded else out
 
 
@@ -36,12 +45,12 @@ def _usable(features) -> None:
         raise ValueError("the features have been released")
 
 
-def _labels(features) -> np.ndarray:
+def _labels(features, name: str = "NaiveBayes", reasons: tuple[str, str] = _NB_REASONS) -> np.ndarray:
     """The distinct label values of the features' rows, ascending (every shard's union)."""
     _usable(features)
     if features.label is None:
-        raise ValueError("NaiveBayes needs features with a label")
-    return _on_device(features, lambda engine, rows: engine.nb_labels(rows))
+        raise ValueError(f"{name} needs features with a label")
+    return _on_device(features, lambda engine, rows: engine.nb_labels(rows), name=name, reasons=reasons)
 
 
 def model_arrays(sums: np.ndarray, counts: np.ndarray, smoothing: float) -> tuple[np.ndarray, np.ndarray]:
@@ -141,6 +150,174 @@ def metrics(labels: np.ndarray, confusion: np.ndarray) -> tuple[float, float]:
         f1 += f * count / n
         tp_total += tp
     return f1, tp_total / n
+
+
+FAMILIES = ("auto", "binomial", "multinomial")
+
+
+def standardization(n: int, total, m2) -> np.ndarray:
+    """The unbiased std of every column from its sum and squared deviations over n rows (0 when n == 1)."""
+    return np.sqrt(m2 / (n - 1)) if n > 1 else np.zeros_like(np.asarray(total, np.float64))
+
+
+def scaled_objective(loss_grad, n: int, std, nc: int, reg_param: float):
+    """Spark's objective in the scaled space x_j / std_j as ``fun(v) -> (value, gradient)`` for :func:`lbfgs.minimize`;
+    v = [w (nc x k, row-major), b (nc)].  ``loss_grad(beta, b)`` gives LogisticAggregator's sums (loss, gradient sums
+    nc x k of multiplier * x_j in the original space, intercept sums) at the effective coefficients beta = w / std (0
+    where std == 0).  value = loss / n + reg/2 * sum(w^2), gradient = (sums_j / std_j) / n + reg * w and b's sums / n."""
+    std = np.asarray(std, np.float64)
+    k, live = len(std), std != 0
+    div = np.where(live, std, 1.0)
+
+    def fun(v):
+        w, b = v[:nc * k].reshape(nc, k), v[nc * k:]
+        loss, g, gb = loss_grad(np.where(live, w / div, 0.0), b)
+        gw = np.where(live, g / div, 0.0) / n + reg_param * w
+        return loss / n + 0.5 * reg_param * float((w * w).sum()), np.concatenate([gw.ravel(), np.asarray(gb) / n])
+
+    return fun
+
+
+def start_point(label_counts, num_classes: int, k: int, multinomial: bool) -> np.ndarray:
+    """Spark's initial point: coefficients 0; binomial intercept log(n_1 / n_0); multinomial intercepts
+    log(n_c + 1) - mean_c log(n_c + 1)."""
+    hist = np.asarray(label_counts[:num_classes], np.float64)
+    nc = num_classes if multinomial else 1
+    v = np.zeros(nc * (k + 1))
+    if multinomial:
+        raw = np.log1p(hist)
+        v[nc * k:] = raw - raw.sum() / len(raw)
+    else:
+        v[k] = math.log(hist[1] / hist[0])
+    return v
+
+
+def unscale(v, std, nc: int, reg_param: float, multinomial: bool) -> tuple[np.ndarray, np.ndarray]:
+    """(coefficient matrix nc x k, intercepts nc) of the scaled-space point v, as Spark leaves them: coef_j / std_j (0
+    where the std is 0); multinomial with reg_param == 0 centres each feature's coefficients across classes; multinomial
+    always centres the intercepts."""
+    std = np.asarray(std, np.float64)
+    k = len(std)
+    w, b = np.array(v[:nc * k]).reshape(nc, k), np.array(v[nc * k:])
+    coef = np.where(std != 0, w / np.where(std != 0, std, 1.0), 0.0)
+    if multinomial and reg_param == 0.0:
+        coef = coef - coef.sum(axis=0) / nc
+    if multinomial:
+        b = b - b.sum() / nc
+    return coef, b
+
+
+class LogisticRegression:
+    """``pyspark.ml.classification.LogisticRegression(maxIter, regParam, tol, family, threshold)`` with its other
+    defaults (``elasticNetParam=0``, ``fitIntercept``, ``standardization``, no ``weightCol``, no bounds) on the GPU."""
+
+    def __init__(self, max_iter: int = 100, reg_param: float = 0.0, tol: float = 1e-6, family: str = "auto",
+                 threshold: float = 0.5):
+        if isinstance(max_iter, bool) or int(max_iter) != max_iter or max_iter < 0:
+            raise ValueError(f"max_iter must be an integer >= 0, not {max_iter!r}")
+        reg, t, th = float(reg_param), float(tol), float(threshold)
+        if not np.isfinite(reg) or reg < 0.0:
+            raise ValueError(f"reg_param must be finite and >= 0, not {reg_param!r}")
+        if not np.isfinite(t) or t <= 0.0:
+            raise ValueError(f"tol must be finite and > 0, not {tol!r}")
+        if family not in FAMILIES:
+            raise ValueError(f"family must be one of {list(FAMILIES)}, not {family!r}")
+        if not 0.0 <= th <= 1.0:
+            raise ValueError(f"threshold must lie in [0, 1], not {threshold!r}")
+        self.max_iter, self.reg_param, self.tol, self.family, self.threshold = int(max_iter), reg, t, family, th
+
+    def fit(self, features) -> "LogisticRegressionModel":
+        """The model of ``features`` (:class:`~builder_frontend.Features` with a label, on one GPU or sharded).  Every
+        label must be an integer >= 0 and every feature finite (InvalidCellError naming the ``_id`` and field of the
+        lowest refused row); numClasses = max label + 1.  No row, a label >= LO_NB_MAX_CLASSES or (binomial ? 2 : C) x k
+        above LO_NB_MAX_THETA are refused, and so is ``family="binomial"`` with more than 2 classes."""
+        from . import lbfgs
+        _usable(features)
+        if features.label is None:
+            raise ValueError("LogisticRegression needs features with a label")
+        k = len(features.fields)
+        least = 2 if self.family == "binomial" else 1        # classes the model has at least: refused before any pass
+        if least * k > N.LO_NB_MAX_THETA:
+            raise N.LoexecError(N.LO_ERR_INVALID, f"{least} classes x {k} features exceed LO_NB_MAX_THETA = "
+                                f"{N.LO_NB_MAX_THETA}")
+        n, total, m2, counts = _on_device(features, lambda engine, rows: engine.lr_stats(rows), name="LogisticRegression",
+                                          reasons=_LR_REASONS)
+        if n == 0:
+            raise N.LoexecError(N.LO_ERR_INVALID, "LogisticRegression needs at least one row")
+        num_classes = int(np.flatnonzero(counts)[-1]) + 1
+        if self.family == "binomial" and num_classes > 2:
+            raise ValueError(f"family='binomial' needs at most 2 classes, the labels give {num_classes}")
+        multinomial = self.family == "multinomial" or (self.family == "auto" and num_classes > 2)
+        if (num_classes if multinomial else 2) * k > N.LO_NB_MAX_THETA:
+            raise N.LoexecError(N.LO_ERR_INVALID, f"{num_classes if multinomial else 2} classes x {k} features exceed "
+                                f"LO_NB_MAX_THETA = {N.LO_NB_MAX_THETA}")
+        nc = num_classes if multinomial else 1
+        std = standardization(n, total, m2)
+        if np.count_nonzero(counts) == 1:                  # constant label: Spark trains nothing
+            intercept = np.zeros(nc)
+            if multinomial:
+                intercept[num_classes - 1] = np.inf
+            else:
+                intercept[0] = np.inf if num_classes == 2 else -np.inf
+            return LogisticRegressionModel(np.zeros((nc, k)), intercept, num_classes, multinomial, features.fields,
+                                           [], 0, self.threshold)
+
+        def loss_grad(beta, b):
+            return _on_device(features, lambda engine, rows: engine.lr_loss_grad(rows, beta, b, multinomial),
+                              name="LogisticRegression", reasons=_LR_REASONS)
+
+        res = lbfgs.minimize(scaled_objective(loss_grad, n, std, nc, self.reg_param),
+                             start_point(counts, num_classes, k, multinomial), self.max_iter, self.tol)
+        coef, intercept = unscale(res.x, std, nc, self.reg_param, multinomial)
+        return LogisticRegressionModel(coef, intercept, num_classes, multinomial, features.fields, res.history,
+                                       res.iterations, self.threshold)
+
+
+class LogisticRegressionModel:
+    """A fitted LogisticRegression model, host data: ``coefficient_matrix`` (float64[C', k]) and ``intercept_vector``
+    (float64[C']) with C' = ``num_classes`` when ``is_multinomial`` else 1; binomial also ``coefficients`` (float64[k])
+    and ``intercept``; ``fields`` it was fitted on; ``objective_history`` (the objective at every optimizer state, the
+    start included; empty for a constant label) and ``iterations``; ``threshold`` of the binomial prediction."""
+
+    def __init__(self, coefficient_matrix, intercept_vector, num_classes, is_multinomial, fields, objective_history=(),
+                 iterations=0, threshold=0.5):
+        self.coefficient_matrix = np.asarray(coefficient_matrix, np.float64)
+        self.intercept_vector = np.asarray(intercept_vector, np.float64)
+        self.num_classes, self.is_multinomial, self.fields = int(num_classes), bool(is_multinomial), list(fields)
+        self.objective_history, self.iterations = list(objective_history), int(iterations)
+        self.threshold = float(threshold)
+        if not self.is_multinomial:
+            self.coefficients, self.intercept = self.coefficient_matrix[0], float(self.intercept_vector[0])
+
+    def _check(self, features) -> None:
+        if list(features.fields) != self.fields:
+            raise ValueError(f"the model was fitted on fields {self.fields}, not {list(features.fields)}")
+
+    def _predict(self, engine, rows, **kw):
+        return engine.lr_predict(rows, self.coefficient_matrix, self.intercept_vector, self.is_multinomial,
+                                 self.threshold, **kw)
+
+    def transform(self, features, raw: bool = False) -> "Predictions":
+        """Spark's ``model.transform``: every row's ``probability`` and ``prediction`` (a class index as float64), and
+        with ``raw`` its ``rawPrediction`` ([-m, m] when binomial), written in HBM on the rows' own devices."""
+        _usable(features)
+        self._check(features)
+        parts = _on_device(features, lambda engine, rows: self._predict(engine, rows, raw=raw), per_part=True,
+                           name="LogisticRegression", reasons=_LR_REASONS)
+        return Predictions(features, parts)
+
+    def evaluate(self, features) -> dict:
+        """``MulticlassClassificationEvaluator`` f1 and accuracy over ``transform(features)``, as
+        :meth:`NaiveBayesModel.evaluate`: ``{"f1", "accuracy", "labels", "confusion"}``."""
+        _usable(features)
+        self._check(features)
+        labels = _labels(features, "LogisticRegression", _LR_REASONS)
+        if len(features.row_ids) == 0:
+            raise N.LoexecError(N.LO_ERR_INVALID, "evaluate needs at least one row")
+        confusion = _on_device(features, lambda engine, rows: self._predict(engine, rows, labels=labels),
+                               name="LogisticRegression", reasons=_LR_REASONS)
+        f1, accuracy = metrics(labels, confusion)
+        return {"f1": f1, "accuracy": accuracy, "labels": labels, "confusion": confusion}
 
 
 class Predictions:

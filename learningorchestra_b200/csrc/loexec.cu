@@ -6,6 +6,7 @@
 #include "loexec.h"
 #include "kernels.cuh"
 #include "naive_bayes.cuh"
+#include "logistic.cuh"
 
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
@@ -2648,6 +2649,88 @@ void nb_tree(HostCall &c, const double *src, int64_t m, size_t slots, double *ds
     }
 }
 
+// lo_nb_predict and lo_lr_predict: the model's C classes (lo::kLrBinomial: C = 1, two outputs per row) over every row,
+// by k_nb_predict with the epilogue `mode`.  The arguments are checked here (ctx and info before).
+int nb_predict(lo_ctx *ctx, const lo_table *x, int64_t ld, int32_t k, int64_t n, const double *pi, const double *theta,
+               int32_t nclasses, int mode, double threshold, lo_table *prob, lo_table *raw, lo_table *pred,
+               const lo_table *y, const double *eval_labels, int32_t neval, int64_t *confusion_out, lo_nb_info *info,
+               lo_host_timing *timing, const char *predict_name, const char *evaluate_name) {
+    const bool eval = confusion_out != nullptr;
+    if (eval && !y) return fail(LO_ERR_INVALID, "evaluate needs y");
+    LO_TRY(check_nb_matrix(ctx, x, ld, k, n, eval ? y : nullptr));
+    const bool binomial = mode == lo::kLrBinomial;
+    LO_TRY(check_nb_caps(binomial ? 2 : nclasses, k));
+    if (!pi || !theta) return fail(LO_ERR_INVALID, "pi or theta is NULL");
+    const int32_t C = nclasses, CO = binomial ? 2 : C;
+    int direct = 0;
+    if (eval) {
+        if (prob || raw || pred) return fail(LO_ERR_INVALID, "evaluate writes no rows: prob, raw and pred must be NULL");
+        LO_TRY(check_nb_classes(eval_labels, neval, "eval_labels", &direct));
+        std::fill(confusion_out, confusion_out + (size_t)neval * CO, (int64_t)0);
+    } else {
+        if (y || eval_labels) return fail(LO_ERR_INVALID, "y and eval_labels go with confusion_out");
+        if (n > 0 && CO > INT64_MAX / 8 / n) return fail(LO_ERR_INVALID, "n * C overflows");
+        LO_TRY(check_float_table(ctx, prob, LO_F64, n * CO, "prob"));
+        LO_TRY(check_float_table(ctx, pred, LO_F64, n, "pred"));
+        if (raw) LO_TRY(check_float_table(ctx, raw, LO_F64, n * CO, "raw"));
+    }
+    HostCall c(ctx, eval ? evaluate_name : predict_name);
+    if (n == 0) return c.finish(timing);
+    // theta j-major for the blocks of classes; raws and the histogram in shared memory when they fit beside the tables
+    std::vector<double> theta_t((size_t)k * C);
+    for (int32_t cc = 0; cc < C; ++cc)
+        for (int32_t j = 0; j < k; ++j) theta_t[(size_t)j * C + cc] = theta[(size_t)cc * k + j];
+    const int64_t base = ((int64_t)k * C + C + lo::kNbTile * (lo::kNbChunk + 1) + (eval ? neval : 0)) * 8;
+    const int64_t raws_bytes = (int64_t)C * lo::kNbTile * 8, hist_bytes = eval ? (int64_t)neval * CO * 4 : 0;
+    const bool raws_smem = base + raws_bytes <= lo::kNbSmemMax;
+    const int64_t with_raws = base + (raws_smem ? raws_bytes : 0);
+    const bool hist_smem = eval && with_raws + hist_bytes <= lo::kNbSmemMax;
+    const int smem = (int)(with_raws + (hist_smem ? hist_bytes : 0));
+    double *d_theta = nullptr, *d_pi = nullptr, *d_evl = nullptr, *raws = nullptr;
+    unsigned long long *conf = nullptr;
+    RefusedCell bad;
+    c.alloc(&d_theta, theta_t.size() * 8);
+    c.alloc(&d_pi, (size_t)C * 8);
+    c.to_dev(d_theta, theta_t.data(), theta_t.size() * 8);
+    c.to_dev(d_pi, pi, (size_t)C * 8);
+    if (eval) {
+        c.alloc(&d_evl, (size_t)neval * 8);
+        c.alloc(&conf, (size_t)neval * CO * 8);
+        c.to_dev(d_evl, eval_labels, (size_t)neval * 8);
+        c.memset(conf, 0, (size_t)neval * CO * 8);
+        bad.arm(c);
+    }
+    auto go = [&](auto kernel, auto tag) {
+        using T = decltype(tag);
+        int per_sm = 0;
+        c.run([&] { return cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem); });
+        c.run([&] { return cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, lo::kNbTile, smem); });
+        const int64_t ntiles = (n + lo::kNbTile - 1) / lo::kNbTile;
+        const int grid = (int)std::min<int64_t>(ntiles, (int64_t)ctx->sm_count * std::max(1, per_sm));
+        if (!raws_smem) c.alloc(&raws, (size_t)grid * raws_bytes);
+        c.mark();
+        c.launch(1, [&] {
+            kernel<<<grid, lo::kNbTile, smem, c.s>>>((const T *)x->base, ld, k, n, d_theta, d_pi, C,
+                                                     prob ? (double *)prob->base : nullptr, raw ? (double *)raw->base : nullptr,
+                                                     pred ? (double *)pred->base : nullptr, y ? (const T *)y->base : nullptr,
+                                                     d_evl, neval, direct, conf, raws, hist_smem ? 1 : 0, bad.word, mode,
+                                                     threshold);
+        });
+        c.mark();
+    };
+    if (x->dtype == LO_F32) {
+        if (eval) go(lo::k_nb_predict<float, true>, 0.0f); else go(lo::k_nb_predict<float, false>, 0.0f);
+    } else {
+        if (eval) go(lo::k_nb_predict<double, true>, 0.0); else go(lo::k_nb_predict<double, false>, 0.0);
+    }
+    if (eval) c.to_host(confusion_out, conf, (size_t)neval * CO * 8);
+    bad.read(c);
+    LO_TRY(c.finish(timing));
+    if (!bad.found(k, info)) return LO_OK;
+    std::fill(confusion_out, confusion_out + (size_t)neval * CO, (int64_t)0);
+    return fail(LO_ERR_INVALID, "row %lld: its label is not one of the evaluated labels", (long long)info->bad_row);
+}
+
 }  // namespace
 
 extern "C" {
@@ -2755,78 +2838,243 @@ int lo_nb_predict(lo_ctx *ctx, const lo_table *x, int64_t ld, int32_t k, int64_t
     LO_TRY(check_ctx(ctx));
     if (!info) return fail(LO_ERR_INVALID, "info is NULL");
     *info = lo_nb_info{-1, -1, 0};
-    const bool eval = confusion_out != nullptr;
-    if (eval && !y) return fail(LO_ERR_INVALID, "evaluate needs y");
-    LO_TRY(check_nb_matrix(ctx, x, ld, k, n, eval ? y : nullptr));
-    LO_TRY(check_nb_caps(nclasses, k));
-    if (!pi || !theta) return fail(LO_ERR_INVALID, "pi or theta is NULL");
-    const int32_t C = nclasses;
-    int direct = 0;
-    if (eval) {
-        if (prob || raw || pred) return fail(LO_ERR_INVALID, "evaluate writes no rows: prob, raw and pred must be NULL");
-        LO_TRY(check_nb_classes(eval_labels, neval, "eval_labels", &direct));
-        std::fill(confusion_out, confusion_out + (size_t)neval * C, (int64_t)0);
-    } else {
-        if (y || eval_labels) return fail(LO_ERR_INVALID, "y and eval_labels go with confusion_out");
-        if (n > 0 && C > INT64_MAX / 8 / n) return fail(LO_ERR_INVALID, "n * C overflows");
-        LO_TRY(check_float_table(ctx, prob, LO_F64, n * C, "prob"));
-        LO_TRY(check_float_table(ctx, pred, LO_F64, n, "pred"));
-        if (raw) LO_TRY(check_float_table(ctx, raw, LO_F64, n * C, "raw"));
+    return nb_predict(ctx, x, ld, k, n, pi, theta, nclasses, lo::kNbSoftmax, 0.0, prob, raw, pred, y, eval_labels, neval, confusion_out,
+                      info, timing, "nb_predict", "nb_evaluate");
+}
+
+}  // extern "C"
+
+static_assert(lo::kLrHist == LO_NB_MAX_CLASSES, "a label bin per class");
+
+namespace {
+
+// The largest power of two R <= kLrTileMax with fixed + R * per_row within kLrSmemMax; 0 when none is
+int lr_rows(int64_t fixed, int64_t per_row) {
+    int R = lo::kLrTileMax;
+    while (R > 0 && fixed + R * per_row > lo::kLrSmemMax) R >>= 1;
+    return R;
+}
+
+int lr_vw(const lo_table *x, int64_t ld) {
+    const int64_t esz = x->dtype == LO_F32 ? 4 : 8;
+    return (uintptr_t)x->base % 16 == 0 && (ld * esz) % 16 == 0 ? (int)(16 / esz) : 1;
+}
+
+// The shape of a stats pass over kc staged columns: one sum per column, G = 256 / kc row groups (at least 1), the label
+// bins of kLrSum beside them.  Every k fits (kc <= kLrStatCols).
+lo::LrShape lr_stats_shape(const lo_table *x, int64_t ld, int kc, bool bins, int *smem) {
+    lo::LrShape sh{};
+    sh.S = kc;
+    sh.kc = kc;
+    sh.ks = kc | 1;
+    sh.G = kc >= lo::kLrThreads ? 1 : lo::kLrThreads / kc;
+    sh.vw = lr_vw(x, ld);
+    const int64_t fixed = (int64_t)sh.G * kc * 8 + (bins ? (lo::kLrHist + 1) * 4 : 0), per_row = ((int64_t)sh.ks + 1) * 8;
+    sh.R = lr_rows(fixed, per_row);
+    *smem = (int)(fixed + sh.R * per_row);
+    return sh;
+}
+
+// The shape of a loss / grad pass of a model of nc rows over k columns: S = 1 + nc (k + 1) sums in blocks of kLrBlockC x
+// kLrBlockJ (plus the loss), G row groups so that about 256 threads own a block, the coefficients in shared memory when
+// that leaves R >= min(32, R without them).  False when no tile fits (not within the caps: the widest, C' = 2 and
+// k = 8192 in f64, fits at R = 1).
+bool lr_model_shape(const lo_table *x, int64_t ld, int32_t k, int32_t nc, lo::LrShape *sh, int *smem) {
+    *sh = lo::LrShape{};
+    sh->S = 1 + nc * (k + 1);
+    sh->kc = k;
+    sh->ks = (k + 1) | 1;
+    sh->vw = lr_vw(x, ld);
+    sh->nbj = (k + 1 + lo::kLrBlockJ - 1) / lo::kLrBlockJ;
+    sh->nb = (nc + lo::kLrBlockC - 1) / lo::kLrBlockC * sh->nbj + 1;
+    sh->G = sh->nb >= lo::kLrThreads ? 1 : lo::kLrThreads / sh->nb;
+    const int64_t fixed = (int64_t)sh->G * sh->S * 8, per_row = ((int64_t)sh->ks + 1 + nc + 1) * 8;
+    const int64_t coef = (int64_t)nc * k * 8;
+    const int bare = lr_rows(fixed, per_row), staged = lr_rows(fixed + coef, per_row);
+    sh->cs = staged > 0 && staged >= std::min(32, bare) ? 1 : 0;
+    sh->R = sh->cs ? staged : bare;
+    *smem = (int)(fixed + (sh->cs ? coef : 0) + sh->R * per_row);
+    return sh->R > 0;
+}
+
+// One pass over rows [0, n) whose CTAs each write `slots` partial sums: rows go in windows whose CTAs' partials fit
+// kNbPartialBytes; launch(r0, r1, partial) runs the pass's kernel over a window, the k_nb_reduce tree adds its partials,
+// then the windows' sums, into sums (device, `slots` doubles).
+template <typename F>
+void lr_windows(HostCall &c, int64_t n, size_t slots, double *sums, F launch) {
+    const int64_t wct = std::max<int64_t>(1, std::min<int64_t>(1 << 20, lo::kNbPartialBytes / (int64_t)(slots * 8)));
+    const int64_t wrows = wct * lo::kLrCtaRows, nw = (n + wrows - 1) / wrows;
+    const int64_t nct = std::min(wct, (n + lo::kLrCtaRows - 1) / lo::kLrCtaRows);
+    const int64_t level1 = (std::max(nct, nw) + lo::kNbFan - 1) / lo::kNbFan;
+    double *partial = nullptr, *wins = nullptr, *buf[2] = {nullptr, nullptr};
+    c.alloc(&partial, (size_t)nct * slots * 8);
+    c.alloc(&wins, (size_t)nw * slots * 8);
+    c.alloc(&buf[0], (size_t)level1 * slots * 8);
+    c.alloc(&buf[1], (size_t)level1 * slots * 8);
+    for (int64_t w = 0; w < nw; ++w) {
+        const int64_t r0 = w * wrows, r1 = std::min(n, r0 + wrows);
+        launch(r0, r1, partial);
+        nb_tree(c, partial, (r1 - r0 + lo::kLrCtaRows - 1) / lo::kLrCtaRows, slots, wins + (size_t)w * slots, buf);
     }
-    HostCall c(ctx, eval ? "nb_evaluate" : "nb_predict");
-    if (n == 0) return c.finish(timing);
-    // theta j-major for the blocks of classes; raws and the histogram in shared memory when they fit beside the tables
-    std::vector<double> theta_t((size_t)k * C);
-    for (int32_t cc = 0; cc < C; ++cc)
-        for (int32_t j = 0; j < k; ++j) theta_t[(size_t)j * C + cc] = theta[(size_t)cc * k + j];
-    const int64_t base = ((int64_t)k * C + C + lo::kNbTile * (lo::kNbChunk + 1) + (eval ? neval : 0)) * 8;
-    const int64_t raws_bytes = (int64_t)C * lo::kNbTile * 8, hist_bytes = eval ? (int64_t)neval * C * 4 : 0;
-    const bool raws_smem = base + raws_bytes <= lo::kNbSmemMax;
-    const int64_t with_raws = base + (raws_smem ? raws_bytes : 0);
-    const bool hist_smem = eval && with_raws + hist_bytes <= lo::kNbSmemMax;
-    const int smem = (int)(with_raws + (hist_smem ? hist_bytes : 0));
-    double *d_theta = nullptr, *d_pi = nullptr, *d_evl = nullptr, *raws = nullptr;
-    unsigned long long *conf = nullptr;
-    RefusedCell bad;
-    c.alloc(&d_theta, theta_t.size() * 8);
-    c.alloc(&d_pi, (size_t)C * 8);
-    c.to_dev(d_theta, theta_t.data(), theta_t.size() * 8);
-    c.to_dev(d_pi, pi, (size_t)C * 8);
-    if (eval) {
-        c.alloc(&d_evl, (size_t)neval * 8);
-        c.alloc(&conf, (size_t)neval * C * 8);
-        c.to_dev(d_evl, eval_labels, (size_t)neval * 8);
-        c.memset(conf, 0, (size_t)neval * C * 8);
-        bad.arm(c);
-    }
-    auto go = [&](auto kernel, auto tag) {
-        using T = decltype(tag);
-        int per_sm = 0;
-        c.run([&] { return cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem); });
-        c.run([&] { return cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, lo::kNbTile, smem); });
-        const int64_t ntiles = (n + lo::kNbTile - 1) / lo::kNbTile;
-        const int grid = (int)std::min<int64_t>(ntiles, (int64_t)ctx->sm_count * std::max(1, per_sm));
-        if (!raws_smem) c.alloc(&raws, (size_t)grid * raws_bytes);
-        c.mark();
+    nb_tree(c, wins, nw, slots, sums, buf);
+}
+
+// one k_lr_stats pass over rows [0, n): sums (device, k doubles) of x (PASS kLrSum: also the label bins and the refused
+// cell) or of (x - mean)^2
+template <typename T, int PASS>
+void lr_stats_pass(HostCall &c, const lo_table *x, int64_t ld, int32_t k, const lo_table *y, int64_t n, const double *mean,
+                   double *sums, unsigned long long *hist, unsigned long long *err) {
+    int smem = 0;
+    const int kc = std::min<int>(k, lo::kLrStatCols);
+    const lo::LrShape sh = lr_stats_shape(x, ld, kc, PASS == lo::kLrSum, &smem);
+    auto kernel = lo::k_lr_stats<T, PASS>;
+    c.run([&] { return cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem); });
+    lr_windows(c, n, (size_t)k, sums, [&](int64_t r0, int64_t r1, double *partial) {
+        const dim3 grid((unsigned)((r1 - r0 + lo::kLrCtaRows - 1) / lo::kLrCtaRows), (unsigned)((k + kc - 1) / kc));
         c.launch(1, [&] {
-            kernel<<<grid, lo::kNbTile, smem, c.s>>>((const T *)x->base, ld, k, n, d_theta, d_pi, C,
-                                                     prob ? (double *)prob->base : nullptr, raw ? (double *)raw->base : nullptr,
-                                                     pred ? (double *)pred->base : nullptr, y ? (const T *)y->base : nullptr,
-                                                     d_evl, neval, direct, conf, raws, hist_smem ? 1 : 0, bad.word);
+            kernel<<<grid, lo::kLrThreads, smem, c.s>>>((const T *)x->base, ld, k, (const T *)y->base, r0, r1, mean, sh,
+                                                        partial, hist, err);
         });
-        c.mark();
-    };
-    if (x->dtype == LO_F32) {
-        if (eval) go(lo::k_nb_predict<float, true>, 0.0f); else go(lo::k_nb_predict<float, false>, 0.0f);
-    } else {
-        if (eval) go(lo::k_nb_predict<double, true>, 0.0); else go(lo::k_nb_predict<double, false>, 0.0);
-    }
-    if (eval) c.to_host(confusion_out, conf, (size_t)neval * C * 8);
+    });
+}
+
+template <typename T, bool MULTI>
+void lr_loss_grad_pass(HostCall &c, const lo_table *x, int64_t ld, int32_t k, const lo_table *y, int64_t n,
+                       const double *coef, const double *icpt, int32_t nc, const lo::LrShape &sh, int smem,
+                       double *sums) {
+    const int S = sh.S;
+    auto kernel = lo::k_lr_loss_grad<T, MULTI>;
+    c.run([&] { return cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem); });
+    lr_windows(c, n, (size_t)S, sums, [&](int64_t r0, int64_t r1, double *partial) {
+        const unsigned grid = (unsigned)((r1 - r0 + lo::kLrCtaRows - 1) / lo::kLrCtaRows);
+        c.launch(1, [&] {
+            kernel<<<grid, lo::kLrThreads, smem, c.s>>>((const T *)x->base, ld, k, (const T *)y->base, r0, r1, coef, icpt,
+                                                        nc, sh, partial);
+        });
+    });
+}
+
+// the model of lo_lr_loss_grad / lo_lr_predict: C' = nclasses rows (1 when binomial) within the caps of lo_nb_predict;
+// training (lo_lr_loss_grad) needs at least 2 classes when multinomial
+int check_lr_model(int32_t nclasses, int32_t multinomial, int32_t k, bool training) {
+    if (multinomial != 0 && multinomial != 1) return fail(LO_ERR_INVALID, "multinomial = %d: 0 or 1", multinomial);
+    if (!multinomial && nclasses != 1)
+        return fail(LO_ERR_INVALID, "a binomial model has one row of coefficients, not %d", nclasses);
+    if (training && multinomial && nclasses < 2)
+        return fail(LO_ERR_INVALID, "a multinomial model of %d class has nothing to train", nclasses);
+    return check_nb_caps(multinomial ? nclasses : 2, k);
+}
+
+}  // namespace
+
+extern "C" {
+
+int lo_lr_stats(lo_ctx *ctx, const lo_table *x, int64_t ld, int32_t k, const lo_table *y, int64_t n, double *sum_out,
+                double *m2_out, int64_t *label_counts_out, lo_nb_info *info, lo_host_timing *timing) {
+    LO_TRY(check_ctx(ctx));
+    if (!info) return fail(LO_ERR_INVALID, "info is NULL");
+    *info = lo_nb_info{-1, -1, 0};
+    if (!y) return fail(LO_ERR_INVALID, "y is NULL");
+    LO_TRY(check_nb_matrix(ctx, x, ld, k, n, y));
+    if (k > LO_NB_MAX_THETA) return fail(LO_ERR_INVALID, "k = %d exceeds LO_NB_MAX_THETA = %d", k, LO_NB_MAX_THETA);
+    if (!sum_out || !m2_out || !label_counts_out) return fail(LO_ERR_INVALID, "sum_out, m2_out or label_counts_out is NULL");
+    std::fill(sum_out, sum_out + k, 0.0);
+    std::fill(m2_out, m2_out + k, 0.0);
+    std::fill(label_counts_out, label_counts_out + LO_NB_MAX_CLASSES, (int64_t)0);
+    HostCall c(ctx, "lr_stats");
+    if (n == 0) return c.finish(timing);
+    double *d_sum = nullptr, *d_mean = nullptr, *d_m2 = nullptr;
+    unsigned long long *hist = nullptr, over = 0;
+    RefusedCell bad;
+    c.alloc(&d_sum, (size_t)k * 8);
+    c.alloc(&d_mean, (size_t)k * 8);
+    c.alloc(&d_m2, (size_t)k * 8);
+    c.alloc(&hist, (lo::kLrHist + 1) * 8);
+    c.memset(hist, 0, (lo::kLrHist + 1) * 8);
+    bad.arm(c);
+    const bool f32 = x->dtype == LO_F32;
+    c.mark();
+    if (f32) lr_stats_pass<float, lo::kLrSum>(c, x, ld, k, y, n, nullptr, d_sum, hist, bad.word);
+    else     lr_stats_pass<double, lo::kLrSum>(c, x, ld, k, y, n, nullptr, d_sum, hist, bad.word);
+    c.mark();
+    static_assert(sizeof(int64_t) == sizeof(unsigned long long), "the bins are read back as int64");
+    c.to_host(sum_out, d_sum, (size_t)k * 8);
+    c.to_host(label_counts_out, hist, (size_t)lo::kLrHist * 8);
+    c.to_host(&over, hist + lo::kLrHist, 8);
     bad.read(c);
+    c.sync();
+    if (c.ok() && bad.key == ~0ull && over == 0) {          // pass 2 about the means of pass 1
+        std::vector<double> mean((size_t)k);
+        for (int32_t j = 0; j < k; ++j) mean[j] = sum_out[j] / (double)n;
+        c.to_dev(d_mean, mean.data(), (size_t)k * 8);
+        c.mark();
+        if (f32) lr_stats_pass<float, lo::kLrM2>(c, x, ld, k, y, n, d_mean, d_m2, nullptr, nullptr);
+        else     lr_stats_pass<double, lo::kLrM2>(c, x, ld, k, y, n, d_mean, d_m2, nullptr, nullptr);
+        c.mark();
+        c.to_host(m2_out, d_m2, (size_t)k * 8);
+    }
     LO_TRY(c.finish(timing));
-    if (!bad.found(k, info)) return LO_OK;
-    std::fill(confusion_out, confusion_out + (size_t)neval * C, (int64_t)0);
-    return fail(LO_ERR_INVALID, "row %lld: its label is not one of the evaluated labels", (long long)info->bad_row);
+    const bool refused = bad.found(k, info);
+    if (!refused && over == 0) return LO_OK;
+    std::fill(sum_out, sum_out + k, 0.0);
+    std::fill(m2_out, m2_out + k, 0.0);
+    std::fill(label_counts_out, label_counts_out + LO_NB_MAX_CLASSES, (int64_t)0);
+    if (!refused)
+        return fail(LO_ERR_INVALID, "%llu rows have a label >= %d: more than LO_NB_MAX_CLASSES classes", over,
+                    LO_NB_MAX_CLASSES);
+    if (info->bad_col == k)
+        return fail(LO_ERR_INVALID, "row %lld: its label is not an integer >= 0", (long long)info->bad_row);
+    return fail(LO_ERR_INVALID, "row %lld, feature %d: NaN or infinite", (long long)info->bad_row, info->bad_col);
+}
+
+int lo_lr_loss_grad(lo_ctx *ctx, const lo_table *x, int64_t ld, int32_t k, const lo_table *y, int64_t n, const double *coef,
+                    const double *intercept, int32_t nclasses, int32_t multinomial, double *out, lo_host_timing *timing) {
+    LO_TRY(check_ctx(ctx));
+    if (!y) return fail(LO_ERR_INVALID, "y is NULL");
+    LO_TRY(check_nb_matrix(ctx, x, ld, k, n, y));
+    LO_TRY(check_lr_model(nclasses, multinomial, k, true));
+    if (!coef || !intercept || !out) return fail(LO_ERR_INVALID, "coef, intercept or out is NULL");
+    const int32_t nc = nclasses;
+    lo::LrShape sh;
+    int smem = 0;
+    if (!lr_model_shape(x, ld, k, nc, &sh, &smem))
+        return fail(LO_ERR_INVALID, "%d classes x %d features: no tile fits the shared memory", nc, k);
+    const size_t slots = 1 + (size_t)nc * (k + 1);
+    std::fill(out, out + slots, 0.0);
+    HostCall c(ctx, "lr_loss_grad");
+    if (n == 0) return c.finish(timing);
+    double *d_coef = nullptr, *d_icpt = nullptr, *d_out = nullptr;
+    c.alloc(&d_coef, (size_t)nc * k * 8);
+    c.alloc(&d_icpt, (size_t)nc * 8);
+    c.alloc(&d_out, slots * 8);
+    c.to_dev(d_coef, coef, (size_t)nc * k * 8);
+    c.to_dev(d_icpt, intercept, (size_t)nc * 8);
+    c.mark();
+    if (x->dtype == LO_F32) {
+        if (multinomial) lr_loss_grad_pass<float, true>(c, x, ld, k, y, n, d_coef, d_icpt, nc, sh, smem, d_out);
+        else             lr_loss_grad_pass<float, false>(c, x, ld, k, y, n, d_coef, d_icpt, nc, sh, smem, d_out);
+    } else {
+        if (multinomial) lr_loss_grad_pass<double, true>(c, x, ld, k, y, n, d_coef, d_icpt, nc, sh, smem, d_out);
+        else             lr_loss_grad_pass<double, false>(c, x, ld, k, y, n, d_coef, d_icpt, nc, sh, smem, d_out);
+    }
+    c.mark();
+    c.to_host(out, d_out, slots * 8);
+    return c.finish(timing);
+}
+
+int lo_lr_predict(lo_ctx *ctx, const lo_table *x, int64_t ld, int32_t k, int64_t n, const double *coef,
+                  const double *intercept, int32_t nclasses, int32_t multinomial, double threshold, lo_table *prob,
+                  lo_table *raw, lo_table *pred, const lo_table *y, const double *eval_labels, int32_t neval,
+                  int64_t *confusion_out, lo_nb_info *info, lo_host_timing *timing) {
+    LO_TRY(check_ctx(ctx));
+    if (!info) return fail(LO_ERR_INVALID, "info is NULL");
+    *info = lo_nb_info{-1, -1, 0};
+    LO_TRY(check_lr_model(nclasses, multinomial, k, false));
+    if (!multinomial && !(threshold >= 0.0 && threshold <= 1.0))
+        return fail(LO_ERR_INVALID, "threshold %g outside [0, 1]", threshold);
+    return nb_predict(ctx, x, ld, k, n, intercept, coef, nclasses, multinomial ? lo::kLrMultinomial : lo::kLrBinomial,
+                      threshold, prob, raw, pred, y, eval_labels,
+                      neval, confusion_out, info, timing, "lr_predict", "lr_evaluate");
 }
 
 }  // extern "C"

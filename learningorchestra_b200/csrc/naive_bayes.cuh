@@ -201,6 +201,40 @@ __device__ __noinline__ int nb_softmax(double *raw, int C) {
     return best;
 }
 
+// BinaryLogisticRegressionModel's raw2probabilityInPlace: p1 = 1 / (1 + exp(-m)) of the margin m (the binomial epilogue
+// of k_nb_predict).  Out of line for the same reason as nb_softmax.
+__device__ __noinline__ double lr_sigmoid(double m) { return 1.0 / (1.0 + exp(-m)); }
+
+// LogisticRegressionModel's multinomial raw2probabilityInPlace and probability2prediction on one row's C raw values
+// (raw[c * kNbTile]): m = the first greatest raw value (Vector.argmax); m == +inf gives probability 1 at its index and 0
+// elsewhere; else e_c = exp(raw_c - m) when m > 0, exp(raw_c) otherwise, summed in c order, p_c = e_c * (1 / sum)
+// (BLAS.scal), and the prediction is Vector.argmax(p).  raw[] receives the probabilities.  Out of line like nb_softmax.
+__device__ __noinline__ int lr_softmax(double *raw, int C) {
+    int at = 0;
+    double m = raw[0];
+    for (int c = 1; c < C; ++c)
+        if (raw[c * kNbTile] > m) { m = raw[c * kNbTile]; at = c; }
+    if (m == INFINITY) {
+        for (int c = 0; c < C; ++c) raw[c * kNbTile] = c == at ? 1.0 : 0.0;
+        return at;
+    }
+    double sum = 0.0;
+    for (int c = 0; c < C; ++c) {
+        const double e = exp(m > 0.0 ? raw[c * kNbTile] - m : raw[c * kNbTile]);
+        raw[c * kNbTile] = e;
+        sum += e;
+    }
+    const double inv = 1.0 / sum;
+    int best = 0;
+    double top = 0.0;
+    for (int c = 0; c < C; ++c) {
+        const double p = raw[c * kNbTile] * inv;
+        raw[c * kNbTile] = p;
+        if (c == 0 || p > top) { best = c; top = p; }
+    }
+    return best;
+}
+
 // Transform / evaluate.  A CTA of kNbTile threads holds thetaT (k x C, j-major) and pi in shared memory and takes tiles
 // of kNbTile rows, one row per thread: chunks of kNbChunk columns are staged as f64 (row stride kNbChunk + 1, so the
 // threads' rows fall on different banks), the raw values of classes c0 .. c0 + kNbBlock are carried in registers over a
@@ -208,7 +242,12 @@ __device__ __noinline__ int nb_softmax(double *raw, int C) {
 // !EVAL: raw (optional), probability and prediction of every row, with streaming stores.  EVAL: nothing per row; the
 // row's label slot a in eval_labels (direct or binary search) and its prediction p count in hist[a * C + p] (shared
 // memory when it fits, flushed once per CTA with integer atomics; else straight into confusion); a label that is not in
-// eval_labels gives the key cell_key(row, k, k) to *err.
+// eval_labels gives the key cell_key(row, k, k) to *err.  mode picks the epilogue (lo_lr_predict): kNbSoftmax NaiveBayes'
+// nb_softmax; kLrBinomial (C = 1, theta the coefficients, pi the intercept) the one raw value m gives two outputs, raw
+// [-m, m], probability [1 - p1, p1] with p1 = lr_sigmoid(m), and prediction p1 > threshold, hist and confusion with 2
+// columns; kLrMultinomial lr_softmax.  A flag rather than a template parameter: the branch is uniform over the launch,
+// and the tiling, staging and dot loop stay one copy per (T, EVAL).
+enum { kNbSoftmax = 0, kLrBinomial = 1, kLrMultinomial = 2 };
 template <typename T, bool EVAL>
 __global__ void __launch_bounds__(kNbTile) k_nb_predict(const T *__restrict__ x, long long ld, int k, long long n,
                                                         const double *__restrict__ theta_t, const double *__restrict__ pi,
@@ -217,8 +256,11 @@ __global__ void __launch_bounds__(kNbTile) k_nb_predict(const T *__restrict__ x,
                                                         const double *__restrict__ eval_labels, int neval, int direct,
                                                         unsigned long long *__restrict__ confusion,
                                                         double *__restrict__ raws_global, int hist_in_smem,
-                                                        unsigned long long *__restrict__ err) {
+                                                        unsigned long long *__restrict__ err, int mode,
+                                                        double threshold) {
     extern __shared__ double nb_smem[];
+    const bool binomial = mode == kLrBinomial;
+    const int CO = binomial ? 2 : C;                        // outputs per row
     double *th = nb_smem;                                   // [k][C]
     double *pis = th + (size_t)k * C;                       // [C]
     double *xt = pis + C;                                   // [kNbTile][kNbChunk + 1]
@@ -230,7 +272,7 @@ __global__ void __launch_bounds__(kNbTile) k_nb_predict(const T *__restrict__ x,
     if (EVAL) {
         for (int i = threadIdx.x; i < neval; i += kNbTile) evl[i] = eval_labels[i];
         if (hist_in_smem)
-            for (int i = threadIdx.x; i < neval * C; i += kNbTile) hist[i] = 0;
+            for (int i = threadIdx.x; i < neval * CO; i += kNbTile) hist[i] = 0;
     }
     const int t = threadIdx.x, warp = t >> 5, lane = t & 31;
     const uint64_t pol = l2_evict_first_policy();
@@ -269,24 +311,39 @@ __global__ void __launch_bounds__(kNbTile) k_nb_predict(const T *__restrict__ x,
         for (int c = 0; c < C; ++c) {
             const double r = __dadd_rn(rr[c * kNbTile], pis[c]);
             rr[c * kNbTile] = r;
-            if (!EVAL && raw_out) __stcs(raw_out + row * C + c, r);
+            if (!EVAL && raw_out && !binomial) __stcs(raw_out + row * C + c, r);
         }
-        const int p = nb_softmax(rr, C);
+        int p;
+        if (binomial) {
+            const double m = rr[0], p1 = lr_sigmoid(m);
+            p = p1 > threshold ? 1 : 0;
+            if (!EVAL) {
+                if (raw_out) {
+                    __stcs(raw_out + row * 2, -m);
+                    __stcs(raw_out + row * 2 + 1, m);
+                }
+                __stcs(prob + row * 2, 1.0 - p1);
+                __stcs(prob + row * 2 + 1, p1);
+            }
+        } else {
+            p = mode == kLrMultinomial ? lr_softmax(rr, C) : nb_softmax(rr, C);
+            if (!EVAL)
+                for (int c = 0; c < C; ++c) __stcs(prob + row * C + c, rr[c * kNbTile]);
+        }
         if (!EVAL) {
-            for (int c = 0; c < C; ++c) __stcs(prob + row * C + c, rr[c * kNbTile]);
             __stcs(pred + row, (double)p);
         } else {
             const int a = nb_class((double)y[row], evl, neval, direct);
             if (a < 0) bad = min(bad, cell_key(row, k, k));
-            else if (hist_in_smem) atomicAdd(&hist[a * C + p], 1u);
-            else atomicAdd(&confusion[(size_t)a * C + p], 1ull);
+            else if (hist_in_smem) atomicAdd(&hist[a * CO + p], 1u);
+            else atomicAdd(&confusion[(size_t)a * CO + p], 1ull);
         }
     }
     if (EVAL) {
         report_cell(bad, err);
         if (hist_in_smem) {
             __syncthreads();
-            for (int i = threadIdx.x; i < neval * C; i += kNbTile)
+            for (int i = threadIdx.x; i < neval * CO; i += kNbTile)
                 if (hist[i]) atomicAdd(&confusion[i], (unsigned long long)hist[i]);
         }
     }

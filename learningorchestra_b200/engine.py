@@ -291,7 +291,8 @@ class DeviceArray:
 
 class InvalidCellError(N.LoexecError):
     """A call refused a cell of the feature matrix: :meth:`Engine.assemble_rows` with ``handle_invalid="error"`` met an
-    invalid cell, :meth:`Engine.nb_fit` / :meth:`Engine.nb_predict` a negative or NaN feature or an unknown label.
+    invalid cell, :meth:`Engine.nb_fit` / :meth:`Engine.nb_predict` a negative or NaN feature or an unknown label,
+    :meth:`Engine.lr_stats` a feature that is not finite or a label that is not an integer >= 0.
     ``row`` is the lowest such row (a source row for assemble_rows, a row of the matrix for the others; global over the
     shards of a :class:`~sharding.ShardedEngine`) and ``position`` its lowest refused column (an index into the sources
     or features; their count: the label).  ``reason``, when given, is the message as a format of ``row`` and
@@ -312,6 +313,7 @@ _ASSEMBLE_REFUSED = ("invalid cell (NaN or code -1) in row {row}, source {positi
 _NB_FEATURE_REFUSED = "row {row}, feature {position}: negative or NaN (NaiveBayes needs values >= 0)"
 _FIT_REFUSED = (_NB_FEATURE_REFUSED, "row {row}: its label is not one of the classes")
 _EVALUATE_REFUSED = (_NB_FEATURE_REFUSED, "row {row}: its label is not one of the evaluated labels")
+_LR_STATS_REFUSED = ("row {row}, feature {position}: NaN or infinite", "row {row}: its label is not an integer >= 0")
 
 
 def _check_cells(rc: int, info, k: int, reasons: tuple[str, str]) -> None:
@@ -1023,6 +1025,78 @@ class Engine:
                                             None, C.byref(info), C.byref(t)))
         _report(timing, t)
         return PredictedRows(prob, rawt, pred, n, nc)
+
+    def lr_stats(self, part: AssembledRows, timing: dict | None = None) -> tuple[int, np.ndarray, np.ndarray, np.ndarray]:
+        """(n, sum float64[k], m2 float64[k], label_counts int64[LO_NB_MAX_CLASSES]) of ``part``'s n rows
+        (``lo_lr_stats``): the f64 sum of every column, the sum of its squared deviations from ``sum / n`` and the rows of
+        each label 0, 1, ....  A
+        feature that is not finite, or a label that is not an integer >= 0, raises :class:`InvalidCellError` naming the
+        lowest row (``position`` the feature; k: the label); a label >= LO_NB_MAX_CLASSES raises LoexecError.
+        ``timing``: a dict to receive the call's lo_host_timing fields."""
+        if part.y is None:
+            raise ValueError("the rows have no label")
+        total, m2 = np.zeros(part.k, np.float64), np.zeros(part.k, np.float64)
+        counts = np.zeros(N.LO_NB_MAX_CLASSES, np.int64)
+        info, t = N.NbInfo(), N.HostTiming()
+        rc = self._lib.lo_lr_stats(self._ctx, part.x._h, part.k, part.k, part.y._h, part.nkept,
+                                   total.ctypes.data_as(C.c_void_p), m2.ctypes.data_as(C.c_void_p),
+                                   counts.ctypes.data_as(C.c_void_p), C.byref(info), C.byref(t))
+        _check_cells(rc, info, part.k, _LR_STATS_REFUSED)
+        _report(timing, t)
+        return part.nkept, total, m2, counts
+
+    def lr_loss_grad(self, part: AssembledRows, coef, intercept, multinomial: bool,
+                     timing: dict | None = None) -> tuple[float, np.ndarray, np.ndarray]:
+        """LogisticAggregator's sums over ``part`` at one point (``lo_lr_loss_grad``): ``coef`` float64[C', k] the
+        effective coefficients (Spark's over the column std), ``intercept`` float64[C'] (C' = 1 when binomial).  Returns
+        (loss sum, gradient sums float64[C', k] of multiplier_c * x_j, intercept sums float64[C'])."""
+        coef = np.ascontiguousarray(coef, dtype=np.float64)
+        intercept = np.ascontiguousarray(intercept, dtype=np.float64)
+        nc = len(intercept)
+        if part.y is None:
+            raise ValueError("the rows have no label")
+        if coef.shape != (nc, part.k):
+            raise ValueError(f"coef has shape {coef.shape}, ({nc}, {part.k}) expected")
+        out = np.zeros(1 + nc * (part.k + 1), np.float64)
+        t = N.HostTiming()
+        N.check(self._lib.lo_lr_loss_grad(self._ctx, part.x._h, part.k, part.k, part.y._h, part.nkept,
+                                          coef.ctypes.data_as(C.c_void_p), intercept.ctypes.data_as(C.c_void_p), nc,
+                                          int(bool(multinomial)), out.ctypes.data_as(C.c_void_p), C.byref(t)))
+        _report(timing, t)
+        return float(out[0]), out[1:1 + nc * part.k].reshape(nc, part.k), out[1 + nc * part.k:]
+
+    def lr_predict(self, part: AssembledRows, coef, intercept, multinomial: bool, threshold: float = 0.5,
+                   raw: bool = False, labels=None, timing: dict | None = None):
+        """A LogisticRegression model (``coef`` float64[C', k], ``intercept`` float64[C']; C' = 1 when binomial) over
+        ``part`` (``lo_lr_predict``), as :meth:`nb_predict`: ``labels`` None gives a :class:`PredictedRows` (2 columns
+        when binomial), else the int64[len(labels), C] confusion counts.  Binomial: prediction p1 > ``threshold``."""
+        coef = np.ascontiguousarray(coef, dtype=np.float64)
+        intercept = np.ascontiguousarray(intercept, dtype=np.float64)
+        nc, n = len(intercept), part.nkept
+        if coef.shape != (nc, part.k):
+            raise ValueError(f"coef has shape {coef.shape}, ({nc}, {part.k}) expected")
+        nout = nc if multinomial else 2
+        info, t = N.NbInfo(), N.HostTiming()
+        args = (self._ctx, part.x._h, part.k, part.k, n, coef.ctypes.data_as(C.c_void_p),
+                intercept.ctypes.data_as(C.c_void_p), nc, int(bool(multinomial)), float(threshold))
+        if labels is not None:
+            if part.y is None:
+                raise ValueError("the rows have no label")
+            lab = np.ascontiguousarray(labels, dtype=np.float64)
+            conf = np.zeros((len(lab), nout), np.int64)
+            rc = self._lib.lo_lr_predict(*args, None, None, None, part.y._h, lab.ctypes.data_as(C.c_void_p), len(lab),
+                                         conf.ctypes.data_as(C.c_void_p), C.byref(info), C.byref(t))
+            _check_cells(rc, info, part.k, _EVALUATE_REFUSED)
+            _report(timing, t)
+            return conf
+        with _Owned() as owned:
+            prob = owned.own(self.table("f64", n * nout, 1))
+            pred = owned.own(self.table("f64", n, 1))
+            rawt = owned.own(self.table("f64", n * nout, 1) if raw else None)
+            N.check(self._lib.lo_lr_predict(*args, prob._h, rawt._h if rawt is not None else None, pred._h, None, None, 0,
+                                            None, C.byref(info), C.byref(t)))
+        _report(timing, t)
+        return PredictedRows(prob, rawt, pred, n, nout)
 
     def value_counts_f64_host(self, values: np.ndarray):
         """(keys float64[g], counts uint64[g]) — exact value counts of a numeric column (GPU hash group-by),

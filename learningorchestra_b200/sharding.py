@@ -777,6 +777,43 @@ class ShardedEngine:
             confusion = confusion + c
         return confusion
 
+    def lr_stats(self, parts):
+        """``Engine.lr_stats`` over the shards, each on its own device from a host thread of its own.  Returns (n, sum,
+        m2, label_counts) of every row: the sums and counts added in shard order, the squared deviations combined by
+        Chan's formula in shard order.  A refused row is raised as the lowest over all shards, its row global."""
+        got = self._each("lr_stats", lambda i: self.engines[i].lr_stats(parts[i]), first_rows=_firsts(parts))
+        n, total, m2, counts = got[0]
+        for m, s, q, c in got[1:]:
+            if m == 0:
+                continue
+            delta = s / m - total / n if n else 0.0
+            m2 = m2 + q + delta * delta * (n * m / (n + m))
+            n, total, counts = n + m, total + s, counts + c
+        return n, total, m2, counts
+
+    def lr_loss_grad(self, parts, coef, intercept, multinomial: bool):
+        """``Engine.lr_loss_grad`` over the shards, each on its own device from a host thread of its own; the loss and
+        the gradient sums added on the host in shard order."""
+        got = self._each("lr_loss_grad", lambda i: self.engines[i].lr_loss_grad(parts[i], coef, intercept, multinomial))
+        loss, grad, icpt = got[0]
+        for lo_, g, b in got[1:]:
+            loss, grad, icpt = loss + lo_, grad + g, icpt + b
+        return loss, grad, icpt
+
+    def lr_predict(self, parts, coef, intercept, multinomial: bool, threshold: float = 0.5, raw: bool = False,
+                   labels=None):
+        """``Engine.lr_predict`` over the shards, as :meth:`nb_predict`: one ``PredictedRows`` per member, or the
+        members' confusion counts summed."""
+        got = self._each("lr_predict", lambda i: self.engines[i].lr_predict(parts[i], coef, intercept, multinomial,
+                                                                            threshold, raw, labels),
+                         undo=(lambda p: p.free()) if labels is None else None, first_rows=_firsts(parts))
+        if labels is None:
+            return got
+        confusion = got[0]
+        for c in got[1:]:
+            confusion = confusion + c
+        return confusion
+
     @property
     def resident(self):
         """Datasets kept in HBM between requests, rows sharded over the group (:mod:`table_cache`)."""
