@@ -531,14 +531,16 @@ int lo_nb_predict(lo_ctx *ctx, const lo_table *x, int64_t ld, int32_t k, int64_t
  * device passes.  DESIGN.md §3.6.3.
  *
  * lo_lr_stats: sum_out[j] (host double[k]) = the f64 sum of column j; m2_out[j] (host double[k]) = the f64 sum of
- * (x_j - sum_out[j] / n)^2 (a second pass, after the first is read back); label_counts_out[c] (host
- * int64[LO_NB_MAX_CLASSES]) = the rows labelled c.  Every label must be an integer >= 0 (NaN, +-inf, negative and
+ * (x_j - sum_out[j] / n)^2 (a second pass, after the first is read back), exactly 0 when column j holds one value
+ * (its least and greatest value equal as doubles, so a column of +0 and -0 is constant); label_counts_out[c] (host
+ * int64[LO_NB_MAX_CLASSES]) = the rows labelled c.  lo_lr_stats_range also writes min_out[j] / max_out[j] (host
+ * double[k]), column j's least / greatest value (0 when n == 0 or the call fails), which shards combine.  Every label must be an integer >= 0 (NaN, +-inf, negative and
  * fractional labels are refused) and every feature finite; else the call fails with LO_ERR_INVALID and info->bad_row /
  * bad_col name the lowest refused row and its lowest refused column (k: the label).  A label >= LO_NB_MAX_CLASSES fails
  * with LO_ERR_INVALID and info->bad_row = -1.  A failed call leaves the outputs zero.  Sums as lo_lr_loss_grad's.
  * Launches: none when n == 0; per pass and window of rows, one k_lr_stats and its k_nb_reduce levels, then the levels over
  * the windows (pass 2 only when pass 1 refused nothing).  Bytes: x read twice, y once.  timing: h2d_bytes the means,
- * d2h_bytes the sums, the label counts and the error word.
+ * d2h_bytes the sums, the min / max, the label counts and the error word.
  *
  * lo_lr_loss_grad: LogisticAggregator at one point.  The model is nclasses rows c of k effective coefficients coef[c * k +
  * j] (host; Spark's coefficient over the column's std, 0 where the std is 0) and intercept[c] (host double[nclasses]).
@@ -571,6 +573,9 @@ int lo_nb_predict(lo_ctx *ctx, const lo_table *x, int64_t ld, int32_t k, int64_t
  * within these caps fits lo_lr_loss_grad's tile in shared memory; a shape that did not would be refused the same way. */
 int lo_lr_stats(lo_ctx *ctx, const lo_table *x, int64_t ld, int32_t k, const lo_table *y, int64_t n, double *sum_out,
                 double *m2_out, int64_t *label_counts_out, lo_nb_info *info, lo_host_timing *timing);
+int lo_lr_stats_range(lo_ctx *ctx, const lo_table *x, int64_t ld, int32_t k, const lo_table *y, int64_t n,
+                      double *sum_out, double *m2_out, double *min_out, double *max_out, int64_t *label_counts_out,
+                      lo_nb_info *info, lo_host_timing *timing);
 int lo_lr_loss_grad(lo_ctx *ctx, const lo_table *x, int64_t ld, int32_t k, const lo_table *y, int64_t n, const double *coef,
                     const double *intercept, int32_t nclasses, int32_t multinomial, double *out, lo_host_timing *timing);
 int lo_lr_predict(lo_ctx *ctx, const lo_table *x, int64_t ld, int32_t k, int64_t n, const double *coef,

@@ -178,6 +178,8 @@ SIGNATURES = {
                                 C.c_int32, _P, C.POINTER(NbInfo), C.POINTER(HostTiming)]),
     "lo_lr_stats": (C.c_int, [_P, _P, C.c_int64, C.c_int32, _P, C.c_int64, _P, _P, _P, C.POINTER(NbInfo),
                               C.POINTER(HostTiming)]),
+    "lo_lr_stats_range": (C.c_int, [_P, _P, C.c_int64, C.c_int32, _P, C.c_int64, _P, _P, _P, _P, _P, C.POINTER(NbInfo),
+                                    C.POINTER(HostTiming)]),
     "lo_lr_loss_grad": (C.c_int, [_P, _P, C.c_int64, C.c_int32, _P, C.c_int64, _P, _P, C.c_int32, C.c_int32, _P,
                                   C.POINTER(HostTiming)]),
     "lo_lr_predict": (C.c_int, [_P, _P, C.c_int64, C.c_int32, C.c_int64, _P, _P, C.c_int32, C.c_int32, C.c_double, _P,

@@ -2860,8 +2860,9 @@ int lr_vw(const lo_table *x, int64_t ld) {
     return (uintptr_t)x->base % 16 == 0 && (ld * esz) % 16 == 0 ? (int)(16 / esz) : 1;
 }
 
-// The shape of a stats pass over kc staged columns: one sum per column, G = 256 / kc row groups (at least 1), the label
-// bins of kLrSum beside them.  Every k fits (kc <= kLrStatCols).
+// The shape of a stats pass over kc staged columns: one sum per column, G = 256 / kc row groups (at least 1), the min /
+// max and the label bins of kLrSum beside them.  Every k fits (kc <= kLrStatCols).  R does not set a sum's order where
+// G = 1, and where G > 1 it is kLrTileMax whether kLrSum's min / max are there or not.
 lo::LrShape lr_stats_shape(const lo_table *x, int64_t ld, int kc, bool bins, int *smem) {
     lo::LrShape sh{};
     sh.S = kc;
@@ -2869,7 +2870,8 @@ lo::LrShape lr_stats_shape(const lo_table *x, int64_t ld, int kc, bool bins, int
     sh.ks = kc | 1;
     sh.G = kc >= lo::kLrThreads ? 1 : lo::kLrThreads / kc;
     sh.vw = lr_vw(x, ld);
-    const int64_t fixed = (int64_t)sh.G * kc * 8 + (bins ? (lo::kLrHist + 1) * 4 : 0), per_row = ((int64_t)sh.ks + 1) * 8;
+    const int64_t fixed = (int64_t)sh.G * kc * 8 * (bins ? 3 : 1) + (bins ? (lo::kLrHist + 1) * 4 : 0);
+    const int64_t per_row = ((int64_t)sh.ks + 1) * 8;
     sh.R = lr_rows(fixed, per_row);
     *smem = (int)(fixed + sh.R * per_row);
     return sh;
@@ -2919,11 +2921,11 @@ void lr_windows(HostCall &c, int64_t n, size_t slots, double *sums, F launch) {
     nb_tree(c, wins, nw, slots, sums, buf);
 }
 
-// one k_lr_stats pass over rows [0, n): sums (device, k doubles) of x (PASS kLrSum: also the label bins and the refused
-// cell) or of (x - mean)^2
+// one k_lr_stats pass over rows [0, n): sums (device, k doubles) of x (PASS kLrSum: also the columns' min / max in ext,
+// the label bins and the refused cell) or of (x - mean)^2
 template <typename T, int PASS>
 void lr_stats_pass(HostCall &c, const lo_table *x, int64_t ld, int32_t k, const lo_table *y, int64_t n, const double *mean,
-                   double *sums, unsigned long long *hist, unsigned long long *err) {
+                   double *sums, unsigned long long *hist, unsigned long long *ext, unsigned long long *err) {
     int smem = 0;
     const int kc = std::min<int>(k, lo::kLrStatCols);
     const lo::LrShape sh = lr_stats_shape(x, ld, kc, PASS == lo::kLrSum, &smem);
@@ -2933,7 +2935,7 @@ void lr_stats_pass(HostCall &c, const lo_table *x, int64_t ld, int32_t k, const 
         const dim3 grid((unsigned)((r1 - r0 + lo::kLrCtaRows - 1) / lo::kLrCtaRows), (unsigned)((k + kc - 1) / kc));
         c.launch(1, [&] {
             kernel<<<grid, lo::kLrThreads, smem, c.s>>>((const T *)x->base, ld, k, (const T *)y->base, r0, r1, mean, sh,
-                                                        partial, hist, err);
+                                                        partial, hist, ext, err);
         });
     });
 }
@@ -2969,36 +2971,45 @@ int check_lr_model(int32_t nclasses, int32_t multinomial, int32_t k, bool traini
 
 extern "C" {
 
-int lo_lr_stats(lo_ctx *ctx, const lo_table *x, int64_t ld, int32_t k, const lo_table *y, int64_t n, double *sum_out,
-                double *m2_out, int64_t *label_counts_out, lo_nb_info *info, lo_host_timing *timing) {
+int lo_lr_stats_range(lo_ctx *ctx, const lo_table *x, int64_t ld, int32_t k, const lo_table *y, int64_t n,
+                      double *sum_out, double *m2_out, double *min_out, double *max_out, int64_t *label_counts_out,
+                      lo_nb_info *info, lo_host_timing *timing) {
     LO_TRY(check_ctx(ctx));
     if (!info) return fail(LO_ERR_INVALID, "info is NULL");
     *info = lo_nb_info{-1, -1, 0};
     if (!y) return fail(LO_ERR_INVALID, "y is NULL");
     LO_TRY(check_nb_matrix(ctx, x, ld, k, n, y));
     if (k > LO_NB_MAX_THETA) return fail(LO_ERR_INVALID, "k = %d exceeds LO_NB_MAX_THETA = %d", k, LO_NB_MAX_THETA);
-    if (!sum_out || !m2_out || !label_counts_out) return fail(LO_ERR_INVALID, "sum_out, m2_out or label_counts_out is NULL");
-    std::fill(sum_out, sum_out + k, 0.0);
-    std::fill(m2_out, m2_out + k, 0.0);
-    std::fill(label_counts_out, label_counts_out + LO_NB_MAX_CLASSES, (int64_t)0);
+    if (!sum_out || !m2_out || !min_out || !max_out || !label_counts_out)
+        return fail(LO_ERR_INVALID, "sum_out, m2_out, min_out, max_out or label_counts_out is NULL");
+    auto clear = [&] {
+        for (double *o : {sum_out, m2_out, min_out, max_out}) std::fill(o, o + k, 0.0);
+        std::fill(label_counts_out, label_counts_out + LO_NB_MAX_CLASSES, (int64_t)0);
+    };
+    clear();
     HostCall c(ctx, "lr_stats");
     if (n == 0) return c.finish(timing);
     double *d_sum = nullptr, *d_mean = nullptr, *d_m2 = nullptr;
-    unsigned long long *hist = nullptr, over = 0;
+    unsigned long long *hist = nullptr, *ext = nullptr, over = 0;
+    std::vector<unsigned long long> ordered((size_t)2 * k);
     RefusedCell bad;
     c.alloc(&d_sum, (size_t)k * 8);
     c.alloc(&d_mean, (size_t)k * 8);
     c.alloc(&d_m2, (size_t)k * 8);
     c.alloc(&hist, (lo::kLrHist + 1) * 8);
+    c.alloc(&ext, (size_t)2 * k * 8);
     c.memset(hist, 0, (lo::kLrHist + 1) * 8);
+    c.memset(ext, 0xff, (size_t)k * 8);                    // the identities: all ones for the min, 0 for the max
+    c.memset(ext + k, 0, (size_t)k * 8);
     bad.arm(c);
     const bool f32 = x->dtype == LO_F32;
     c.mark();
-    if (f32) lr_stats_pass<float, lo::kLrSum>(c, x, ld, k, y, n, nullptr, d_sum, hist, bad.word);
-    else     lr_stats_pass<double, lo::kLrSum>(c, x, ld, k, y, n, nullptr, d_sum, hist, bad.word);
+    if (f32) lr_stats_pass<float, lo::kLrSum>(c, x, ld, k, y, n, nullptr, d_sum, hist, ext, bad.word);
+    else     lr_stats_pass<double, lo::kLrSum>(c, x, ld, k, y, n, nullptr, d_sum, hist, ext, bad.word);
     c.mark();
     static_assert(sizeof(int64_t) == sizeof(unsigned long long), "the bins are read back as int64");
     c.to_host(sum_out, d_sum, (size_t)k * 8);
+    c.to_host(ordered.data(), ext, (size_t)2 * k * 8);
     c.to_host(label_counts_out, hist, (size_t)lo::kLrHist * 8);
     c.to_host(&over, hist + lo::kLrHist, 8);
     bad.read(c);
@@ -3008,23 +3019,41 @@ int lo_lr_stats(lo_ctx *ctx, const lo_table *x, int64_t ld, int32_t k, const lo_
         for (int32_t j = 0; j < k; ++j) mean[j] = sum_out[j] / (double)n;
         c.to_dev(d_mean, mean.data(), (size_t)k * 8);
         c.mark();
-        if (f32) lr_stats_pass<float, lo::kLrM2>(c, x, ld, k, y, n, d_mean, d_m2, nullptr, nullptr);
-        else     lr_stats_pass<double, lo::kLrM2>(c, x, ld, k, y, n, d_mean, d_m2, nullptr, nullptr);
+        if (f32) lr_stats_pass<float, lo::kLrM2>(c, x, ld, k, y, n, d_mean, d_m2, nullptr, nullptr, nullptr);
+        else     lr_stats_pass<double, lo::kLrM2>(c, x, ld, k, y, n, d_mean, d_m2, nullptr, nullptr, nullptr);
         c.mark();
         c.to_host(m2_out, d_m2, (size_t)k * 8);
     }
     LO_TRY(c.finish(timing));
     const bool refused = bad.found(k, info);
-    if (!refused && over == 0) return LO_OK;
-    std::fill(sum_out, sum_out + k, 0.0);
-    std::fill(m2_out, m2_out + k, 0.0);
-    std::fill(label_counts_out, label_counts_out + LO_NB_MAX_CLASSES, (int64_t)0);
+    if (!refused && over == 0) {
+        // back from lo::lr_ordered; a column whose min equals its max (as doubles: -0 == +0) has m2 exactly 0, not the
+        // n ulp^2 that its rounded mean sum / n leaves
+        for (int32_t j = 0; j < k; ++j) {
+            for (int side = 0; side < 2; ++side) {
+                const unsigned long long o = ordered[(size_t)side * k + j];
+                const unsigned long long b = o >> 63 ? o & ~(1ull << 63) : ~o;
+                std::memcpy(side ? &max_out[j] : &min_out[j], &b, 8);
+            }
+            if (min_out[j] == max_out[j]) m2_out[j] = 0.0;
+        }
+        return LO_OK;
+    }
+    clear();
     if (!refused)
         return fail(LO_ERR_INVALID, "%llu rows have a label >= %d: more than LO_NB_MAX_CLASSES classes", over,
                     LO_NB_MAX_CLASSES);
     if (info->bad_col == k)
         return fail(LO_ERR_INVALID, "row %lld: its label is not an integer >= 0", (long long)info->bad_row);
     return fail(LO_ERR_INVALID, "row %lld, feature %d: NaN or infinite", (long long)info->bad_row, info->bad_col);
+}
+
+int lo_lr_stats(lo_ctx *ctx, const lo_table *x, int64_t ld, int32_t k, const lo_table *y, int64_t n, double *sum_out,
+                double *m2_out, int64_t *label_counts_out, lo_nb_info *info, lo_host_timing *timing) {
+    // the range's outputs for a k the call accepts (any other k is refused before they are touched)
+    std::vector<double> least(k >= 1 && k <= LO_NB_MAX_THETA ? (size_t)k : 0), most(least.size());
+    return lo_lr_stats_range(ctx, x, ld, k, y, n, sum_out, m2_out, least.data(), most.data(), label_counts_out, info,
+                             timing);
 }
 
 int lo_lr_loss_grad(lo_ctx *ctx, const lo_table *x, int64_t ld, int32_t k, const lo_table *y, int64_t n, const double *coef,

@@ -1,8 +1,8 @@
 // logistic.cuh — Spark 2.4's LogisticRegression over the feature matrix in HBM (lo_lr_stats, lo_lr_loss_grad;
 // DESIGN.md §3.6.3).  Included by loexec.cu after naive_bayes.cuh, whose read-once loads it uses; the partials it writes
 // are reduced by k_nb_reduce, and transform / evaluate run in k_nb_predict (its binomial epilogue is lr_sigmoid).
-//   * k_lr_stats<T, PASS>: per-column sums of x (PASS kLrSum, with the label histogram and the refused cells) or of
-//     (x_j - mean_j)^2 (PASS kLrM2).
+//   * k_lr_stats<T, PASS>: per-column sums of x (PASS kLrSum, with each column's min and max, the label histogram and
+//     the refused cells) or of (x_j - mean_j)^2 (PASS kLrM2).
 //   * k_lr_loss_grad<T, MULTI>: LogisticAggregator's loss and gradient sums at one point, one read of every row.
 // Both add every sum in a fixed order, in per-thread runs of at most kLrCtaRows rows, with no floating-point atomics.
 #pragma once
@@ -35,6 +35,12 @@ struct LrShape {
     int nb;     // loss / grad: blocks of kLrBlockC x kLrBlockJ sums, plus one for the loss
     int cs;     // loss / grad: the coefficients staged in shared memory (else read from global memory)
 };
+
+// A double's order as a u64 (-0 below +0), so that integer atomicMin / atomicMax find a column's min and max
+__device__ __forceinline__ unsigned long long lr_ordered(double v) {
+    const unsigned long long b = (unsigned long long)__double_as_longlong(v);
+    return b >> 63 ? ~b : b | (1ull << 63);
+}
 
 // Spark's MLUtils.log1pExp
 __device__ __forceinline__ double lr_log1p_exp(double v) { return v > 0.0 ? v + log1p(exp(-v)) : log1p(exp(v)); }
@@ -81,7 +87,9 @@ __device__ __forceinline__ void lr_stage(const T *__restrict__ x, long long ld, 
 // own acc[g][.] (one more block adds the loss).  Sum slots: 0 the loss, 1 + c k + j the multiplier_c x_j, 1 + C' k + c
 // the multiplier_c (column k).  Every sum has one owner thread and a fixed row order.  At the end acc[0..G)[s] is added
 // in g order into
-// partial[b * pstride + chunk * kc + s].  kLrSum also counts the labels (integer-valued, >= 0; bin kLrHist: >= kLrHist)
+// partial[b * pstride + chunk * kc + s].  kLrSum also keeps every (g, s)'s min and max of the column (in shared memory
+// beside acc) and merges them per column into ext[j] (lr_ordered min) and ext[k + j] (max) by integer atomics, which
+// are exact in any order, so a constant column is known as one whatever the sum's rounding; it also counts the labels (integer-valued, >= 0; bin kLrHist: >= kLrHist)
 // into hist_out by integer atomics and gives the lowest refused cell's key to *err: a feature that is not finite, or a
 // label (column k) that is NaN, infinite, negative or fractional.
 template <typename T, int MODE>   // MODE: kLrSum, kLrM2, 2 + binomial / multinomial
@@ -89,7 +97,8 @@ __device__ __forceinline__ void lr_pass(const T *__restrict__ x, long long ld, i
                                         long long row0, long long row1, const double *__restrict__ coef,
                                         const double *__restrict__ icpt, int nc, const double *__restrict__ mean,
                                         LrShape sh, double *__restrict__ partial, long long pstride,
-                                        unsigned long long *__restrict__ hist_out, unsigned long long *__restrict__ err) {
+                                        unsigned long long *__restrict__ hist_out, unsigned long long *__restrict__ ext,
+                                        unsigned long long *__restrict__ err) {
     constexpr bool MODEL = MODE >= 2, MULTI = MODE == 3;
     extern __shared__ double lr_smem[];
     const int R = sh.R, G = sh.G, ks = sh.ks;
@@ -102,10 +111,16 @@ __device__ __forceinline__ void lr_pass(const T *__restrict__ x, long long ld, i
     double *lossr = mult + (MODEL ? (size_t)R * nc : 0);           // [R]
     double *acc = lossr + (MODEL ? R : 0);                         // [G][sh.S]
     double *coef_s = acc + (size_t)G * sh.S;                       // [nc][k] (MODEL, sh.cs)
-    unsigned *hist = reinterpret_cast<unsigned *>(acc + (size_t)G * sh.S);     // [kLrHist + 1] (kLrSum)
+    double *lo = acc + (size_t)G * sh.S, *hi = lo + (size_t)G * sh.S;                // [G][sh.S] each (kLrSum)
+    unsigned *hist = reinterpret_cast<unsigned *>(hi + (size_t)G * sh.S);       // [kLrHist + 1] (kLrSum)
     for (int i = threadIdx.x; i < G * sh.S; i += kLrThreads) acc[i] = 0.0;
-    if (MODE == kLrSum)
+    if (MODE == kLrSum) {
+        for (int i = threadIdx.x; i < G * sh.S; i += kLrThreads) {
+            lo[i] = INFINITY;
+            hi[i] = -INFINITY;
+        }
         for (int i = threadIdx.x; i <= kLrHist; i += kLrThreads) hist[i] = 0;
+    }
     if (MODEL && sh.cs)
         for (int i = threadIdx.x; i < nc * k; i += kLrThreads) coef_s[i] = coef[i];
     const double *cf = MODEL && sh.cs ? coef_s : coef;
@@ -220,7 +235,15 @@ __device__ __forceinline__ void lr_pass(const T *__restrict__ x, long long ld, i
             const int g = u / S, s = u - g * S;
             double a = acc[g * sh.S + s];
             if (MODE == kLrSum) {
-                for (int r = g; r < nr; r += G) a += xs[r * ks + s];
+                double l = lo[g * sh.S + s], h = hi[g * sh.S + s];
+                for (int r = g; r < nr; r += G) {
+                    const double v = xs[r * ks + s];
+                    a += v;
+                    l = fmin(l, v);
+                    h = fmax(h, v);
+                }
+                lo[g * sh.S + s] = l;
+                hi[g * sh.S + s] = h;
             } else {
                 const double mu = __ldg(mean + j0 + s);
                 for (int r = g; r < nr; r += G) {
@@ -238,6 +261,15 @@ __device__ __forceinline__ void lr_pass(const T *__restrict__ x, long long ld, i
         double v = acc[s];
         for (int g = 1; g < G; ++g) v += acc[g * sh.S + s];
         out[s] = v;
+        if (MODE == kLrSum) {
+            double l = lo[s], h = hi[s];
+            for (int g = 1; g < G; ++g) {
+                l = fmin(l, lo[g * sh.S + s]);
+                h = fmax(h, hi[g * sh.S + s]);
+            }
+            atomicMin(&ext[j0 + s], lr_ordered(l));
+            atomicMax(&ext[k + j0 + s], lr_ordered(h));
+        }
     }
     if (MODE == kLrSum && blockIdx.y == 0)
         for (int i = threadIdx.x; i <= kLrHist; i += kLrThreads)
@@ -249,8 +281,9 @@ __global__ void __launch_bounds__(kLrThreads) k_lr_stats(const T *__restrict__ x
                                                          long long row0, long long row1, const double *__restrict__ mean,
                                                          LrShape sh, double *__restrict__ partial,
                                                          unsigned long long *__restrict__ hist,
+                                                         unsigned long long *__restrict__ ext,
                                                          unsigned long long *__restrict__ err) {
-    lr_pass<T, PASS>(x, ld, k, y, row0, row1, nullptr, nullptr, 0, mean, sh, partial, k, hist, err);
+    lr_pass<T, PASS>(x, ld, k, y, row0, row1, nullptr, nullptr, 0, mean, sh, partial, k, hist, ext, err);
 }
 
 template <typename T, bool MULTI>
@@ -258,7 +291,7 @@ __global__ void __launch_bounds__(kLrThreads) k_lr_loss_grad(const T *__restrict
                                                              const T *__restrict__ y, long long row0, long long row1,
                                                              const double *__restrict__ coef, const double *__restrict__ icpt,
                                                              int nc, LrShape sh, double *__restrict__ partial) {
-    lr_pass<T, MULTI ? 3 : 2>(x, ld, k, y, row0, row1, coef, icpt, nc, nullptr, sh, partial, sh.S, nullptr, nullptr);
+    lr_pass<T, MULTI ? 3 : 2>(x, ld, k, y, row0, row1, coef, icpt, nc, nullptr, sh, partial, sh.S, nullptr, nullptr, nullptr);
 }
 
 }  // namespace lo

@@ -367,6 +367,17 @@ class AssembledRows:
                 t.free()
 
 
+class ColumnStats(tuple):
+    """What :meth:`Engine.lr_stats` returns: the tuple (n, sum, m2, label_counts), and ``min`` / ``max`` (float64[k]),
+    every column's least and greatest value, by which :meth:`ShardedEngine.lr_stats` finds the columns that hold one
+    value over all shards."""
+
+    def __new__(cls, n, total, m2, counts, least, most):
+        self = super().__new__(cls, (n, total, m2, counts))
+        self.min, self.max = least, most
+        return self
+
+
 class PredictedRows:
     """What :meth:`Engine.nb_predict` wrote for one device's rows: ``prob`` (n x C f64, row-major), ``pred`` (n f64 class
     indices) and ``raw`` (n x C f64, or None).  :meth:`probability` / :meth:`prediction` / :meth:`raw_view` view them in
@@ -1026,24 +1037,27 @@ class Engine:
         _report(timing, t)
         return PredictedRows(prob, rawt, pred, n, nc)
 
-    def lr_stats(self, part: AssembledRows, timing: dict | None = None) -> tuple[int, np.ndarray, np.ndarray, np.ndarray]:
+    def lr_stats(self, part: AssembledRows, timing: dict | None = None) -> "ColumnStats":
         """(n, sum float64[k], m2 float64[k], label_counts int64[LO_NB_MAX_CLASSES]) of ``part``'s n rows
-        (``lo_lr_stats``): the f64 sum of every column, the sum of its squared deviations from ``sum / n`` and the rows of
-        each label 0, 1, ....  A
+        (``lo_lr_stats_range``), a :class:`ColumnStats`: the f64 sum of every column, the sum of its squared deviations
+        from ``sum / n`` (exactly 0 for a constant column) and the rows of each label 0, 1, ...; ``.min`` / ``.max`` every
+        column's least and greatest value.  A
         feature that is not finite, or a label that is not an integer >= 0, raises :class:`InvalidCellError` naming the
         lowest row (``position`` the feature; k: the label); a label >= LO_NB_MAX_CLASSES raises LoexecError.
         ``timing``: a dict to receive the call's lo_host_timing fields."""
         if part.y is None:
             raise ValueError("the rows have no label")
         total, m2 = np.zeros(part.k, np.float64), np.zeros(part.k, np.float64)
+        least, most = np.zeros(part.k, np.float64), np.zeros(part.k, np.float64)
         counts = np.zeros(N.LO_NB_MAX_CLASSES, np.int64)
         info, t = N.NbInfo(), N.HostTiming()
-        rc = self._lib.lo_lr_stats(self._ctx, part.x._h, part.k, part.k, part.y._h, part.nkept,
-                                   total.ctypes.data_as(C.c_void_p), m2.ctypes.data_as(C.c_void_p),
-                                   counts.ctypes.data_as(C.c_void_p), C.byref(info), C.byref(t))
+        rc = self._lib.lo_lr_stats_range(self._ctx, part.x._h, part.k, part.k, part.y._h, part.nkept,
+                                         total.ctypes.data_as(C.c_void_p), m2.ctypes.data_as(C.c_void_p),
+                                         least.ctypes.data_as(C.c_void_p), most.ctypes.data_as(C.c_void_p),
+                                         counts.ctypes.data_as(C.c_void_p), C.byref(info), C.byref(t))
         _check_cells(rc, info, part.k, _LR_STATS_REFUSED)
         _report(timing, t)
-        return part.nkept, total, m2, counts
+        return ColumnStats(part.nkept, total, m2, counts, least, most)
 
     def lr_loss_grad(self, part: AssembledRows, coef, intercept, multinomial: bool,
                      timing: dict | None = None) -> tuple[float, np.ndarray, np.ndarray]:

@@ -780,7 +780,10 @@ class ShardedEngine:
     def lr_stats(self, parts):
         """``Engine.lr_stats`` over the shards, each on its own device from a host thread of its own.  Returns (n, sum,
         m2, label_counts) of every row: the sums and counts added in shard order, the squared deviations combined by
-        Chan's formula in shard order.  A refused row is raised as the lowest over all shards, its row global."""
+        Chan's formula in shard order, and exactly 0 for a column whose every row holds one value (the shards' rounded
+        means of it may differ).  A refused row is raised as the lowest over all shards, its row global."""
+        import numpy as np
+        from .engine import ColumnStats
         got = self._each("lr_stats", lambda i: self.engines[i].lr_stats(parts[i]), first_rows=_firsts(parts))
         n, total, m2, counts = got[0]
         for m, s, q, c in got[1:]:
@@ -789,6 +792,11 @@ class ShardedEngine:
             delta = s / m - total / n if n else 0.0
             m2 = m2 + q + delta * delta * (n * m / (n + m))
             n, total, counts = n + m, total + s, counts + c
+        held = [g for g in got if g[0] > 0]
+        if held and all(isinstance(g, ColumnStats) for g in held):     # every member's column range known
+            least = np.min([g.min for g in held], axis=0)
+            most = np.max([g.max for g in held], axis=0)
+            m2 = np.where(least == most, 0.0, m2)
         return n, total, m2, counts
 
     def lr_loss_grad(self, parts, coef, intercept, multinomial: bool):

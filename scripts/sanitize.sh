@@ -29,9 +29,15 @@ echo "memcheck (refused cells) rc=$? log=$refused_log"; tail -3 "$refused_log"
 # memcheck of the LogisticRegression kernels (stats, loss / gradient, the binomial predict; every shape, cap and
 # refusal); its log goes to a temporary directory
 lr_log="$(mktemp -d)/sanitizer_memcheck_logistic.txt"
-timeout 1800 compute-sanitizer --tool memcheck --error-exitcode 1 python -m pytest tests/test_gpu_logistic.py -q \
-    > "$lr_log" 2>&1
+timeout 1800 compute-sanitizer --tool memcheck --error-exitcode 1 python -m pytest tests/test_gpu_logistic.py \
+    tests/test_gpu_logistic_exact.py -q > "$lr_log" 2>&1
 echo "memcheck (logistic) rc=$? log=$lr_log"; tail -3 "$lr_log"
+# racecheck of k_lr_stats / k_lr_loss_grad (four shared-memory phases per tile) over every launch shape; its log goes to
+# a temporary directory
+lr_race_log="$(mktemp -d)/sanitizer_racecheck_logistic.txt"
+timeout 1800 compute-sanitizer --tool racecheck --error-exitcode 1 python -m pytest tests/test_gpu_logistic_exact.py -q \
+    -k "shape" > "$lr_race_log" 2>&1
+echo "racecheck (logistic) rc=$? log=$lr_race_log"; tail -3 "$lr_race_log"
 # memcheck of the number parser and the resident formatter on every entry point, without the million-row cases: a read
 # past the last staged cell shows here (the CPU harness puts a NUL after it)
 parse_log="$(mktemp -d)/sanitizer_memcheck_parse.txt"

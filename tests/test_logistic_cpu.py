@@ -13,7 +13,7 @@ import logistic_oracle as lo
 from learningorchestra_b200 import _native, lbfgs
 from learningorchestra_b200.classifier import (LogisticRegression, LogisticRegressionModel, NaiveBayes, scaled_objective,
                                                standardization, start_point, unscale)
-from learningorchestra_b200.engine import InvalidCellError
+from learningorchestra_b200.engine import ColumnStats, InvalidCellError
 from learningorchestra_b200.sharding import ShardedEngine
 
 from test_naive_bayes_cpu import _sass_with_offsets
@@ -44,6 +44,32 @@ def test_ctypes_mirror_of_the_logistic_entry_points_matches_the_header():
                                                                C.c_int32, P, T])
     assert _native.SIGNATURES["lo_lr_predict"] == (C.c_int, [P, P, C.c_int64, C.c_int32, C.c_int64, P, P, C.c_int32,
                                                              C.c_int32, C.c_double, P, P, P, P, P, C.c_int32, P, I, T])
+
+
+def test_ctypes_mirror_of_lo_lr_stats_range_matches_the_header():
+    text = re.sub(r"/\*.*?\*/", "", HEADER.read_text(), flags=re.S)
+    params = [p.strip() for p in re.search(r"\blo_lr_stats_range\s*\(([^)]*)\)", text).group(1).split(",")]
+    assert params == ["lo_ctx *ctx", "const lo_table *x", "int64_t ld", "int32_t k", "const lo_table *y", "int64_t n",
+                      "double *sum_out", "double *m2_out", "double *min_out", "double *max_out",
+                      "int64_t *label_counts_out", "lo_nb_info *info", "lo_host_timing *timing"]
+    P, T, I = C.c_void_p, C.POINTER(_native.HostTiming), C.POINTER(_native.NbInfo)
+    assert _native.SIGNATURES["lo_lr_stats_range"] == (C.c_int, [P, P, C.c_int64, C.c_int32, P, C.c_int64, P, P, P, P, P,
+                                                                 I, T])
+
+
+def test_launch_shape_mirror_matches_logistic_cuh():
+    """tests/test_gpu_logistic_exact.py picks its parameter sets from a restatement of lr_stats_shape / lr_model_shape:
+    its constants are csrc/logistic.cuh's, its formulas loexec.cu's, and its sets still reach every launch shape."""
+    import test_gpu_logistic_exact as ex
+    csrc = HEADER.parent.parent / "learningorchestra_b200" / "csrc"
+    found = {name: eval(value) for name, value in
+             re.findall(r"constexpr int (kLr\w+) = ([0-9 *]+);", (csrc / "logistic.cuh").read_text())}
+    assert found == ex.CONSTANTS
+    assert all(ex.shape_coverage().values()), ex.shape_coverage()
+    cu = (csrc / "loexec.cu").read_text()
+    assert "(int64_t)sh.G * kc * 8 * (bins ? 3 : 1) + (bins ? (lo::kLrHist + 1) * 4 : 0)" in cu
+    assert "fixed = (int64_t)sh->G * sh->S * 8, per_row = ((int64_t)sh->ks + 1 + nc + 1) * 8" in cu
+    assert "sh->cs = staged > 0 && staged >= std::min(32, bare) ? 1 : 0;" in cu
 
 
 def test_logistic_kernels_in_the_sass(built):
@@ -238,6 +264,39 @@ def test_fit_through_one_engine_and_shards_agree(nc):
     assert one.objective_history[0] >= one.objective_history[-1] and len(one.objective_history) == one.iterations + 1
     if nc == 2:
         assert one.coefficients.shape == (3,) and one.intercept == one.intercept_vector[0]
+
+
+class _RangeEngine(_Engine):
+    """Stands in for Engine with its column range: m2 exactly 0 where a part's column holds one value."""
+
+    def lr_stats(self, part):
+        n, total, m2, out = super().lr_stats(part)
+        least, most = (part.hx.min(0), part.hx.max(0)) if n else (np.zeros(part.k), np.zeros(part.k))
+        return ColumnStats(n, total, np.where(least == most, 0.0, m2), out, least, most)
+
+
+def test_shards_give_a_column_constant_over_all_of_them_m2_exactly_zero():
+    """Chan's delta between two shards' rounded means of 123.456 (300 and 700 rows) is not 0; the merged min / max zero
+    it.  A column constant in each shard but not over all (123.456 then 0.2) keeps its M2, and so does a plain one; a
+    part without rows does not count."""
+    rng = np.random.default_rng(0)
+    n = 1000
+    x = np.stack([np.full(n, 123.456), np.where(np.arange(n) < 300, 123.456, 0.2), rng.normal(size=n)], 1)
+    y = (rng.random(n) < 0.5).astype(np.float64)
+    cuts = ((0, 0), (0, 300), (300, 1000))
+    parts = [_Part(x[a:b], y[a:b]) for a, b in cuts]
+    got_n, total, m2, _c = _sharded_with(_RangeEngine, len(cuts)).lr_stats(parts)
+    plain = _sharded(len(cuts)).lr_stats(parts)[2]
+    assert got_n == n and plain[0] != 0.0                           # the bug the merged range fixes
+    assert m2[0] == 0.0
+    np.testing.assert_array_equal(m2[1:], plain[1:])
+    assert abs(m2[1] - 300 * 700 / 1000 * (123.456 - 0.2) ** 2) <= 1e-12 * m2[1]
+
+
+def _sharded_with(engine_cls, world):
+    sh = _sharded(world)
+    sh.engines = [engine_cls() for _ in range(world)]
+    return sh
 
 
 def test_edges_constant_label_zero_std_and_max_iter_zero():
