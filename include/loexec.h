@@ -583,6 +583,56 @@ int lo_lr_predict(lo_ctx *ctx, const lo_table *x, int64_t ld, int32_t k, int64_t
                   lo_table *raw, lo_table *pred, const lo_table *y, const double *eval_labels, int32_t neval,
                   int64_t *confusion_out, lo_nb_info *info, lo_host_timing *timing);
 
+/* Spark 2.4's DecisionTreeClassifier over the matrix of lo_assemble_rows (DESIGN.md §3.6.4): the device sorts the
+ * columns, answers the rank queries of the host's split search, bins every value, counts every tree level and applies
+ * the tree; the host chooses the thresholds and the splits from those counts.  The features and labels are first
+ * checked by lo_lr_stats_range (finite features, integer labels >= 0); these calls do not check them again.
+ *
+ * lo_dt_sort: columns [j0, j0 + kc) of x (n rows of k at stride ld, LO_F32 / LO_F64), each as n sorted
+ *   order-preserving codes (-0.0 as 0.0; unsigned order = value order) in keys[c * n ..] (a table of x's dtype holding
+ *   the codes' bits, >= kc * n elements).  ndistinct_out[c] (int64[kc]) = the column's distinct values; where that is
+ *   <= cap, values_out[c * cap ..] (f64, ascending) and counts_out[c * cap ..] (int64) hold them and their rows.
+ *   Scratch: about kc * n codes and CUB's storage.  n >= 2^31 or cap outside [0, LO_DT_MAX_BINS + 1] is refused.
+ * lo_dt_rank: for m probe codes probes[i] (uint64; the low 32 bits for LO_F32 keys) of column cols[i] of lo_dt_sort's
+ *   keys: lt_out[i] = #(codes < probe), le_out[i] = #(codes <= probe).  A timing of NULL records no events.
+ * lo_dt_bin: codes[r * kp + j] (LO_U8, >= n * kp, 16-byte aligned, kp a multiple of 16 >= k) = Spark's findBin of
+ *   x[r][j] widened to f64 in thresholds[j * tstride ..][0 .. nthr[j]) (ascending f64; equal neighbours allowed):
+ *   java.util.Arrays.binarySearch step for step, its hit's index or its insertion point (without equal thresholds, the
+ *   count of thresholds below x).  tstride in [1, LO_DT_MAX_BINS - 1]; descending or NaN thresholds are refused.
+ * lo_dt_level: one tree level of nnodes node slots over the n rows of codes and labels y (LO_F32 / LO_F64, integers in
+ *   [0, nclasses)).  A row's slot: src NULL, the root (route 0, nnodes 1); route 1, its parent's slot p = src[r] (LO_I32;
+ *   -1 a leaf) sent by splits[p * 4 ..] = (feature, bin, left, right) to left when its code of feature is <= bin, else to
+ *   right (-1: a leaf child; feature -1: the parent is a leaf); route 0, src[r].  dst (LO_I32, may be NULL with one node
+ *   group) receives the slots.  hist_out (host int64[nnodes][k][nbins][nclasses]) = the rows of each (slot, feature,
+ *   bin, class).  shape_out (int32[4], may be NULL) = the launch shape: 16-byte loads (1/0), features per chunk, nodes
+ *   per pass, passes.  Refused before any launch: nbins outside [1, LO_DT_MAX_BINS], nclasses outside [1,
+ *   LO_DT_MAX_CLASSES], k * nbins * nclasses * 8 above LO_DT_PASS_HIST (one node's histogram), a split out of range.
+ *   A code >= nbins or a label that is not an integer in [0, nclasses) is never counted: the call fails with
+ *   LO_ERR_INVALID naming the lowest such row (and feature) and hist_out zeroed.  Host memory: hist_out holds the whole
+ *   level, nnodes * k * nbins * nclasses int64.
+ * lo_dt_predict: a tree of nnodes nodes in arrays — feature (int32, -1 for a leaf), threshold (f64), left / right
+ *   (int32, after the node) and counts (f64 [nnodes][nclasses], a leaf's class counts) — over x, as lo_nb_predict's
+ *   transform and evaluate: a row goes left when its value widened to f64 is <= the threshold; raw = the leaf's counts,
+ *   probability = raw / sum, prediction = the first argmax; evaluate counts (label slot, prediction) and refuses a label
+ *   not in eval_labels (info->bad_row).  A node out of range or a child not after its parent is refused. */
+#define LO_DT_MAX_BINS     256          /* a bin index is a byte */
+#define LO_DT_MAX_CLASSES  100          /* Spark's maxNumClasses */
+#define LO_DT_PASS_HIST    1073741824   /* bytes of one level pass's u64 histogram */
+int lo_dt_sort(lo_ctx *ctx, const lo_table *x, int64_t ld, int32_t k, int64_t n, int32_t j0, int32_t kc, lo_table *keys,
+               int32_t cap, int64_t *ndistinct_out, double *values_out, int64_t *counts_out, lo_host_timing *timing);
+int lo_dt_rank(lo_ctx *ctx, const lo_table *keys, int64_t n, int32_t kc, int32_t m, const int32_t *cols,
+               const uint64_t *probes, int64_t *lt_out, int64_t *le_out, lo_host_timing *timing);
+int lo_dt_bin(lo_ctx *ctx, const lo_table *x, int64_t ld, int32_t k, int64_t n, const double *thresholds,
+              const int32_t *nthr, int32_t tstride, lo_table *codes, int64_t kp, lo_host_timing *timing);
+int lo_dt_level(lo_ctx *ctx, const lo_table *codes, int64_t kp, int32_t k, const lo_table *y, int64_t n, int32_t nbins,
+                int32_t nclasses, const lo_table *src, int32_t route, lo_table *dst, int32_t nparents,
+                const int32_t *splits, int32_t nnodes, int64_t *hist_out, int32_t *shape_out, lo_host_timing *timing);
+int lo_dt_predict(lo_ctx *ctx, const lo_table *x, int64_t ld, int32_t k, int64_t n, int32_t nnodes, const int32_t *feature,
+                  const double *threshold, const int32_t *left, const int32_t *right, const double *counts,
+                  int32_t nclasses, lo_table *prob, lo_table *raw, lo_table *pred, const lo_table *y,
+                  const double *eval_labels, int32_t neval, int64_t *confusion_out, lo_nb_info *info,
+                  lo_host_timing *timing);
+
 /* Number -> text for one column: the reference's "string" cast, str(v) / None -> "" (data_type_handler_image/
  * data_type_update.py:22-28), for every cell at once on the GPU.  The inverse of lo_parse_number_host.
  * status[i] uses the LO_NUM_* codes above: FLOAT -> repr(float) (shortest round-trip digits, CPython's notation),

@@ -40,6 +40,9 @@ LO_TEXT_STAGE_SLOTS = 512
 LO_INVALID_ERROR, LO_INVALID_SKIP, LO_INVALID_KEEP = 0, 1, 2
 LO_NB_MAX_CLASSES = 1024
 LO_NB_MAX_THETA = 16384
+LO_DT_MAX_BINS = 256
+LO_DT_MAX_CLASSES = 100
+LO_DT_PASS_HIST = 1 << 30
 LO_ABI_VERSION = 7
 
 _ERR_NAMES = {
@@ -184,6 +187,15 @@ SIGNATURES = {
                                   C.POINTER(HostTiming)]),
     "lo_lr_predict": (C.c_int, [_P, _P, C.c_int64, C.c_int32, C.c_int64, _P, _P, C.c_int32, C.c_int32, C.c_double, _P,
                                 _P, _P, _P, _P, C.c_int32, _P, C.POINTER(NbInfo), C.POINTER(HostTiming)]),
+    "lo_dt_sort": (C.c_int, [_P, _P, C.c_int64, C.c_int32, C.c_int64, C.c_int32, C.c_int32, _P, C.c_int32, _P, _P, _P,
+                             C.POINTER(HostTiming)]),
+    "lo_dt_rank": (C.c_int, [_P, _P, C.c_int64, C.c_int32, C.c_int32, _P, _P, _P, _P, C.POINTER(HostTiming)]),
+    "lo_dt_bin": (C.c_int, [_P, _P, C.c_int64, C.c_int32, C.c_int64, _P, _P, C.c_int32, _P, C.c_int64,
+                            C.POINTER(HostTiming)]),
+    "lo_dt_level": (C.c_int, [_P, _P, C.c_int64, C.c_int32, _P, C.c_int64, C.c_int32, C.c_int32, _P, C.c_int32, _P,
+                              C.c_int32, _P, C.c_int32, _P, _P, C.POINTER(HostTiming)]),
+    "lo_dt_predict": (C.c_int, [_P, _P, C.c_int64, C.c_int32, C.c_int64, C.c_int32, _P, _P, _P, _P, _P, C.c_int32, _P, _P,
+                                _P, _P, _P, C.c_int32, _P, C.POINTER(NbInfo), C.POINTER(HostTiming)]),
     "lo_format_number_host": (C.c_int, [_P, _P, _P, C.c_int64, _P, _P, C.c_int64, C.POINTER(HostTiming)]),
     "lo_parse_text_to_table": (C.c_int, [_P, _P, _P, C.c_int32, C.POINTER(ParseSummary), C.POINTER(HostTiming)]),
     "lo_format_table_to_text": (C.c_int, [_P, _P, C.c_int32, C.POINTER(Validity), C.POINTER(Validity), C.POINTER(_P),

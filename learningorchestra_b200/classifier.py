@@ -1,13 +1,15 @@
-"""The builder's "NB" and "LR" classifiers on the GPU: Spark 2.4's multinomial ``NaiveBayes`` and ``LogisticRegression``
-(``builder_image/builder.py:55-61``) fitted on, applied to and evaluated over the feature matrix in HBM
-(:meth:`DeviceFrame.features`), on one GPU or on every shard of a local :class:`~sharding.ShardedEngine`.  DESIGN.md
-§3.6.2 and §3.6.3 state the semantics.
+"""The builder's "NB", "LR" and "DT" classifiers on the GPU: Spark 2.4's multinomial ``NaiveBayes``,
+``LogisticRegression`` and ``DecisionTreeClassifier`` (``builder_image/builder.py:55-61``) fitted on, applied to and
+evaluated over the feature matrix in HBM (:meth:`DeviceFrame.features`), on one GPU or on every shard of a local
+:class:`~sharding.ShardedEngine`.  DESIGN.md §3.6.2 to §3.6.4 state the semantics.
 
 NaiveBayes: the device computes the class counts and per-class feature sums (``lo_nb_fit``); LogisticRegression: the
 column statistics and label counts (``lo_lr_stats``) and one pass of loss and gradient sums per function evaluation of
 the host's L-BFGS (``lo_lr_loss_grad``, :mod:`lbfgs`).  Both compute every row's raw values, probabilities and prediction
 (``lo_nb_predict`` / ``lo_lr_predict``) and the confusion counts of an evaluation on the device; the models' arrays and
-the evaluator's metrics are computed here, on the host, from those."""
+the evaluator's metrics are computed here, on the host, from those.  DecisionTreeClassifier: the device sorts the
+columns, answers rank queries, bins the values and counts every tree level (``lo_dt_*``); :mod:`tree` chooses the
+thresholds and splits from those counts."""
 from __future__ import annotations
 
 import math
@@ -344,3 +346,138 @@ class Predictions:
 
     def __exit__(self, *exc):
         self.release()
+
+
+_DT_SORT_BUDGET = 2 << 30      # bytes of sorted codes and sort scratch per column batch of lo_dt_sort
+
+
+class DecisionTreeClassifier:
+    """``pyspark.ml.classification.DecisionTreeClassifier(maxDepth, maxBins, minInstancesPerNode, minInfoGain,
+    impurity)`` with its other defaults (every feature continuous, no ``weightCol``, no ``thresholds``) on the GPU.
+    max_bins above LO_DT_MAX_BINS (256) is refused: a bin index is a byte on the device."""
+
+    def __init__(self, max_depth: int = 5, max_bins: int = 32, min_instances_per_node: int = 1,
+                 min_info_gain: float = 0.0, impurity: str = "gini"):
+        from . import tree as T
+
+        def integer(v, name, lo, hi=None):
+            if isinstance(v, bool) or not isinstance(v, (int, np.integer)) or v < lo or (hi is not None and v > hi):
+                span = f"in [{lo}, {hi}]" if hi is not None else f">= {lo}"
+                raise ValueError(f"{name} must be an integer {span}, not {v!r}")
+            return int(v)
+
+        self.max_depth = integer(max_depth, "max_depth", 0, T.MAX_DEPTH)
+        self.max_bins = integer(max_bins, "max_bins", 2, T.MAX_BINS)
+        self.min_instances_per_node = integer(min_instances_per_node, "min_instances_per_node", 1)
+        g = float(min_info_gain)
+        if not np.isfinite(g) or g < 0.0:
+            raise ValueError(f"min_info_gain must be finite and >= 0, not {min_info_gain!r}")
+        self.min_info_gain = g
+        if not isinstance(impurity, str) or impurity.lower() not in T.IMPURITIES:
+            raise ValueError(f"impurity must be one of {list(T.IMPURITIES)}, not {impurity!r}")
+        self.impurity = impurity.lower()
+
+    def fit(self, features) -> "DecisionTreeClassificationModel":
+        """The tree of ``features`` (:class:`~builder_frontend.Features` with a label, on one GPU or sharded).  Every
+        label must be an integer >= 0 and every feature finite (InvalidCellError naming the ``_id`` and field of the
+        lowest refused row); numClasses = max label + 1.  No row, more than LO_DT_MAX_CLASSES classes or a one-node
+        histogram (k x min(max_bins, n) x C x 8 bytes) above LO_DT_PASS_HIST are refused."""
+        from . import tree as T
+        _usable(features)
+        if features.label is None:
+            raise ValueError("DecisionTreeClassifier needs features with a label")
+        name, k = "DecisionTreeClassifier", len(features.fields)
+        n, _total, _m2, counts = _on_device(features, lambda engine, rows: engine.lr_stats(rows), name=name,
+                                            reasons=_LR_REASONS)
+        if n == 0:
+            raise N.LoexecError(N.LO_ERR_INVALID, "DecisionTreeClassifier needs at least one row")
+        num_classes = int(np.flatnonzero(counts)[-1]) + 1
+        if num_classes > N.LO_DT_MAX_CLASSES:
+            raise N.LoexecError(N.LO_ERR_INVALID, f"{num_classes} classes exceed LO_DT_MAX_CLASSES = "
+                                f"{N.LO_DT_MAX_CLASSES}")
+        if k * min(self.max_bins, n) * num_classes * 8 > N.LO_DT_PASS_HIST:
+            raise N.LoexecError(N.LO_ERR_INVALID, f"{k} features x {min(self.max_bins, n)} bins x {num_classes} classes: "
+                                f"one node's histogram exceeds LO_DT_PASS_HIST = {N.LO_DT_PASS_HIST} bytes")
+        thresholds, rounds = self._thresholds(features, n, k)
+        nbins = max(len(t) for t in thresholds) + 1
+        binned = _on_device(features, lambda engine, rows: engine.dt_bin(rows, thresholds), name=name)
+        try:
+            def level(splits, nnodes):
+                return _on_device(features, lambda engine, rows: engine.dt_level(rows, binned, nbins, num_classes,
+                                                                                splits, nnodes), name=name)
+
+            tree, _shapes = T.grow(level, thresholds, num_classes, self.max_depth, self.impurity,
+                                   self.min_instances_per_node, self.min_info_gain)
+        finally:
+            for b in binned if isinstance(binned, list) else [binned]:
+                b.free()
+        model = DecisionTreeClassificationModel(tree, features.fields, thresholds)
+        model.rank_rounds = rounds
+        return model
+
+    def _thresholds(self, features, n: int, k: int) -> tuple[list, int]:
+        """Every column's split thresholds: the columns sorted on the device in batches within _DT_SORT_BUDGET, each
+        batch's distinct values merged or its order statistics found by rank rounds (:func:`tree.column_thresholds`),
+        and its sorted copies freed before the next."""
+        from . import tree as T
+        f32 = features._parts[0].x.dtype_code == N.LO_F32
+        per_col = 2 * (4 if f32 else 8) * max(n, 1)
+        kc = max(1, min(k, _DT_SORT_BUDGET // per_col))
+        cap = T.num_splits(self.max_bins, n) + 1
+        out, rounds = [], 0
+        for j0 in range(0, k, kc):
+            w = min(kc, k - j0)
+            got = _on_device(features, lambda engine, rows: engine.dt_sort(rows, j0, w, cap),
+                             name="DecisionTreeClassifier")
+            members = got if isinstance(got, list) else [got]
+            try:
+                distinct = [T.merge_distinct([m.distinct[c] for m in members]) for c in range(w)]
+
+                def rank(cols, codes):
+                    return _on_device(features, lambda engine, rows: engine.dt_rank(got, cols, codes),
+                                      name="DecisionTreeClassifier")
+
+                thr, r = T.column_thresholds(n, self.max_bins, distinct, rank, f32, w)
+            finally:
+                for m in members:
+                    m.free()
+            out += thr
+            rounds += r
+        return out, rounds
+
+
+class DecisionTreeClassificationModel:
+    """A fitted decision tree, host data: ``tree`` (:class:`~tree.Tree`: the node arrays feature, threshold, left, right,
+    counts, prediction, impurity and gain), ``depth``, ``num_nodes``, ``num_classes``, the ``fields`` it was fitted on
+    and every column's split ``thresholds``."""
+
+    def __init__(self, tree, fields, thresholds=None):
+        self.tree, self.fields, self.thresholds = tree, list(fields), thresholds
+        self.depth, self.num_nodes, self.num_classes = tree.depth, tree.num_nodes, tree.num_classes
+
+    def _check(self, features) -> None:
+        if list(features.fields) != self.fields:
+            raise ValueError(f"the model was fitted on fields {self.fields}, not {list(features.fields)}")
+
+    def transform(self, features, raw: bool = False) -> "Predictions":
+        """Spark's ``model.transform``: every row's ``probability`` (the leaf's class counts over their sum) and
+        ``prediction`` (a class index as float64), and with ``raw`` its ``rawPrediction`` (the leaf's counts), written in
+        HBM on the rows' own devices."""
+        _usable(features)
+        self._check(features)
+        parts = _on_device(features, lambda engine, rows: engine.dt_predict(rows, self.tree, raw=raw), per_part=True,
+                           name="DecisionTreeClassifier", reasons=_LR_REASONS)
+        return Predictions(features, parts)
+
+    def evaluate(self, features) -> dict:
+        """``MulticlassClassificationEvaluator`` f1 and accuracy over ``transform(features)``, as
+        :meth:`NaiveBayesModel.evaluate`: ``{"f1", "accuracy", "labels", "confusion"}``."""
+        _usable(features)
+        self._check(features)
+        labels = _labels(features, "DecisionTreeClassifier", _LR_REASONS)
+        if len(features.row_ids) == 0:
+            raise N.LoexecError(N.LO_ERR_INVALID, "evaluate needs at least one row")
+        confusion = _on_device(features, lambda engine, rows: engine.dt_predict(rows, self.tree, labels=labels),
+                               name="DecisionTreeClassifier", reasons=_LR_REASONS)
+        f1, accuracy = metrics(labels, confusion)
+        return {"f1": f1, "accuracy": accuracy, "labels": labels, "confusion": confusion}

@@ -7,6 +7,7 @@
 #include "kernels.cuh"
 #include "naive_bayes.cuh"
 #include "logistic.cuh"
+#include "tree.cuh"
 
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
@@ -3104,6 +3105,416 @@ int lo_lr_predict(lo_ctx *ctx, const lo_table *x, int64_t ld, int32_t k, int64_t
     return nb_predict(ctx, x, ld, k, n, intercept, coef, nclasses, multinomial ? lo::kLrMultinomial : lo::kLrBinomial,
                       threshold, prob, raw, pred, y, eval_labels,
                       neval, confusion_out, info, timing, "lr_predict", "lr_evaluate");
+}
+
+}  // extern "C"
+
+static_assert(lo::kDtMaxBins == LO_DT_MAX_BINS && lo::kDtMaxClasses == LO_DT_MAX_CLASSES &&
+              lo::kDtPassHist == LO_DT_PASS_HIST, "loexec.h documents the tree's caps");
+
+namespace {
+
+// a table of `dtype` on the context's device holding at least `need` elements
+int check_typed_table(const lo_ctx *ctx, const lo_table *t, int dtype, int64_t need, const char *name) {
+    if (!t) return fail(LO_ERR_INVALID, "%s is NULL", name);
+    if (t->dtype != dtype) return fail(LO_ERR_INVALID, "%s has dtype %d, %d expected", name, t->dtype, dtype);
+    if (t->device != ctx->device) return fail(LO_ERR_INVALID, "%s lives on device %d, the context on %d", name, t->device, ctx->device);
+    if (t->nrows < need)
+        return fail(LO_ERR_INVALID, "%s holds %lld elements, %lld needed", name, (long long)t->nrows, (long long)need);
+    return LO_OK;
+}
+
+int check_dt_classes(int32_t nclasses) {
+    if (nclasses < 1 || nclasses > LO_DT_MAX_CLASSES)
+        return fail(LO_ERR_INVALID, "%d classes outside [1, LO_DT_MAX_CLASSES = %d]", nclasses, LO_DT_MAX_CLASSES);
+    return LO_OK;
+}
+
+// The launch shape of a level of nnodes nodes (lo_dt_level): a feature's histogram of one node takes cell = nbins * C
+// u32 counters; a CTA holds gn nodes x fc features of them within kDtHistSmem.  fc is a multiple of 16 (16-byte code
+// loads) when 16 cells fit, else as many single features as fit (scalar loads); gn as many nodes as fit beside, and as
+// keep the pass's u64 histogram within kDtPassHist.  passes = node groups, each one pass over the rows.
+struct DtShape { int vec, fc, gn, passes, smem; };
+DtShape dt_shape(int32_t k, int32_t nbins, int32_t C, int32_t nnodes) {
+    DtShape sh{};
+    const int64_t cell = (int64_t)nbins * C * 4, cells = lo::kDtHistSmem / cell;
+    const int64_t kpad = ((int64_t)k + lo::kDtVec - 1) / lo::kDtVec * lo::kDtVec;
+    sh.vec = cells >= lo::kDtVec;
+    sh.fc = (int)(sh.vec ? std::min<int64_t>(kpad, cells / lo::kDtVec * lo::kDtVec) : std::min<int64_t>(k, cells));
+    const int64_t by_smem = cells / sh.fc, by_pass = lo::kDtPassHist / ((int64_t)k * nbins * C * 8);
+    sh.gn = (int)std::max<int64_t>(1, std::min<int64_t>({(int64_t)std::max(nnodes, 1), by_smem, by_pass}));
+    sh.passes = (std::max(nnodes, 1) + sh.gn - 1) / sh.gn;
+    sh.smem = (int)((int64_t)sh.gn * sh.fc * cell);
+    return sh;
+}
+
+template <typename K>
+void dt_sort_columns(HostCall &c, const lo_table *x, int64_t ld, int64_t n, int32_t j0, int32_t kc, K *out, int32_t cap,
+                     unsigned long long *count, unsigned long long *fkey, long long *fpos) {
+    K *keys = nullptr;
+    void *tmp = nullptr;
+    size_t tmp_bytes = 0;
+    c.alloc(&keys, (size_t)n * kc * sizeof(K));
+    c.run([&] { return cub::DeviceRadixSort::SortKeys(nullptr, tmp_bytes, keys, out, n, 0, (int)sizeof(K) * 8, c.s); });
+    c.alloc(&tmp, tmp_bytes);
+    c.mark();
+    const int grid = (int)std::min<int64_t>((n * kc + lo::kDtThreads - 1) / lo::kDtThreads, (int64_t)c.ctx->sm_count * 8);
+    c.launch(1, [&] {
+        if constexpr (sizeof(K) == 4) lo::k_dt_keys<float><<<grid, lo::kDtThreads, 0, c.s>>>((const float *)x->base, ld, j0, kc, n, keys);
+        else lo::k_dt_keys<double><<<grid, lo::kDtThreads, 0, c.s>>>((const double *)x->base, ld, j0, kc, n, keys);
+    });
+    for (int32_t j = 0; j < kc; ++j)
+        c.launch(1, [&] {
+            return cub::DeviceRadixSort::SortKeys(tmp, tmp_bytes, keys + (size_t)j * n, out + (size_t)j * n, n, 0,
+                                                  (int)sizeof(K) * 8, c.s);
+        });
+    c.drop(keys);
+    c.drop(tmp);
+    const dim3 dgrid((unsigned)std::min<int64_t>((n + lo::kDtThreads - 1) / lo::kDtThreads, (int64_t)c.ctx->sm_count * 4),
+                     (unsigned)kc);
+    c.launch(1, [&] { lo::k_dt_distinct<K><<<dgrid, lo::kDtThreads, 0, c.s>>>(out, n, cap, count, fkey, fpos); });
+    c.mark();
+}
+
+// the value of an order-preserving code (lo::dt_code), widened to f64
+double dt_value(uint64_t code, bool f32) {
+    if (f32) {
+        const uint32_t o = (uint32_t)code, b = o >> 31 ? o & 0x7fffffffu : ~o;
+        float v;
+        std::memcpy(&v, &b, 4);
+        return (double)v;
+    }
+    const uint64_t b = code >> 63 ? code & ~(1ull << 63) : ~code;
+    double v;
+    std::memcpy(&v, &b, 8);
+    return v;
+}
+
+}  // namespace
+
+extern "C" {
+
+int lo_dt_sort(lo_ctx *ctx, const lo_table *x, int64_t ld, int32_t k, int64_t n, int32_t j0, int32_t kc, lo_table *keys,
+               int32_t cap, int64_t *ndistinct_out, double *values_out, int64_t *counts_out, lo_host_timing *timing) {
+    LO_TRY(check_ctx(ctx));
+    if (n >= (1ll << 31)) return fail(LO_ERR_INVALID, "n = %lld: CUB's sort takes fewer than 2^31 rows", (long long)n);
+    LO_TRY(check_nb_matrix(ctx, x, ld, k, n, nullptr));
+    if (j0 < 0 || kc < 1 || j0 + (int64_t)kc > k) return fail(LO_ERR_INVALID, "columns [%d, %d + %d) outside [0, %d)", j0, j0, kc, k);
+    if (cap < 0 || cap > LO_DT_MAX_BINS + 1) return fail(LO_ERR_INVALID, "cap = %d outside [0, %d]", cap, LO_DT_MAX_BINS + 1);
+    LO_TRY(check_typed_table(ctx, keys, x->dtype, n * kc, "keys"));
+    if (!ndistinct_out || (cap > 0 && (!values_out || !counts_out)))
+        return fail(LO_ERR_INVALID, "ndistinct_out, values_out or counts_out is NULL");
+    std::fill(ndistinct_out, ndistinct_out + kc, (int64_t)0);
+    HostCall c(ctx, "dt_sort");
+    if (n == 0) return c.finish(timing);
+    const bool f32 = x->dtype == LO_F32;
+    const size_t slots = (size_t)kc * std::max(cap, 1);
+    unsigned long long *count = nullptr, *fkey = nullptr;
+    long long *fpos = nullptr;
+    c.alloc(&count, (size_t)kc * 8);
+    c.alloc(&fkey, slots * 8);
+    c.alloc(&fpos, slots * 8);
+    c.memset(count, 0, (size_t)kc * 8);
+    if (f32) dt_sort_columns<unsigned>(c, x, ld, n, j0, kc, (unsigned *)keys->base, cap, count, fkey, fpos);
+    else     dt_sort_columns<unsigned long long>(c, x, ld, n, j0, kc, (unsigned long long *)keys->base, cap, count, fkey, fpos);
+    std::vector<unsigned long long> key(slots), cnt((size_t)kc);
+    std::vector<long long> pos(slots);
+    c.to_host(cnt.data(), count, (size_t)kc * 8);
+    c.to_host(key.data(), fkey, slots * 8);
+    c.to_host(pos.data(), fpos, slots * 8);
+    LO_TRY(c.finish(timing));
+    for (int32_t j = 0; j < kc; ++j) {
+        const int64_t d = (int64_t)cnt[j];
+        ndistinct_out[j] = d;
+        if (d > cap) continue;
+        // the run starts by position are the distinct values ascending; a run ends where the next starts
+        std::vector<std::pair<long long, unsigned long long>> runs((size_t)d);
+        for (int64_t i = 0; i < d; ++i) runs[i] = {pos[(size_t)j * cap + i], key[(size_t)j * cap + i]};
+        std::sort(runs.begin(), runs.end());
+        for (int64_t i = 0; i < d; ++i) {
+            values_out[(size_t)j * cap + i] = dt_value(runs[i].second, f32);
+            counts_out[(size_t)j * cap + i] = (i + 1 < d ? runs[i + 1].first : n) - runs[i].first;
+        }
+    }
+    return LO_OK;
+}
+
+int lo_dt_rank(lo_ctx *ctx, const lo_table *keys, int64_t n, int32_t kc, int32_t m, const int32_t *cols,
+               const uint64_t *probes, int64_t *lt_out, int64_t *le_out, lo_host_timing *timing) {
+    LO_TRY(check_ctx(ctx));
+    if (!keys) return fail(LO_ERR_INVALID, "keys is NULL");
+    if (keys->dtype != LO_F32 && keys->dtype != LO_F64) return fail(LO_ERR_INVALID, "keys must be LO_F32 or LO_F64");
+    if (n < 0 || kc < 1 || m < 0) return fail(LO_ERR_INVALID, "n = %lld, kc = %d, m = %d", (long long)n, kc, m);
+    LO_TRY(check_typed_table(ctx, keys, keys->dtype, n * kc, "keys"));
+    if (m > 0 && (!cols || !probes || !lt_out || !le_out)) return fail(LO_ERR_INVALID, "cols, probes, lt_out or le_out is NULL");
+    for (int32_t i = 0; i < m; ++i)
+        if (cols[i] < 0 || cols[i] >= kc) return fail(LO_ERR_INVALID, "cols[%d] = %d outside [0, %d)", i, cols[i], kc);
+    HostCall c(ctx, "dt_rank", timing != nullptr);
+    if (m == 0 || n == 0) {
+        std::fill(lt_out, lt_out + m, (int64_t)0);
+        std::fill(le_out, le_out + m, (int64_t)0);
+        return c.finish(timing);
+    }
+    int *d_cols = nullptr;
+    unsigned long long *d_probe = nullptr;
+    long long *d_lt = nullptr, *d_le = nullptr;
+    c.alloc(&d_cols, (size_t)m * 4);
+    c.alloc(&d_probe, (size_t)m * 8);
+    c.alloc(&d_lt, (size_t)m * 8);
+    c.alloc(&d_le, (size_t)m * 8);
+    c.to_dev(d_cols, cols, (size_t)m * 4);
+    c.to_dev(d_probe, probes, (size_t)m * 8);
+    const unsigned grid = (unsigned)((m + lo::kDtThreads - 1) / lo::kDtThreads);
+    c.mark();
+    c.launch(1, [&] {
+        if (keys->dtype == LO_F32)
+            lo::k_dt_rank<unsigned><<<grid, lo::kDtThreads, 0, c.s>>>((const unsigned *)keys->base, n, m, d_cols, d_probe, d_lt, d_le);
+        else
+            lo::k_dt_rank<unsigned long long><<<grid, lo::kDtThreads, 0, c.s>>>((const unsigned long long *)keys->base, n, m,
+                                                                               d_cols, d_probe, d_lt, d_le);
+    });
+    c.mark();
+    c.to_host(lt_out, d_lt, (size_t)m * 8);
+    c.to_host(le_out, d_le, (size_t)m * 8);
+    return c.finish(timing);
+}
+
+int lo_dt_bin(lo_ctx *ctx, const lo_table *x, int64_t ld, int32_t k, int64_t n, const double *thresholds,
+              const int32_t *nthr, int32_t tstride, lo_table *codes, int64_t kp, lo_host_timing *timing) {
+    LO_TRY(check_ctx(ctx));
+    LO_TRY(check_nb_matrix(ctx, x, ld, k, n, nullptr));
+    if (tstride < 1 || tstride > LO_DT_MAX_BINS - 1) return fail(LO_ERR_INVALID, "tstride = %d outside [1, %d]", tstride, LO_DT_MAX_BINS - 1);
+    if (!thresholds || !nthr) return fail(LO_ERR_INVALID, "thresholds or nthr is NULL");
+    for (int32_t j = 0; j < k; ++j) {
+        if (nthr[j] < 0 || nthr[j] > tstride) return fail(LO_ERR_INVALID, "nthr[%d] = %d outside [0, %d]", j, nthr[j], tstride);
+        for (int32_t i = 1; i < nthr[j]; ++i)
+            if (!(thresholds[(size_t)j * tstride + i] >= thresholds[(size_t)j * tstride + i - 1]))
+                return fail(LO_ERR_INVALID, "the thresholds of column %d are not ascending (or NaN)", j);
+    }
+    if (kp < k || kp % lo::kDtVec) return fail(LO_ERR_INVALID, "kp = %lld: a multiple of 16 >= k", (long long)kp);
+    LO_TRY(check_typed_table(ctx, codes, LO_U8, n * kp, "codes"));
+    if ((uintptr_t)codes->base % 16) return fail(LO_ERR_INVALID, "codes must start 16-byte aligned");
+    HostCall c(ctx, "dt_bin");
+    if (n == 0) return c.finish(timing);
+    // column chunks of a multiple of 16 whose thresholds fit kDtBinSmem (at least 48 columns of 255 thresholds)
+    const int kc = std::min<int>((k + lo::kDtVec - 1) / lo::kDtVec * lo::kDtVec,
+                                 lo::kDtBinSmem / (tstride * 8 + 4) / lo::kDtVec * lo::kDtVec);
+    const int smem = kc * tstride * 8 + kc * 4;
+    double *d_thr = nullptr;
+    int *d_n = nullptr;
+    c.alloc(&d_thr, (size_t)k * tstride * 8);
+    c.alloc(&d_n, (size_t)k * 4);
+    c.to_dev(d_thr, thresholds, (size_t)k * tstride * 8);
+    c.to_dev(d_n, nthr, (size_t)k * 4);
+    const size_t esz = x->dtype == LO_F32 ? 4 : 8;
+    const bool vec = (uintptr_t)x->base % 16 == 0 && (ld * (int64_t)esz) % 16 == 0;
+    auto go = [&](auto kernel, auto tag) {
+        using T = decltype(tag);
+        c.run([&] { return cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem); });
+        const dim3 grid((unsigned)std::min<int64_t>((n * kc / (16 / esz) + lo::kDtThreads - 1) / lo::kDtThreads,
+                                                    (int64_t)ctx->sm_count * 8),
+                        (unsigned)((k + kc - 1) / kc));
+        c.mark();
+        c.launch(1, [&] {
+            kernel<<<grid, lo::kDtThreads, smem, c.s>>>((const T *)x->base, ld, k, n, d_thr, d_n, tstride, kc,
+                                                        (unsigned char *)codes->base, kp);
+        });
+        c.mark();
+    };
+    if (x->dtype == LO_F32) {
+        if (vec) go(lo::k_dt_bin<float, 4>, 0.0f); else go(lo::k_dt_bin<float, 1>, 0.0f);
+    } else {
+        if (vec) go(lo::k_dt_bin<double, 2>, 0.0); else go(lo::k_dt_bin<double, 1>, 0.0);
+    }
+    return c.finish(timing);
+}
+
+int lo_dt_level(lo_ctx *ctx, const lo_table *codes, int64_t kp, int32_t k, const lo_table *y, int64_t n, int32_t nbins,
+                int32_t nclasses, const lo_table *src, int32_t route, lo_table *dst, int32_t nparents,
+                const int32_t *splits, int32_t nnodes, int64_t *hist_out, int32_t *shape_out, lo_host_timing *timing) {
+    LO_TRY(check_ctx(ctx));
+    if (k < 1) return fail(LO_ERR_INVALID, "k = %d: at least one feature", k);
+    if (kp < k || kp % lo::kDtVec) return fail(LO_ERR_INVALID, "kp = %lld: a multiple of 16 >= k", (long long)kp);
+    if (n < 0) return fail(LO_ERR_INVALID, "n = %lld is negative", (long long)n);
+    LO_TRY(check_typed_table(ctx, codes, LO_U8, n * kp, "codes"));
+    if ((uintptr_t)codes->base % 16) return fail(LO_ERR_INVALID, "codes must start 16-byte aligned");
+    LO_TRY(check_float_table(ctx, y, 0, n, "y"));
+    if (nbins < 1 || nbins > LO_DT_MAX_BINS) return fail(LO_ERR_INVALID, "nbins = %d outside [1, %d]", nbins, LO_DT_MAX_BINS);
+    LO_TRY(check_dt_classes(nclasses));
+    if ((int64_t)k * nbins * nclasses * 8 > LO_DT_PASS_HIST)
+        return fail(LO_ERR_INVALID, "%d features x %d bins x %d classes: one node's histogram exceeds LO_DT_PASS_HIST = %lld "
+                    "bytes", k, nbins, nclasses, (long long)LO_DT_PASS_HIST);
+    if (nnodes < 1) return fail(LO_ERR_INVALID, "nnodes = %d: at least one", nnodes);
+    if (route != 0 && route != 1) return fail(LO_ERR_INVALID, "route = %d: 0 or 1", route);
+    if (src) LO_TRY(check_typed_table(ctx, src, LO_I32, n, "src"));
+    else if (route || nnodes != 1) return fail(LO_ERR_INVALID, "without src every row is at the root: route 0, one node");
+    if (dst) LO_TRY(check_typed_table(ctx, dst, LO_I32, n, "dst"));
+    if (route) {
+        if (nparents < 1 || !splits) return fail(LO_ERR_INVALID, "routing needs the parents' splits");
+        for (int32_t p = 0; p < nparents; ++p) {
+            const int32_t *s = splits + (size_t)p * 4;
+            if (s[0] < 0) continue;
+            if (s[0] >= k || s[1] < 0 || s[1] >= nbins || s[2] < -1 || s[2] >= nnodes || s[3] < -1 || s[3] >= nnodes)
+                return fail(LO_ERR_INVALID, "split %d = (%d, %d, %d, %d) is out of range", p, s[0], s[1], s[2], s[3]);
+        }
+    }
+    if (!hist_out) return fail(LO_ERR_INVALID, "hist_out is NULL");
+    const DtShape sh = dt_shape(k, nbins, nclasses, nnodes);
+    if (shape_out) {
+        shape_out[0] = sh.vec;
+        shape_out[1] = sh.fc;
+        shape_out[2] = sh.gn;
+        shape_out[3] = sh.passes;
+    }
+    if (sh.passes > 1 && !dst) return fail(LO_ERR_INVALID, "%d node groups need dst to keep the rows' slots", sh.passes);
+    const size_t per_node = (size_t)k * nbins * nclasses;
+    std::fill(hist_out, hist_out + per_node * nnodes, (int64_t)0);
+    HostCall c(ctx, "dt_level");
+    if (n == 0) return c.finish(timing);
+    int *d_split = nullptr;
+    unsigned long long *d_hist = nullptr;
+    RefusedCell bad;
+    bad.arm(c);
+    const int np = route ? nparents : 0;
+    if (np) {
+        std::vector<int32_t> soa((size_t)np * 4);        // feature, bin, left, right: one array each
+        for (int32_t p = 0; p < np; ++p)
+            for (int f = 0; f < 4; ++f) soa[(size_t)f * np + p] = splits[(size_t)p * 4 + f];
+        c.alloc(&d_split, soa.size() * 4);
+        c.to_dev(d_split, soa.data(), soa.size() * 4);
+    }
+    c.alloc(&d_hist, per_node * sh.gn * 8);
+    auto go = [&](auto kernel, auto tag) {
+        using T = decltype(tag);
+        int per_sm = 0;
+        c.run([&] { return cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, sh.smem); });
+        c.run([&] { return cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, lo::kDtThreads, sh.smem); });
+        const int nchunks = (k + sh.fc - 1) / sh.fc;
+        const int64_t want = (int64_t)ctx->sm_count * std::max(1, per_sm) / nchunks;
+        const dim3 grid((unsigned)std::max<int64_t>(1, std::min<int64_t>((n + lo::kDtThreads - 1) / lo::kDtThreads, want)),
+                        (unsigned)nchunks);
+        c.mark();
+        for (int pass = 0; pass < sh.passes; ++pass) {
+            const int g0 = pass * sh.gn, gn = std::min(sh.gn, nnodes - g0);
+            // the first pass routes (and writes dst); the later ones read the slots it wrote
+            const int *from = pass == 0 ? (src ? (const int *)src->base : nullptr) : (const int *)dst->base;
+            c.memset(d_hist, 0, per_node * gn * 8);
+            c.launch(1, [&] {
+                kernel<<<grid, lo::kDtThreads, sh.smem, c.s>>>((const unsigned char *)codes->base, kp, k, (const T *)y->base,
+                                                               n, nbins, nclasses, from, pass == 0 ? route : 0,
+                                                               pass == 0 && dst ? (int *)dst->base : nullptr,
+                                                               d_split, d_split + np, d_split + 2 * np, d_split + 3 * np,
+                                                               g0, gn, sh.fc, d_hist, bad.word);
+            });
+            c.to_host(hist_out + per_node * g0, d_hist, per_node * gn * 8);
+            c.sync();                                       // d_hist is reused by the next pass
+        }
+        c.mark();
+    };
+    if (y->dtype == LO_F32) {
+        if (sh.vec) go(lo::k_dt_level<float, true>, 0.0f); else go(lo::k_dt_level<float, false>, 0.0f);
+    } else {
+        if (sh.vec) go(lo::k_dt_level<double, true>, 0.0); else go(lo::k_dt_level<double, false>, 0.0);
+    }
+    bad.read(c);
+    LO_TRY(c.finish(timing));
+    if (bad.key == ~0ull) return LO_OK;
+    int64_t row = 0;
+    int32_t col = 0;
+    lo::cell_of_key(bad.key, k, &row, &col);
+    std::fill(hist_out, hist_out + per_node * nnodes, (int64_t)0);
+    if (col == k) return fail(LO_ERR_INVALID, "row %lld: its label is not a class in [0, %d)", (long long)row, nclasses);
+    return fail(LO_ERR_INVALID, "row %lld, feature %d: code >= nbins = %d", (long long)row, col, nbins);
+}
+
+int lo_dt_predict(lo_ctx *ctx, const lo_table *x, int64_t ld, int32_t k, int64_t n, int32_t nnodes, const int32_t *feature,
+                  const double *threshold, const int32_t *left, const int32_t *right, const double *counts,
+                  int32_t nclasses, lo_table *prob, lo_table *raw, lo_table *pred, const lo_table *y,
+                  const double *eval_labels, int32_t neval, int64_t *confusion_out, lo_nb_info *info,
+                  lo_host_timing *timing) {
+    LO_TRY(check_ctx(ctx));
+    if (!info) return fail(LO_ERR_INVALID, "info is NULL");
+    *info = lo_nb_info{-1, -1, 0};
+    const bool eval = confusion_out != nullptr;
+    if (eval && !y) return fail(LO_ERR_INVALID, "evaluate needs y");
+    LO_TRY(check_nb_matrix(ctx, x, ld, k, n, eval ? y : nullptr));
+    LO_TRY(check_dt_classes(nclasses));
+    const int32_t C = nclasses, M = nnodes;
+    if (M < 1 || !feature || !threshold || !left || !right || !counts)
+        return fail(LO_ERR_INVALID, "a tree of %d nodes: feature, threshold, left, right and counts are needed", M);
+    // every path ends: an internal node's children come after it
+    for (int32_t i = 0; i < M; ++i) {
+        if (feature[i] < -1 || feature[i] >= k) return fail(LO_ERR_INVALID, "node %d: feature %d outside [-1, %d)", i, feature[i], k);
+        if (feature[i] >= 0 && !(left[i] > i && left[i] < M && right[i] > i && right[i] < M))
+            return fail(LO_ERR_INVALID, "node %d: children %d, %d must lie in (%d, %d)", i, left[i], right[i], i, M);
+    }
+    int direct = 0;
+    if (eval) {
+        if (prob || raw || pred) return fail(LO_ERR_INVALID, "evaluate writes no rows: prob, raw and pred must be NULL");
+        LO_TRY(check_nb_classes(eval_labels, neval, "eval_labels", &direct));
+        std::fill(confusion_out, confusion_out + (size_t)neval * C, (int64_t)0);
+    } else {
+        if (y || eval_labels) return fail(LO_ERR_INVALID, "y and eval_labels go with confusion_out");
+        LO_TRY(check_float_table(ctx, prob, LO_F64, n * C, "prob"));
+        LO_TRY(check_float_table(ctx, pred, LO_F64, n, "pred"));
+        if (raw) LO_TRY(check_float_table(ctx, raw, LO_F64, n * C, "raw"));
+    }
+    HostCall c(ctx, eval ? "dt_evaluate" : "dt_predict");
+    if (n == 0) return c.finish(timing);
+    const int64_t tree_bytes = (int64_t)M * 8 + ((int64_t)3 * M + 1) / 2 * 8;
+    const int64_t evl_bytes = eval ? (int64_t)neval * 8 : 0, hist_bytes = eval ? (int64_t)neval * C * 4 : 0;
+    const bool tree_smem = tree_bytes + evl_bytes <= lo::kDtTreeSmem;
+    const int64_t fixed = (tree_smem ? tree_bytes : 0) + evl_bytes;
+    const bool hist_smem = eval && fixed + hist_bytes <= lo::kDtTreeSmem;
+    const int smem = (int)(fixed + (hist_smem ? hist_bytes : 0));
+    int *d_int = nullptr;
+    double *d_thr = nullptr, *d_cnt = nullptr, *d_evl = nullptr;
+    unsigned long long *conf = nullptr;
+    RefusedCell bad;
+    c.alloc(&d_int, (size_t)M * 12);
+    c.alloc(&d_thr, (size_t)M * 8);
+    c.alloc(&d_cnt, (size_t)M * C * 8);
+    c.to_dev(d_int, feature, (size_t)M * 4);
+    c.to_dev(d_int + M, left, (size_t)M * 4);
+    c.to_dev(d_int + 2 * M, right, (size_t)M * 4);
+    c.to_dev(d_thr, threshold, (size_t)M * 8);
+    c.to_dev(d_cnt, counts, (size_t)M * C * 8);
+    if (eval) {
+        c.alloc(&d_evl, (size_t)neval * 8);
+        c.alloc(&conf, (size_t)neval * C * 8);
+        c.to_dev(d_evl, eval_labels, (size_t)neval * 8);
+        c.memset(conf, 0, (size_t)neval * C * 8);
+        bad.arm(c);
+    }
+    auto go = [&](auto kernel, auto tag) {
+        using T = decltype(tag);
+        int per_sm = 0;
+        c.run([&] { return cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem); });
+        c.run([&] { return cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, lo::kDtThreads, smem); });
+        const int grid = (int)std::min<int64_t>((n + lo::kDtThreads - 1) / lo::kDtThreads,
+                                                (int64_t)ctx->sm_count * std::max(1, per_sm));
+        c.mark();
+        c.launch(1, [&] {
+            kernel<<<grid, lo::kDtThreads, smem, c.s>>>((const T *)x->base, ld, k, n, M, d_int, d_thr, d_int + M, d_int + 2 * M,
+                                                        d_cnt, C, tree_smem ? 1 : 0, prob ? (double *)prob->base : nullptr,
+                                                        raw ? (double *)raw->base : nullptr,
+                                                        pred ? (double *)pred->base : nullptr,
+                                                        y ? (const T *)y->base : nullptr, d_evl, neval, direct, conf,
+                                                        hist_smem ? 1 : 0, bad.word);
+        });
+        c.mark();
+    };
+    if (x->dtype == LO_F32) {
+        if (eval) go(lo::k_dt_predict<float, true>, 0.0f); else go(lo::k_dt_predict<float, false>, 0.0f);
+    } else {
+        if (eval) go(lo::k_dt_predict<double, true>, 0.0); else go(lo::k_dt_predict<double, false>, 0.0);
+    }
+    if (eval) c.to_host(confusion_out, conf, (size_t)neval * C * 8);
+    bad.read(c);
+    LO_TRY(c.finish(timing));
+    if (!bad.found(k, info)) return LO_OK;
+    std::fill(confusion_out, confusion_out + (size_t)neval * C, (int64_t)0);
+    return fail(LO_ERR_INVALID, "row %lld: its label is not one of the evaluated labels", (long long)info->bad_row);
 }
 
 }  // extern "C"

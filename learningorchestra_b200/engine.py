@@ -401,6 +401,50 @@ class PredictedRows:
                 t.free()
 
 
+class SortedColumns:
+    """What :meth:`Engine.dt_sort` made: ``keys`` (a table holding kc sorted columns of n order-preserving codes),
+    ``f32`` (32-bit codes), ``distinct`` per column (ndistinct, values or None, counts or None).  :meth:`free` frees the
+    keys and may be called again."""
+
+    def __init__(self, keys: "DeviceTable", n: int, kc: int, f32: bool, distinct: list):
+        self.keys, self.n, self.kc, self.f32, self.distinct = keys, int(n), int(kc), bool(f32), distinct
+
+    def free(self) -> None:
+        if self.keys is not None:
+            self.keys.free()
+        self.keys = None
+
+
+class BinnedRows:
+    """What :meth:`Engine.dt_bin` made for one device's rows: ``codes`` (LO_U8, n rows at :func:`code_pitch` (k)) and
+    ``slots``, two LO_I32 tables of the rows' node slots that the levels write in turn (``cur`` the latest).  :meth:`free`
+    frees them and may be called again."""
+
+    def __init__(self, codes: "DeviceTable", slots: list):
+        self.codes, self.slots, self.cur = codes, slots, 0
+
+    def free(self) -> None:
+        for t in [self.codes, *self.slots]:
+            t.free()
+
+
+def code_pitch(k: int) -> int:
+    """The row pitch in bytes of the bin code matrix of k features: a multiple of 16, for 16-byte loads."""
+    return (k + 15) // 16 * 16
+
+
+def _threshold_table(thresholds, k: int):
+    """(f64 [k, tstride] thresholds padded, int32[k] counts, tstride >= 1) of per-column threshold lists."""
+    if len(thresholds) != k:
+        raise ValueError(f"{len(thresholds)} threshold lists for {k} features")
+    nthr = np.array([len(t) for t in thresholds], np.int32)
+    tstride = max(1, int(nthr.max()) if k else 1)
+    thr = np.zeros((k, tstride), np.float64)
+    for j, t in enumerate(thresholds):
+        thr[j, :len(t)] = t
+    return thr, nthr, tstride
+
+
 ASSEMBLE_MODES = {"error": N.LO_INVALID_ERROR, "skip": N.LO_INVALID_SKIP, "keep": N.LO_INVALID_KEEP}
 ASSEMBLE_DTYPES = {"float32": "f32", "float64": "f64"}
 
@@ -1111,6 +1155,102 @@ class Engine:
                                             None, C.byref(info), C.byref(t)))
         _report(timing, t)
         return PredictedRows(prob, rawt, pred, n, nout)
+
+    def dt_sort(self, part: AssembledRows, j0: int, kc: int, cap: int, timing: dict | None = None) -> "SortedColumns":
+        """Columns [j0, j0 + kc) of ``part`` sorted on the device as order-preserving codes (``lo_dt_sort``), with every
+        column's distinct values and their counts where there are at most ``cap`` of them."""
+        n, f32 = part.nkept, part.x.dtype_code == N.LO_F32
+        nd = np.zeros(kc, np.int64)
+        vals = np.zeros((kc, max(cap, 1)), np.float64)
+        cnts = np.zeros((kc, max(cap, 1)), np.int64)
+        t = N.HostTiming()
+        with _Owned() as owned:
+            keys = owned.own(self.table("f32" if f32 else "f64", max(n * kc, 1), 1))
+            N.check(self._lib.lo_dt_sort(self._ctx, part.x._h, part.k, part.k, n, int(j0), int(kc), keys._h, int(cap),
+                                         nd.ctypes.data_as(C.c_void_p), vals.ctypes.data_as(C.c_void_p),
+                                         cnts.ctypes.data_as(C.c_void_p), C.byref(t)))
+        _report(timing, t)
+        distinct = [(int(d), vals[c, :d].copy() if d <= cap else None, cnts[c, :d].copy() if d <= cap else None)
+                    for c, d in enumerate(nd)]
+        return SortedColumns(keys, n, kc, f32, distinct)
+
+    def dt_rank(self, sorted_cols: "SortedColumns", cols, codes) -> tuple[np.ndarray, np.ndarray]:
+        """(lt, le) int64 of every probe: the codes of column cols[i] below / up to codes[i] (``lo_dt_rank``)."""
+        cols = np.ascontiguousarray(cols, np.int32)
+        codes = np.ascontiguousarray(codes, np.uint64)
+        lt, le = np.zeros(len(cols), np.int64), np.zeros(len(cols), np.int64)
+        N.check(self._lib.lo_dt_rank(self._ctx, sorted_cols.keys._h, sorted_cols.n, sorted_cols.kc, len(cols),
+                                     cols.ctypes.data_as(C.c_void_p), codes.ctypes.data_as(C.c_void_p),
+                                     lt.ctypes.data_as(C.c_void_p), le.ctypes.data_as(C.c_void_p), None))
+        return lt, le
+
+    def dt_bin(self, part: AssembledRows, thresholds, timing: dict | None = None) -> "BinnedRows":
+        """The bin code of every value of ``part`` (``lo_dt_bin``): Spark's findBin, java.util.Arrays.binarySearch of the
+        column's ascending thresholds (without equal thresholds, the count of them below the value), in an LO_U8 table
+        of n rows at pitch :func:`code_pitch` (k), with the two slot tables the levels use."""
+        thr, nthr, tstride = _threshold_table(thresholds, part.k)
+        kp = code_pitch(part.k)
+        t = N.HostTiming()
+        with _Owned() as owned:
+            codes = owned.own(self.table("u8", max(part.nkept * kp, 1), 1))
+            slots = [owned.own(self.table("i32", max(part.nkept, 1), 1)) for _ in range(2)]
+            N.check(self._lib.lo_dt_bin(self._ctx, part.x._h, part.k, part.k, part.nkept, thr.ctypes.data_as(C.c_void_p),
+                                        nthr.ctypes.data_as(C.c_void_p), tstride, codes._h, kp, C.byref(t)))
+        _report(timing, t)
+        return BinnedRows(codes, slots)
+
+    def dt_level(self, part: AssembledRows, binned: "BinnedRows", nbins: int, nclasses: int, splits, nnodes: int,
+                 shape: list | None = None, timing: dict | None = None) -> np.ndarray:
+        """One tree level over ``part``'s rows (``lo_dt_level``): int64 (nnodes, k, nbins, nclasses) counts of (node
+        slot, feature, bin, class).  ``splits`` None: the root level; else int32 (parents, 4) rows (feature, bin, left
+        slot, right slot) of the previous level's nodes, by which the rows are routed (their slots ping-pong between
+        ``binned``'s two tables).  ``shape``: a list to receive the launch shape (16-byte loads, features per chunk,
+        nodes per pass, passes).  The whole level comes back to the host, however many node groups the device used.  A
+        code >= nbins or a label outside [0, nclasses) raises LoexecError naming the row."""
+        k = part.k
+        hist = np.zeros((nnodes, k, nbins, nclasses), np.int64)
+        sp = np.ascontiguousarray(splits if splits is not None else np.zeros((0, 4)), np.int32)
+        src = None if splits is None else binned.slots[binned.cur]
+        dst = binned.slots[0 if splits is None else 1 - binned.cur]
+        sh = np.zeros(4, np.int32)
+        t = N.HostTiming()
+        N.check(self._lib.lo_dt_level(self._ctx, binned.codes._h, code_pitch(k), k, part.y._h, part.nkept, int(nbins),
+                                      int(nclasses), src._h if src is not None else None, int(splits is not None),
+                                      dst._h, len(sp), sp.ctypes.data_as(C.c_void_p), int(nnodes),
+                                      hist.ctypes.data_as(C.c_void_p), sh.ctypes.data_as(C.c_void_p), C.byref(t)))
+        binned.cur = binned.slots.index(dst)
+        if shape is not None:
+            shape[:] = [int(v) for v in sh]
+        _report(timing, t)
+        return hist
+
+    def dt_predict(self, part: AssembledRows, tree, raw: bool = False, labels=None, timing: dict | None = None):
+        """A tree (:class:`~tree.Tree`) over ``part`` (``lo_dt_predict``), as :meth:`nb_predict`: ``labels`` None gives a
+        :class:`PredictedRows` of C columns, else the int64[len(labels), C] confusion counts."""
+        n, C_ = part.nkept, tree.num_classes
+        arrs = [np.ascontiguousarray(a, dt) for a, dt in ((tree.feature, np.int32), (tree.threshold, np.float64),
+                                                          (tree.left, np.int32), (tree.right, np.int32),
+                                                          (tree.counts, np.float64))]
+        info, t = N.NbInfo(), N.HostTiming()
+        args = (self._ctx, part.x._h, part.k, part.k, n, tree.num_nodes, *[a.ctypes.data_as(C.c_void_p) for a in arrs], C_)
+        if labels is not None:
+            if part.y is None:
+                raise ValueError("the rows have no label")
+            lab = np.ascontiguousarray(labels, dtype=np.float64)
+            conf = np.zeros((len(lab), C_), np.int64)
+            rc = self._lib.lo_dt_predict(*args, None, None, None, part.y._h, lab.ctypes.data_as(C.c_void_p), len(lab),
+                                         conf.ctypes.data_as(C.c_void_p), C.byref(info), C.byref(t))
+            _check_cells(rc, info, part.k, _EVALUATE_REFUSED)
+            _report(timing, t)
+            return conf
+        with _Owned() as owned:
+            prob = owned.own(self.table("f64", max(n * C_, 1), 1))
+            pred = owned.own(self.table("f64", max(n, 1), 1))
+            rawt = owned.own(self.table("f64", max(n * C_, 1), 1) if raw else None)
+            N.check(self._lib.lo_dt_predict(*args, prob._h, rawt._h if rawt is not None else None, pred._h, None, None, 0,
+                                            None, C.byref(info), C.byref(t)))
+        _report(timing, t)
+        return PredictedRows(prob, rawt, pred, n, C_)
 
     def value_counts_f64_host(self, values: np.ndarray):
         """(keys float64[g], counts uint64[g]) — exact value counts of a numeric column (GPU hash group-by),

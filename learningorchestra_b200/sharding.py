@@ -822,6 +822,48 @@ class ShardedEngine:
             confusion = confusion + c
         return confusion
 
+    def dt_sort(self, parts, j0: int, kc: int, cap: int) -> list:
+        """``Engine.dt_sort`` on every member, each on its own device from a host thread of its own: one
+        ``SortedColumns`` per member (each sorts only its own rows)."""
+        return self._each("dt_sort", lambda i: self.engines[i].dt_sort(parts[i], j0, kc, cap), undo=lambda s: s.free())
+
+    def dt_rank(self, sorted_cols: list, cols, codes):
+        """``Engine.dt_rank`` on every member's sorted columns; the counts added in shard order: ranks in the union."""
+        got = self._each("dt_rank", lambda i: self.engines[i].dt_rank(sorted_cols[i], cols, codes))
+        lt, le = got[0]
+        for a, b in got[1:]:
+            lt, le = lt + a, le + b
+        return lt, le
+
+    def dt_bin(self, parts, thresholds) -> list:
+        """``Engine.dt_bin`` on every member: one ``BinnedRows`` per member."""
+        return self._each("dt_bin", lambda i: self.engines[i].dt_bin(parts[i], thresholds), undo=lambda b: b.free())
+
+    def dt_level(self, parts, binned: list, nbins: int, nclasses: int, splits, nnodes: int, shape: list | None = None):
+        """``Engine.dt_level`` on every member over the same splits; the integer histograms added in shard order, so
+        they do not depend on the cut.  ``shape`` receives the first member's launch shape."""
+        shapes = [[] for _ in parts]
+        got = self._each("dt_level", lambda i: self.engines[i].dt_level(parts[i], binned[i], nbins, nclasses, splits,
+                                                                        nnodes, shapes[i]))
+        if shape is not None:
+            shape[:] = shapes[0]
+        hist = got[0]
+        for h in got[1:]:
+            hist = hist + h
+        return hist
+
+    def dt_predict(self, parts, tree, raw: bool = False, labels=None):
+        """``Engine.dt_predict`` over the shards, as :meth:`nb_predict`: one ``PredictedRows`` per member, or the
+        members' confusion counts summed; a refused row is raised as the lowest over all shards, its row global."""
+        got = self._each("dt_predict", lambda i: self.engines[i].dt_predict(parts[i], tree, raw, labels),
+                         undo=(lambda p: p.free()) if labels is None else None, first_rows=_firsts(parts))
+        if labels is None:
+            return got
+        confusion = got[0]
+        for c in got[1:]:
+            confusion = confusion + c
+        return confusion
+
     @property
     def resident(self):
         """Datasets kept in HBM between requests, rows sharded over the group (:mod:`table_cache`)."""

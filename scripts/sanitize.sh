@@ -38,6 +38,15 @@ lr_race_log="$(mktemp -d)/sanitizer_racecheck_logistic.txt"
 timeout 1800 compute-sanitizer --tool racecheck --error-exitcode 1 python -m pytest tests/test_gpu_logistic_exact.py -q \
     -k "shape" > "$lr_race_log" 2>&1
 echo "racecheck (logistic) rc=$? log=$lr_race_log"; tail -3 "$lr_race_log"
+# memcheck and racecheck of the DecisionTree kernels (sort, distinct, rank, bin, every level route, predict, evaluate;
+# the caps and refusals); their logs go to a temporary directory
+dt_log="$(mktemp -d)/sanitizer_memcheck_tree.txt"
+timeout 1800 compute-sanitizer --tool memcheck --error-exitcode 1 python -m pytest tests/test_gpu_tree.py -q > "$dt_log" 2>&1
+echo "memcheck (tree) rc=$? log=$dt_log"; tail -3 "$dt_log"
+dt_race_log="$(mktemp -d)/sanitizer_racecheck_tree.txt"
+timeout 1800 compute-sanitizer --tool racecheck --error-exitcode 1 python -m pytest tests/test_gpu_tree.py -q \
+    -k "route or edges" > "$dt_race_log" 2>&1
+echo "racecheck (tree) rc=$? log=$dt_race_log"; tail -3 "$dt_race_log"
 # memcheck of the number parser and the resident formatter on every entry point, without the million-row cases: a read
 # past the last staged cell shows here (the CPU harness puts a NUL after it)
 parse_log="$(mktemp -d)/sanitizer_memcheck_parse.txt"
