@@ -633,6 +633,43 @@ int lo_dt_predict(lo_ctx *ctx, const lo_table *x, int64_t ld, int32_t k, int64_t
                   const double *eval_labels, int32_t neval, int64_t *confusion_out, lo_nb_info *info,
                   lo_host_timing *timing);
 
+/* Spark 2.4's GBTClassifier (logistic loss, DESIGN.md §3.6.5) over the matrix of lo_assemble_rows: regression trees
+ * grown on lo_dt_bin's codes from exact fixed-point sums of the residuals, and the fit's margins and residuals kept on
+ * the device.  The features are first checked by lo_lr_stats_range; these calls do not check them again.
+ *
+ * lo_gb_level: lo_dt_level with the residuals (LO_F64, n) in place of the labels: words_out (host uint64[nnodes][k]
+ *   [nbins][LO_GB_WORDS]) = per (slot, feature, bin) the rows' count, the sum of (q1 + 2^60) and the sum of q2 as 128-bit
+ *   integers (lo word, hi word), q1 = rint(r * 2^58), q2 = rint((r * r) * 2^58).  Sums of several calls (shards) add
+ *   as 128-bit integers.  A residual that is NaN or outside [-4, 4] is never counted: the call fails with
+ *   LO_ERR_INVALID naming the lowest such row and words_out zeroed.  Otherwise as lo_dt_level, with k * nbins *
+ *   LO_GB_WORDS * 8 bytes per node within LO_DT_PASS_HIST.
+ * lo_gb_stats (host only): (count, sum, sumsq) of lo_gb_level's words (nnodes nodes): total_out[g * 3 ..] of every row
+ *   of node g, left_out / right_out [((g * k + j) * nsplits + i) * 3 ..] of the rows whose code of feature j is <= i /
+ *   > i, for the splits i < nsplits (< nbins).  Prefix and difference on the integers; each statistic then rounded to
+ *   f64 once (the sums as sum(q1) * 2^-58 and sum(q2) * 2^-58).
+ * lo_gb_update: after tree nnodes (the arrays of lo_dt_predict, value = the leaf's prediction) of weight `weight`:
+ *   margin[r] += value[leaf] * weight, residual[r] = 4y' / (1 + exp(2y' margin[r])) with y' = 2y - 1 (LO_F64 tables of
+ *   n).  nnodes 0 initialises: margin = 0, residual = y'.  A label other than 0 or 1 fails with LO_ERR_INVALID and
+ *   info->bad_row / bad_col (k).
+ * lo_gb_predict: the margin m of ntrees trees (nodes [start[t], start[t + 1]) of the arrays, children as indices into
+ *   them; start[0] = 0), sum of value[leaf] * weight[t] in tree order, as lo_dt_predict's transform and evaluate with
+ *   two classes: raw = [-m, m], probability = [1 / (1 + exp(2m)), 1 - that], prediction = m > 0. */
+#define LO_GB_WORDS        5            /* count, sum of q1 + 2^60 (lo, hi), sum of q2 (lo, hi) */
+int lo_gb_level(lo_ctx *ctx, const lo_table *codes, int64_t kp, int32_t k, const lo_table *residual, int64_t n,
+                int32_t nbins, const lo_table *src, int32_t route, lo_table *dst, int32_t nparents, const int32_t *splits,
+                int32_t nnodes, uint64_t *words_out, int32_t *shape_out, lo_host_timing *timing);
+int lo_gb_stats(const uint64_t *words, int64_t nnodes, int32_t k, int32_t nbins, int32_t nsplits, double *left_out,
+                double *right_out, double *total_out);
+int lo_gb_update(lo_ctx *ctx, const lo_table *x, int64_t ld, int32_t k, const lo_table *y, int64_t n, int32_t nnodes,
+                 const int32_t *feature, const double *threshold, const int32_t *left, const int32_t *right,
+                 const double *value, double weight, lo_table *margin, lo_table *residual, lo_nb_info *info,
+                 lo_host_timing *timing);
+int lo_gb_predict(lo_ctx *ctx, const lo_table *x, int64_t ld, int32_t k, int64_t n, int32_t ntrees, const int32_t *start,
+                  const double *weight, int32_t nnodes, const int32_t *feature, const double *threshold,
+                  const int32_t *left, const int32_t *right, const double *value, lo_table *prob, lo_table *raw,
+                  lo_table *pred, const lo_table *y, const double *eval_labels, int32_t neval, int64_t *confusion_out,
+                  lo_nb_info *info, lo_host_timing *timing);
+
 /* Number -> text for one column: the reference's "string" cast, str(v) / None -> "" (data_type_handler_image/
  * data_type_update.py:22-28), for every cell at once on the GPU.  The inverse of lo_parse_number_host.
  * status[i] uses the LO_NUM_* codes above: FLOAT -> repr(float) (shortest round-trip digits, CPython's notation),

@@ -1,7 +1,7 @@
-"""The builder's "NB", "LR" and "DT" classifiers on the GPU: Spark 2.4's multinomial ``NaiveBayes``,
-``LogisticRegression`` and ``DecisionTreeClassifier`` (``builder_image/builder.py:55-61``) fitted on, applied to and
-evaluated over the feature matrix in HBM (:meth:`DeviceFrame.features`), on one GPU or on every shard of a local
-:class:`~sharding.ShardedEngine`.  DESIGN.md §3.6.2 to §3.6.4 state the semantics.
+"""The builder's "NB", "LR", "DT" and "GB" classifiers on the GPU: Spark 2.4's multinomial ``NaiveBayes``,
+``LogisticRegression``, ``DecisionTreeClassifier`` and ``GBTClassifier`` (``builder_image/builder.py:55-61``) fitted on,
+applied to and evaluated over the feature matrix in HBM (:meth:`DeviceFrame.features`), on one GPU or on every shard of
+a local :class:`~sharding.ShardedEngine`.  DESIGN.md §3.6.2 to §3.6.5 state the semantics.
 
 NaiveBayes: the device computes the class counts and per-class feature sums (``lo_nb_fit``); LogisticRegression: the
 column statistics and label counts (``lo_lr_stats``) and one pass of loss and gradient sums per function evaluation of
@@ -9,7 +9,8 @@ the host's L-BFGS (``lo_lr_loss_grad``, :mod:`lbfgs`).  Both compute every row's
 (``lo_nb_predict`` / ``lo_lr_predict``) and the confusion counts of an evaluation on the device; the models' arrays and
 the evaluator's metrics are computed here, on the host, from those.  DecisionTreeClassifier: the device sorts the
 columns, answers rank queries, bins the values and counts every tree level (``lo_dt_*``); :mod:`tree` chooses the
-thresholds and splits from those counts."""
+thresholds and splits from those counts.  GBTClassifier grows its regression trees on the same codes from exact
+fixed-point residual sums (``lo_gb_level``) and keeps every row's margin and residual on the device (``lo_gb_update``)."""
 from __future__ import annotations
 
 import math
@@ -351,6 +352,42 @@ class Predictions:
 _DT_SORT_BUDGET = 2 << 30      # bytes of sorted codes and sort scratch per column batch of lo_dt_sort
 
 
+def split_thresholds(features, n: int, k: int, max_bins: int, name: str) -> tuple[list, int]:
+    """Every column's split thresholds (DecisionTreeClassifier and GBTClassifier): the columns sorted on the device in
+    batches within _DT_SORT_BUDGET, each batch's distinct values merged or its order statistics found by rank rounds
+    (:func:`tree.column_thresholds`), and its sorted copies freed before the next.  Returns (thresholds, rank rounds)."""
+    from . import tree as T
+    f32 = features._parts[0].x.dtype_code == N.LO_F32
+    per_col = 2 * (4 if f32 else 8) * max(n, 1)
+    kc = max(1, min(k, _DT_SORT_BUDGET // per_col))
+    cap = T.num_splits(max_bins, n) + 1
+    out, rounds = [], 0
+    for j0 in range(0, k, kc):
+        w = min(kc, k - j0)
+        got = _on_device(features, lambda engine, rows: engine.dt_sort(rows, j0, w, cap), name=name)
+        members = got if isinstance(got, list) else [got]
+        try:
+            distinct = [T.merge_distinct([m.distinct[c] for m in members]) for c in range(w)]
+
+            def rank(cols, codes):
+                return _on_device(features, lambda engine, rows: engine.dt_rank(got, cols, codes), name=name)
+
+            thr, r = T.column_thresholds(n, max_bins, distinct, rank, f32, w)
+        finally:
+            for m in members:
+                m.free()
+        out += thr
+        rounds += r
+    return out, rounds
+
+
+def _integer(v, name, lo, hi=None):
+    if isinstance(v, bool) or not isinstance(v, (int, np.integer)) or v < lo or (hi is not None and v > hi):
+        span = f"in [{lo}, {hi}]" if hi is not None else f">= {lo}"
+        raise ValueError(f"{name} must be an integer {span}, not {v!r}")
+    return int(v)
+
+
 class DecisionTreeClassifier:
     """``pyspark.ml.classification.DecisionTreeClassifier(maxDepth, maxBins, minInstancesPerNode, minInfoGain,
     impurity)`` with its other defaults (every feature continuous, no ``weightCol``, no ``thresholds``) on the GPU.
@@ -359,16 +396,9 @@ class DecisionTreeClassifier:
     def __init__(self, max_depth: int = 5, max_bins: int = 32, min_instances_per_node: int = 1,
                  min_info_gain: float = 0.0, impurity: str = "gini"):
         from . import tree as T
-
-        def integer(v, name, lo, hi=None):
-            if isinstance(v, bool) or not isinstance(v, (int, np.integer)) or v < lo or (hi is not None and v > hi):
-                span = f"in [{lo}, {hi}]" if hi is not None else f">= {lo}"
-                raise ValueError(f"{name} must be an integer {span}, not {v!r}")
-            return int(v)
-
-        self.max_depth = integer(max_depth, "max_depth", 0, T.MAX_DEPTH)
-        self.max_bins = integer(max_bins, "max_bins", 2, T.MAX_BINS)
-        self.min_instances_per_node = integer(min_instances_per_node, "min_instances_per_node", 1)
+        self.max_depth = _integer(max_depth, "max_depth", 0, T.MAX_DEPTH)
+        self.max_bins = _integer(max_bins, "max_bins", 2, T.MAX_BINS)
+        self.min_instances_per_node = _integer(min_instances_per_node, "min_instances_per_node", 1)
         g = float(min_info_gain)
         if not np.isfinite(g) or g < 0.0:
             raise ValueError(f"min_info_gain must be finite and >= 0, not {min_info_gain!r}")
@@ -398,7 +428,7 @@ class DecisionTreeClassifier:
         if k * min(self.max_bins, n) * num_classes * 8 > N.LO_DT_PASS_HIST:
             raise N.LoexecError(N.LO_ERR_INVALID, f"{k} features x {min(self.max_bins, n)} bins x {num_classes} classes: "
                                 f"one node's histogram exceeds LO_DT_PASS_HIST = {N.LO_DT_PASS_HIST} bytes")
-        thresholds, rounds = self._thresholds(features, n, k)
+        thresholds, rounds = split_thresholds(features, n, k, self.max_bins, name)
         nbins = max(len(t) for t in thresholds) + 1
         binned = _on_device(features, lambda engine, rows: engine.dt_bin(rows, thresholds), name=name)
         try:
@@ -414,36 +444,6 @@ class DecisionTreeClassifier:
         model = DecisionTreeClassificationModel(tree, features.fields, thresholds)
         model.rank_rounds = rounds
         return model
-
-    def _thresholds(self, features, n: int, k: int) -> tuple[list, int]:
-        """Every column's split thresholds: the columns sorted on the device in batches within _DT_SORT_BUDGET, each
-        batch's distinct values merged or its order statistics found by rank rounds (:func:`tree.column_thresholds`),
-        and its sorted copies freed before the next."""
-        from . import tree as T
-        f32 = features._parts[0].x.dtype_code == N.LO_F32
-        per_col = 2 * (4 if f32 else 8) * max(n, 1)
-        kc = max(1, min(k, _DT_SORT_BUDGET // per_col))
-        cap = T.num_splits(self.max_bins, n) + 1
-        out, rounds = [], 0
-        for j0 in range(0, k, kc):
-            w = min(kc, k - j0)
-            got = _on_device(features, lambda engine, rows: engine.dt_sort(rows, j0, w, cap),
-                             name="DecisionTreeClassifier")
-            members = got if isinstance(got, list) else [got]
-            try:
-                distinct = [T.merge_distinct([m.distinct[c] for m in members]) for c in range(w)]
-
-                def rank(cols, codes):
-                    return _on_device(features, lambda engine, rows: engine.dt_rank(got, cols, codes),
-                                      name="DecisionTreeClassifier")
-
-                thr, r = T.column_thresholds(n, self.max_bins, distinct, rank, f32, w)
-            finally:
-                for m in members:
-                    m.free()
-            out += thr
-            rounds += r
-        return out, rounds
 
 
 class DecisionTreeClassificationModel:
@@ -479,5 +479,131 @@ class DecisionTreeClassificationModel:
             raise N.LoexecError(N.LO_ERR_INVALID, "evaluate needs at least one row")
         confusion = _on_device(features, lambda engine, rows: engine.dt_predict(rows, self.tree, labels=labels),
                                name="DecisionTreeClassifier", reasons=_LR_REASONS)
+        f1, accuracy = metrics(labels, confusion)
+        return {"f1": f1, "accuracy": accuracy, "labels": labels, "confusion": confusion}
+
+
+_GB_REASONS = ("is NaN or infinite", "is not a label 0 or 1")
+
+
+class GBTClassifier:
+    """``pyspark.ml.classification.GBTClassifier(maxIter, stepSize, maxDepth, maxBins, minInstancesPerNode,
+    minInfoGain)`` with its other defaults (``lossType="logistic"``, ``subsamplingRate=1``, every feature and every row
+    in every tree, no validation, no ``weightCol``, no ``thresholds``) on the GPU (DESIGN.md §3.6.5).  max_iter 0 is
+    refused, and so is max_bins above LO_DT_MAX_BINS (256): a bin index is a byte on the device."""
+
+    def __init__(self, max_iter: int = 20, step_size: float = 0.1, max_depth: int = 5, max_bins: int = 32,
+                 min_instances_per_node: int = 1, min_info_gain: float = 0.0):
+        from . import tree as T
+        self.max_iter = _integer(max_iter, "max_iter", 1)
+        st = float(step_size) if isinstance(step_size, (int, float, np.floating)) and not isinstance(step_size, bool) \
+            else float("nan")
+        if not 0.0 < st <= 1.0:
+            raise ValueError(f"step_size must lie in (0, 1], not {step_size!r}")
+        self.step_size = st
+        self.max_depth = _integer(max_depth, "max_depth", 0, T.MAX_DEPTH)
+        self.max_bins = _integer(max_bins, "max_bins", 2, T.MAX_BINS)
+        self.min_instances_per_node = _integer(min_instances_per_node, "min_instances_per_node", 1)
+        g = float(min_info_gain)
+        if not np.isfinite(g) or g < 0.0:
+            raise ValueError(f"min_info_gain must be finite and >= 0, not {min_info_gain!r}")
+        self.min_info_gain = g
+
+    def fit(self, features) -> "GBTClassificationModel":
+        """The boosted trees of ``features`` (:class:`~builder_frontend.Features` with a label, on one GPU or sharded).
+        Every label must be 0 or 1 and every feature finite (InvalidCellError naming the ``_id`` and field of the lowest
+        refused cell over both checks).  No row, or a one-node level (k x min(max_bins, n) x 40 bytes) above LO_DT_PASS_HIST, is
+        refused.  The margins and residuals stay on the device, the trees are chosen here from each level's sums."""
+        from . import tree as T
+        _usable(features)
+        if features.label is None:
+            raise ValueError("GBTClassifier needs features with a label")
+        name, k = "GBTClassifier", len(features.fields)
+        from .engine import InvalidCellError
+        # the labels (lo_gb_update's first call) and the features (lo_lr_stats_range) are both checked, and the lowest
+        # refused cell of the two is raised, as one pass over both would find it
+        refused, rows, binned = [], None, None
+        try:
+            rows = _on_device(features, lambda engine, part: engine.gb_update(part), name=name, reasons=_GB_REASONS)
+        except InvalidCellError as e:
+            refused.append(e)
+        try:
+            try:
+                n = _on_device(features, lambda engine, part: engine.lr_stats(part), name=name, reasons=_GB_REASONS)[0]
+            except InvalidCellError as e:
+                refused.append(e)
+            except N.LoexecError:                    # a label >= LO_NB_MAX_CLASSES: already a refused label cell
+                if not refused:
+                    raise
+            if refused:
+                raise min(refused, key=lambda e: (e.row, e.position))
+            if n == 0:
+                raise N.LoexecError(N.LO_ERR_INVALID, "GBTClassifier needs at least one row")
+            if k * min(self.max_bins, n) * N.LO_GB_WORDS * 8 > N.LO_DT_PASS_HIST:
+                raise N.LoexecError(N.LO_ERR_INVALID, f"{k} features x {min(self.max_bins, n)} bins x "
+                                    f"{N.LO_GB_WORDS} words: one node's histogram exceeds LO_DT_PASS_HIST = "
+                                    f"{N.LO_DT_PASS_HIST} bytes")
+            thresholds, _rounds = split_thresholds(features, n, k, self.max_bins, name)
+            nbins = max(len(t) for t in thresholds) + 1
+            binned = _on_device(features, lambda engine, part: engine.dt_bin(part, thresholds), name=name)
+            trees, weights = [], []
+            for m in range(self.max_iter):
+                def level(splits, nnodes):
+                    return _on_device(features, lambda engine, part: engine.gb_level(part, binned, rows, nbins, splits,
+                                                                                    nnodes), name=name)
+
+                tree, _shapes = T.grow(level, thresholds, 0, self.max_depth, T.VARIANCE, self.min_instances_per_node,
+                                       self.min_info_gain)
+                weight = 1.0 if m == 0 else self.step_size
+                trees.append(tree)
+                weights.append(weight)
+                if m + 1 < self.max_iter:
+                    _on_device(features, lambda engine, part: engine.gb_update(part, rows, tree, weight), name=name,
+                               reasons=_GB_REASONS)
+        finally:
+            for held in (rows, binned):
+                for b in held if isinstance(held, list) else [held] if held is not None else []:
+                    b.free()
+        return GBTClassificationModel(trees, weights, features.fields, thresholds)
+
+
+class GBTClassificationModel:
+    """A fitted GBT model, host data: ``trees`` (regression :class:`~tree.Tree` s in breadth-first arrays: feature,
+    threshold, left, right, prediction, impurity, gain and ``counts`` the node's (count, sum, sumSq)), ``tree_weights``
+    ([1.0, step_size, ...]), ``num_classes`` (2), ``total_num_nodes``, the ``fields`` it was fitted on and every column's
+    split ``thresholds``."""
+
+    def __init__(self, trees, tree_weights, fields, thresholds=None):
+        self.trees, self.tree_weights = list(trees), np.asarray(tree_weights, np.float64)
+        self.fields, self.thresholds = list(fields), thresholds
+        self.num_classes = 2
+        self.total_num_nodes = sum(t.num_nodes for t in self.trees)
+
+    def _check(self, features) -> None:
+        if list(features.fields) != self.fields:
+            raise ValueError(f"the model was fitted on fields {self.fields}, not {list(features.fields)}")
+
+    def transform(self, features, raw: bool = False) -> "Predictions":
+        """Spark's ``model.transform``: every row's ``probability`` ([1 / (1 + exp(2m)), the rest] of the margin m) and
+        ``prediction`` (m > 0), and with ``raw`` its ``rawPrediction`` ([-m, m]), written in HBM on the rows' own
+        devices."""
+        _usable(features)
+        self._check(features)
+        parts = _on_device(features, lambda engine, rows: engine.gb_predict(rows, self.trees, self.tree_weights,
+                                                                            raw=raw), per_part=True,
+                           name="GBTClassifier", reasons=_GB_REASONS)
+        return Predictions(features, parts)
+
+    def evaluate(self, features) -> dict:
+        """``MulticlassClassificationEvaluator`` f1 and accuracy over ``transform(features)``, as
+        :meth:`NaiveBayesModel.evaluate`: ``{"f1", "accuracy", "labels", "confusion"}``."""
+        _usable(features)
+        self._check(features)
+        labels = _labels(features, "GBTClassifier", _GB_REASONS)
+        if len(features.row_ids) == 0:
+            raise N.LoexecError(N.LO_ERR_INVALID, "evaluate needs at least one row")
+        confusion = _on_device(features, lambda engine, rows: engine.gb_predict(rows, self.trees, self.tree_weights,
+                                                                                labels=labels),
+                               name="GBTClassifier", reasons=_GB_REASONS)
         f1, accuracy = metrics(labels, confusion)
         return {"f1": f1, "accuracy": accuracy, "labels": labels, "confusion": confusion}

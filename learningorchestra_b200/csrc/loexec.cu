@@ -3110,7 +3110,7 @@ int lo_lr_predict(lo_ctx *ctx, const lo_table *x, int64_t ld, int32_t k, int64_t
 }  // extern "C"
 
 static_assert(lo::kDtMaxBins == LO_DT_MAX_BINS && lo::kDtMaxClasses == LO_DT_MAX_CLASSES &&
-              lo::kDtPassHist == LO_DT_PASS_HIST, "loexec.h documents the tree's caps");
+              lo::kDtPassHist == LO_DT_PASS_HIST && lo::kGbWords == LO_GB_WORDS, "loexec.h documents the tree's caps");
 
 namespace {
 
@@ -3130,14 +3130,14 @@ int check_dt_classes(int32_t nclasses) {
     return LO_OK;
 }
 
-// The launch shape of a level of nnodes nodes (lo_dt_level): a feature's histogram of one node takes cell = nbins * C
-// u32 counters; a CTA holds gn nodes x fc features of them within kDtHistSmem.  fc is a multiple of 16 (16-byte code
+// The launch shape of a level of nnodes nodes (lo_dt_level, lo_gb_level): a feature's histogram of one node takes cell =
+// nbins * C counters of wbytes (lo_dt_level: u32 class counts; lo_gb_level: C = 5 u64 words); a CTA holds gn nodes x fc features of them within kDtHistSmem.  fc is a multiple of 16 (16-byte code
 // loads) when 16 cells fit, else as many single features as fit (scalar loads); gn as many nodes as fit beside, and as
 // keep the pass's u64 histogram within kDtPassHist.  passes = node groups, each one pass over the rows.
 struct DtShape { int vec, fc, gn, passes, smem; };
-DtShape dt_shape(int32_t k, int32_t nbins, int32_t C, int32_t nnodes) {
+DtShape dt_shape(int32_t k, int32_t nbins, int32_t C, int32_t nnodes, int32_t wbytes = 4) {
     DtShape sh{};
-    const int64_t cell = (int64_t)nbins * C * 4, cells = lo::kDtHistSmem / cell;
+    const int64_t cell = (int64_t)nbins * C * wbytes, cells = lo::kDtHistSmem / cell;
     const int64_t kpad = ((int64_t)k + lo::kDtVec - 1) / lo::kDtVec * lo::kDtVec;
     sh.vec = cells >= lo::kDtVec;
     sh.fc = (int)(sh.vec ? std::min<int64_t>(kpad, cells / lo::kDtVec * lo::kDtVec) : std::min<int64_t>(k, cells));
@@ -3188,6 +3188,110 @@ double dt_value(uint64_t code, bool f32) {
     double v;
     std::memcpy(&v, &b, 8);
     return v;
+}
+
+// The checks and passes of one tree level shared by lo_dt_level and lo_gb_level: C u64 words per (node, feature, bin)
+// in hist_out, counted one node group of the launch shape at a time by k_dt_level over the labels y (GB false; C
+// classes, u32 counters of wbytes 4 in shared memory) or by k_gb_level over the residuals y (GB true; C = kGbWords
+// u64 words).  *key receives the lowest refused cell's key (~0: none); hist_out is zeroed when there is one.
+template <bool GB, typename T>
+int tree_level(lo_ctx *ctx, const char *name, const char *per_bin, const T *y, int32_t C, int32_t wbytes,
+               const lo_table *codes, int64_t kp, int32_t k, int64_t n, int32_t nbins, const lo_table *src,
+               int32_t route, lo_table *dst, int32_t nparents, const int32_t *splits, int32_t nnodes, int64_t *hist_out,
+               int32_t *shape_out, lo_host_timing *timing, unsigned long long *key) {
+    *key = ~0ull;
+    if (k < 1) return fail(LO_ERR_INVALID, "k = %d: at least one feature", k);
+    if (kp < k || kp % lo::kDtVec) return fail(LO_ERR_INVALID, "kp = %lld: a multiple of 16 >= k", (long long)kp);
+    if (n < 0) return fail(LO_ERR_INVALID, "n = %lld is negative", (long long)n);
+    LO_TRY(check_typed_table(ctx, codes, LO_U8, n * kp, "codes"));
+    if ((uintptr_t)codes->base % 16) return fail(LO_ERR_INVALID, "codes must start 16-byte aligned");
+    if (nbins < 1 || nbins > LO_DT_MAX_BINS) return fail(LO_ERR_INVALID, "nbins = %d outside [1, %d]", nbins, LO_DT_MAX_BINS);
+    if ((int64_t)k * nbins * C * 8 > LO_DT_PASS_HIST)
+        return fail(LO_ERR_INVALID, "%d features x %d bins x %d %s: one node's histogram exceeds LO_DT_PASS_HIST = %lld "
+                    "bytes", k, nbins, C, per_bin, (long long)LO_DT_PASS_HIST);
+    if (nnodes < 1) return fail(LO_ERR_INVALID, "nnodes = %d: at least one", nnodes);
+    if (route != 0 && route != 1) return fail(LO_ERR_INVALID, "route = %d: 0 or 1", route);
+    if (src) LO_TRY(check_typed_table(ctx, src, LO_I32, n, "src"));
+    else if (route || nnodes != 1) return fail(LO_ERR_INVALID, "without src every row is at the root: route 0, one node");
+    if (dst) LO_TRY(check_typed_table(ctx, dst, LO_I32, n, "dst"));
+    if (route) {
+        if (nparents < 1 || !splits) return fail(LO_ERR_INVALID, "routing needs the parents' splits");
+        for (int32_t p = 0; p < nparents; ++p) {
+            const int32_t *s = splits + (size_t)p * 4;
+            if (s[0] < 0) continue;
+            if (s[0] >= k || s[1] < 0 || s[1] >= nbins || s[2] < -1 || s[2] >= nnodes || s[3] < -1 || s[3] >= nnodes)
+                return fail(LO_ERR_INVALID, "split %d = (%d, %d, %d, %d) is out of range", p, s[0], s[1], s[2], s[3]);
+        }
+    }
+    if (!hist_out) return fail(LO_ERR_INVALID, "hist_out is NULL");
+    const DtShape sh = dt_shape(k, nbins, C, nnodes, wbytes);
+    if (shape_out) {
+        shape_out[0] = sh.vec;
+        shape_out[1] = sh.fc;
+        shape_out[2] = sh.gn;
+        shape_out[3] = sh.passes;
+    }
+    if (sh.passes > 1 && !dst) return fail(LO_ERR_INVALID, "%d node groups need dst to keep the rows' slots", sh.passes);
+    const size_t per_node = (size_t)k * nbins * C;
+    std::fill(hist_out, hist_out + per_node * nnodes, (int64_t)0);
+    HostCall c(ctx, name);
+    if (n == 0) return c.finish(timing);
+    int *d_split = nullptr;
+    unsigned long long *d_hist = nullptr;
+    RefusedCell bad;
+    bad.arm(c);
+    const int np = route ? nparents : 0;
+    if (np) {
+        std::vector<int32_t> soa((size_t)np * 4);        // feature, bin, left, right: one array each
+        for (int32_t p = 0; p < np; ++p)
+            for (int f = 0; f < 4; ++f) soa[(size_t)f * np + p] = splits[(size_t)p * 4 + f];
+        c.alloc(&d_split, soa.size() * 4);
+        c.to_dev(d_split, soa.data(), soa.size() * 4);
+    }
+    c.alloc(&d_hist, per_node * sh.gn * 8);
+    auto go = [&](auto kernel) {
+        int per_sm = 0;
+        c.run([&] { return cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, sh.smem); });
+        c.run([&] { return cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, lo::kDtThreads, sh.smem); });
+        const int nchunks = (k + sh.fc - 1) / sh.fc;
+        const int64_t want = (int64_t)ctx->sm_count * std::max(1, per_sm) / nchunks;
+        const dim3 grid((unsigned)std::max<int64_t>(1, std::min<int64_t>((n + lo::kDtThreads - 1) / lo::kDtThreads, want)),
+                        (unsigned)nchunks);
+        c.mark();
+        for (int pass = 0; pass < sh.passes; ++pass) {
+            const int g0 = pass * sh.gn, gn = std::min(sh.gn, nnodes - g0);
+            // the first pass routes (and writes dst); the later ones read the slots it wrote
+            const int *from = pass == 0 ? (src ? (const int *)src->base : nullptr) : (const int *)dst->base;
+            c.memset(d_hist, 0, per_node * gn * 8);
+            c.launch(1, [&] {
+                int *to = pass == 0 && dst ? (int *)dst->base : nullptr;
+                const int how = pass == 0 ? route : 0;
+                if constexpr (GB)
+                    kernel<<<grid, lo::kDtThreads, sh.smem, c.s>>>((const unsigned char *)codes->base, kp, k, y, n, nbins,
+                                                                   from, how, to, d_split, d_split + np,
+                                                                   d_split + 2 * np, d_split + 3 * np, g0, gn, sh.fc,
+                                                                   d_hist, bad.word);
+                else
+                    kernel<<<grid, lo::kDtThreads, sh.smem, c.s>>>((const unsigned char *)codes->base, kp, k, y, n, nbins,
+                                                                   C, from, how, to, d_split, d_split + np,
+                                                                   d_split + 2 * np, d_split + 3 * np, g0, gn, sh.fc,
+                                                                   d_hist, bad.word);
+            });
+            c.to_host(hist_out + per_node * g0, d_hist, per_node * gn * 8);
+            c.sync();                                       // d_hist is reused by the next pass
+        }
+        c.mark();
+    };
+    if constexpr (GB) {
+        if (sh.vec) go(lo::k_gb_level<true>); else go(lo::k_gb_level<false>);
+    } else {
+        if (sh.vec) go(lo::k_dt_level<T, true>); else go(lo::k_dt_level<T, false>);
+    }
+    bad.read(c);
+    LO_TRY(c.finish(timing));
+    *key = bad.key;
+    if (bad.key != ~0ull) std::fill(hist_out, hist_out + per_node * nnodes, (int64_t)0);
+    return LO_OK;
 }
 
 }  // namespace
@@ -3333,96 +3437,22 @@ int lo_dt_level(lo_ctx *ctx, const lo_table *codes, int64_t kp, int32_t k, const
                 int32_t nclasses, const lo_table *src, int32_t route, lo_table *dst, int32_t nparents,
                 const int32_t *splits, int32_t nnodes, int64_t *hist_out, int32_t *shape_out, lo_host_timing *timing) {
     LO_TRY(check_ctx(ctx));
-    if (k < 1) return fail(LO_ERR_INVALID, "k = %d: at least one feature", k);
-    if (kp < k || kp % lo::kDtVec) return fail(LO_ERR_INVALID, "kp = %lld: a multiple of 16 >= k", (long long)kp);
     if (n < 0) return fail(LO_ERR_INVALID, "n = %lld is negative", (long long)n);
-    LO_TRY(check_typed_table(ctx, codes, LO_U8, n * kp, "codes"));
-    if ((uintptr_t)codes->base % 16) return fail(LO_ERR_INVALID, "codes must start 16-byte aligned");
     LO_TRY(check_float_table(ctx, y, 0, n, "y"));
-    if (nbins < 1 || nbins > LO_DT_MAX_BINS) return fail(LO_ERR_INVALID, "nbins = %d outside [1, %d]", nbins, LO_DT_MAX_BINS);
     LO_TRY(check_dt_classes(nclasses));
-    if ((int64_t)k * nbins * nclasses * 8 > LO_DT_PASS_HIST)
-        return fail(LO_ERR_INVALID, "%d features x %d bins x %d classes: one node's histogram exceeds LO_DT_PASS_HIST = %lld "
-                    "bytes", k, nbins, nclasses, (long long)LO_DT_PASS_HIST);
-    if (nnodes < 1) return fail(LO_ERR_INVALID, "nnodes = %d: at least one", nnodes);
-    if (route != 0 && route != 1) return fail(LO_ERR_INVALID, "route = %d: 0 or 1", route);
-    if (src) LO_TRY(check_typed_table(ctx, src, LO_I32, n, "src"));
-    else if (route || nnodes != 1) return fail(LO_ERR_INVALID, "without src every row is at the root: route 0, one node");
-    if (dst) LO_TRY(check_typed_table(ctx, dst, LO_I32, n, "dst"));
-    if (route) {
-        if (nparents < 1 || !splits) return fail(LO_ERR_INVALID, "routing needs the parents' splits");
-        for (int32_t p = 0; p < nparents; ++p) {
-            const int32_t *s = splits + (size_t)p * 4;
-            if (s[0] < 0) continue;
-            if (s[0] >= k || s[1] < 0 || s[1] >= nbins || s[2] < -1 || s[2] >= nnodes || s[3] < -1 || s[3] >= nnodes)
-                return fail(LO_ERR_INVALID, "split %d = (%d, %d, %d, %d) is out of range", p, s[0], s[1], s[2], s[3]);
-        }
-    }
-    if (!hist_out) return fail(LO_ERR_INVALID, "hist_out is NULL");
-    const DtShape sh = dt_shape(k, nbins, nclasses, nnodes);
-    if (shape_out) {
-        shape_out[0] = sh.vec;
-        shape_out[1] = sh.fc;
-        shape_out[2] = sh.gn;
-        shape_out[3] = sh.passes;
-    }
-    if (sh.passes > 1 && !dst) return fail(LO_ERR_INVALID, "%d node groups need dst to keep the rows' slots", sh.passes);
-    const size_t per_node = (size_t)k * nbins * nclasses;
-    std::fill(hist_out, hist_out + per_node * nnodes, (int64_t)0);
-    HostCall c(ctx, "dt_level");
-    if (n == 0) return c.finish(timing);
-    int *d_split = nullptr;
-    unsigned long long *d_hist = nullptr;
-    RefusedCell bad;
-    bad.arm(c);
-    const int np = route ? nparents : 0;
-    if (np) {
-        std::vector<int32_t> soa((size_t)np * 4);        // feature, bin, left, right: one array each
-        for (int32_t p = 0; p < np; ++p)
-            for (int f = 0; f < 4; ++f) soa[(size_t)f * np + p] = splits[(size_t)p * 4 + f];
-        c.alloc(&d_split, soa.size() * 4);
-        c.to_dev(d_split, soa.data(), soa.size() * 4);
-    }
-    c.alloc(&d_hist, per_node * sh.gn * 8);
-    auto go = [&](auto kernel, auto tag) {
-        using T = decltype(tag);
-        int per_sm = 0;
-        c.run([&] { return cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, sh.smem); });
-        c.run([&] { return cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, lo::kDtThreads, sh.smem); });
-        const int nchunks = (k + sh.fc - 1) / sh.fc;
-        const int64_t want = (int64_t)ctx->sm_count * std::max(1, per_sm) / nchunks;
-        const dim3 grid((unsigned)std::max<int64_t>(1, std::min<int64_t>((n + lo::kDtThreads - 1) / lo::kDtThreads, want)),
-                        (unsigned)nchunks);
-        c.mark();
-        for (int pass = 0; pass < sh.passes; ++pass) {
-            const int g0 = pass * sh.gn, gn = std::min(sh.gn, nnodes - g0);
-            // the first pass routes (and writes dst); the later ones read the slots it wrote
-            const int *from = pass == 0 ? (src ? (const int *)src->base : nullptr) : (const int *)dst->base;
-            c.memset(d_hist, 0, per_node * gn * 8);
-            c.launch(1, [&] {
-                kernel<<<grid, lo::kDtThreads, sh.smem, c.s>>>((const unsigned char *)codes->base, kp, k, (const T *)y->base,
-                                                               n, nbins, nclasses, from, pass == 0 ? route : 0,
-                                                               pass == 0 && dst ? (int *)dst->base : nullptr,
-                                                               d_split, d_split + np, d_split + 2 * np, d_split + 3 * np,
-                                                               g0, gn, sh.fc, d_hist, bad.word);
-            });
-            c.to_host(hist_out + per_node * g0, d_hist, per_node * gn * 8);
-            c.sync();                                       // d_hist is reused by the next pass
-        }
-        c.mark();
-    };
-    if (y->dtype == LO_F32) {
-        if (sh.vec) go(lo::k_dt_level<float, true>, 0.0f); else go(lo::k_dt_level<float, false>, 0.0f);
-    } else {
-        if (sh.vec) go(lo::k_dt_level<double, true>, 0.0); else go(lo::k_dt_level<double, false>, 0.0);
-    }
-    bad.read(c);
-    LO_TRY(c.finish(timing));
-    if (bad.key == ~0ull) return LO_OK;
+    unsigned long long key = ~0ull;
+    if (y->dtype == LO_F32)
+        LO_TRY(tree_level<false>(ctx, "dt_level", "classes", (const float *)y->base, nclasses, 4,
+                          codes, kp, k, n, nbins, src, route, dst, nparents, splits, nnodes, hist_out, shape_out, timing,
+                          &key));
+    else
+        LO_TRY(tree_level<false>(ctx, "dt_level", "classes", (const double *)y->base, nclasses,
+                          4, codes, kp, k, n, nbins, src, route, dst, nparents, splits, nnodes, hist_out, shape_out,
+                          timing, &key));
+    if (key == ~0ull) return LO_OK;
     int64_t row = 0;
     int32_t col = 0;
-    lo::cell_of_key(bad.key, k, &row, &col);
-    std::fill(hist_out, hist_out + per_node * nnodes, (int64_t)0);
+    lo::cell_of_key(key, k, &row, &col);
     if (col == k) return fail(LO_ERR_INVALID, "row %lld: its label is not a class in [0, %d)", (long long)row, nclasses);
     return fail(LO_ERR_INVALID, "row %lld, feature %d: code >= nbins = %d", (long long)row, col, nbins);
 }
@@ -3514,6 +3544,236 @@ int lo_dt_predict(lo_ctx *ctx, const lo_table *x, int64_t ld, int32_t k, int64_t
     LO_TRY(c.finish(timing));
     if (!bad.found(k, info)) return LO_OK;
     std::fill(confusion_out, confusion_out + (size_t)neval * C, (int64_t)0);
+    return fail(LO_ERR_INVALID, "row %lld: its label is not one of the evaluated labels", (long long)info->bad_row);
+}
+
+int lo_gb_level(lo_ctx *ctx, const lo_table *codes, int64_t kp, int32_t k, const lo_table *residual, int64_t n,
+                int32_t nbins, const lo_table *src, int32_t route, lo_table *dst, int32_t nparents, const int32_t *splits,
+                int32_t nnodes, uint64_t *words_out, int32_t *shape_out, lo_host_timing *timing) {
+    LO_TRY(check_ctx(ctx));
+    if (n < 0) return fail(LO_ERR_INVALID, "n = %lld is negative", (long long)n);
+    LO_TRY(check_typed_table(ctx, residual, LO_F64, n, "residual"));
+    unsigned long long key = ~0ull;
+    LO_TRY(tree_level<true>(ctx, "gb_level", "words", (const double *)residual->base, LO_GB_WORDS, 8, codes, kp, k,
+                      n, nbins, src, route, dst, nparents, splits, nnodes, reinterpret_cast<int64_t *>(words_out),
+                      shape_out, timing, &key));
+    if (key == ~0ull) return LO_OK;
+    int64_t row = 0;
+    int32_t col = 0;
+    lo::cell_of_key(key, k, &row, &col);
+    if (col == k) return fail(LO_ERR_INVALID, "row %lld: its residual is NaN or outside [-4, 4]", (long long)row);
+    return fail(LO_ERR_INVALID, "row %lld, feature %d: code >= nbins = %d", (long long)row, col, nbins);
+}
+
+}  // extern "C"
+
+namespace {
+
+// the nodes [lo, hi) of one tree: features in [-1, k), an internal node's children inside (i, hi)
+int check_tree_nodes(const int32_t *feature, const int32_t *left, const int32_t *right, int32_t lo, int32_t hi, int32_t k) {
+    for (int32_t i = lo; i < hi; ++i) {
+        if (feature[i] < -1 || feature[i] >= k) return fail(LO_ERR_INVALID, "node %d: feature %d outside [-1, %d)", i, feature[i], k);
+        if (feature[i] >= 0 && !(left[i] > i && left[i] < hi && right[i] > i && right[i] < hi))
+            return fail(LO_ERR_INVALID, "node %d: children %d, %d must lie in (%d, %d)", i, left[i], right[i], i, hi);
+    }
+    return LO_OK;
+}
+
+// a 128-bit sum of lo_gb_level's words at w (lo, hi) as an integer
+__int128 gb_word(const uint64_t *w) { return (__int128)(((unsigned __int128)w[1] << 64) | w[0]); }
+
+}  // namespace
+
+extern "C" {
+
+int lo_gb_stats(const uint64_t *words, int64_t nnodes, int32_t k, int32_t nbins, int32_t nsplits, double *left_out,
+                double *right_out, double *total_out) {
+    if (!words || !total_out || (nsplits > 0 && (!left_out || !right_out)))
+        return fail(LO_ERR_INVALID, "words, left_out, right_out or total_out is NULL");
+    if (nnodes < 0 || k < 1 || nbins < 1 || nbins > LO_DT_MAX_BINS || nsplits < 0 || nsplits >= nbins)
+        return fail(LO_ERR_INVALID, "nnodes = %lld, k = %d, nbins = %d, nsplits = %d", (long long)nnodes, k, nbins, nsplits);
+    const double scale = 0x1p-58;
+    // (count, sum, sumsq) of integer sums: the count exact, Σq1 = Σ(q1 + 2^60) - 2^60 count, each rounded once
+    auto put = [&](double *o, __int128 cnt, __int128 s1, __int128 s2) {
+        o[0] = (double)cnt;
+        o[1] = (double)(s1 - (cnt << 60)) * scale;
+        o[2] = (double)s2 * scale;
+    };
+    const int W = LO_GB_WORDS;
+    for (int64_t g = 0; g < nnodes; ++g) {
+        const uint64_t *node = words + (size_t)g * k * nbins * W;
+        __int128 tc = 0, t1 = 0, t2 = 0;
+        for (int32_t b = 0; b < nbins; ++b) {           // every row of the node is in one bin of feature 0
+            const uint64_t *w = node + (size_t)b * W;
+            tc += (__int128)w[0];
+            t1 += gb_word(w + 1);
+            t2 += gb_word(w + 3);
+        }
+        put(total_out + g * 3, tc, t1, t2);
+        for (int32_t j = 0; j < k && nsplits > 0; ++j) {
+            __int128 lc = 0, l1 = 0, l2 = 0;
+            for (int32_t i = 0; i < nsplits; ++i) {
+                const uint64_t *w = node + ((size_t)j * nbins + i) * W;
+                lc += (__int128)w[0];
+                l1 += gb_word(w + 1);
+                l2 += gb_word(w + 3);
+                const size_t at = (((size_t)g * k + j) * nsplits + i) * 3;
+                put(left_out + at, lc, l1, l2);
+                put(right_out + at, tc - lc, t1 - l1, t2 - l2);
+            }
+        }
+    }
+    return LO_OK;
+}
+
+int lo_gb_update(lo_ctx *ctx, const lo_table *x, int64_t ld, int32_t k, const lo_table *y, int64_t n, int32_t nnodes,
+                 const int32_t *feature, const double *threshold, const int32_t *left, const int32_t *right,
+                 const double *value, double weight, lo_table *margin, lo_table *residual, lo_nb_info *info,
+                 lo_host_timing *timing) {
+    LO_TRY(check_ctx(ctx));
+    if (!info) return fail(LO_ERR_INVALID, "info is NULL");
+    *info = lo_nb_info{-1, -1, 0};
+    if (!y) return fail(LO_ERR_INVALID, "y is NULL");
+    LO_TRY(check_nb_matrix(ctx, x, ld, k, n, y));
+    LO_TRY(check_typed_table(ctx, margin, LO_F64, n, "margin"));
+    LO_TRY(check_typed_table(ctx, residual, LO_F64, n, "residual"));
+    const int32_t M = nnodes;
+    if (M < 0) return fail(LO_ERR_INVALID, "nnodes = %d is negative", M);
+    if (M > 0) {
+        if (!feature || !threshold || !left || !right || !value)
+            return fail(LO_ERR_INVALID, "a tree of %d nodes: feature, threshold, left, right and value are needed", M);
+        LO_TRY(check_tree_nodes(feature, left, right, 0, M, k));
+        if (!std::isfinite(weight)) return fail(LO_ERR_INVALID, "weight %g is not finite", weight);
+    }
+    HostCall c(ctx, M ? "gb_update" : "gb_init");
+    if (n == 0) return c.finish(timing);
+    int *d_int = nullptr;
+    double *d_dbl = nullptr;
+    RefusedCell bad;
+    bad.arm(c);
+    if (M > 0) {
+        c.alloc(&d_int, (size_t)M * 12);
+        c.alloc(&d_dbl, (size_t)M * 16);
+        c.to_dev(d_int, feature, (size_t)M * 4);
+        c.to_dev(d_int + M, left, (size_t)M * 4);
+        c.to_dev(d_int + 2 * M, right, (size_t)M * 4);
+        c.to_dev(d_dbl, threshold, (size_t)M * 8);
+        c.to_dev(d_dbl + M, value, (size_t)M * 8);
+    }
+    auto go = [&](auto kernel, auto tag) {
+        using T = decltype(tag);
+        int per_sm = 0;
+        c.run([&] { return cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, lo::kDtThreads, 0); });
+        const int grid = (int)std::min<int64_t>((n + lo::kDtThreads - 1) / lo::kDtThreads,
+                                                (int64_t)ctx->sm_count * std::max(1, per_sm));
+        c.mark();
+        c.launch(1, [&] {
+            kernel<<<grid, lo::kDtThreads, 0, c.s>>>((const T *)x->base, ld, k, n, (const T *)y->base, M, d_int, d_dbl,
+                                                     d_int ? d_int + M : nullptr, d_int ? d_int + 2 * M : nullptr,
+                                                     d_dbl ? d_dbl + M : nullptr, weight, (double *)margin->base,
+                                                     (double *)residual->base, bad.word);
+        });
+        c.mark();
+    };
+    if (x->dtype == LO_F32) go(lo::k_gb_update<float>, 0.0f); else go(lo::k_gb_update<double>, 0.0);
+    bad.read(c);
+    LO_TRY(c.finish(timing));
+    if (!bad.found(k, info)) return LO_OK;
+    return fail(LO_ERR_INVALID, "row %lld: its label is not 0 or 1", (long long)info->bad_row);
+}
+
+int lo_gb_predict(lo_ctx *ctx, const lo_table *x, int64_t ld, int32_t k, int64_t n, int32_t ntrees, const int32_t *start,
+                  const double *weight, int32_t nnodes, const int32_t *feature, const double *threshold,
+                  const int32_t *left, const int32_t *right, const double *value, lo_table *prob, lo_table *raw,
+                  lo_table *pred, const lo_table *y, const double *eval_labels, int32_t neval, int64_t *confusion_out,
+                  lo_nb_info *info, lo_host_timing *timing) {
+    LO_TRY(check_ctx(ctx));
+    if (!info) return fail(LO_ERR_INVALID, "info is NULL");
+    *info = lo_nb_info{-1, -1, 0};
+    const bool eval = confusion_out != nullptr;
+    if (eval && !y) return fail(LO_ERR_INVALID, "evaluate needs y");
+    LO_TRY(check_nb_matrix(ctx, x, ld, k, n, eval ? y : nullptr));
+    const int32_t M = nnodes;
+    if (ntrees < 1 || M < ntrees || !start || !weight || !feature || !threshold || !left || !right || !value)
+        return fail(LO_ERR_INVALID, "a forest of %d trees and %d nodes: start, weight, feature, threshold, left, right and "
+                    "value are needed", ntrees, M);
+    for (int32_t t = 0; t < ntrees; ++t) {
+        const int32_t lo = start[t], hi = t + 1 < ntrees ? start[t + 1] : M;
+        if (t == 0 && lo != 0)
+            return fail(LO_ERR_INVALID, "start[0] = %d: the first tree starts at node 0", lo);
+        if (!(hi > lo && hi <= M)) return fail(LO_ERR_INVALID, "tree %d: nodes [%d, %d) of %d", t, lo, hi, M);
+        LO_TRY(check_tree_nodes(feature, left, right, lo, hi, k));
+        if (!std::isfinite(weight[t])) return fail(LO_ERR_INVALID, "weight[%d] = %g is not finite", t, weight[t]);
+    }
+    int direct = 0;
+    if (eval) {
+        if (prob || raw || pred) return fail(LO_ERR_INVALID, "evaluate writes no rows: prob, raw and pred must be NULL");
+        LO_TRY(check_nb_classes(eval_labels, neval, "eval_labels", &direct));
+        std::fill(confusion_out, confusion_out + (size_t)neval * 2, (int64_t)0);
+    } else {
+        if (y || eval_labels) return fail(LO_ERR_INVALID, "y and eval_labels go with confusion_out");
+        neval = 0;
+        LO_TRY(check_float_table(ctx, prob, LO_F64, n * 2, "prob"));
+        LO_TRY(check_float_table(ctx, pred, LO_F64, n, "pred"));
+        if (raw) LO_TRY(check_float_table(ctx, raw, LO_F64, n * 2, "raw"));
+    }
+    HostCall c(ctx, eval ? "gb_evaluate" : "gb_predict");
+    if (n == 0) return c.finish(timing);
+    const int64_t forest_bytes = ((int64_t)2 * M + ntrees) * 8 + ((int64_t)3 * M + ntrees) * 4;
+    const int64_t evl_bytes = (int64_t)neval * 8, hist_bytes = eval ? (int64_t)neval * 2 * 4 : 0;
+    const bool forest_smem = forest_bytes + evl_bytes <= lo::kDtTreeSmem;
+    const int64_t fixed = (forest_smem ? forest_bytes : 0) + evl_bytes;
+    const bool hist_smem = eval && fixed + hist_bytes <= lo::kDtTreeSmem;
+    const int smem = (int)(fixed + (hist_smem ? hist_bytes : 0));
+    int *d_int = nullptr;
+    double *d_dbl = nullptr, *d_evl = nullptr;
+    unsigned long long *conf = nullptr;
+    RefusedCell bad;
+    c.alloc(&d_int, ((size_t)3 * M + ntrees) * 4);
+    c.alloc(&d_dbl, ((size_t)2 * M + ntrees) * 8);
+    c.to_dev(d_int, feature, (size_t)M * 4);
+    c.to_dev(d_int + M, left, (size_t)M * 4);
+    c.to_dev(d_int + 2 * M, right, (size_t)M * 4);
+    c.to_dev(d_int + 3 * M, start, (size_t)ntrees * 4);
+    c.to_dev(d_dbl, threshold, (size_t)M * 8);
+    c.to_dev(d_dbl + M, value, (size_t)M * 8);
+    c.to_dev(d_dbl + 2 * M, weight, (size_t)ntrees * 8);
+    if (eval) {
+        c.alloc(&d_evl, (size_t)neval * 8);
+        c.alloc(&conf, (size_t)neval * 2 * 8);
+        c.to_dev(d_evl, eval_labels, (size_t)neval * 8);
+        c.memset(conf, 0, (size_t)neval * 2 * 8);
+        bad.arm(c);
+    }
+    auto go = [&](auto kernel, auto tag) {
+        using T = decltype(tag);
+        int per_sm = 0;
+        c.run([&] { return cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem); });
+        c.run([&] { return cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, lo::kDtThreads, smem); });
+        const int grid = (int)std::min<int64_t>((n + lo::kDtThreads - 1) / lo::kDtThreads,
+                                                (int64_t)ctx->sm_count * std::max(1, per_sm));
+        c.mark();
+        c.launch(1, [&] {
+            kernel<<<grid, lo::kDtThreads, smem, c.s>>>((const T *)x->base, ld, k, n, ntrees, M, d_int + 3 * M, d_dbl + 2 * M,
+                                                        d_int, d_dbl, d_int + M, d_int + 2 * M, d_dbl + M,
+                                                        forest_smem ? 1 : 0, prob ? (double *)prob->base : nullptr,
+                                                        raw ? (double *)raw->base : nullptr,
+                                                        pred ? (double *)pred->base : nullptr,
+                                                        y ? (const T *)y->base : nullptr, d_evl, neval, direct, conf,
+                                                        hist_smem ? 1 : 0, bad.word);
+        });
+        c.mark();
+    };
+    if (x->dtype == LO_F32) {
+        if (eval) go(lo::k_gb_predict<float, true>, 0.0f); else go(lo::k_gb_predict<float, false>, 0.0f);
+    } else {
+        if (eval) go(lo::k_gb_predict<double, true>, 0.0); else go(lo::k_gb_predict<double, false>, 0.0);
+    }
+    if (eval) c.to_host(confusion_out, conf, (size_t)neval * 2 * 8);
+    bad.read(c);
+    LO_TRY(c.finish(timing));
+    if (!bad.found(k, info)) return LO_OK;
+    std::fill(confusion_out, confusion_out + (size_t)neval * 2, (int64_t)0);
     return fail(LO_ERR_INVALID, "row %lld: its label is not one of the evaluated labels", (long long)info->bad_row);
 }
 

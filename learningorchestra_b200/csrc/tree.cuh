@@ -1,5 +1,5 @@
-// tree.cuh — Spark 2.4's DecisionTreeClassifier over the feature matrix in HBM (lo_dt_sort, lo_dt_rank, lo_dt_bin,
-// lo_dt_level, lo_dt_predict; DESIGN.md §3.6.4).  Included by loexec.cu after naive_bayes.cuh, whose loads and class
+// tree.cuh — Spark 2.4's DecisionTreeClassifier and GBTClassifier over the feature matrix in HBM (lo_dt_sort,
+// lo_dt_rank, lo_dt_bin, lo_dt_level, lo_dt_predict; lo_gb_level, lo_gb_update, lo_gb_predict; DESIGN.md §3.6.4-5).  Included by loexec.cu after naive_bayes.cuh, whose loads and class
 // lookup it uses.
 //   * k_dt_keys + CUB's radix sort + k_dt_distinct (split candidates): every column as sorted order-preserving codes
 //     (-0.0 as 0.0), its count of distinct values and, when few, those values with their first positions.
@@ -7,8 +7,10 @@
 //   * k_dt_bin: every value's bin, Java's Arrays.binarySearch of its column's thresholds as findBin reads it (without
 //     equal thresholds, the count of thresholds < x), as a byte in an n x kp code matrix.
 //   * k_dt_level: one tree level — routes every row by its node's split and counts (node, feature, bin, class); codes
-//     >= nbins and labels outside [0, C) are refused, never counted.
+//     >= nbins and labels outside [0, C) are refused, never counted.  k_gb_level: the same pass counting GBT's exact
+//     fixed-point residual sums.
 //   * k_dt_predict<T, EVAL>: walks the tree per row; raw = the leaf's class counts, probability = raw / sum.
+//   * k_gb_update<T>: GBT's margins F and residuals r after each tree; k_gb_predict<T, EVAL>: the forest's margin.
 #pragma once
 
 namespace lo {
@@ -236,6 +238,108 @@ __global__ void __launch_bounds__(kDtThreads) k_dt_level(const unsigned char *__
     }
 }
 
+// GBT's regression sums per (node, feature, bin) (DESIGN.md §3.6.5): kGbWords u64 words, the count, Σ(q1 + 2^60) and
+// Σq2 as 128-bit (lo, hi) pairs, with q1 = rint(r 2^58), q2 = rint(fl(r r) 2^58) of the row's residual r.  A 64-bit add
+// carries into the hi word only when the lo word wraps, so every sum is exact in any order of the atomics.
+constexpr int kGbWords = 5;                          // LO_GB_WORDS: count, Σ(q1 + 2^60) lo / hi, Σq2 lo / hi
+
+// a residual's addends: |r| <= 4 (every residual of a fit) keeps q1 + 2^60 in [0, 2^61] and q2 in [0, 2^62]; NaN or
+// anything larger is refused (false)
+__device__ __forceinline__ bool gb_addends(double r, unsigned long long &q1, unsigned long long &q2) {
+    if (!(fabs(r) <= 4.0)) return false;
+    q1 = (unsigned long long)(__double2ll_rn(r * 0x1p58) + (1ll << 60));
+    q2 = (unsigned long long)__double2ll_rn(__dmul_rn(r, r) * 0x1p58);
+    return true;
+}
+__device__ __forceinline__ void add128(unsigned long long *lo, unsigned long long v) {
+    const unsigned long long old = atomicAdd(lo, v);
+    if (old + v < old) atomicAdd(lo + 1, 1ull);
+}
+// one row into a bin's words h (shared memory)
+__device__ __forceinline__ void gb_add(unsigned long long *h, unsigned long long q1, unsigned long long q2) {
+    atomicAdd(h, 1ull);
+    add128(h + 1, q1);
+    add128(h + 3, q2);
+}
+// a bin's words h (shared memory) into out (global memory), each 128-bit pair with the lo word's carry
+__device__ __forceinline__ void gb_flush(unsigned long long *out, const unsigned long long *h) {
+    atomicAdd(out, h[0]);
+    for (int p = 1; p < kGbWords; p += 2) {
+        const unsigned long long old = atomicAdd(out + p, h[p]);
+        atomicAdd(out + p + 1, h[p + 1] + (old + h[p] < old ? 1ull : 0ull));
+    }
+}
+
+// k_dt_level's pass counting GBT's sums: the same routing, refusals, launch shape and 16-byte code loads (DecisionTree
+// keeps its own kernel, which stays as it was).  A row whose slot lies in the pass's node group adds its count and
+// sums to hist[slot - g0][f][code][kGbWords] for each feature f of the CTA's chunk: u64 words in shared memory,
+// flushed once per CTA into out ([gn][k][nbins][kGbWords]).  A code >= nbins or a refused residual (gb_addends) is
+// never counted: the lowest such cell's key (cell_key; col k: the residual) goes to *err.  VEC does not unroll the 16
+// codes of a 16-byte load: unrolled, the carry branches keep convergence state on the stack.
+template <bool VEC>
+__global__ void __launch_bounds__(kDtThreads) k_gb_level(const unsigned char *__restrict__ codes, long long kp, int k,
+                                                         const double *__restrict__ res, long long n, int nbins,
+                                                         const int *__restrict__ src, int route, int *__restrict__ dst,
+                                                         const int *__restrict__ sfeat, const int *__restrict__ sbin,
+                                                         const int *__restrict__ left, const int *__restrict__ right,
+                                                         int g0, int gn, int fc, unsigned long long *__restrict__ out,
+                                                         unsigned long long *__restrict__ err) {
+    extern __shared__ unsigned long long gb_hist[];
+    const int cell = nbins * kGbWords, j0 = blockIdx.y * fc, fw = min(fc, k - j0);
+    const int cells = gn * fc * cell;
+    for (int i = threadIdx.x; i < cells; i += kDtThreads) gb_hist[i] = 0;
+    __syncthreads();
+    const uint64_t pol = l2_evict_first_policy();
+    const bool write = dst != nullptr && blockIdx.y == 0;
+    unsigned long long bad = ~0ull;
+    for (long long r = blockIdx.x * (long long)kDtThreads + threadIdx.x; r < n; r += (long long)gridDim.x * kDtThreads) {
+        const unsigned char *row = codes + r * kp;
+        int s = 0;
+        if (src) {
+            s = src[r];
+            if (route && s >= 0) {
+                const int f = sfeat[s];
+                s = f < 0 ? -1 : (int)row[f] <= sbin[s] ? left[s] : right[s];
+            }
+        }
+        if (write) dst[r] = s;
+        if (s < g0 || s >= g0 + gn) continue;
+        unsigned long long q1, q2;
+        if (!gb_addends(res[r], q1, q2)) {                 // refused: never counted
+            bad = min(bad, cell_key(r, k, k));
+            continue;
+        }
+        unsigned long long *h = gb_hist + (size_t)(s - g0) * fc * cell;
+        if constexpr (VEC) {
+            for (int q = 0; q < fw; q += kDtVec) {
+                unsigned long long a, b;
+                ldg_v2u64_stream(row + j0 + q, pol, a, b);
+#pragma unroll 1
+                for (int w = 0; w < kDtVec; ++w) {
+                    if (q + w >= fw) break;
+                    const unsigned code = (unsigned)((w < 8 ? a >> (8 * w) : b >> (8 * (w - 8))) & 0xff);
+                    if (code >= (unsigned)nbins) bad = min(bad, cell_key(r, k, j0 + q + w));
+                    else gb_add(&h[(size_t)(q + w) * cell + code * kGbWords], q1, q2);
+                }
+            }
+        } else {
+            for (int w = 0; w < fw; ++w) {
+                const unsigned code = row[j0 + w];
+                if (code >= (unsigned)nbins) bad = min(bad, cell_key(r, k, j0 + w));
+                else gb_add(&h[(size_t)w * cell + code * kGbWords], q1, q2);
+            }
+        }
+    }
+    report_cell(bad, err);
+    __syncthreads();
+    for (int i = threadIdx.x * kGbWords; i < cells; i += kDtThreads * kGbWords) {
+        if (!gb_hist[i]) continue;
+        const int g = i / (fc * cell), rest = i - g * fc * cell, f = rest / cell;
+        if (f >= fw) continue;
+        gb_flush(&out[((size_t)g * k + j0 + f) * cell + (rest - f * cell)], gb_hist + i);
+    }
+}
+
 // Transform / evaluate.  One row per thread: from node 0, an internal node (feat >= 0) sends the row left when its value
 // widened to f64 is <= the node's threshold.  The leaf's class counts (counts[node * C ..]) are the raw values, the
 // probabilities raw_c / sum (IEEE division, sum in c order) and the prediction their first argmax.  The tree's
@@ -310,6 +414,121 @@ __global__ void __launch_bounds__(kDtThreads) k_dt_predict(const T *__restrict__
         if (hist_in_smem) {
             __syncthreads();
             for (int i = threadIdx.x; i < neval * C; i += kDtThreads)
+                if (hist[i]) atomicAdd(&confusion[i], (unsigned long long)hist[i]);
+        }
+    }
+}
+
+// GBT's pass after each tree (DESIGN.md §3.6.5), one row per thread.  M == 0 initialises: F = 0, r = y' = 2y - 1.
+// Else the row walks the tree (as k_dt_predict, on its raw values), F += value[leaf] * weight and r = -LogLoss.gradient
+// = 4y' / (1 + exp(2y' F)), each operation rounded on its own (no fused multiply-add).  A label other than 0 or 1 is
+// refused (cell_key(row, k, k) to *err) and its row left as it was.
+template <typename T>
+__global__ void __launch_bounds__(kDtThreads) k_gb_update(const T *__restrict__ x, long long ld, int k, long long n,
+                                                          const T *__restrict__ y, int M, const int *__restrict__ feat,
+                                                          const double *__restrict__ thr, const int *__restrict__ left,
+                                                          const int *__restrict__ right, const double *__restrict__ value,
+                                                          double weight, double *__restrict__ F, double *__restrict__ res,
+                                                          unsigned long long *__restrict__ err) {
+    unsigned long long bad = ~0ull;
+    for (long long r = blockIdx.x * (long long)kDtThreads + threadIdx.x; r < n; r += (long long)gridDim.x * kDtThreads) {
+        const double lab = (double)y[r];
+        if (!(lab == 0.0 || lab == 1.0)) {
+            bad = min(bad, cell_key(r, k, k));
+            continue;
+        }
+        const double yp = lab == 1.0 ? 1.0 : -1.0;
+        if (M == 0) {
+            F[r] = 0.0;
+            res[r] = yp;
+            continue;
+        }
+        int node = 0, f;
+        while ((f = feat[node]) >= 0) node = (double)x[r * ld + f] <= thr[node] ? left[node] : right[node];
+        const double m = __dadd_rn(F[r], __dmul_rn(value[node], weight));
+        F[r] = m;
+        res[r] = __ddiv_rn(4.0 * yp, __dadd_rn(1.0, exp(__dmul_rn(2.0 * yp, m))));
+    }
+    report_cell(bad, err);
+}
+
+// GBT transform / evaluate, one row per thread: the margin m = sum over trees t (in order, from 0.0) of value[leaf_t] *
+// weight[t], tree t's nodes from start[t] (children as indices into the whole forest).  raw = [-m, m], probability[0]
+// = 1 / (1 + exp(2m)), probability[1] = 1 - probability[0], prediction = m > 0.  The forest sits in shared memory when
+// `forest_smem` (else it is read from global memory).  EVAL: nothing per row; (label slot, prediction) counts, as
+// k_dt_predict counts them.
+template <typename T, bool EVAL>
+__global__ void __launch_bounds__(kDtThreads) k_gb_predict(const T *__restrict__ x, long long ld, int k, long long n,
+                                                           int ntrees, int M, const int *__restrict__ start,
+                                                           const double *__restrict__ weight, const int *__restrict__ feat,
+                                                           const double *__restrict__ thr, const int *__restrict__ left,
+                                                           const int *__restrict__ right, const double *__restrict__ value,
+                                                           int forest_smem, double *__restrict__ prob,
+                                                           double *__restrict__ raw_out, double *__restrict__ pred,
+                                                           const T *__restrict__ y, const double *__restrict__ eval_labels,
+                                                           int neval, int direct, unsigned long long *__restrict__ confusion,
+                                                           int hist_in_smem, unsigned long long *__restrict__ err) {
+    extern __shared__ double dt_smem[];
+    const double *th = thr, *va = value, *wt = weight;
+    const int *fe = feat, *le = left, *ri = right, *st = start;
+    double *evl = dt_smem;
+    unsigned *hist_at = reinterpret_cast<unsigned *>(dt_smem + neval);
+    if (forest_smem) {
+        double *ts = dt_smem, *vs = ts + M, *ws = vs + M;
+        evl = ws + ntrees;
+        int *fs = reinterpret_cast<int *>(evl + neval), *ls = fs + M, *rs = ls + M, *ss = rs + M;
+        for (int i = threadIdx.x; i < M; i += kDtThreads) {
+            ts[i] = thr[i];
+            vs[i] = value[i];
+            fs[i] = feat[i];
+            ls[i] = left[i];
+            rs[i] = right[i];
+        }
+        for (int i = threadIdx.x; i < ntrees; i += kDtThreads) {
+            ws[i] = weight[i];
+            ss[i] = start[i];
+        }
+        th = ts, va = vs, wt = ws, fe = fs, le = ls, ri = rs, st = ss;
+        hist_at = reinterpret_cast<unsigned *>(ss + ntrees);
+    }
+    unsigned *hist = nullptr;
+    if (EVAL) {
+        hist = hist_at;
+        for (int i = threadIdx.x; i < neval; i += kDtThreads) evl[i] = eval_labels[i];
+        if (hist_in_smem)
+            for (int i = threadIdx.x; i < neval * 2; i += kDtThreads) hist[i] = 0;
+    }
+    __syncthreads();
+    unsigned long long bad = ~0ull;
+    for (long long r = blockIdx.x * (long long)kDtThreads + threadIdx.x; r < n; r += (long long)gridDim.x * kDtThreads) {
+        double m = 0.0;
+        for (int t = 0; t < ntrees; ++t) {
+            int node = st[t], f;
+            while ((f = fe[node]) >= 0) node = (double)x[r * ld + f] <= th[node] ? le[node] : ri[node];
+            m = __dadd_rn(m, __dmul_rn(va[node], wt[t]));
+        }
+        const int best = m > 0.0 ? 1 : 0;
+        if (!EVAL) {
+            const double p0 = __ddiv_rn(1.0, __dadd_rn(1.0, exp(__dmul_rn(2.0, m))));
+            __stcs(prob + 2 * r, p0);
+            __stcs(prob + 2 * r + 1, __dsub_rn(1.0, p0));
+            if (raw_out) {
+                __stcs(raw_out + 2 * r, -m);
+                __stcs(raw_out + 2 * r + 1, m);
+            }
+            __stcs(pred + r, (double)best);
+        } else {
+            const int a = nb_class((double)y[r], evl, neval, direct);
+            if (a < 0) bad = min(bad, cell_key(r, k, k));
+            else if (hist_in_smem) atomicAdd(&hist[a * 2 + best], 1u);
+            else atomicAdd(&confusion[(size_t)a * 2 + best], 1ull);
+        }
+    }
+    if (EVAL) {
+        report_cell(bad, err);
+        if (hist_in_smem) {
+            __syncthreads();
+            for (int i = threadIdx.x; i < neval * 2; i += kDtThreads)
                 if (hist[i]) atomicAdd(&confusion[i], (unsigned long long)hist[i]);
         }
     }

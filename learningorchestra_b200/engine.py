@@ -314,6 +314,7 @@ _NB_FEATURE_REFUSED = "row {row}, feature {position}: negative or NaN (NaiveBaye
 _FIT_REFUSED = (_NB_FEATURE_REFUSED, "row {row}: its label is not one of the classes")
 _EVALUATE_REFUSED = (_NB_FEATURE_REFUSED, "row {row}: its label is not one of the evaluated labels")
 _LR_STATS_REFUSED = ("row {row}, feature {position}: NaN or infinite", "row {row}: its label is not an integer >= 0")
+_GB_REFUSED = (_NB_FEATURE_REFUSED, "row {row}: its label is not 0 or 1")
 
 
 def _check_cells(rc: int, info, k: int, reasons: tuple[str, str]) -> None:
@@ -426,6 +427,39 @@ class BinnedRows:
     def free(self) -> None:
         for t in [self.codes, *self.slots]:
             t.free()
+
+
+class BoostRows:
+    """What :meth:`Engine.gb_update` keeps for one device's rows during a GBT fit: ``margin`` (F) and ``residual`` (r),
+    two LO_F64 tables of n.  :meth:`free` frees them and may be called again."""
+
+    def __init__(self, margin: "DeviceTable", residual: "DeviceTable"):
+        self.margin, self.residual = margin, residual
+
+    def free(self) -> None:
+        for t in (self.margin, self.residual):
+            t.free()
+
+
+def _tree_args(tree):
+    """(feature int32, threshold f64, left int32, right int32, prediction f64) of a regression tree, contiguous."""
+    return [np.ascontiguousarray(a, dt) for a, dt in ((tree.feature, np.int32), (tree.threshold, np.float64),
+                                                      (tree.left, np.int32), (tree.right, np.int32),
+                                                      (tree.prediction, np.float64))]
+
+
+def forest_arrays(trees):
+    """The forest of lo_gb_predict: (start int32[ntrees], nodes, feature, threshold, left, right, value) with every
+    tree's children shifted to indices into the concatenation."""
+    start, at, cols = [], 0, [[] for _ in range(5)]
+    for t in trees:
+        start.append(at)
+        f, th, le, ri, v = _tree_args(t)
+        for c, a in zip(cols, (f, th, np.where(le >= 0, le + at, -1), np.where(ri >= 0, ri + at, -1), v)):
+            c.append(a)
+        at += t.num_nodes
+    dts = (np.int32, np.float64, np.int32, np.int32, np.float64)
+    return (np.array(start, np.int32), at, *[np.ascontiguousarray(np.concatenate(c), dt) for c, dt in zip(cols, dts)])
 
 
 def code_pitch(k: int) -> int:
@@ -1251,6 +1285,82 @@ class Engine:
                                             None, C.byref(info), C.byref(t)))
         _report(timing, t)
         return PredictedRows(prob, rawt, pred, n, C_)
+
+    def gb_update(self, part: AssembledRows, rows: "BoostRows | None" = None, tree=None, weight: float = 1.0,
+                  timing: dict | None = None) -> "BoostRows":
+        """GBT's margins and residuals over ``part`` (``lo_gb_update``).  ``tree`` None: a new :class:`BoostRows` with F =
+        0 and r = 2y - 1; else ``rows`` after the regression tree (:class:`~tree.Tree`) of weight ``weight``: F +=
+        prediction * weight, r = 4y' / (1 + exp(2y'F)).  A label other than 0 or 1 raises :class:`InvalidCellError`
+        (``position`` k)."""
+        if part.y is None:
+            raise ValueError("the rows have no label")
+        n = part.nkept
+        info, t = N.NbInfo(), N.HostTiming()
+        with _Owned() as owned:
+            if rows is None:
+                rows = BoostRows(owned.own(self.table("f64", max(n, 1), 1)), owned.own(self.table("f64", max(n, 1), 1)))
+            arrs = _tree_args(tree) if tree is not None else []
+            ptrs = [a.ctypes.data_as(C.c_void_p) for a in arrs] or [None] * 5
+            rc = self._lib.lo_gb_update(self._ctx, part.x._h, part.k, part.k, part.y._h, n,
+                                        tree.num_nodes if tree is not None else 0, *ptrs, float(weight),
+                                        rows.margin._h, rows.residual._h, C.byref(info), C.byref(t))
+            _check_cells(rc, info, part.k, _GB_REFUSED)
+        _report(timing, t)
+        return rows
+
+    def gb_level(self, part: AssembledRows, binned: "BinnedRows", rows: "BoostRows", nbins: int, splits, nnodes: int,
+                 shape: list | None = None, timing: dict | None = None) -> np.ndarray:
+        """One regression-tree level over ``part``'s rows (``lo_gb_level``), routed as :meth:`dt_level`: uint64 (nnodes, k,
+        nbins, LO_GB_WORDS) words of (node slot, feature, bin) — the count and the 128-bit fixed-point sums of the rows'
+        residuals and their squares (:func:`tree.word_stats` reads them)."""
+        k = part.k
+        words = np.zeros((nnodes, k, nbins, N.LO_GB_WORDS), np.uint64)
+        sp = np.ascontiguousarray(splits if splits is not None else np.zeros((0, 4)), np.int32)
+        src = None if splits is None else binned.slots[binned.cur]
+        dst = binned.slots[0 if splits is None else 1 - binned.cur]
+        sh = np.zeros(4, np.int32)
+        t = N.HostTiming()
+        N.check(self._lib.lo_gb_level(self._ctx, binned.codes._h, code_pitch(k), k, rows.residual._h, part.nkept,
+                                      int(nbins), src._h if src is not None else None, int(splits is not None),
+                                      dst._h, len(sp), sp.ctypes.data_as(C.c_void_p), int(nnodes),
+                                      words.ctypes.data_as(C.c_void_p), sh.ctypes.data_as(C.c_void_p), C.byref(t)))
+        binned.cur = binned.slots.index(dst)
+        if shape is not None:
+            shape[:] = [int(v) for v in sh]
+        _report(timing, t)
+        return words
+
+    def gb_predict(self, part: AssembledRows, trees, weights, raw: bool = False, labels=None,
+                   timing: dict | None = None):
+        """A GBT forest (regression :class:`~tree.Tree` s and their weights) over ``part`` (``lo_gb_predict``), as
+        :meth:`nb_predict` with two classes: ``labels`` None gives a :class:`PredictedRows`, else the int64[len(labels),
+        2] confusion counts."""
+        start, M, *arrs = forest_arrays(trees)
+        w = np.ascontiguousarray(weights, np.float64)
+        if len(w) != len(trees):
+            raise ValueError(f"{len(w)} weights for {len(trees)} trees")
+        n = part.nkept
+        info, t = N.NbInfo(), N.HostTiming()
+        args = (self._ctx, part.x._h, part.k, part.k, n, len(trees), start.ctypes.data_as(C.c_void_p),
+                w.ctypes.data_as(C.c_void_p), M, *[a.ctypes.data_as(C.c_void_p) for a in arrs])
+        if labels is not None:
+            if part.y is None:
+                raise ValueError("the rows have no label")
+            lab = np.ascontiguousarray(labels, dtype=np.float64)
+            conf = np.zeros((len(lab), 2), np.int64)
+            rc = self._lib.lo_gb_predict(*args, None, None, None, part.y._h, lab.ctypes.data_as(C.c_void_p), len(lab),
+                                         conf.ctypes.data_as(C.c_void_p), C.byref(info), C.byref(t))
+            _check_cells(rc, info, part.k, _EVALUATE_REFUSED)
+            _report(timing, t)
+            return conf
+        with _Owned() as owned:
+            prob = owned.own(self.table("f64", max(n * 2, 1), 1))
+            pred = owned.own(self.table("f64", max(n, 1), 1))
+            rawt = owned.own(self.table("f64", max(n * 2, 1), 1) if raw else None)
+            N.check(self._lib.lo_gb_predict(*args, prob._h, rawt._h if rawt is not None else None, pred._h, None, None, 0,
+                                            None, C.byref(info), C.byref(t)))
+        _report(timing, t)
+        return PredictedRows(prob, rawt, pred, n, 2)
 
     def value_counts_f64_host(self, values: np.ndarray):
         """(keys float64[g], counts uint64[g]) — exact value counts of a numeric column (GPU hash group-by),

@@ -864,6 +864,39 @@ class ShardedEngine:
             confusion = confusion + c
         return confusion
 
+    def gb_update(self, parts, rows: list | None = None, tree=None, weight: float = 1.0) -> list:
+        """``Engine.gb_update`` on every member: one ``BoostRows`` per member (made when ``rows`` is None); a refused
+        label is raised as the lowest over all shards, its row global."""
+        return self._each("gb_update", lambda i: self.engines[i].gb_update(parts[i], rows[i] if rows else None, tree,
+                                                                           weight),
+                          undo=(lambda b: b.free()) if rows is None else None, first_rows=_firsts(parts))
+
+    def gb_level(self, parts, binned: list, rows: list, nbins: int, splits, nnodes: int, shape: list | None = None):
+        """``Engine.gb_level`` on every member over the same splits; the 128-bit words added as integers in shard order
+        (:func:`tree.add_words`), so they do not depend on the cut.  ``shape`` receives the first member's launch shape."""
+        from .tree import add_words
+        shapes = [[] for _ in parts]
+        got = self._each("gb_level", lambda i: self.engines[i].gb_level(parts[i], binned[i], rows[i], nbins, splits,
+                                                                        nnodes, shapes[i]))
+        if shape is not None:
+            shape[:] = shapes[0]
+        words = got[0]
+        for w in got[1:]:
+            words = add_words(words, w)
+        return words
+
+    def gb_predict(self, parts, trees, weights, raw: bool = False, labels=None):
+        """``Engine.gb_predict`` over the shards, as :meth:`nb_predict`: one ``PredictedRows`` per member, or the
+        members' confusion counts summed; a refused row is raised as the lowest over all shards, its row global."""
+        got = self._each("gb_predict", lambda i: self.engines[i].gb_predict(parts[i], trees, weights, raw, labels),
+                         undo=(lambda p: p.free()) if labels is None else None, first_rows=_firsts(parts))
+        if labels is None:
+            return got
+        confusion = got[0]
+        for c in got[1:]:
+            confusion = confusion + c
+        return confusion
+
     @property
     def resident(self):
         """Datasets kept in HBM between requests, rows sharded over the group (:mod:`table_cache`)."""

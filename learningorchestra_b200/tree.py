@@ -14,6 +14,8 @@ MAX_CLASSES = 100           # Spark's Classifier.getNumClasses maxNumClasses
 EPSILON = 2.220446049250313e-16     # Spark's Utils.EPSILON: 2^-52
 DOUBLE_MIN = -np.finfo(np.float64).max   # Scala's Double.MinValue: the gain of an invalid split
 IMPURITIES = ("gini", "entropy")
+VARIANCE = "variance"       # GBT's regression trees (DESIGN.md §3.6.5): the level gives lo_gb_level's words
+WORDS = 5                   # LO_GB_WORDS: count, sum of q1 + 2^60 (lo, hi), sum of q2 (lo, hi) per (node, feature, bin)
 
 
 def num_splits(max_bins: int, n: int) -> int:
@@ -239,9 +241,15 @@ def best_splits(hist: np.ndarray, nthr: np.ndarray, kind: str, min_instances: in
     right = total[:, None, None, :] - left
     lc = left.sum(axis=3).astype(np.float64)
     rc = right.sum(axis=3).astype(np.float64)
+    return _choose(out, node_imp, left, right, lc, rc, impurity(left, lc, kind), impurity(right, rc, kind), nthr,
+                   min_instances, min_info_gain)
+
+
+def _choose(out, node_imp, left, right, lc, rc, limp, rimp, nthr, min_instances, min_info_gain):
+    """binsToBestSplit's choice from every candidate's (nodes, k, ns) counts lc / rc and impurities limp / rimp:
+    calculateImpurityStats' gain, the minInstancesPerNode and minInfoGain rules and the first maximum."""
+    nodes, k, ns = lc.shape
     tc = lc + rc
-    limp = impurity(left, lc, kind)
-    rimp = impurity(right, rc, kind)
     with np.errstate(invalid="ignore", divide="ignore"):
         wl = lc / tc
         wr = rc / tc
@@ -261,6 +269,56 @@ def best_splits(hist: np.ndarray, nthr: np.ndarray, kind: str, min_instances: in
     return out
 
 
+def add_words(a: np.ndarray, b: np.ndarray) -> np.ndarray:
+    """Two uint64 arrays of lo_gb_level's words (..., WORDS) added as integers: the counts, and each 128-bit (lo, hi)
+    sum with the lo word's carry into the hi word — exact, so shards add in any order to the same words."""
+    a, b = np.asarray(a, np.uint64), np.asarray(b, np.uint64)
+    out = a + b
+    for p in (1, 3):
+        out[..., p + 1] += (out[..., p] < a[..., p]).astype(np.uint64)
+    return out
+
+
+def word_stats(words: np.ndarray, nsplits: int):
+    """(left, right, total) f64 statistics (count, sum, sumsq) of lo_gb_level's words (nodes, k, nbins, WORDS):
+    lo_gb_stats' integer prefix over the bins, right = total - left, each statistic rounded to f64 once."""
+    import ctypes as C
+    from . import _native as N
+    words = np.ascontiguousarray(words, np.uint64)
+    nodes, k, nbins, _w = words.shape
+    left = np.zeros((nodes, k, nsplits, 3))
+    right = np.zeros((nodes, k, nsplits, 3))
+    total = np.zeros((nodes, 3))
+    N.check(N.load().lo_gb_stats(words.ctypes.data_as(C.c_void_p), nodes, k, nbins, nsplits,
+                                 left.ctypes.data_as(C.c_void_p), right.ctypes.data_as(C.c_void_p),
+                                 total.ctypes.data_as(C.c_void_p)))
+    return left, right, total
+
+
+def variance(stats: np.ndarray) -> np.ndarray:
+    """Spark's Variance.calculate of (..., 3) statistics (count, sum, sumSq): 0 where count == 0, else
+    (sumSq - sum * sum / count) / count."""
+    cnt, s, sq = stats[..., 0], stats[..., 1], stats[..., 2]
+    safe = np.where(cnt == 0, 1.0, cnt)
+    return np.where(cnt == 0, 0.0, (sq - s * s / safe) / safe)
+
+
+def variance_splits(words: np.ndarray, nthr: np.ndarray, min_instances: int, min_info_gain: float):
+    """:func:`best_splits` for regression trees from lo_gb_level's words: ``total`` / ``left`` / ``right`` are the
+    (count, sum, sumSq) statistics and the impurities Variance's."""
+    nodes, k = words.shape[:2]
+    ns = max(int(nthr.max()) if k else 0, 0)
+    left, right, total = word_stats(words, ns)
+    out = {"total": total, "impurity": variance(total)}
+    if ns == 0:
+        out.update(feature=np.full(nodes, -1), bin=np.zeros(nodes, np.int64), gain=np.full(nodes, DOUBLE_MIN),
+                   valid=np.zeros(nodes, bool), left=np.zeros_like(total), right=np.zeros_like(total),
+                   left_impurity=np.zeros(nodes), right_impurity=np.zeros(nodes))
+        return out
+    return _choose(out, out["impurity"], left, right, left[..., 0], right[..., 0], variance(left), variance(right), nthr,
+                   min_instances, min_info_gain)
+
+
 class Tree:
     """A fitted tree in arrays, node 0 the root, children after their parent: ``feature`` (int32, -1 for a leaf),
     ``threshold`` and ``bin`` (the split: left when x <= threshold, i.e. code <= bin), ``left`` / ``right`` (int32, -1
@@ -272,11 +330,14 @@ class Tree:
         self.threshold = np.asarray(threshold, np.float64)
         self.left = np.asarray(left, np.int32)
         self.right = np.asarray(right, np.int32)
-        self.counts = np.asarray(counts, np.float64).reshape(len(self.feature), num_classes)
+        self.counts = np.asarray(counts, np.float64).reshape(len(self.feature), num_classes or 3)
         self.impurity = np.asarray(impurity_, np.float64)
         self.gain = np.asarray(gain, np.float64)
         self.num_classes = int(num_classes)
         self.prediction = self.counts.argmax(axis=1).astype(np.float64) if len(self.feature) else np.zeros(0)
+        if num_classes == 0:                 # a regression tree: counts are (count, sum, sumSq), prediction sum / count
+            with np.errstate(invalid="ignore", divide="ignore"):
+                self.prediction = self.counts[:, 1] / self.counts[:, 0]
 
     @property
     def num_nodes(self) -> int:
@@ -295,7 +356,9 @@ def grow(level, thresholds, num_classes: int, max_depth: int, kind: str, min_ins
     """Spark's level-wise growth and toNode(prune = true).  ``level(splits, nnodes) -> hist`` counts one level: splits
     None for the root, else int32 (parents, 4) rows (feature, bin, left slot, right slot) of the previous level's nodes
     in slot order (feature -1: the node did not split; slot -1: a leaf child); hist int64 (nnodes, k, nbins, C).
-    Returns a :class:`Tree` and the per-level histograms' node counts."""
+    ``kind`` VARIANCE grows a regression tree (num_classes 0): hist is lo_gb_level's uint64 words (nnodes, k, nbins,
+    WORDS) and a node's counts its (count, sum, sumSq).  Returns a :class:`Tree` and the per-level histograms' node
+    counts."""
     nthr = np.array([len(t) for t in thresholds], np.int64)
     # learning nodes: dict(depth, stats: counts / impurity / gain / valid, split, children, leaf)
     nodes = [dict(depth=0, counts=None, impurity=None, gain=np.nan, valid=True, split=None, kids=None)]
@@ -305,7 +368,10 @@ def grow(level, thresholds, num_classes: int, max_depth: int, kind: str, min_ins
     while active:
         hist = level(splits, len(active))
         shapes.append(len(active))
-        best = best_splits(hist, nthr, kind, min_instances, min_info_gain)
+        if kind == VARIANCE:
+            best = variance_splits(hist, nthr, min_instances, min_info_gain)
+        else:
+            best = best_splits(hist, nthr, kind, min_instances, min_info_gain)
         nxt, rows = [], []
         for s, idx in enumerate(active):
             node = nodes[idx]
@@ -341,9 +407,12 @@ def grow(level, thresholds, num_classes: int, max_depth: int, kind: str, min_ins
 
 
 def _to_tree(nodes, num_classes: int) -> Tree:
-    """toNode(prune = true) into breadth-first arrays: two leaf children of equal prediction merge into a leaf with the
-    parent's impurity and counts (bottom-up, so merges cascade); an invalid split search leaves impurity -1."""
+    """toNode(prune = true) into breadth-first arrays: two leaf children of equal prediction (the first argmax of the
+    counts; a regression tree's sum / count, as f64) merge into a leaf with the parent's impurity and counts (bottom-up,
+    so merges cascade); an invalid split search leaves impurity -1."""
     def prediction(counts):
+        if num_classes == 0:
+            return float(counts[1] / counts[0])
         return int(np.argmax(counts))
 
     def build(i):
@@ -372,4 +441,4 @@ def _to_tree(nodes, num_classes: int) -> Tree:
         base = at + 1 + len(queue)
         left.append(base), right.append(base + 1)
         queue += [nd[5], nd[6]]
-    return Tree(feature, threshold, left, right, np.array(counts).reshape(-1, num_classes), imps, gains, num_classes)
+    return Tree(feature, threshold, left, right, np.array(counts).reshape(-1, num_classes or 3), imps, gains, num_classes)

@@ -47,6 +47,15 @@ dt_race_log="$(mktemp -d)/sanitizer_racecheck_tree.txt"
 timeout 1800 compute-sanitizer --tool racecheck --error-exitcode 1 python -m pytest tests/test_gpu_tree.py -q \
     -k "route or edges" > "$dt_race_log" 2>&1
 echo "racecheck (tree) rc=$? log=$dt_race_log"; tail -3 "$dt_race_log"
+# memcheck and racecheck of the GBT kernels (every level route with 128-bit sums, update, predict, evaluate; the edges and
+# refusals); their logs go to a temporary directory
+gb_log="$(mktemp -d)/sanitizer_memcheck_gbt.txt"
+timeout 1800 compute-sanitizer --tool memcheck --error-exitcode 1 python -m pytest tests/test_gpu_gbt.py -q > "$gb_log" 2>&1
+echo "memcheck (gbt) rc=$? log=$gb_log"; tail -3 "$gb_log"
+gb_race_log="$(mktemp -d)/sanitizer_racecheck_gbt.txt"
+timeout 1800 compute-sanitizer --tool racecheck --error-exitcode 1 python -m pytest tests/test_gpu_gbt.py -q \
+    -k "route or edges" > "$gb_race_log" 2>&1
+echo "racecheck (gbt) rc=$? log=$gb_race_log"; tail -3 "$gb_race_log"
 # memcheck of the number parser and the resident formatter on every entry point, without the million-row cases: a read
 # past the last staged cell shows here (the CPU harness puts a NUL after it)
 parse_log="$(mktemp -d)/sanitizer_memcheck_parse.txt"
