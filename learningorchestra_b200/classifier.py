@@ -48,11 +48,28 @@ def _usable(features) -> None:
         raise ValueError("the features have been released")
 
 
-def _labels(features, name: str = "NaiveBayes", reasons: tuple[str, str] = _NB_REASONS) -> np.ndarray:
-    """The distinct label values of the features' rows, ascending (every shard's union)."""
+def _labelled(features, name: str) -> None:
+    """The fits' preamble: refuses released features, and features without a label."""
     _usable(features)
     if features.label is None:
         raise ValueError(f"{name} needs features with a label")
+
+
+def _some_rows(n: int, name: str) -> None:
+    """Refuses a call ``name`` over no row."""
+    if n == 0:
+        raise N.LoexecError(N.LO_ERR_INVALID, f"{name} needs at least one row")
+
+
+def _free(held) -> None:
+    """Frees device results: a list of them (one per shard), one, or None."""
+    for h in held if isinstance(held, list) else [] if held is None else [held]:
+        h.free()
+
+
+def _labels(features, name: str = "NaiveBayes", reasons: tuple[str, str] = _NB_REASONS) -> np.ndarray:
+    """The distinct label values of the features' rows, ascending (every shard's union)."""
+    _labelled(features, name)
     return _on_device(features, lambda engine, rows: engine.nb_labels(rows), name=name, reasons=reasons)
 
 
@@ -86,8 +103,7 @@ class NaiveBayes:
         LO_NB_MAX_THETA or no row at all are refused, and so is a negative or NaN feature (InvalidCellError naming the
         ``_id`` and field of the lowest such row)."""
         classes = _labels(features)
-        if len(features.row_ids) == 0:
-            raise N.LoexecError(N.LO_ERR_INVALID, "NaiveBayes needs at least one row")
+        _some_rows(len(features.row_ids), "NaiveBayes")
         k = len(features.fields)
         if len(classes) * k > N.LO_NB_MAX_THETA:
             raise N.LoexecError(N.LO_ERR_INVALID, f"{len(classes)} classes x {k} features exceed LO_NB_MAX_THETA = "
@@ -97,14 +113,11 @@ class NaiveBayes:
         return NaiveBayesModel(classes, pi, theta, features.fields, sums, counts)
 
 
-class NaiveBayesModel:
-    """A fitted multinomial NaiveBayes model, host data: ``labels`` (float64[C], the class values ascending), ``pi``
-    (float64[C]), ``theta`` (float64[C, k]) and the ``fields`` it was fitted on; ``sums`` / ``counts`` are the device's
-    per-class feature sums and row counts it was made from."""
-
-    def __init__(self, labels, pi, theta, fields, sums=None, counts=None):
-        self.labels, self.pi, self.theta = np.asarray(labels, np.float64), np.asarray(pi, np.float64), np.asarray(theta, np.float64)
-        self.fields, self.sums, self.counts = list(fields), sums, counts
+class _Model:
+    """What every fitted classifier shares: the ``fields`` it was fitted on, ``transform`` and ``evaluate``.  A model
+    states ``_name`` and ``_reasons`` (the words of a refused cell, see :func:`_on_device`) and supplies
+    ``_predict(engine, rows, raw, labels)``, its engine's ``*_predict`` call."""
+    _name, _reasons = "NaiveBayes", _NB_REASONS
 
     def _check(self, features) -> None:
         if list(features.fields) != self.fields:
@@ -115,8 +128,8 @@ class NaiveBayesModel:
         with ``raw`` its ``rawPrediction``, written in HBM on the rows' own devices."""
         _usable(features)
         self._check(features)
-        parts = _on_device(features, lambda engine, rows: engine.nb_predict(rows, self.pi, self.theta, raw=raw),
-                           per_part=True)
+        parts = _on_device(features, lambda engine, rows: self._predict(engine, rows, raw=raw), per_part=True,
+                           name=self._name, reasons=self._reasons)
         return Predictions(features, parts)
 
     def evaluate(self, features) -> dict:
@@ -125,12 +138,25 @@ class NaiveBayesModel:
         ``confusion[a, p]`` counts the rows labelled ``labels[a]`` predicted as class index p."""
         _usable(features)
         self._check(features)
-        labels = _labels(features)
-        if len(features.row_ids) == 0:
-            raise N.LoexecError(N.LO_ERR_INVALID, "evaluate needs at least one row")
-        confusion = _on_device(features, lambda engine, rows: engine.nb_predict(rows, self.pi, self.theta, labels=labels))
+        labels = _labels(features, self._name, self._reasons)
+        _some_rows(len(features.row_ids), "evaluate")
+        confusion = _on_device(features, lambda engine, rows: self._predict(engine, rows, labels=labels),
+                               name=self._name, reasons=self._reasons)
         f1, accuracy = metrics(labels, confusion)
         return {"f1": f1, "accuracy": accuracy, "labels": labels, "confusion": confusion}
+
+
+class NaiveBayesModel(_Model):
+    """A fitted multinomial NaiveBayes model, host data: ``labels`` (float64[C], the class values ascending), ``pi``
+    (float64[C]), ``theta`` (float64[C, k]) and the ``fields`` it was fitted on; ``sums`` / ``counts`` are the device's
+    per-class feature sums and row counts it was made from."""
+
+    def __init__(self, labels, pi, theta, fields, sums=None, counts=None):
+        self.labels, self.pi, self.theta = np.asarray(labels, np.float64), np.asarray(pi, np.float64), np.asarray(theta, np.float64)
+        self.fields, self.sums, self.counts = list(fields), sums, counts
+
+    def _predict(self, engine, rows, raw=False, labels=None):
+        return engine.nb_predict(rows, self.pi, self.theta, raw=raw, labels=labels)
 
 
 def metrics(labels: np.ndarray, confusion: np.ndarray) -> tuple[float, float]:
@@ -235,9 +261,7 @@ class LogisticRegression:
         lowest refused row); numClasses = max label + 1.  No row, a label >= LO_NB_MAX_CLASSES or (binomial ? 2 : C) x k
         above LO_NB_MAX_THETA are refused, and so is ``family="binomial"`` with more than 2 classes."""
         from . import lbfgs
-        _usable(features)
-        if features.label is None:
-            raise ValueError("LogisticRegression needs features with a label")
+        _labelled(features, "LogisticRegression")
         k = len(features.fields)
         least = 2 if self.family == "binomial" else 1        # classes the model has at least: refused before any pass
         if least * k > N.LO_NB_MAX_THETA:
@@ -245,8 +269,7 @@ class LogisticRegression:
                                 f"{N.LO_NB_MAX_THETA}")
         n, total, m2, counts = _on_device(features, lambda engine, rows: engine.lr_stats(rows), name="LogisticRegression",
                                           reasons=_LR_REASONS)
-        if n == 0:
-            raise N.LoexecError(N.LO_ERR_INVALID, "LogisticRegression needs at least one row")
+        _some_rows(n, "LogisticRegression")
         num_classes = int(np.flatnonzero(counts)[-1]) + 1
         if self.family == "binomial" and num_classes > 2:
             raise ValueError(f"family='binomial' needs at most 2 classes, the labels give {num_classes}")
@@ -276,11 +299,12 @@ class LogisticRegression:
                                        res.iterations, self.threshold)
 
 
-class LogisticRegressionModel:
+class LogisticRegressionModel(_Model):
     """A fitted LogisticRegression model, host data: ``coefficient_matrix`` (float64[C', k]) and ``intercept_vector``
     (float64[C']) with C' = ``num_classes`` when ``is_multinomial`` else 1; binomial also ``coefficients`` (float64[k])
     and ``intercept``; ``fields`` it was fitted on; ``objective_history`` (the objective at every optimizer state, the
     start included; empty for a constant label) and ``iterations``; ``threshold`` of the binomial prediction."""
+    _name, _reasons = "LogisticRegression", _LR_REASONS
 
     def __init__(self, coefficient_matrix, intercept_vector, num_classes, is_multinomial, fields, objective_history=(),
                  iterations=0, threshold=0.5):
@@ -292,35 +316,14 @@ class LogisticRegressionModel:
         if not self.is_multinomial:
             self.coefficients, self.intercept = self.coefficient_matrix[0], float(self.intercept_vector[0])
 
-    def _check(self, features) -> None:
-        if list(features.fields) != self.fields:
-            raise ValueError(f"the model was fitted on fields {self.fields}, not {list(features.fields)}")
-
-    def _predict(self, engine, rows, **kw):
+    def _predict(self, engine, rows, raw=False, labels=None):
         return engine.lr_predict(rows, self.coefficient_matrix, self.intercept_vector, self.is_multinomial,
-                                 self.threshold, **kw)
+                                 self.threshold, raw=raw, labels=labels)
 
     def transform(self, features, raw: bool = False) -> "Predictions":
         """Spark's ``model.transform``: every row's ``probability`` and ``prediction`` (a class index as float64), and
         with ``raw`` its ``rawPrediction`` ([-m, m] when binomial), written in HBM on the rows' own devices."""
-        _usable(features)
-        self._check(features)
-        parts = _on_device(features, lambda engine, rows: self._predict(engine, rows, raw=raw), per_part=True,
-                           name="LogisticRegression", reasons=_LR_REASONS)
-        return Predictions(features, parts)
-
-    def evaluate(self, features) -> dict:
-        """``MulticlassClassificationEvaluator`` f1 and accuracy over ``transform(features)``, as
-        :meth:`NaiveBayesModel.evaluate`: ``{"f1", "accuracy", "labels", "confusion"}``."""
-        _usable(features)
-        self._check(features)
-        labels = _labels(features, "LogisticRegression", _LR_REASONS)
-        if len(features.row_ids) == 0:
-            raise N.LoexecError(N.LO_ERR_INVALID, "evaluate needs at least one row")
-        confusion = _on_device(features, lambda engine, rows: self._predict(engine, rows, labels=labels),
-                               name="LogisticRegression", reasons=_LR_REASONS)
-        f1, accuracy = metrics(labels, confusion)
-        return {"f1": f1, "accuracy": accuracy, "labels": labels, "confusion": confusion}
+        return super().transform(features, raw)
 
 
 class Predictions:
@@ -374,8 +377,7 @@ def split_thresholds(features, n: int, k: int, max_bins: int, name: str) -> tupl
 
             thr, r = T.column_thresholds(n, max_bins, distinct, rank, f32, w)
         finally:
-            for m in members:
-                m.free()
+            _free(got)
         out += thr
         rounds += r
     return out, rounds
@@ -388,6 +390,18 @@ def _integer(v, name, lo, hi=None):
     return int(v)
 
 
+def _tree_params(est, max_depth, max_bins, min_instances_per_node, min_info_gain) -> None:
+    """Checks and sets the tree parameters DecisionTreeClassifier and GBTClassifier share, with Spark's bounds."""
+    from . import tree as T
+    est.max_depth = _integer(max_depth, "max_depth", 0, T.MAX_DEPTH)
+    est.max_bins = _integer(max_bins, "max_bins", 2, T.MAX_BINS)
+    est.min_instances_per_node = _integer(min_instances_per_node, "min_instances_per_node", 1)
+    g = float(min_info_gain)
+    if not np.isfinite(g) or g < 0.0:
+        raise ValueError(f"min_info_gain must be finite and >= 0, not {min_info_gain!r}")
+    est.min_info_gain = g
+
+
 class DecisionTreeClassifier:
     """``pyspark.ml.classification.DecisionTreeClassifier(maxDepth, maxBins, minInstancesPerNode, minInfoGain,
     impurity)`` with its other defaults (every feature continuous, no ``weightCol``, no ``thresholds``) on the GPU.
@@ -396,13 +410,7 @@ class DecisionTreeClassifier:
     def __init__(self, max_depth: int = 5, max_bins: int = 32, min_instances_per_node: int = 1,
                  min_info_gain: float = 0.0, impurity: str = "gini"):
         from . import tree as T
-        self.max_depth = _integer(max_depth, "max_depth", 0, T.MAX_DEPTH)
-        self.max_bins = _integer(max_bins, "max_bins", 2, T.MAX_BINS)
-        self.min_instances_per_node = _integer(min_instances_per_node, "min_instances_per_node", 1)
-        g = float(min_info_gain)
-        if not np.isfinite(g) or g < 0.0:
-            raise ValueError(f"min_info_gain must be finite and >= 0, not {min_info_gain!r}")
-        self.min_info_gain = g
+        _tree_params(self, max_depth, max_bins, min_instances_per_node, min_info_gain)
         if not isinstance(impurity, str) or impurity.lower() not in T.IMPURITIES:
             raise ValueError(f"impurity must be one of {list(T.IMPURITIES)}, not {impurity!r}")
         self.impurity = impurity.lower()
@@ -413,14 +421,11 @@ class DecisionTreeClassifier:
         lowest refused row); numClasses = max label + 1.  No row, more than LO_DT_MAX_CLASSES classes or a one-node
         histogram (k x min(max_bins, n) x C x 8 bytes) above LO_DT_PASS_HIST are refused."""
         from . import tree as T
-        _usable(features)
-        if features.label is None:
-            raise ValueError("DecisionTreeClassifier needs features with a label")
         name, k = "DecisionTreeClassifier", len(features.fields)
+        _labelled(features, name)
         n, _total, _m2, counts = _on_device(features, lambda engine, rows: engine.lr_stats(rows), name=name,
                                             reasons=_LR_REASONS)
-        if n == 0:
-            raise N.LoexecError(N.LO_ERR_INVALID, "DecisionTreeClassifier needs at least one row")
+        _some_rows(n, name)
         num_classes = int(np.flatnonzero(counts)[-1]) + 1
         if num_classes > N.LO_DT_MAX_CLASSES:
             raise N.LoexecError(N.LO_ERR_INVALID, f"{num_classes} classes exceed LO_DT_MAX_CLASSES = "
@@ -439,48 +444,30 @@ class DecisionTreeClassifier:
             tree, _shapes = T.grow(level, thresholds, num_classes, self.max_depth, self.impurity,
                                    self.min_instances_per_node, self.min_info_gain)
         finally:
-            for b in binned if isinstance(binned, list) else [binned]:
-                b.free()
+            _free(binned)
         model = DecisionTreeClassificationModel(tree, features.fields, thresholds)
         model.rank_rounds = rounds
         return model
 
 
-class DecisionTreeClassificationModel:
+class DecisionTreeClassificationModel(_Model):
     """A fitted decision tree, host data: ``tree`` (:class:`~tree.Tree`: the node arrays feature, threshold, left, right,
     counts, prediction, impurity and gain), ``depth``, ``num_nodes``, ``num_classes``, the ``fields`` it was fitted on
     and every column's split ``thresholds``."""
+    _name, _reasons = "DecisionTreeClassifier", _LR_REASONS
 
     def __init__(self, tree, fields, thresholds=None):
         self.tree, self.fields, self.thresholds = tree, list(fields), thresholds
         self.depth, self.num_nodes, self.num_classes = tree.depth, tree.num_nodes, tree.num_classes
 
-    def _check(self, features) -> None:
-        if list(features.fields) != self.fields:
-            raise ValueError(f"the model was fitted on fields {self.fields}, not {list(features.fields)}")
+    def _predict(self, engine, rows, raw=False, labels=None):
+        return engine.dt_predict(rows, self.tree, raw=raw, labels=labels)
 
     def transform(self, features, raw: bool = False) -> "Predictions":
         """Spark's ``model.transform``: every row's ``probability`` (the leaf's class counts over their sum) and
         ``prediction`` (a class index as float64), and with ``raw`` its ``rawPrediction`` (the leaf's counts), written in
         HBM on the rows' own devices."""
-        _usable(features)
-        self._check(features)
-        parts = _on_device(features, lambda engine, rows: engine.dt_predict(rows, self.tree, raw=raw), per_part=True,
-                           name="DecisionTreeClassifier", reasons=_LR_REASONS)
-        return Predictions(features, parts)
-
-    def evaluate(self, features) -> dict:
-        """``MulticlassClassificationEvaluator`` f1 and accuracy over ``transform(features)``, as
-        :meth:`NaiveBayesModel.evaluate`: ``{"f1", "accuracy", "labels", "confusion"}``."""
-        _usable(features)
-        self._check(features)
-        labels = _labels(features, "DecisionTreeClassifier", _LR_REASONS)
-        if len(features.row_ids) == 0:
-            raise N.LoexecError(N.LO_ERR_INVALID, "evaluate needs at least one row")
-        confusion = _on_device(features, lambda engine, rows: engine.dt_predict(rows, self.tree, labels=labels),
-                               name="DecisionTreeClassifier", reasons=_LR_REASONS)
-        f1, accuracy = metrics(labels, confusion)
-        return {"f1": f1, "accuracy": accuracy, "labels": labels, "confusion": confusion}
+        return super().transform(features, raw)
 
 
 _GB_REASONS = ("is NaN or infinite", "is not a label 0 or 1")
@@ -494,20 +481,13 @@ class GBTClassifier:
 
     def __init__(self, max_iter: int = 20, step_size: float = 0.1, max_depth: int = 5, max_bins: int = 32,
                  min_instances_per_node: int = 1, min_info_gain: float = 0.0):
-        from . import tree as T
         self.max_iter = _integer(max_iter, "max_iter", 1)
         st = float(step_size) if isinstance(step_size, (int, float, np.floating)) and not isinstance(step_size, bool) \
             else float("nan")
         if not 0.0 < st <= 1.0:
             raise ValueError(f"step_size must lie in (0, 1], not {step_size!r}")
         self.step_size = st
-        self.max_depth = _integer(max_depth, "max_depth", 0, T.MAX_DEPTH)
-        self.max_bins = _integer(max_bins, "max_bins", 2, T.MAX_BINS)
-        self.min_instances_per_node = _integer(min_instances_per_node, "min_instances_per_node", 1)
-        g = float(min_info_gain)
-        if not np.isfinite(g) or g < 0.0:
-            raise ValueError(f"min_info_gain must be finite and >= 0, not {min_info_gain!r}")
-        self.min_info_gain = g
+        _tree_params(self, max_depth, max_bins, min_instances_per_node, min_info_gain)
 
     def fit(self, features) -> "GBTClassificationModel":
         """The boosted trees of ``features`` (:class:`~builder_frontend.Features` with a label, on one GPU or sharded).
@@ -515,10 +495,8 @@ class GBTClassifier:
         refused cell over both checks).  No row, or a one-node level (k x min(max_bins, n) x 40 bytes) above LO_DT_PASS_HIST, is
         refused.  The margins and residuals stay on the device, the trees are chosen here from each level's sums."""
         from . import tree as T
-        _usable(features)
-        if features.label is None:
-            raise ValueError("GBTClassifier needs features with a label")
         name, k = "GBTClassifier", len(features.fields)
+        _labelled(features, name)
         from .engine import InvalidCellError
         # the labels (lo_gb_update's first call) and the features (lo_lr_stats_range) are both checked, and the lowest
         # refused cell of the two is raised, as one pass over both would find it
@@ -537,8 +515,7 @@ class GBTClassifier:
                     raise
             if refused:
                 raise min(refused, key=lambda e: (e.row, e.position))
-            if n == 0:
-                raise N.LoexecError(N.LO_ERR_INVALID, "GBTClassifier needs at least one row")
+            _some_rows(n, name)
             if k * min(self.max_bins, n) * N.LO_GB_WORDS * 8 > N.LO_DT_PASS_HIST:
                 raise N.LoexecError(N.LO_ERR_INVALID, f"{k} features x {min(self.max_bins, n)} bins x "
                                     f"{N.LO_GB_WORDS} words: one node's histogram exceeds LO_DT_PASS_HIST = "
@@ -561,17 +538,17 @@ class GBTClassifier:
                     _on_device(features, lambda engine, part: engine.gb_update(part, rows, tree, weight), name=name,
                                reasons=_GB_REASONS)
         finally:
-            for held in (rows, binned):
-                for b in held if isinstance(held, list) else [held] if held is not None else []:
-                    b.free()
+            _free(rows)
+            _free(binned)
         return GBTClassificationModel(trees, weights, features.fields, thresholds)
 
 
-class GBTClassificationModel:
+class GBTClassificationModel(_Model):
     """A fitted GBT model, host data: ``trees`` (regression :class:`~tree.Tree` s in breadth-first arrays: feature,
     threshold, left, right, prediction, impurity, gain and ``counts`` the node's (count, sum, sumSq)), ``tree_weights``
     ([1.0, step_size, ...]), ``num_classes`` (2), ``total_num_nodes``, the ``fields`` it was fitted on and every column's
     split ``thresholds``."""
+    _name, _reasons = "GBTClassifier", _GB_REASONS
 
     def __init__(self, trees, tree_weights, fields, thresholds=None):
         self.trees, self.tree_weights = list(trees), np.asarray(tree_weights, np.float64)
@@ -579,31 +556,11 @@ class GBTClassificationModel:
         self.num_classes = 2
         self.total_num_nodes = sum(t.num_nodes for t in self.trees)
 
-    def _check(self, features) -> None:
-        if list(features.fields) != self.fields:
-            raise ValueError(f"the model was fitted on fields {self.fields}, not {list(features.fields)}")
+    def _predict(self, engine, rows, raw=False, labels=None):
+        return engine.gb_predict(rows, self.trees, self.tree_weights, raw=raw, labels=labels)
 
     def transform(self, features, raw: bool = False) -> "Predictions":
         """Spark's ``model.transform``: every row's ``probability`` ([1 / (1 + exp(2m)), the rest] of the margin m) and
         ``prediction`` (m > 0), and with ``raw`` its ``rawPrediction`` ([-m, m]), written in HBM on the rows' own
         devices."""
-        _usable(features)
-        self._check(features)
-        parts = _on_device(features, lambda engine, rows: engine.gb_predict(rows, self.trees, self.tree_weights,
-                                                                            raw=raw), per_part=True,
-                           name="GBTClassifier", reasons=_GB_REASONS)
-        return Predictions(features, parts)
-
-    def evaluate(self, features) -> dict:
-        """``MulticlassClassificationEvaluator`` f1 and accuracy over ``transform(features)``, as
-        :meth:`NaiveBayesModel.evaluate`: ``{"f1", "accuracy", "labels", "confusion"}``."""
-        _usable(features)
-        self._check(features)
-        labels = _labels(features, "GBTClassifier", _GB_REASONS)
-        if len(features.row_ids) == 0:
-            raise N.LoexecError(N.LO_ERR_INVALID, "evaluate needs at least one row")
-        confusion = _on_device(features, lambda engine, rows: engine.gb_predict(rows, self.trees, self.tree_weights,
-                                                                                labels=labels),
-                               name="GBTClassifier", reasons=_GB_REASONS)
-        f1, accuracy = metrics(labels, confusion)
-        return {"f1": f1, "accuracy": accuracy, "labels": labels, "confusion": confusion}
+        return super().transform(features, raw)

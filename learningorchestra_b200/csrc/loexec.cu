@@ -2650,86 +2650,138 @@ void nb_tree(HostCall &c, const double *src, int64_t m, size_t slots, double *ds
     }
 }
 
-// lo_nb_predict and lo_lr_predict: the model's C classes (lo::kLrBinomial: C = 1, two outputs per row) over every row,
-// by k_nb_predict with the epilogue `mode`.  The arguments are checked here (ctx and info before).
-int nb_predict(lo_ctx *ctx, const lo_table *x, int64_t ld, int32_t k, int64_t n, const double *pi, const double *theta,
-               int32_t nclasses, int mode, double threshold, lo_table *prob, lo_table *raw, lo_table *pred,
-               const lo_table *y, const double *eval_labels, int32_t neval, int64_t *confusion_out, lo_nb_info *info,
-               lo_host_timing *timing, const char *predict_name, const char *evaluate_name) {
-    const bool eval = confusion_out != nullptr;
-    if (eval && !y) return fail(LO_ERR_INVALID, "evaluate needs y");
-    LO_TRY(check_nb_matrix(ctx, x, ld, k, n, eval ? y : nullptr));
-    const bool binomial = mode == lo::kLrBinomial;
-    LO_TRY(check_nb_caps(binomial ? 2 : nclasses, k));
-    if (!pi || !theta) return fail(LO_ERR_INVALID, "pi or theta is NULL");
-    const int32_t C = nclasses, CO = binomial ? 2 : C;
+// check_ctx, then info cleared: no refused cell
+int start_info(const lo_ctx *ctx, lo_nb_info *info) {
+    LO_TRY(check_ctx(ctx));
+    if (!info) return fail(LO_ERR_INVALID, "info is NULL");
+    *info = lo_nb_info{-1, -1, 0};
+    return LO_OK;
+}
+
+// The frame of the transform / evaluate entry points (lo_nb_predict, lo_lr_predict, lo_dt_predict, lo_gb_predict), CO
+// outputs per row.  Evaluate (confusion_out given) writes no rows: the kernel counts (label slot, prediction) into the
+// neval x CO matrix (lo::Confusion) and lowers the refusal word for a label that is not in eval_labels.  Transform
+// writes prob, pred and (when given) raw.  An entry point calls check_x, its model checks, check_out, opens its HostCall
+// as call(prefix), stages its model, then stage, grid and its launch, and returns finish.
+struct PredictFrame {
+    const lo_table *y;
+    const double *eval_labels;
+    int32_t neval, CO = 0;
+    int64_t *confusion_out;
+    const bool eval;
     int direct = 0;
-    if (eval) {
-        if (prob || raw || pred) return fail(LO_ERR_INVALID, "evaluate writes no rows: prob, raw and pred must be NULL");
-        LO_TRY(check_nb_classes(eval_labels, neval, "eval_labels", &direct));
-        std::fill(confusion_out, confusion_out + (size_t)neval * CO, (int64_t)0);
-    } else {
+    std::string name;
+    double *d_evl = nullptr;
+    unsigned long long *conf = nullptr;
+    RefusedCell bad;
+
+    PredictFrame(const lo_table *y_, const double *labels, int32_t neval_, int64_t *confusion)
+        : y(y_), eval_labels(labels), neval(neval_), confusion_out(confusion), eval(confusion != nullptr) {}
+    // evaluate's y, then the matrix and (evaluate) its labels
+    int check_x(const lo_ctx *ctx, const lo_table *x, int64_t ld, int32_t k, int64_t n) const {
+        if (eval && !y) return fail(LO_ERR_INVALID, "evaluate needs y");
+        return check_nb_matrix(ctx, x, ld, k, n, eval ? y : nullptr);
+    }
+    // the outputs of CO columns: evaluate's labels (confusion_out zeroed), or transform's tables (neval becomes 0)
+    int check_out(const lo_ctx *ctx, int64_t n, int32_t co, const lo_table *prob, const lo_table *raw, const lo_table *pred) {
+        CO = co;
+        if (eval) {
+            if (prob || raw || pred) return fail(LO_ERR_INVALID, "evaluate writes no rows: prob, raw and pred must be NULL");
+            LO_TRY(check_nb_classes(eval_labels, neval, "eval_labels", &direct));
+            std::fill(confusion_out, confusion_out + (size_t)neval * CO, (int64_t)0);
+            return LO_OK;
+        }
         if (y || eval_labels) return fail(LO_ERR_INVALID, "y and eval_labels go with confusion_out");
+        neval = 0;
         if (n > 0 && CO > INT64_MAX / 8 / n) return fail(LO_ERR_INVALID, "n * C overflows");
         LO_TRY(check_float_table(ctx, prob, LO_F64, n * CO, "prob"));
         LO_TRY(check_float_table(ctx, pred, LO_F64, n, "pred"));
         if (raw) LO_TRY(check_float_table(ctx, raw, LO_F64, n * CO, "raw"));
+        return LO_OK;
     }
-    HostCall c(ctx, eval ? evaluate_name : predict_name);
-    if (n == 0) return c.finish(timing);
-    // theta j-major for the blocks of classes; raws and the histogram in shared memory when they fit beside the tables
-    std::vector<double> theta_t((size_t)k * C);
-    for (int32_t cc = 0; cc < C; ++cc)
-        for (int32_t j = 0; j < k; ++j) theta_t[(size_t)j * C + cc] = theta[(size_t)cc * k + j];
-    const int64_t base = ((int64_t)k * C + C + lo::kNbTile * (lo::kNbChunk + 1) + (eval ? neval : 0)) * 8;
-    const int64_t raws_bytes = (int64_t)C * lo::kNbTile * 8, hist_bytes = eval ? (int64_t)neval * CO * 4 : 0;
-    const bool raws_smem = base + raws_bytes <= lo::kNbSmemMax;
-    const int64_t with_raws = base + (raws_smem ? raws_bytes : 0);
-    const bool hist_smem = eval && with_raws + hist_bytes <= lo::kNbSmemMax;
-    const int smem = (int)(with_raws + (hist_smem ? hist_bytes : 0));
-    double *d_theta = nullptr, *d_pi = nullptr, *d_evl = nullptr, *raws = nullptr;
-    unsigned long long *conf = nullptr;
-    RefusedCell bad;
-    c.alloc(&d_theta, theta_t.size() * 8);
-    c.alloc(&d_pi, (size_t)C * 8);
-    c.to_dev(d_theta, theta_t.data(), theta_t.size() * 8);
-    c.to_dev(d_pi, pi, (size_t)C * 8);
-    if (eval) {
+    // the call's name: <prefix>_evaluate or <prefix>_predict
+    const char *call(const char *prefix) {
+        name = std::string(prefix) + (eval ? "_evaluate" : "_predict");
+        return name.c_str();
+    }
+    // evaluate: the labels uploaded, the counts zeroed and the refusal word armed
+    void stage(HostCall &c) {
+        if (!eval) return;
         c.alloc(&d_evl, (size_t)neval * 8);
         c.alloc(&conf, (size_t)neval * CO * 8);
         c.to_dev(d_evl, eval_labels, (size_t)neval * 8);
         c.memset(conf, 0, (size_t)neval * CO * 8);
         bad.arm(c);
     }
-    auto go = [&](auto kernel, auto tag) {
-        using T = decltype(tag);
+    // CTAs of `threads` with smem bytes: as many as the SMs hold at once, at most `units`
+    template <typename K> static int grid(HostCall &c, K kernel, int threads, int smem, int64_t units) {
         int per_sm = 0;
         c.run([&] { return cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem); });
-        c.run([&] { return cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, lo::kNbTile, smem); });
-        const int64_t ntiles = (n + lo::kNbTile - 1) / lo::kNbTile;
-        const int grid = (int)std::min<int64_t>(ntiles, (int64_t)ctx->sm_count * std::max(1, per_sm));
+        c.run([&] { return cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, threads, smem); });
+        return (int)std::min<int64_t>(units, (int64_t)c.ctx->sm_count * std::max(1, per_sm));
+    }
+    // evaluate's counts back; a refused label names its row, confusion_out zeroed
+    int finish(HostCall &c, int32_t k, lo_nb_info *info, lo_host_timing *timing) {
+        if (eval) c.to_host(confusion_out, conf, (size_t)neval * CO * 8);
+        bad.read(c);
+        LO_TRY(c.finish(timing));
+        if (!bad.found(k, info)) return LO_OK;
+        std::fill(confusion_out, confusion_out + (size_t)neval * CO, (int64_t)0);
+        return fail(LO_ERR_INVALID, "row %lld: its label is not one of the evaluated labels", (long long)info->bad_row);
+    }
+};
+
+// lo_nb_predict and lo_lr_predict: the model's C classes (lo::kLrBinomial: C = 1, two outputs per row) over every row,
+// by k_nb_predict with the epilogue `mode`.  The arguments are checked here (ctx and info before).
+int nb_predict(lo_ctx *ctx, const lo_table *x, int64_t ld, int32_t k, int64_t n, const double *pi, const double *theta,
+               int32_t nclasses, int mode, double threshold, lo_table *prob, lo_table *raw, lo_table *pred,
+               const lo_table *y, const double *eval_labels, int32_t neval, int64_t *confusion_out, lo_nb_info *info,
+               lo_host_timing *timing, const char *prefix) {
+    PredictFrame f(y, eval_labels, neval, confusion_out);
+    LO_TRY(f.check_x(ctx, x, ld, k, n));
+    const bool binomial = mode == lo::kLrBinomial;
+    LO_TRY(check_nb_caps(binomial ? 2 : nclasses, k));
+    if (!pi || !theta) return fail(LO_ERR_INVALID, "pi or theta is NULL");
+    const int32_t C = nclasses;
+    LO_TRY(f.check_out(ctx, n, binomial ? 2 : C, prob, raw, pred));
+    HostCall c(ctx, f.call(prefix));
+    if (n == 0) return c.finish(timing);
+    // theta j-major for the blocks of classes; raws and the histogram in shared memory when they fit beside the tables
+    std::vector<double> theta_t((size_t)k * C);
+    for (int32_t cc = 0; cc < C; ++cc)
+        for (int32_t j = 0; j < k; ++j) theta_t[(size_t)j * C + cc] = theta[(size_t)cc * k + j];
+    const int64_t base = ((int64_t)k * C + C + lo::kNbTile * (lo::kNbChunk + 1) + f.neval) * 8;
+    const int64_t raws_bytes = (int64_t)C * lo::kNbTile * 8, hist_bytes = (int64_t)f.neval * f.CO * 4;
+    const bool raws_smem = base + raws_bytes <= lo::kNbSmemMax;
+    const int64_t with_raws = base + (raws_smem ? raws_bytes : 0);
+    const bool hist_smem = f.eval && with_raws + hist_bytes <= lo::kNbSmemMax;
+    const int smem = (int)(with_raws + (hist_smem ? hist_bytes : 0));
+    double *d_theta = nullptr, *d_pi = nullptr, *raws = nullptr;
+    c.alloc(&d_theta, theta_t.size() * 8);
+    c.alloc(&d_pi, (size_t)C * 8);
+    c.to_dev(d_theta, theta_t.data(), theta_t.size() * 8);
+    c.to_dev(d_pi, pi, (size_t)C * 8);
+    f.stage(c);
+    auto go = [&](auto kernel, auto tag) {
+        using T = decltype(tag);
+        const int grid = f.grid(c, kernel, lo::kNbTile, smem, (n + lo::kNbTile - 1) / lo::kNbTile);
         if (!raws_smem) c.alloc(&raws, (size_t)grid * raws_bytes);
         c.mark();
         c.launch(1, [&] {
             kernel<<<grid, lo::kNbTile, smem, c.s>>>((const T *)x->base, ld, k, n, d_theta, d_pi, C,
                                                      prob ? (double *)prob->base : nullptr, raw ? (double *)raw->base : nullptr,
                                                      pred ? (double *)pred->base : nullptr, y ? (const T *)y->base : nullptr,
-                                                     d_evl, neval, direct, conf, raws, hist_smem ? 1 : 0, bad.word, mode,
-                                                     threshold);
+                                                     f.d_evl, f.neval, f.direct, f.conf, raws, hist_smem ? 1 : 0,
+                                                     f.bad.word, mode, threshold);
         });
         c.mark();
     };
     if (x->dtype == LO_F32) {
-        if (eval) go(lo::k_nb_predict<float, true>, 0.0f); else go(lo::k_nb_predict<float, false>, 0.0f);
+        if (f.eval) go(lo::k_nb_predict<float, true>, 0.0f); else go(lo::k_nb_predict<float, false>, 0.0f);
     } else {
-        if (eval) go(lo::k_nb_predict<double, true>, 0.0); else go(lo::k_nb_predict<double, false>, 0.0);
+        if (f.eval) go(lo::k_nb_predict<double, true>, 0.0); else go(lo::k_nb_predict<double, false>, 0.0);
     }
-    if (eval) c.to_host(confusion_out, conf, (size_t)neval * CO * 8);
-    bad.read(c);
-    LO_TRY(c.finish(timing));
-    if (!bad.found(k, info)) return LO_OK;
-    std::fill(confusion_out, confusion_out + (size_t)neval * CO, (int64_t)0);
-    return fail(LO_ERR_INVALID, "row %lld: its label is not one of the evaluated labels", (long long)info->bad_row);
+    return f.finish(c, k, info, timing);
 }
 
 }  // namespace
@@ -2836,11 +2888,9 @@ int lo_nb_predict(lo_ctx *ctx, const lo_table *x, int64_t ld, int32_t k, int64_t
                   int32_t nclasses, lo_table *prob, lo_table *raw, lo_table *pred, const lo_table *y,
                   const double *eval_labels, int32_t neval, int64_t *confusion_out, lo_nb_info *info,
                   lo_host_timing *timing) {
-    LO_TRY(check_ctx(ctx));
-    if (!info) return fail(LO_ERR_INVALID, "info is NULL");
-    *info = lo_nb_info{-1, -1, 0};
-    return nb_predict(ctx, x, ld, k, n, pi, theta, nclasses, lo::kNbSoftmax, 0.0, prob, raw, pred, y, eval_labels, neval, confusion_out,
-                      info, timing, "nb_predict", "nb_evaluate");
+    LO_TRY(start_info(ctx, info));
+    return nb_predict(ctx, x, ld, k, n, pi, theta, nclasses, lo::kNbSoftmax, 0.0, prob, raw, pred, y, eval_labels, neval,
+                      confusion_out, info, timing, "nb");
 }
 
 }  // extern "C"
@@ -3096,15 +3146,12 @@ int lo_lr_predict(lo_ctx *ctx, const lo_table *x, int64_t ld, int32_t k, int64_t
                   const double *intercept, int32_t nclasses, int32_t multinomial, double threshold, lo_table *prob,
                   lo_table *raw, lo_table *pred, const lo_table *y, const double *eval_labels, int32_t neval,
                   int64_t *confusion_out, lo_nb_info *info, lo_host_timing *timing) {
-    LO_TRY(check_ctx(ctx));
-    if (!info) return fail(LO_ERR_INVALID, "info is NULL");
-    *info = lo_nb_info{-1, -1, 0};
+    LO_TRY(start_info(ctx, info));
     LO_TRY(check_lr_model(nclasses, multinomial, k, false));
     if (!multinomial && !(threshold >= 0.0 && threshold <= 1.0))
         return fail(LO_ERR_INVALID, "threshold %g outside [0, 1]", threshold);
     return nb_predict(ctx, x, ld, k, n, intercept, coef, nclasses, multinomial ? lo::kLrMultinomial : lo::kLrBinomial,
-                      threshold, prob, raw, pred, y, eval_labels,
-                      neval, confusion_out, info, timing, "lr_predict", "lr_evaluate");
+                      threshold, prob, raw, pred, y, eval_labels, neval, confusion_out, info, timing, "lr");
 }
 
 }  // extern "C"
@@ -3121,6 +3168,16 @@ int check_typed_table(const lo_ctx *ctx, const lo_table *t, int dtype, int64_t n
     if (t->device != ctx->device) return fail(LO_ERR_INVALID, "%s lives on device %d, the context on %d", name, t->device, ctx->device);
     if (t->nrows < need)
         return fail(LO_ERR_INVALID, "%s holds %lld elements, %lld needed", name, (long long)t->nrows, (long long)need);
+    return LO_OK;
+}
+
+// the nodes [lo, hi) of one tree: features in [-1, k), an internal node's children inside (i, hi)
+int check_tree_nodes(const int32_t *feature, const int32_t *left, const int32_t *right, int32_t lo, int32_t hi, int32_t k) {
+    for (int32_t i = lo; i < hi; ++i) {
+        if (feature[i] < -1 || feature[i] >= k) return fail(LO_ERR_INVALID, "node %d: feature %d outside [-1, %d)", i, feature[i], k);
+        if (feature[i] >= 0 && !(left[i] > i && left[i] < hi && right[i] > i && right[i] < hi))
+            return fail(LO_ERR_INVALID, "node %d: children %d, %d must lie in (%d, %d)", i, left[i], right[i], i, hi);
+    }
     return LO_OK;
 }
 
@@ -3462,45 +3519,25 @@ int lo_dt_predict(lo_ctx *ctx, const lo_table *x, int64_t ld, int32_t k, int64_t
                   int32_t nclasses, lo_table *prob, lo_table *raw, lo_table *pred, const lo_table *y,
                   const double *eval_labels, int32_t neval, int64_t *confusion_out, lo_nb_info *info,
                   lo_host_timing *timing) {
-    LO_TRY(check_ctx(ctx));
-    if (!info) return fail(LO_ERR_INVALID, "info is NULL");
-    *info = lo_nb_info{-1, -1, 0};
-    const bool eval = confusion_out != nullptr;
-    if (eval && !y) return fail(LO_ERR_INVALID, "evaluate needs y");
-    LO_TRY(check_nb_matrix(ctx, x, ld, k, n, eval ? y : nullptr));
+    LO_TRY(start_info(ctx, info));
+    PredictFrame f(y, eval_labels, neval, confusion_out);
+    LO_TRY(f.check_x(ctx, x, ld, k, n));
     LO_TRY(check_dt_classes(nclasses));
     const int32_t C = nclasses, M = nnodes;
     if (M < 1 || !feature || !threshold || !left || !right || !counts)
         return fail(LO_ERR_INVALID, "a tree of %d nodes: feature, threshold, left, right and counts are needed", M);
-    // every path ends: an internal node's children come after it
-    for (int32_t i = 0; i < M; ++i) {
-        if (feature[i] < -1 || feature[i] >= k) return fail(LO_ERR_INVALID, "node %d: feature %d outside [-1, %d)", i, feature[i], k);
-        if (feature[i] >= 0 && !(left[i] > i && left[i] < M && right[i] > i && right[i] < M))
-            return fail(LO_ERR_INVALID, "node %d: children %d, %d must lie in (%d, %d)", i, left[i], right[i], i, M);
-    }
-    int direct = 0;
-    if (eval) {
-        if (prob || raw || pred) return fail(LO_ERR_INVALID, "evaluate writes no rows: prob, raw and pred must be NULL");
-        LO_TRY(check_nb_classes(eval_labels, neval, "eval_labels", &direct));
-        std::fill(confusion_out, confusion_out + (size_t)neval * C, (int64_t)0);
-    } else {
-        if (y || eval_labels) return fail(LO_ERR_INVALID, "y and eval_labels go with confusion_out");
-        LO_TRY(check_float_table(ctx, prob, LO_F64, n * C, "prob"));
-        LO_TRY(check_float_table(ctx, pred, LO_F64, n, "pred"));
-        if (raw) LO_TRY(check_float_table(ctx, raw, LO_F64, n * C, "raw"));
-    }
-    HostCall c(ctx, eval ? "dt_evaluate" : "dt_predict");
+    LO_TRY(check_tree_nodes(feature, left, right, 0, M, k));
+    LO_TRY(f.check_out(ctx, n, C, prob, raw, pred));
+    HostCall c(ctx, f.call("dt"));
     if (n == 0) return c.finish(timing);
     const int64_t tree_bytes = (int64_t)M * 8 + ((int64_t)3 * M + 1) / 2 * 8;
-    const int64_t evl_bytes = eval ? (int64_t)neval * 8 : 0, hist_bytes = eval ? (int64_t)neval * C * 4 : 0;
+    const int64_t evl_bytes = (int64_t)f.neval * 8, hist_bytes = (int64_t)f.neval * C * 4;
     const bool tree_smem = tree_bytes + evl_bytes <= lo::kDtTreeSmem;
     const int64_t fixed = (tree_smem ? tree_bytes : 0) + evl_bytes;
-    const bool hist_smem = eval && fixed + hist_bytes <= lo::kDtTreeSmem;
+    const bool hist_smem = f.eval && fixed + hist_bytes <= lo::kDtTreeSmem;
     const int smem = (int)(fixed + (hist_smem ? hist_bytes : 0));
     int *d_int = nullptr;
-    double *d_thr = nullptr, *d_cnt = nullptr, *d_evl = nullptr;
-    unsigned long long *conf = nullptr;
-    RefusedCell bad;
+    double *d_thr = nullptr, *d_cnt = nullptr;
     c.alloc(&d_int, (size_t)M * 12);
     c.alloc(&d_thr, (size_t)M * 8);
     c.alloc(&d_cnt, (size_t)M * C * 8);
@@ -3509,42 +3546,27 @@ int lo_dt_predict(lo_ctx *ctx, const lo_table *x, int64_t ld, int32_t k, int64_t
     c.to_dev(d_int + 2 * M, right, (size_t)M * 4);
     c.to_dev(d_thr, threshold, (size_t)M * 8);
     c.to_dev(d_cnt, counts, (size_t)M * C * 8);
-    if (eval) {
-        c.alloc(&d_evl, (size_t)neval * 8);
-        c.alloc(&conf, (size_t)neval * C * 8);
-        c.to_dev(d_evl, eval_labels, (size_t)neval * 8);
-        c.memset(conf, 0, (size_t)neval * C * 8);
-        bad.arm(c);
-    }
+    f.stage(c);
     auto go = [&](auto kernel, auto tag) {
         using T = decltype(tag);
-        int per_sm = 0;
-        c.run([&] { return cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem); });
-        c.run([&] { return cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, lo::kDtThreads, smem); });
-        const int grid = (int)std::min<int64_t>((n + lo::kDtThreads - 1) / lo::kDtThreads,
-                                                (int64_t)ctx->sm_count * std::max(1, per_sm));
+        const int grid = f.grid(c, kernel, lo::kDtThreads, smem, (n + lo::kDtThreads - 1) / lo::kDtThreads);
         c.mark();
         c.launch(1, [&] {
             kernel<<<grid, lo::kDtThreads, smem, c.s>>>((const T *)x->base, ld, k, n, M, d_int, d_thr, d_int + M, d_int + 2 * M,
                                                         d_cnt, C, tree_smem ? 1 : 0, prob ? (double *)prob->base : nullptr,
                                                         raw ? (double *)raw->base : nullptr,
                                                         pred ? (double *)pred->base : nullptr,
-                                                        y ? (const T *)y->base : nullptr, d_evl, neval, direct, conf,
-                                                        hist_smem ? 1 : 0, bad.word);
+                                                        y ? (const T *)y->base : nullptr, f.d_evl, f.neval, f.direct, f.conf,
+                                                        hist_smem ? 1 : 0, f.bad.word);
         });
         c.mark();
     };
     if (x->dtype == LO_F32) {
-        if (eval) go(lo::k_dt_predict<float, true>, 0.0f); else go(lo::k_dt_predict<float, false>, 0.0f);
+        if (f.eval) go(lo::k_dt_predict<float, true>, 0.0f); else go(lo::k_dt_predict<float, false>, 0.0f);
     } else {
-        if (eval) go(lo::k_dt_predict<double, true>, 0.0); else go(lo::k_dt_predict<double, false>, 0.0);
+        if (f.eval) go(lo::k_dt_predict<double, true>, 0.0); else go(lo::k_dt_predict<double, false>, 0.0);
     }
-    if (eval) c.to_host(confusion_out, conf, (size_t)neval * C * 8);
-    bad.read(c);
-    LO_TRY(c.finish(timing));
-    if (!bad.found(k, info)) return LO_OK;
-    std::fill(confusion_out, confusion_out + (size_t)neval * C, (int64_t)0);
-    return fail(LO_ERR_INVALID, "row %lld: its label is not one of the evaluated labels", (long long)info->bad_row);
+    return f.finish(c, k, info, timing);
 }
 
 int lo_gb_level(lo_ctx *ctx, const lo_table *codes, int64_t kp, int32_t k, const lo_table *residual, int64_t n,
@@ -3568,16 +3590,6 @@ int lo_gb_level(lo_ctx *ctx, const lo_table *codes, int64_t kp, int32_t k, const
 }  // extern "C"
 
 namespace {
-
-// the nodes [lo, hi) of one tree: features in [-1, k), an internal node's children inside (i, hi)
-int check_tree_nodes(const int32_t *feature, const int32_t *left, const int32_t *right, int32_t lo, int32_t hi, int32_t k) {
-    for (int32_t i = lo; i < hi; ++i) {
-        if (feature[i] < -1 || feature[i] >= k) return fail(LO_ERR_INVALID, "node %d: feature %d outside [-1, %d)", i, feature[i], k);
-        if (feature[i] >= 0 && !(left[i] > i && left[i] < hi && right[i] > i && right[i] < hi))
-            return fail(LO_ERR_INVALID, "node %d: children %d, %d must lie in (%d, %d)", i, left[i], right[i], i, hi);
-    }
-    return LO_OK;
-}
 
 // a 128-bit sum of lo_gb_level's words at w (lo, hi) as an integer
 __int128 gb_word(const uint64_t *w) { return (__int128)(((unsigned __int128)w[1] << 64) | w[0]); }
@@ -3687,12 +3699,9 @@ int lo_gb_predict(lo_ctx *ctx, const lo_table *x, int64_t ld, int32_t k, int64_t
                   const int32_t *left, const int32_t *right, const double *value, lo_table *prob, lo_table *raw,
                   lo_table *pred, const lo_table *y, const double *eval_labels, int32_t neval, int64_t *confusion_out,
                   lo_nb_info *info, lo_host_timing *timing) {
-    LO_TRY(check_ctx(ctx));
-    if (!info) return fail(LO_ERR_INVALID, "info is NULL");
-    *info = lo_nb_info{-1, -1, 0};
-    const bool eval = confusion_out != nullptr;
-    if (eval && !y) return fail(LO_ERR_INVALID, "evaluate needs y");
-    LO_TRY(check_nb_matrix(ctx, x, ld, k, n, eval ? y : nullptr));
+    LO_TRY(start_info(ctx, info));
+    PredictFrame f(y, eval_labels, neval, confusion_out);
+    LO_TRY(f.check_x(ctx, x, ld, k, n));
     const int32_t M = nnodes;
     if (ntrees < 1 || M < ntrees || !start || !weight || !feature || !threshold || !left || !right || !value)
         return fail(LO_ERR_INVALID, "a forest of %d trees and %d nodes: start, weight, feature, threshold, left, right and "
@@ -3705,30 +3714,17 @@ int lo_gb_predict(lo_ctx *ctx, const lo_table *x, int64_t ld, int32_t k, int64_t
         LO_TRY(check_tree_nodes(feature, left, right, lo, hi, k));
         if (!std::isfinite(weight[t])) return fail(LO_ERR_INVALID, "weight[%d] = %g is not finite", t, weight[t]);
     }
-    int direct = 0;
-    if (eval) {
-        if (prob || raw || pred) return fail(LO_ERR_INVALID, "evaluate writes no rows: prob, raw and pred must be NULL");
-        LO_TRY(check_nb_classes(eval_labels, neval, "eval_labels", &direct));
-        std::fill(confusion_out, confusion_out + (size_t)neval * 2, (int64_t)0);
-    } else {
-        if (y || eval_labels) return fail(LO_ERR_INVALID, "y and eval_labels go with confusion_out");
-        neval = 0;
-        LO_TRY(check_float_table(ctx, prob, LO_F64, n * 2, "prob"));
-        LO_TRY(check_float_table(ctx, pred, LO_F64, n, "pred"));
-        if (raw) LO_TRY(check_float_table(ctx, raw, LO_F64, n * 2, "raw"));
-    }
-    HostCall c(ctx, eval ? "gb_evaluate" : "gb_predict");
+    LO_TRY(f.check_out(ctx, n, 2, prob, raw, pred));
+    HostCall c(ctx, f.call("gb"));
     if (n == 0) return c.finish(timing);
     const int64_t forest_bytes = ((int64_t)2 * M + ntrees) * 8 + ((int64_t)3 * M + ntrees) * 4;
-    const int64_t evl_bytes = (int64_t)neval * 8, hist_bytes = eval ? (int64_t)neval * 2 * 4 : 0;
+    const int64_t evl_bytes = (int64_t)f.neval * 8, hist_bytes = (int64_t)f.neval * 2 * 4;
     const bool forest_smem = forest_bytes + evl_bytes <= lo::kDtTreeSmem;
     const int64_t fixed = (forest_smem ? forest_bytes : 0) + evl_bytes;
-    const bool hist_smem = eval && fixed + hist_bytes <= lo::kDtTreeSmem;
+    const bool hist_smem = f.eval && fixed + hist_bytes <= lo::kDtTreeSmem;
     const int smem = (int)(fixed + (hist_smem ? hist_bytes : 0));
     int *d_int = nullptr;
-    double *d_dbl = nullptr, *d_evl = nullptr;
-    unsigned long long *conf = nullptr;
-    RefusedCell bad;
+    double *d_dbl = nullptr;
     c.alloc(&d_int, ((size_t)3 * M + ntrees) * 4);
     c.alloc(&d_dbl, ((size_t)2 * M + ntrees) * 8);
     c.to_dev(d_int, feature, (size_t)M * 4);
@@ -3738,20 +3734,10 @@ int lo_gb_predict(lo_ctx *ctx, const lo_table *x, int64_t ld, int32_t k, int64_t
     c.to_dev(d_dbl, threshold, (size_t)M * 8);
     c.to_dev(d_dbl + M, value, (size_t)M * 8);
     c.to_dev(d_dbl + 2 * M, weight, (size_t)ntrees * 8);
-    if (eval) {
-        c.alloc(&d_evl, (size_t)neval * 8);
-        c.alloc(&conf, (size_t)neval * 2 * 8);
-        c.to_dev(d_evl, eval_labels, (size_t)neval * 8);
-        c.memset(conf, 0, (size_t)neval * 2 * 8);
-        bad.arm(c);
-    }
+    f.stage(c);
     auto go = [&](auto kernel, auto tag) {
         using T = decltype(tag);
-        int per_sm = 0;
-        c.run([&] { return cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem); });
-        c.run([&] { return cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, lo::kDtThreads, smem); });
-        const int grid = (int)std::min<int64_t>((n + lo::kDtThreads - 1) / lo::kDtThreads,
-                                                (int64_t)ctx->sm_count * std::max(1, per_sm));
+        const int grid = f.grid(c, kernel, lo::kDtThreads, smem, (n + lo::kDtThreads - 1) / lo::kDtThreads);
         c.mark();
         c.launch(1, [&] {
             kernel<<<grid, lo::kDtThreads, smem, c.s>>>((const T *)x->base, ld, k, n, ntrees, M, d_int + 3 * M, d_dbl + 2 * M,
@@ -3759,22 +3745,17 @@ int lo_gb_predict(lo_ctx *ctx, const lo_table *x, int64_t ld, int32_t k, int64_t
                                                         forest_smem ? 1 : 0, prob ? (double *)prob->base : nullptr,
                                                         raw ? (double *)raw->base : nullptr,
                                                         pred ? (double *)pred->base : nullptr,
-                                                        y ? (const T *)y->base : nullptr, d_evl, neval, direct, conf,
-                                                        hist_smem ? 1 : 0, bad.word);
+                                                        y ? (const T *)y->base : nullptr, f.d_evl, f.neval, f.direct, f.conf,
+                                                        hist_smem ? 1 : 0, f.bad.word);
         });
         c.mark();
     };
     if (x->dtype == LO_F32) {
-        if (eval) go(lo::k_gb_predict<float, true>, 0.0f); else go(lo::k_gb_predict<float, false>, 0.0f);
+        if (f.eval) go(lo::k_gb_predict<float, true>, 0.0f); else go(lo::k_gb_predict<float, false>, 0.0f);
     } else {
-        if (eval) go(lo::k_gb_predict<double, true>, 0.0); else go(lo::k_gb_predict<double, false>, 0.0);
+        if (f.eval) go(lo::k_gb_predict<double, true>, 0.0); else go(lo::k_gb_predict<double, false>, 0.0);
     }
-    if (eval) c.to_host(confusion_out, conf, (size_t)neval * 2 * 8);
-    bad.read(c);
-    LO_TRY(c.finish(timing));
-    if (!bad.found(k, info)) return LO_OK;
-    std::fill(confusion_out, confusion_out + (size_t)neval * 2, (int64_t)0);
-    return fail(LO_ERR_INVALID, "row %lld: its label is not one of the evaluated labels", (long long)info->bad_row);
+    return f.finish(c, k, info, timing);
 }
 
 }  // extern "C"

@@ -39,6 +39,41 @@ __device__ __forceinline__ int nb_class(double v, const double *cls, int C, bool
     return lo < C && cls[lo] == v ? lo : -1;
 }
 
+// The confusion counts of an evaluate pass (the EVAL form of k_nb_predict, k_dt_predict and k_gb_predict): CO
+// predictions per label, NT threads per CTA.  The kernel places evl ([neval] f64) and hist ([neval][CO] u32) in its
+// shared memory.  stage() copies eval_labels to evl and, with smem, zeroes hist; the kernel syncs before the first
+// count.  count() adds a row's (label slot, prediction) to hist (smem) or straight to confusion, or keeps the lowest key
+// cell_key(row, k, k) of a label that is not in eval_labels.  finish() reports that key to *err and flushes hist into
+// confusion with integer atomics.
+template <int NT>
+struct Confusion {
+    double *evl;
+    unsigned *hist;
+    unsigned long long *confusion;
+    int neval, CO, direct, smem;
+    unsigned long long bad = ~0ull;
+
+    __device__ __forceinline__ void stage(const double *eval_labels) {
+        for (int i = threadIdx.x; i < neval; i += NT) evl[i] = eval_labels[i];
+        if (smem)
+            for (int i = threadIdx.x; i < neval * CO; i += NT) hist[i] = 0;
+    }
+    __device__ __forceinline__ void count(double label, int p, long long row, int k) {
+        const int a = nb_class(label, evl, neval, direct);
+        if (a < 0) bad = min(bad, cell_key(row, k, k));
+        else if (smem) atomicAdd(&hist[a * CO + p], 1u);
+        else atomicAdd(&confusion[(size_t)a * CO + p], 1ull);
+    }
+    __device__ __forceinline__ void finish(unsigned long long *err) {
+        report_cell(bad, err);
+        if (smem) {
+            __syncthreads();
+            for (int i = threadIdx.x; i < neval * CO; i += NT)
+                if (hist[i]) atomicAdd(&confusion[i], (unsigned long long)hist[i]);
+        }
+    }
+};
+
 // an LO_F32 label vector widened to f64 for the group-by of lo_nb_labels (exact)
 __global__ void __launch_bounds__(256) k_nb_widen(const float *__restrict__ in, long long n, double *__restrict__ out) {
     for (long long i = blockIdx.x * 256ll + threadIdx.x; i < n; i += (long long)gridDim.x * 256) out[i] = (double)in[i];
@@ -239,13 +274,11 @@ __device__ __noinline__ int lr_softmax(double *raw, int C) {
 // of kNbTile rows, one row per thread: chunks of kNbChunk columns are staged as f64 (row stride kNbChunk + 1, so the
 // threads' rows fall on different banks), the raw values of classes c0 .. c0 + kNbBlock are carried in registers over a
 // chunk and parked in raws (shared memory when it fits, else this CTA's slice of global scratch; [c * kNbTile + t]).
-// !EVAL: raw (optional), probability and prediction of every row, with streaming stores.  EVAL: nothing per row; the
-// row's label slot a in eval_labels (direct or binary search) and its prediction p count in hist[a * C + p] (shared
-// memory when it fits, flushed once per CTA with integer atomics; else straight into confusion); a label that is not in
-// eval_labels gives the key cell_key(row, k, k) to *err.  mode picks the epilogue (lo_lr_predict): kNbSoftmax NaiveBayes'
-// nb_softmax; kLrBinomial (C = 1, theta the coefficients, pi the intercept) the one raw value m gives two outputs, raw
-// [-m, m], probability [1 - p1, p1] with p1 = lr_sigmoid(m), and prediction p1 > threshold, hist and confusion with 2
-// columns; kLrMultinomial lr_softmax.  A flag rather than a template parameter: the branch is uniform over the launch,
+// !EVAL: raw (optional), probability and prediction of every row, with streaming stores.  EVAL: nothing per row; each
+// row's (label, prediction) counts in a Confusion whose evl and hist follow the tables.  mode picks the epilogue
+// (lo_lr_predict): kNbSoftmax NaiveBayes' nb_softmax; kLrBinomial (C = 1, theta the coefficients, pi the intercept) the
+// one raw value m gives two outputs, raw [-m, m], probability [1 - p1, p1] with p1 = lr_sigmoid(m), and prediction p1 >
+// threshold, with 2 confusion columns; kLrMultinomial lr_softmax.  A flag rather than a template parameter: the branch is uniform over the launch,
 // and the tiling, staging and dot loop stay one copy per (T, EVAL).
 enum { kNbSoftmax = 0, kLrBinomial = 1, kLrMultinomial = 2 };
 template <typename T, bool EVAL>
@@ -267,17 +300,13 @@ __global__ void __launch_bounds__(kNbTile) k_nb_predict(const T *__restrict__ x,
     double *evl = xt + kNbTile * (kNbChunk + 1);            // [neval] (EVAL)
     double *raws = raws_global ? raws_global + (size_t)blockIdx.x * C * kNbTile : evl + (EVAL ? neval : 0);
     unsigned *hist = reinterpret_cast<unsigned *>(evl + (EVAL ? neval : 0) + (raws_global ? 0 : (size_t)C * kNbTile));
+    Confusion<kNbTile> cm{evl, hist, confusion, neval, CO, direct, hist_in_smem};
     for (int i = threadIdx.x; i < k * C; i += kNbTile) th[i] = theta_t[i];
     for (int i = threadIdx.x; i < C; i += kNbTile) pis[i] = pi[i];
-    if (EVAL) {
-        for (int i = threadIdx.x; i < neval; i += kNbTile) evl[i] = eval_labels[i];
-        if (hist_in_smem)
-            for (int i = threadIdx.x; i < neval * CO; i += kNbTile) hist[i] = 0;
-    }
+    if (EVAL) cm.stage(eval_labels);
     const int t = threadIdx.x, warp = t >> 5, lane = t & 31;
     const uint64_t pol = l2_evict_first_policy();
     const long long ntiles = (n + kNbTile - 1) / kNbTile;
-    unsigned long long bad = ~0ull;
     for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
         const long long row0 = tile * kNbTile;
         const int nr = (int)min((long long)kNbTile, n - row0);
@@ -330,23 +359,10 @@ __global__ void __launch_bounds__(kNbTile) k_nb_predict(const T *__restrict__ x,
             if (!EVAL)
                 for (int c = 0; c < C; ++c) __stcs(prob + row * C + c, rr[c * kNbTile]);
         }
-        if (!EVAL) {
-            __stcs(pred + row, (double)p);
-        } else {
-            const int a = nb_class((double)y[row], evl, neval, direct);
-            if (a < 0) bad = min(bad, cell_key(row, k, k));
-            else if (hist_in_smem) atomicAdd(&hist[a * CO + p], 1u);
-            else atomicAdd(&confusion[(size_t)a * CO + p], 1ull);
-        }
+        if (!EVAL) __stcs(pred + row, (double)p);
+        else cm.count((double)y[row], p, row, k);
     }
-    if (EVAL) {
-        report_cell(bad, err);
-        if (hist_in_smem) {
-            __syncthreads();
-            for (int i = threadIdx.x; i < neval * CO; i += kNbTile)
-                if (hist[i]) atomicAdd(&confusion[i], (unsigned long long)hist[i]);
-        }
-    }
+    if (EVAL) cm.finish(err);
 }
 
 }  // namespace lo

@@ -344,8 +344,8 @@ __global__ void __launch_bounds__(kDtThreads) k_gb_level(const unsigned char *__
 // widened to f64 is <= the node's threshold.  The leaf's class counts (counts[node * C ..]) are the raw values, the
 // probabilities raw_c / sum (IEEE division, sum in c order) and the prediction their first argmax.  The tree's
 // structure sits in shared memory when `tree_smem` (else it is read from global memory).  !EVAL: raw (optional),
-// probability and prediction of every row with streaming stores.  EVAL: nothing per row; (label slot, prediction)
-// counts in hist, as k_nb_predict counts them; a label not in eval_labels gives the key cell_key(row, k, k) to *err.
+// probability and prediction of every row with streaming stores.  EVAL: nothing per row; (label, prediction) counts in
+// a Confusion (naive_bayes.cuh) whose evl and hist follow the tree.
 template <typename T, bool EVAL>
 __global__ void __launch_bounds__(kDtThreads) k_dt_predict(const T *__restrict__ x, long long ld, int k, long long n,
                                                            int M, const int *__restrict__ feat,
@@ -360,7 +360,6 @@ __global__ void __launch_bounds__(kDtThreads) k_dt_predict(const T *__restrict__
     const double *th = thr;
     const int *fe = feat, *le = left, *ri = right;
     double *evl = dt_smem;
-    unsigned *hist = nullptr;
     if (tree_smem) {
         double *ts = dt_smem;
         int *fs = reinterpret_cast<int *>(ts + M);
@@ -376,14 +375,9 @@ __global__ void __launch_bounds__(kDtThreads) k_dt_predict(const T *__restrict__
         ri = fs + 2 * M;
         evl = ts + M + (3 * M + 1) / 2;
     }
-    if (EVAL) {
-        hist = reinterpret_cast<unsigned *>(evl + neval);
-        for (int i = threadIdx.x; i < neval; i += kDtThreads) evl[i] = eval_labels[i];
-        if (hist_in_smem)
-            for (int i = threadIdx.x; i < neval * C; i += kDtThreads) hist[i] = 0;
-    }
+    Confusion<kDtThreads> cm{evl, reinterpret_cast<unsigned *>(evl + neval), confusion, neval, C, direct, hist_in_smem};
+    if (EVAL) cm.stage(eval_labels);
     __syncthreads();
-    unsigned long long bad = ~0ull;
     for (long long r = blockIdx.x * (long long)kDtThreads + threadIdx.x; r < n; r += (long long)gridDim.x * kDtThreads) {
         int node = 0, f;
         while ((f = fe[node]) >= 0) node = (double)x[r * ld + f] <= th[node] ? le[node] : ri[node];
@@ -400,23 +394,10 @@ __global__ void __launch_bounds__(kDtThreads) k_dt_predict(const T *__restrict__
             }
             if (c == 0 || p > top) { best = c; top = p; }
         }
-        if (!EVAL) {
-            __stcs(pred + r, (double)best);
-        } else {
-            const int a = nb_class((double)y[r], evl, neval, direct);
-            if (a < 0) bad = min(bad, cell_key(r, k, k));
-            else if (hist_in_smem) atomicAdd(&hist[a * C + best], 1u);
-            else atomicAdd(&confusion[(size_t)a * C + best], 1ull);
-        }
+        if (!EVAL) __stcs(pred + r, (double)best);
+        else cm.count((double)y[r], best, r, k);
     }
-    if (EVAL) {
-        report_cell(bad, err);
-        if (hist_in_smem) {
-            __syncthreads();
-            for (int i = threadIdx.x; i < neval * C; i += kDtThreads)
-                if (hist[i]) atomicAdd(&confusion[i], (unsigned long long)hist[i]);
-        }
-    }
+    if (EVAL) cm.finish(err);
 }
 
 // GBT's pass after each tree (DESIGN.md §3.6.5), one row per thread.  M == 0 initialises: F = 0, r = y' = 2y - 1.
@@ -455,8 +436,8 @@ __global__ void __launch_bounds__(kDtThreads) k_gb_update(const T *__restrict__ 
 // GBT transform / evaluate, one row per thread: the margin m = sum over trees t (in order, from 0.0) of value[leaf_t] *
 // weight[t], tree t's nodes from start[t] (children as indices into the whole forest).  raw = [-m, m], probability[0]
 // = 1 / (1 + exp(2m)), probability[1] = 1 - probability[0], prediction = m > 0.  The forest sits in shared memory when
-// `forest_smem` (else it is read from global memory).  EVAL: nothing per row; (label slot, prediction) counts, as
-// k_dt_predict counts them.
+// `forest_smem` (else it is read from global memory).  EVAL: nothing per row; (label, prediction) counts in a
+// Confusion, as in k_dt_predict.
 template <typename T, bool EVAL>
 __global__ void __launch_bounds__(kDtThreads) k_gb_predict(const T *__restrict__ x, long long ld, int k, long long n,
                                                            int ntrees, int M, const int *__restrict__ start,
@@ -491,15 +472,9 @@ __global__ void __launch_bounds__(kDtThreads) k_gb_predict(const T *__restrict__
         th = ts, va = vs, wt = ws, fe = fs, le = ls, ri = rs, st = ss;
         hist_at = reinterpret_cast<unsigned *>(ss + ntrees);
     }
-    unsigned *hist = nullptr;
-    if (EVAL) {
-        hist = hist_at;
-        for (int i = threadIdx.x; i < neval; i += kDtThreads) evl[i] = eval_labels[i];
-        if (hist_in_smem)
-            for (int i = threadIdx.x; i < neval * 2; i += kDtThreads) hist[i] = 0;
-    }
+    Confusion<kDtThreads> cm{evl, hist_at, confusion, neval, 2, direct, hist_in_smem};
+    if (EVAL) cm.stage(eval_labels);
     __syncthreads();
-    unsigned long long bad = ~0ull;
     for (long long r = blockIdx.x * (long long)kDtThreads + threadIdx.x; r < n; r += (long long)gridDim.x * kDtThreads) {
         double m = 0.0;
         for (int t = 0; t < ntrees; ++t) {
@@ -518,20 +493,10 @@ __global__ void __launch_bounds__(kDtThreads) k_gb_predict(const T *__restrict__
             }
             __stcs(pred + r, (double)best);
         } else {
-            const int a = nb_class((double)y[r], evl, neval, direct);
-            if (a < 0) bad = min(bad, cell_key(r, k, k));
-            else if (hist_in_smem) atomicAdd(&hist[a * 2 + best], 1u);
-            else atomicAdd(&confusion[(size_t)a * 2 + best], 1ull);
+            cm.count((double)y[r], best, r, k);
         }
     }
-    if (EVAL) {
-        report_cell(bad, err);
-        if (hist_in_smem) {
-            __syncthreads();
-            for (int i = threadIdx.x; i < neval * 2; i += kDtThreads)
-                if (hist[i]) atomicAdd(&confusion[i], (unsigned long long)hist[i]);
-        }
-    }
+    if (EVAL) cm.finish(err);
 }
 
 }  // namespace lo

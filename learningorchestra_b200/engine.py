@@ -1091,29 +1091,37 @@ class Engine:
         :class:`InvalidCellError`.  ``timing``: a dict to receive the call's lo_host_timing fields."""
         pi = np.ascontiguousarray(pi, dtype=np.float64)
         theta = np.ascontiguousarray(theta, dtype=np.float64)
-        nc, n = len(pi), part.nkept
+        nc = len(pi)
         if theta.shape != (nc, part.k):
             raise ValueError(f"theta has shape {theta.shape}, ({nc}, {part.k}) expected")
+        return self._predict(self._lib.lo_nb_predict, (pi.ctypes.data_as(C.c_void_p), theta.ctypes.data_as(C.c_void_p),
+                                                      nc), part, nc, raw, labels, timing)
+
+    def _predict(self, fn, model: tuple, part: AssembledRows, nout: int, raw: bool, labels, timing: dict | None):
+        """The transform / evaluate body of the ``*_predict`` calls: ``fn`` the library's entry point, ``model`` its
+        arguments after (ctx, x, ld, k, n), ``nout`` the outputs per row.  ``labels`` None: a :class:`PredictedRows`;
+        else the int64[len(labels), nout] confusion counts, a label not in ``labels`` raising :class:`InvalidCellError`."""
+        n = part.nkept
         info, t = N.NbInfo(), N.HostTiming()
-        args = (self._ctx, part.x._h, part.k, part.k, n, pi.ctypes.data_as(C.c_void_p), theta.ctypes.data_as(C.c_void_p), nc)
+        args = (self._ctx, part.x._h, part.k, part.k, n, *model)
         if labels is not None:
             if part.y is None:
                 raise ValueError("the rows have no label")
             lab = np.ascontiguousarray(labels, dtype=np.float64)
-            conf = np.zeros((len(lab), nc), np.int64)
-            rc = self._lib.lo_nb_predict(*args, None, None, None, part.y._h, lab.ctypes.data_as(C.c_void_p), len(lab),
-                                         conf.ctypes.data_as(C.c_void_p), C.byref(info), C.byref(t))
+            conf = np.zeros((len(lab), nout), np.int64)
+            rc = fn(*args, None, None, None, part.y._h, lab.ctypes.data_as(C.c_void_p), len(lab),
+                    conf.ctypes.data_as(C.c_void_p), C.byref(info), C.byref(t))
             _check_cells(rc, info, part.k, _EVALUATE_REFUSED)
             _report(timing, t)
             return conf
         with _Owned() as owned:
-            prob = owned.own(self.table("f64", n * nc, 1))
+            prob = owned.own(self.table("f64", n * nout, 1))
             pred = owned.own(self.table("f64", n, 1))
-            rawt = owned.own(self.table("f64", n * nc, 1) if raw else None)
-            N.check(self._lib.lo_nb_predict(*args, prob._h, rawt._h if rawt is not None else None, pred._h, None, None, 0,
-                                            None, C.byref(info), C.byref(t)))
+            rawt = owned.own(self.table("f64", n * nout, 1) if raw else None)
+            N.check(fn(*args, prob._h, rawt._h if rawt is not None else None, pred._h, None, None, 0, None, C.byref(info),
+                       C.byref(t)))
         _report(timing, t)
-        return PredictedRows(prob, rawt, pred, n, nc)
+        return PredictedRows(prob, rawt, pred, n, nout)
 
     def lr_stats(self, part: AssembledRows, timing: dict | None = None) -> "ColumnStats":
         """(n, sum float64[k], m2 float64[k], label_counts int64[LO_NB_MAX_CLASSES]) of ``part``'s n rows
@@ -1164,31 +1172,12 @@ class Engine:
         when binomial), else the int64[len(labels), C] confusion counts.  Binomial: prediction p1 > ``threshold``."""
         coef = np.ascontiguousarray(coef, dtype=np.float64)
         intercept = np.ascontiguousarray(intercept, dtype=np.float64)
-        nc, n = len(intercept), part.nkept
+        nc = len(intercept)
         if coef.shape != (nc, part.k):
             raise ValueError(f"coef has shape {coef.shape}, ({nc}, {part.k}) expected")
-        nout = nc if multinomial else 2
-        info, t = N.NbInfo(), N.HostTiming()
-        args = (self._ctx, part.x._h, part.k, part.k, n, coef.ctypes.data_as(C.c_void_p),
-                intercept.ctypes.data_as(C.c_void_p), nc, int(bool(multinomial)), float(threshold))
-        if labels is not None:
-            if part.y is None:
-                raise ValueError("the rows have no label")
-            lab = np.ascontiguousarray(labels, dtype=np.float64)
-            conf = np.zeros((len(lab), nout), np.int64)
-            rc = self._lib.lo_lr_predict(*args, None, None, None, part.y._h, lab.ctypes.data_as(C.c_void_p), len(lab),
-                                         conf.ctypes.data_as(C.c_void_p), C.byref(info), C.byref(t))
-            _check_cells(rc, info, part.k, _EVALUATE_REFUSED)
-            _report(timing, t)
-            return conf
-        with _Owned() as owned:
-            prob = owned.own(self.table("f64", n * nout, 1))
-            pred = owned.own(self.table("f64", n, 1))
-            rawt = owned.own(self.table("f64", n * nout, 1) if raw else None)
-            N.check(self._lib.lo_lr_predict(*args, prob._h, rawt._h if rawt is not None else None, pred._h, None, None, 0,
-                                            None, C.byref(info), C.byref(t)))
-        _report(timing, t)
-        return PredictedRows(prob, rawt, pred, n, nout)
+        model = (coef.ctypes.data_as(C.c_void_p), intercept.ctypes.data_as(C.c_void_p), nc, int(bool(multinomial)),
+                 float(threshold))
+        return self._predict(self._lib.lo_lr_predict, model, part, nc if multinomial else 2, raw, labels, timing)
 
     def dt_sort(self, part: AssembledRows, j0: int, kc: int, cap: int, timing: dict | None = None) -> "SortedColumns":
         """Columns [j0, j0 + kc) of ``part`` sorted on the device as order-preserving codes (``lo_dt_sort``), with every
@@ -1241,50 +1230,38 @@ class Engine:
         ``binned``'s two tables).  ``shape``: a list to receive the launch shape (16-byte loads, features per chunk,
         nodes per pass, passes).  The whole level comes back to the host, however many node groups the device used.  A
         code >= nbins or a label outside [0, nclasses) raises LoexecError naming the row."""
+        hist = np.zeros((nnodes, part.k, nbins, nclasses), np.int64)
+        return self._level(self._lib.lo_dt_level, (part.y._h, part.nkept, int(nbins), int(nclasses)), part, binned,
+                           splits, nnodes, hist, shape, timing)
+
+    def _level(self, fn, lead: tuple, part: AssembledRows, binned: "BinnedRows", splits, nnodes: int, out: np.ndarray,
+               shape: list | None, timing: dict | None) -> np.ndarray:
+        """The level pass of :meth:`dt_level` / :meth:`gb_level`: ``fn`` the library's entry point, ``lead`` its
+        arguments after (ctx, codes, kp, k), ``out`` the array it fills.  The rows' slots ping-pong between ``binned``'s
+        two tables; ``shape`` receives the launch shape."""
         k = part.k
-        hist = np.zeros((nnodes, k, nbins, nclasses), np.int64)
         sp = np.ascontiguousarray(splits if splits is not None else np.zeros((0, 4)), np.int32)
         src = None if splits is None else binned.slots[binned.cur]
         dst = binned.slots[0 if splits is None else 1 - binned.cur]
         sh = np.zeros(4, np.int32)
         t = N.HostTiming()
-        N.check(self._lib.lo_dt_level(self._ctx, binned.codes._h, code_pitch(k), k, part.y._h, part.nkept, int(nbins),
-                                      int(nclasses), src._h if src is not None else None, int(splits is not None),
-                                      dst._h, len(sp), sp.ctypes.data_as(C.c_void_p), int(nnodes),
-                                      hist.ctypes.data_as(C.c_void_p), sh.ctypes.data_as(C.c_void_p), C.byref(t)))
+        N.check(fn(self._ctx, binned.codes._h, code_pitch(k), k, *lead, src._h if src is not None else None,
+                   int(splits is not None), dst._h, len(sp), sp.ctypes.data_as(C.c_void_p), int(nnodes),
+                   out.ctypes.data_as(C.c_void_p), sh.ctypes.data_as(C.c_void_p), C.byref(t)))
         binned.cur = binned.slots.index(dst)
         if shape is not None:
             shape[:] = [int(v) for v in sh]
         _report(timing, t)
-        return hist
+        return out
 
     def dt_predict(self, part: AssembledRows, tree, raw: bool = False, labels=None, timing: dict | None = None):
         """A tree (:class:`~tree.Tree`) over ``part`` (``lo_dt_predict``), as :meth:`nb_predict`: ``labels`` None gives a
         :class:`PredictedRows` of C columns, else the int64[len(labels), C] confusion counts."""
-        n, C_ = part.nkept, tree.num_classes
         arrs = [np.ascontiguousarray(a, dt) for a, dt in ((tree.feature, np.int32), (tree.threshold, np.float64),
                                                           (tree.left, np.int32), (tree.right, np.int32),
                                                           (tree.counts, np.float64))]
-        info, t = N.NbInfo(), N.HostTiming()
-        args = (self._ctx, part.x._h, part.k, part.k, n, tree.num_nodes, *[a.ctypes.data_as(C.c_void_p) for a in arrs], C_)
-        if labels is not None:
-            if part.y is None:
-                raise ValueError("the rows have no label")
-            lab = np.ascontiguousarray(labels, dtype=np.float64)
-            conf = np.zeros((len(lab), C_), np.int64)
-            rc = self._lib.lo_dt_predict(*args, None, None, None, part.y._h, lab.ctypes.data_as(C.c_void_p), len(lab),
-                                         conf.ctypes.data_as(C.c_void_p), C.byref(info), C.byref(t))
-            _check_cells(rc, info, part.k, _EVALUATE_REFUSED)
-            _report(timing, t)
-            return conf
-        with _Owned() as owned:
-            prob = owned.own(self.table("f64", max(n * C_, 1), 1))
-            pred = owned.own(self.table("f64", max(n, 1), 1))
-            rawt = owned.own(self.table("f64", max(n * C_, 1), 1) if raw else None)
-            N.check(self._lib.lo_dt_predict(*args, prob._h, rawt._h if rawt is not None else None, pred._h, None, None, 0,
-                                            None, C.byref(info), C.byref(t)))
-        _report(timing, t)
-        return PredictedRows(prob, rawt, pred, n, C_)
+        model = (tree.num_nodes, *[a.ctypes.data_as(C.c_void_p) for a in arrs], tree.num_classes)
+        return self._predict(self._lib.lo_dt_predict, model, part, tree.num_classes, raw, labels, timing)
 
     def gb_update(self, part: AssembledRows, rows: "BoostRows | None" = None, tree=None, weight: float = 1.0,
                   timing: dict | None = None) -> "BoostRows":
@@ -1313,22 +1290,9 @@ class Engine:
         """One regression-tree level over ``part``'s rows (``lo_gb_level``), routed as :meth:`dt_level`: uint64 (nnodes, k,
         nbins, LO_GB_WORDS) words of (node slot, feature, bin) — the count and the 128-bit fixed-point sums of the rows'
         residuals and their squares (:func:`tree.word_stats` reads them)."""
-        k = part.k
-        words = np.zeros((nnodes, k, nbins, N.LO_GB_WORDS), np.uint64)
-        sp = np.ascontiguousarray(splits if splits is not None else np.zeros((0, 4)), np.int32)
-        src = None if splits is None else binned.slots[binned.cur]
-        dst = binned.slots[0 if splits is None else 1 - binned.cur]
-        sh = np.zeros(4, np.int32)
-        t = N.HostTiming()
-        N.check(self._lib.lo_gb_level(self._ctx, binned.codes._h, code_pitch(k), k, rows.residual._h, part.nkept,
-                                      int(nbins), src._h if src is not None else None, int(splits is not None),
-                                      dst._h, len(sp), sp.ctypes.data_as(C.c_void_p), int(nnodes),
-                                      words.ctypes.data_as(C.c_void_p), sh.ctypes.data_as(C.c_void_p), C.byref(t)))
-        binned.cur = binned.slots.index(dst)
-        if shape is not None:
-            shape[:] = [int(v) for v in sh]
-        _report(timing, t)
-        return words
+        words = np.zeros((nnodes, part.k, nbins, N.LO_GB_WORDS), np.uint64)
+        return self._level(self._lib.lo_gb_level, (rows.residual._h, part.nkept, int(nbins)), part, binned, splits,
+                           nnodes, words, shape, timing)
 
     def gb_predict(self, part: AssembledRows, trees, weights, raw: bool = False, labels=None,
                    timing: dict | None = None):
@@ -1339,28 +1303,9 @@ class Engine:
         w = np.ascontiguousarray(weights, np.float64)
         if len(w) != len(trees):
             raise ValueError(f"{len(w)} weights for {len(trees)} trees")
-        n = part.nkept
-        info, t = N.NbInfo(), N.HostTiming()
-        args = (self._ctx, part.x._h, part.k, part.k, n, len(trees), start.ctypes.data_as(C.c_void_p),
-                w.ctypes.data_as(C.c_void_p), M, *[a.ctypes.data_as(C.c_void_p) for a in arrs])
-        if labels is not None:
-            if part.y is None:
-                raise ValueError("the rows have no label")
-            lab = np.ascontiguousarray(labels, dtype=np.float64)
-            conf = np.zeros((len(lab), 2), np.int64)
-            rc = self._lib.lo_gb_predict(*args, None, None, None, part.y._h, lab.ctypes.data_as(C.c_void_p), len(lab),
-                                         conf.ctypes.data_as(C.c_void_p), C.byref(info), C.byref(t))
-            _check_cells(rc, info, part.k, _EVALUATE_REFUSED)
-            _report(timing, t)
-            return conf
-        with _Owned() as owned:
-            prob = owned.own(self.table("f64", max(n * 2, 1), 1))
-            pred = owned.own(self.table("f64", max(n, 1), 1))
-            rawt = owned.own(self.table("f64", max(n * 2, 1), 1) if raw else None)
-            N.check(self._lib.lo_gb_predict(*args, prob._h, rawt._h if rawt is not None else None, pred._h, None, None, 0,
-                                            None, C.byref(info), C.byref(t)))
-        _report(timing, t)
-        return PredictedRows(prob, rawt, pred, n, 2)
+        model = (len(trees), start.ctypes.data_as(C.c_void_p), w.ctypes.data_as(C.c_void_p), M,
+                 *[a.ctypes.data_as(C.c_void_p) for a in arrs])
+        return self._predict(self._lib.lo_gb_predict, model, part, 2, raw, labels, timing)
 
     def value_counts_f64_host(self, values: np.ndarray):
         """(keys float64[g], counts uint64[g]) — exact value counts of a numeric column (GPU hash group-by),

@@ -560,6 +560,28 @@ class ShardedEngine:
             raise other[0]
         raise min((e.moved(first_rows[i]) for i, e in failed), key=lambda e: (e.row, e.position))
 
+    def _summed(self, what: str, fn, first_rows=None, add=None, shape: list | None = None):
+        """``fn(i)`` on every member through :meth:`_each`, the results added in shard order: by ``add(total, r)``, else
+        ``+`` (item by item over a tuple), so integer sums do not depend on the cut.  With ``shape``, ``fn(i, s)`` fills
+        a list s of its own and ``shape`` receives the first member's."""
+        shapes = [[] for _ in range(self.nlocal)]
+        got = self._each(what, fn if shape is None else lambda i: fn(i, shapes[i]), first_rows=first_rows)
+        if shape is not None:
+            shape[:] = shapes[0]
+        add = add or (lambda a, b: tuple(x + y for x, y in zip(a, b)) if isinstance(a, tuple) else a + b)
+        total = got[0]
+        for r in got[1:]:
+            total = add(total, r)
+        return total
+
+    def _predicted(self, what: str, fn, parts, labels):
+        """A ``*_predict`` call ``fn(i)`` on every member: transform (``labels`` None) gives one ``PredictedRows`` per
+        member, evaluate the members' confusion counts summed; a refused row is raised as the lowest over all shards,
+        its row global."""
+        if labels is None:
+            return self._each(what, fn, undo=lambda p: p.free(), first_rows=_firsts(parts))
+        return self._summed(what, fn, first_rows=_firsts(parts))
+
     def parse_text_into(self, table: ShardedTable, col: int, text: ShardedText) -> dict:
         """``Engine.parse_text_into`` over a sharded table: piece i of ``text`` and shard i of ``table`` hold the same rows
         (both cut at :meth:`bounds`), so every member parses its piece into its shard on its own device, from a host
@@ -758,24 +780,14 @@ class ShardedEngine:
         the sums and counts are added on the host in shard order, so integer-valued features give the single-GPU sums
         bit for bit.  A refused row is raised as the lowest over all shards, its row global (rows of the earlier shards
         counted first)."""
-        got = self._each("nb_fit", lambda i: self.engines[i].nb_fit(parts[i], classes), first_rows=_firsts(parts))
-        sums, counts = got[0]
-        for s, c in got[1:]:
-            sums, counts = sums + s, counts + c
-        return sums, counts
+        return self._summed("nb_fit", lambda i: self.engines[i].nb_fit(parts[i], classes), first_rows=_firsts(parts))
 
     def nb_predict(self, parts, pi, theta, raw: bool = False, labels=None):
         """``Engine.nb_predict`` over the shards, each on its own device from a host thread of its own.  Transform: one
         ``PredictedRows`` per member.  Evaluate (``labels``): the members' confusion counts summed; a refused row is
         raised as the lowest over all shards, its row global."""
-        got = self._each("nb_predict", lambda i: self.engines[i].nb_predict(parts[i], pi, theta, raw, labels),
-                         undo=(lambda p: p.free()) if labels is None else None, first_rows=_firsts(parts))
-        if labels is None:
-            return got
-        confusion = got[0]
-        for c in got[1:]:
-            confusion = confusion + c
-        return confusion
+        return self._predicted("nb_predict", lambda i: self.engines[i].nb_predict(parts[i], pi, theta, raw, labels),
+                               parts, labels)
 
     def lr_stats(self, parts):
         """``Engine.lr_stats`` over the shards, each on its own device from a host thread of its own.  Returns (n, sum,
@@ -802,25 +814,16 @@ class ShardedEngine:
     def lr_loss_grad(self, parts, coef, intercept, multinomial: bool):
         """``Engine.lr_loss_grad`` over the shards, each on its own device from a host thread of its own; the loss and
         the gradient sums added on the host in shard order."""
-        got = self._each("lr_loss_grad", lambda i: self.engines[i].lr_loss_grad(parts[i], coef, intercept, multinomial))
-        loss, grad, icpt = got[0]
-        for lo_, g, b in got[1:]:
-            loss, grad, icpt = loss + lo_, grad + g, icpt + b
-        return loss, grad, icpt
+        return self._summed("lr_loss_grad", lambda i: self.engines[i].lr_loss_grad(parts[i], coef, intercept,
+                                                                                   multinomial))
 
     def lr_predict(self, parts, coef, intercept, multinomial: bool, threshold: float = 0.5, raw: bool = False,
                    labels=None):
         """``Engine.lr_predict`` over the shards, as :meth:`nb_predict`: one ``PredictedRows`` per member, or the
         members' confusion counts summed."""
-        got = self._each("lr_predict", lambda i: self.engines[i].lr_predict(parts[i], coef, intercept, multinomial,
-                                                                            threshold, raw, labels),
-                         undo=(lambda p: p.free()) if labels is None else None, first_rows=_firsts(parts))
-        if labels is None:
-            return got
-        confusion = got[0]
-        for c in got[1:]:
-            confusion = confusion + c
-        return confusion
+        return self._predicted("lr_predict", lambda i: self.engines[i].lr_predict(parts[i], coef, intercept, multinomial,
+                                                                                  threshold, raw, labels),
+                               parts, labels)
 
     def dt_sort(self, parts, j0: int, kc: int, cap: int) -> list:
         """``Engine.dt_sort`` on every member, each on its own device from a host thread of its own: one
@@ -829,11 +832,7 @@ class ShardedEngine:
 
     def dt_rank(self, sorted_cols: list, cols, codes):
         """``Engine.dt_rank`` on every member's sorted columns; the counts added in shard order: ranks in the union."""
-        got = self._each("dt_rank", lambda i: self.engines[i].dt_rank(sorted_cols[i], cols, codes))
-        lt, le = got[0]
-        for a, b in got[1:]:
-            lt, le = lt + a, le + b
-        return lt, le
+        return self._summed("dt_rank", lambda i: self.engines[i].dt_rank(sorted_cols[i], cols, codes))
 
     def dt_bin(self, parts, thresholds) -> list:
         """``Engine.dt_bin`` on every member: one ``BinnedRows`` per member."""
@@ -842,27 +841,14 @@ class ShardedEngine:
     def dt_level(self, parts, binned: list, nbins: int, nclasses: int, splits, nnodes: int, shape: list | None = None):
         """``Engine.dt_level`` on every member over the same splits; the integer histograms added in shard order, so
         they do not depend on the cut.  ``shape`` receives the first member's launch shape."""
-        shapes = [[] for _ in parts]
-        got = self._each("dt_level", lambda i: self.engines[i].dt_level(parts[i], binned[i], nbins, nclasses, splits,
-                                                                        nnodes, shapes[i]))
-        if shape is not None:
-            shape[:] = shapes[0]
-        hist = got[0]
-        for h in got[1:]:
-            hist = hist + h
-        return hist
+        return self._summed("dt_level", lambda i, sh=None: self.engines[i].dt_level(parts[i], binned[i], nbins, nclasses,
+                                                                                    splits, nnodes, sh), shape=shape)
 
     def dt_predict(self, parts, tree, raw: bool = False, labels=None):
         """``Engine.dt_predict`` over the shards, as :meth:`nb_predict`: one ``PredictedRows`` per member, or the
         members' confusion counts summed; a refused row is raised as the lowest over all shards, its row global."""
-        got = self._each("dt_predict", lambda i: self.engines[i].dt_predict(parts[i], tree, raw, labels),
-                         undo=(lambda p: p.free()) if labels is None else None, first_rows=_firsts(parts))
-        if labels is None:
-            return got
-        confusion = got[0]
-        for c in got[1:]:
-            confusion = confusion + c
-        return confusion
+        return self._predicted("dt_predict", lambda i: self.engines[i].dt_predict(parts[i], tree, raw, labels), parts,
+                               labels)
 
     def gb_update(self, parts, rows: list | None = None, tree=None, weight: float = 1.0) -> list:
         """``Engine.gb_update`` on every member: one ``BoostRows`` per member (made when ``rows`` is None); a refused
@@ -875,27 +861,15 @@ class ShardedEngine:
         """``Engine.gb_level`` on every member over the same splits; the 128-bit words added as integers in shard order
         (:func:`tree.add_words`), so they do not depend on the cut.  ``shape`` receives the first member's launch shape."""
         from .tree import add_words
-        shapes = [[] for _ in parts]
-        got = self._each("gb_level", lambda i: self.engines[i].gb_level(parts[i], binned[i], rows[i], nbins, splits,
-                                                                        nnodes, shapes[i]))
-        if shape is not None:
-            shape[:] = shapes[0]
-        words = got[0]
-        for w in got[1:]:
-            words = add_words(words, w)
-        return words
+        return self._summed("gb_level", lambda i, sh=None: self.engines[i].gb_level(parts[i], binned[i], rows[i], nbins,
+                                                                                    splits, nnodes, sh),
+                            add=add_words, shape=shape)
 
     def gb_predict(self, parts, trees, weights, raw: bool = False, labels=None):
         """``Engine.gb_predict`` over the shards, as :meth:`nb_predict`: one ``PredictedRows`` per member, or the
         members' confusion counts summed; a refused row is raised as the lowest over all shards, its row global."""
-        got = self._each("gb_predict", lambda i: self.engines[i].gb_predict(parts[i], trees, weights, raw, labels),
-                         undo=(lambda p: p.free()) if labels is None else None, first_rows=_firsts(parts))
-        if labels is None:
-            return got
-        confusion = got[0]
-        for c in got[1:]:
-            confusion = confusion + c
-        return confusion
+        return self._predicted("gb_predict", lambda i: self.engines[i].gb_predict(parts[i], trees, weights, raw, labels),
+                               parts, labels)
 
     @property
     def resident(self):

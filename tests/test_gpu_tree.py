@@ -215,6 +215,27 @@ def test_class_cap_at_its_boundary(engine):
         _free(parts)
 
 
+@pytest.mark.parametrize("cuts", [1, 3])
+def test_evaluate_counts_on_both_routes(engine, cuts):
+    """100 classes: their 100 labels' counts (39 KiB) sit in shared memory beside the tree; 300 evaluated labels (117
+    KiB, past kDtTreeSmem = 96 KiB) are counted straight into global memory."""
+    x, y = _data(3000, 3, 2, seed=8)
+    y[:98] = np.arange(2, 100)
+    m, root = _check_fit(engine, x, y, cuts, max_depth=3)
+    assert m.num_classes == 100
+    _raw, _prob, pred = to.transform(root, x)
+    y_eval = (np.arange(len(y)) % 300) * 0.5
+    feats, parts = _on(engine, x, y_eval, cuts)
+    try:
+        ev = m.evaluate(feats)
+    finally:
+        _free(parts)
+    labels = np.unique(y_eval)
+    want = np.zeros((len(labels), 100), np.int64)
+    np.add.at(want, (np.searchsorted(labels, y_eval), pred.astype(np.int64)), 1)
+    np.testing.assert_array_equal(ev["confusion"], want)
+
+
 def test_equal_adjacent_thresholds_fit_like_spark(engine):
     """Midpoints of three neighbouring doubles round to one value: two equal thresholds, binned by Java's binary search."""
     rng = np.random.default_rng(21)
