@@ -670,6 +670,35 @@ int lo_gb_predict(lo_ctx *ctx, const lo_table *x, int64_t ld, int32_t k, int64_t
                   lo_table *pred, const lo_table *y, const double *eval_labels, int32_t neval, int64_t *confusion_out,
                   lo_nb_info *info, lo_host_timing *timing);
 
+/* Spark 2.4's RandomForestClassifier over the matrix of lo_assemble_rows (DESIGN.md §3.6.6): many classification trees
+ * grown together on lo_dt_bin's codes, each row counted in each tree with a bagging weight drawn from a counter-based
+ * hash, each node over its own feature subset.  The features and labels are first checked by lo_lr_stats_range.
+ *
+ * lo_rf_level: one level of trees tree0 .. tree0 + ntrees - 1, as lo_dt_level with these differences.  Row r's slot in
+ *   batch tree t is src[t * n + r] / dst[t * n + r] (LO_I32 tables of >= ntrees * n), numbered across the batch in tree
+ *   order, as are the parents' splits; without src (route 0) row r is at slot t of tree t, so nnodes = ntrees.  The
+ *   row's weight in tree t is #{j : u >= draw[j]} over the ascending table draw[0 .. ndraw) (ndraw in [1,
+ *   LO_RF_MAX_DRAWS]), u = mix(mix(mix(seed) ^ (tree0 + t)) ^ (row0 + r)) with mix splitmix64's step (add
+ *   0x9E3779B97F4A7C15, then its finaliser), row0 the global index of row 0; a row of weight 0 is not counted.  Node s
+ *   counts only its m features features[s * m .. + m) (in [0, k)): hist_out (host int64[nnodes][m][nbins][nclasses]) =
+ *   the weights of each (slot, listed feature, bin, class).  m * nbins * nclasses * 8 above LO_DT_PASS_HIST is refused.
+ *   The counts are integers: they depend on neither the batch, the node groups nor the grid.
+ * lo_rf_predict: a forest of ntrees trees (nodes [start[t], start[t + 1]) of the arrays of lo_dt_predict, children as
+ *   indices into them; start[0] = 0) with votes (f64 [nnodes][nclasses], a leaf's counts over their total, 0 for a leaf
+ *   of no counts), as lo_dt_predict's transform and evaluate: raw_c = the sum of the rows' leaves' votes in tree order
+ *   from 0.0, probability = raw / sum (IEEE division), prediction = the first argmax of raw. */
+#define LO_RF_MAX_DRAWS    32           /* entries of a bagging threshold table */
+int lo_rf_level(lo_ctx *ctx, const lo_table *codes, int64_t kp, int32_t k, const lo_table *y, int64_t n, int64_t row0,
+                int32_t nbins, int32_t nclasses, uint64_t seed, int32_t tree0, int32_t ntrees, const uint64_t *draw,
+                int32_t ndraw, const int32_t *features, int32_t m, const lo_table *src, int32_t route, lo_table *dst,
+                int32_t nparents, const int32_t *splits, int32_t nnodes, int64_t *hist_out, int32_t *shape_out,
+                lo_host_timing *timing);
+int lo_rf_predict(lo_ctx *ctx, const lo_table *x, int64_t ld, int32_t k, int64_t n, int32_t ntrees, const int32_t *start,
+                  int32_t nnodes, const int32_t *feature, const double *threshold, const int32_t *left,
+                  const int32_t *right, const double *votes, int32_t nclasses, lo_table *prob, lo_table *raw,
+                  lo_table *pred, const lo_table *y, const double *eval_labels, int32_t neval, int64_t *confusion_out,
+                  lo_nb_info *info, lo_host_timing *timing);
+
 /* Number -> text for one column: the reference's "string" cast, str(v) / None -> "" (data_type_handler_image/
  * data_type_update.py:22-28), for every cell at once on the GPU.  The inverse of lo_parse_number_host.
  * status[i] uses the LO_NUM_* codes above: FLOAT -> repr(float) (shortest round-trip digits, CPython's notation),

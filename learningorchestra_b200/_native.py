@@ -44,6 +44,7 @@ LO_DT_MAX_BINS = 256
 LO_DT_MAX_CLASSES = 100
 LO_DT_PASS_HIST = 1 << 30
 LO_GB_WORDS = 5
+LO_RF_MAX_DRAWS = 32
 LO_ABI_VERSION = 7
 
 _ERR_NAMES = {
@@ -204,6 +205,11 @@ SIGNATURES = {
                                _P, C.POINTER(NbInfo), C.POINTER(HostTiming)]),
     "lo_gb_predict": (C.c_int, [_P, _P, C.c_int64, C.c_int32, C.c_int64, C.c_int32, _P, _P, C.c_int32, _P, _P, _P, _P, _P,
                                 _P, _P, _P, _P, _P, C.c_int32, _P, C.POINTER(NbInfo), C.POINTER(HostTiming)]),
+    "lo_rf_level": (C.c_int, [_P, _P, C.c_int64, C.c_int32, _P, C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.c_uint64,
+                              C.c_int32, C.c_int32, _P, C.c_int32, _P, C.c_int32, _P, C.c_int32, _P, C.c_int32, _P,
+                              C.c_int32, _P, _P, C.POINTER(HostTiming)]),
+    "lo_rf_predict": (C.c_int, [_P, _P, C.c_int64, C.c_int32, C.c_int64, C.c_int32, _P, C.c_int32, _P, _P, _P, _P, _P,
+                                C.c_int32, _P, _P, _P, _P, _P, C.c_int32, _P, C.POINTER(NbInfo), C.POINTER(HostTiming)]),
     "lo_format_number_host": (C.c_int, [_P, _P, _P, C.c_int64, _P, _P, C.c_int64, C.POINTER(HostTiming)]),
     "lo_parse_text_to_table": (C.c_int, [_P, _P, _P, C.c_int32, C.POINTER(ParseSummary), C.POINTER(HostTiming)]),
     "lo_format_table_to_text": (C.c_int, [_P, _P, C.c_int32, C.POINTER(Validity), C.POINTER(Validity), C.POINTER(_P),

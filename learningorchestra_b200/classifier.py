@@ -1,7 +1,8 @@
-"""The builder's "NB", "LR", "DT" and "GB" classifiers on the GPU: Spark 2.4's multinomial ``NaiveBayes``,
-``LogisticRegression``, ``DecisionTreeClassifier`` and ``GBTClassifier`` (``builder_image/builder.py:55-61``) fitted on,
-applied to and evaluated over the feature matrix in HBM (:meth:`DeviceFrame.features`), on one GPU or on every shard of
-a local :class:`~sharding.ShardedEngine`.  DESIGN.md §3.6.2 to §3.6.5 state the semantics.
+"""The builder's five classifiers on the GPU: Spark 2.4's multinomial ``NaiveBayes`` ("NB"), ``LogisticRegression``
+("LR"), ``DecisionTreeClassifier`` ("DT"), ``GBTClassifier`` ("GB") and ``RandomForestClassifier`` ("RF")
+(``builder_image/builder.py:55-61``) fitted on, applied to and evaluated over the feature matrix in HBM
+(:meth:`DeviceFrame.features`), on one GPU or on every shard of a local :class:`~sharding.ShardedEngine`.  DESIGN.md
+§3.6.2 to §3.6.6 state the semantics.
 
 NaiveBayes: the device computes the class counts and per-class feature sums (``lo_nb_fit``); LogisticRegression: the
 column statistics and label counts (``lo_lr_stats``) and one pass of loss and gradient sums per function evaluation of
@@ -10,7 +11,10 @@ the host's L-BFGS (``lo_lr_loss_grad``, :mod:`lbfgs`).  Both compute every row's
 the evaluator's metrics are computed here, on the host, from those.  DecisionTreeClassifier: the device sorts the
 columns, answers rank queries, bins the values and counts every tree level (``lo_dt_*``); :mod:`tree` chooses the
 thresholds and splits from those counts.  GBTClassifier grows its regression trees on the same codes from exact
-fixed-point residual sums (``lo_gb_level``) and keeps every row's margin and residual on the device (``lo_gb_update``)."""
+fixed-point residual sums (``lo_gb_level``) and keeps every row's margin and residual on the device (``lo_gb_update``).
+RandomForestClassifier grows batches of trees together on the same codes, one pass per level of the whole batch
+(``lo_rf_level``), each row weighted by its counter-based bagging draw and each node over its own feature subset; the
+forest's votes are summed per row on the device (``lo_rf_predict``)."""
 from __future__ import annotations
 
 import math
@@ -563,4 +567,102 @@ class GBTClassificationModel(_Model):
         """Spark's ``model.transform``: every row's ``probability`` ([1 / (1 + exp(2m)), the rest] of the margin m) and
         ``prediction`` (m > 0), and with ``raw`` its ``rawPrediction`` ([-m, m]), written in HBM on the rows' own
         devices."""
+        return super().transform(features, raw)
+
+
+_RF_SLOT_BUDGET = 2 << 30      # bytes of the two int32 slot tables of one batch of trees (ntrees * n rows each)
+
+
+class RandomForestClassifier:
+    """``pyspark.ml.classification.RandomForestClassifier(numTrees, maxDepth, maxBins, minInstancesPerNode,
+    minInfoGain, impurity, featureSubsetStrategy, subsamplingRate, seed)`` with its other defaults (every feature
+    continuous, no ``weightCol``, no ``thresholds``) on the GPU (DESIGN.md §3.6.6).  Bagging and the feature subsets
+    are counter-based hashes of ``seed``, so a forest is the same on one GPU and on any shard cut.  max_bins above
+    LO_DT_MAX_BINS (256) is refused: a bin index is a byte on the device."""
+
+    def __init__(self, num_trees: int = 20, max_depth: int = 5, max_bins: int = 32, min_instances_per_node: int = 1,
+                 min_info_gain: float = 0.0, impurity: str = "gini", feature_subset_strategy: str = "auto",
+                 subsampling_rate: float = 1.0, seed: int | None = None):
+        from . import tree as T
+        self.num_trees = _integer(num_trees, "num_trees", 1)
+        _tree_params(self, max_depth, max_bins, min_instances_per_node, min_info_gain)
+        if not isinstance(impurity, str) or impurity.lower() not in T.IMPURITIES:
+            raise ValueError(f"impurity must be one of {list(T.IMPURITIES)}, not {impurity!r}")
+        self.impurity = impurity.lower()
+        T.subset_size(feature_subset_strategy, 1, self.num_trees)          # refuses an unknown strategy now
+        self.feature_subset_strategy = feature_subset_strategy
+        rate = float(subsampling_rate) if isinstance(subsampling_rate, (int, float, np.floating)) \
+            and not isinstance(subsampling_rate, bool) else float("nan")
+        if not 0.0 < rate <= 1.0:
+            raise ValueError(f"subsampling_rate must lie in (0, 1], not {subsampling_rate!r}")
+        self.subsampling_rate = rate
+        self.seed = T.DEFAULT_SEED if seed is None else _integer(seed, "seed", -(1 << 63), (1 << 63) - 1)
+
+    def fit(self, features) -> "RandomForestClassificationModel":
+        """The forest of ``features`` (:class:`~builder_frontend.Features` with a label, on one GPU or sharded).  Every
+        label must be an integer >= 0 and every feature finite (InvalidCellError naming the ``_id`` and field of the
+        lowest refused row); numClasses = max label + 1.  No row, more than LO_DT_MAX_CLASSES classes or a one-node
+        histogram (m x min(max_bins, n) x C x 8 bytes, m the features a node searches) above LO_DT_PASS_HIST are
+        refused.  The trees grow in batches whose slot tables fit _RF_SLOT_BUDGET, one level pass per batch level."""
+        from . import tree as T
+        name, k = "RandomForestClassifier", len(features.fields)
+        _labelled(features, name)
+        n, _total, _m2, counts = _on_device(features, lambda engine, rows: engine.lr_stats(rows), name=name,
+                                            reasons=_LR_REASONS)
+        _some_rows(n, name)
+        num_classes = int(np.flatnonzero(counts)[-1]) + 1
+        if num_classes > N.LO_DT_MAX_CLASSES:
+            raise N.LoexecError(N.LO_ERR_INVALID, f"{num_classes} classes exceed LO_DT_MAX_CLASSES = "
+                                f"{N.LO_DT_MAX_CLASSES}")
+        m = T.subset_size(self.feature_subset_strategy, k, self.num_trees)
+        if m * min(self.max_bins, n) * num_classes * 8 > N.LO_DT_PASS_HIST:
+            raise N.LoexecError(N.LO_ERR_INVALID, f"{m} features x {min(self.max_bins, n)} bins x {num_classes} classes: "
+                                f"one node's histogram exceeds LO_DT_PASS_HIST = {N.LO_DT_PASS_HIST} bytes")
+        draw = T.draw_table(self.num_trees, self.subsampling_rate)
+        thresholds, _rounds = split_thresholds(features, n, k, self.max_bins, name)
+        nbins = max(len(t) for t in thresholds) + 1
+        batch = max(1, min(self.num_trees, _RF_SLOT_BUDGET // (8 * n)))
+        binned = _on_device(features, lambda engine, rows: engine.dt_bin(rows, thresholds), name=name)
+        trees = []
+        try:
+            for tree0 in range(0, self.num_trees, batch):
+                ntrees = min(batch, self.num_trees - tree0)
+
+                def level(splits, nnodes, feats):
+                    return _on_device(features, lambda engine, rows: engine.rf_level(
+                        rows, binned, nbins, num_classes, self.seed, draw, tree0, ntrees, splits, feats), name=name)
+
+                grown, _shapes = T.grow(level, thresholds, num_classes, self.max_depth, self.impurity,
+                                        self.min_instances_per_node, self.min_info_gain, trees=ntrees,
+                                        subsets=lambda t, node: T.feature_subset(self.seed, tree0 + t, node, k, m))
+                trees += grown
+        finally:
+            _free(binned)
+        model = RandomForestClassificationModel(trees, features.fields, thresholds, m)
+        model.tree_batch = batch
+        return model
+
+
+class RandomForestClassificationModel(_Model):
+    """A fitted random forest, host data: ``trees`` (classification :class:`~tree.Tree` s: the node arrays feature,
+    threshold, left, right, counts (bagging-weighted class counts), prediction, impurity and gain), ``tree_weights``
+    (all 1.0), ``num_classes``, ``total_num_nodes``, the ``fields`` it was fitted on, every column's split
+    ``thresholds``, ``feature_subset`` (the features each node searched) and, after a fit, ``tree_batch`` (the trees
+    grown together per level pass)."""
+    _name, _reasons = "RandomForestClassifier", _LR_REASONS
+
+    def __init__(self, trees, fields, thresholds=None, feature_subset=None):
+        self.trees, self.fields, self.thresholds = list(trees), list(fields), thresholds
+        self.tree_weights = np.ones(len(self.trees))
+        self.num_classes = self.trees[0].num_classes
+        self.total_num_nodes = sum(t.num_nodes for t in self.trees)
+        self.feature_subset = feature_subset
+
+    def _predict(self, engine, rows, raw=False, labels=None):
+        return engine.rf_predict(rows, self.trees, raw=raw, labels=labels)
+
+    def transform(self, features, raw: bool = False) -> "Predictions":
+        """Spark's ``model.transform``: every row's ``rawPrediction`` (with ``raw``; the sum over trees of the leaf's
+        class counts over their total), ``probability`` (raw over its sum) and ``prediction`` (the first argmax of
+        raw, a class index as float64), written in HBM on the rows' own devices."""
         return super().transform(features, raw)

@@ -2658,11 +2658,11 @@ int start_info(const lo_ctx *ctx, lo_nb_info *info) {
     return LO_OK;
 }
 
-// The frame of the transform / evaluate entry points (lo_nb_predict, lo_lr_predict, lo_dt_predict, lo_gb_predict), CO
-// outputs per row.  Evaluate (confusion_out given) writes no rows: the kernel counts (label slot, prediction) into the
-// neval x CO matrix (lo::Confusion) and lowers the refusal word for a label that is not in eval_labels.  Transform
-// writes prob, pred and (when given) raw.  An entry point calls check_x, its model checks, check_out, opens its HostCall
-// as call(prefix), stages its model, then stage, grid and its launch, and returns finish.
+// The frame of the transform / evaluate entry points (lo_nb_predict, lo_lr_predict, lo_dt_predict, lo_gb_predict,
+// lo_rf_predict), CO outputs per row.  Evaluate (confusion_out given) writes no rows: the kernel counts (label slot,
+// prediction) into the neval x CO matrix (lo::Confusion) and lowers the refusal word for a label that is not in
+// eval_labels.  Transform writes prob, pred and (when given) raw.  An entry point calls check_x, its model checks,
+// check_out, opens its HostCall as call(prefix), stages its model, then stage, grid and its launch, and returns finish.
 struct PredictFrame {
     const lo_table *y;
     const double *eval_labels;
@@ -3157,7 +3157,8 @@ int lo_lr_predict(lo_ctx *ctx, const lo_table *x, int64_t ld, int32_t k, int64_t
 }  // extern "C"
 
 static_assert(lo::kDtMaxBins == LO_DT_MAX_BINS && lo::kDtMaxClasses == LO_DT_MAX_CLASSES &&
-              lo::kDtPassHist == LO_DT_PASS_HIST && lo::kGbWords == LO_GB_WORDS, "loexec.h documents the tree's caps");
+              lo::kDtPassHist == LO_DT_PASS_HIST && lo::kGbWords == LO_GB_WORDS && lo::kRfMaxDraws == LO_RF_MAX_DRAWS,
+              "loexec.h documents the tree's caps");
 
 namespace {
 
@@ -3187,16 +3188,18 @@ int check_dt_classes(int32_t nclasses) {
     return LO_OK;
 }
 
-// The launch shape of a level of nnodes nodes (lo_dt_level, lo_gb_level): a feature's histogram of one node takes cell =
-// nbins * C counters of wbytes (lo_dt_level: u32 class counts; lo_gb_level: C = 5 u64 words); a CTA holds gn nodes x fc features of them within kDtHistSmem.  fc is a multiple of 16 (16-byte code
-// loads) when 16 cells fit, else as many single features as fit (scalar loads); gn as many nodes as fit beside, and as
-// keep the pass's u64 histogram within kDtPassHist.  passes = node groups, each one pass over the rows.
+// The launch shape of a level of nnodes nodes (lo_dt_level, lo_gb_level, lo_rf_level with k its nodes' m features): a
+// feature's histogram of one node takes cell = nbins * C counters of wbytes (lo_dt_level, lo_rf_level: u32 class counts;
+// lo_gb_level: C = 5 u64 words); a CTA holds gn nodes x fc features of them within kDtHistSmem.  fc is a multiple of 16
+// (16-byte code loads) when 16 cells fit and `vec`, else as many single features as fit (scalar loads); gn as many nodes
+// as fit beside, and as keep the pass's u64 histogram within kDtPassHist.  passes = node groups, each one pass over the
+// rows.
 struct DtShape { int vec, fc, gn, passes, smem; };
-DtShape dt_shape(int32_t k, int32_t nbins, int32_t C, int32_t nnodes, int32_t wbytes = 4) {
+DtShape dt_shape(int32_t k, int32_t nbins, int32_t C, int32_t nnodes, int32_t wbytes = 4, bool vec = true) {
     DtShape sh{};
     const int64_t cell = (int64_t)nbins * C * wbytes, cells = lo::kDtHistSmem / cell;
     const int64_t kpad = ((int64_t)k + lo::kDtVec - 1) / lo::kDtVec * lo::kDtVec;
-    sh.vec = cells >= lo::kDtVec;
+    sh.vec = vec && cells >= lo::kDtVec;
     sh.fc = (int)(sh.vec ? std::min<int64_t>(kpad, cells / lo::kDtVec * lo::kDtVec) : std::min<int64_t>(k, cells));
     const int64_t by_smem = cells / sh.fc, by_pass = lo::kDtPassHist / ((int64_t)k * nbins * C * 8);
     sh.gn = (int)std::max<int64_t>(1, std::min<int64_t>({(int64_t)std::max(nnodes, 1), by_smem, by_pass}));
@@ -3247,30 +3250,30 @@ double dt_value(uint64_t code, bool f32) {
     return v;
 }
 
-// The checks and passes of one tree level shared by lo_dt_level and lo_gb_level: C u64 words per (node, feature, bin)
-// in hist_out, counted one node group of the launch shape at a time by k_dt_level over the labels y (GB false; C
-// classes, u32 counters of wbytes 4 in shared memory) or by k_gb_level over the residuals y (GB true; C = kGbWords
-// u64 words).  *key receives the lowest refused cell's key (~0: none); hist_out is zeroed when there is one.
-template <bool GB, typename T>
-int tree_level(lo_ctx *ctx, const char *name, const char *per_bin, const T *y, int32_t C, int32_t wbytes,
-               const lo_table *codes, int64_t kp, int32_t k, int64_t n, int32_t nbins, const lo_table *src,
-               int32_t route, lo_table *dst, int32_t nparents, const int32_t *splits, int32_t nnodes, int64_t *hist_out,
-               int32_t *shape_out, lo_host_timing *timing, unsigned long long *key) {
-    *key = ~0ull;
+// The arguments every level pass checks (tree_level, lo_rf_level), in this order: k, kp, n, the code matrix, nbins, one
+// node's histogram of kf features x nbins x C u64 within LO_DT_PASS_HIST, nnodes, route, the slot tables src / dst of
+// `slots` entries (without src: route 0 and `roots` nodes, every row at its tree's root), the parents' splits, hist_out.
+int check_level(const lo_ctx *ctx, const char *per_bin, int32_t C, const lo_table *codes, int64_t kp, int32_t k,
+                int64_t n, int32_t nbins, int32_t kf, const lo_table *src, int32_t route, const lo_table *dst,
+                int64_t slots, int32_t roots, int32_t nparents, const int32_t *splits, int32_t nnodes,
+                const int64_t *hist_out) {
     if (k < 1) return fail(LO_ERR_INVALID, "k = %d: at least one feature", k);
     if (kp < k || kp % lo::kDtVec) return fail(LO_ERR_INVALID, "kp = %lld: a multiple of 16 >= k", (long long)kp);
     if (n < 0) return fail(LO_ERR_INVALID, "n = %lld is negative", (long long)n);
     LO_TRY(check_typed_table(ctx, codes, LO_U8, n * kp, "codes"));
     if ((uintptr_t)codes->base % 16) return fail(LO_ERR_INVALID, "codes must start 16-byte aligned");
     if (nbins < 1 || nbins > LO_DT_MAX_BINS) return fail(LO_ERR_INVALID, "nbins = %d outside [1, %d]", nbins, LO_DT_MAX_BINS);
-    if ((int64_t)k * nbins * C * 8 > LO_DT_PASS_HIST)
+    if ((int64_t)kf * nbins * C * 8 > LO_DT_PASS_HIST)
         return fail(LO_ERR_INVALID, "%d features x %d bins x %d %s: one node's histogram exceeds LO_DT_PASS_HIST = %lld "
-                    "bytes", k, nbins, C, per_bin, (long long)LO_DT_PASS_HIST);
+                    "bytes", kf, nbins, C, per_bin, (long long)LO_DT_PASS_HIST);
     if (nnodes < 1) return fail(LO_ERR_INVALID, "nnodes = %d: at least one", nnodes);
     if (route != 0 && route != 1) return fail(LO_ERR_INVALID, "route = %d: 0 or 1", route);
-    if (src) LO_TRY(check_typed_table(ctx, src, LO_I32, n, "src"));
-    else if (route || nnodes != 1) return fail(LO_ERR_INVALID, "without src every row is at the root: route 0, one node");
-    if (dst) LO_TRY(check_typed_table(ctx, dst, LO_I32, n, "dst"));
+    if (src) LO_TRY(check_typed_table(ctx, src, LO_I32, slots, "src"));
+    else if (roots == 1 && (route || nnodes != 1))
+        return fail(LO_ERR_INVALID, "without src every row is at the root: route 0, one node");
+    else if (route || nnodes != roots)
+        return fail(LO_ERR_INVALID, "without src every row is at its tree's root: route 0, %d nodes", roots);
+    if (dst) LO_TRY(check_typed_table(ctx, dst, LO_I32, slots, "dst"));
     if (route) {
         if (nparents < 1 || !splits) return fail(LO_ERR_INVALID, "routing needs the parents' splits");
         for (int32_t p = 0; p < nparents; ++p) {
@@ -3281,6 +3284,60 @@ int tree_level(lo_ctx *ctx, const char *name, const char *per_bin, const T *y, i
         }
     }
     if (!hist_out) return fail(LO_ERR_INVALID, "hist_out is NULL");
+    return LO_OK;
+}
+
+// the parents' splits (rows feature, bin, left, right) on the device as four arrays of np each (np 0: none)
+int *level_splits(HostCall &c, int32_t np, const int32_t *splits) {
+    if (!np) return nullptr;
+    int *d_split = nullptr;
+    std::vector<int32_t> soa((size_t)np * 4);
+    for (int32_t p = 0; p < np; ++p)
+        for (int f = 0; f < 4; ++f) soa[(size_t)f * np + p] = splits[(size_t)p * 4 + f];
+    c.alloc(&d_split, soa.size() * 4);
+    c.to_dev(d_split, soa.data(), soa.size() * 4);
+    return d_split;
+}
+
+// The node-group passes of a level (tree_level, lo_rf_level) by `kernel` with smem bytes: the grid from occupancy over
+// the chunks of sh.fc of kf features, then per group [g0, g0 + gn) of the launch shape d_hist zeroed, launch(grid,
+// from, how, to, g0, gn) enqueued and its per_node * gn words copied to hist_out.  The first pass routes (how = route)
+// from src and writes dst; the later ones read the slots it wrote.
+template <typename K, typename L>
+void level_passes(HostCall &c, K kernel, int smem, const DtShape &sh, int32_t kf, int64_t n, int32_t nnodes,
+                  size_t per_node, const lo_table *src, int32_t route, lo_table *dst, unsigned long long *d_hist,
+                  int64_t *hist_out, L launch) {
+    int per_sm = 0;
+    c.run([&] { return cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem); });
+    c.run([&] { return cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, lo::kDtThreads, smem); });
+    const int nchunks = (kf + sh.fc - 1) / sh.fc;
+    const int64_t want = (int64_t)c.ctx->sm_count * std::max(1, per_sm) / nchunks;
+    const dim3 grid((unsigned)std::max<int64_t>(1, std::min<int64_t>((n + lo::kDtThreads - 1) / lo::kDtThreads, want)),
+                    (unsigned)nchunks);
+    c.mark();
+    for (int pass = 0; pass < sh.passes; ++pass) {
+        const int g0 = pass * sh.gn, gn = std::min(sh.gn, nnodes - g0);
+        const int *from = pass == 0 ? (src ? (const int *)src->base : nullptr) : (const int *)dst->base;
+        c.memset(d_hist, 0, per_node * gn * 8);
+        c.launch(1, [&] { launch(grid, from, pass == 0 ? route : 0, pass == 0 && dst ? (int *)dst->base : nullptr, g0, gn); });
+        c.to_host(hist_out + per_node * g0, d_hist, per_node * gn * 8);
+        c.sync();                                       // d_hist is reused by the next pass
+    }
+    c.mark();
+}
+
+// The checks and passes of one tree level shared by lo_dt_level and lo_gb_level: C u64 words per (node, feature, bin)
+// in hist_out, counted one node group of the launch shape at a time by k_dt_level over the labels y (GB false; C
+// classes, u32 counters of wbytes 4 in shared memory) or by k_gb_level over the residuals y (GB true; C = kGbWords
+// u64 words).  *key receives the lowest refused cell's key (~0: none); hist_out is zeroed when there is one.
+template <bool GB, typename T>
+int tree_level(lo_ctx *ctx, const char *name, const char *per_bin, const T *y, int32_t C, int32_t wbytes,
+               const lo_table *codes, int64_t kp, int32_t k, int64_t n, int32_t nbins, const lo_table *src,
+               int32_t route, lo_table *dst, int32_t nparents, const int32_t *splits, int32_t nnodes, int64_t *hist_out,
+               int32_t *shape_out, lo_host_timing *timing, unsigned long long *key) {
+    *key = ~0ull;
+    LO_TRY(check_level(ctx, per_bin, C, codes, kp, k, n, nbins, k, src, route, dst, n, 1, nparents, splits, nnodes,
+                       hist_out));
     const DtShape sh = dt_shape(k, nbins, C, nnodes, wbytes);
     if (shape_out) {
         shape_out[0] = sh.vec;
@@ -3293,51 +3350,26 @@ int tree_level(lo_ctx *ctx, const char *name, const char *per_bin, const T *y, i
     std::fill(hist_out, hist_out + per_node * nnodes, (int64_t)0);
     HostCall c(ctx, name);
     if (n == 0) return c.finish(timing);
-    int *d_split = nullptr;
     unsigned long long *d_hist = nullptr;
     RefusedCell bad;
     bad.arm(c);
     const int np = route ? nparents : 0;
-    if (np) {
-        std::vector<int32_t> soa((size_t)np * 4);        // feature, bin, left, right: one array each
-        for (int32_t p = 0; p < np; ++p)
-            for (int f = 0; f < 4; ++f) soa[(size_t)f * np + p] = splits[(size_t)p * 4 + f];
-        c.alloc(&d_split, soa.size() * 4);
-        c.to_dev(d_split, soa.data(), soa.size() * 4);
-    }
+    int *d_split = level_splits(c, np, splits);
     c.alloc(&d_hist, per_node * sh.gn * 8);
     auto go = [&](auto kernel) {
-        int per_sm = 0;
-        c.run([&] { return cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, sh.smem); });
-        c.run([&] { return cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, lo::kDtThreads, sh.smem); });
-        const int nchunks = (k + sh.fc - 1) / sh.fc;
-        const int64_t want = (int64_t)ctx->sm_count * std::max(1, per_sm) / nchunks;
-        const dim3 grid((unsigned)std::max<int64_t>(1, std::min<int64_t>((n + lo::kDtThreads - 1) / lo::kDtThreads, want)),
-                        (unsigned)nchunks);
-        c.mark();
-        for (int pass = 0; pass < sh.passes; ++pass) {
-            const int g0 = pass * sh.gn, gn = std::min(sh.gn, nnodes - g0);
-            // the first pass routes (and writes dst); the later ones read the slots it wrote
-            const int *from = pass == 0 ? (src ? (const int *)src->base : nullptr) : (const int *)dst->base;
-            c.memset(d_hist, 0, per_node * gn * 8);
-            c.launch(1, [&] {
-                int *to = pass == 0 && dst ? (int *)dst->base : nullptr;
-                const int how = pass == 0 ? route : 0;
-                if constexpr (GB)
-                    kernel<<<grid, lo::kDtThreads, sh.smem, c.s>>>((const unsigned char *)codes->base, kp, k, y, n, nbins,
-                                                                   from, how, to, d_split, d_split + np,
-                                                                   d_split + 2 * np, d_split + 3 * np, g0, gn, sh.fc,
-                                                                   d_hist, bad.word);
-                else
-                    kernel<<<grid, lo::kDtThreads, sh.smem, c.s>>>((const unsigned char *)codes->base, kp, k, y, n, nbins,
-                                                                   C, from, how, to, d_split, d_split + np,
-                                                                   d_split + 2 * np, d_split + 3 * np, g0, gn, sh.fc,
-                                                                   d_hist, bad.word);
-            });
-            c.to_host(hist_out + per_node * g0, d_hist, per_node * gn * 8);
-            c.sync();                                       // d_hist is reused by the next pass
-        }
-        c.mark();
+        level_passes(c, kernel, sh.smem, sh, k, n, nnodes, per_node, src, route, dst, d_hist, hist_out,
+                     [&](dim3 grid, const int *from, int how, int *to, int g0, int gn) {
+            if constexpr (GB)
+                kernel<<<grid, lo::kDtThreads, sh.smem, c.s>>>((const unsigned char *)codes->base, kp, k, y, n, nbins,
+                                                               from, how, to, d_split, d_split + np,
+                                                               d_split + 2 * np, d_split + 3 * np, g0, gn, sh.fc,
+                                                               d_hist, bad.word);
+            else
+                kernel<<<grid, lo::kDtThreads, sh.smem, c.s>>>((const unsigned char *)codes->base, kp, k, y, n, nbins,
+                                                               C, from, how, to, d_split, d_split + np,
+                                                               d_split + 2 * np, d_split + 3 * np, g0, gn, sh.fc,
+                                                               d_hist, bad.word);
+        });
     };
     if constexpr (GB) {
         if (sh.vec) go(lo::k_gb_level<true>); else go(lo::k_gb_level<false>);
@@ -3754,6 +3786,139 @@ int lo_gb_predict(lo_ctx *ctx, const lo_table *x, int64_t ld, int32_t k, int64_t
         if (f.eval) go(lo::k_gb_predict<float, true>, 0.0f); else go(lo::k_gb_predict<float, false>, 0.0f);
     } else {
         if (f.eval) go(lo::k_gb_predict<double, true>, 0.0); else go(lo::k_gb_predict<double, false>, 0.0);
+    }
+    return f.finish(c, k, info, timing);
+}
+
+int lo_rf_level(lo_ctx *ctx, const lo_table *codes, int64_t kp, int32_t k, const lo_table *y, int64_t n, int64_t row0,
+                int32_t nbins, int32_t nclasses, uint64_t seed, int32_t tree0, int32_t ntrees, const uint64_t *draw,
+                int32_t ndraw, const int32_t *features, int32_t m, const lo_table *src, int32_t route, lo_table *dst,
+                int32_t nparents, const int32_t *splits, int32_t nnodes, int64_t *hist_out, int32_t *shape_out,
+                lo_host_timing *timing) {
+    LO_TRY(check_ctx(ctx));
+    if (n < 0) return fail(LO_ERR_INVALID, "n = %lld is negative", (long long)n);
+    LO_TRY(check_float_table(ctx, y, 0, n, "y"));
+    LO_TRY(check_dt_classes(nclasses));
+    if (ntrees < 1 || tree0 < 0 || row0 < 0)
+        return fail(LO_ERR_INVALID, "ntrees = %d, tree0 = %d, row0 = %lld: trees >= 1, indices >= 0", ntrees, tree0,
+                    (long long)row0);
+    if (n > INT64_MAX / ntrees) return fail(LO_ERR_INVALID, "ntrees * n overflows");
+    if (ndraw < 1 || ndraw > LO_RF_MAX_DRAWS || !draw)
+        return fail(LO_ERR_INVALID, "ndraw = %d outside [1, LO_RF_MAX_DRAWS = %d] (or draw NULL)", ndraw, LO_RF_MAX_DRAWS);
+    for (int32_t j = 1; j < ndraw; ++j)
+        if (draw[j] < draw[j - 1]) return fail(LO_ERR_INVALID, "draw is not ascending at %d", j);
+    if (m < 1 || m > k) return fail(LO_ERR_INVALID, "m = %d features per node outside [1, k = %d]", m, k);
+    LO_TRY(check_level(ctx, "classes", nclasses, codes, kp, k, n, nbins, m, src, route, dst, n * ntrees, ntrees, nparents,
+                       splits, nnodes, hist_out));
+    if (!features) return fail(LO_ERR_INVALID, "features is NULL");
+    for (int64_t i = 0; i < (int64_t)nnodes * m; ++i)
+        if (features[i] < 0 || features[i] >= k)
+            return fail(LO_ERR_INVALID, "features[%lld] = %d outside [0, %d)", (long long)i, features[i], k);
+    const DtShape sh = dt_shape(m, nbins, nclasses, nnodes, 4, false);
+    if (shape_out) {
+        shape_out[0] = sh.vec;
+        shape_out[1] = sh.fc;
+        shape_out[2] = sh.gn;
+        shape_out[3] = sh.passes;
+    }
+    if (sh.passes > 1 && !dst) return fail(LO_ERR_INVALID, "%d node groups need dst to keep the rows' slots", sh.passes);
+    const size_t per_node = (size_t)m * nbins * nclasses;
+    std::fill(hist_out, hist_out + per_node * nnodes, (int64_t)0);
+    HostCall c(ctx, "rf_level");
+    if (n == 0) return c.finish(timing);
+    unsigned long long *d_hist = nullptr, *d_draw = nullptr;
+    int *d_feat = nullptr;
+    RefusedCell bad;
+    bad.arm(c);
+    const int np = route ? nparents : 0;
+    int *d_split = level_splits(c, np, splits);
+    c.alloc(&d_draw, (size_t)ndraw * 8);
+    c.alloc(&d_feat, (size_t)nnodes * m * 4);
+    c.to_dev(d_draw, draw, (size_t)ndraw * 8);
+    c.to_dev(d_feat, features, (size_t)nnodes * m * 4);
+    c.alloc(&d_hist, per_node * sh.gn * 8);
+    const int smem = ndraw * 8 + sh.smem;
+    auto go = [&](auto kernel, auto tag) {
+        using T = decltype(tag);
+        level_passes(c, kernel, smem, sh, m, n, nnodes, per_node, src, route, dst, d_hist, hist_out,
+                     [&](dim3 grid, const int *from, int how, int *to, int g0, int gn) {
+            kernel<<<grid, lo::kDtThreads, smem, c.s>>>((const unsigned char *)codes->base, kp, k, (const T *)y->base, n,
+                                                        row0, nbins, nclasses, (unsigned long long)seed, tree0, ntrees,
+                                                        d_draw, ndraw, d_feat, m, from, how, to, d_split, d_split + np,
+                                                        d_split + 2 * np, d_split + 3 * np, g0, gn, sh.fc, d_hist,
+                                                        bad.word);
+        });
+    };
+    if (y->dtype == LO_F32) go(lo::k_rf_level<float>, 0.0f); else go(lo::k_rf_level<double>, 0.0);
+    bad.read(c);
+    LO_TRY(c.finish(timing));
+    if (bad.key == ~0ull) return LO_OK;
+    std::fill(hist_out, hist_out + per_node * nnodes, (int64_t)0);
+    int64_t row = 0;
+    int32_t col = 0;
+    lo::cell_of_key(bad.key, k, &row, &col);
+    if (col == k) return fail(LO_ERR_INVALID, "row %lld: its label is not a class in [0, %d)", (long long)row, nclasses);
+    return fail(LO_ERR_INVALID, "row %lld, feature %d: code >= nbins = %d", (long long)row, col, nbins);
+}
+
+int lo_rf_predict(lo_ctx *ctx, const lo_table *x, int64_t ld, int32_t k, int64_t n, int32_t ntrees, const int32_t *start,
+                  int32_t nnodes, const int32_t *feature, const double *threshold, const int32_t *left,
+                  const int32_t *right, const double *votes, int32_t nclasses, lo_table *prob, lo_table *raw,
+                  lo_table *pred, const lo_table *y, const double *eval_labels, int32_t neval, int64_t *confusion_out,
+                  lo_nb_info *info, lo_host_timing *timing) {
+    LO_TRY(start_info(ctx, info));
+    PredictFrame f(y, eval_labels, neval, confusion_out);
+    LO_TRY(f.check_x(ctx, x, ld, k, n));
+    LO_TRY(check_dt_classes(nclasses));
+    const int32_t M = nnodes, C = nclasses;
+    if (ntrees < 1 || M < ntrees || !start || !feature || !threshold || !left || !right || !votes)
+        return fail(LO_ERR_INVALID, "a forest of %d trees and %d nodes: start, feature, threshold, left, right and votes "
+                    "are needed", ntrees, M);
+    for (int32_t t = 0; t < ntrees; ++t) {
+        const int32_t lo = start[t], hi = t + 1 < ntrees ? start[t + 1] : M;
+        if (t == 0 && lo != 0) return fail(LO_ERR_INVALID, "start[0] = %d: the first tree starts at node 0", lo);
+        if (!(hi > lo && hi <= M)) return fail(LO_ERR_INVALID, "tree %d: nodes [%d, %d) of %d", t, lo, hi, M);
+        LO_TRY(check_tree_nodes(feature, left, right, lo, hi, k));
+    }
+    LO_TRY(f.check_out(ctx, n, C, prob, raw, pred));
+    HostCall c(ctx, f.call("rf"));
+    if (n == 0) return c.finish(timing);
+    const int64_t forest_bytes = ((int64_t)M + (int64_t)M * C) * 8 + ((int64_t)3 * M + ntrees) * 4;
+    const int64_t evl_bytes = (int64_t)f.neval * 8, hist_bytes = (int64_t)f.neval * C * 4;
+    const bool forest_smem = forest_bytes + evl_bytes <= lo::kDtTreeSmem;
+    const int64_t fixed = (forest_smem ? forest_bytes : 0) + evl_bytes;
+    const bool hist_smem = f.eval && fixed + hist_bytes <= lo::kDtTreeSmem;
+    const int smem = (int)(fixed + (hist_smem ? hist_bytes : 0));
+    int *d_int = nullptr;
+    double *d_dbl = nullptr;
+    c.alloc(&d_int, ((size_t)3 * M + ntrees) * 4);
+    c.alloc(&d_dbl, ((size_t)M + (size_t)M * C) * 8);
+    c.to_dev(d_int, feature, (size_t)M * 4);
+    c.to_dev(d_int + M, left, (size_t)M * 4);
+    c.to_dev(d_int + 2 * M, right, (size_t)M * 4);
+    c.to_dev(d_int + 3 * M, start, (size_t)ntrees * 4);
+    c.to_dev(d_dbl, threshold, (size_t)M * 8);
+    c.to_dev(d_dbl + M, votes, (size_t)M * C * 8);
+    f.stage(c);
+    auto go = [&](auto kernel, auto tag) {
+        using T = decltype(tag);
+        const int grid = f.grid(c, kernel, lo::kDtThreads, smem, (n + lo::kDtThreads - 1) / lo::kDtThreads);
+        c.mark();
+        c.launch(1, [&] {
+            kernel<<<grid, lo::kDtThreads, smem, c.s>>>((const T *)x->base, ld, k, n, ntrees, M, d_int + 3 * M, d_int, d_dbl,
+                                                        d_int + M, d_int + 2 * M, d_dbl + M, C, forest_smem ? 1 : 0,
+                                                        prob ? (double *)prob->base : nullptr,
+                                                        raw ? (double *)raw->base : nullptr,
+                                                        pred ? (double *)pred->base : nullptr,
+                                                        y ? (const T *)y->base : nullptr, f.d_evl, f.neval, f.direct, f.conf,
+                                                        hist_smem ? 1 : 0, f.bad.word);
+        });
+        c.mark();
+    };
+    if (x->dtype == LO_F32) {
+        if (f.eval) go(lo::k_rf_predict<float, true>, 0.0f); else go(lo::k_rf_predict<float, false>, 0.0f);
+    } else {
+        if (f.eval) go(lo::k_rf_predict<double, true>, 0.0); else go(lo::k_rf_predict<double, false>, 0.0);
     }
     return f.finish(c, k, info, timing);
 }

@@ -11,6 +11,8 @@
 //     fixed-point residual sums.
 //   * k_dt_predict<T, EVAL>: walks the tree per row; raw = the leaf's class counts, probability = raw / sum.
 //   * k_gb_update<T>: GBT's margins F and residuals r after each tree; k_gb_predict<T, EVAL>: the forest's margin.
+//   * k_rf_level<T>: one level of a batch of RandomForest trees, each row counted with its bagging weight over its
+//     node's feature subset; k_rf_predict<T, EVAL>: the forest's votes (lo_rf_level, lo_rf_predict, §3.6.6).
 #pragma once
 
 namespace lo {
@@ -491,6 +493,186 @@ __global__ void __launch_bounds__(kDtThreads) k_gb_predict(const T *__restrict__
                 __stcs(raw_out + 2 * r, -m);
                 __stcs(raw_out + 2 * r + 1, m);
             }
+            __stcs(pred + r, (double)best);
+        } else {
+            cm.count((double)y[r], best, r, k);
+        }
+    }
+    if (EVAL) cm.finish(err);
+}
+
+// ---- RandomForestClassifier (DESIGN.md §3.6.6) ----------------------------------------------------------------------
+constexpr int kRfMaxDraws = 32;              // LO_RF_MAX_DRAWS: entries of a bagging threshold table
+constexpr int kRfVotes = 8;                  // k_rf_predict's per-row votes held in registers per walk of the forest
+
+// splitmix64's step: the golden-ratio increment, then its finaliser
+__device__ __forceinline__ unsigned long long rf_mix(unsigned long long z) {
+    z += 0x9E3779B97F4A7C15ull;
+    z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+    z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+    return z ^ (z >> 31);
+}
+
+// A row's bagging weight in a tree: u = rf_mix(rf_mix(key ^ tree) ^ row) with key = rf_mix(seed), weight = #{j : u >=
+// draw[j]} over the ascending table (so the count of its leading entries <= u)
+__device__ __forceinline__ unsigned rf_weight(unsigned long long key, long long tree, long long row,
+                                              const unsigned long long *draw, int ndraw) {
+    const unsigned long long u = rf_mix(rf_mix(key ^ (unsigned long long)tree) ^ (unsigned long long)row);
+    int w = 0;
+    while (w < ndraw && u >= draw[w]) ++w;
+    return (unsigned)w;
+}
+
+// One level of a batch of ntrees trees (global indices tree0 ..) over every row: k_dt_level's pass with each row's
+// bagging weight and per-node feature subsets.  Row r's slot in tree t lives at src[t * n + r] (src NULL: the root, slot
+// t), numbered across the batch in tree order, and is routed by its parent's split as in k_dt_level; CTAs of
+// blockIdx.y == 0 write it to dst.  A (row, tree) whose slot lies in [g0, g0 + gn) and whose weight w (rf_weight of the
+// global row row0 + r) is not 0 adds w to hist[slot - g0][q][code][class] for each q of the CTA's chunk [blockIdx.y * fc,
+// + fc) of the node's m features feats[slot * m ..]: u32 counters in shared memory after the draw table, flushed once per
+// CTA into out ([gn][m][nbins][C], u64).  A code >= nbins or a label that is not a class is never counted: the lowest
+// such cell's key goes to *err.
+template <typename T>
+__global__ void __launch_bounds__(kDtThreads) k_rf_level(const unsigned char *__restrict__ codes, long long kp, int k,
+                                                         const T *__restrict__ y, long long n, long long row0, int nbins,
+                                                         int C, unsigned long long seed, int tree0, int ntrees,
+                                                         const unsigned long long *__restrict__ draw, int ndraw,
+                                                         const int *__restrict__ feats, int m, const int *__restrict__ src,
+                                                         int route, int *__restrict__ dst, const int *__restrict__ sfeat,
+                                                         const int *__restrict__ sbin, const int *__restrict__ left,
+                                                         const int *__restrict__ right, int g0, int gn, int fc,
+                                                         unsigned long long *__restrict__ out,
+                                                         unsigned long long *__restrict__ err) {
+    extern __shared__ unsigned long long rf_smem[];
+    unsigned long long *dr = rf_smem;
+    unsigned *hist = reinterpret_cast<unsigned *>(rf_smem + ndraw);
+    const int cell = nbins * C, q0 = blockIdx.y * fc, fw = min(fc, m - q0);
+    const int cells = gn * fc * cell;
+    for (int i = threadIdx.x; i < ndraw; i += kDtThreads) dr[i] = draw[i];
+    for (int i = threadIdx.x; i < cells; i += kDtThreads) hist[i] = 0;
+    __syncthreads();
+    const unsigned long long key = rf_mix(seed);
+    const bool write = dst != nullptr && blockIdx.y == 0;
+    unsigned long long bad = ~0ull;
+    for (long long r = blockIdx.x * (long long)kDtThreads + threadIdx.x; r < n; r += (long long)gridDim.x * kDtThreads) {
+        const unsigned char *row = codes + r * kp;
+        const double lab = (double)y[r];
+        const int cls = (int)lab;
+        const bool is_class = lab >= 0.0 && lab < (double)C && (double)cls == lab;
+        for (int t = 0; t < ntrees; ++t) {
+            int s = t;
+            if (src) {
+                s = src[t * n + r];
+                if (route && s >= 0) {
+                    const int f = sfeat[s];
+                    s = f < 0 ? -1 : (int)row[f] <= sbin[s] ? left[s] : right[s];
+                }
+            }
+            if (write) dst[t * n + r] = s;
+            if (s < g0 || s >= g0 + gn) continue;
+            const unsigned w = rf_weight(key, (long long)tree0 + t, row0 + r, dr, ndraw);
+            if (!w) continue;
+            if (!is_class) {                                    // not a class: refused, never counted
+                bad = min(bad, cell_key(r, k, k));
+                continue;
+            }
+            unsigned *h = hist + (size_t)(s - g0) * fc * cell + cls;
+            const int *fl = feats + (size_t)s * m + q0;
+            for (int q = 0; q < fw; ++q) {
+                const int f = __ldg(fl + q);
+                const unsigned code = row[f];
+                if (code >= (unsigned)nbins) bad = min(bad, cell_key(r, k, f));
+                else atomicAdd(&h[(size_t)q * cell + code * C], w);
+            }
+        }
+    }
+    report_cell(bad, err);
+    __syncthreads();
+    for (int i = threadIdx.x; i < cells; i += kDtThreads) {
+        const unsigned v = hist[i];
+        if (!v) continue;
+        const int g = i / (fc * cell), rest = i - g * fc * cell, q = rest / cell;
+        if (q >= fw) continue;
+        atomicAdd(&out[((size_t)g * m + q0 + q) * cell + (rest - q * cell)], (unsigned long long)v);
+    }
+}
+
+// RandomForest transform / evaluate, one row per thread: raw_c = the sum over trees t (in order, from 0.0) of
+// votes[leaf_t * C + c], the leaf's class counts over their total as the host computed them (0 for a leaf of no
+// counts); probability = raw / sum (IEEE division, sum in c order), prediction = the first argmax of raw.  Tree t's
+// nodes start at start[t] (children as indices into the whole forest).  The votes are kept in registers kRfVotes
+// classes at a time, the forest walked once per such group; with C above kRfVotes the raw values wait in the row's
+// probability slice until the sum is known.  The forest (structure and votes) sits in shared memory when `forest_smem`
+// (else it is read from global memory).  EVAL: nothing per row; (label, prediction) counts in a Confusion, as in
+// k_dt_predict.
+template <typename T, bool EVAL>
+__global__ void __launch_bounds__(kDtThreads) k_rf_predict(const T *__restrict__ x, long long ld, int k, long long n,
+                                                           int ntrees, int M, const int *__restrict__ start,
+                                                           const int *__restrict__ feat, const double *__restrict__ thr,
+                                                           const int *__restrict__ left, const int *__restrict__ right,
+                                                           const double *__restrict__ votes, int C, int forest_smem,
+                                                           double *__restrict__ prob, double *__restrict__ raw_out,
+                                                           double *__restrict__ pred, const T *__restrict__ y,
+                                                           const double *__restrict__ eval_labels, int neval, int direct,
+                                                           unsigned long long *__restrict__ confusion, int hist_in_smem,
+                                                           unsigned long long *__restrict__ err) {
+    extern __shared__ double dt_smem[];
+    const double *th = thr, *vo = votes;
+    const int *fe = feat, *le = left, *ri = right, *st = start;
+    double *evl = dt_smem;
+    unsigned *hist_at = reinterpret_cast<unsigned *>(dt_smem + neval);
+    if (forest_smem) {
+        double *ts = dt_smem, *vs = ts + M;
+        evl = vs + (size_t)M * C;
+        int *fs = reinterpret_cast<int *>(evl + neval), *ls = fs + M, *rs = ls + M, *ss = rs + M;
+        for (int i = threadIdx.x; i < M; i += kDtThreads) {
+            ts[i] = thr[i];
+            fs[i] = feat[i];
+            ls[i] = left[i];
+            rs[i] = right[i];
+        }
+        for (int i = threadIdx.x; i < M * C; i += kDtThreads) vs[i] = votes[i];
+        for (int i = threadIdx.x; i < ntrees; i += kDtThreads) ss[i] = start[i];
+        th = ts, vo = vs, fe = fs, le = ls, ri = rs, st = ss;
+        hist_at = reinterpret_cast<unsigned *>(ss + ntrees);
+    }
+    Confusion<kDtThreads> cm{evl, hist_at, confusion, neval, C, direct, hist_in_smem};
+    if (EVAL) cm.stage(eval_labels);
+    __syncthreads();
+    for (long long r = blockIdx.x * (long long)kDtThreads + threadIdx.x; r < n; r += (long long)gridDim.x * kDtThreads) {
+        const T *xr = x + r * ld;
+        double sum = 0.0, top = 0.0;
+        int best = 0;
+        for (int c0 = 0; c0 < C; c0 += kRfVotes) {
+            double v[kRfVotes];
+#pragma unroll
+            for (int i = 0; i < kRfVotes; ++i) v[i] = 0.0;
+            for (int t = 0; t < ntrees; ++t) {
+                int node = st[t], f;
+                while ((f = fe[node]) >= 0) node = (double)xr[f] <= th[node] ? le[node] : ri[node];
+                const double *lv = vo + (size_t)node * C + c0;
+#pragma unroll
+                for (int i = 0; i < kRfVotes; ++i)
+                    if (c0 + i < C) v[i] = __dadd_rn(v[i], lv[i]);
+            }
+#pragma unroll
+            for (int i = 0; i < kRfVotes; ++i) {
+                const int c = c0 + i;
+                if (c < C) {
+                    sum = __dadd_rn(sum, v[i]);
+                    if (c == 0 || v[i] > top) { best = c; top = v[i]; }
+                    if (!EVAL && raw_out) __stcs(raw_out + r * C + c, v[i]);
+                    if (!EVAL && C > kRfVotes) prob[r * C + c] = v[i];
+                }
+            }
+            if (!EVAL && C <= kRfVotes) {
+#pragma unroll
+                for (int i = 0; i < kRfVotes; ++i)
+                    if (i < C) __stcs(prob + r * C + i, __ddiv_rn(v[i], sum));
+            }
+        }
+        if (!EVAL) {
+            if (C > kRfVotes)
+                for (int c = 0; c < C; ++c) prob[r * C + c] = __ddiv_rn(prob[r * C + c], sum);
             __stcs(pred + r, (double)best);
         } else {
             cm.count((double)y[r], best, r, k);

@@ -418,8 +418,8 @@ class SortedColumns:
 
 class BinnedRows:
     """What :meth:`Engine.dt_bin` made for one device's rows: ``codes`` (LO_U8, n rows at :func:`code_pitch` (k)) and
-    ``slots``, two LO_I32 tables of the rows' node slots that the levels write in turn (``cur`` the latest).  :meth:`free`
-    frees them and may be called again."""
+    ``slots``, two LO_I32 tables of the rows' node slots that the levels write in turn (``cur`` the latest; n long, or
+    ntrees * n once :meth:`Engine.rf_level` grew a batch of trees).  :meth:`free` frees them and may be called again."""
 
     def __init__(self, codes: "DeviceTable", slots: list):
         self.codes, self.slots, self.cur = codes, slots, 0
@@ -1236,8 +1236,8 @@ class Engine:
 
     def _level(self, fn, lead: tuple, part: AssembledRows, binned: "BinnedRows", splits, nnodes: int, out: np.ndarray,
                shape: list | None, timing: dict | None) -> np.ndarray:
-        """The level pass of :meth:`dt_level` / :meth:`gb_level`: ``fn`` the library's entry point, ``lead`` its
-        arguments after (ctx, codes, kp, k), ``out`` the array it fills.  The rows' slots ping-pong between ``binned``'s
+        """The level pass of :meth:`dt_level` / :meth:`gb_level` / :meth:`rf_level`: ``fn`` the library's entry point,
+        ``lead`` its arguments after (ctx, codes, kp, k), ``out`` the array it fills.  The rows' slots ping-pong between ``binned``'s
         two tables; ``shape`` receives the launch shape."""
         k = part.k
         sp = np.ascontiguousarray(splits if splits is not None else np.zeros((0, 4)), np.int32)
@@ -1306,6 +1306,42 @@ class Engine:
         model = (len(trees), start.ctypes.data_as(C.c_void_p), w.ctypes.data_as(C.c_void_p), M,
                  *[a.ctypes.data_as(C.c_void_p) for a in arrs])
         return self._predict(self._lib.lo_gb_predict, model, part, 2, raw, labels, timing)
+
+    def rf_level(self, part: AssembledRows, binned: "BinnedRows", nbins: int, nclasses: int, seed: int, draw,
+                 tree0: int, ntrees: int, splits, features, row0: int = 0, shape: list | None = None,
+                 timing: dict | None = None) -> np.ndarray:
+        """One level of RandomForest trees tree0 .. tree0 + ntrees - 1 over ``part``'s rows (``lo_rf_level``): int64
+        (nnodes, m, nbins, nclasses) sums of the rows' bagging weights per (node slot, listed feature, bin, class).
+        ``features`` int32 (nnodes, m) lists each node's features; ``splits`` as :meth:`dt_level`, numbered across the
+        batch in tree order (None: the root level, nnodes = ntrees).  ``draw`` is the bagging table
+        (:func:`tree.draw_table`), ``seed`` the forest's seed and ``row0`` the global index of the part's first row.
+        The rows' slots in every tree ping-pong between ``binned``'s two tables, made ntrees * n long at the root."""
+        feats = np.ascontiguousarray(features, np.int32)
+        nnodes, m = feats.shape
+        dr = np.ascontiguousarray(draw, np.uint64)
+        n = part.nkept
+        if splits is None and binned.slots[0].nrows < ntrees * n:
+            with _Owned() as owned:
+                slots = [owned.own(self.table("i32", ntrees * n, 1)) for _ in range(2)]
+            for t in binned.slots:
+                t.free()
+            binned.slots, binned.cur = slots, 0
+        hist = np.zeros((nnodes, m, nbins, nclasses), np.int64)
+        lead = (part.y._h, n, int(row0), int(nbins), int(nclasses), int(seed) & ((1 << 64) - 1), int(tree0),
+                int(ntrees), dr.ctypes.data_as(C.c_void_p), len(dr), feats.ctypes.data_as(C.c_void_p), m)
+        return self._level(self._lib.lo_rf_level, lead, part, binned, splits, nnodes, hist, shape, timing)
+
+    def rf_predict(self, part: AssembledRows, trees, raw: bool = False, labels=None, timing: dict | None = None):
+        """A RandomForest (classification :class:`~tree.Tree` s) over ``part`` (``lo_rf_predict``), as
+        :meth:`nb_predict`: ``labels`` None gives a :class:`PredictedRows` of C columns, else the int64[len(labels), C]
+        confusion counts.  Every leaf votes its counts over their total (:func:`tree.votes`)."""
+        from .tree import votes
+        start, M, feature, threshold, left, right, _value = forest_arrays(trees)
+        vo = np.ascontiguousarray(np.concatenate([votes(t) for t in trees]), np.float64)
+        nc = trees[0].num_classes
+        model = (len(trees), start.ctypes.data_as(C.c_void_p), M,
+                 *[a.ctypes.data_as(C.c_void_p) for a in (feature, threshold, left, right, vo)], nc)
+        return self._predict(self._lib.lo_rf_predict, model, part, nc, raw, labels, timing)
 
     def value_counts_f64_host(self, values: np.ndarray):
         """(keys float64[g], counts uint64[g]) — exact value counts of a numeric column (GPU hash group-by),

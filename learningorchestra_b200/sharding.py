@@ -871,6 +871,21 @@ class ShardedEngine:
         return self._predicted("gb_predict", lambda i: self.engines[i].gb_predict(parts[i], trees, weights, raw, labels),
                                parts, labels)
 
+    def rf_level(self, parts, binned: list, nbins: int, nclasses: int, seed: int, draw, tree0: int, ntrees: int, splits,
+                 features, shape: list | None = None):
+        """``Engine.rf_level`` on every member over the same splits and feature lists, each member's ``row0`` its first
+        row in the rows of all of them, so every cut draws the same bagging weights; the integer histograms added in
+        shard order, so they do not depend on the cut.  ``shape`` receives the first member's launch shape."""
+        firsts = _firsts(parts)
+        return self._summed("rf_level", lambda i, sh=None: self.engines[i].rf_level(
+            parts[i], binned[i], nbins, nclasses, seed, draw, tree0, ntrees, splits, features, firsts[i], sh), shape=shape)
+
+    def rf_predict(self, parts, trees, raw: bool = False, labels=None):
+        """``Engine.rf_predict`` over the shards, as :meth:`nb_predict`: one ``PredictedRows`` per member, or the
+        members' confusion counts summed; a refused row is raised as the lowest over all shards, its row global."""
+        return self._predicted("rf_predict", lambda i: self.engines[i].rf_predict(parts[i], trees, raw, labels), parts,
+                               labels)
+
     @property
     def resident(self):
         """Datasets kept in HBM between requests, rows sharded over the group (:mod:`table_cache`)."""

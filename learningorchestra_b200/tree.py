@@ -1,7 +1,9 @@
-"""Host side of the builder's "DT" classifier (Spark 2.4's DecisionTreeClassifier, DESIGN.md §3.6.4): the split
-candidates of every column from the device's sorted columns and rank counts, the level-wise growth from the device's
-(node, feature, bin, class) histograms, the pruning and the model's arrays.  Nothing here touches the device: the
-callers hand in the counts (:mod:`classifier` on an ``Engine`` or ``ShardedEngine``, the tests with numpy stand-ins)."""
+"""Host side of the builder's tree classifiers (Spark 2.4's DecisionTreeClassifier, GBTClassifier and
+RandomForestClassifier, DESIGN.md §3.6.4 to §3.6.6): the split candidates of every column from the device's sorted
+columns and rank counts, the level-wise growth of one tree or of several in lockstep from the device's (node, feature,
+bin, class) histograms, the pruning and the model's arrays, and RandomForest's bagging tables, feature subsets and
+votes.  Nothing here touches the device: the callers hand in the counts (:mod:`classifier` on an ``Engine`` or
+``ShardedEngine``, the tests with numpy stand-ins)."""
 from __future__ import annotations
 
 import math
@@ -16,6 +18,7 @@ DOUBLE_MIN = -np.finfo(np.float64).max   # Scala's Double.MinValue: the gain of 
 IMPURITIES = ("gini", "entropy")
 VARIANCE = "variance"       # GBT's regression trees (DESIGN.md §3.6.5): the level gives lo_gb_level's words
 WORDS = 5                   # LO_GB_WORDS: count, sum of q1 + 2^60 (lo, hi), sum of q2 (lo, hi) per (node, feature, bin)
+MAX_DRAWS = 32              # LO_RF_MAX_DRAWS: entries of a bagging threshold table
 
 
 def num_splits(max_bins: int, n: int) -> int:
@@ -220,12 +223,14 @@ def impurity(counts: np.ndarray, total: np.ndarray, kind: str) -> np.ndarray:
     return np.where(total == 0, 0.0, out)
 
 
-def best_splits(hist: np.ndarray, nthr: np.ndarray, kind: str, min_instances: int, min_info_gain: float):
+def best_splits(hist: np.ndarray, nthr: np.ndarray, kind: str, min_instances: int, min_info_gain: float,
+                features: np.ndarray | None = None):
     """binsToBestSplit for every node of a level at once.  hist: int64 (nodes, k, nbins, C).  The left counts of split i
-    are the prefix over bins 0 .. i, the right ones the node's total minus them.  Returns a dict of per-node arrays:
-    ``feature`` (-1: no feature has a split), ``bin``, ``gain`` (Double.MinValue when invalid), ``impurity`` (the
-    node's), ``left`` / ``right`` (class counts), ``left_impurity`` / ``right_impurity``, ``valid`` and ``total`` (the
-    node's class counts)."""
+    are the prefix over bins 0 .. i, the right ones the node's total minus them.  ``nthr``: the splits of each of the k
+    features (k,), or of each node's (nodes, k) when ``features`` (int (nodes, k), ascending) lists every node's own
+    features, hist's feature axis following them.  Returns a dict of per-node arrays: ``feature`` (-1: no feature has a
+    split), ``bin``, ``gain`` (Double.MinValue when invalid), ``impurity`` (the node's), ``left`` / ``right`` (class
+    counts), ``left_impurity`` / ``right_impurity``, ``valid`` and ``total`` (the node's class counts)."""
     nodes, k, nbins, C = hist.shape
     total = hist[:, 0].sum(axis=1)                              # (nodes, C)
     tsum = total.sum(axis=1).astype(np.float64)
@@ -241,29 +246,35 @@ def best_splits(hist: np.ndarray, nthr: np.ndarray, kind: str, min_instances: in
     right = total[:, None, None, :] - left
     lc = left.sum(axis=3).astype(np.float64)
     rc = right.sum(axis=3).astype(np.float64)
-    return _choose(out, node_imp, left, right, lc, rc, impurity(left, lc, kind), impurity(right, rc, kind), nthr,
-                   min_instances, min_info_gain)
+    out = _choose(out, node_imp, left, right, lc, rc, impurity(left, lc, kind), impurity(right, rc, kind), nthr,
+                  min_instances, min_info_gain)
+    if features is not None:
+        f = out["feature"]
+        out["feature"] = np.where(f >= 0, np.asarray(features)[np.arange(nodes), np.maximum(f, 0)], -1)
+    return out
 
 
 def _choose(out, node_imp, left, right, lc, rc, limp, rimp, nthr, min_instances, min_info_gain):
     """binsToBestSplit's choice from every candidate's (nodes, k, ns) counts lc / rc and impurities limp / rimp:
-    calculateImpurityStats' gain, the minInstancesPerNode and minInfoGain rules and the first maximum."""
+    calculateImpurityStats' gain, the minInstancesPerNode and minInfoGain rules and the first maximum.  ``nthr``: (k,)
+    splits per feature, or (nodes, k) per node."""
     nodes, k, ns = lc.shape
     tc = lc + rc
     with np.errstate(invalid="ignore", divide="ignore"):
         wl = lc / tc
         wr = rc / tc
         gain = node_imp[:, None, None] - wl * limp - wr * rimp
-    real = np.arange(ns)[None, :] < nthr[:, None]              # (k, ns): split i exists for feature j
+    real = np.arange(ns) < np.asarray(nthr)[..., None]         # (k, ns) or (nodes, k, ns): split i exists for feature j
+    real = real if real.ndim == 3 else real[None]
     ok = (lc >= min_instances) & (rc >= min_instances)
     ok &= ~(gain < min_info_gain)
     gain = np.where(ok, gain, DOUBLE_MIN)
-    gain = np.where(real[None], gain, -np.inf)                  # never chosen over a real split, valid or not
+    gain = np.where(real, gain, -np.inf)                        # never chosen over a real split, valid or not
     flat = gain.reshape(nodes, -1)
     at = flat.argmax(axis=1)                                    # the first maximum: features, then splits, in order
     j, i = np.divmod(at, ns)
     r = np.arange(nodes)
-    has = real.any()
+    has = real.reshape(len(real), -1).any(axis=1)               # per node (one for all with per-feature nthr)
     out.update(feature=np.where(has, j, -1), bin=i, gain=flat[r, at], valid=ok[r, j, i] & has,
                left=left[r, j, i], right=right[r, j, i], left_impurity=limp[r, j, i], right_impurity=rimp[r, j, i])
     return out
@@ -352,26 +363,36 @@ class Tree:
         return int(d.max()) if self.num_nodes else 0
 
 
-def grow(level, thresholds, num_classes: int, max_depth: int, kind: str, min_instances: int, min_info_gain: float):
+def grow(level, thresholds, num_classes: int, max_depth: int, kind: str, min_instances: int, min_info_gain: float,
+         trees: int | None = None, subsets=None):
     """Spark's level-wise growth and toNode(prune = true).  ``level(splits, nnodes) -> hist`` counts one level: splits
     None for the root, else int32 (parents, 4) rows (feature, bin, left slot, right slot) of the previous level's nodes
     in slot order (feature -1: the node did not split; slot -1: a leaf child); hist int64 (nnodes, k, nbins, C).
     ``kind`` VARIANCE grows a regression tree (num_classes 0): hist is lo_gb_level's uint64 words (nnodes, k, nbins,
     WORDS) and a node's counts its (count, sum, sumSq).  Returns a :class:`Tree` and the per-level histograms' node
-    counts."""
+    counts.  ``trees``: that many trees grow in lockstep, one level call for all of them, their nodes in slot order tree
+    by tree (the root level's slot t is tree t's root), and the result is a list of Trees.  ``subsets(t, node)``: the
+    ascending features tree t's node (Spark's index: root 1, children 2i and 2i + 1) searches; the level is then called
+    as ``level(splits, nnodes, features)`` with features int32 (nnodes, m) and hist's feature axis following them."""
     nthr = np.array([len(t) for t in thresholds], np.int64)
-    # learning nodes: dict(depth, stats: counts / impurity / gain / valid, split, children, leaf)
-    nodes = [dict(depth=0, counts=None, impurity=None, gain=np.nan, valid=True, split=None, kids=None)]
-    active = [0]                      # the learning nodes of this level, in slot order
+    # learning nodes: dict(tree, id, depth, stats: counts / impurity / gain / valid, split, children)
+    nodes = [dict(tree=t, id=1, depth=0, counts=None, impurity=None, gain=np.nan, valid=True, split=None, kids=None)
+             for t in range(1 if trees is None else trees)]
+    active = list(range(len(nodes)))  # the learning nodes of this level, in slot order
     splits = None
     shapes = []
     while active:
-        hist = level(splits, len(active))
+        feats = None
+        if subsets is None:
+            hist = level(splits, len(active))
+        else:
+            feats = np.array([subsets(nodes[i]["tree"], nodes[i]["id"]) for i in active], np.int32)
+            hist = level(splits, len(active), feats)
         shapes.append(len(active))
         if kind == VARIANCE:
             best = variance_splits(hist, nthr, min_instances, min_info_gain)
         else:
-            best = best_splits(hist, nthr, kind, min_instances, min_info_gain)
+            best = best_splits(hist, nthr if feats is None else nthr[feats], kind, min_instances, min_info_gain, feats)
         nxt, rows = [], []
         for s, idx in enumerate(active):
             node = nodes[idx]
@@ -388,11 +409,11 @@ def grow(level, thresholds, num_classes: int, max_depth: int, kind: str, min_ins
             child_leaf = d + 1 == max_depth
             kids = []
             slots = []
-            for side in ("left", "right"):
+            for side, cid in (("left", 2 * node["id"]), ("right", 2 * node["id"] + 1)):
                 imp = best[side + "_impurity"][s]
                 leaf = child_leaf or abs(imp) < EPSILON
-                nodes.append(dict(depth=d + 1, counts=best[side][s], impurity=imp, gain=np.nan, valid=True,
-                                  split=None, kids=None))
+                nodes.append(dict(tree=node["tree"], id=cid, depth=d + 1, counts=best[side][s], impurity=imp,
+                                  gain=np.nan, valid=True, split=None, kids=None))
                 kids.append(len(nodes) - 1)
                 if leaf:
                     slots.append(-1)
@@ -403,13 +424,14 @@ def grow(level, thresholds, num_classes: int, max_depth: int, kind: str, min_ins
             rows.append((j, i, slots[0], slots[1]))
         splits = np.array(rows, np.int32).reshape(-1, 4)
         active = nxt
-    return _to_tree(nodes, num_classes), shapes
+    grown = [_to_tree(nodes, num_classes, t) for t in range(1 if trees is None else trees)]
+    return (grown[0] if trees is None else grown), shapes
 
 
-def _to_tree(nodes, num_classes: int) -> Tree:
-    """toNode(prune = true) into breadth-first arrays: two leaf children of equal prediction (the first argmax of the
-    counts; a regression tree's sum / count, as f64) merge into a leaf with the parent's impurity and counts (bottom-up,
-    so merges cascade); an invalid split search leaves impurity -1."""
+def _to_tree(nodes, num_classes: int, root: int = 0) -> Tree:
+    """toNode(prune = true) of the tree whose root is nodes[root] into breadth-first arrays: two leaf children of equal
+    prediction (the first argmax of the counts; a regression tree's sum / count, as f64) merge into a leaf with the
+    parent's impurity and counts (bottom-up, so merges cascade); an invalid split search leaves impurity -1."""
     def prediction(counts):
         if num_classes == 0:
             return float(counts[1] / counts[0])
@@ -425,9 +447,9 @@ def _to_tree(nodes, num_classes: int) -> Tree:
             return ("leaf", np.asarray(n["counts"], np.float64), float(n["impurity"]))
         return ("split", np.asarray(n["counts"], np.float64), float(n["impurity"]), float(n["gain"]), n["split"], l, r)
 
-    root = build(0)
+    top = build(root)
     feature, threshold, left, right, counts, imps, gains = [], [], [], [], [], [], []
-    queue = [root]
+    queue = [top]
     while queue:
         nd = queue.pop(0)
         at = len(feature)
@@ -442,3 +464,101 @@ def _to_tree(nodes, num_classes: int) -> Tree:
         left.append(base), right.append(base + 1)
         queue += [nd[5], nd[6]]
     return Tree(feature, threshold, left, right, np.array(counts).reshape(-1, num_classes or 3), imps, gains, num_classes)
+
+
+# ---- RandomForest (DESIGN.md §3.6.6): bagging, feature subsets, votes ---------------------------------------------
+M64 = (1 << 64) - 1
+STRATEGIES = ("auto", "all", "onethird", "sqrt", "log2")
+
+
+def java_hash(text: str) -> int:
+    """java.lang.String.hashCode as a signed 32-bit int (UTF-16 code units; these names are ASCII)."""
+    h = 0
+    for ch in text:
+        h = (31 * h + ord(ch)) & 0xFFFFFFFF
+    return h - (1 << 32) if h >> 31 else h
+
+
+# Spark's HasSeed default: this.getClass.getName.hashCode.toLong
+DEFAULT_SEED = java_hash("org.apache.spark.ml.classification.RandomForestClassifier")
+
+
+def splitmix(z):
+    """splitmix64's step of uint64 values: add the golden-ratio increment, then the finaliser (k_rf_level's rf_mix)."""
+    with np.errstate(over="ignore"):
+        z = np.asarray(z, np.uint64) + np.uint64(0x9E3779B97F4A7C15)
+        z = (z ^ (z >> np.uint64(30))) * np.uint64(0xBF58476D1CE4E5B9)
+        z = (z ^ (z >> np.uint64(27))) * np.uint64(0x94D049BB133111EB)
+        return z ^ (z >> np.uint64(31))
+
+
+def subset_size(strategy: str, k: int, num_trees: int) -> int:
+    """The features m a node searches (DecisionTreeMetadata.buildMetadata): "auto" is "all" for one tree, else "sqrt";
+    "all" k, "sqrt" ceil(sqrt k), "log2" max(1, ceil(log2 k)), "onethird" ceil(k / 3), an integer string n: min(n,
+    k), a real string r in (0, 1]: ceil(r k), each in f64 as Spark computes it.  Anything else is a ValueError."""
+    import re
+    s = strategy.lower() if isinstance(strategy, str) else None
+    if s == "auto":
+        s = "all" if num_trees == 1 else "sqrt"
+    if s == "all":
+        return k
+    if s == "sqrt":
+        return int(math.ceil(math.sqrt(k)))
+    if s == "log2":
+        return max(1, int(math.ceil(math.log(k) / math.log(2))))
+    if s == "onethird":
+        return int(math.ceil(k / 3.0))
+    if s is not None and re.fullmatch(r"[1-9]\d*", s):
+        return min(int(s), k)
+    if s is not None and re.fullmatch(r"0?\.\d*[1-9]\d*|1\.0+", s):
+        return int(math.ceil(float(s) * k))
+    raise ValueError(f"feature_subset_strategy must be one of {list(STRATEGIES)}, an integer n > 0 or a real in (0, 1] "
+                     f"as a string, not {strategy!r}")
+
+
+def draw_table(num_trees: int, rate: float) -> list[int]:
+    """The bagging thresholds T (ascending u64) of lo_rf_level: a row's weight is #{j : u >= T_j}.  One tree at rate 1:
+    [0] (every weight 1); one tree below rate 1: Bernoulli, [floor(2^64 (1 - rate))]; several trees: Poisson(rate),
+    T_j = floor(2^64 P(X <= j)) for j = 0 and every later j whose T_j is below 2^64 - 1.  Computed in 60-digit decimal
+    from the exact value of ``rate`` (e^-rate correctly rounded there), never with floating exp."""
+    from decimal import ROUND_FLOOR, Decimal, localcontext
+    from fractions import Fraction
+    if num_trees == 1:
+        return [0] if rate == 1.0 else [math.floor((1 - Fraction(rate)) * (1 << 64))]
+    with localcontext() as ctx:
+        ctx.prec = 60
+        lam = Decimal(rate)
+        term = (-lam).exp()
+        cdf, out, j = term, [], 0
+        while True:
+            t = int((cdf * (1 << 64)).to_integral_value(rounding=ROUND_FLOOR))
+            if j > 0 and t >= M64:
+                break
+            out.append(min(t, M64))
+            j += 1
+            term = term * lam / j
+            cdf += term
+    if len(out) > MAX_DRAWS:
+        raise ValueError(f"the bagging table of rate {rate!r} needs {len(out)} entries, LO_RF_MAX_DRAWS = {MAX_DRAWS}")
+    return out
+
+
+def feature_subset(seed: int, tree: int, node: int, k: int, m: int) -> np.ndarray:
+    """The m features (ascending) node ``node`` (Spark's index) of tree ``tree`` searches: those with the m least keys
+    splitmix(splitmix(splitmix(splitmix(~seed) ^ tree) ^ node) ^ j), ties by feature index; every feature when m == k."""
+    if m >= k:
+        return np.arange(k, dtype=np.int32)
+    base = splitmix(splitmix(splitmix(np.uint64(~seed & M64)) ^ np.uint64(tree)) ^ np.uint64(node))
+    keys = splitmix(base ^ np.arange(k, dtype=np.uint64))
+    return np.sort(np.lexsort((np.arange(k), keys))[:m]).astype(np.int32)
+
+
+def votes(tree: Tree) -> np.ndarray:
+    """Every node's class counts over their total (summed in class order), each division rounded on its own; 0 for a
+    node of no counts, so that such a leaf casts no vote (RandomForestClassificationModel.predictRaw)."""
+    counts = tree.counts
+    total = np.zeros(len(counts))
+    for c in range(counts.shape[1]):
+        total = total + counts[:, c]
+    with np.errstate(invalid="ignore", divide="ignore"):
+        return np.where(total[:, None] == 0, 0.0, counts / total[:, None])

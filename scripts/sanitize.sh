@@ -56,6 +56,15 @@ gb_race_log="$(mktemp -d)/sanitizer_racecheck_gbt.txt"
 timeout 1800 compute-sanitizer --tool racecheck --error-exitcode 1 python -m pytest tests/test_gpu_gbt.py -q \
     -k "route or edges" > "$gb_race_log" 2>&1
 echo "racecheck (gbt) rc=$? log=$gb_race_log"; tail -3 "$gb_race_log"
+# memcheck and racecheck of the RandomForest kernels (every level route and tree batch, transform and evaluate with
+# votes in registers and in the row's slice; the edges and refusals); their logs go to a temporary directory
+rf_log="$(mktemp -d)/sanitizer_memcheck_rf.txt"
+timeout 1800 compute-sanitizer --tool memcheck --error-exitcode 1 python -m pytest tests/test_gpu_rf.py -q > "$rf_log" 2>&1
+echo "memcheck (rf) rc=$? log=$rf_log"; tail -3 "$rf_log"
+rf_race_log="$(mktemp -d)/sanitizer_racecheck_rf.txt"
+timeout 1800 compute-sanitizer --tool racecheck --error-exitcode 1 python -m pytest tests/test_gpu_rf.py -q \
+    -k "route or edges" > "$rf_race_log" 2>&1
+echo "racecheck (rf) rc=$? log=$rf_race_log"; tail -3 "$rf_race_log"
 # memcheck of the number parser and the resident formatter on every entry point, without the million-row cases: a read
 # past the last staged cell shows here (the CPU harness puts a NUL after it)
 parse_log="$(mktemp -d)/sanitizer_memcheck_parse.txt"
