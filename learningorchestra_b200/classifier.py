@@ -17,6 +17,7 @@ RandomForestClassifier grows batches of trees together on the same codes, one pa
 forest's votes are summed per row on the device (``lo_rf_predict``)."""
 from __future__ import annotations
 
+import contextlib
 import math
 
 import numpy as np
@@ -406,6 +407,54 @@ def _tree_params(est, max_depth, max_bins, min_instances_per_node, min_info_gain
     est.min_info_gain = g
 
 
+def _impurity(impurity) -> str:
+    """DecisionTreeClassifier's and RandomForestClassifier's ``impurity``, one of tree.IMPURITIES in any case."""
+    from . import tree as T
+    if not isinstance(impurity, str) or impurity.lower() not in T.IMPURITIES:
+        raise ValueError(f"impurity must be one of {list(T.IMPURITIES)}, not {impurity!r}")
+    return impurity.lower()
+
+
+def _rate(v, name: str) -> float:
+    """A real in (0, 1]: GBTClassifier's ``step_size``, RandomForestClassifier's ``subsampling_rate``."""
+    r = float(v) if isinstance(v, (int, float, np.floating)) and not isinstance(v, bool) else float("nan")
+    if not 0.0 < r <= 1.0:
+        raise ValueError(f"{name} must lie in (0, 1], not {v!r}")
+    return r
+
+
+def _classes(features, name: str) -> tuple[int, int]:
+    """(n, numClasses = max label + 1) of DecisionTreeClassifier's and RandomForestClassifier's features (lo_lr_stats:
+    every label an integer >= 0 and every feature finite).  No row and more than LO_DT_MAX_CLASSES classes are refused."""
+    _labelled(features, name)
+    n, _total, _m2, counts = _on_device(features, lambda engine, rows: engine.lr_stats(rows), name=name,
+                                        reasons=_LR_REASONS)
+    _some_rows(n, name)
+    num_classes = int(np.flatnonzero(counts)[-1]) + 1
+    if num_classes > N.LO_DT_MAX_CLASSES:
+        raise N.LoexecError(N.LO_ERR_INVALID, f"{num_classes} classes exceed LO_DT_MAX_CLASSES = "
+                            f"{N.LO_DT_MAX_CLASSES}")
+    return n, num_classes
+
+
+@contextlib.contextmanager
+def _binned(features, n: int, max_bins: int, name: str, kf: int, per_bin: int, unit: str):
+    """The tree fits' codes, after refusing a one-node histogram (kf features x min(max_bins, n) bins x per_bin u64
+    ``unit``) above LO_DT_PASS_HIST: yields (:func:`split_thresholds`' thresholds and rank rounds, nbins, the rows binned
+    on the device by ``dt_bin``) and frees the codes when the block ends."""
+    k = len(features.fields)
+    if kf * min(max_bins, n) * per_bin * 8 > N.LO_DT_PASS_HIST:
+        raise N.LoexecError(N.LO_ERR_INVALID, f"{kf} features x {min(max_bins, n)} bins x {per_bin} {unit}: one node's "
+                            f"histogram exceeds LO_DT_PASS_HIST = {N.LO_DT_PASS_HIST} bytes")
+    thresholds, rounds = split_thresholds(features, n, k, max_bins, name)
+    nbins = max(len(t) for t in thresholds) + 1
+    binned = _on_device(features, lambda engine, rows: engine.dt_bin(rows, thresholds), name=name)
+    try:
+        yield thresholds, rounds, nbins, binned
+    finally:
+        _free(binned)
+
+
 class DecisionTreeClassifier:
     """``pyspark.ml.classification.DecisionTreeClassifier(maxDepth, maxBins, minInstancesPerNode, minInfoGain,
     impurity)`` with its other defaults (every feature continuous, no ``weightCol``, no ``thresholds``) on the GPU.
@@ -413,11 +462,8 @@ class DecisionTreeClassifier:
 
     def __init__(self, max_depth: int = 5, max_bins: int = 32, min_instances_per_node: int = 1,
                  min_info_gain: float = 0.0, impurity: str = "gini"):
-        from . import tree as T
         _tree_params(self, max_depth, max_bins, min_instances_per_node, min_info_gain)
-        if not isinstance(impurity, str) or impurity.lower() not in T.IMPURITIES:
-            raise ValueError(f"impurity must be one of {list(T.IMPURITIES)}, not {impurity!r}")
-        self.impurity = impurity.lower()
+        self.impurity = _impurity(impurity)
 
     def fit(self, features) -> "DecisionTreeClassificationModel":
         """The tree of ``features`` (:class:`~builder_frontend.Features` with a label, on one GPU or sharded).  Every
@@ -426,29 +472,14 @@ class DecisionTreeClassifier:
         histogram (k x min(max_bins, n) x C x 8 bytes) above LO_DT_PASS_HIST are refused."""
         from . import tree as T
         name, k = "DecisionTreeClassifier", len(features.fields)
-        _labelled(features, name)
-        n, _total, _m2, counts = _on_device(features, lambda engine, rows: engine.lr_stats(rows), name=name,
-                                            reasons=_LR_REASONS)
-        _some_rows(n, name)
-        num_classes = int(np.flatnonzero(counts)[-1]) + 1
-        if num_classes > N.LO_DT_MAX_CLASSES:
-            raise N.LoexecError(N.LO_ERR_INVALID, f"{num_classes} classes exceed LO_DT_MAX_CLASSES = "
-                                f"{N.LO_DT_MAX_CLASSES}")
-        if k * min(self.max_bins, n) * num_classes * 8 > N.LO_DT_PASS_HIST:
-            raise N.LoexecError(N.LO_ERR_INVALID, f"{k} features x {min(self.max_bins, n)} bins x {num_classes} classes: "
-                                f"one node's histogram exceeds LO_DT_PASS_HIST = {N.LO_DT_PASS_HIST} bytes")
-        thresholds, rounds = split_thresholds(features, n, k, self.max_bins, name)
-        nbins = max(len(t) for t in thresholds) + 1
-        binned = _on_device(features, lambda engine, rows: engine.dt_bin(rows, thresholds), name=name)
-        try:
+        n, num_classes = _classes(features, name)
+        with _binned(features, n, self.max_bins, name, k, num_classes, "classes") as (thresholds, rounds, nbins, binned):
             def level(splits, nnodes):
                 return _on_device(features, lambda engine, rows: engine.dt_level(rows, binned, nbins, num_classes,
                                                                                 splits, nnodes), name=name)
 
             tree, _shapes = T.grow(level, thresholds, num_classes, self.max_depth, self.impurity,
                                    self.min_instances_per_node, self.min_info_gain)
-        finally:
-            _free(binned)
         model = DecisionTreeClassificationModel(tree, features.fields, thresholds)
         model.rank_rounds = rounds
         return model
@@ -486,11 +517,7 @@ class GBTClassifier:
     def __init__(self, max_iter: int = 20, step_size: float = 0.1, max_depth: int = 5, max_bins: int = 32,
                  min_instances_per_node: int = 1, min_info_gain: float = 0.0):
         self.max_iter = _integer(max_iter, "max_iter", 1)
-        st = float(step_size) if isinstance(step_size, (int, float, np.floating)) and not isinstance(step_size, bool) \
-            else float("nan")
-        if not 0.0 < st <= 1.0:
-            raise ValueError(f"step_size must lie in (0, 1], not {step_size!r}")
-        self.step_size = st
+        self.step_size = _rate(step_size, "step_size")
         _tree_params(self, max_depth, max_bins, min_instances_per_node, min_info_gain)
 
     def fit(self, features) -> "GBTClassificationModel":
@@ -504,7 +531,7 @@ class GBTClassifier:
         from .engine import InvalidCellError
         # the labels (lo_gb_update's first call) and the features (lo_lr_stats_range) are both checked, and the lowest
         # refused cell of the two is raised, as one pass over both would find it
-        refused, rows, binned = [], None, None
+        refused, rows = [], None
         try:
             rows = _on_device(features, lambda engine, part: engine.gb_update(part), name=name, reasons=_GB_REASONS)
         except InvalidCellError as e:
@@ -520,30 +547,23 @@ class GBTClassifier:
             if refused:
                 raise min(refused, key=lambda e: (e.row, e.position))
             _some_rows(n, name)
-            if k * min(self.max_bins, n) * N.LO_GB_WORDS * 8 > N.LO_DT_PASS_HIST:
-                raise N.LoexecError(N.LO_ERR_INVALID, f"{k} features x {min(self.max_bins, n)} bins x "
-                                    f"{N.LO_GB_WORDS} words: one node's histogram exceeds LO_DT_PASS_HIST = "
-                                    f"{N.LO_DT_PASS_HIST} bytes")
-            thresholds, _rounds = split_thresholds(features, n, k, self.max_bins, name)
-            nbins = max(len(t) for t in thresholds) + 1
-            binned = _on_device(features, lambda engine, part: engine.dt_bin(part, thresholds), name=name)
             trees, weights = [], []
-            for m in range(self.max_iter):
-                def level(splits, nnodes):
-                    return _on_device(features, lambda engine, part: engine.gb_level(part, binned, rows, nbins, splits,
-                                                                                    nnodes), name=name)
+            with _binned(features, n, self.max_bins, name, k, N.LO_GB_WORDS, "words") as (thresholds, _, nbins, binned):
+                for m in range(self.max_iter):
+                    def level(splits, nnodes):
+                        return _on_device(features, lambda engine, part: engine.gb_level(part, binned, rows, nbins,
+                                                                                        splits, nnodes), name=name)
 
-                tree, _shapes = T.grow(level, thresholds, 0, self.max_depth, T.VARIANCE, self.min_instances_per_node,
-                                       self.min_info_gain)
-                weight = 1.0 if m == 0 else self.step_size
-                trees.append(tree)
-                weights.append(weight)
-                if m + 1 < self.max_iter:
-                    _on_device(features, lambda engine, part: engine.gb_update(part, rows, tree, weight), name=name,
-                               reasons=_GB_REASONS)
+                    tree, _shapes = T.grow(level, thresholds, 0, self.max_depth, T.VARIANCE,
+                                           self.min_instances_per_node, self.min_info_gain)
+                    weight = 1.0 if m == 0 else self.step_size
+                    trees.append(tree)
+                    weights.append(weight)
+                    if m + 1 < self.max_iter:
+                        _on_device(features, lambda engine, part: engine.gb_update(part, rows, tree, weight), name=name,
+                                   reasons=_GB_REASONS)
         finally:
             _free(rows)
-            _free(binned)
         return GBTClassificationModel(trees, weights, features.fields, thresholds)
 
 
@@ -586,16 +606,10 @@ class RandomForestClassifier:
         from . import tree as T
         self.num_trees = _integer(num_trees, "num_trees", 1)
         _tree_params(self, max_depth, max_bins, min_instances_per_node, min_info_gain)
-        if not isinstance(impurity, str) or impurity.lower() not in T.IMPURITIES:
-            raise ValueError(f"impurity must be one of {list(T.IMPURITIES)}, not {impurity!r}")
-        self.impurity = impurity.lower()
+        self.impurity = _impurity(impurity)
         T.subset_size(feature_subset_strategy, 1, self.num_trees)          # refuses an unknown strategy now
         self.feature_subset_strategy = feature_subset_strategy
-        rate = float(subsampling_rate) if isinstance(subsampling_rate, (int, float, np.floating)) \
-            and not isinstance(subsampling_rate, bool) else float("nan")
-        if not 0.0 < rate <= 1.0:
-            raise ValueError(f"subsampling_rate must lie in (0, 1], not {subsampling_rate!r}")
-        self.subsampling_rate = rate
+        self.subsampling_rate = _rate(subsampling_rate, "subsampling_rate")
         self.seed = T.DEFAULT_SEED if seed is None else _integer(seed, "seed", -(1 << 63), (1 << 63) - 1)
 
     def fit(self, features) -> "RandomForestClassificationModel":
@@ -606,25 +620,12 @@ class RandomForestClassifier:
         refused.  The trees grow in batches whose slot tables fit _RF_SLOT_BUDGET, one level pass per batch level."""
         from . import tree as T
         name, k = "RandomForestClassifier", len(features.fields)
-        _labelled(features, name)
-        n, _total, _m2, counts = _on_device(features, lambda engine, rows: engine.lr_stats(rows), name=name,
-                                            reasons=_LR_REASONS)
-        _some_rows(n, name)
-        num_classes = int(np.flatnonzero(counts)[-1]) + 1
-        if num_classes > N.LO_DT_MAX_CLASSES:
-            raise N.LoexecError(N.LO_ERR_INVALID, f"{num_classes} classes exceed LO_DT_MAX_CLASSES = "
-                                f"{N.LO_DT_MAX_CLASSES}")
+        n, num_classes = _classes(features, name)
         m = T.subset_size(self.feature_subset_strategy, k, self.num_trees)
-        if m * min(self.max_bins, n) * num_classes * 8 > N.LO_DT_PASS_HIST:
-            raise N.LoexecError(N.LO_ERR_INVALID, f"{m} features x {min(self.max_bins, n)} bins x {num_classes} classes: "
-                                f"one node's histogram exceeds LO_DT_PASS_HIST = {N.LO_DT_PASS_HIST} bytes")
         draw = T.draw_table(self.num_trees, self.subsampling_rate)
-        thresholds, _rounds = split_thresholds(features, n, k, self.max_bins, name)
-        nbins = max(len(t) for t in thresholds) + 1
         batch = max(1, min(self.num_trees, _RF_SLOT_BUDGET // (8 * n)))
-        binned = _on_device(features, lambda engine, rows: engine.dt_bin(rows, thresholds), name=name)
         trees = []
-        try:
+        with _binned(features, n, self.max_bins, name, m, num_classes, "classes") as (thresholds, _, nbins, binned):
             for tree0 in range(0, self.num_trees, batch):
                 ntrees = min(batch, self.num_trees - tree0)
 
@@ -636,8 +637,6 @@ class RandomForestClassifier:
                                         self.min_instances_per_node, self.min_info_gain, trees=ntrees,
                                         subsets=lambda t, node: T.feature_subset(self.seed, tree0 + t, node, k, m))
                 trees += grown
-        finally:
-            _free(binned)
         model = RandomForestClassificationModel(trees, features.fields, thresholds, m)
         model.tree_batch = batch
         return model

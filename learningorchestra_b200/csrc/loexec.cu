@@ -2713,6 +2713,16 @@ struct PredictFrame {
         c.memset(conf, 0, (size_t)neval * CO * 8);
         bad.arm(c);
     }
+    // The shared memory of a tree model's kernel (k_dt_predict, k_gb_predict, k_rf_predict): its model_bytes when they
+    // fit lo::kDtTreeSmem beside evaluate's labels (*model_smem), then evaluate's counts when they fit too (*hist_smem);
+    // returns the bytes
+    int tree_smem(int64_t model_bytes, bool *model_smem, bool *hist_smem) const {
+        const int64_t evl_bytes = (int64_t)neval * 8, hist_bytes = (int64_t)neval * CO * 4;
+        *model_smem = model_bytes + evl_bytes <= lo::kDtTreeSmem;
+        const int64_t fixed = (*model_smem ? model_bytes : 0) + evl_bytes;
+        *hist_smem = eval && fixed + hist_bytes <= lo::kDtTreeSmem;
+        return (int)(fixed + (*hist_smem ? hist_bytes : 0));
+    }
     // CTAs of `threads` with smem bytes: as many as the SMs hold at once, at most `units`
     template <typename K> static int grid(HostCall &c, K kernel, int threads, int smem, int64_t units) {
         int per_sm = 0;
@@ -3182,6 +3192,38 @@ int check_tree_nodes(const int32_t *feature, const int32_t *left, const int32_t 
     return LO_OK;
 }
 
+// The trees of a forest of M nodes (lo_gb_predict, lo_rf_predict): tree t holds the nodes [start[t], start[t + 1]) (the
+// last up to M), the first from node 0, each checked by check_tree_nodes and then, when weight is given, its weight[t]
+int check_forest(const int32_t *start, int32_t ntrees, int32_t M, const int32_t *feature, const int32_t *left,
+                 const int32_t *right, int32_t k, const double *weight) {
+    for (int32_t t = 0; t < ntrees; ++t) {
+        const int32_t lo = start[t], hi = t + 1 < ntrees ? start[t + 1] : M;
+        if (t == 0 && lo != 0) return fail(LO_ERR_INVALID, "start[0] = %d: the first tree starts at node 0", lo);
+        if (!(hi > lo && hi <= M)) return fail(LO_ERR_INVALID, "tree %d: nodes [%d, %d) of %d", t, lo, hi, M);
+        LO_TRY(check_tree_nodes(feature, left, right, lo, hi, k));
+        if (weight && !std::isfinite(weight[t])) return fail(LO_ERR_INVALID, "weight[%d] = %g is not finite", t, weight[t]);
+    }
+    return LO_OK;
+}
+
+// A tree's or a forest's node arrays on the device as the tree kernels read them: *ints = feature, left, right (M each)
+// and start (ntrees: a forest's first nodes; 0 for one tree); *dbls = threshold (M), the per-node payload (pay values: a
+// leaf value, class counts or votes) and weight (ntrees when given: GBT's forest)
+void stage_nodes(HostCall &c, int32_t M, const int32_t *feature, const int32_t *left, const int32_t *right,
+                 const double *threshold, const double *payload, size_t pay, int32_t ntrees, const int32_t *start,
+                 const double *weight, int **ints, double **dbls) {
+    const size_t nw = weight ? (size_t)ntrees : 0;
+    c.alloc(ints, ((size_t)3 * M + ntrees) * 4);
+    c.alloc(dbls, ((size_t)M + pay + nw) * 8);
+    c.to_dev(*ints, feature, (size_t)M * 4);
+    c.to_dev(*ints + M, left, (size_t)M * 4);
+    c.to_dev(*ints + 2 * M, right, (size_t)M * 4);
+    if (ntrees) c.to_dev(*ints + 3 * M, start, (size_t)ntrees * 4);
+    c.to_dev(*dbls, threshold, (size_t)M * 8);
+    c.to_dev(*dbls + M, payload, pay * 8);
+    if (nw) c.to_dev(*dbls + M + pay, weight, nw * 8);
+}
+
 int check_dt_classes(int32_t nclasses) {
     if (nclasses < 1 || nclasses > LO_DT_MAX_CLASSES)
         return fail(LO_ERR_INVALID, "%d classes outside [1, LO_DT_MAX_CLASSES = %d]", nclasses, LO_DT_MAX_CLASSES);
@@ -3250,7 +3292,7 @@ double dt_value(uint64_t code, bool f32) {
     return v;
 }
 
-// The arguments every level pass checks (tree_level, lo_rf_level), in this order: k, kp, n, the code matrix, nbins, one
+// The arguments every level pass checks (tree_level), in this order: k, kp, n, the code matrix, nbins, one
 // node's histogram of kf features x nbins x C u64 within LO_DT_PASS_HIST, nnodes, route, the slot tables src / dst of
 // `slots` entries (without src: route 0 and `roots` nodes, every row at its tree's root), the parents' splits, hist_out.
 int check_level(const lo_ctx *ctx, const char *per_bin, int32_t C, const lo_table *codes, int64_t kp, int32_t k,
@@ -3299,46 +3341,41 @@ int *level_splits(HostCall &c, int32_t np, const int32_t *splits) {
     return d_split;
 }
 
-// The node-group passes of a level (tree_level, lo_rf_level) by `kernel` with smem bytes: the grid from occupancy over
-// the chunks of sh.fc of kf features, then per group [g0, g0 + gn) of the launch shape d_hist zeroed, launch(grid,
-// from, how, to, g0, gn) enqueued and its per_node * gn words copied to hist_out.  The first pass routes (how = route)
-// from src and writes dst; the later ones read the slots it wrote.
-template <typename K, typename L>
-void level_passes(HostCall &c, K kernel, int smem, const DtShape &sh, int32_t kf, int64_t n, int32_t nnodes,
-                  size_t per_node, const lo_table *src, int32_t route, lo_table *dst, unsigned long long *d_hist,
-                  int64_t *hist_out, L launch) {
-    int per_sm = 0;
-    c.run([&] { return cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem); });
-    c.run([&] { return cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, lo::kDtThreads, smem); });
-    const int nchunks = (kf + sh.fc - 1) / sh.fc;
-    const int64_t want = (int64_t)c.ctx->sm_count * std::max(1, per_sm) / nchunks;
-    const dim3 grid((unsigned)std::max<int64_t>(1, std::min<int64_t>((n + lo::kDtThreads - 1) / lo::kDtThreads, want)),
-                    (unsigned)nchunks);
-    c.mark();
-    for (int pass = 0; pass < sh.passes; ++pass) {
-        const int g0 = pass * sh.gn, gn = std::min(sh.gn, nnodes - g0);
-        const int *from = pass == 0 ? (src ? (const int *)src->base : nullptr) : (const int *)dst->base;
-        c.memset(d_hist, 0, per_node * gn * 8);
-        c.launch(1, [&] { launch(grid, from, pass == 0 ? route : 0, pass == 0 && dst ? (int *)dst->base : nullptr, g0, gn); });
-        c.to_host(hist_out + per_node * g0, d_hist, per_node * gn * 8);
-        c.sync();                                       // d_hist is reused by the next pass
-    }
-    c.mark();
-}
+// One node-group pass of a level as tree_level hands it to its caller's launch: the grid, the shared-memory bytes and
+// stream, the slots read (from, routed when how) and written (to), the parents' splits as the four arrays of
+// level_splits, the node group [g0, g0 + gn), and the histogram and refusal word the kernel writes.
+struct LevelPass {
+    dim3 grid;
+    int smem;
+    cudaStream_t s;
+    const int *from;
+    int how;
+    int *to;
+    const int *sfeat, *sbin, *left, *right;
+    int g0, gn;
+    unsigned long long *hist, *err;
+};
 
-// The checks and passes of one tree level shared by lo_dt_level and lo_gb_level: C u64 words per (node, feature, bin)
-// in hist_out, counted one node group of the launch shape at a time by k_dt_level over the labels y (GB false; C
-// classes, u32 counters of wbytes 4 in shared memory) or by k_gb_level over the residuals y (GB true; C = kGbWords
-// u64 words).  *key receives the lowest refused cell's key (~0: none); hist_out is zeroed when there is one.
-template <bool GB, typename T>
-int tree_level(lo_ctx *ctx, const char *name, const char *per_bin, const T *y, int32_t C, int32_t wbytes,
-               const lo_table *codes, int64_t kp, int32_t k, int64_t n, int32_t nbins, const lo_table *src,
-               int32_t route, lo_table *dst, int32_t nparents, const int32_t *splits, int32_t nnodes, int64_t *hist_out,
-               int32_t *shape_out, lo_host_timing *timing, unsigned long long *key) {
-    *key = ~0ull;
-    LO_TRY(check_level(ctx, per_bin, C, codes, kp, k, n, nbins, k, src, route, dst, n, 1, nparents, splits, nnodes,
-                       hist_out));
-    const DtShape sh = dt_shape(k, nbins, C, nnodes, wbytes);
+// The frame of one tree level (lo_dt_level, lo_gb_level, lo_rf_level): C u64 words per (node, feature, bin) of the kf
+// features each node counts, in hist_out, counted one node group of the launch shape at a time.  What differs is passed
+// in: kf (k, or lo_rf_level's m), the slot tables' length and roots (n and 1, or ntrees * n and ntrees), the counters'
+// width wbytes and `vec` of dt_shape, `check` (the caller's checks after check_level), `prefix` shared-memory bytes
+// before the histogram, and `go(c, sh, run)`, which uploads the caller's own tables and picks the kernel for run(kernel,
+// launch), launch(const LevelPass &) enqueuing one pass.  run sizes the grid from occupancy over the chunks of sh.fc
+// features, then per node group d_hist is zeroed, the pass enqueued and its per_node * gn words copied to hist_out.  The
+// first pass routes (how = route) from src and writes dst; the later ones read the slots it wrote.  A refused cell
+// (lo::cell_key; col k: the row's label or residual) zeroes hist_out and is raised as "row R: <refused>" or as a code
+// >= nbins.
+template <typename Check, typename Go>
+int tree_level(lo_ctx *ctx, const char *name, const char *per_bin, const char *refused, int32_t C, int32_t wbytes,
+               bool vec, const lo_table *codes, int64_t kp, int32_t k, int32_t kf, int64_t n, int32_t nbins,
+               const lo_table *src, int32_t route, lo_table *dst, int64_t slots, int32_t roots, int32_t nparents,
+               const int32_t *splits, int32_t nnodes, int64_t *hist_out, int32_t *shape_out, lo_host_timing *timing,
+               int prefix, Check check, Go go) {
+    LO_TRY(check_level(ctx, per_bin, C, codes, kp, k, n, nbins, kf, src, route, dst, slots, roots, nparents, splits,
+                       nnodes, hist_out));
+    LO_TRY(check());
+    const DtShape sh = dt_shape(kf, nbins, C, nnodes, wbytes, vec);
     if (shape_out) {
         shape_out[0] = sh.vec;
         shape_out[1] = sh.fc;
@@ -3346,7 +3383,7 @@ int tree_level(lo_ctx *ctx, const char *name, const char *per_bin, const T *y, i
         shape_out[3] = sh.passes;
     }
     if (sh.passes > 1 && !dst) return fail(LO_ERR_INVALID, "%d node groups need dst to keep the rows' slots", sh.passes);
-    const size_t per_node = (size_t)k * nbins * C;
+    const size_t per_node = (size_t)kf * nbins * C;
     std::fill(hist_out, hist_out + per_node * nnodes, (int64_t)0);
     HostCall c(ctx, name);
     if (n == 0) return c.finish(timing);
@@ -3355,33 +3392,47 @@ int tree_level(lo_ctx *ctx, const char *name, const char *per_bin, const T *y, i
     bad.arm(c);
     const int np = route ? nparents : 0;
     int *d_split = level_splits(c, np, splits);
-    c.alloc(&d_hist, per_node * sh.gn * 8);
-    auto go = [&](auto kernel) {
-        level_passes(c, kernel, sh.smem, sh, k, n, nnodes, per_node, src, route, dst, d_hist, hist_out,
-                     [&](dim3 grid, const int *from, int how, int *to, int g0, int gn) {
-            if constexpr (GB)
-                kernel<<<grid, lo::kDtThreads, sh.smem, c.s>>>((const unsigned char *)codes->base, kp, k, y, n, nbins,
-                                                               from, how, to, d_split, d_split + np,
-                                                               d_split + 2 * np, d_split + 3 * np, g0, gn, sh.fc,
-                                                               d_hist, bad.word);
-            else
-                kernel<<<grid, lo::kDtThreads, sh.smem, c.s>>>((const unsigned char *)codes->base, kp, k, y, n, nbins,
-                                                               C, from, how, to, d_split, d_split + np,
-                                                               d_split + 2 * np, d_split + 3 * np, g0, gn, sh.fc,
-                                                               d_hist, bad.word);
-        });
-    };
-    if constexpr (GB) {
-        if (sh.vec) go(lo::k_gb_level<true>); else go(lo::k_gb_level<false>);
-    } else {
-        if (sh.vec) go(lo::k_dt_level<T, true>); else go(lo::k_dt_level<T, false>);
-    }
+    const int smem = prefix + sh.smem;
+    go(c, sh, [&](auto kernel, auto launch) {
+        c.alloc(&d_hist, per_node * sh.gn * 8);
+        int per_sm = 0;
+        c.run([&] { return cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem); });
+        c.run([&] { return cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, lo::kDtThreads, smem); });
+        const int nchunks = (kf + sh.fc - 1) / sh.fc;
+        const int64_t want = (int64_t)c.ctx->sm_count * std::max(1, per_sm) / nchunks;
+        const dim3 grid((unsigned)std::max<int64_t>(1, std::min<int64_t>((n + lo::kDtThreads - 1) / lo::kDtThreads, want)),
+                        (unsigned)nchunks);
+        c.mark();
+        for (int pass = 0; pass < sh.passes; ++pass) {
+            const int g0 = pass * sh.gn, gn = std::min(sh.gn, nnodes - g0);
+            const int *from = pass == 0 ? (src ? (const int *)src->base : nullptr) : (const int *)dst->base;
+            int *to = pass == 0 && dst ? (int *)dst->base : nullptr;
+            c.memset(d_hist, 0, per_node * gn * 8);
+            c.launch(1, [&] {
+                launch(LevelPass{grid, smem, c.s, from, pass == 0 ? route : 0, to, d_split, d_split + np,
+                                 d_split + 2 * np, d_split + 3 * np, g0, gn, d_hist, bad.word});
+            });
+            c.to_host(hist_out + per_node * g0, d_hist, per_node * gn * 8);
+            c.sync();                                   // d_hist is reused by the next pass
+        }
+        c.mark();
+    });
     bad.read(c);
     LO_TRY(c.finish(timing));
-    *key = bad.key;
-    if (bad.key != ~0ull) std::fill(hist_out, hist_out + per_node * nnodes, (int64_t)0);
-    return LO_OK;
+    if (bad.key == ~0ull) return LO_OK;
+    std::fill(hist_out, hist_out + per_node * nnodes, (int64_t)0);
+    int64_t row = 0;
+    int32_t col = 0;
+    lo::cell_of_key(bad.key, k, &row, &col);
+    if (col == k) return fail(LO_ERR_INVALID, "row %lld: %s", (long long)row, refused);
+    return fail(LO_ERR_INVALID, "row %lld, feature %d: code >= nbins = %d", (long long)row, col, nbins);
 }
+
+// lo_dt_level's and lo_rf_level's refusal of a label: "its label is not a class in [0, C)"
+std::string not_a_class(int32_t C) { return "its label is not a class in [0, " + std::to_string(C) + ")"; }
+
+// tree_level's `check` of lo_dt_level and lo_gb_level: nothing beyond check_level
+int no_check() { return LO_OK; }
 
 }  // namespace
 
@@ -3529,21 +3580,24 @@ int lo_dt_level(lo_ctx *ctx, const lo_table *codes, int64_t kp, int32_t k, const
     if (n < 0) return fail(LO_ERR_INVALID, "n = %lld is negative", (long long)n);
     LO_TRY(check_float_table(ctx, y, 0, n, "y"));
     LO_TRY(check_dt_classes(nclasses));
-    unsigned long long key = ~0ull;
-    if (y->dtype == LO_F32)
-        LO_TRY(tree_level<false>(ctx, "dt_level", "classes", (const float *)y->base, nclasses, 4,
-                          codes, kp, k, n, nbins, src, route, dst, nparents, splits, nnodes, hist_out, shape_out, timing,
-                          &key));
-    else
-        LO_TRY(tree_level<false>(ctx, "dt_level", "classes", (const double *)y->base, nclasses,
-                          4, codes, kp, k, n, nbins, src, route, dst, nparents, splits, nnodes, hist_out, shape_out,
-                          timing, &key));
-    if (key == ~0ull) return LO_OK;
-    int64_t row = 0;
-    int32_t col = 0;
-    lo::cell_of_key(key, k, &row, &col);
-    if (col == k) return fail(LO_ERR_INVALID, "row %lld: its label is not a class in [0, %d)", (long long)row, nclasses);
-    return fail(LO_ERR_INVALID, "row %lld, feature %d: code >= nbins = %d", (long long)row, col, nbins);
+    return tree_level(ctx, "dt_level", "classes", not_a_class(nclasses).c_str(), nclasses, 4, true, codes, kp, k, k, n,
+                      nbins, src, route, dst, n, 1, nparents, splits, nnodes, hist_out, shape_out, timing, 0, no_check,
+                      [&](HostCall &, const DtShape &sh, auto run) {
+        auto go = [&](auto kernel, auto tag) {
+            using T = decltype(tag);
+            run(kernel, [&](const LevelPass &p) {
+                kernel<<<p.grid, lo::kDtThreads, p.smem, p.s>>>((const unsigned char *)codes->base, kp, k,
+                                                                (const T *)y->base, n, nbins, nclasses, p.from, p.how,
+                                                                p.to, p.sfeat, p.sbin, p.left, p.right, p.g0, p.gn,
+                                                                sh.fc, p.hist, p.err);
+            });
+        };
+        if (y->dtype == LO_F32) {
+            if (sh.vec) go(lo::k_dt_level<float, true>, 0.0f); else go(lo::k_dt_level<float, false>, 0.0f);
+        } else {
+            if (sh.vec) go(lo::k_dt_level<double, true>, 0.0); else go(lo::k_dt_level<double, false>, 0.0);
+        }
+    });
 }
 
 int lo_dt_predict(lo_ctx *ctx, const lo_table *x, int64_t ld, int32_t k, int64_t n, int32_t nnodes, const int32_t *feature,
@@ -3562,30 +3616,19 @@ int lo_dt_predict(lo_ctx *ctx, const lo_table *x, int64_t ld, int32_t k, int64_t
     LO_TRY(f.check_out(ctx, n, C, prob, raw, pred));
     HostCall c(ctx, f.call("dt"));
     if (n == 0) return c.finish(timing);
-    const int64_t tree_bytes = (int64_t)M * 8 + ((int64_t)3 * M + 1) / 2 * 8;
-    const int64_t evl_bytes = (int64_t)f.neval * 8, hist_bytes = (int64_t)f.neval * C * 4;
-    const bool tree_smem = tree_bytes + evl_bytes <= lo::kDtTreeSmem;
-    const int64_t fixed = (tree_smem ? tree_bytes : 0) + evl_bytes;
-    const bool hist_smem = f.eval && fixed + hist_bytes <= lo::kDtTreeSmem;
-    const int smem = (int)(fixed + (hist_smem ? hist_bytes : 0));
+    bool tree_smem, hist_smem;
+    const int smem = f.tree_smem((int64_t)M * 8 + ((int64_t)3 * M + 1) / 2 * 8, &tree_smem, &hist_smem);
     int *d_int = nullptr;
-    double *d_thr = nullptr, *d_cnt = nullptr;
-    c.alloc(&d_int, (size_t)M * 12);
-    c.alloc(&d_thr, (size_t)M * 8);
-    c.alloc(&d_cnt, (size_t)M * C * 8);
-    c.to_dev(d_int, feature, (size_t)M * 4);
-    c.to_dev(d_int + M, left, (size_t)M * 4);
-    c.to_dev(d_int + 2 * M, right, (size_t)M * 4);
-    c.to_dev(d_thr, threshold, (size_t)M * 8);
-    c.to_dev(d_cnt, counts, (size_t)M * C * 8);
+    double *d_dbl = nullptr;
+    stage_nodes(c, M, feature, left, right, threshold, counts, (size_t)M * C, 0, nullptr, nullptr, &d_int, &d_dbl);
     f.stage(c);
     auto go = [&](auto kernel, auto tag) {
         using T = decltype(tag);
         const int grid = f.grid(c, kernel, lo::kDtThreads, smem, (n + lo::kDtThreads - 1) / lo::kDtThreads);
         c.mark();
         c.launch(1, [&] {
-            kernel<<<grid, lo::kDtThreads, smem, c.s>>>((const T *)x->base, ld, k, n, M, d_int, d_thr, d_int + M, d_int + 2 * M,
-                                                        d_cnt, C, tree_smem ? 1 : 0, prob ? (double *)prob->base : nullptr,
+            kernel<<<grid, lo::kDtThreads, smem, c.s>>>((const T *)x->base, ld, k, n, M, d_int, d_dbl, d_int + M, d_int + 2 * M,
+                                                        d_dbl + M, C, tree_smem ? 1 : 0, prob ? (double *)prob->base : nullptr,
                                                         raw ? (double *)raw->base : nullptr,
                                                         pred ? (double *)pred->base : nullptr,
                                                         y ? (const T *)y->base : nullptr, f.d_evl, f.neval, f.direct, f.conf,
@@ -3607,16 +3650,20 @@ int lo_gb_level(lo_ctx *ctx, const lo_table *codes, int64_t kp, int32_t k, const
     LO_TRY(check_ctx(ctx));
     if (n < 0) return fail(LO_ERR_INVALID, "n = %lld is negative", (long long)n);
     LO_TRY(check_typed_table(ctx, residual, LO_F64, n, "residual"));
-    unsigned long long key = ~0ull;
-    LO_TRY(tree_level<true>(ctx, "gb_level", "words", (const double *)residual->base, LO_GB_WORDS, 8, codes, kp, k,
-                      n, nbins, src, route, dst, nparents, splits, nnodes, reinterpret_cast<int64_t *>(words_out),
-                      shape_out, timing, &key));
-    if (key == ~0ull) return LO_OK;
-    int64_t row = 0;
-    int32_t col = 0;
-    lo::cell_of_key(key, k, &row, &col);
-    if (col == k) return fail(LO_ERR_INVALID, "row %lld: its residual is NaN or outside [-4, 4]", (long long)row);
-    return fail(LO_ERR_INVALID, "row %lld, feature %d: code >= nbins = %d", (long long)row, col, nbins);
+    return tree_level(ctx, "gb_level", "words", "its residual is NaN or outside [-4, 4]", LO_GB_WORDS, 8, true, codes, kp,
+                      k, k, n, nbins, src, route, dst, n, 1, nparents, splits, nnodes,
+                      reinterpret_cast<int64_t *>(words_out), shape_out, timing, 0, no_check,
+                      [&](HostCall &, const DtShape &sh, auto run) {
+        auto go = [&](auto kernel) {
+            run(kernel, [&](const LevelPass &p) {
+                kernel<<<p.grid, lo::kDtThreads, p.smem, p.s>>>((const unsigned char *)codes->base, kp, k,
+                                                                (const double *)residual->base, n, nbins, p.from, p.how,
+                                                                p.to, p.sfeat, p.sbin, p.left, p.right, p.g0, p.gn,
+                                                                sh.fc, p.hist, p.err);
+            });
+        };
+        if (sh.vec) go(lo::k_gb_level<true>); else go(lo::k_gb_level<false>);
+    });
 }
 
 }  // extern "C"
@@ -3695,15 +3742,7 @@ int lo_gb_update(lo_ctx *ctx, const lo_table *x, int64_t ld, int32_t k, const lo
     double *d_dbl = nullptr;
     RefusedCell bad;
     bad.arm(c);
-    if (M > 0) {
-        c.alloc(&d_int, (size_t)M * 12);
-        c.alloc(&d_dbl, (size_t)M * 16);
-        c.to_dev(d_int, feature, (size_t)M * 4);
-        c.to_dev(d_int + M, left, (size_t)M * 4);
-        c.to_dev(d_int + 2 * M, right, (size_t)M * 4);
-        c.to_dev(d_dbl, threshold, (size_t)M * 8);
-        c.to_dev(d_dbl + M, value, (size_t)M * 8);
-    }
+    if (M > 0) stage_nodes(c, M, feature, left, right, threshold, value, (size_t)M, 0, nullptr, nullptr, &d_int, &d_dbl);
     auto go = [&](auto kernel, auto tag) {
         using T = decltype(tag);
         int per_sm = 0;
@@ -3738,34 +3777,15 @@ int lo_gb_predict(lo_ctx *ctx, const lo_table *x, int64_t ld, int32_t k, int64_t
     if (ntrees < 1 || M < ntrees || !start || !weight || !feature || !threshold || !left || !right || !value)
         return fail(LO_ERR_INVALID, "a forest of %d trees and %d nodes: start, weight, feature, threshold, left, right and "
                     "value are needed", ntrees, M);
-    for (int32_t t = 0; t < ntrees; ++t) {
-        const int32_t lo = start[t], hi = t + 1 < ntrees ? start[t + 1] : M;
-        if (t == 0 && lo != 0)
-            return fail(LO_ERR_INVALID, "start[0] = %d: the first tree starts at node 0", lo);
-        if (!(hi > lo && hi <= M)) return fail(LO_ERR_INVALID, "tree %d: nodes [%d, %d) of %d", t, lo, hi, M);
-        LO_TRY(check_tree_nodes(feature, left, right, lo, hi, k));
-        if (!std::isfinite(weight[t])) return fail(LO_ERR_INVALID, "weight[%d] = %g is not finite", t, weight[t]);
-    }
+    LO_TRY(check_forest(start, ntrees, M, feature, left, right, k, weight));
     LO_TRY(f.check_out(ctx, n, 2, prob, raw, pred));
     HostCall c(ctx, f.call("gb"));
     if (n == 0) return c.finish(timing);
-    const int64_t forest_bytes = ((int64_t)2 * M + ntrees) * 8 + ((int64_t)3 * M + ntrees) * 4;
-    const int64_t evl_bytes = (int64_t)f.neval * 8, hist_bytes = (int64_t)f.neval * 2 * 4;
-    const bool forest_smem = forest_bytes + evl_bytes <= lo::kDtTreeSmem;
-    const int64_t fixed = (forest_smem ? forest_bytes : 0) + evl_bytes;
-    const bool hist_smem = f.eval && fixed + hist_bytes <= lo::kDtTreeSmem;
-    const int smem = (int)(fixed + (hist_smem ? hist_bytes : 0));
+    bool forest_smem, hist_smem;
+    const int smem = f.tree_smem(((int64_t)2 * M + ntrees) * 8 + ((int64_t)3 * M + ntrees) * 4, &forest_smem, &hist_smem);
     int *d_int = nullptr;
     double *d_dbl = nullptr;
-    c.alloc(&d_int, ((size_t)3 * M + ntrees) * 4);
-    c.alloc(&d_dbl, ((size_t)2 * M + ntrees) * 8);
-    c.to_dev(d_int, feature, (size_t)M * 4);
-    c.to_dev(d_int + M, left, (size_t)M * 4);
-    c.to_dev(d_int + 2 * M, right, (size_t)M * 4);
-    c.to_dev(d_int + 3 * M, start, (size_t)ntrees * 4);
-    c.to_dev(d_dbl, threshold, (size_t)M * 8);
-    c.to_dev(d_dbl + M, value, (size_t)M * 8);
-    c.to_dev(d_dbl + 2 * M, weight, (size_t)ntrees * 8);
+    stage_nodes(c, M, feature, left, right, threshold, value, (size_t)M, ntrees, start, weight, &d_int, &d_dbl);
     f.stage(c);
     auto go = [&](auto kernel, auto tag) {
         using T = decltype(tag);
@@ -3808,57 +3828,34 @@ int lo_rf_level(lo_ctx *ctx, const lo_table *codes, int64_t kp, int32_t k, const
     for (int32_t j = 1; j < ndraw; ++j)
         if (draw[j] < draw[j - 1]) return fail(LO_ERR_INVALID, "draw is not ascending at %d", j);
     if (m < 1 || m > k) return fail(LO_ERR_INVALID, "m = %d features per node outside [1, k = %d]", m, k);
-    LO_TRY(check_level(ctx, "classes", nclasses, codes, kp, k, n, nbins, m, src, route, dst, n * ntrees, ntrees, nparents,
-                       splits, nnodes, hist_out));
-    if (!features) return fail(LO_ERR_INVALID, "features is NULL");
-    for (int64_t i = 0; i < (int64_t)nnodes * m; ++i)
-        if (features[i] < 0 || features[i] >= k)
-            return fail(LO_ERR_INVALID, "features[%lld] = %d outside [0, %d)", (long long)i, features[i], k);
-    const DtShape sh = dt_shape(m, nbins, nclasses, nnodes, 4, false);
-    if (shape_out) {
-        shape_out[0] = sh.vec;
-        shape_out[1] = sh.fc;
-        shape_out[2] = sh.gn;
-        shape_out[3] = sh.passes;
-    }
-    if (sh.passes > 1 && !dst) return fail(LO_ERR_INVALID, "%d node groups need dst to keep the rows' slots", sh.passes);
-    const size_t per_node = (size_t)m * nbins * nclasses;
-    std::fill(hist_out, hist_out + per_node * nnodes, (int64_t)0);
-    HostCall c(ctx, "rf_level");
-    if (n == 0) return c.finish(timing);
-    unsigned long long *d_hist = nullptr, *d_draw = nullptr;
-    int *d_feat = nullptr;
-    RefusedCell bad;
-    bad.arm(c);
-    const int np = route ? nparents : 0;
-    int *d_split = level_splits(c, np, splits);
-    c.alloc(&d_draw, (size_t)ndraw * 8);
-    c.alloc(&d_feat, (size_t)nnodes * m * 4);
-    c.to_dev(d_draw, draw, (size_t)ndraw * 8);
-    c.to_dev(d_feat, features, (size_t)nnodes * m * 4);
-    c.alloc(&d_hist, per_node * sh.gn * 8);
-    const int smem = ndraw * 8 + sh.smem;
-    auto go = [&](auto kernel, auto tag) {
-        using T = decltype(tag);
-        level_passes(c, kernel, smem, sh, m, n, nnodes, per_node, src, route, dst, d_hist, hist_out,
-                     [&](dim3 grid, const int *from, int how, int *to, int g0, int gn) {
-            kernel<<<grid, lo::kDtThreads, smem, c.s>>>((const unsigned char *)codes->base, kp, k, (const T *)y->base, n,
-                                                        row0, nbins, nclasses, (unsigned long long)seed, tree0, ntrees,
-                                                        d_draw, ndraw, d_feat, m, from, how, to, d_split, d_split + np,
-                                                        d_split + 2 * np, d_split + 3 * np, g0, gn, sh.fc, d_hist,
-                                                        bad.word);
-        });
+    auto check = [&] {
+        if (!features) return fail(LO_ERR_INVALID, "features is NULL");
+        for (int64_t i = 0; i < (int64_t)nnodes * m; ++i)
+            if (features[i] < 0 || features[i] >= k)
+                return fail(LO_ERR_INVALID, "features[%lld] = %d outside [0, %d)", (long long)i, features[i], k);
+        return LO_OK;
     };
-    if (y->dtype == LO_F32) go(lo::k_rf_level<float>, 0.0f); else go(lo::k_rf_level<double>, 0.0);
-    bad.read(c);
-    LO_TRY(c.finish(timing));
-    if (bad.key == ~0ull) return LO_OK;
-    std::fill(hist_out, hist_out + per_node * nnodes, (int64_t)0);
-    int64_t row = 0;
-    int32_t col = 0;
-    lo::cell_of_key(bad.key, k, &row, &col);
-    if (col == k) return fail(LO_ERR_INVALID, "row %lld: its label is not a class in [0, %d)", (long long)row, nclasses);
-    return fail(LO_ERR_INVALID, "row %lld, feature %d: code >= nbins = %d", (long long)row, col, nbins);
+    return tree_level(ctx, "rf_level", "classes", not_a_class(nclasses).c_str(), nclasses, 4, false, codes, kp, k, m, n,
+                      nbins, src, route, dst, n * ntrees, ntrees, nparents, splits, nnodes, hist_out, shape_out, timing,
+                      ndraw * 8, check, [&](HostCall &c, const DtShape &sh, auto run) {
+        unsigned long long *d_draw = nullptr;
+        int *d_feat = nullptr;
+        c.alloc(&d_draw, (size_t)ndraw * 8);
+        c.alloc(&d_feat, (size_t)nnodes * m * 4);
+        c.to_dev(d_draw, draw, (size_t)ndraw * 8);
+        c.to_dev(d_feat, features, (size_t)nnodes * m * 4);
+        auto go = [&](auto kernel, auto tag) {
+            using T = decltype(tag);
+            run(kernel, [&](const LevelPass &p) {
+                kernel<<<p.grid, lo::kDtThreads, p.smem, p.s>>>((const unsigned char *)codes->base, kp, k,
+                                                                (const T *)y->base, n, row0, nbins, nclasses,
+                                                                (unsigned long long)seed, tree0, ntrees, d_draw, ndraw,
+                                                                d_feat, m, p.from, p.how, p.to, p.sfeat, p.sbin, p.left,
+                                                                p.right, p.g0, p.gn, sh.fc, p.hist, p.err);
+            });
+        };
+        if (y->dtype == LO_F32) go(lo::k_rf_level<float>, 0.0f); else go(lo::k_rf_level<double>, 0.0);
+    });
 }
 
 int lo_rf_predict(lo_ctx *ctx, const lo_table *x, int64_t ld, int32_t k, int64_t n, int32_t ntrees, const int32_t *start,
@@ -3874,31 +3871,16 @@ int lo_rf_predict(lo_ctx *ctx, const lo_table *x, int64_t ld, int32_t k, int64_t
     if (ntrees < 1 || M < ntrees || !start || !feature || !threshold || !left || !right || !votes)
         return fail(LO_ERR_INVALID, "a forest of %d trees and %d nodes: start, feature, threshold, left, right and votes "
                     "are needed", ntrees, M);
-    for (int32_t t = 0; t < ntrees; ++t) {
-        const int32_t lo = start[t], hi = t + 1 < ntrees ? start[t + 1] : M;
-        if (t == 0 && lo != 0) return fail(LO_ERR_INVALID, "start[0] = %d: the first tree starts at node 0", lo);
-        if (!(hi > lo && hi <= M)) return fail(LO_ERR_INVALID, "tree %d: nodes [%d, %d) of %d", t, lo, hi, M);
-        LO_TRY(check_tree_nodes(feature, left, right, lo, hi, k));
-    }
+    LO_TRY(check_forest(start, ntrees, M, feature, left, right, k, nullptr));
     LO_TRY(f.check_out(ctx, n, C, prob, raw, pred));
     HostCall c(ctx, f.call("rf"));
     if (n == 0) return c.finish(timing);
-    const int64_t forest_bytes = ((int64_t)M + (int64_t)M * C) * 8 + ((int64_t)3 * M + ntrees) * 4;
-    const int64_t evl_bytes = (int64_t)f.neval * 8, hist_bytes = (int64_t)f.neval * C * 4;
-    const bool forest_smem = forest_bytes + evl_bytes <= lo::kDtTreeSmem;
-    const int64_t fixed = (forest_smem ? forest_bytes : 0) + evl_bytes;
-    const bool hist_smem = f.eval && fixed + hist_bytes <= lo::kDtTreeSmem;
-    const int smem = (int)(fixed + (hist_smem ? hist_bytes : 0));
+    bool forest_smem, hist_smem;
+    const int smem = f.tree_smem(((int64_t)M + (int64_t)M * C) * 8 + ((int64_t)3 * M + ntrees) * 4, &forest_smem,
+                                 &hist_smem);
     int *d_int = nullptr;
     double *d_dbl = nullptr;
-    c.alloc(&d_int, ((size_t)3 * M + ntrees) * 4);
-    c.alloc(&d_dbl, ((size_t)M + (size_t)M * C) * 8);
-    c.to_dev(d_int, feature, (size_t)M * 4);
-    c.to_dev(d_int + M, left, (size_t)M * 4);
-    c.to_dev(d_int + 2 * M, right, (size_t)M * 4);
-    c.to_dev(d_int + 3 * M, start, (size_t)ntrees * 4);
-    c.to_dev(d_dbl, threshold, (size_t)M * 8);
-    c.to_dev(d_dbl + M, votes, (size_t)M * C * 8);
+    stage_nodes(c, M, feature, left, right, threshold, votes, (size_t)M * C, ntrees, start, nullptr, &d_int, &d_dbl);
     f.stage(c);
     auto go = [&](auto kernel, auto tag) {
         using T = decltype(tag);

@@ -166,10 +166,44 @@ __global__ void __launch_bounds__(kDtThreads) k_dt_bin(const T *__restrict__ x, 
     }
 }
 
-// One pass of a tree level over every row.  A row's slot at this level: src == NULL, the root (0); route, its parent's
-// slot p = src[r] sent by the parent's split (sfeat[p] < 0: the parent is a leaf, so is the row: -1) to left[p] when
-// its code of feature sfeat[p] is <= sbin[p], else right[p] (-1: a leaf child); !route, src[r] itself.  CTAs of
-// blockIdx.y == 0 write the slot to dst (when given).  A row whose slot lies in the pass's node group [g0, g0 + gn)
+// A row's slot at this level from its slot s at the previous one (k_dt_level, k_gb_level, k_rf_level): route, s sent by
+// its split (sfeat[s] < 0: s is a leaf, so is the row: -1) to left[s] when the row's code of feature sfeat[s] is <=
+// sbin[s], else right[s] (-1: a leaf child); !route, s itself.
+__device__ __forceinline__ int dt_route(int s, int route, const unsigned char *row, const int *__restrict__ sfeat,
+                                        const int *__restrict__ sbin, const int *__restrict__ left,
+                                        const int *__restrict__ right) {
+    if (route && s >= 0) {
+        const int f = sfeat[s];
+        s = f < 0 ? -1 : (int)row[f] <= sbin[s] ? left[s] : right[s];
+    }
+    return s;
+}
+
+// The leaf a row xr reaches from `node` (k_dt_predict, k_gb_update, k_gb_predict, k_rf_predict): an internal node (fe
+// >= 0) sends it left when its value of feature fe[node] widened to f64 is <= th[node].
+template <typename T>
+__device__ __forceinline__ int dt_walk(const T *xr, int node, const int *fe, const double *th, const int *le,
+                                       const int *ri) {
+    int f;
+    while ((f = fe[node]) >= 0) node = (double)xr[f] <= th[node] ? le[node] : ri[node];
+    return node;
+}
+
+// A CTA's u32 counters hist[gn][fc][cell] into out[gn][kf][cell] (u64, integer atomics) from feature j0 of the kf
+// (k_dt_level, k_rf_level): the fw features of its chunk, zero counters skipped.
+__device__ __forceinline__ void dt_flush(const unsigned *hist, int cells, int fc, int cell, int fw, int kf, int j0,
+                                         unsigned long long *__restrict__ out) {
+    for (int i = threadIdx.x; i < cells; i += kDtThreads) {
+        const unsigned v = hist[i];
+        if (!v) continue;
+        const int g = i / (fc * cell), rest = i - g * fc * cell, f = rest / cell;
+        if (f >= fw) continue;
+        atomicAdd(&out[((size_t)g * kf + j0 + f) * cell + (rest - f * cell)], (unsigned long long)v);
+    }
+}
+
+// One pass of a tree level over every row.  A row's slot at this level: src == NULL, the root (0); else dt_route of
+// src[r].  CTAs of blockIdx.y == 0 write the slot to dst (when given).  A row whose slot lies in the pass's node group [g0, g0 + gn)
 // adds one to hist[slot - g0][f][code][class] for each feature f of the CTA's chunk [blockIdx.y * fc, + fc): u32
 // counters in shared memory, flushed once per CTA into out ([gn][k][nbins][C], u64) with integer atomics.  VEC: the
 // chunk's codes of a row in 16-byte loads (fc and the code pitch kp multiples of 16).  A code >= nbins or a label that
@@ -192,14 +226,7 @@ __global__ void __launch_bounds__(kDtThreads) k_dt_level(const unsigned char *__
     unsigned long long bad = ~0ull;
     for (long long r = blockIdx.x * (long long)kDtThreads + threadIdx.x; r < n; r += (long long)gridDim.x * kDtThreads) {
         const unsigned char *row = codes + r * kp;
-        int s = 0;
-        if (src) {
-            s = src[r];
-            if (route && s >= 0) {
-                const int f = sfeat[s];
-                s = f < 0 ? -1 : (int)row[f] <= sbin[s] ? left[s] : right[s];
-            }
-        }
+        const int s = src ? dt_route(src[r], route, row, sfeat, sbin, left, right) : 0;
         if (write) dst[r] = s;
         if (s < g0 || s >= g0 + gn) continue;
         const double lab = (double)y[r];
@@ -231,13 +258,7 @@ __global__ void __launch_bounds__(kDtThreads) k_dt_level(const unsigned char *__
     }
     report_cell(bad, err);
     __syncthreads();
-    for (int i = threadIdx.x; i < cells; i += kDtThreads) {
-        const unsigned v = dt_hist[i];
-        if (!v) continue;
-        const int g = i / (fc * cell), rest = i - g * fc * cell, f = rest / cell;
-        if (f >= fw) continue;
-        atomicAdd(&out[((size_t)g * k + j0 + f) * cell + (rest - f * cell)], (unsigned long long)v);
-    }
+    dt_flush(dt_hist, cells, fc, cell, fw, k, j0, out);
 }
 
 // GBT's regression sums per (node, feature, bin) (DESIGN.md §3.6.5): kGbWords u64 words, the count, Σ(q1 + 2^60) and
@@ -296,14 +317,7 @@ __global__ void __launch_bounds__(kDtThreads) k_gb_level(const unsigned char *__
     unsigned long long bad = ~0ull;
     for (long long r = blockIdx.x * (long long)kDtThreads + threadIdx.x; r < n; r += (long long)gridDim.x * kDtThreads) {
         const unsigned char *row = codes + r * kp;
-        int s = 0;
-        if (src) {
-            s = src[r];
-            if (route && s >= 0) {
-                const int f = sfeat[s];
-                s = f < 0 ? -1 : (int)row[f] <= sbin[s] ? left[s] : right[s];
-            }
-        }
+        const int s = src ? dt_route(src[r], route, row, sfeat, sbin, left, right) : 0;
         if (write) dst[r] = s;
         if (s < g0 || s >= g0 + gn) continue;
         unsigned long long q1, q2;
@@ -381,9 +395,7 @@ __global__ void __launch_bounds__(kDtThreads) k_dt_predict(const T *__restrict__
     if (EVAL) cm.stage(eval_labels);
     __syncthreads();
     for (long long r = blockIdx.x * (long long)kDtThreads + threadIdx.x; r < n; r += (long long)gridDim.x * kDtThreads) {
-        int node = 0, f;
-        while ((f = fe[node]) >= 0) node = (double)x[r * ld + f] <= th[node] ? le[node] : ri[node];
-        const double *cnt = counts + (size_t)node * C;
+        const double *cnt = counts + (size_t)dt_walk(x + r * ld, 0, fe, th, le, ri) * C;
         double sum = 0.0;
         for (int c = 0; c < C; ++c) sum += cnt[c];
         int best = 0;
@@ -426,8 +438,7 @@ __global__ void __launch_bounds__(kDtThreads) k_gb_update(const T *__restrict__ 
             res[r] = yp;
             continue;
         }
-        int node = 0, f;
-        while ((f = feat[node]) >= 0) node = (double)x[r * ld + f] <= thr[node] ? left[node] : right[node];
+        const int node = dt_walk(x + r * ld, 0, feat, thr, left, right);
         const double m = __dadd_rn(F[r], __dmul_rn(value[node], weight));
         F[r] = m;
         res[r] = __ddiv_rn(4.0 * yp, __dadd_rn(1.0, exp(__dmul_rn(2.0 * yp, m))));
@@ -479,11 +490,7 @@ __global__ void __launch_bounds__(kDtThreads) k_gb_predict(const T *__restrict__
     __syncthreads();
     for (long long r = blockIdx.x * (long long)kDtThreads + threadIdx.x; r < n; r += (long long)gridDim.x * kDtThreads) {
         double m = 0.0;
-        for (int t = 0; t < ntrees; ++t) {
-            int node = st[t], f;
-            while ((f = fe[node]) >= 0) node = (double)x[r * ld + f] <= th[node] ? le[node] : ri[node];
-            m = __dadd_rn(m, __dmul_rn(va[node], wt[t]));
-        }
+        for (int t = 0; t < ntrees; ++t) m = __dadd_rn(m, __dmul_rn(va[dt_walk(x + r * ld, st[t], fe, th, le, ri)], wt[t]));
         const int best = m > 0.0 ? 1 : 0;
         if (!EVAL) {
             const double p0 = __ddiv_rn(1.0, __dadd_rn(1.0, exp(__dmul_rn(2.0, m))));
@@ -559,14 +566,7 @@ __global__ void __launch_bounds__(kDtThreads) k_rf_level(const unsigned char *__
         const int cls = (int)lab;
         const bool is_class = lab >= 0.0 && lab < (double)C && (double)cls == lab;
         for (int t = 0; t < ntrees; ++t) {
-            int s = t;
-            if (src) {
-                s = src[t * n + r];
-                if (route && s >= 0) {
-                    const int f = sfeat[s];
-                    s = f < 0 ? -1 : (int)row[f] <= sbin[s] ? left[s] : right[s];
-                }
-            }
+            const int s = src ? dt_route(src[t * n + r], route, row, sfeat, sbin, left, right) : t;
             if (write) dst[t * n + r] = s;
             if (s < g0 || s >= g0 + gn) continue;
             const unsigned w = rf_weight(key, (long long)tree0 + t, row0 + r, dr, ndraw);
@@ -587,13 +587,7 @@ __global__ void __launch_bounds__(kDtThreads) k_rf_level(const unsigned char *__
     }
     report_cell(bad, err);
     __syncthreads();
-    for (int i = threadIdx.x; i < cells; i += kDtThreads) {
-        const unsigned v = hist[i];
-        if (!v) continue;
-        const int g = i / (fc * cell), rest = i - g * fc * cell, q = rest / cell;
-        if (q >= fw) continue;
-        atomicAdd(&out[((size_t)g * m + q0 + q) * cell + (rest - q * cell)], (unsigned long long)v);
-    }
+    dt_flush(hist, cells, fc, cell, fw, m, q0, out);
 }
 
 // RandomForest transform / evaluate, one row per thread: raw_c = the sum over trees t (in order, from 0.0) of
@@ -647,9 +641,7 @@ __global__ void __launch_bounds__(kDtThreads) k_rf_predict(const T *__restrict__
 #pragma unroll
             for (int i = 0; i < kRfVotes; ++i) v[i] = 0.0;
             for (int t = 0; t < ntrees; ++t) {
-                int node = st[t], f;
-                while ((f = fe[node]) >= 0) node = (double)xr[f] <= th[node] ? le[node] : ri[node];
-                const double *lv = vo + (size_t)node * C + c0;
+                const double *lv = vo + (size_t)dt_walk(xr, st[t], fe, th, le, ri) * C + c0;
 #pragma unroll
                 for (int i = 0; i < kRfVotes; ++i)
                     if (c0 + i < C) v[i] = __dadd_rn(v[i], lv[i]);

@@ -441,21 +441,16 @@ class BoostRows:
             t.free()
 
 
-def _tree_args(tree):
-    """(feature int32, threshold f64, left int32, right int32, prediction f64) of a regression tree, contiguous."""
-    return [np.ascontiguousarray(a, dt) for a, dt in ((tree.feature, np.int32), (tree.threshold, np.float64),
-                                                      (tree.left, np.int32), (tree.right, np.int32),
-                                                      (tree.prediction, np.float64))]
-
-
-def forest_arrays(trees):
-    """The forest of lo_gb_predict: (start int32[ntrees], nodes, feature, threshold, left, right, value) with every
-    tree's children shifted to indices into the concatenation."""
+def node_arrays(trees, payload):
+    """The node arrays of a tree (lo_dt_predict, lo_gb_update) or a forest (lo_gb_predict, lo_rf_predict): (start
+    int32[ntrees], nodes, feature int32, threshold f64, left int32, right int32, payload f64) with every tree's children
+    shifted to indices into the concatenation; ``payload(tree)`` is a tree's per-node values (its class counts, leaf
+    values or votes), one row per node."""
     start, at, cols = [], 0, [[] for _ in range(5)]
     for t in trees:
         start.append(at)
-        f, th, le, ri, v = _tree_args(t)
-        for c, a in zip(cols, (f, th, np.where(le >= 0, le + at, -1), np.where(ri >= 0, ri + at, -1), v)):
+        for c, a in zip(cols, (t.feature, t.threshold, np.where(t.left >= 0, t.left + at, -1),
+                               np.where(t.right >= 0, t.right + at, -1), payload(t))):
             c.append(a)
         at += t.num_nodes
     dts = (np.int32, np.float64, np.int32, np.int32, np.float64)
@@ -1257,10 +1252,8 @@ class Engine:
     def dt_predict(self, part: AssembledRows, tree, raw: bool = False, labels=None, timing: dict | None = None):
         """A tree (:class:`~tree.Tree`) over ``part`` (``lo_dt_predict``), as :meth:`nb_predict`: ``labels`` None gives a
         :class:`PredictedRows` of C columns, else the int64[len(labels), C] confusion counts."""
-        arrs = [np.ascontiguousarray(a, dt) for a, dt in ((tree.feature, np.int32), (tree.threshold, np.float64),
-                                                          (tree.left, np.int32), (tree.right, np.int32),
-                                                          (tree.counts, np.float64))]
-        model = (tree.num_nodes, *[a.ctypes.data_as(C.c_void_p) for a in arrs], tree.num_classes)
+        _start, M, *arrs = node_arrays([tree], lambda t: t.counts)
+        model = (M, *[a.ctypes.data_as(C.c_void_p) for a in arrs], tree.num_classes)
         return self._predict(self._lib.lo_dt_predict, model, part, tree.num_classes, raw, labels, timing)
 
     def gb_update(self, part: AssembledRows, rows: "BoostRows | None" = None, tree=None, weight: float = 1.0,
@@ -1276,7 +1269,7 @@ class Engine:
         with _Owned() as owned:
             if rows is None:
                 rows = BoostRows(owned.own(self.table("f64", max(n, 1), 1)), owned.own(self.table("f64", max(n, 1), 1)))
-            arrs = _tree_args(tree) if tree is not None else []
+            arrs = node_arrays([tree], lambda t: t.prediction)[2:] if tree is not None else []
             ptrs = [a.ctypes.data_as(C.c_void_p) for a in arrs] or [None] * 5
             rc = self._lib.lo_gb_update(self._ctx, part.x._h, part.k, part.k, part.y._h, n,
                                         tree.num_nodes if tree is not None else 0, *ptrs, float(weight),
@@ -1299,7 +1292,7 @@ class Engine:
         """A GBT forest (regression :class:`~tree.Tree` s and their weights) over ``part`` (``lo_gb_predict``), as
         :meth:`nb_predict` with two classes: ``labels`` None gives a :class:`PredictedRows`, else the int64[len(labels),
         2] confusion counts."""
-        start, M, *arrs = forest_arrays(trees)
+        start, M, *arrs = node_arrays(trees, lambda t: t.prediction)
         w = np.ascontiguousarray(weights, np.float64)
         if len(w) != len(trees):
             raise ValueError(f"{len(w)} weights for {len(trees)} trees")
@@ -1336,11 +1329,9 @@ class Engine:
         :meth:`nb_predict`: ``labels`` None gives a :class:`PredictedRows` of C columns, else the int64[len(labels), C]
         confusion counts.  Every leaf votes its counts over their total (:func:`tree.votes`)."""
         from .tree import votes
-        start, M, feature, threshold, left, right, _value = forest_arrays(trees)
-        vo = np.ascontiguousarray(np.concatenate([votes(t) for t in trees]), np.float64)
+        start, M, *arrs = node_arrays(trees, votes)
         nc = trees[0].num_classes
-        model = (len(trees), start.ctypes.data_as(C.c_void_p), M,
-                 *[a.ctypes.data_as(C.c_void_p) for a in (feature, threshold, left, right, vo)], nc)
+        model = (len(trees), start.ctypes.data_as(C.c_void_p), M, *[a.ctypes.data_as(C.c_void_p) for a in arrs], nc)
         return self._predict(self._lib.lo_rf_predict, model, part, nc, raw, labels, timing)
 
     def value_counts_f64_host(self, values: np.ndarray):

@@ -238,10 +238,7 @@ def best_splits(hist: np.ndarray, nthr: np.ndarray, kind: str, min_instances: in
     out = {"total": total, "impurity": node_imp}
     ns = max(int(nthr.max()) if k else 0, 0)
     if ns == 0:
-        out.update(feature=np.full(nodes, -1), bin=np.zeros(nodes, np.int64), gain=np.full(nodes, DOUBLE_MIN),
-                   valid=np.zeros(nodes, bool), left=np.zeros_like(total), right=np.zeros_like(total),
-                   left_impurity=np.zeros(nodes), right_impurity=np.zeros(nodes))
-        return out
+        return _no_split(out, nodes)
     left = np.cumsum(hist[:, :, :ns], axis=2)                   # (nodes, k, ns, C): split i = bins 0 .. i
     right = total[:, None, None, :] - left
     lc = left.sum(axis=3).astype(np.float64)
@@ -251,6 +248,16 @@ def best_splits(hist: np.ndarray, nthr: np.ndarray, kind: str, min_instances: in
     if features is not None:
         f = out["feature"]
         out["feature"] = np.where(f >= 0, np.asarray(features)[np.arange(nodes), np.maximum(f, 0)], -1)
+    return out
+
+
+def _no_split(out, nodes: int):
+    """:func:`best_splits`' result when no feature has a split: every node without a feature, its gain Double.MinValue
+    and its children's counts and impurities 0."""
+    total = out["total"]
+    out.update(feature=np.full(nodes, -1), bin=np.zeros(nodes, np.int64), gain=np.full(nodes, DOUBLE_MIN),
+               valid=np.zeros(nodes, bool), left=np.zeros_like(total), right=np.zeros_like(total),
+               left_impurity=np.zeros(nodes), right_impurity=np.zeros(nodes))
     return out
 
 
@@ -322,10 +329,7 @@ def variance_splits(words: np.ndarray, nthr: np.ndarray, min_instances: int, min
     left, right, total = word_stats(words, ns)
     out = {"total": total, "impurity": variance(total)}
     if ns == 0:
-        out.update(feature=np.full(nodes, -1), bin=np.zeros(nodes, np.int64), gain=np.full(nodes, DOUBLE_MIN),
-                   valid=np.zeros(nodes, bool), left=np.zeros_like(total), right=np.zeros_like(total),
-                   left_impurity=np.zeros(nodes), right_impurity=np.zeros(nodes))
-        return out
+        return _no_split(out, nodes)
     return _choose(out, out["impurity"], left, right, left[..., 0], right[..., 0], variance(left), variance(right), nthr,
                    min_instances, min_info_gain)
 

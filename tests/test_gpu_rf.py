@@ -7,12 +7,13 @@ import pytest
 
 import rf_oracle as ro
 import tree_oracle as to
+from learningorchestra_b200 import _native as N
 from learningorchestra_b200 import classifier as CL
 from learningorchestra_b200 import tree as T
 from learningorchestra_b200.classifier import DecisionTreeClassifier, RandomForestClassifier
 from learningorchestra_b200.engine import InvalidCellError
 from test_gpu_naive_bayes import _free, _host
-from test_gpu_tree import _data, _on, _same_tree
+from test_gpu_tree import _data, _on, _part, _same_tree
 
 pytestmark = pytest.mark.gpu
 
@@ -212,3 +213,29 @@ def test_refusals(engine, what):
             RandomForestClassifier(num_trees=3).fit(feats)
     finally:
         _free(parts)
+
+
+def test_level_refusals_name_the_cell(engine):
+    """lo_rf_level refuses a code >= nbins and a label that is not a class with lo_dt_level's messages, and leaves
+    hist_out zeroed although the pass counted the other rows."""
+    import ctypes as C
+    x, y = _data(300, 3, 2, seed=13)
+    part = _part(engine, x, y)
+    try:
+        binned = engine.dt_bin(part, [to.splits(x[:, j], 8) for j in range(3)])
+        try:
+            feats = np.array([[0, 1, 2], [2, 0, 1]], np.int32)
+            tab = np.ascontiguousarray(T.draw_table(2, 1.0), np.uint64)
+            assert engine.rf_level(part, binned, 8, 2, T.DEFAULT_SEED, tab, 0, 2, None, feats).sum() > 0
+            for nbins, nclasses, want in ((2, 2, r"row \d+, feature \d: code >= nbins = 2"),
+                                          (8, 1, r"row \d+: its label is not a class in \[0, 1\)")):
+                hist = np.full((2, 3, nbins, nclasses), 7, np.int64)
+                lead = (part.y._h, part.nkept, 0, nbins, nclasses, T.DEFAULT_SEED, 0, 2, tab.ctypes.data_as(C.c_void_p),
+                        len(tab), feats.ctypes.data_as(C.c_void_p), 3)
+                with pytest.raises(N.LoexecError, match=want):
+                    engine._level(engine._lib.lo_rf_level, lead, part, binned, None, 2, hist, None, None)
+                assert not hist.any()
+        finally:
+            binned.free()
+    finally:
+        part.free()
