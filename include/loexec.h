@@ -432,6 +432,22 @@ int lo_text_codes(lo_ctx *ctx, const lo_text *t, lo_table *out, int32_t col, int
 int lo_text_codes_shards(lo_ctx *root, const lo_text *const *shards, const int64_t *row0, int32_t nshards,
                          lo_table *const *out, int32_t col, int64_t *first_rows_out, int64_t capacity,
                          int64_t *ndistinct, lo_host_timing *timing);
+/* Codes of a resident text column against another column's dictionary: the test data of a model coded as its training
+ * data was.  `dictionary` (resident on ctx, no null cell) holds the cells of codes 0, 1, ...; row i of column `col` of
+ * `out` (checked as in lo_text_codes) receives c when its cell equals dictionary cell c byte for byte, else -1: a null
+ * row, or a cell the dictionary does not hold.  *unseen = the non-null cells the dictionary does not hold.  The device
+ * builds a hash table of the dictionary's cells (k_hash_count_str's hash, slot format and compare) and probes it with
+ * every cell of the column; no cell crosses PCIe.  The codes do not depend on the table's layout, so a column cut into
+ * shards is coded shard by shard, each against the dictionary resident on its own device.
+ * Refused with LO_ERR_INVALID before anything is launched: NULL cells, dictionary or unseen; either made on another
+ * context; `out` failing lo_text_codes' checks against `cells`; a dictionary with a null cell.  After the launches: a
+ * dictionary that holds a cell twice (the codes are written all the same).
+ * Launches: 1 (insert) when the dictionary has a cell, plus 1 (probe) when the column has a row.  Bytes moved: the
+ * dictionary's cells and offsets read once and 8 bytes per table slot (at least twice the dictionary's cells, 1024 or
+ * more) written; the column's offsets, validity and cells read once and 4 bytes written per row, plus the compared
+ * dictionary cells.  timing: kernel_ms the two kernels, h2d_bytes 0, d2h_bytes the two counts (16). */
+int lo_text_codes_in(lo_ctx *ctx, const lo_text *cells, const lo_text *dictionary, lo_table *out, int32_t col,
+                     int64_t *unseen, lo_host_timing *timing);
 
 /* The feature matrix of a model's training step: Spark 2.4's VectorAssembler(inputCols, outputCol="features") plus its
  * "label" column (builder_image/builder.py:99-134), from k source columns in HBM into one row-major matrix, on the GPU.
@@ -466,6 +482,28 @@ typedef struct lo_assemble_info {
 int lo_assemble_rows(lo_ctx *ctx, const lo_table *const *src, const int32_t *src_col, int32_t k, const lo_table *label,
                      int32_t label_col, int32_t mode, lo_table *x, int64_t ld, lo_table *y, int64_t *kept_rows,
                      lo_assemble_info *info, lo_host_timing *timing);
+
+/* Spark's Dataset.randomSplit over n rows of a feature matrix of lo_assemble_rows (DESIGN.md §3.6.7): x holds n rows of
+ * k values (row stride k, LO_F32 or LO_F64, column 0), y (optional) n labels of x's dtype, ids (host int64[n]) each row's
+ * _id.  Row i goes to split s when bounds[s] <= u < bounds[s + 1], u = (splitmix64(splitmix64(~seed) ^ ids[i]) >> 11) *
+ * 2^-53; bounds (host f64[nsplits + 1]) are finite and ascend from bounds[0] = 0 (the last may round a little above or
+ * below 1), and a row whose u is at or above bounds[nsplits] goes to no split.  A row's split depends on (seed, _id) alone, so it is the same for any cut of the rows.
+ * For each split s the call allocates x_out[s] (sizes[s] * k elements) and, with y, y_out[s] (sizes[s]) on ctx's device,
+ * LO_F32 or LO_F64 as x, and writes the split's rows there in row order, bit for bit; src_rows (host int64[n]) receives
+ * every split's source rows (indices into x) in order, split after split.  The caller frees the tables.
+ * Refused with LO_ERR_INVALID before anything is enqueued: k < 1; n < 0; x not LO_F32 / LO_F64, on another device or
+ * smaller than n * k; y of another dtype, on another device or smaller than n; NULL ids with n > 0; nsplits outside
+ * [1, LO_SPLIT_MAX]; NULL bounds; bounds[0] != 0; a bound below the one before it, or not finite; NULL x_out or sizes;
+ * NULL src_rows with n > 0; y without y_out or y_out without y.  A failed call leaves no table allocated.
+ * Launches: none when n == 0; else 3 (count per tile of 1024 rows and split, scan of the counts, scatter).  The host reads
+ * the split sizes between the scan and the scatter.  Bytes moved: 8 n (ids) by the count pass; 8 n + n (k + 1) e read and
+ * m (k + 1) e + 8 m written by the scatter (e the dtype's bytes, m the rows that land in a split, the label's e only with
+ * y).  timing: kernel_ms the count, scan and scatter, h2d_bytes the ids, bounds and output pointers, d2h_bytes the split
+ * sizes and src_rows. */
+#define LO_SPLIT_MAX 32
+int lo_random_split(lo_ctx *ctx, const lo_table *x, int32_t k, const lo_table *y, int64_t n, const int64_t *ids,
+                    const double *bounds, int32_t nsplits, uint64_t seed, lo_table **x_out, lo_table **y_out,
+                    int64_t *sizes, int64_t *src_rows, lo_host_timing *timing);
 
 /* Spark 2.4's multinomial NaiveBayes (ml.classification.NaiveBayes with smoothing, no weightCol, no thresholds;
  * builder_image/builder.py:55-61's "NB") over a feature matrix of lo_assemble_rows: x holds n rows of k features

@@ -45,6 +45,7 @@ LO_DT_MAX_CLASSES = 100
 LO_DT_PASS_HIST = 1 << 30
 LO_GB_WORDS = 5
 LO_RF_MAX_DRAWS = 32
+LO_SPLIT_MAX = 32
 LO_ABI_VERSION = 7
 
 _ERR_NAMES = {
@@ -174,6 +175,9 @@ SIGNATURES = {
     "lo_text_codes": (C.c_int, [_P, _P, _P, C.c_int32, _P, C.c_int64, C.POINTER(C.c_int64), C.POINTER(HostTiming)]),
     "lo_text_codes_shards": (C.c_int, [_P, C.POINTER(_P), C.POINTER(C.c_int64), C.c_int32, C.POINTER(_P), C.c_int32, _P,
                                        C.c_int64, C.POINTER(C.c_int64), C.POINTER(HostTiming)]),
+    "lo_text_codes_in": (C.c_int, [_P, _P, _P, _P, C.c_int32, C.POINTER(C.c_int64), C.POINTER(HostTiming)]),
+    "lo_random_split": (C.c_int, [_P, _P, C.c_int32, _P, C.c_int64, _P, _P, C.c_int32, C.c_uint64, C.POINTER(_P),
+                                  C.POINTER(_P), _P, _P, C.POINTER(HostTiming)]),
     "lo_assemble_rows": (C.c_int, [_P, C.POINTER(_P), C.POINTER(C.c_int32), C.c_int32, _P, C.c_int32, C.c_int32, _P,
                                    C.c_int64, _P, _P, C.POINTER(AssembleInfo), C.POINTER(HostTiming)]),
     "lo_nb_labels": (C.c_int, [_P, _P, C.c_int64, _P, C.c_int64, C.POINTER(C.c_int64), C.POINTER(HostTiming)]),

@@ -54,12 +54,17 @@ class DeviceFrame:
     A text field (``device_frame(..., text=True)``) is a column of int32 dictionary codes instead, ``kinds[name] ==
     "text"``: -1 for a null row, else the index of its cell in ``dictionaries[name]``, the Arrow array of the distinct
     cells in the order of their first rows.  The frame owns those code tables (they are not cached) and frees them in
-    :meth:`release`.  Holds a lease on the resident dataset: call :meth:`release` (or use ``with``) when the consumer is
-    done."""
+    :meth:`release`.  A frame made with ``dictionaries`` codes the text fields named there by the given dictionaries
+    instead (-1 also for a cell the dictionary does not hold).  ``made`` lists every :class:`Features` made from the frame
+    (by :meth:`features` or a split of those), so an owner can release them all.  Holds a lease on the resident dataset:
+    call :meth:`release` (or use ``with``) when the consumer is done."""
 
-    def __init__(self, cache, data, fields, codes=None):
+    def __init__(self, cache, data, fields, codes=None, given=(), source=None):
         self._cache, self._data = cache, data
         self._codes = dict(codes or {})          # text field -> (code table, dictionary)
+        self._given = set(given)                 # text fields coded by a dictionary the caller gave
+        self.source = source                     # (database, filename) the frame was read from
+        self.made = []                           # every Features made from this frame, splits included
         self.fields = list(fields)
         self.ids = data.ids
         shards = getattr(data.table, "shards", [data.table])
@@ -99,7 +104,10 @@ class DeviceFrame:
             parts = engine.assemble_rows([self._source(f) for f in fields],
                                          self._source(label) if label is not None else None, dtype, handle_invalid)
         except InvalidCellError as e:
-            raise named_cell(e, fields, label, self.ids, "features", ("is null or NaN (handle_invalid='error')",) * 2) from None
+            name = label if e.position == len(fields) else fields[e.position]
+            reason = ("is null, NaN or missing from its dictionary (handle_invalid='error')" if name in self._given
+                      else "is null or NaN (handle_invalid='error')")
+            raise named_cell(e, fields, label, self.ids, "features", (reason, reason)) from None
         return Features(self, parts if isinstance(engine, ShardedEngine) else [parts], fields, label, dtype)
 
     def _source(self, f):
@@ -150,6 +158,33 @@ class Features:
         ids = np.asarray(frame.ids)
         self.row_ids = np.concatenate([ids[p.first:p.first + p.nkept] if p.kept is None else ids[p.rows]
                                        for p in self._parts]) if self._parts else np.zeros(0, np.int64)
+        frame.made.append(self)
+
+    def random_split(self, weights, seed: int | None = None) -> list:
+        """Spark's ``randomSplit(weights, seed)`` on the device: one :class:`Features` per weight, each owning its tables,
+        its rows in this one's order.  Row ``_id`` goes to split s when ``bounds[s] <= u < bounds[s + 1]``, where the
+        bounds are the weights over their sum summed from 0.0 in float64 (:func:`~engine.split_bounds`) and u =
+        (splitmix64(splitmix64(~seed) ^ _id) >> 11) * 2^-53, so a split holds the same rows on one GPU, on any shard cut
+        and whatever rows ``handle_invalid`` left out; a row whose u is at or above a last bound that rounded below 1.0
+        lands in no split.  ``seed`` None: ``engine.SPLIT_SEED``.  A zero weight gives an empty split.  These features
+        stay valid.  An empty list, a negative or non-finite weight, a zero sum or more than LO_SPLIT_MAX weights raise
+        ValueError before anything is launched."""
+        import numpy as np
+
+        from .engine import SPLIT_SEED, split_bounds
+        from .sharding import ShardedEngine
+        bounds = split_bounds(weights)
+        seed = SPLIT_SEED if seed is None else int(seed)
+        if not self._parts:
+            raise ValueError("the features have been released")
+        engine = self._frame._cache.engine
+        cuts = np.cumsum([0] + [p.nkept for p in self._parts])
+        ids = [self.row_ids[cuts[i]:cuts[i + 1]] for i in range(len(self._parts))]
+        if isinstance(engine, ShardedEngine):
+            per_split = engine.random_split(self._parts, ids, bounds, seed)
+        else:
+            per_split = [[p] for p in engine.random_split(self._parts[0], ids[0], bounds, seed)]
+        return [Features(self._frame, parts, self.fields, self.label, self.dtype) for parts in per_split]
 
     def release(self):
         parts, self._parts = self._parts, []
@@ -163,13 +198,18 @@ class Features:
         self.release()
 
 
-def device_frame(database, filename, engine, text: bool = False) -> DeviceFrame:
+def device_frame(database, filename, engine, text: bool = False, dictionaries=None) -> DeviceFrame:
     """``Builder.__file_processor``'s frame (data rows, metadata columns dropped) handed over ON THE DEVICE: the
     numeric fields of the dataset as zero-copy views of the resident slabs (``builder_image/builder.py:172-194`` loads
     the same frame into Spark).  ``text``: the fields of the store that are text (:class:`~table_cache.Snapshot`'s rule;
     mixed fields stay out) join it as int32 dictionary codes made on the device from the resident text columns — the
     same columns ``/histograms`` counts, uploaded only when none is resident yet; the fields keep the store's order.
-    Without ``text`` the frame holds the number fields alone — use :func:`file_processor` for the host form."""
+    Without ``text`` the frame holds the number fields alone — use :func:`file_processor` for the host form.
+    ``dictionaries`` (with ``text``): field -> Arrow dictionary, usually another frame's ``dictionaries`` (a model's
+    training data).  A text field named there is coded against it on the device (``lo_text_codes_in``): code c for a
+    cell equal to ``dictionary[c]``, -1 (invalid) for a null or a cell the dictionary does not hold, and
+    ``frame.dictionaries[f]`` is the given dictionary.  Other text fields keep their own dictionaries; names that are not
+    text fields of the dataset are ignored."""
     if getattr(database, "has_columns", lambda _f: False)(filename):
         names = [f for f in database.column_names(filename) if f not in METADATA_FIELDS]
         numeric = [f for f in names if getattr(database.column(filename, f), "kind", "") == "number"]
@@ -178,25 +218,31 @@ def device_frame(database, filename, engine, text: bool = False) -> DeviceFrame:
         numeric = [f for f in names if rows and columnar.numeric_column([d.get(f) for d in rows]) is not None]
     if not text:
         data = engine.resident.ensure(database, filename, numeric)
-        return DeviceFrame(engine.resident, data, numeric)
+        return DeviceFrame(engine.resident, data, numeric, source=(database, filename))
     from .engine import text_dictionary
     from .table_cache import Snapshot
     snap = Snapshot(database, filename)
     words = [f for f in names if f not in numeric and snap.field(f).text is not None]
     data = engine.resident.ensure(database, filename, numeric, text=words, snapshot=snap)
+    given = {f: d for f, d in (dictionaries or {}).items() if f in words}
     codes = {}
     try:
         for f in words:
             cells = data.texts[f]
             table = engine.table("i32", cells.n, 1)
             codes[f] = (table, None)             # freed below if its codes fail
-            codes[f] = (table, text_dictionary(cells.arr, engine.text_codes(cells, table, 0)))
+            if f in given:
+                engine.text_codes_in(cells, given[f], table, 0)
+                codes[f] = (table, given[f])
+            else:
+                codes[f] = (table, text_dictionary(cells.arr, engine.text_codes(cells, table, 0)))
     except BaseException:
         for table, _dictionary in codes.values():
             table.free()
         engine.resident.release(data)
         raise
-    return DeviceFrame(engine.resident, data, [f for f in names if f in numeric or f in codes], codes)
+    return DeviceFrame(engine.resident, data, [f for f in names if f in numeric or f in codes], codes, given,
+                       source=(database, filename))
 
 
 def _frame(fields, rows, packed, resident):

@@ -114,6 +114,27 @@ class ObjectColumn:
         return ObjectColumn([self.values[int(i)] for i in index])
 
 
+class ProbabilityColumn:
+    """A prediction dataset's ``probability``: the n x C float64 matrix of a classifier's class probabilities.  A row's
+    cell is the list of its C floats, as the reference stores ``probability.toArray().tolist()``; the lists are built
+    only for the rows that are read.  Its ``kind`` is ``"object"``, so readers treat it like any column of list cells."""
+    kind = "object"
+
+    def __init__(self, matrix):
+        self.matrix = np.ascontiguousarray(matrix, dtype=np.float64)
+        if self.matrix.ndim != 2:
+            raise ValueError(f"a probability column is an n x C matrix, not of shape {self.matrix.shape}")
+
+    def __len__(self):
+        return self.matrix.shape[0]
+
+    def to_pylist(self, start=0, stop=None):
+        return self.matrix[start:stop].tolist()
+
+    def take(self, index):
+        return ProbabilityColumn(self.matrix[np.asarray(index, dtype=np.int64)])
+
+
 def column_from_values(values):
     """Classify a list of document values: all ``str`` / None -> TextColumn; all int / float / None (no bool, ints that
     float64 holds exactly) -> NumberColumn; anything else -> ObjectColumn."""

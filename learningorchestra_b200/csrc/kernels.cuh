@@ -1254,12 +1254,19 @@ __host__ __device__ __forceinline__ unsigned long long hash_bytes(const uint8_t 
     return splitmix64(h);
 }
 
-__device__ __forceinline__ bool same_cell(const uint8_t *chars, const long long *offsets, long long a, long long b) {
-    const long long a0 = offsets[a], b0 = offsets[b], la = offsets[a + 1] - a0;
-    if (la != offsets[b + 1] - b0) return false;
-    for (long long i = 0; i < la; ++i)
-        if (chars[a0 + i] != chars[b0 + i]) return false;
+// the cell of len bytes at p equals cell b of (chars, offsets)
+__device__ __forceinline__ bool cell_is(const uint8_t *p, long long len, const uint8_t *chars, const long long *offsets,
+                                        long long b) {
+    const long long b0 = offsets[b];
+    if (len != offsets[b + 1] - b0) return false;
+    for (long long i = 0; i < len; ++i)
+        if (p[i] != chars[b0 + i]) return false;
     return true;
+}
+
+__device__ __forceinline__ bool same_cell(const uint8_t *chars, const long long *offsets, long long a, long long b) {
+    const long long a0 = offsets[a];
+    return cell_is(chars + a0, offsets[a + 1] - a0, chars, offsets, b);
 }
 
 // The slot of the group of slot word `mine` (tag | representative row) whose cell hashes to h, in the global table;
@@ -1520,6 +1527,58 @@ __global__ void k_remap_codes(int *__restrict__ codes, long long n, const uint8_
                               const unsigned long long *__restrict__ slot_code) {
     for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
         if (text_row_live(valid_mask, valid_bitmap, bit0, i)) codes[i] = (int)slot_code[(unsigned)codes[i]];
+}
+
+// ---------------------------------------------------------------------------------------------
+// codes of a TEXT column against a given dictionary (lo_text_codes_in): k_dict_insert puts every cell of the dictionary
+// into a table of k_hash_count_str's slot format (row = the cell's code); k_dict_codes probes it with every live cell of
+// the column, in str_table_slot's probe order, comparing bytes with cell_is.  The codes do not depend on the table's
+// layout, so they are the same for any cut of the column.
+// ---------------------------------------------------------------------------------------------
+// Dictionary cell i lands in its slot; a cell that meets an equal cell of another code there is a repeat: *repeats
+// counts them (one per cell beyond the first of its value, whichever of them won the slot).
+__global__ void __launch_bounds__(256) k_dict_insert(const uint8_t *__restrict__ chars, const long long *__restrict__ offsets,
+                                                     long long n, unsigned long long *__restrict__ slots,
+                                                     unsigned long long mask, unsigned long long *__restrict__ repeats) {
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+        const unsigned long long h = hash_bytes(chars + offsets[i], offsets[i + 1] - offsets[i]);
+        const unsigned long long mine = ((h >> 31) << 31) | (unsigned long long)i;
+        const unsigned long long s = str_table_slot(chars, offsets, slots, mask, h, mine);
+        if (*(volatile unsigned long long *)(slots + s) != mine) atomicAdd(repeats, 1ull);
+    }
+}
+
+// codes[i] = the code of row i's cell in the dictionary (dchars / doffsets) whose table is `slots`; -1 for a null row or a
+// cell the dictionary does not hold, and *unseen counts the latter.
+__global__ void __launch_bounds__(256) k_dict_codes(const uint8_t *__restrict__ chars, const long long *__restrict__ offsets,
+                                                    long long n, const uint8_t *__restrict__ valid_mask,
+                                                    const uint8_t *__restrict__ valid_bitmap, int bit0,
+                                                    const uint8_t *__restrict__ dchars, const long long *__restrict__ doffsets,
+                                                    const unsigned long long *__restrict__ slots, unsigned long long mask,
+                                                    int *__restrict__ codes, unsigned long long *__restrict__ unseen) {
+    for (long long i0 = blockIdx.x * (long long)blockDim.x; i0 < n; i0 += (long long)gridDim.x * blockDim.x) {
+        const long long i = i0 + threadIdx.x;
+        const bool live = i < n && text_row_live(valid_mask, valid_bitmap, bit0, i);
+        int code = -1;
+        if (live) {
+            const uint8_t *p = chars + offsets[i];
+            const long long len = offsets[i + 1] - offsets[i];
+            const unsigned long long h = hash_bytes(p, len);
+            for (unsigned long long s = splitmix64(h) & mask;; s = (s + 1) & mask) {
+                const unsigned long long cur = slots[s];
+                if (cur == kEmptyKey) break;
+                if ((cur >> 31) == (h >> 31) && cell_is(p, len, dchars, doffsets, (long long)(cur & 0x7FFFFFFFull))) {
+                    code = (int)(cur & 0x7FFFFFFFull);
+                    break;
+                }
+            }
+            codes[i] = code;
+        } else if (i < n) {
+            codes[i] = -1;
+        }
+        const unsigned miss = __ballot_sync(0xffffffffu, live && code < 0);
+        if ((threadIdx.x & 31) == 0 && miss) atomicAdd(unseen, (unsigned long long)__popc(miss));
+    }
 }
 
 // R-semantics cast "number" (data_type_update.py:40-43): one cell per thread, CPython float() grammar,
@@ -1932,6 +1991,116 @@ __global__ void __launch_bounds__(kAsmThreads) k_assemble_rows(const AsmSrc *__r
     } else {
         for (int r = warp; r < nout; r += kAsmThreads / 32)
             if (lane < kc) base[(long long)r * ld + lane] = tile[r][lane];
+    }
+}
+
+// ---------------------------------------------------------------------------------------------
+// Spark's randomSplit over the feature matrix (lo_random_split): row i goes to split s when bounds[s] <= u < bounds[s + 1],
+// u = (splitmix64(key ^ id[i]) >> 11) * 2^-53 and key = splitmix64(~seed), so a row's split depends only on the seed and
+// its _id.  An order-preserving multi-way partition: k_split_count counts each tile's rows per split, an exclusive scan
+// of those counts (split-major) gives every (split, tile) its first output row, and k_split_scatter writes each tile's
+// rows of each split there in row order.
+// ---------------------------------------------------------------------------------------------
+constexpr int kSplitMax = 32;             // LO_SPLIT_MAX
+constexpr int kSplitThreads = 256;
+constexpr int kSplitRounds = 4;
+constexpr int kSplitRows = kSplitThreads * kSplitRounds;   // rows per tile (one CTA)
+
+// the split of the row with this _id, -1 when u is at or above the last bound (a last bound rounded below 1)
+__device__ __forceinline__ int split_of(unsigned long long key, long long id, const double *bounds, int nsplits) {
+    const double u = (double)(splitmix64(key ^ (unsigned long long)id) >> 11) * 0x1.0p-53;
+    for (int s = 0; s < nsplits; ++s)
+        if (u < bounds[s + 1]) return s;
+    return -1;
+}
+
+// counts[s * ntiles + t] = the rows of tile t in split s
+__global__ void __launch_bounds__(kSplitThreads) k_split_count(const long long *__restrict__ ids, long long n,
+                                                               unsigned long long key, const double *__restrict__ bounds,
+                                                               int nsplits, unsigned long long *__restrict__ counts) {
+    __shared__ double sb[kSplitMax + 1];
+    __shared__ unsigned cnt[kSplitMax];
+    for (int s = threadIdx.x; s <= nsplits; s += kSplitThreads) sb[s] = bounds[s];
+    for (int s = threadIdx.x; s < nsplits; s += kSplitThreads) cnt[s] = 0;
+    __syncthreads();
+    const long long row0 = (long long)blockIdx.x * kSplitRows;
+#pragma unroll
+    for (int q = 0; q < kSplitRounds; ++q) {
+        const long long i = row0 + q * kSplitThreads + threadIdx.x;
+        const int s = i < n ? split_of(key, ids[i], sb, nsplits) : -1;
+        const unsigned peers = __match_any_sync(0xffffffffu, s);
+        if (s >= 0 && (int)(threadIdx.x & 31) == __ffs(peers) - 1) atomicAdd(&cnt[s], (unsigned)__popc(peers));
+    }
+    __syncthreads();
+    for (int s = threadIdx.x; s < nsplits; s += kSplitThreads) counts[(long long)s * gridDim.x + blockIdx.x] = cnt[s];
+}
+
+// The tile's rows of split s go to rows off[s * ntiles + t] - off[s * ntiles] .. of that split, in row order: x_out[s]
+// (k values a row), y_out[s] (y NULL: none) and src_out[s] (the row's index i).  Per round of 256 rows each warp ranks
+// its lanes by split (match.any), the warps' counts are scanned in shared memory, and the round's rows are copied
+// with the whole CTA walking the round's k * 256 contiguous input elements.
+template <typename T>
+__global__ void __launch_bounds__(kSplitThreads) k_split_scatter(const T *__restrict__ x, int k, const T *__restrict__ y,
+                                                                 const long long *__restrict__ ids, long long n,
+                                                                 unsigned long long key, const double *__restrict__ bounds,
+                                                                 int nsplits, const unsigned long long *__restrict__ off,
+                                                                 T *const *__restrict__ x_out, T *const *__restrict__ y_out,
+                                                                 long long *const *__restrict__ src_out) {
+    constexpr int kWarps = kSplitThreads / 32;
+    __shared__ double sb[kSplitMax + 1];
+    __shared__ long long base[kSplitMax];         // the next output row of each split
+    __shared__ unsigned wcnt[kWarps][kSplitMax];  // a round's rows per warp and split, then their exclusive scan
+    __shared__ unsigned total[kSplitMax];
+    __shared__ long long dst[kSplitThreads];
+    __shared__ signed char spl[kSplitThreads];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    for (int s = threadIdx.x; s <= nsplits; s += kSplitThreads) sb[s] = bounds[s];
+    for (int s = threadIdx.x; s < nsplits; s += kSplitThreads)
+        base[s] = (long long)(off[(long long)s * gridDim.x + blockIdx.x] - off[(long long)s * gridDim.x]);
+    const long long row0 = (long long)blockIdx.x * kSplitRows;
+    const int dr = kSplitThreads / k, dc = kSplitThreads % k;   // the copy's stride in (row, column)
+    for (int q = 0; q < kSplitRounds; ++q) {
+        const long long r0 = row0 + q * kSplitThreads;
+        if (r0 >= n) break;                       // uniform over the CTA
+        for (int e = threadIdx.x; e < kWarps * nsplits; e += kSplitThreads) wcnt[e / nsplits][e % nsplits] = 0;
+        __syncthreads();
+        const long long i = r0 + threadIdx.x;
+        const int s = i < n ? split_of(key, ids[i], sb, nsplits) : -1;
+        const unsigned peers = __match_any_sync(0xffffffffu, s);
+        const unsigned rank = __popc(peers & ((1u << lane) - 1));
+        if (s >= 0 && rank == 0) wcnt[warp][s] = (unsigned)__popc(peers);
+        __syncthreads();
+        for (int t = threadIdx.x; t < nsplits; t += kSplitThreads) {
+            unsigned run = 0;
+#pragma unroll
+            for (int w = 0; w < kWarps; ++w) {
+                const unsigned c = wcnt[w][t];
+                wcnt[w][t] = run;
+                run += c;
+            }
+            total[t] = run;
+        }
+        __syncthreads();
+        spl[threadIdx.x] = (signed char)s;
+        if (s >= 0) {
+            const long long o = base[s] + wcnt[warp][s] + rank;
+            dst[threadIdx.x] = o;
+            if (y) y_out[s][o] = y[i];
+            src_out[s][o] = i;
+        }
+        __syncthreads();
+        for (int t = threadIdx.x; t < nsplits; t += kSplitThreads) base[t] += total[t];
+        const long long len = min((long long)kSplitThreads, n - r0) * k;
+        const T *src = x + r0 * k;
+        int r = threadIdx.x / k, c = threadIdx.x % k;
+        for (long long e = threadIdx.x; e < len; e += kSplitThreads) {
+            const int sr = spl[r];
+            if (sr >= 0) x_out[sr][dst[r] * k + c] = src[e];
+            r += dr;
+            c += dc;
+            if (c >= k) { c -= k; ++r; }
+        }
+        __syncthreads();
     }
 }
 

@@ -2160,6 +2160,47 @@ int lo_text_codes_shards(lo_ctx *root, const lo_text *const *shards, const int64
     return rc;
 }
 
+// Codes of a resident text column against a resident dictionary (loexec.h): the dictionary's table (k_dict_insert, which
+// counts repeated cells), then one probe of every cell of the column (k_dict_codes, which counts unseen cells); the
+// host reads both counts once at the end.
+int lo_text_codes_in(lo_ctx *ctx, const lo_text *cells, const lo_text *dictionary, lo_table *out, int32_t col,
+                     int64_t *unseen, lo_host_timing *timing) {
+    LO_TRY(check_ctx(ctx));
+    if (!cells || !dictionary) return fail(LO_ERR_INVALID, "cells or dictionary is NULL");
+    if (cells->ctx != ctx || dictionary->ctx != ctx) return fail(LO_ERR_INVALID, "a text column belongs to another context");
+    LO_TRY(check_codes_out(cells, out, col, "out"));
+    if (!unseen) return fail(LO_ERR_INVALID, "unseen is NULL");
+    if (dictionary->nulls) return fail(LO_ERR_INVALID, "the dictionary holds %lld null cells", (long long)dictionary->nulls);
+    *unseen = 0;
+    HostCall c(ctx, "text_codes_in");
+    const int64_t nd = dictionary->n, n = cells->n;
+    const unsigned long long nslots = slots_for(nd);
+    unsigned long long *slots = nullptr, *counts = nullptr, host[2] = {0, 0};   // repeated dictionary cells, unseen cells
+    c.alloc(&slots, nslots * 8);
+    c.alloc(&counts, 16);
+    c.memset(slots, 0xFF, nslots * 8);
+    c.memset(counts, 0, 16);
+    c.mark();
+    if (nd > 0)
+        c.launch(1, [&] {
+            lo::k_dict_insert<<<grid_for(ctx, nd), 256, 0, c.s>>>(dictionary->cols.chars, dictionary->cols.offsets, nd, slots,
+                                                                   nslots - 1, counts);
+        });
+    if (n > 0)
+        c.launch(1, [&] {
+            const TextCols &t = cells->cols;
+            lo::k_dict_codes<<<grid_for(ctx, n), 256, 0, c.s>>>(t.chars, t.offsets, n, t.mask, t.bitmap, t.bit0,
+                                                                 dictionary->cols.chars, dictionary->cols.offsets, slots,
+                                                                 nslots - 1, codes_col(out, col), counts + 1);
+        });
+    c.mark();
+    c.to_host(host, counts, 16);
+    LO_TRY(c.finish(timing));
+    if (host[0]) return fail(LO_ERR_INVALID, "the dictionary holds a cell more than once (%llu repeats)", host[0]);
+    *unseen = (int64_t)host[1];
+    return LO_OK;
+}
+
 // text -> number for one column of cells (R-semantics "number" cast).  chars: all cells back to back;
 // offsets[i] .. offsets[i+1] delimit cell i.  values[i] = the binary64 CPython's float() returns,
 // status[i] in {0 float, 1 integer-valued, 2 empty string, 3 invalid (ValueError), 4 not decidable on device}.
@@ -2580,6 +2621,133 @@ int lo_assemble_rows(lo_ctx *ctx, const lo_table *const *src, const int32_t *src
     if (kept_rows && !skip)
         for (int64_t i = 0; i < n; ++i) kept_rows[i] = i;
     return LO_OK;
+}
+
+}  // extern "C"
+
+namespace {
+
+static_assert(lo::kSplitMax == LO_SPLIT_MAX, "loexec.h documents the split cap");
+
+template <typename T>
+void launch_split(HostCall &c, const lo_table *x, int32_t k, const lo_table *y, const long long *ids, int64_t n,
+                  unsigned long long key, const double *bounds, int32_t nsplits, const unsigned long long *off,
+                  void *const *xo, void *const *yo, long long *const *so, unsigned ntiles) {
+    c.launch(1, [&] {
+        lo::k_split_scatter<T><<<ntiles, lo::kSplitThreads, 0, c.s>>>((const T *)x->base, k, y ? (const T *)y->base : nullptr,
+                                                                      ids, n, key, bounds, nsplits, off, (T *const *)xo,
+                                                                      (T *const *)yo, so);
+    });
+}
+
+}  // namespace
+
+extern "C" {
+
+// Spark's randomSplit over n rows of a feature matrix (loexec.h): count, scan, read the split sizes, allocate the
+// outputs at their exact sizes, scatter.
+int lo_random_split(lo_ctx *ctx, const lo_table *x, int32_t k, const lo_table *y, int64_t n, const int64_t *ids,
+                    const double *bounds, int32_t nsplits, uint64_t seed, lo_table **x_out, lo_table **y_out,
+                    int64_t *sizes, int64_t *src_rows, lo_host_timing *timing) {
+    LO_TRY(check_ctx(ctx));
+    if (k < 1) return fail(LO_ERR_INVALID, "k = %d: at least one feature", k);
+    LO_TRY(check_matrix_shape(k, k, n));
+    LO_TRY(check_float_table(ctx, x, 0, n * k, "x"));
+    if (y) LO_TRY(check_float_table(ctx, y, x->dtype, n, "y"));
+    if (n > 0 && !ids) return fail(LO_ERR_INVALID, "ids is NULL");
+    if (nsplits < 1 || nsplits > LO_SPLIT_MAX) return fail(LO_ERR_INVALID, "nsplits = %d outside [1, %d]", nsplits, LO_SPLIT_MAX);
+    if (!bounds) return fail(LO_ERR_INVALID, "bounds is NULL");
+    if (bounds[0] != 0.0) return fail(LO_ERR_INVALID, "bounds[0] = %g: the first bound is 0", bounds[0]);
+    for (int s = 0; s < nsplits; ++s)
+        if (!(bounds[s + 1] >= bounds[s]) || !std::isfinite(bounds[s + 1]))
+            return fail(LO_ERR_INVALID, "bounds[%d] = %g: finite bounds ascend from 0", s + 1, bounds[s + 1]);
+    if (!x_out || !sizes || (n > 0 && !src_rows)) return fail(LO_ERR_INVALID, "x_out, sizes or src_rows is NULL");
+    if (!y != !y_out) return fail(LO_ERR_INVALID, "y and y_out go together");
+    for (int s = 0; s < nsplits; ++s) {
+        x_out[s] = nullptr;
+        if (y_out) y_out[s] = nullptr;
+        sizes[s] = 0;
+    }
+    const unsigned long long key = lo::splitmix64(~seed);
+    const int64_t ntiles = (n + lo::kSplitRows - 1) / lo::kSplitRows;
+    const size_t es = x->dtype == LO_F64 ? 8 : 4;
+    HostCall c(ctx, "random_split");
+    long long *d_ids = nullptr, *d_src = nullptr;
+    double *d_bounds = nullptr;
+    unsigned long long *off = nullptr;
+    void *tmp = nullptr;
+    size_t tmp_bytes = 0;
+    const int64_t ncounts = (int64_t)nsplits * ntiles;
+    std::vector<unsigned long long> starts((size_t)nsplits + 1, 0);
+    if (n > 0) {
+        c.alloc(&d_ids, (size_t)n * 8);
+        c.alloc(&d_bounds, (size_t)(nsplits + 1) * 8);
+        c.alloc(&off, (size_t)(ncounts + 1) * 8);
+        c.to_dev(d_ids, ids, (size_t)n * 8);
+        c.to_dev(d_bounds, bounds, (size_t)(nsplits + 1) * 8);
+        c.memset(off + ncounts, 0, 8);
+        c.run([&] { return cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, off, ncounts + 1, c.s); });
+        c.alloc(&tmp, tmp_bytes);
+        c.mark();
+        c.launch(1, [&] {
+            lo::k_split_count<<<(unsigned)ntiles, lo::kSplitThreads, 0, c.s>>>(d_ids, n, key, d_bounds, nsplits, off);
+        });
+        c.launch(1, [&] { return cub::DeviceScan::ExclusiveSum(tmp, tmp_bytes, off, ncounts + 1, c.s); });
+        c.mark();
+        for (int s = 0; s <= nsplits; ++s) c.to_host(&starts[s], off + (int64_t)s * ntiles, 8);
+        c.sync();
+        c.drop(tmp);
+    }
+    // the outputs, at their sizes; a failed call frees them
+    std::vector<lo_table *> made;
+    auto table = [&](int64_t rows) -> lo_table * {
+        lo_table *t = nullptr;
+        c.check([&] { return lo_table_alloc(ctx, x->dtype, rows, 1, &t); });
+        if (t) made.push_back(t);
+        return t;
+    };
+    std::vector<void *> xo((size_t)nsplits), yo((size_t)nsplits);
+    std::vector<long long *> so((size_t)nsplits);
+    if (n > 0) c.alloc(&d_src, (size_t)std::max<unsigned long long>(starts[nsplits], 1) * 8);
+    for (int s = 0; s < nsplits && c.ok(); ++s) {
+        sizes[s] = (int64_t)(starts[s + 1] - starts[s]);
+        lo_table *tx = table(sizes[s] * k), *ty = y ? table(sizes[s]) : nullptr;
+        x_out[s] = tx;
+        if (y_out) y_out[s] = ty;
+        xo[s] = tx ? tx->base : nullptr;
+        yo[s] = ty ? ty->base : nullptr;
+        so[s] = d_src ? d_src + starts[s] : nullptr;
+    }
+    if (n > 0) {
+        void **d_ptrs = nullptr;
+        c.alloc(&d_ptrs, (size_t)nsplits * 3 * sizeof(void *));
+        std::vector<void *> ptrs(xo);
+        ptrs.insert(ptrs.end(), yo.begin(), yo.end());
+        ptrs.insert(ptrs.end(), so.begin(), so.end());
+        c.to_dev(d_ptrs, ptrs.data(), ptrs.size() * sizeof(void *));
+        c.mark();
+        if (es == 8)
+            launch_split<double>(c, x, k, y, d_ids, n, key, d_bounds, nsplits, off, d_ptrs, d_ptrs + nsplits,
+                                 (long long *const *)(d_ptrs + 2 * nsplits), (unsigned)ntiles);
+        else
+            launch_split<float>(c, x, k, y, d_ids, n, key, d_bounds, nsplits, off, d_ptrs, d_ptrs + nsplits,
+                                (long long *const *)(d_ptrs + 2 * nsplits), (unsigned)ntiles);
+        c.mark();
+        c.to_host(src_rows, d_src, (size_t)starts[nsplits] * 8);
+        c.sync();                            // ptrs is read by the copy before it goes out of scope
+    }
+    const int rc = c.finish(timing);
+    if (rc != LO_OK) {
+        const std::string msg = g_err;
+        for (lo_table *t : made) lo_table_free(ctx, t);
+        for (int s = 0; s < nsplits; ++s) {
+            x_out[s] = nullptr;
+            if (y_out) y_out[s] = nullptr;
+            sizes[s] = 0;
+        }
+        g_err = msg;
+    }
+    return rc;
 }
 
 }  // extern "C"

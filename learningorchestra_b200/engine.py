@@ -13,6 +13,7 @@ from __future__ import annotations
 import contextlib
 import ctypes as C
 import io
+import math
 import os
 import threading
 from typing import Iterable, Sequence
@@ -485,6 +486,32 @@ def assemble_args(handle_invalid: str, dtype: str) -> tuple[int, str]:
     if dtype not in ASSEMBLE_DTYPES:
         raise ValueError(f"dtype must be one of {sorted(ASSEMBLE_DTYPES)}, not {dtype!r}")
     return ASSEMBLE_MODES[handle_invalid], ASSEMBLE_DTYPES[dtype]
+
+
+SPLIT_SEED = 0x5EED_5B17       # Features.random_split's seed when none is given
+
+
+def split_bounds(weights) -> np.ndarray:
+    """The bounds (float64[len(weights) + 1]) of Spark's ``randomSplit(weights)``: each weight over their sum, summed
+    in order from 0.0 in float64, as Spark computes them; a last bound may round below 1.0.  Refuses an empty list, a
+    negative or non-finite weight, a zero sum and more than LO_SPLIT_MAX weights (ValueError)."""
+    w = [float(v) for v in weights]
+    if not w:
+        raise ValueError("random_split needs at least one weight")
+    if len(w) > N.LO_SPLIT_MAX:
+        raise ValueError(f"{len(w)} weights: at most LO_SPLIT_MAX = {N.LO_SPLIT_MAX} splits")
+    if any(not math.isfinite(v) or v < 0.0 for v in w):
+        raise ValueError(f"weights must be finite and >= 0, not {list(weights)!r}")
+    total = 0.0
+    for v in w:
+        total += v
+    if not total > 0.0:
+        raise ValueError("the weights sum to 0")
+    bounds, run = [0.0], 0.0
+    for v in w:
+        run += v / total
+        bounds.append(run)
+    return np.array(bounds, np.float64)
 
 
 class DeviceTable:
@@ -1017,6 +1044,24 @@ class Engine:
         return _first_rows(lambda rows, cap, nd, t: self._lib.lo_text_codes(
             self._ctx, text._h, table._h, int(col), rows, cap, nd, t), text.n - text.nulls, timing)
 
+    def text_codes_in(self, text: DeviceText, dictionary, table: DeviceTable, col: int, timing: dict | None = None) -> int:
+        """Codes of a resident text column against ``dictionary`` (an Arrow string array without nulls, another column's
+        :func:`text_dictionary`; ``lo_text_codes_in``) into int32 column ``col`` of ``table``: c where the cell equals
+        ``dictionary[c]``, -1 for a null row or a cell the dictionary does not hold.  The dictionary is uploaded for the
+        call and freed after it; no cell of ``text`` crosses PCIe.  Returns the non-null cells the dictionary does not
+        hold.  A dictionary holding a cell twice raises LoexecError LO_ERR_INVALID.  ``timing``: a dict to receive the
+        call's lo_host_timing fields."""
+        if text._h is None:
+            raise ValueError("the text column has been freed")
+        d = self.text(dictionary)
+        try:
+            unseen, t = C.c_int64(), N.HostTiming()
+            N.check(self._lib.lo_text_codes_in(self._ctx, text._h, d._h, table._h, int(col), C.byref(unseen), C.byref(t)))
+        finally:
+            d.free()
+        _report(timing, t)
+        return int(unseen.value)
+
     def assemble_rows(self, sources, label=None, dtype: str = "float32", handle_invalid: str = "error",
                       timing: dict | None = None) -> AssembledRows:
         """Spark's ``VectorAssembler`` on the device (``lo_assemble_rows``): row i of the result is the value of every
@@ -1047,6 +1092,41 @@ class Engine:
             _check_cells(rc, info, k, _ASSEMBLE_REFUSED)
         _report(timing, t)
         return AssembledRows(x, y, rows[:info.nkept] if rows is not None else None, k, info.nkept)
+
+    def random_split(self, part: AssembledRows, ids, bounds, seed: int, timing: dict | None = None) -> list:
+        """Spark's ``randomSplit`` of ``part``'s rows on the device (``lo_random_split``): one :class:`AssembledRows` per
+        split, each owning tables of exactly its rows, in row order, bit for bit.  ``ids`` (int64, one per row) are the
+        rows' ``_id``; row i goes to split s when ``bounds[s] <= u < bounds[s + 1]`` for u drawn from (``seed``,
+        ``ids[i]``) alone (:func:`split_bounds`).  ``part`` stays valid.  ``timing``: a dict to receive the call's
+        lo_host_timing fields."""
+        ids = np.ascontiguousarray(ids, dtype=np.int64)
+        b = np.ascontiguousarray(bounds, dtype=np.float64)
+        ns, n = len(b) - 1, part.nkept
+        if len(ids) != n:
+            raise ValueError(f"{len(ids)} ids for {n} rows")
+        if part.x._h is None or (part.y is not None and part.y._h is None):
+            raise ValueError("the rows have been freed")
+        xs, ys = (C.c_void_p * max(ns, 1))(), (C.c_void_p * max(ns, 1))()
+        sizes, src = np.zeros(max(ns, 1), np.int64), np.empty(max(n, 1), np.int64)
+        t = N.HostTiming()
+        N.check(self._lib.lo_random_split(self._ctx, part.x._h, part.k, part.y._h if part.y is not None else None, n,
+                                          ids.ctypes.data_as(C.c_void_p), b.ctypes.data_as(C.c_void_p), ns,
+                                          C.c_uint64(int(seed) & 0xFFFFFFFFFFFFFFFF), xs,
+                                          ys if part.y is not None else None, sizes.ctypes.data_as(C.c_void_p),
+                                          src.ctypes.data_as(C.c_void_p), C.byref(t)))
+        _report(timing, t)
+        out, at = [], 0
+        for s in range(ns):
+            m = int(sizes[s])
+            rows = src[at:at + m].copy()
+            at += m
+            kept = rows if part.kept is None else part.kept[rows]
+            x = DeviceTable(self, C.c_void_p(xs[s]))
+            y = DeviceTable(self, C.c_void_p(ys[s])) if part.y is not None else None
+            a = AssembledRows(x, y, kept, part.k, m)
+            a.first = part.first
+            out.append(a)
+        return out
 
     def nb_labels(self, part: AssembledRows) -> np.ndarray:
         """The distinct label values of ``part`` (an :class:`AssembledRows` with ``y``), ascending, -0.0 as 0.0

@@ -1,4 +1,4 @@
-"""REST surface of the three hot-path services on werkzeug (Flask is not installed here), reproducing the
+"""REST surface of the hot-path services on werkzeug (Flask is not installed here), reproducing the
 routes, JSON keys, status codes, messages and GET-URI bodies of the reference:
 
   POST  /projections   projection_image/server.py:72-154      201 / 409 / 406
@@ -9,6 +9,8 @@ routes, JSON keys, status codes, messages and GET-URI bodies of the reference:
                        {"datasetName", "datasetURI"}; 201 / 409 "duplicated dataset name" / 406 "invalid url"
                        (utils.py:78-95).  Only file:// URIs and local paths are read (no network here); rows land as
                        columns (column_store)
+  POST  /models        builder_image/server.py:67-161          201 / 406: fits, evaluates and writes the predictions of
+                       every classifier of "classifiersList" (builder.Builder); one URI per entry, duplicates included
 
 Optional extension keys (absent from the reference, ignored by it): ``castTo``, ``bins``, ``range``.
 The gateway paths of ``krakend/krakend.json:143-365`` map 1:1 onto these routes (INTEGRATION.md).
@@ -21,11 +23,12 @@ from werkzeug.exceptions import HTTPException
 from werkzeug.routing import Map, Rule
 from werkzeug.wrappers import Request, Response
 
+from .builder import Builder
 from .data_type_update import DataType
 from .histogram import Histogram
 from .projection import Projection
-from .utils import (Database, DataTypeMetadata, DataTypeRequest, HistogramMetadata, HistogramRequest,
-                    ProjectionMetadata, ProjectionRequest)
+from .utils import (BuilderMetadata, BuilderRequest, Database, DataTypeMetadata, DataTypeRequest, HistogramMetadata,
+                    HistogramRequest, ProjectionMetadata, ProjectionRequest)
 
 HTTP_STATUS_CODE_SUCCESS = 200
 HTTP_STATUS_CODE_SUCCESS_CREATED = 201
@@ -40,6 +43,8 @@ DATATYPE_URI_GET = "/api/learningOrchestra/v1/dataset/"
 DATATYPE_URI_PARAMS = "?query={}&limit=20&skip=0"
 HISTOGRAM_URI_GET = "/api/learningOrchestra/v1/explore/histogram/"
 HISTOGRAM_URI_PARAMS = "?query={}&limit=10&skip=0"
+BUILDER_URI_GET = "/api/learningOrchestra/v1/builder/sparkml/"
+BUILDER_URI_PARAMS = "?query={}&limit=10&skip=0"
 
 DATABASE_URL, DATABASE_REPLICA_SET, DATABASE_NAME = "mongodb://in-process", "replica_set", "database"
 
@@ -61,12 +66,14 @@ def _first_error(checks):
 class App:
     def __init__(self, database: Database, engine, synchronous: bool = False):
         self.database, self.engine, self.synchronous = database, engine, synchronous
+        self.last_job = None            # the job the latest request started (its timings, its future)
         self.url_map = Map([
             Rule("/projections", endpoint="projection", methods=["POST"]),
             Rule("/fieldTypes", endpoint="datatype", methods=["PATCH"]),
             Rule("/histograms", endpoint="histogram", methods=["POST"]),
             Rule("/files/<filename>", endpoint="read", methods=["GET"]),
             Rule("/files", endpoint="ingest", methods=["POST"]),
+            Rule("/models", endpoint="models", methods=["POST"]),
         ])
 
     # ---- POST /projections -----------------------------------------------------------------------------
@@ -122,6 +129,27 @@ class App:
         self._maybe_wait(job)
         return _json({MESSAGE_RESULT: f"{HISTOGRAM_URI_GET}{out}{HISTOGRAM_URI_PARAMS}"}, HTTP_STATUS_CODE_SUCCESS_CREATED)
 
+    # ---- POST /models (builder_image/server.py:67-161) ------------------------------------------------------------
+    def on_models(self, request):
+        body = request.get_json()
+        train, test, classifiers = body["trainDatasetName"], body["testDatasetName"], body["classifiersList"]
+        v = BuilderRequest(self.database)
+        err = _first_error([
+            (v.filename_validator, (train,), HTTP_STATUS_CODE_NOT_ACCEPTABLE),
+            (v.filename_validator, (test,), HTTP_STATUS_CODE_NOT_ACCEPTABLE),
+            (v.model_classifiers_validator, (classifiers,), HTTP_STATUS_CODE_NOT_ACCEPTABLE),
+            (v.finished_processing_validator, (train,), HTTP_STATUS_CODE_NOT_ACCEPTABLE),
+            (v.finished_processing_validator, (test,), HTTP_STATUS_CODE_NOT_ACCEPTABLE)])
+        if err is not None:
+            return err
+        url_train = Database.collection_database_url(DATABASE_URL, DATABASE_NAME, train, DATABASE_REPLICA_SET)
+        url_test = Database.collection_database_url(DATABASE_URL, DATABASE_NAME, test, DATABASE_REPLICA_SET)
+        job = Builder(self.database, BuilderMetadata(self.database), self.engine)
+        job.build(body["modelingCode"], list(classifiers), train, test, url_train, url_test)
+        self._maybe_wait(job)
+        return _json({MESSAGE_RESULT: [f"{BUILDER_URI_GET}{Database.create_prediction_filename(test, c)}{BUILDER_URI_PARAMS}"
+                                       for c in classifiers]}, HTTP_STATUS_CODE_SUCCESS_CREATED)
+
     # ---- GET /files/<name>?skip&limit&query (database_api_image/server.py:52-80) ------------------------
     def on_read(self, request, filename):
         limit, skip = 20, 0
@@ -149,6 +177,7 @@ class App:
         return _json({MESSAGE_RESULT: f"{DATATYPE_URI_GET}{filename}?query={{}}&limit=10&skip=0"}, HTTP_STATUS_CODE_SUCCESS_CREATED)
 
     def _maybe_wait(self, job):
+        self.last_job = job
         if self.synchronous:
             try:
                 job.wait()
@@ -176,11 +205,12 @@ def create_app(database: Database | None = None, engine=None, synchronous: bool 
 
 
 def main() -> None:
-    """``python -m learningorchestra_b200.server``: the three hot-path routes on one werkzeug dev server (the reference
-    runs three Flask processes with ``app.run(host, port)``, e.g. ``projection_image/server.py:157-161``).
+    """``python -m learningorchestra_b200.server``: the routes above, ``POST /models`` included, on one werkzeug dev server
+    (the reference runs one Flask process per service with ``app.run(host, port)``, e.g.
+    ``projection_image/server.py:157-161``).
     LOEXEC_HOST / LOEXEC_PORT select the bind address; LOEXEC_DEVICES (e.g. "0,1,2,3"; default: every visible GPU)
     the devices — with more than one, every binned histogram / castTo projection shards the resident table over them
-    (``sharding.open_engine`` -> ``lo_group_create_local``)."""
+    (``sharding.open_engine`` -> ``lo_group_create_local``), and so does every ``POST /models`` job's frames."""
     import os
 
     from werkzeug.serving import run_simple

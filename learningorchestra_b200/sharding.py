@@ -745,6 +745,25 @@ class ShardedEngine:
             self.engines[0]._ctx, shards, row0, len(shards), self._tables(table), int(col), rows, cap, nd, t),
             text.n - text.nulls, timing)
 
+    def text_codes_in(self, text: ShardedText, dictionary, table: ShardedTable, col: int) -> int:
+        """``Engine.text_codes_in`` of a :class:`ShardedText` into int32 column ``col`` of ``table``, both cut at the
+        same rows: the dictionary is uploaded once to every member's device and each piece is coded there, from a host
+        thread of its own.  The codes do not depend on the cut.  Returns the unseen cells summed over the pieces."""
+        self._every_row("text_codes_in")
+        if not isinstance(text, ShardedText):
+            raise TypeError("text_codes_in takes a ShardedText (ShardedEngine.text)")
+        text.check_cut(table)
+        return sum(self._each("text_codes_in", lambda i: self.engines[i].text_codes_in(
+            text.pieces[i], dictionary, table.shards[i], col)))
+
+    def random_split(self, parts, ids, bounds, seed: int) -> list:
+        """``Engine.random_split`` of every member's rows on its own device (``ids[i]`` the ``_id`` of parts[i]'s rows):
+        one list per split, each holding one ``AssembledRows`` per member.  A row's split depends on its ``_id`` and the
+        seed alone, so the splits hold the same rows for any cut."""
+        got = self._each("random_split", lambda i: self.engines[i].random_split(parts[i], ids[i], bounds, seed),
+                         undo=lambda splits: [p.free() for p in splits])
+        return [list(per_split) for per_split in zip(*got)]
+
     def assemble_rows(self, sources, label=None, dtype: str = "float32", handle_invalid: str = "error") -> list:
         """``Engine.assemble_rows`` over sharded tables: ``sources`` / ``label`` are ``(ShardedTable, col)`` pairs cut at
         the same rows, and every member assembles its own shard's rows on its own device, from a host thread of its own;

@@ -12,6 +12,8 @@ files (same class / method names, same documents, same messages):
     ``data_type_handler_image/utils.py:6-31``): identical documents and call signatures.
   * ``ProjectionRequest`` / ``HistogramRequest`` / ``DataTypeRequest`` — the three ``UserRequest``
     validators with the reference's message strings (``*/utils.py`` UserRequest).
+  * ``BuilderMetadata`` / ``BuilderRequest`` — the builder's ``Metadata`` and ``UserRequest``
+    (``builder_image/utils.py:45-86`` and ``:89-131``), for ``POST /models``.
 """
 from __future__ import annotations
 
@@ -122,6 +124,11 @@ class Database:
                f"?replicaSet={database_replica_set}&authSource=admin"
 
     @staticmethod
+    def create_prediction_filename(parent_filename: str, classifier_name: str) -> str:
+        """``builder_image/utils.py:38-41``: the dataset a classifier's predictions of ``parent_filename`` go to."""
+        return f"{parent_filename}{classifier_name}"
+
+    @staticmethod
     def collection_from_url(url: str) -> str:
         """Inverse of ``collection_database_url``: the collection name Spark would have opened."""
         tail = url.rsplit("/", 1)[-1].split("?", 1)[0]
@@ -176,6 +183,27 @@ class DataTypeMetadata:
         self.database_connector.insert_one_in_file(filename, {
             "datasetName": filename, "timeCreated": _now(), "_id": 0, "finished": False,
             "type": "transform/dataType"})
+
+    def update_finished_flag(self, filename, flag):
+        self.database_connector.update_one(filename, {"finished": flag}, {"_id": 0})
+
+
+class BuilderMetadata:
+    """``builder_image/utils.py:45-86``: one prediction dataset per classifier, replaced when it exists."""
+
+    def __init__(self, database):
+        self.database_connector = database
+        self.metadata_document = {"_id": 0, "type": "builder/sparkml", "finished": False}
+
+    def create_file(self, classifier_name, train_filename, test_filename):
+        metadata = self.metadata_document.copy()
+        metadata["parentDatasetName"] = [train_filename, test_filename]
+        metadata["timeCreated"] = _now()
+        metadata["classifier"] = classifier_name
+        metadata["datasetName"] = Database.create_prediction_filename(test_filename, classifier_name)
+        self.database_connector.delete_file(metadata["datasetName"])
+        self.database_connector.insert_one_in_file(metadata["datasetName"], metadata)
+        return metadata
 
     def update_finished_flag(self, filename, flag):
         self.database_connector.update_one(filename, {"finished": flag}, {"_id": 0})
@@ -251,3 +279,15 @@ class DataTypeRequest(_UserRequestBase):
         for field in fields:
             if fields[field] not in (self.NUMBER_TYPE, self.STRING_TYPE, self.FLOAT32_TYPE):
                 raise Exception(self.MESSAGE_INVALID_FIELDS)
+
+
+class BuilderRequest(_UserRequestBase):
+    """``builder_image/utils.py:89-131``, checked in ``analyse_request_errors``' order (``builder_image/server.py``)."""
+    MESSAGE_INVALID_FILENAME = "invalid input dataset name"
+    MESSAGE_INVALID_CLASSIFIER = "invalid classifier name"
+    CLASSIFIERS = ("LR", "DT", "RF", "GB", "NB")
+
+    def model_classifiers_validator(self, classifiers_list):
+        for classifier_name in classifiers_list:
+            if classifier_name not in self.CLASSIFIERS:
+                raise Exception(self.MESSAGE_INVALID_CLASSIFIER)
